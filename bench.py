@@ -10,7 +10,7 @@ GPU, each rank denoises its own 4 images (weak scaling, the only collective is o
 conditioning embeddings before step 0).  `value` times K steps with the latents resident in HBM; `e2e` times
 the same K steps through the module boundary with the latents coming from / returning to pinned host memory
 every step.  `--impl reference` times the reference algorithm's CPU path (the oracle port of the reference
-modules -- /root/reference itself is Python and absent on the GPU box) on the host cores.
+modules; the reference itself is Python) on the host cores.
 """
 import argparse
 import json
@@ -44,7 +44,8 @@ def measured_peaks():
             d = json.load(f)
         return dict(tflops_burst=d.get("bf16_tflops"), tflops_sustained=d.get("bf16_tflops_sustained"),
                     hbm_gbs=d.get("hbm_gbs"), source="MEASURED_PEAKS.json")
-    return dict(tflops_burst=1590.0, tflops_sustained=1400.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA's H100 SXM data sheet (dense FP16, HBM3, for a card allowed 700 W): a ceiling, not a measured rate
+    return dict(tflops_burst=989.0, tflops_sustained=None, hbm_gbs=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -246,7 +247,7 @@ def workload_config(args, world):
             "latent": [args.height // 8, args.width // 8], "images_per_gpu": args.batch,
             "unet_batch_per_gpu": 2 * args.batch, "global_images": args.batch * world, "context_tokens": 32,
             "unet_params": 1228661768 + 0, "parallelism": f"dp{world} (replicas, one conditioning broadcast)",
-            "l2": "per-step working set (2.5 GB weights + activations) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "per-step working set (2.5 GB weights + activations) exceeds the 50 MB L2; no explicit flush"}
 
 
 # BASELINE.json configs other than the metric config, as per-GPU step geometries (name, images per GPU, latent H, W, inpaint)
@@ -280,10 +281,10 @@ def step_roofline(plan, ms_per_step, n_unet, H, W, peaks, reps=2):
     peak = peaks["tflops_sustained"] or peaks["tflops_burst"]
     step_flops = uo.algorithmic_flops(uo.CONFIG_2_2, n_unet, H, W, 32)
     return {
-        "bound": "tensor", "kernel": "conv_gemm_kernel (3x3 / 1x1 / Conv1d implicit GEMM, tcgen05)",
+        "bound": "tensor", "kernel": "conv_gemm_kernel (3x3 / 1x1 / Conv1d implicit GEMM, wgmma)",
         "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
         "frac_of_burst": achieved / peaks["tflops_burst"] if peaks["tflops_burst"] else None, "traffic": None,
-        "peak_source": f"{peaks['source']} bf16_tflops_sustained (kernel timed inside a long step); burst "
+        "peak_source": f"{peaks['source']}: sustained {peaks['tflops_sustained']} (kernel timed inside a long step), burst "
                        f"{peaks['tflops_burst']}",
         "flops_note": "algorithmic FLOPs of the REFERENCE graph; the three up-ResBlock convs execute 4/9 of theirs (3x3 over a "
                       "nearest-2x upsampling = four 2x2 phase convolutions, DESIGN.md section 3)",
@@ -302,6 +303,11 @@ def run_k2(args):
     from kandinsky2 import ops
     from kandinsky2.model.gaussian_diffusion import FusedStep, create_ddpm_v22
     world, rank, local = dist_setup(args.gpus)
+    if args.dump_outputs:
+        # the per-layer autotuner may pick a split-K factor by event timing, and a K split changes the fp32 summation order;
+        # with only the bit-identical candidates (N tile, epilogue sets) two runs of one build compute the same latents
+        from kandinsky2 import launch_plan
+        launch_plan.TUNE_SMALL_M = 0
     ops.set_tuning(4, 0 if os.environ.get("K2_PDL", "1") == "0" else 1)  # programmatic dependent launch of the step's kernels
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
@@ -386,6 +392,12 @@ def run_k2(args):
     sampler.start()
     ms = timed(one_step, args.steps)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # what the timed path hands back to its caller: the latents after the last timed step (same arguments -> same seeded
+        # inputs and the same number of steps before it, so two builds can be compared output for output)
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), x.float().cpu().numpy())
     ms_per_step = ms / args.steps
     value = world * 1e3 / ms_per_step
 
@@ -422,15 +434,6 @@ def run_k2(args):
                 json.dump([dict(i=i, kind=k, gflop=fl / 1e9, us=ms * 1e3, tflops=(fl / (ms * 1e-3) / 1e12 if ms > 0 else 0))
                            for i, (k, fl, ms) in enumerate(det)], f)
         line["roofline"] = step_roofline(step.plan, ms_per_step, 2 * B, H, W, peaks)
-        # DRAM traffic of the dominant kernel comes from an ncu launch list of this same step (it cannot be measured inside
-        # an un-profiled run): profiles/conv_traffic_r2.json carries the commit it was measured at
-        traffic_file = os.path.join(ROOT, "profiles", "conv_traffic_r2.json")
-        if os.path.exists(traffic_file):
-            with open(traffic_file) as f:
-                tf = json.load(f)
-            line["roofline"]["traffic"] = tf["dram_bytes_per_launch"]
-            line["roofline"]["traffic_note"] = tf["note"]
-            line["roofline"]["traffic_measured_at_commit"] = tf.get("commit")
     if rank == 0 and world == 1 and not args.no_configs:
         # the other BASELINE configs' per-GPU step geometry: steps/s (graph replay, latents resident) + the same roofline object
         cfgs = {}
@@ -521,7 +524,12 @@ def main():
     ap.add_argument("--no-images", action="store_true", help="skip the whole-call images/s measurement")
     ap.add_argument("--no-configs", action="store_true", help="skip the other BASELINE configs' step geometries (N=1 only)")
     ap.add_argument("--inpaint", action="store_true", help="main workload = the inpainting UNet (9-channel stem)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the latents of the last timed step to DIR/latents.npy (float32); the layer autotuner then "
+                         "only chooses among bit-identical launch configurations")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "k2":
+        ap.error("--dump-outputs writes the outputs of the k2 arm only")
     if args.impl == "reference":
         run_reference(args)
     elif args.impl == "torch_gpu":

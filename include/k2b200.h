@@ -1,4 +1,4 @@
-/* k2b200.h -- C ABI of libk2b200.so, the B200 (sm_100a) kernel library behind the Kandinsky-2
+/* k2b200.h -- C ABI of libk2b200.so, the H100 (sm_90a) kernel library behind the Kandinsky-2
  * denoising hot path.
  *
  * The reference (ai-forever/Kandinsky-2) has no FFI: its "operator API" for this path is the set of
@@ -15,7 +15,7 @@
  *   - every launch is enqueued on the caller's stream (pass torch.cuda.current_stream().cuda_stream);
  *   - activations are NHWC fp16 ("rows" = pixels, row stride `ld*` in ELEMENTS so that a tensor may
  *     be a channel slice of a wider buffer); weights are pre-packed by the host (layout per function);
- *   - there is no CPU fallback: without an sm_100 device every call fails.
+ *   - there is no CPU fallback: without an sm_90 device every call fails.
  */
 #ifndef K2B200_H_
 #define K2B200_H_
@@ -34,24 +34,16 @@ int k2_version(void);
 long long k2_launch_count(void);
 void k2_reset_launch_count(void);
 /* Tuning knobs: key 0 = force conv/GEMM N tile (0 = auto); key 1 = split-K (0 auto, 1 off, n>1 forced);
- * key 2 = CTA-pair kernel (0 auto, 1 off, 2 on); key 3 = halo 3x3 kernel (0 off, 1-4 layout variants);
- * key 4 = programmatic dependent launch (0/1); key 5 = cycles by which the attention kernel's second query tile starts late
- * (default 1200; each query tile has its own MMA-issuing thread, so the two tiles' softmax phases stay apart);
- * key 6 = attention softmax arithmetic: n = eighths (0..3) of the exponentials evaluated on the FMA pipe instead of MUFU,
- * + 10 = scale-and-subtract as packed FFMA2, + 30 = FFMA2 and packed FADD2 row sums (bit-identical to the same n), 200 = traced
- * (default 0); keys 7 / 8 = low / high 32 bits of a device buffer (384 x u64) that the traced attention variant fills with
- * clock64 stamps of CTA (0,0,0) -- diagnostics only, see profiles/attn_probe.py; key 9 = attention softmax layout (1 = 16 warps,
- * half a score row per thread, default; 0 = 8 warps, one row per thread);
- * key 10 = default number of epilogue warp sets of the CTA-pair conv kernel (1; 2 = 384-thread variant whose second set drains
- * the other half of the 64-column pairs: bit-identical results, faster where the K loop is short).  Keys 0, 1, 2 and 10 are
- * process-wide defaults; k2_conv_gemm_cfg overrides them per call.  key 11 = blocks per SM the GroupNorm apply grids are sized
- * for (0 = each kernel's real occupancy, i.e. one full wave; 4 = the round-1 sizing); key 12 = tail split of the CTA-pair conv
- * kernel's last partial wave (0 off, default; 1 = where the K loop is long enough to pay for the hand-over; 2 = wherever
- * possible: tests and probes). */
+ * key 2 = CTA-pair conv kernel (0 auto, 1 off; 2 = on is refused: sm_90 has no CTA-pair MMA);
+ * key 4 = programmatic dependent launch (0/1); key 9 = attention query rows per CTA (1 = 128, 8 warps, default; 0 = 64,
+ * 4 warps; bit-identical results); key 10 = default number of epilogue warp sets of the conv kernel (1 = the first
+ * consumer warpgroup; 2 = both consumer warpgroups, each draining half of the 64-column pairs, for N tiles 128 and 256 -- N tile
+ * 192 runs with one set: bit-identical results, faster where the K loop is short).  Keys 0, 1, 2 and 10 are process-wide defaults; k2_conv_gemm_cfg overrides them per call.
+ * key 11 = blocks per SM the GroupNorm apply grids are sized for (0 = each kernel's real occupancy, i.e. one full wave). */
 int k2_set_tuning(int key, int value);
 
 /* ---------------------------------------------------------------------------------------------
- * Convolution / GEMM on tcgen05 tensor cores.
+ * Convolution / GEMM on wgmma tensor cores.
  * Replaces nn.Conv2d 3x3 (unet.py:152,180,426,562; movq_modules.py:139-148), nn.Conv2d 1x1
  * (unet.py:191; movq_modules.py:150-157,188-199) and nn.Conv1d k=1 (unet.py:251,257,258).
  *
@@ -67,20 +59,14 @@ int k2_set_tuning(int key, int value);
  * workspace (may be NULL): caller-owned scratch for split-K.  Where a cycle model of the launch (waves of work units x
  * K chunks per unit, plus the second pass) says so -- small M with a huge K -- K is split over several CTAs that write
  * fp32 partial tiles [split][M][Cout] there, and a second launch sums them in a fixed order (+bias, +residual) --
- * deterministic, no atomics.  The split-K partials use the LOWER half of the workspace.  The UPPER half serves the tail
- * split of the CTA-pair kernel (tuning key 12, off by default: measured neutral inside the power-capped step): when the last wave of work units would occupy only part of
- * the CTA pairs, each of its units is cut into 2..4 parts along K that run on the idle pairs, and the owning part adds the
- * others' fp32 accumulator tiles (handed over through the upper half, fixed summation order) before its ordinary epilogue --
- * one launch, same outputs and GroupNorm partials, a different (still deterministic) fp32 summation order.  The last
- * 64 KB of the workspace are hand-over flags: they must be ZERO before the first launch that uses the workspace; the library
- * leaves them zero after every launch.  Launches sharing a workspace must be stream-ordered.
+ * deterministic, no atomics.  Launches sharing a workspace must be stream-ordered.
  * gn_partial (may be NULL): fp32 [row groups][Cout][2]; when given and the launch qualifies (fp16 output, Cout % 64 == 0,
  * N tile >= 64) the launch also emits (sum, sum of squares) partials of the ROUNDED output, image-major, which
  * k2_gn_finalize turns into GroupNorm statistics -- the consumer's statistics pass disappears.  Row groups: one per M tile
  * when a tile lies inside one image; one per (image, spatial tile) for the (16 pixel x 8 image) tiles of tiny images; 16-row
  * groups from the second pass of a split-K launch.  gn_partial must hold max(M tiles*4, M/16)*Cout*2 floats
  * (k2_gn_scratch_floats); info[5] / info[6] tell what was written.
- * info (HOST pointer, may be NULL): int[7] = {N tile, CTA-pair mode, split-K factor, M tiles, images per tile,
+ * info (HOST pointer, may be NULL): int[7] = {N tile, CTA-pair mode (always 0 on sm_90), split-K factor, M tiles, images per tile,
  * gn_partial written (0 no / 1 epilogue / 2 split-K pass), row groups written in total}.
  * taps = 4 (allowed for a single source, fp16 output, no residual, H and W even): the source is [NB, H/2, W/2, C] and the call
  * computes the 3x3 convolution over its NEAREST-2x UPSAMPLING (unet.py:67-77 + :199-203; movq_modules.py:93-97) without
@@ -102,9 +88,9 @@ int k2_conv_gemm(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const vo
                  k2_stream_t stream);
 
 /* k2_conv_gemm with the launch configuration chosen by the caller instead of the library's cycle model:
- * cfg (HOST pointer, may be NULL = k2_conv_gemm) = int[4] {N tile (16/64/128/192/256), CTA-pair kernel (1 off, 2 on),
- * split-K factor (1 = off), epilogue warp sets of the CTA-pair kernel (1 or 2)}; a 0 entry keeps the automatic choice.
- * N tile, pair mode and epilogue sets never change a result bit (same K order per output element); the split factor does.
+ * cfg (HOST pointer, may be NULL = k2_conv_gemm) = int[4] {N tile (16/64/128/192/256), CTA-pair kernel (1 off; 2 is refused
+ * on sm_90), split-K factor (1 = off), epilogue warp sets (1 or 2)}; a 0 entry keeps the automatic choice.
+ * N tile and epilogue sets never change a result bit (same K order per output element); the split factor does.
  * The UNet / MoVQ launch plans time the candidates once per distinct layer shape and bake the winner into their CUDA graph.
  * w_batch_stride (elements, multiple of 8; 0 = one weight matrix): > 0 makes the call a BATCHED GEMM -- image n of the NB
  * images multiplies Wp + n * w_batch_stride.  This is how the MoVQ AttnBlock (movq_modules.py:201-225) runs without a loop
@@ -115,16 +101,12 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
                      int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
                      const int* cfg, long long w_batch_stride, k2_stream_t stream);
 
-/* The decisions k2_conv_gemm takes for a geometry -- M tile box, N tile, CTA-pair mode, split-K factor, how the GroupNorm
+/* The decisions k2_conv_gemm takes for a geometry -- M tile box, N tile, split-K factor, how the GroupNorm
  * partials come out -- without touching a pointer or the GPU (host arithmetic only; for tests, tooling and the caller's
  * scratch sizing).  taps: 9 if any source is a 3x3, else 1; Ktot as for k2_conv_gemm; workspace_bytes 0 = no workspace;
  * info = int[7] with the meaning given above. */
 int k2_conv_plan(int NB, int H, int W, int taps, int Ktot, int Cout, int out_mode, long long workspace_bytes,
                  int want_gn_partial, int* info);
-
-/* K parts the last partial wave's units were cut into (tail split, see k2_conv_gemm) by the most recent k2_conv_gemm /
- * k2_conv_gemm_cfg / k2_conv_plan call of this thread: 1 = not used.  Diagnostics for tests and tooling. */
-int k2_conv_last_tail_split(void);
 
 /* ---------------------------------------------------------------------------------------------
  * GroupNorm (32 groups in the UNet) statistics + fused apply.
@@ -164,7 +146,7 @@ int k2_gn_apply_fold(const void* src0, int C0, int ld0, const void* src1, int C1
                      int ldx, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Attention, head dim 64, online softmax, on tcgen05 (QK^T and PV) with encoder K/V prepended.
+ * Attention, head dim 64, online softmax, on mma.sync tensor cores (QK^T and PV) with encoder K/V prepended.
  * Replaces QKVAttention.forward (unet.py:286-340) incl. the optional flash-attn path (:303-332).
  *   qkv   fp16 [B, T, ldq] rows; head h owns channels [h*hs, (h+1)*hs) with q at +q_off, k at +k_off,
  *         v at +v_off (reference layout: hs=192, 0/64/128 -- unet.py:296).
@@ -179,7 +161,8 @@ int k2_attention_d64(const void* qkv, int ldq, int hs, int q_off, int k_off, int
 /* One head of width 512 over T tokens, no [T, T] score matrix: the MoVQ AttnBlock (movq_modules.py:201-225; the encoder's
  * twin vqgan_blocks.py:186-240).  qkv fp16 rows [B, T, ldq] with q / k / v at element offsets q_off / k_off / v_off (512 channels
  * each); out fp16 [B, T, ldo] (512 channels); scale multiplies q.k (the reference: C ** -0.5).  A CTA owns 128 queries and half
- * of the output channels (TMEM holds 256 columns of O + two score buffers), so the score tile is computed twice per query tile. */
+ * of the output channels (an fp32 O row of 256 channels fills 128 registers per thread), so the score tile is computed twice
+ * per query tile. */
 int k2_attention_d512(const void* qkv, int ldq, int q_off, int k_off, int v_off, int B, int T, float scale, void* out, int ldo,
                       k2_stream_t stream);
 

@@ -17,16 +17,7 @@ static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
 static int g_force_bn = 0;
 static int g_force_split = 0;  // 0 auto, 1 off, n>1 forced
-static int g_force_2cta = 0;   // 0 auto, 1 off, 2 on
-static int g_tail_split = 0;  // tuning key 12: stream-K over a CTA-pair launch's last, partial wave: 0 off (default), 1 where the
-                              // model says it pays, 2 wherever possible (tests / probes).  Measured (profiles/README.md):
-                              // 9-14 % on the level-2 2304 -> 1152 convolutions timed alone, nothing inside the power-capped
-                              // step (a partial wave's busy SMs clock higher), and it costs bit-identical results across
-                              // batch slots -> off.
-static int g_attn_stagger = 1200;  // cycles query tile 1 starts late (independent MMA issuers keep the offset): 218 -> 200 us at level 1, profiles/attn_probe_r2.txt
-static int g_attn_poly = 0;  // measured: the softmax is not MUFU-bound (profiles/README.md), offloading only adds instructions
 static int g_pdl = 0;          // programmatic dependent launch of the step's kernels
-static int g_halo_mode = 0;    // 0 off; 1/2: dense halo rows (pitch 10) without/with base offset; 3/4: pitch 16
 
 
 void set_error(const std::string& msg) { g_err = msg; }
@@ -40,12 +31,8 @@ bool pdl_enabled() { return g_pdl != 0; }
 static int g_conv_epi_sets = 1;
 static int g_gn_bps = 0;
 int gn_apply_blocks_per_sm() { return g_gn_bps; }
-int attention_stagger() { return g_attn_stagger; }
-int attention_poly_mode() { return g_attn_poly; }
-static int g_attn_half = 1;  // measured: 224 vs 235 us at the level-1 geometry (profiles/attn_probe_r2.txt)
+static int g_attn_half = 1;
 int attention_half_rows() { return g_attn_half; }
-static unsigned long long g_attn_trace = 0;
-unsigned long long* attention_trace_buffer() { return reinterpret_cast<unsigned long long*>(g_attn_trace); }
 
 int num_sms() {
   static int n = 0;
@@ -53,7 +40,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;  // H100 SXM
   }
   return n;
 }
@@ -78,7 +65,7 @@ static EncodeTiledFn get_encode_fn() {
 int encode_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                     const uint64_t* strides_bytes, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return fail("cuTensorMapEncodeTiled unavailable (no CUDA driver / not an sm_100 box)");
+  if (!fn) return fail("cuTensorMapEncodeTiled unavailable (no CUDA driver)");
   cuuint64_t gdim[5];
   cuuint64_t gstr[4];
   cuuint32_t bx[5];
@@ -150,86 +137,56 @@ static void choose_tile(int NB, int H, int W, int& TN, int& TH, int& TW, bool si
 }
 
 
-// Everything k2_conv_gemm decides before it touches a pointer: the M tile box, N tile, CTA-pair mode, split-K factor and
-// how the fused GroupNorm partials come out.  Pure host arithmetic (k2_conv_plan exposes it for tests and tooling).
+// Everything k2_conv_gemm decides before it touches a pointer: the M tile box, N tile, split-K factor and how the fused
+// GroupNorm partials come out.  Pure host arithmetic (k2_conv_plan exposes it for tests and tooling).
 struct ConvPlan {
   int TN, TH, TW, tiles_w, tiles_h, tiles_n, m_tiles;
-  int halo_pitch, halo_bo;
   int m_tiles_phase;  // up2: tile slots per output phase
-  int BN, two_cta, splits;
+  int BN, splits;
   int fuse_stats, row_groups;
-  int es;  // epilogue warp sets of the CTA-pair kernel (1 or 2)
-  int tail_first, tail_count, tail_split, tail_kps;  // stream-K over the last partial wave (tail_split <= 1: off; else 4 = slot
-                                                     // stride), tail_kps = K chunks per CTA pair's span
+  int es;  // epilogue warp sets (1 or 2)
 };
 
-// Workspace layout: split-K partial sums use the lower half; the upper half holds the tail-split hand-over tiles, its last
-// 64 KB the hand-over flags (zero whenever no conv launch is in flight: the caller zeroes them once, owners reset them).
-constexpr long long TAIL_FLAG_BYTES = 64 << 10;
-
-// cfg (may be null): per-call overrides {N tile, CTA-pair mode (1 off / 2 on), split-K factor, epilogue warp sets}; 0 = the
-// process-wide tuning knob, else automatic.  The caller's launch plan bakes its choice per launch (kandinsky2/model/unet.py).
+// cfg (may be null): per-call overrides {N tile, CTA-pair mode (0 / 1 = single CTA, the only kernel on sm_90), split-K factor,
+// epilogue warp sets}; 0 = the process-wide tuning knob, else automatic.  The caller's launch plan bakes its choice per launch (kandinsky2/model/unet.py).
 static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, int out_mode, bool has_workspace,
                       long long workspace_bytes, bool want_gn, ConvPlan& pl, const int* cfg = nullptr, bool up2 = false,
                       bool w_batched = false) {
   // up2: NB/H/W are the SOURCE geometry; every box is visited once per output phase (4x the tiles, same K loop)
   const int g_force_bn = (cfg && cfg[0]) ? cfg[0] : k2::g_force_bn;
-  const int g_force_2cta = (cfg && cfg[1]) ? cfg[1] : k2::g_force_2cta;
   const int g_force_split = (cfg && cfg[2]) ? cfg[2] : k2::g_force_split;
   pl.es = (cfg && cfg[3]) ? cfg[3] : k2::g_conv_epi_sets;
-  // halo kernel (one (8+2)x(16+2) activation box per K chunk instead of nine shifted boxes): 3x3 convolutions whose
-  // image tiles exactly into 8 x 16 pixel boxes -- measured slower than nine shifted boxes, tuning knob 3, off by default
-  pl.halo_pitch = 0;
-  pl.halo_bo = 0;
-  if (g_halo_mode > 0 && any9 && W % 8 == 0 && H % 16 == 0 && out_mode == 0 && Cout > 64 && g_force_2cta != 1) {
-    pl.halo_pitch = (g_halo_mode <= 2) ? 10 : 16;
-    pl.halo_bo = (g_halo_mode == 2 || g_halo_mode == 4) ? 1 : 0;
-  }
-  if (pl.halo_pitch) {
-    pl.TN = 1;
-    pl.TH = 16;
-    pl.TW = 8;
-  } else {
-    choose_tile(NB, H, W, pl.TN, pl.TH, pl.TW, w_batched);
-  }
+  choose_tile(NB, H, W, pl.TN, pl.TH, pl.TW, w_batched);
   pl.tiles_w = (W + pl.TW - 1) / pl.TW;
   pl.tiles_h = (H + pl.TH - 1) / pl.TH;
   pl.tiles_n = (NB + pl.TN - 1) / pl.TN;
   pl.m_tiles = pl.tiles_w * pl.tiles_h * pl.tiles_n;
   pl.m_tiles_phase = pl.m_tiles;
 
-  // Tile width N, CTA-pair mode and split-K factor from a cycle model fitted to the B200 sweeps
-  // (profiles/conv_sweep_r1.txt, conv_sweep_small_r1.txt, conv_small_k_r1.txt):
-  //   one K chunk of a work unit costs 2*BN + 60 cycles in the CTA-pair kernel (MMA time of the 256 x BN x 64 product +
-  //   pipeline hand-over), a unit adds ~2000 cycles of exposed prologue / epilogue, the launch takes
-  //   ceil(units / slots) waves of those, and a split-K launch pays the second pass (fixed ~4000 cycles + its traffic at
-  //   ~2200 B/cycle).  The CTA-pair kernel wins wherever Cout > 64 (half of the weight tile per CTA); among its N tiles
-  //   the model picks 192 / 128 where they divide Cout better or give a fuller last wave, and splits K only where the
-  //   tile count would leave most SM pairs idle.
+  // Tile width N and split-K factor from a cycle model of the sm_90 kernel (its MMA and operand rates, not a fit to
+  // measurements): one K chunk of a 128 x BN x 64 work unit costs 4*BN + 60 cycles (2048 fp16 FMA/clk/SM, the operand
+  // stream of 16 KB + BN*128 B per chunk stays below that at BN >= 128), a unit adds ~2000 cycles of exposed prologue /
+  // epilogue, the launch takes ceil(units / SMs) waves of those, and a split-K launch pays the second pass (fixed ~4000
+  // cycles + its traffic at ~1800 B/cycle of HBM).  Among the N tiles the model picks 192 / 128 where they divide Cout better
+  // or give a fuller last wave, and splits K only where the tile count would leave most SMs idle.
   int BN = g_force_bn;
   int splits = 1;
-  int two_cta = (Cout > 64 && g_force_2cta != 1) ? 1 : 0;
-  if (g_force_2cta == 2 && Cout > 64) two_cta = 1;
-  if (pl.halo_pitch) two_cta = 1;
-  // per-image weights: the two boxes of a CTA pair share one weight tile, so a pair must not straddle two images
-  if (w_batched && (pl.tiles_w * pl.tiles_h) % 2 != 0) two_cta = 0;
   const long long M_total = static_cast<long long>(NB) * H * W;
-  const bool can_split = !pl.halo_pitch && !up2 && !w_batched && has_workspace && out_mode == 0 && Cout % 8 == 0;
+  const bool can_split = !up2 && !w_batched && has_workspace && out_mode == 0 && Cout % 8 == 0;
   auto split_ok = [&](int sp) {
     if (sp == 1) return true;
     const int kps = (kchunks + sp - 1) / sp;
     return can_split && kps >= 8 && (sp - 1) * kps < kchunks &&
-           static_cast<long long>(sp) * M_total * Cout * 4 <= workspace_bytes / 2;  // upper half: tail-split hand-over
+           static_cast<long long>(sp) * M_total * Cout * 4 <= workspace_bytes;
   };
-  auto model = [&](int bn, int sp, bool pair) {
+  auto model = [&](int bn, int sp) {
     const long long nt = (Cout + bn - 1) / bn;
-    const long long units = static_cast<long long>(pair ? (pl.m_tiles + 1) / 2 : pl.m_tiles) * nt * sp * (up2 ? 4 : 1);
-    const long long slots = pair ? num_sms() / 2 : num_sms();
+    const long long units = static_cast<long long>(pl.m_tiles) * nt * sp * (up2 ? 4 : 1);
+    const long long slots = num_sms();
     const long long waves = (units + slots - 1) / slots;
     const long long kps = (kchunks + sp - 1) / sp;
-    const long long chunk = pair ? 2 * bn + 60 : (bn >= 256 ? 768 : 2 * bn + 160);  // 1-CTA: operand-bandwidth bound
-    long long cost = waves * (kps * chunk + 2000);
-    if (sp > 1) cost += 4000 + (static_cast<long long>(sp) + 1) * M_total * Cout * 4 / 2200;
+    long long cost = waves * (kps * (4LL * bn + 60) + 2000);
+    if (sp > 1) cost += 4000 + (static_cast<long long>(sp) + 1) * M_total * Cout * 4 / 1800;
     return cost;
   };
   if (BN == 0) {
@@ -238,7 +195,6 @@ static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, in
     else if (Cout <= 128) BN = 128;
     else BN = 0;  // chosen below together with the split factor
   }
-  if (two_cta && BN != 0 && BN < 128) two_cta = 0;
   {
     const int cand[3] = {256, 192, 128};
     long long best = -1;
@@ -248,9 +204,8 @@ static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, in
       if (BN && ci > 0) break;
       for (int sp = 1; sp <= 8; ++sp) {
         if (g_force_split > 0 && sp != g_force_split) continue;
-        if (pl.halo_pitch && sp > 1) continue;
         if (!split_ok(sp)) continue;
-        const long long c = model(bn, sp, two_cta != 0);
+        const long long c = model(bn, sp);
         if (best < 0 || c < best) {  // ties keep the wider tile / the smaller split (visited first)
           best = c;
           best_bn = bn;
@@ -262,49 +217,7 @@ static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, in
     splits = best_sp;
   }
   pl.BN = BN;
-  pl.two_cta = two_cta;
   pl.splits = splits;
-  if (up2) {  // tile slots per phase: even in pair mode, so that both boxes of a CTA pair belong to the same phase
-    pl.m_tiles_phase = two_cta ? (pl.m_tiles + 1) / 2 * 2 : pl.m_tiles;
-  }
-
-  // Tail split = stream-K over the LAST wave only (profiles/README.md, "level-2 wave quantisation"): units = m_pairs x n_tiles
-  // on P = SMs / 2 CTA pairs; when the last wave holds R < P units, their K loops laid end to end (R x kchunks chunks) are cut
-  // into P equal spans of L chunks, one per pair, so the wave takes L / kchunks of a unit's time instead of a whole unit.  A tile
-  // is then the sum of up to 4 K parts computed by different pairs: the part with the tile's first chunk adds the others' fp32
-  // accumulators in its epilogue (k2_conv_gemm.cu), in a fixed order.  Same outputs / GroupNorm partials layout, a different
-  // (deterministic) fp32 summation order than the unsplit launch.  L >= kchunks / 3 bounds the parts per tile.
-  pl.tail_first = pl.tail_count = pl.tail_kps = 0;
-  pl.tail_split = 1;
-  if (g_tail_split && two_cta && splits == 1 && !pl.halo_pitch && out_mode == 0 && Cout % 64 == 0 && BN % 64 == 0 && has_workspace) {
-    const int m_pairs = ((up2 ? 4 * pl.m_tiles_phase : pl.m_tiles) + 1) / 2;
-    const int units = m_pairs * ((Cout + BN - 1) / BN);
-    const int P = num_sms() / 2;
-    const int R = units % P;
-    if (R > 0 && kchunks >= 16) {
-      long long L = (static_cast<long long>(R) * kchunks + P - 1) / P;
-      L = std::max<long long>(L, (kchunks + 2) / 3);
-      int max_parts = 1;
-      for (int t = 0; t < R; ++t) {
-        const long long first = static_cast<long long>(t) * kchunks / L;
-        const long long last = std::min((static_cast<long long>(t + 1) * kchunks - 1) / L, (static_cast<long long>(R) * kchunks - 1) / L);
-        max_parts = std::max(max_parts, static_cast<int>(last - first + 1));
-      }
-      const long long buf_bytes = static_cast<long long>(R) * 2 * 3 * 128 * BN * 4;
-      const long long flag_bytes = static_cast<long long>(R) * 2 * 3 * 8 * 4;
-      // the hand-over (partner tiles through L2, the owner's epilogue after them) costs ~8 us that nothing overlaps: the K
-      // time saved, (kchunks - L) chunks of 2*BN + 60 cycles, must be a multiple of that (profiles/tail_probe_r2.txt: a gain at
-      // K = 162 / 324 chunks, a loss at 54 chunks and for the 18-chunk qkv GEMMs)
-      const long long saved_cycles = (kchunks - L) * (2LL * BN + 60);
-      if ((saved_cycles >= 26000 || (g_tail_split == 2 && L < kchunks)) && max_parts <= 4 && buf_bytes <= workspace_bytes / 2 - TAIL_FLAG_BYTES &&
-          flag_bytes <= TAIL_FLAG_BYTES) {
-        pl.tail_first = units - R;
-        pl.tail_count = R;
-        pl.tail_split = 4;  // slot stride: up to 3 partner parts per CTA half of a tile
-        pl.tail_kps = static_cast<int>(L);
-      }
-    }
-  }
 
   // fused GroupNorm partial statistics: from the epilogue when a tile never straddles two images (one partial per M
   // tile: the epilogue folds its four warps) or when it holds 16 pixels of each of 8 images (one partial per (image,
@@ -323,11 +236,10 @@ static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, in
   }
 }
 
-static thread_local int g_last_tail_split = 1;
 static void plan_to_info(const ConvPlan& pl, int* info) {
-  g_last_tail_split = pl.tail_split;
   if (!info) return;
-  info[0] = pl.BN; info[1] = pl.two_cta; info[2] = pl.splits; info[3] = pl.m_tiles; info[4] = pl.TN;
+  info[0] = pl.BN; info[1] = 0;  // CTA-pair mode: there is no CTA-pair kernel on sm_90
+  info[2] = pl.splits; info[3] = pl.m_tiles; info[4] = pl.TN;
   info[5] = pl.fuse_stats; info[6] = pl.row_groups;
 }
 
@@ -340,7 +252,6 @@ extern "C" {
 const char* k2_last_error(void) { return g_err.c_str(); }
 int k2_version(void) { return 100; }
 long long k2_launch_count(void) { return g_launches.load(); }
-int k2_conv_last_tail_split(void) { return g_last_tail_split; }
 void k2_reset_launch_count(void) { g_launches.store(0); }
 int k2_set_tuning(int key, int value) {
   if (key == 0) {
@@ -351,31 +262,15 @@ int k2_set_tuning(int key, int value) {
     g_force_split = value;
     return 0;
   }
-  if (key == 2) {
-    g_force_2cta = value;
-    return 0;
-  }
-  if (key == 3) {
-    g_halo_mode = value;
+  if (key == 2) {  // CTA-pair mode: 0 auto / 1 off are the same single-CTA kernel; sm_90 has no CTA-pair MMA
+    if (value == 2) return fail("k2_set_tuning: no CTA-pair conv kernel on sm_90");
     return 0;
   }
   if (key == 4) {
     g_pdl = value;
     return 0;
   }
-  if (key == 5) {
-    g_attn_stagger = value;
-    return 0;
-  }
-  if (key == 12) {
-    g_tail_split = value;
-    return 0;
-  }
-  if (key == 6) {
-    g_attn_poly = value;
-    return 0;
-  }
-  if (key == 10) {  // epilogue warp sets of the CTA-pair conv kernel: 1 (validated) or 2 (round-2 candidate)
+  if (key == 10) {  // epilogue warp sets of the conv kernel: 1 (consumer warpgroup 0) or 2 (both consumer warpgroups)
     g_conv_epi_sets = (value == 2) ? 2 : 1;
     return 0;
   }
@@ -383,16 +278,8 @@ int k2_set_tuning(int key, int value) {
     g_gn_bps = value;
     return 0;
   }
-  if (key == 9) {  // attention softmax layout: 0 = one thread per score row (8 warps), 1 = half a row per thread (16 warps)
+  if (key == 9) {  // attention query rows per CTA: 1 = 128 (8 warps), 0 = 64 (4 warps)
     g_attn_half = value ? 1 : 0;
-    return 0;
-  }
-  if (key == 7) {  // diagnostics: device address of the attention trace buffer, low / high 32 bits
-    g_attn_trace = (g_attn_trace & 0xffffffff00000000ull) | static_cast<unsigned int>(value);
-    return 0;
-  }
-  if (key == 8) {
-    g_attn_trace = (g_attn_trace & 0xffffffffull) | (static_cast<unsigned long long>(static_cast<unsigned int>(value)) << 32);
     return 0;
   }
 
@@ -418,6 +305,7 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
                "conv_gemm_cfg: N tile must be 0, 16, 64, 128, 192 or 256");
     K2_REQUIRE(cfg[1] >= 0 && cfg[1] <= 2 && cfg[2] >= 0 && cfg[2] <= 8 && cfg[3] >= 0 && cfg[3] <= 2,
                "conv_gemm_cfg: pair mode in 0..2, splits in 0..8, epilogue sets in 0..2");
+    K2_REQUIRE(cfg[1] != 2, "conv_gemm_cfg: no CTA-pair conv kernel on sm_90");
   }
   K2_REQUIRE(nsrc >= 1 && nsrc <= 3, "conv_gemm: 1..3 sources");
   K2_REQUIRE(NB > 0 && H > 0 && W > 0 && Cout > 0, "conv_gemm: bad geometry");
@@ -460,14 +348,12 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
   ConvPlan pl;
   plan_conv(NB, H, W, any9 || up2, kchunks, Cout, out_mode, workspace != nullptr, workspace_bytes, gn_partial != nullptr, pl,
             cfg, up2, w_batched);
-  K2_REQUIRE(!w_batched || (!up2 && pl.TN == 1 && !pl.halo_pitch), "conv_gemm_cfg: batched weights need single-image tiles");
+  K2_REQUIRE(!w_batched || (!up2 && pl.TN == 1), "conv_gemm_cfg: batched weights need single-image tiles");
   p.w_batched = w_batched ? 1 : 0;
   plan_to_info(pl, info);
   p.TN = pl.TN;
   p.TH = pl.TH;
   p.TW = pl.TW;
-  p.halo_pitch = pl.halo_pitch;
-  p.halo_bo = pl.halo_bo;
   p.tiles_w = pl.tiles_w;
   p.tiles_h = pl.tiles_h;
   p.tiles_n = pl.tiles_n;
@@ -482,34 +368,20 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
     uint64_t str[3] = {static_cast<uint64_t>(src.ld) * 2, static_cast<uint64_t>(src.ld) * 2 * W,
                        static_cast<uint64_t>(src.ld) * 2 * W * H};
     uint32_t box[4] = {64, static_cast<uint32_t>(p.TW), static_cast<uint32_t>(p.TH), static_cast<uint32_t>(p.TN)};
-    if (pl.halo_pitch && src.taps == 9) {
-      box[1] = static_cast<uint32_t>(pl.halo_pitch);
-      box[2] = 18;
-    }
     if (encode_tmap_f16(&p.tmA[s], src.ptr, 4, dims, str, box)) return -1;
   }
-  const int BN = pl.BN, splits = pl.splits, two_cta = pl.two_cta, fuse_stats = pl.fuse_stats;
-  p.two_cta = two_cta;
+  const int BN = pl.BN, splits = pl.splits, fuse_stats = pl.fuse_stats;
   p.splits = splits;
   p.k_per_split = (kchunks + splits - 1) / splits;
   p.M_total = static_cast<long long>(NB) * H * W * (up2 ? 4 : 1);
   p.ws = reinterpret_cast<float*>(workspace);
-  p.tail_first = pl.tail_first;
-  p.tail_count = pl.tail_count;
-  p.tail_split = pl.tail_split;
-  p.tail_kps = pl.tail_kps;
-  if (pl.tail_split > 1) {
-    char* wsb = reinterpret_cast<char*>(workspace);
-    p.tail_buf = reinterpret_cast<float*>(wsb + (workspace_bytes / 2 / 256) * 256);
-    p.tail_flags = reinterpret_cast<unsigned int*>(wsb + ((workspace_bytes - TAIL_FLAG_BYTES) / 256) * 256);
-  }
   p.n_tiles = (Cout + BN - 1) / BN;
   p.Cout = Cout;
   {
     uint64_t dims[3] = {static_cast<uint64_t>(Ktot), static_cast<uint64_t>(w_rows), static_cast<uint64_t>(w_batched ? NB : 1)};
     uint64_t str[2] = {static_cast<uint64_t>(ldw) * 2,
                        (w_batched ? static_cast<uint64_t>(w_batch_stride) : static_cast<uint64_t>(ldw) * w_rows) * 2};
-    uint32_t box[3] = {64, static_cast<uint32_t>(two_cta ? BN / 2 : BN), 1};
+    uint32_t box[3] = {64, static_cast<uint32_t>(BN), 1};
     if (encode_tmap_f16(&p.tmB, w_packed, 3, dims, str, box)) return -1;
   }
   p.bias = bias;

@@ -1,38 +1,20 @@
-// k2_attention.cu -- fused softmax(Q K^T) V for head dim 64 on tcgen05 tensor cores (flash-style, no
-// [T, Tkv] score matrix in HBM).
+// k2_attention.cu -- fused softmax(Q K^T * scale) V on sm_90 tensor cores (mma.sync m16n8k16, fp16 in / fp32 accumulate),
+// flash-style: no [T, Tkv] score matrix in HBM.  One kernel template serves both attention shapes of the model:
+//   head dim 64  (k2_attention_d64): QKVAttention.forward (kandinsky2/model/unet.py:286-340): the two torch.einsum calls
+//                (:335,:339), the fp32 softmax (:338), the torch.cat that prepends the encoder K/V (:300-302) and the optional
+//                flash-attn path (:303-332).  Keys / values are read from TWO buffers -- encoder tokens first, then the
+//                spatial tokens -- so the concat never exists.
+//   head dim 512 (k2_attention_d512): the single-head MoVQ AttnBlock (kandinsky2/vqgan/movq_modules.py:201-225; encoder twin
+//                vqgan_blocks.py:186-240).  Its output channels are split over two CTAs (DV = 256 each): an fp32 O row of 256
+//                channels is 128 registers per thread, the full 512 would not fit next to the scores.  8 warps = 128 queries
+//                per CTA, 16-key blocks.
 //
-// Replaces QKVAttention.forward (kandinsky2/model/unet.py:286-340): the two torch.einsum calls (:335,:339),
-// the fp32 softmax (:338), the torch.cat that prepends the encoder K/V (:300-302) and the optional
-// flash-attn path (:303-332).  Keys/values are read from TWO buffers -- encoder tokens first, then the
-// spatial tokens -- so the concat never exists.
-//
-// One CTA = one (batch, head, 2 x 128-query tiles); K/V tiles are shared by both query tiles.  Per query tile t and
-// 128-key block j:
-//     S_t(j) = Q_t K(j)^T        tcgen05.mma  M128 N128 K64   -> TMEM  (one 128-column fp32 S buffer per tile)
-//     P_t(j) = exp2(S*c - m)     4 softmax warps per tile, ONE THREAD PER SCORE ROW (128 keys in registers): tcgen05.ld ->
-//                                registers, thread-local row maximum (FMNMX3), exponentials -> fp16 pairs -> TENSOR memory
-//                                (tcgen05.st, 64 columns per tile)
-//     O_t   += P_t(j) V(j)       tcgen05.mma  M128 N64 K128 with the A operand read from tensor memory
-//                                (tcgen05.mma [d], [a_tmem], b_desc) -> TMEM; O accumulated there, rescaled by the softmax
-//                                warps only when a row maximum has outgrown the stale one by 2^8 -- exact either way
-//     out = O_t / l              at the end.
-// TMEM: S_t at t*128, O_t at 256 + t*64, P_t at 384 + t*64 -> all 512 columns.  V tiles are used as an MN-major B operand
-// exactly as TMA lands them ([key][64 d] rows), so V is never transposed.
-// Warp roles (384 threads): warp0 TMA producer (Q once, K/V ring of 4 stages), warp1 MMA issuer, warp2 TMEM allocator,
-// warps 4-11 softmax + epilogue (tile = (w-4)/4, TMEM lane quarter = w%4); setmaxnreg moves registers from the control
-// warpgroup (56) to the softmax warpgroups (224: 128 scores + 64 packed P words + the exponentials in flight).
-// Pipeline per tile: the warps release S_t as soon as the scores sit in their registers (s_free) and the issuer answers with
-// the next score product; block j+1's scores are pulled in INSIDE block j's exponentials, chunk by chunk as registers free
-// up, and folded into the next row maximum one chunk later, so a block starts with its maximum already known.  The PV(j-1)
-// barrier is only waited for after 96 of the block's 128 exponentials (P is held in registers until then).  MMA order per
-// key block and tile: P_t(j) V(j) when p_full_t(j) arrives, then S_t(j+2).
-//
-// History / measurements (profiles/README.md, profiles/attn_probe.py, profiles/pipe_probe.cu): the round-1 kernel used 16
-// softmax warps with half a row each, exchanged the row maximum through shared memory + a named barrier, and staged P in
-// shared memory (64 KB of stores + 64 KB of operand reads per key block, a fence.proxy.async per block); its clock64 trace
-// showed 2300 cycles of MUFU-saturated exponentials + 1700 cycles of hand-over chain per block.  This kernel: 251 -> 228 us at
-// the level-1 geometry (T = 2304, 12 heads, batch 8).  MUFU.EX2 retires one warp-wide instruction per 8 cycles per
-// sub-partition (pipe_probe); two warps per sub-partition reach 9.4 cycles with this instruction mix.
+// CTA = NW warps, 16 query rows per warp; per key block of BKV keys:
+//     S = Q K^T            Q fragments (ldmatrix) x K fragments (ldmatrix) from shared memory, fp32 in registers
+//     m = max(m, rowmax S * c), P = exp2(S * c - m), l = l * alpha + rowsum P, O = O * alpha + fp16(P) V
+//   P goes from the score accumulators straight into the A fragments of the PV product (same register layout), V is read
+//   with ldmatrix.trans as it lies in memory ([key][channel] rows).  K / V blocks are double-buffered with cp.async.
+//   P is rounded to fp16 before PV (as in the reference's fp16 mode, unet.py:338); the row sums use the unrounded fp32 P.
 #include <string.h>
 
 #include <algorithm>
@@ -42,662 +24,218 @@
 #include "k2_internal.h"
 
 namespace k2 {
+
 namespace {
 
-constexpr int BQ = 128;         // queries per softmax warpgroup (one query tile)
-constexpr int QT = 2;           // query tiles per CTA
-constexpr int BKV = 128;        // keys per block
-constexpr int HD = 64;          // head dim
-constexpr int TILE_BYTES = 128 * HD * 2;  // 16 KB: one Q / K / V tile
-constexpr int SMEM_Q = 0;
-constexpr int KV_STAGES = 4;
-constexpr int SMEM_KV = QT * TILE_BYTES;
-constexpr int SMEM_TOTAL = SMEM_KV + KV_STAGES * 2 * TILE_BYTES + 1024;  // dynamic: Q + the K/V ring (+ alignment slack)
-static_assert(SMEM_KV % 1024 == 0, "K/V tiles must sit on the 1024 B swizzle period");
-// The mbarriers and the HALF layout's exchange buffer are STATIC shared memory: their shared-window addresses are link-time
-// constants.  As offsets from the 1024 B-aligned dynamic base they cost the softmax warps ~10 uniform instructions per
-// barrier operation (the aligned base is re-derived from the generic pointer each time: the compiler rematerialises rather
-// than spend one of the warps' 96 registers), ~60 of the ~440 instructions a warp issued per key block.
-constexpr int XCH_FLOATS = 1536;  // fp32 [tile][parity][half][128] block maxima, then [tile][half][128] row sums
-// HALF = false: 4 control warps + 8 softmax warps, one thread per score row (tile = (w-4)/4, TMEM lane quarter = w%4)
-// HALF = true : 4 control warps + 16 softmax warps, half a row per thread (tile = (w-4)/8, key half = ((w-4)/4)%2)
-constexpr int nthreads(bool half) { return 128 + (half ? 512 : 256); }
-constexpr int TMEM_COLS = 512;  // S: 2 x 128, O: 2 x 64, P: 2 x 64
-constexpr int TM_S = 0;         // S of tile t at TM_S + t*128
-constexpr int TM_O = 256;       // O of tile t at TM_O + t*64
-constexpr int TM_P = 384;       // P of tile t as fp16 pairs (64 columns for 128 keys) at TM_P + t*64
-constexpr float RESCALE_GAP = 8.f;  // log2 units the running max may lag before O is rescaled (P <= 2^8 in fp16)
-
-// volatile: keeps its place in the instruction stream relative to the other ex2v (the softmax software pipeline)
-__device__ __forceinline__ float ex2v(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-// 640 threads: warp0 TMA producer, warp1 MMA issuer, warp2 TMEM allocator, warp3 idle, warps 4-19 softmax
-// (query tile = (w-4)/8, key half = ((w-4)/4)%2, TMEM lane quarter = w%4).
-// POLY: bit i set -> element i (mod 8) of every score row takes the MUFU-free exp2 (k2_common.cuh), bit 15 -> traced.
-// Diagnostics (POLY bit 0x8000 + tuning keys 7/8): CTA (0,0,0) stamps clock64() at the hand-over points of key blocks
-// TRACE_J0 .. TRACE_J0+TRACE_NJ-1 into trace[role][block][point]; role 0/1 = first warp of each softmax warpgroup, 2 = MMA issuer.
-constexpr int TRACE_J0 = 0;
-constexpr int TRACE_NJ = 16;
-template <int POLY>
-__device__ __forceinline__ void trace_pt(const AttnParams& p, int role, int j, int point) {
-  if constexpr ((POLY & 0x8000) != 0) {
-    if (p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j >= TRACE_J0 && j < TRACE_J0 + TRACE_NJ)
-      p.trace[(role * TRACE_NJ + (j - TRACE_J0)) * 8 + point] = static_cast<unsigned long long>(clock64());
-  }
+__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
+  __half2 h = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// PK: bit 0 -> scale-and-subtract as FFMA2 (two scores per instruction), bit 1 -> row sums as FADD2
-template <int POLY, bool HALF, int PK>
-__global__ void __launch_bounds__(nthreads(HALF), 1) attention_d64_kernel(const __grid_constant__ AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  __shared__ __align__(8) uint64_t bars[24];
-  __shared__ __align__(1024) float xch_buf[XCH_FLOATS];
-  __shared__ uint32_t tmem_slot;
-  uint64_t* q_full = bars;                     // 1
-  uint64_t* kv_full = bars + 1;                // KV_STAGES
-  uint64_t* kv_empty = kv_full + KV_STAGES;  // KV_STAGES
-  uint64_t* s_full = kv_empty + KV_STAGES;   // QT
-  uint64_t* p_full = s_full + QT;              // QT
-  uint64_t* pv_done = p_full + QT;             // QT: P_t(j) V(j) retired -> O_t current, P_t columns reusable
-  uint64_t* s_free = pv_done + QT;             // QT: S_t(j) is in the warpgroup's registers -> S_t(j+1) may be issued
-  uint32_t* tmem_ptr = &tmem_slot;
+template <int D, int DV, int NW, int BKV>
+struct FlashCfg {
+  static constexpr int BQ = 16 * NW;
+  static constexpr int QP = D + 8;    // row pitch (halves) of Q / K tiles: 16-byte ldmatrix rows on distinct bank groups
+  static constexpr int VP = DV + 8;
+  static constexpr int Q_BYTES = BQ * QP * 2;
+  static constexpr int K_BYTES = BKV * QP * 2;
+  static constexpr int V_BYTES = BKV * VP * 2;
+  static constexpr int SMEM_BYTES = Q_BYTES + 2 * (K_BYTES + V_BYTES);
+};
 
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (QT * BQ);
-  const int head = blockIdx.y;
+// grid: (query tiles, heads * D / DV, B); blockIdx.y = head * (D / DV) + output-channel split
+template <int D, int DV, int NW, int BKV>
+__global__ void __launch_bounds__(NW * 32, 1) flash_attention_kernel(const FlashParams p) {
+  using C = FlashCfg<D, DV, NW, BKV>;
+  constexpr int NSPLIT = D / DV;
+  extern __shared__ __align__(16) uint8_t smem[];
+  __half* sQ = reinterpret_cast<__half*>(smem);
+  __half* sK = reinterpret_cast<__half*>(smem + C::Q_BYTES);                  // [2][BKV][QP]
+  __half* sV = reinterpret_cast<__half*>(smem + C::Q_BYTES + 2 * C::K_BYTES);  // [2][BKV][VP]
+
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5;
+  const int lane = tid & 31;
+  const int q0 = blockIdx.x * C::BQ;
+  const int head = blockIdx.y / NSPLIT;
+  const int dsplit = blockIdx.y - head * NSPLIT;
   const int b = blockIdx.z;
-  const int nctx = (p.Tc + BKV - 1) / BKV;
-  const int nsp = (p.T + BKV - 1) / BKV;
-  const int nblk = nctx + nsp;
-  const int ntile = (q0 + BQ < p.T) ? 2 : 1;  // the second query tile may not exist
+  const int Tkv = p.Tc + p.T;
+  const int nblk = (Tkv + BKV - 1) / BKV;
 
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmQKV);
-    if (p.Tc > 0) tma_prefetch_desc(&p.tmEnc);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    mbar_init(q_full, 1);
-    for (int i = 0; i < KV_STAGES; ++i) {
-      mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], ntile);  // one tcgen05.commit arrival per query tile's issuer
-    }
-    for (int i = 0; i < QT; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], HALF ? 8 : 4);  // one arrival per softmax warp of the tile
-      mbar_init(&pv_done[i], 1);
-      mbar_init(&s_free[i], HALF ? 8 : 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp_idx == 2) {
-    tmem_alloc(tmem_ptr, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_wait();
   pdl_launch();
-  // register re-partition (per warpgroup): the control warps hand most of theirs to the softmax warps, whose 128-score row,
-  // 16 packed P words and the exponentials in flight need ~200
-  if (warp_idx < 4) {
-  if constexpr (HALF) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-  }
-  if (warp_idx == 0) {
-    // ===================================== TMA producer =====================================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, ntile * TILE_BYTES);
-      for (int t = 0; t < ntile; ++t)
-        tma_load_3d(smem + SMEM_Q + t * TILE_BYTES, &p.tmQKV, q_full, head * p.hs + p.q_off, q0 + t * BQ, b);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < nblk; ++j) {
-        mbar_wait(&kv_empty[stage], phase ^ 1);
-        uint8_t* sK = smem + SMEM_KV + stage * 2 * TILE_BYTES;
-        uint8_t* sV = sK + TILE_BYTES;
-        mbar_arrive_expect_tx(&kv_full[stage], 2 * TILE_BYTES);
-        if (j < nctx) {
-          tma_load_3d(sK, &p.tmEnc, &kv_full[stage], head * p.ehs + p.ek_off, j * BKV, b);
-          tma_load_3d(sV, &p.tmEnc, &kv_full[stage], head * p.ehs + p.ev_off, j * BKV, b);
-        } else {
-          const int kv0 = (j - nctx) * BKV;
-          tma_load_3d(sK, &p.tmQKV, &kv_full[stage], head * p.hs + p.k_off, kv0, b);
-          tma_load_3d(sV, &p.tmQKV, &kv_full[stage], head * p.hs + p.v_off, kv0, b);
-        }
-        if (++stage == KV_STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp_idx == 1 || warp_idx == 3) {
-    // ===================================== MMA issuers =======================================
-    // One issuing thread PER QUERY TILE (warp 1: tile 0, warp 3: tile 1).  With a single issuer serving the tiles in turn
-    // (wait p_full[0], issue, wait p_full[1], issue, ...) each tile's next step waited for the other tile's softmax: the
-    // two tiles ran in lock-step, all sixteen softmax warps took their exponentials at the same time (MUFU saturated for
-    // ~2100 of every ~3600 cycles, idle for the rest: profiles/README.md) and a start-up offset was pulled back within one
-    // key block.  Independent issuers leave the tiles coupled only through the K/V ring (kv_empty counts one arrival per
-    // tile), so tile 1's deliberate start-up delay (stagger_cycles) persists and one tile's exponentials fall into the
-    // other's hand-over phase.
-    const int t = warp_idx >> 1;
-    if (t < ntile && elect_one()) {
-      constexpr uint32_t idesc_s = make_idesc_f16(BQ, BKV, 0, 0);  // Q (K-major) x K (K-major)
-      constexpr uint32_t idesc_o = make_idesc_f16(BQ, HD, 0, 1);   // P (K-major, tensor memory) x V (MN-major)
-      auto issue_pv = [&](int jb, int stage_b) {
-        const uint32_t v_addr = smem_u32(smem + SMEM_KV + stage_b * 2 * TILE_BYTES + TILE_BYTES);
-        const uint32_t d = tmem_base + TM_O + t * HD;
-        const uint32_t a = tmem_base + TM_P + t * 64;
-#pragma unroll
-        for (int k = 0; k < BKV / 16; ++k) {
-          // A: 16 keys = 8 columns of fp16 pairs; B: V [128 keys][64 d] (MN-major), 16 keys = 16 rows of 128 B
-          umma_f16_ts(d, a + k * 8, make_sw128_desc(v_addr + k * 2048), idesc_o, (jb > 0 || k > 0) ? 1u : 0u);
-        }
-      };
-      auto issue_s = [&](int stage_b) {
-        const uint64_t adesc = make_sw128_desc(smem_u32(smem + SMEM_Q + t * TILE_BYTES));
-        const uint64_t bdesc = make_sw128_desc(smem_u32(smem + SMEM_KV + stage_b * 2 * TILE_BYTES));
-        const uint32_t d = tmem_base + TM_S + t * BKV;
-#pragma unroll
-        for (int k = 0; k < HD / 16; ++k)
-          umma_f16(d, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc_s, k != 0);
-        umma_commit(&s_full[t]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-      if (t == 1 && p.stagger_cycles > 0) {
-        // de-phase the two query tiles (tuning key 5): tile 1 starts this many cycles late
-        const long long t0 = clock64();
-        while (clock64() - t0 < p.stagger_cycles) {
-        }
-      }
-      issue_s(0);
-      if (nblk > 1) {
-        mbar_wait(&kv_full[1], 0);
-        mbar_wait(&s_free[t], 0);
-        tc_fence_after();
-        issue_s(1);
-      }
-      for (int j = 0; j < nblk; ++j) {
-        const int stage = j % KV_STAGES;
-        mbar_wait(&p_full[t], j & 1);
-        trace_pt<POLY>(p, 2, j, t * 4 + 0);
-        tc_fence_after();
-        issue_pv(j, stage);
-        umma_commit(&pv_done[t]);
-        umma_commit(&kv_empty[stage]);  // one arrival per tile: the stage is free when both tiles' PV(j) have retired
-        trace_pt<POLY>(p, 2, j, t * 4 + 1);
-        if (j + 2 < nblk) {
-          const int j2 = j + 2;
-          mbar_wait(&kv_full[j2 % KV_STAGES], (j2 / KV_STAGES) & 1);
-          mbar_wait(&s_free[t], (j + 1) & 1);
-          trace_pt<POLY>(p, 2, j, t * 4 + 2);
-          tc_fence_after();
-          issue_s(j2 % KV_STAGES);
-          trace_pt<POLY>(p, 2, j, t * 4 + 3);
-        }
-      }
+
+  {  // Q tile (rows past T are zero-filled)
+    constexpr int CPR = D / 8;  // 16-byte chunks per row
+    for (int i = tid; i < C::BQ * CPR; i += NW * 32) {
+      const int r = i / CPR, c = i - r * CPR;
+      const int q = q0 + r;
+      const __half* src = p.qkv + (static_cast<long long>(b) * p.T + (q < p.T ? q : 0)) * p.ldq + head * p.hs + p.q_off + c * 8;
+      cp_async_16(smem_u32(sQ + r * C::QP + c * 8), src, q < p.T ? 16 : 0);
     }
   }
-  } else {
-    // ===================================== softmax warps + epilogue ===========================
-    if constexpr (HALF) {
-    // ------------- 16 softmax warps: thread (t, h, row) owns keys [64h, 64h + 64) of one score row -------------
-    // Four softmax warps per sub-partition instead of two: the exponentials saturate the MUFU pipe (9.0 cycles per
-    // warp-wide ex2 against 12 with two warps, profiles/README.md) at the price of one shared-memory exchange + named
-    // barrier per block for the two halves of a row to agree on the maximum.
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 104;");
-    const int sw = warp_idx - 4;
-    const int t = sw >> 3;                        // query tile
-    const int h = (sw >> 2) & 1;                  // key half of the 128-key block
-    const int ew = warp_idx & 3;                  // TMEM lane quarter
-    const int row = ew * 32 + lane;               // query row in the tile == TMEM lane
-    if (t < ntile) {
-      const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16);
-      // addresses pinned in one register each (pin_reg; the 104-register budget has room for two): the tile's four
-      // mbarriers (s_full, p_full, pv_done, s_free are consecutive pairs: +0, +16, +32, +48) and its exchange slot
-      const uint32_t s_addr = lane_addr + TM_S + t * BKV + h * 64;
-      const uint32_t o_addr = lane_addr + TM_O + t * HD + h * 32;
-      const uint32_t p_tm = lane_addr + TM_P + t * 64 + h * 32;
-      const uint32_t bar_t = pin_reg(smem_u32(&s_full[t]));
-      constexpr uint32_t B_SFULL = 0, B_PFULL = 16, B_PVDONE = 32, B_SFREE = 48;
-      // fp32 [tile][parity][half][row] block maxima; the buffer is 1024 B-aligned, so the partner half's slot is own ^ 512
-      const uint32_t xch_own = pin_reg(smem_u32(xch_buf) + t * 2048 + h * 512 + row * 4);
-      float m_used = 0.f;   // the (possibly stale) maximum the exponentials are taken against, log2 domain
-      float l_run = 0.f;    // this half's share of the row sum
-      const float c = p.scale_log2e;
-      const bool tr = (ew == 0 && lane == 0 && h == 0);
-      // only the last encoder block and the last spatial block can be ragged: their key counts are fixed before the loop
-      const int v_ctx_tail = p.Tc - (nctx - 1) * BKV - h * 64, v_sp_tail = p.T - (nsp - 1) * BKV - h * 64;
-      auto block_valid = [&](int j) { return (j == nctx - 1) ? v_ctx_tail : (j == nblk - 1) ? v_sp_tail : BKV; };
-      float mxa = -INFINITY, mxb = -INFINITY;
-      auto land = [&](uint32_t (&sv)[32], int chunk, int valid) {
-        if (valid < 64) {  // ragged tail / short encoder block (block-uniform branch): masked scores -> -inf
-          asm volatile("" ::: "memory");
-          const uint32_t ninf = __float_as_uint(-INFINITY);
-#pragma unroll
-          for (int e = 0; e < 32; ++e)
-            if (chunk * 32 + e >= valid) sv[e] = ninf;
-        }
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) {
-          mxa = fmax3(mxa, __uint_as_float(sv[e]), __uint_as_float(sv[e + 1]));
-          mxb = fmax3(mxb, __uint_as_float(sv[e + 2]), __uint_as_float(sv[e + 3]));
-        }
-      };
-      // the two halves of a row agree on the block maximum: shared memory, double-buffered by block parity, one
-      // 256-thread named barrier per block
-      auto exchange = [&](int jb) {
-        const uint32_t slot = xch_own + (jb & 1) * 1024;
-        const float m_half = fmaxf(mxa, mxb) * c;
-        sts_f32(slot, m_half);
-        named_bar_sync(1 + t, 256);
-        mxa = -INFINITY;
-        mxb = -INFINITY;
-        return fmaxf(m_half, lds_f32(slot ^ 512));
-      };
-
-      uint32_t s0[32], s1[32];
-      mbar_wait_lean_s(bar_t + B_SFULL, 0);
-      tc_fence_after();
-      tmem_ld_32x32b_x32(s_addr, s0);
-      tmem_ld_32x32b_x32(s_addr + 32, s1);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_s(bar_t + B_SFREE);
-      {
-        const int v0 = block_valid(0);
-        land(s0, 0, v0);
-        land(s1, 1, v0);
-      }
-      float m_blk = exchange(0);
-
-      for (int j = 0; j < nblk; ++j) {
-        const bool more = j + 1 < nblk;
-        const int vnext = more ? block_valid(j + 1) : 64;
-        if (tr) trace_pt<POLY>(p, t, j, 0);
-        float alpha = 1.f;
-        bool any_grow = false;
-        if (j == 0) {
-          m_used = m_blk;
-        } else {
-          // both halves of a row see the same m_blk and m_used, so they take the same decision
-          const bool grow = m_blk > m_used + RESCALE_GAP;
-          any_grow = __any_sync(0xffffffffu, grow);
-          if (grow) {
-            alpha = ex2(m_used - m_blk);
-            m_used = m_blk;
-          }
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 1);
-        float l0 = 0.f, l1 = 0.f;
-        uint32_t pk[16];
-        const uint64_t c2 = pack_f32x2(c, c), nm2 = pack_f32x2(-m_used, -m_used);
-        uint64_t l2 = pack_f32x2(0.f, 0.f);
-        auto emit = [&](const uint32_t (&sv)[32]) {
-#pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            float a0, a1;
-            if constexpr ((PK & 1) != 0) {  // FFMA2: both scores of a pair in one instruction
-              unpack_f32x2(fma_f32x2(pack_f32x2(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), c2, nm2), a0, a1);
-            } else {
-              a0 = fmaf(__uint_as_float(sv[e]), c, -m_used);
-              a1 = fmaf(__uint_as_float(sv[e + 1]), c, -m_used);
-            }
-            const float p0 = ((POLY >> (e & 7)) & 1) ? ex2_poly(a0) : ex2(a0);
-            const float p1 = ((POLY >> ((e + 1) & 7)) & 1) ? ex2_poly(a1) : ex2(a1);
-            if constexpr ((PK & 2) != 0) {
-              l2 = add_f32x2(l2, pack_f32x2(p0, p1));  // FADD2
-            } else {
-              l0 += p0;
-              l1 += p1;
-            }
-            __half2 hh = __floats2half2_rn(p0, p1);
-            pk[e >> 1] = *reinterpret_cast<uint32_t*>(&hh);
-          }
-        };
-        emit(s0);
-        if (more) {  // S_t(j+1) has been complete for a long time (issued right after s_free(j)): no stall here
-          mbar_wait_lean_s(bar_t + B_SFULL, (j + 1) & 1);
-          tc_fence_after();
-          tmem_ld_32x32b_x32(s_addr, s0);
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 2);
-        // P_t's columns and O_t are needed only now: PV(j-1) had 32 exponentials of four warps (~1000 cycles) to retire
-        if (j > 0) {
-          mbar_wait_lean_s(bar_t + B_PVDONE, (j - 1) & 1);
-          tc_fence_after();
-          if (any_grow) {
-#pragma unroll 1
-            for (int oc = 0; oc < 32; oc += 8) {  // rare path: this half rescales 32 of the row's 64 O columns
-              uint32_t o[8];
-              tmem_ld_32x32b_x8(o_addr + oc, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 8; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-              tmem_st_32x32b_x8(o_addr + oc, o);
-            }
-            l_run *= alpha;
-          }
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 3);
-        tmem_st_32x32b_x16(p_tm, pk);  // keys 2c, 2c+1 of this half in column c of the row's lane
-        emit(s1);
-        tmem_st_32x32b_x16(p_tm + 16, pk);
-        if (more) {
-          tmem_ld_wait();
-          land(s0, 0, vnext);
-          tmem_ld_32x32b_x32(s_addr + 32, s1);
-        }
-        if constexpr ((PK & 2) != 0) unpack_f32x2(l2, l0, l1);
-        l_run += l0 + l1;
-        if (tr) trace_pt<POLY>(p, t, j, 4);
-        // P_t(j) complete in tensor memory, O_t accesses retired -> let the MMA warp go
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_s(bar_t + B_PFULL);
-        if (more) {
-          tmem_ld_wait();
-          land(s1, 1, vnext);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_s(bar_t + B_SFREE);
-          m_blk = exchange(j + 1);
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 5);
-      }
-      // epilogue: O / l, each half writes 32 of the 64 channels
-      const uint32_t lx = smem_u32(xch_buf) + 4096 + t * 1024 + row * 4;
-      sts_f32(lx + h * 512, l_run);
-      mbar_wait_lean_s(bar_t + B_PVDONE, (nblk - 1) & 1);
-      tc_fence_after();
-      tmem_ld_32x32b_x32(o_addr, s0);
-      tmem_ld_wait();
-      named_bar_sync(1 + t, 256);
-      const float l_tot = lds_f32(lx) + lds_f32(lx + 512);
-      const int q = q0 + t * BQ + row;
-      if (q < p.T) {
-        const float inv = 1.f / l_tot;
-        __half* orow = p.out + (static_cast<long long>(b) * p.T + q) * p.ldo + head * HD + h * 32;
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 ov;
-          __half2* oh = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            oh[e] = __floats2half2_rn(__uint_as_float(s0[v * 8 + 2 * e]) * inv, __uint_as_float(s0[v * 8 + 2 * e + 1]) * inv);
-          *reinterpret_cast<uint4*>(orow + v * 8) = ov;
-        }
+  auto load_kv = [&](int jb, int st) {
+    constexpr int KC = D / 8, VC = DV / 8;
+    for (int i = tid; i < BKV * (KC + VC); i += NW * 32) {
+      const int r = i / (KC + VC), c = i - r * (KC + VC);
+      const int key = jb * BKV + r;
+      const bool ok = key < Tkv;
+      const bool from_enc = key < p.Tc;
+      const __half* row = from_enc ? p.enc + (static_cast<long long>(b) * p.Tc + key) * p.lde + head * p.ehs
+                                   : p.qkv + (static_cast<long long>(b) * p.T + (ok ? key - p.Tc : 0)) * p.ldq + head * p.hs;
+      if (c < KC) {
+        const __half* src = row + (from_enc ? p.ek_off : p.k_off) + c * 8;
+        cp_async_16(smem_u32(sK + (st * BKV + r) * C::QP + c * 8), ok ? src : p.qkv, ok ? 16 : 0);
+      } else {
+        const __half* src = row + (from_enc ? p.ev_off : p.v_off) + dsplit * DV + (c - KC) * 8;
+        cp_async_16(smem_u32(sV + (st * BKV + r) * C::VP + (c - KC) * 8), ok ? src : p.qkv, ok ? 16 : 0);
       }
     }
+  };
+  load_kv(0, 0);
+  cp_async_commit();
+
+  const float c = p.scale_log2e;
+  float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
+  float o[DV / 8][4];
+#pragma unroll
+  for (int n = 0; n < DV / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+
+  const uint32_t q_lane = smem_u32(sQ + (warp * 16 + (lane & 15)) * C::QP + (lane >> 4) * 8);
+  for (int jb = 0; jb < nblk; ++jb) {
+    const int st = jb & 1;
+    if (jb + 1 < nblk) {
+      load_kv(jb + 1, st ^ 1);
+      cp_async_commit();
+      cp_async_wait<1>();
     } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int t = (warp_idx - 4) >> 2;            // query tile
-    const int ew = warp_idx & 3;                  // TMEM lane quarter
-    const int row = ew * 32 + lane;               // query row in the tile == TMEM lane
-    if (t < ntile) {
-      const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16);
-      const uint32_t s_addr = lane_addr + TM_S + t * BKV;
-      const uint32_t o_addr = lane_addr + TM_O + t * HD;
-      const uint32_t p_tm = lane_addr + TM_P + t * 64;
-      float m_used = 0.f;   // the (possibly stale) maximum the exponentials are taken against, log2 domain
-      float l_run = 0.f;    // row sum
-      const float c = p.scale_log2e;
-      const bool tr = (ew == 0 && lane == 0);
-      // only the last encoder block and the last spatial block can be ragged: their key counts are fixed before the loop
-      const int v_ctx_tail = p.Tc - (nctx - 1) * BKV, v_sp_tail = p.T - (nsp - 1) * BKV;
-      auto block_valid = [&](int j) { return (j == nctx - 1) ? v_ctx_tail : (j == nblk - 1) ? v_sp_tail : BKV; };
-      // a 32-score chunk that has just landed in registers: mask the keys past the end of a ragged / short block
-      // (block-uniform branch) and fold the chunk into the row maximum of ITS block (two FMNMX3 chains)
-      float mxa = -INFINITY, mxb = -INFINITY;
-      auto land = [&](uint32_t (&sv)[32], int chunk, int valid) {
-        if (valid < BKV) {
-          // the empty volatile asm keeps this a real (block-uniform) branch: without it the masks are if-converted into
-          // three instructions per score that every full block executes too (400 of the loop's 1180 instructions)
-          asm volatile("" ::: "memory");
-          const uint32_t ninf = __float_as_uint(-INFINITY);
-#pragma unroll
-          for (int e = 0; e < 32; ++e)
-            if (chunk * 32 + e >= valid) sv[e] = ninf;
-        }
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) {
-          mxa = fmax3(mxa, __uint_as_float(sv[e]), __uint_as_float(sv[e + 1]));
-          mxb = fmax3(mxb, __uint_as_float(sv[e + 2]), __uint_as_float(sv[e + 3]));
-        }
-      };
+      cp_async_wait<0>();
+    }
+    __syncthreads();
 
-      // S_t(0) -> registers.  From then on block j+1's scores are pulled in INSIDE block j's exponentials, one 32-score chunk
-      // as soon as its registers are free, and its row maximum is folded chunk by chunk one chunk later (after the load
-      // has landed), so when block j ends the next maximum is one FMNMX away: the MUFU pipe never waits for a
-      // load -> maximum -> compare chain (the first row-per-thread version idled ~1400 of every ~3500 cycles there).
-      uint32_t s0[32], s1[32], s2[32], s3[32];
-      mbar_wait_lean(&s_full[t], 0);
-      tc_fence_after();
-      tmem_ld_32x32b_x32(s_addr, s0);
-      tmem_ld_32x32b_x32(s_addr + 32, s1);
-      tmem_ld_32x32b_x32(s_addr + 64, s2);
-      tmem_ld_32x32b_x32(s_addr + 96, s3);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_free[t]);
-      {
-        const int v0 = block_valid(0);
-        land(s0, 0, v0);
-        land(s1, 1, v0);
-        land(s2, 2, v0);
-        land(s3, 3, v0);
-      }
-
-      for (int j = 0; j < nblk; ++j) {
-        const bool more = j + 1 < nblk;
-        const int vnext = more ? block_valid(j + 1) : BKV;
-        if (tr) trace_pt<POLY>(p, t, j, 0);
-        const float m_blk = fmaxf(mxa, mxb) * c;
-        mxa = -INFINITY;
-        mxb = -INFINITY;
-        // O_t lives in TMEM and is rescaled only when some row's maximum has outgrown the stale one by 2^8: exact
-        // arithmetic either way (numerator and denominator share m_used), far fewer TMEM round trips.  The decision
-        // needs no barrier; the rescale itself (rare) waits for PV(j-1) below, with 96 exponentials already done.
-        float alpha = 1.f;
-        bool any_grow = false;
-        if (j == 0) {
-          m_used = m_blk;
-        } else {
-          const bool grow = m_blk > m_used + RESCALE_GAP;
-          any_grow = __any_sync(0xffffffffu, grow);
-          if (grow) {
-            alpha = ex2(m_used - m_blk);
-            m_used = m_blk;
-          }
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 1);
-        // P = exp2(S*c - m_used) -> fp16 pairs, 16 words per 32-key chunk
-        float l0 = 0.f, l1 = 0.f;
-        const uint64_t c2 = pack_f32x2(c, c), nm2 = pack_f32x2(-m_used, -m_used);
-        uint64_t l2 = pack_f32x2(0.f, 0.f);
-        auto emit = [&](const uint32_t (&sv)[32], uint32_t (&packed)[16]) {
+    // S = Q K^T for this warp's 16 rows x BKV keys
+    float s[BKV / 8][4];
 #pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            float a0, a1;
-            if constexpr ((PK & 1) != 0) {  // FFMA2: both scores of a pair in one instruction
-              unpack_f32x2(fma_f32x2(pack_f32x2(__uint_as_float(sv[e]), __uint_as_float(sv[e + 1])), c2, nm2), a0, a1);
-            } else {
-              a0 = fmaf(__uint_as_float(sv[e]), c, -m_used);
-              a1 = fmaf(__uint_as_float(sv[e + 1]), c, -m_used);
-            }
-            const float p0 = ((POLY >> (e & 7)) & 1) ? ex2_poly(a0) : ex2(a0);
-            const float p1 = ((POLY >> ((e + 1) & 7)) & 1) ? ex2_poly(a1) : ex2(a1);
-            if constexpr ((PK & 2) != 0) {
-              l2 = add_f32x2(l2, pack_f32x2(p0, p1));  // FADD2
-            } else {
-              l0 += p0;
-              l1 += p1;
-            }
-            __half2 hh = __floats2half2_rn(p0, p1);
-            packed[e >> 1] = *reinterpret_cast<uint32_t*>(&hh);
-          }
-        };
-        uint32_t pk0[16], pk1[16], pk2[16], pk3[16];
-        emit(s0, pk0);
-        if (more) {  // S_t(j+1) has been complete for a long time (issued right after s_free(j)): no stall here
-          mbar_wait_lean(&s_full[t], (j + 1) & 1);
-          tc_fence_after();
-          tmem_ld_32x32b_x32(s_addr, s0);
-        }
-        emit(s1, pk1);
-        if (more) {
-          tmem_ld_wait();
-          land(s0, 0, vnext);
-          tmem_ld_32x32b_x32(s_addr + 32, s1);
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 2);
-        emit(s2, pk2);
-        if (more) {
-          tmem_ld_wait();
-          land(s1, 1, vnext);
-          tmem_ld_32x32b_x32(s_addr + 64, s2);
-        }
-        // P_t's columns and O_t are needed only now: PV(j-1) had three chunks of exponentials to retire
-        if (j > 0) {
-          mbar_wait_lean(&pv_done[t], (j - 1) & 1);
-          tc_fence_after();
-          if (any_grow) {
-#pragma unroll 1
-            for (int oc = 0; oc < HD; oc += 8) {  // rare path, 8 columns at a time
-              uint32_t o[8];
-              tmem_ld_32x32b_x8(o_addr + oc, o);
-              tmem_ld_wait();
+    for (int n = 0; n < BKV / 8; ++n) s[n][0] = s[n][1] = s[n][2] = s[n][3] = 0.f;
+    const uint32_t k_lane = smem_u32(sK + (st * BKV + ((lane >> 4) << 3) + (lane & 7)) * C::QP + ((lane >> 3) & 1) * 8);
+#pragma unroll 4
+    for (int kk = 0; kk < D / 16; ++kk) {
+      uint32_t a[4];
+      ldmatrix_x4(a, q_lane + kk * 32);
 #pragma unroll
-              for (int e = 0; e < 8; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-              tmem_st_32x32b_x8(o_addr + oc, o);
-            }
-            l_run *= alpha;
-          }
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 3);
-        tmem_st_32x32b_x16(p_tm, pk0);  // keys 2c, 2c+1 of the block in column c of the row's lane
-        tmem_st_32x32b_x16(p_tm + 16, pk1);
-        tmem_st_32x32b_x16(p_tm + 32, pk2);
-        emit(s3, pk3);
-        tmem_st_32x32b_x16(p_tm + 48, pk3);
-        if (more) {
-          tmem_ld_wait();
-          land(s2, 2, vnext);
-          tmem_ld_32x32b_x32(s_addr + 96, s3);
-        }
-        if constexpr ((PK & 2) != 0) unpack_f32x2(l2, l0, l1);
-        l_run += l0 + l1;
-        if (tr) trace_pt<POLY>(p, t, j, 4);
-        // P_t(j) complete in tensor memory, O_t accesses retired -> let the MMA warp go
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[t]);
-        if (more) {
-          tmem_ld_wait();
-          land(s3, 3, vnext);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s_free[t]);
-        }
-        if (tr) trace_pt<POLY>(p, t, j, 5);
-      }
-      // epilogue: O / l, one 128-byte output row per thread
-      mbar_wait_lean(&pv_done[t], (nblk - 1) & 1);
-      tc_fence_after();
-      tmem_ld_32x32b_x32(o_addr, s0);
-      tmem_ld_32x32b_x32(o_addr + 32, s1);
-      tmem_ld_wait();
-      const int q = q0 + t * BQ + row;
-      if (q < p.T) {
-        const float inv = 1.f / l_run;
-        __half* orow = p.out + (static_cast<long long>(b) * p.T + q) * p.ldo + head * HD;
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 ov;
-          __half2* oh = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            oh[e] = __floats2half2_rn(__uint_as_float(s0[v * 8 + 2 * e]) * inv, __uint_as_float(s0[v * 8 + 2 * e + 1]) * inv);
-          *reinterpret_cast<uint4*>(orow + v * 8) = ov;
-        }
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          uint4 ov;
-          __half2* oh = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            oh[e] = __floats2half2_rn(__uint_as_float(s1[v * 8 + 2 * e]) * inv, __uint_as_float(s1[v * 8 + 2 * e + 1]) * inv);
-          *reinterpret_cast<uint4*>(orow + 32 + v * 8) = ov;
-        }
+      for (int n = 0; n < BKV / 8; n += 2) {
+        uint32_t bk[4];
+        ldmatrix_x4(bk, k_lane + n * 8 * C::QP * 2 + kk * 32);
+        mma_16816(s[n], a, bk[0], bk[1]);
+        mma_16816(s[n + 1], a, bk[2], bk[3]);
       }
     }
-    }  // HALF
+
+    // online softmax over the block (rows lane / 4 and lane / 4 + 8 of the warp's 16)
+    const int kbase = jb * BKV + 2 * (lane & 3);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int n = 0; n < BKV / 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = kbase + n * 8 + (e & 1);
+        s[n][e] = key < Tkv ? s[n][e] * c : -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], s[n][e]);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_r[h], mx[h]);  // finite: every block holds at least one valid key
+      alpha[h] = ex2(m_r[h] - m_new);            // 0 for the first block
+      m_r[h] = m_new;
+    }
+    float ls[2] = {0.f, 0.f};
+#pragma unroll
+    for (int n = 0; n < BKV / 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        s[n][e] = ex2(s[n][e] - m_r[e >> 1]);
+        ls[e >> 1] += s[n][e];
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_r[h] = l_r[h] * alpha[h] + ls[h];
+#pragma unroll
+    for (int n = 0; n < DV / 8; ++n) {
+      o[n][0] *= alpha[0];
+      o[n][1] *= alpha[0];
+      o[n][2] *= alpha[1];
+      o[n][3] *= alpha[1];
+    }
+
+    // O += fp16(P) V
+    const uint32_t v_lane = smem_u32(sV + (st * BKV + ((lane >> 3) & 1) * 8 + (lane & 7)) * C::VP + (lane >> 4) * 8);
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+      uint32_t a[4];
+      a[0] = pack_h2(s[2 * kk][0], s[2 * kk][1]);
+      a[1] = pack_h2(s[2 * kk][2], s[2 * kk][3]);
+      a[2] = pack_h2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+      a[3] = pack_h2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+#pragma unroll
+      for (int n = 0; n < DV / 8; n += 2) {
+        uint32_t bv[4];
+        ldmatrix_x4_trans(bv, v_lane + (kk * 16 * C::VP + n * 8) * 2);
+        mma_16816(o[n], a, bv[0], bv[1]);
+        mma_16816(o[n + 1], a, bv[2], bv[3]);
+      }
+    }
+    __syncthreads();  // the next iteration's prefetch overwrites this stage
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // out = O / l
+  l_r[0] += __shfl_xor_sync(0xffffffffu, l_r[0], 1);
+  l_r[0] += __shfl_xor_sync(0xffffffffu, l_r[0], 2);
+  l_r[1] += __shfl_xor_sync(0xffffffffu, l_r[1], 1);
+  l_r[1] += __shfl_xor_sync(0xffffffffu, l_r[1], 2);
+  const float inv[2] = {1.f / l_r[0], 1.f / l_r[1]};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int q = q0 + warp * 16 + (lane >> 2) + 8 * h;
+    if (q >= p.T) continue;
+    __half* orow = p.out + (static_cast<long long>(b) * p.T + q) * p.ldo + head * p.ohs + dsplit * DV + 2 * (lane & 3);
+#pragma unroll
+    for (int n = 0; n < DV / 8; ++n)
+      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_h2(o[n][2 * h] * inv[h], o[n][2 * h + 1] * inv[h]);
   }
 }
 
-template <int POLY, bool HALF, int PK>
-static int launch_variant2(const AttnParams& p, cudaStream_t stream) {
+template <int D, int DV, int NW, int BKV>
+int launch_flash(const FlashParams& p, cudaStream_t stream) {
+  using C = FlashCfg<D, DV, NW, BKV>;
   static bool attr_set = false;
   if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(attention_d64_kernel<POLY, HALF, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       SMEM_TOTAL));
+    K2_CHECK_CUDA(cudaFuncSetAttribute(flash_attention_kernel<D, DV, NW, BKV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       C::SMEM_BYTES));
     attr_set = true;
   }
-  dim3 grid((p.T + QT * BQ - 1) / (QT * BQ), p.heads, p.B);
-  K2_CHECK_CUDA(launch_k(attention_d64_kernel<POLY, HALF, PK>, grid, dim3(nthreads(HALF)), SMEM_TOTAL, stream, p));
+  dim3 grid((p.T + C::BQ - 1) / C::BQ, p.heads * (D / DV), p.B);
+  K2_CHECK_CUDA(launch_k(flash_attention_kernel<D, DV, NW, BKV>, grid, dim3(NW * 32), C::SMEM_BYTES, stream, p));
   return 0;
-}
-template <int POLY, int PK = 0>
-static int launch_variant(const AttnParams& p, cudaStream_t stream) {
-  return attention_half_rows() ? launch_variant2<POLY, true, PK>(p, stream) : launch_variant2<POLY, false, PK>(p, stream);
 }
 
 }  // namespace
 
-int launch_attention_d64(const AttnParams& p, cudaStream_t stream) {
-  // tuning key 6: n = eighths of the exponentials evaluated without MUFU (ex2_poly), + 10 x (1: FFMA2, 3: FFMA2 + FADD2)
-  switch (attention_poly_mode()) {
-    case 0: return launch_variant<0x00>(p, stream);
-    case 1: return launch_variant<0x10>(p, stream);
-    case 2: return launch_variant<0x24>(p, stream);
-    case 3: return launch_variant<0x52>(p, stream);
-    case 10: return launch_variant<0x00, 1>(p, stream);
-    case 11: return launch_variant<0x10, 1>(p, stream);
-    case 12: return launch_variant<0x24, 1>(p, stream);
-    case 30: return launch_variant<0x00, 3>(p, stream);
-    case 31: return launch_variant<0x10, 3>(p, stream);
-    case 32: return launch_variant<0x24, 3>(p, stream);
-    case 200: return launch_variant<0x8000>(p, stream);  // traced (clock64 stamps of CTA (0,0,0), profiles/attn_probe.py)
-    default: return launch_variant<0x00>(p, stream);
-  }
+int launch_attention(const FlashParams& p, int head_dim, cudaStream_t stream) {
+  // head width 512: 8 warps x 16-key blocks (Q 130 KB + two K / V stages 49 KB of shared memory) -- 7.5 ms at the MoVQ 768 x 768
+  // geometry on an H100 SXM at 700 W, against 12.0 ms with 4 warps x 32-key blocks (one CTA of 4 warps per SM)
+  if (head_dim == 512) return launch_flash<512, 256, 8, 16>(p, stream);
+  // tuning key 9: query rows per CTA, 128 (8 warps, default) or 64 (4 warps); every warp computes its rows the same way
+  return attention_half_rows() ? launch_flash<64, 64, 8, 64>(p, stream) : launch_flash<64, 64, 4, 64>(p, stream);
 }
 
 }  // namespace k2
@@ -713,36 +251,26 @@ extern "C" int k2_attention_d64(const void* qkv, int ldq, int hs, int q_off, int
   K2_REQUIRE((enc != nullptr) == (Tc > 0), "attention_d64: enc and Tc go together");
   K2_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
              "attention_d64: 16-byte alignment");
-  AttnParams p;
-  memset(&p, 0, sizeof p);
-  {
-    const int width = (heads - 1) * hs + std::max(std::max(q_off, k_off), v_off) + 64;
-    K2_REQUIRE(width <= ldq, "attention_d64: qkv row narrower than heads*hs");
-    uint64_t dims[3] = {static_cast<uint64_t>(width), static_cast<uint64_t>(T), static_cast<uint64_t>(B)};
-    uint64_t str[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * T};
-    uint32_t box[3] = {64, 128, 1};
-    if (encode_tmap_f16(&p.tmQKV, qkv, 3, dims, str, box)) return -1;
-  }
+  K2_REQUIRE((heads - 1) * hs + std::max(std::max(q_off, k_off), v_off) + 64 <= ldq,
+             "attention_d64: qkv row narrower than heads*hs");
   if (Tc > 0) {
     K2_REQUIRE(lde % 8 == 0 && ehs % 8 == 0 && ek_off % 8 == 0 && ev_off % 8 == 0 &&
                    (reinterpret_cast<uintptr_t>(enc) & 15) == 0,
                "attention_d64: encoder strides/alignment");
-    const int width = (heads - 1) * ehs + std::max(ek_off, ev_off) + 64;
-    K2_REQUIRE(width <= lde, "attention_d64: encoder row narrower than heads*ehs");
-    uint64_t dims[3] = {static_cast<uint64_t>(width), static_cast<uint64_t>(Tc), static_cast<uint64_t>(B)};
-    uint64_t str[2] = {static_cast<uint64_t>(lde) * 2, static_cast<uint64_t>(lde) * 2 * Tc};
-    uint32_t box[3] = {64, 128, 1};
-    if (encode_tmap_f16(&p.tmEnc, enc, 3, dims, str, box)) return -1;
+    K2_REQUIRE((heads - 1) * ehs + std::max(ek_off, ev_off) + 64 <= lde, "attention_d64: encoder row narrower than heads*ehs");
   }
+  FlashParams p;
+  memset(&p, 0, sizeof p);
+  p.qkv = reinterpret_cast<const __half*>(qkv);
+  p.ldq = ldq; p.hs = hs; p.q_off = q_off; p.k_off = k_off; p.v_off = v_off;
+  p.enc = reinterpret_cast<const __half*>(enc);
+  p.lde = lde; p.ehs = ehs; p.ek_off = ek_off; p.ev_off = ev_off;
   p.B = B; p.heads = heads; p.T = T; p.Tc = Tc;
-  p.hs = hs; p.q_off = q_off; p.k_off = k_off; p.v_off = v_off;
-  p.ehs = ehs; p.ek_off = ek_off; p.ev_off = ev_off;
   p.out = reinterpret_cast<__half*>(out);
   p.ldo = ldo;
+  p.ohs = 64;
   p.scale_log2e = scale * 1.4426950408889634f;
-  p.stagger_cycles = attention_stagger();
-  p.trace = attention_trace_buffer();
-  int rc = launch_attention_d64(p, static_cast<cudaStream_t>(stream));
+  int rc = launch_attention(p, 64, static_cast<cudaStream_t>(stream));
   if (rc == 0) count_launch();
   return rc;
 }

@@ -1,5 +1,5 @@
-// k2_common.cuh -- sm_100a PTX wrappers shared by the k2b200 kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), descriptors.
+// k2_common.cuh -- sm_90a PTX wrappers shared by the k2b200 kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait), descriptors, mma.sync / ldmatrix.
 // Everything here is inline PTX; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -122,247 +122,92 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tm, ui
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA issue, commit, TMEM loads
+// wgmma (sm_90a warpgroup MMA): D[64 x N, registers of the 128 threads of one warpgroup] (+)= A[smem] * B[smem]
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M rows = TMEM lanes, K elements packed two fp16 per 32-bit column,
-// 8 columns per K = 16 step) is read from tensor memory, so it never crosses shared memory.  A must be K-major.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives when all previously issued MMAs of this thread are complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets lane (base_lane+i), cols c..c+31
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// store 32 consecutive 32-bit columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// Descriptors (bit layouts per the sm_100 UMMA spec; cf. cute/arch/mma_sm100_desc.hpp)
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, tile rows of 128 bytes packed at a 128 B pitch
-// (what a TMA box with a 64 x fp16 inner dimension and CU_TENSOR_MAP_SWIZZLE_128B writes).
-//   K-major operand : rows = M/N index, the 128 B row = 64 K elements; 8-row groups 1024 B apart (SBO).
-//   MN-major operand: rows = K index, the 128 B row = 64 M/N elements; 8-row groups 1024 B apart (SBO).
-// bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2=SW128)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, 128-byte swizzle, K-major tile rows of 128 bytes (64 fp16) packed at a 128 B pitch, 8-row
+// groups 1024 B apart (what a TMA box with a 64 x fp16 inner dimension and CU_TENSOR_MAP_SWIZZLE_128B writes).  A K step of
+// 16 elements inside the swizzle row advances the start address by 32 bytes (+2 in the address field).
+// bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout (1 = SW128)
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;             // LBO (ignored for one swizzle atom along the leading dim)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO = 1024 B between 8-row groups
-  d |= static_cast<uint64_t>(1) << 46;             // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 16;          // LBO (ignored for one swizzle atom along K)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;  // SBO = 1024 B between 8-row groups
+  d |= static_cast<uint64_t>(1) << 62;          // SWIZZLE_128B
   return d;
 }
-// General form: explicit stride between 8-row groups (SBO) and matrix base offset (bits [49,52): the phase of the
-// 128B-swizzle pattern at the start address, (addr >> 7) & 7, for operands that do not start on a 1024 B boundary).
-__device__ __forceinline__ uint64_t make_sw128_desc_ex(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t base_offset) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// Instruction descriptor for kind::f16, fp16 A/B, fp32 accumulate.
-//   [4,6) c_format=1 (f32) | [7,10) a_format=0 (f16) | [10,13) b_format=0 | 15 a_major | 16 b_major
-//   [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-
-// ----------------------------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variants: a CTA pair of one cluster cooperates on M=256 tiles.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address of the same variable in the CTA of rank `rank` (shared::cluster window)
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// Remote arrive on the pair leader's "accumulator drained" barrier.  What the arrival publishes is TMEM state, ordered by
-// tcgen05.wait::ld + tcgen05.fence::before_thread_sync on this side and tcgen05.fence::after_thread_sync on the waiter's; no
-// generic-proxy memory needs to become visible, so the arrive is RELAXED.  Round 1 used .release.cluster, which ptxas lowers to
-// MEMBAR.ALL.CTA + MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR: every epilogue warp waited, once per tile, until the tile's global
-// stores were visible GPU-wide before it released the accumulator (ncu source page of the proj GEMM, profiles/README.md).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit: the barrier of the pair's leader
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4}], [%2];"
-      ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(void* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5}], [%2];"
-      ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1,
-                                             int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// Accumulator layout (m64nN, fp32): thread t of the warpgroup, warp w = t / 32, lane l: d[i] holds row 16 w + l / 4 + 8 ((i / 2) & 1),
+// column 8 (i / 4) + 2 (l & 3) + (i & 1).  Both operands K-major (no transpose), scale 1.
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives (once) on the barrier at the same shared offset in every CTA of `mask` when the MMAs issued so far retire
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// Programmatic dependent launch: every kernel of the step waits here (before its first global-memory access) for the
-// previous kernel in the stream to complete, and immediately lets the next kernel's CTAs be scheduled, so their
-// launch latency and prologue (barrier init, TMEM allocation, descriptor prefetch) overlap this kernel's execution.
-// Both are no-ops for a launch without the programmatic-serialization attribute.
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// register budget of a warp-specialised kernel: the producer warpgroup gives registers back, the MMA warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// ----------------------------------------------------------------------------------------------
+// mma.sync m16n8k16 (fp16 in, fp32 accumulate) and ldmatrix, for the attention kernels
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
+}
+// 16-byte global -> shared copy (L2 only); src_bytes < 16 zero-fills the rest
+__device__ __forceinline__ void cp_async_16(uint32_t saddr, const void* gptr, int src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(gptr), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
 __device__ __forceinline__ void sts_v4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
@@ -376,121 +221,24 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
   return v;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
 // named barrier among `count` threads (count % 32 == 0); id 0 is __syncthreads'
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-// arrive without waiting: the other `count - (arriving threads)` threads complete the barrier with bar.sync
-__device__ __forceinline__ void named_bar_arrive(int id, int count) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
-}
+// Programmatic dependent launch: every kernel of the step waits here (before its first global-memory access) for the
+// previous kernel in the stream to complete, and immediately lets the next kernel's CTAs be scheduled, so their
+// launch latency and prologue (barrier init, descriptor prefetch) overlap this kernel's execution.
+// Both are no-ops for a launch without the programmatic-serialization attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// x * sigmoid(x) with one MUFU.EX2 and one MUFU.RCP (an IEEE division here costs ~10 extra instructions per element,
-// and GroupNorm+SiLU touches 1.3 G elements per step)
-// On B200 the MUFU (XU) pipe retires 8 lanes/clk/SM -- a warp-wide ex2 / rcp / tanh occupies it for 16 cycles -- and both
-// GroupNorm+SiLU (1.3 G elements per step) and the attention softmax are bound by it, so every transcendental counts:
-// SiLU as h + h*tanh(h), h = x/2 (ONE MUFU.TANH, rel. error 2^-11, below the fp16 rounding of the stored result)
-// instead of ex2 + rcp (two).
+// x * sigmoid(x) as h + h*tanh(h), h = x/2: ONE MUFU.TANH (rel. error 2^-11, below the fp16 rounding of the stored result)
+// instead of ex2 + rcp -- GroupNorm+SiLU touches 1.3 G elements per step and the MUFU pipe is the narrow one.
 __device__ __forceinline__ float silu_f(float x) {
   const float h = 0.5f * x;
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
   return fmaf(h, t, h);
-}
-// 2^x on the FMA/ALU pipes only (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], degree-4 minimax
-// polynomial for 2^f (max rel. error 2.7e-6), exponent added to the bit pattern.  Valid for x <= 126; x < -126
-// (including -inf) returns 2^-126 ~ 0.
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float t = x + 12582912.f;            // 1.5 * 2^23: the integer part lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);
-  float p = fmaf(0.009560510516166687f, f, 0.05591703951358795f);
-  p = fmaf(p, f, 0.24024981260299683f);
-  p = fmaf(p, f, 0.6931219696998596f);
-  p = fmaf(p, f, 0.9999991655349731f);
-  return __int_as_float(__float_as_int(p) + ((__float_as_int(t) - 0x4B400000) << 23));
-}
-
-// Packed fp32 pairs (sm_100 FFMA2 / FADD2): one issue slot for two lanes' worth of arithmetic.  The attention softmax is
-// issue-limited next to its MUFU work (profiles/README.md: 7.8 instructions per exponential before, IPC 0.6 per sub-partition
-// with the MUFU pipe 61 % busy), so the scale-and-subtract and the row sum go two elements per instruction.
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// explicit shared-window accesses: pointers derived from the aligned dynamic-shared base lose their address space and
-// become generic LD / ST otherwise
-__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
-  return v;
-}
-
-// Same mbarrier operations on a 32-bit shared-window address (kept in one register by the caller, see pin_reg).
-__device__ __forceinline__ bool mbar_try_wait_s(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.b32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_lean_s(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_s(bar, parity)) return;
-  long long t0 = clock64();
-  while (!mbar_try_wait_s(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) __trap();
-  }
-}
-__device__ __forceinline__ void mbar_arrive_s(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// Makes a value opaque to the optimiser: it stays in ONE register instead of being re-derived (rematerialised) from
-// %tid / kernel parameters at every use -- what ptxas otherwise does for the softmax warps' tensor-memory, barrier and
-// exchange addresses (~8 instructions per use, ~60 per key block).
-__device__ __forceinline__ uint32_t pin_reg(uint32_t v) {
-  asm volatile("mov.b32 %0, %0;" : "+r"(v));
-  return v;
-}
-
-// GPU-scope release store / acquire load of a flag in global memory (hand-over of data written with ordinary stores before a
-// __threadfence on the producer side; the consumer reads the data with ld.global.cg after the acquire).
-__device__ __forceinline__ void st_release_gpu(unsigned int* addr, unsigned int v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* addr) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(addr) : "memory");
-  return v;
 }
 
 }  // namespace k2

@@ -1,4 +1,4 @@
-// k2_conv_gemm.cu -- im2col-free 3x3 / 1x1 convolution and plain GEMM on tcgen05 tensor cores.
+// k2_conv_gemm.cu -- im2col-free 3x3 / 1x1 convolution and plain GEMM on sm_90a warpgroup MMA (wgmma) tensor cores.
 //
 // Replaces the cuDNN / cuBLAS call sites of the reference hot path:
 //   nn.Conv2d 3x3   kandinsky2/model/unet.py:152,180,426,562 ; vqgan/movq_modules.py:139-148,268-270
@@ -10,14 +10,17 @@
 //     For tap (dy, dx) the A operand is the SAME box shifted by (dy, dx), fetched with ONE 4-D TMA
 //     whose out-of-bounds elements are zero-filled by the hardware: conv padding costs nothing and no
 //     im2col buffer exists in HBM or smem.
-//   * Up to three A "segments" accumulate into the same TMEM tile: the 3x3 conv input plus 1x1 skip
+//   * Up to three A "segments" accumulate into the same accumulator tile: the 3x3 conv input plus 1x1 skip
 //     inputs (raw x, optionally split in two for the un-materialised torch.cat of the up path). This is
 //     how ResBlock's  skip_connection(x) + conv(h)  (unet.py:220) becomes a single kernel.
 //   * Weights are pre-packed [Cout][K] fp16, K = concat over segments/taps/channels, loaded by 2-D TMA.
-//   * Warp roles (256 threads): warp0 = TMA producer, warp1 = tcgen05.mma issuer, warp2 = TMEM alloc,
-//     warps4-7 = epilogue (tcgen05.ld -> +bias (+residual) -> fp16 -> global). Persistent over tiles,
-//     smem ring of STAGES (A 16 KB + B BN*128 B), TMEM accumulator double-buffered (2 x BN columns) so
-//     the epilogue of tile i overlaps the mainloop of tile i+1.
+//   * Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = wgmma consumers, rows
+//     [0, 64) and [64, 128) of the M tile (m64nNk16, N = 64 per instruction -- 16 for the N = 16 output heads -- both operands
+//     K-major from the 128 B-swizzled TMA tiles).  Persistent over tiles, smem ring of STAGES (A 16 KB + B BN*128 B).
+//   * Epilogue: the consumers park their register accumulators, BNC columns at a time, in a shared-memory tile with one fp32
+//     row per output pixel; the epilogue warps then read it one ROW per thread (warp ew of a set owns rows [32 ew, 32 ew + 32))
+//     -> + bias (+ residual) -> fp16 rows, fp32 split-K partials or fp32 NCHW, plus the fused GroupNorm partial statistics.
+//     The producer keeps prefetching the next tile's operands meanwhile.
 #include <stdio.h>
 
 #include "k2_common.cuh"
@@ -30,19 +33,27 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
+constexpr int ACC_PAD = 4;                  // fp32 row pitch BNC + 4: row-per-thread float4 reads hit distinct banks
 
 constexpr int EPI_STAGE_FLOATS = 32 * 33;              // per-warp staging: 4224 B (4096 used)
 constexpr int EPI_BYTES = 4 * EPI_STAGE_FLOATS * 4 + 4 * 256 * 4;  // + per-warp bias copy (<= 256 columns)
+constexpr int SMEM_LIMIT = 227 * 1024;                 // sm_90 opt-in maximum per block
 
-template <int BN>
+// ES = number of epilogue warp SETS (each set = 4 warps covering the 128 accumulator rows).  ES = 1: the warps of consumer
+// warpgroup 0; ES = 2: both consumer warpgroups, set `es` handling the 64-column pairs jp with jp % 2 == es of a staged pass.
+template <int BN, int ES>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 4 : (BN >= 192 ? 5 : (BN >= 128 ? 6 : 8));
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
+  // columns staged per epilogue pass: 64 (one pass per 64-column block); 128 with two epilogue sets so that both have work
+  static constexpr int BNC = (BN < 64) ? BN : (ES == 2 ? 128 : 64);
+  static_assert(ES == 1 || BN % 128 == 0, "two epilogue sets need N tiles of 128 or 256");
+  static constexpr int ACC_BYTES = BM * (BNC + ACC_PAD) * 4;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int STAT_BYTES = EPI_BYTES;  // epilogue staging (output transpose, residual, statistics) + bias copies
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + STAT_BYTES + 1024;  // +1024 alignment slack
+  static constexpr int FIXED = ACC_BYTES + ES * EPI_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
+  static constexpr int STAGES = (SMEM_LIMIT - FIXED) / STAGE_BYTES > 6 ? 6 : (SMEM_LIMIT - FIXED) / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
+  static_assert(STAGES >= 2, "conv_gemm: shared memory does not hold two pipeline stages");
 };
 
 // up2 (3x3 conv over the nearest-2x upsampled source as four 2x2 phase convolutions): m_idx = phase * m_tiles_phase + box
@@ -63,33 +74,39 @@ __device__ __forceinline__ void decode_m_tile(const ConvGemmParams& p, int m_idx
   n0 = tn_i * p.TN;
 }
 
-// Epilogue of one (128-row x BN-column) accumulator tile held in this CTA's TMEM at column `acc_col`:
-// tcgen05.ld -> + bias (+ residual) -> fp16 rows (out_mode 0), fp32 split-K partials (out_mode 2) or fp32 NCHW
-// (out_mode 1).
-//
-// A thread owns one accumulator ROW (TMEM lane), so storing straight from registers makes every warp store touch 32
-// different cache lines with 16 bytes each (and every residual load likewise): with short K loops (the attention
-// qkv / proj GEMMs, 12..24 chunks) that epilogue, not the tensor core, set the pace (profiles/conv_small_k.py).  The
-// fp16 / split-K paths therefore go through a per-warp shared-memory transpose (32 rows x 128 B, 16-byte pieces XOR-
-// swizzled by the row): registers -> smem by row, smem -> global with 8 lanes per row, i.e. 4 complete 128-byte lines
-// per store instruction; the residual comes in the same way (coalesced load -> smem -> own row), the bias is read as
-// broadcast LDS.128 from a per-warp copy, and the fused GroupNorm statistics are column sums over the staged fp16 tile.
+// N consecutive fp32 of a staged accumulator row, as raw bits
+template <int N>
+__device__ __forceinline__ void acc_ld(const float* src, uint32_t (&r)[N]) {
+#pragma unroll
+  for (int v = 0; v < N / 4; ++v) {
+    const float4 t = *reinterpret_cast<const float4*>(src + 4 * v);
+    r[4 * v] = __float_as_uint(t.x);
+    r[4 * v + 1] = __float_as_uint(t.y);
+    r[4 * v + 2] = __float_as_uint(t.z);
+    r[4 * v + 3] = __float_as_uint(t.w);
+  }
+}
 
-// ES = number of epilogue warp SETS (each set = 4 warps covering the 4 TMEM lane quarters).  ES = 1 is the validated
-// configuration; with ES = 2 (384-thread variant of the CTA-pair kernel, tuning key 10, round-2 candidate) set `es` handles
-// the 64-column pairs jp with jp % 2 == es, so two warps per scheduler drain the accumulator.
-template <int BN, int ES = 1, bool TAIL = false>
-__device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t tmem_base, int acc_col, int ew, int lane,
-                                              int n0, int y0, int x0, int n_idx, int split, int m_idx, float* stat_smem,
-                                              int es_arg = 0, int phase = 0, int tail_role = 0, int tail_slot = 0, int tail_np = 0) {
-  // tail_role (CTA-pair kernel only): 0 = ordinary tile; 1 = a K part >= 1 of a tail-split tile: the raw fp32 accumulator goes
-  // to p.tail_buf slot tail_slot, then the warp raises its flag; 2 = part 0 (the owner): waits for the flags of slots
-  // tail_slot .. tail_slot + tail_np - 1, adds those partial tiles to its accumulator in a fixed order and carries on with the
-  // normal epilogue (bias, residual, fp16 store, GroupNorm partials): the consumers cannot tell a tail-split tile from another.
+// Epilogue of one (128-row x BN-column) pass of an accumulator tile staged in shared memory (`acc`, pitch BN + ACC_PAD):
+// + bias (+ residual) -> fp16 rows (out_mode 0), fp32 split-K partials (out_mode 2) or fp32 NCHW (out_mode 1).  `cbase` is
+// the output column of staged column 0.
+//
+// A thread owns one accumulator ROW, so storing straight from registers makes every warp store touch 32 different cache
+// lines with 16 bytes each (and every residual load likewise): with short K loops (the attention qkv / proj GEMMs, 12..24
+// chunks) that epilogue, not the tensor core, sets the pace.  The fp16 / split-K paths therefore go through a per-warp
+// shared-memory transpose (32 rows x 128 B, 16-byte pieces XOR-swizzled by the row): registers -> smem by row, smem -> global
+// with 8 lanes per row, i.e. 4 complete 128-byte lines per store instruction; the residual comes in the same way (coalesced
+// load -> smem -> own row), the bias is read as broadcast LDS.128 from a per-warp copy, and the fused GroupNorm statistics
+// are column sums over the staged fp16 tile.
+template <int BN, int ES>
+__device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, const float* acc, int ew, int lane, int n0, int y0,
+                                              int x0, int cbase, int split, int m_idx, float* stat_smem, int es_arg,
+                                              int phase) {
   const int es = (ES == 1) ? 0 : es_arg;
   const int row = ew * 32 + lane;
   const int thw = p.TH * p.TW;
-  constexpr int CH = (BN >= 32) ? 32 : 16;  // columns per tcgen05.ld
+  constexpr int CH = (BN >= 32) ? 32 : 16;  // columns per staged-accumulator read
+  const float* arow = acc + row * (BN + ACC_PAD);  // this thread's accumulator row
       const int tn = row / thw;
       const int rem = row - tn * thw;
       const int th = rem / p.TW;
@@ -111,20 +128,18 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
 #pragma unroll
           for (int i = 0; i < 8; ++i) pix[i] = __shfl_sync(0xffffffffu, my_pix, i * 4 + sub);
           const uint32_t own = stage + lane * 128;
-          const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + static_cast<uint32_t>(acc_col);
           if (p.out_mode == 2) {
             // split-K: raw fp32 partial sums [split][M][Cout] (bias / residual / statistics in the finalize pass)
             float* wsb = p.ws + static_cast<long long>(split) * p.M_total * p.Cout;
 #pragma unroll 1
             for (int j = 0; j < BN / 32; ++j) {
-              const int col0 = n_idx * BN + j * 32;
+              const int col0 = cbase + j * 32;
               if (col0 >= p.Cout) break;
               if constexpr (ES > 1) {
                 if ((j % ES) != es) continue;
               }
               uint32_t r[32];
-              tmem_ld_32x32b_x32(taddr0 + j * 32, r);
-              tmem_ld_wait();
+              acc_ld(arow + j * 32, r);
 #pragma unroll
               for (int v = 0; v < 8; ++v)
                 sts_v4(own + ((v ^ (lane & 7)) << 4), r[v * 4], r[v * 4 + 1], r[v * 4 + 2], r[v * 4 + 3]);
@@ -141,52 +156,16 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
             return;
           }
           constexpr int NP = BN / 64;
-          if (TAIL && tail_role == 1) {
-            // accumulator order: float4 (jp, q) of row r at [(jp * 16 + q) * 128 + r] -- a warp stores / loads 512 contiguous bytes
-            float4* buf = reinterpret_cast<float4*>(p.tail_buf) + static_cast<long long>(tail_slot) * (32 * BN);
-#pragma unroll 1
-            for (int jp = 0; jp < NP; ++jp) {
-              if (n_idx * BN + jp * 64 >= p.Cout || (ES > 1 && (jp % ES) != es)) continue;
-              uint32_t r[64];
-              {
-                uint32_t(&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-                uint32_t(&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-                tmem_ld_32x32b_x32(taddr0 + jp * 64, r0);
-                tmem_ld_32x32b_x32(taddr0 + jp * 64 + 32, r1);
-                tmem_ld_wait();
-              }
-#pragma unroll
-              for (int q = 0; q < 16; ++q)
-                __stcg(buf + (jp * 16 + q) * 128 + row, make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]),
-                                                                   __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3])));
-            }
-            __threadfence();
-            __syncwarp();
-            if (lane == 0) st_release_gpu(p.tail_flags + tail_slot * 8 + es * 4 + ew, 1u);
-            return;
-          }
-          if (TAIL && tail_role == 2) {
-            if (lane == 0) {
-              for (int pt = 0; pt < tail_np; ++pt) {
-                const unsigned int* flag = p.tail_flags + (tail_slot + pt) * 8 + es * 4 + ew;
-                const long long t0 = clock64();
-                while (ld_acquire_gpu(flag) == 0u) {
-                  if (clock64() - t0 > 4000000000LL) __trap();  // a scheduling bug traps instead of hanging the GPU
-                }
-              }
-            }
-            __syncwarp();
-          }
           if (p.bias) {
 #pragma unroll
-            for (int c = lane; c < BN; c += 32) bsm[c] = (n_idx * BN + c < p.Cout) ? __ldg(p.bias + n_idx * BN + c) : 0.f;
+            for (int c = lane; c < BN; c += 32) bsm[c] = (cbase + c < p.Cout) ? __ldg(p.bias + cbase + c) : 0.f;
             __syncwarp();
           }
           __half* outb = reinterpret_cast<__half*>(p.out);
           float4 st[NP];   // fused GroupNorm statistics of this warp's 32 rows: (sum, sumsq) of columns 2l, 2l+1 per pair
           uint4 rpre[8];   // residual of the NEXT 64-column pair, in flight while the current one is processed
           auto load_res = [&](int jp) {
-            const int c0 = n_idx * BN + jp * 64;
+            const int c0 = cbase + jp * 64;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               rpre[i] = make_uint4(0u, 0u, 0u, 0u);
@@ -199,7 +178,7 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
           }
 #pragma unroll
           for (int jp = 0; jp < NP; ++jp) {
-            const int col0 = n_idx * BN + jp * 64;
+            const int col0 = cbase + jp * 64;
             st[jp] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (col0 < p.Cout && (ES == 1 || (jp % ES) == es)) {
               if constexpr (ES > 1) {
@@ -214,35 +193,9 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
                 __syncwarp();
               }
               uint32_t r[64];
-              {
-                uint32_t(&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-                uint32_t(&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-                tmem_ld_32x32b_x32(taddr0 + jp * 64, r0);
-                tmem_ld_32x32b_x32(taddr0 + jp * 64 + 32, r1);
-                if constexpr (ES == 1) {
-                  if (p.residual && jp + 1 < NP) load_res(jp + 1);
-                }
-                tmem_ld_wait();
-              }
-              if (TAIL && tail_role == 2) {
-                for (int pt = 0; pt < tail_np; ++pt) {
-                  const float4* buf = reinterpret_cast<const float4*>(p.tail_buf) + static_cast<long long>(tail_slot + pt) * (32 * BN);
-#pragma unroll
-                  for (int q0 = 0; q0 < 16; q0 += 4) {  // four loads in flight at a time: 16 registers, not 64
-                    float4 t[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) t[u] = __ldcg(buf + (jp * 16 + q0 + u) * 128 + row);
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                      const int q = q0 + u;
-                      r[4 * q] = __float_as_uint(__uint_as_float(r[4 * q]) + t[u].x);
-                      r[4 * q + 1] = __float_as_uint(__uint_as_float(r[4 * q + 1]) + t[u].y);
-                      r[4 * q + 2] = __float_as_uint(__uint_as_float(r[4 * q + 2]) + t[u].z);
-                      r[4 * q + 3] = __float_as_uint(__uint_as_float(r[4 * q + 3]) + t[u].w);
-                    }
-                    asm volatile("" ::: "memory");
-                  }
-                }
+              acc_ld(arow + jp * 64, r);
+              if constexpr (ES == 1) {
+                if (p.residual && jp + 1 < NP) load_res(jp + 1);
               }
 #pragma unroll
               for (int v = 0; v < 8; ++v) {  // 8 columns = one 16-byte piece of the staged row
@@ -311,11 +264,6 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
               __syncwarp();
             }
           }
-          if (TAIL && tail_role == 2) {  // every partial of this warp's rows has been read: the flags are zero again for the next launch
-            __syncwarp();
-            if (lane == 0)
-              for (int pt = 0; pt < tail_np; ++pt) p.tail_flags[(tail_slot + pt) * 8 + es * 4 + ew] = 0u;
-          }
           if (p.gn_part && p.gn_mode == 1) {
             // one partial per (M tile, column): the four warps' sums are folded in a fixed order through the (now idle)
             // staging buffers, so k2_gn_finalize reads a quarter of what per-warp partials would cost
@@ -325,7 +273,7 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
               for (int jp = 0; jp < NP; ++jp) mine[jp * 32 + lane] = st[jp];
               named_bar_sync(1, 128);
               if (ew < NP) {
-                const int col0 = n_idx * BN + ew * 64;
+                const int col0 = cbase + ew * 64;
                 if (col0 < p.Cout) {
                   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -345,7 +293,7 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
               named_bar_sync(1 + es, 128);
               const int jp_f = es + ew * ES;  // warp ew of the set folds the set's ew-th pair
               if (jp_f < NP) {
-                const int col0 = n_idx * BN + jp_f * 64;
+                const int col0 = cbase + jp_f * 64;
                 if (col0 < p.Cout) {
                   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -365,16 +313,9 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
       }
 #pragma unroll 1
       for (int j = 0; j < BN / CH; ++j) {
-        const uint32_t taddr =
-            tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + static_cast<uint32_t>(acc_col + j * CH);
         uint32_t r[CH];
-        if constexpr (CH == 32) {
-          tmem_ld_32x32b_x32(taddr, r);
-        } else {
-          tmem_ld_32x32b_x16(taddr, r);
-        }
-        tmem_ld_wait();
-        const int col0 = n_idx * BN + j * CH;
+        acc_ld(arow + j * CH, r);
+        const int col0 = cbase + j * CH;
         if (valid && col0 < p.Cout) {
           if (p.out_mode == 2) {
             // split-K: raw fp32 partial sums [split][M][Cout] into the workspace (bias/residual in the finalize pass)
@@ -443,54 +384,45 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, uint32_t 
       }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(256, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
-  using C = Cfg<BN>;
+
+template <int BN, int ES>
+__global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
+  using C = Cfg<BN, ES>;
+  constexpr int BNC = C::BNC;
+  constexpr int NJ = (BN >= 64) ? BN / 64 : 1;  // wgmma instructions per K step (N = 64 each, or one N = 16)
+  constexpr int NA = (BN >= 64) ? 32 : 8;       // accumulator registers per instruction
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  float* acc_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);
+  float* stat_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::ACC_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES + C::ACC_BYTES + ES * EPI_BYTES);
   uint64_t* empty_bar = full_bar + C::STAGES;
-  uint64_t* tmem_full = empty_bar + C::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* stat_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::BAR_BYTES);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = warp_idx >> 2;
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmB);
     for (int s = 0; s < 3; ++s)
       if (p.seg_taps[s]) tma_prefetch_desc(&p.tmA[s]);
-  }
-  if (warp_idx == 1 && lane == 0) {
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);  // one arrival per epilogue warp
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp, after its wgmma.wait_group
     }
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc(tmem_ptr, C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_wait();
   pdl_launch();
 
   const int total_tiles = p.m_tiles * p.n_tiles * p.splits;
 
-  if (warp_idx == 0) {
+  if (wg == 0) {
     // ===================================== TMA producer =====================================
-    if (elect_one()) {  // one lane, and ptxas KNOWS it is one: UTCHMMA / UTMALDG operands need no per-lane waterfall loop
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && elect_one()) {
       int stage = 0;
       uint32_t ring_phase = 0;
       const uint32_t tx_bytes = p.a_box_bytes + C::B_STAGE_BYTES;
@@ -515,7 +447,7 @@ __global__ void __launch_bounds__(256, 1) conv_gemm_kernel(const __grid_constant
           const int taps = p.seg_taps[s];
           const int dy = (taps == 9) ? (tap / 3 - 1) : (taps == 4 ? (tap >> 1) + (phase >> 1) - 1 : 0);
           const int dx = (taps == 9) ? (tap % 3 - 1) : (taps == 4 ? (tap & 1) + (phase & 1) - 1 : 0);
-          mbar_wait(&empty_bar[stage], ring_phase ^ 1);
+          mbar_wait_lean(&empty_bar[stage], ring_phase ^ 1);
           uint8_t* sA = smem + stage * C::STAGE_BYTES;
           uint8_t* sB = sA + A_STAGE_BYTES;
           mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
@@ -535,557 +467,80 @@ __global__ void __launch_bounds__(256, 1) conv_gemm_kernel(const __grid_constant
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ===================================== MMA issuer ========================================
-    if (elect_one()) {  // one lane, and ptxas KNOWS it is one: UTCHMMA / UTMALDG operands need no per-lane waterfall loop
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        const int split = tile / (p.m_tiles * p.n_tiles);
-        const int nk = min(p.num_k_chunks, (split + 1) * p.k_per_split) - split * p.k_per_split;
-        for (int kc = 0; kc < nk; ++kc) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint64_t adesc = make_sw128_desc(a_addr);
-          const uint64_t bdesc = make_sw128_desc(a_addr + A_STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // +32 bytes (2 x 16 B units) per 16-element K step inside the 128 B swizzle row
-            umma_f16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
-                     idesc, (kc | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot free once these MMAs retire
-          if (++stage == C::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator ready for the epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp_idx >= 4) {
-    // ===================================== epilogue ==========================================
-    const int ew = warp_idx - 4;  // == warp_idx % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    int acc = 0;
-    uint32_t acc_phase = 0;
+  } else {
+    // ============================ wgmma consumers + epilogue ================================
+    setmaxnreg_inc<232>();
+    const int g = wg - 1;          // accumulator rows [64 g, 64 g + 64)
+    const int w = warp_idx & 3;    // warp of the warpgroup: rows 16 w .. 16 w + 15 of the warpgroup's 64
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int m_idx = tile % p.m_tiles;
       const int n_idx = (tile / p.m_tiles) % p.n_tiles;
       const int split = tile / (p.m_tiles * p.n_tiles);
-      int n0, y0, x0, phase;
-      decode_m_tile(p, m_idx, n0, y0, x0, phase);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      epilogue_tile<BN>(p, tmem_base, acc * BN, ew, lane, n0, y0, x0, n_idx, split, m_idx, stat_smem, 0, phase);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// 2-CTA variant (tcgen05 cta_group::2): a CTA PAIR of one cluster computes a (256 pixel x BN channel) tile.
-// CTA r of the pair owns M tile 2*pair+r: it loads ITS 128-row A box and HALF of the weight tile (BN/2 rows) per
-// K chunk, so the pair pulls 32 KB + BN*128 B per chunk from L2 instead of 2 x (16 KB + BN*128 B) -- the 1-CTA
-// kernel is L2->SM bandwidth bound at ~96 B/clk/SM.  The leader CTA (rank 0) issues the M=256 MMAs, which read both
-// CTAs' shared memory and write each CTA's own TMEM; every TMA of the pair signals the LEADER's full barrier; the
-// MMA commit multicasts the "stage free" / "accumulator ready" arrivals to both CTAs; the peer's epilogue warps arrive
-// remotely on the leader's "accumulator drained" barrier.
-// ------------------------------------------------------------------------------------------------
-template <int BN, int ES = 1>
-struct Cfg2 {
-  static constexpr int B_STAGE_BYTES = (BN / 2) * BK * 2;   // this CTA's half of the weight tile
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // the second epilogue warp set's staging / bias buffers (another EPI_BYTES) cost one pipeline stage
-  static constexpr int STAGES = ((BN >= 256) ? 6 : (BN >= 192 ? 7 : 8)) - (ES - 1);
-  static constexpr int TMEM_COLS = 512;                      // 2 accumulator buffers at columns 0 and 256
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + ES * EPI_BYTES + 1024;
-  static constexpr int THREADS = 128 + 128 * ES;             // 4 control warps + ES sets of 4 epilogue warps
-};
-
-// TAIL: the launch uses the tail split (stream-K over the last partial wave); a separate instantiation, so that the default
-// kernels stay instruction-for-instruction what they were before the feature existed.
-template <int BN, int ES = 1, bool TAIL = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128 + 128 * ES, 1)
-conv_gemm2_kernel(const __grid_constant__ ConvGemmParams p) {
-  using C = Cfg2<BN, ES>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::STAGES;
-  uint64_t* tmem_full = empty_bar + C::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* stat_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 256);
-
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmB);
-    for (int s = 0; s < 3; ++s)
-      if (p.seg_taps[s]) tma_prefetch_desc(&p.tmA[s]);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);   // leader: one arrive.expect_tx covering BOTH CTAs' bytes
-      mbar_init(&empty_bar[i], 1);  // one multicast commit per use
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8 * ES);  // 4 epilogue warps per set x 2 CTAs (only the leader's copy is waited on)
-    }
-    fence_barrier_init();
-  }
-  if (warp_idx == 2) {
-    tmem_alloc2(tmem_ptr, C::TMEM_COLS);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();  // barriers of both CTAs initialised before any remote arrival / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  pdl_wait();
-  pdl_launch();
-
-  const int m_pairs = (p.m_tiles + 1) >> 1;
-  // Work items of this launch: the tiles (x split-K parts), or -- tail split -- the tiles of the full waves followed by ONE
-  // more wave in which the K loops of the remaining tail_count tiles, laid end to end (tail_count x num_k_chunks chunks), are
-  // cut into equal spans of tail_kps chunks, one span per CTA pair (stream-K over the last wave only).  A span covers the
-  // end of one tile and possibly the start of the next: up to two sub-items per pair (items tail_first + pair and
-  // tail_first + num_pairs + pair).  The sub-item holding a tile's first chunk owns the tile (part 0); it is always the
-  // LAST thing its pair does, and it only waits for sub-items that are the FIRST thing their pairs do in this wave: no cycles.
-  const int total_tiles = TAIL ? p.tail_first + 2 * num_pairs : m_pairs * p.n_tiles * p.splits;
-  // -> false: an empty sub-item (all three roles skip it); part < 0: ordinary item; nparts = K parts of the tile
-  auto decode_item = [&](int item, int& tile, int& part, int& nparts, int& split, int& k0, int& k1) -> bool {
-    if (TAIL && item >= p.tail_first) {
-      const int idx = item - p.tail_first;
-      const int sub = idx / num_pairs, i = idx - sub * num_pairs;
-      const int nk = p.num_k_chunks, L = p.tail_kps;
-      const int g0 = i * L, g1 = min(g0 + L, p.tail_count * nk);
-      if (g0 >= g1) return false;
-      int ta = g0 / nk;
-      const int ka0 = g0 - ta * nk, ka1 = min(nk, ka0 + (g1 - g0));
-      if (sub == 0) {
-        k0 = ka0;
-        k1 = ka1;
-      } else {
-        const int rest = (g1 - g0) - (ka1 - ka0);
-        if (rest <= 0) return false;
-        ++ta;
-        k0 = 0;
-        k1 = rest;
-      }
-      const int first_span = (ta * nk) / L;
-      const int last_span = min(((ta + 1) * nk - 1) / L, (p.tail_count * nk - 1) / L);
-      part = i - first_span;
-      nparts = last_span - first_span + 1;
-      tile = p.tail_first + ta;
-      split = 0;
-      return true;
-    }
-    tile = item;
-    part = -1;
-    nparts = 1;
-    split = tile / (m_pairs * p.n_tiles);
-    k0 = split * p.k_per_split;
-    k1 = min(p.num_k_chunks, k0 + p.k_per_split);
-    return true;
-  };
-
-  if (warp_idx == 0) {
-    // ===================================== TMA producer (both CTAs) ==========================
-    if (elect_one()) {  // one lane, and ptxas KNOWS it is one: UTCHMMA / UTMALDG operands need no per-lane waterfall loop
-      int stage = 0;
-      uint32_t ring_phase = 0;
-      const uint32_t tx_bytes = 2u * (p.a_box_bytes + C::B_STAGE_BYTES);
-      for (int item = pair; item < total_tiles; item += num_pairs) {
-        int tile, part, nparts, split, k0, k1;
-        if (!decode_item(item, tile, part, nparts, split, k0, k1)) continue;
-        const int m_idx = (tile % m_pairs) * 2 + static_cast<int>(rank);
-        const int n_idx = (tile / m_pairs) % p.n_tiles;
-        int n0, y0, x0, phase;
-        decode_m_tile(p, m_idx, n0, y0, x0, phase);  // m_idx == m_tiles (odd tail): n0 >= NB -> the box is all zero-fill
-        const int kb = phase * p.num_k_chunks;  // up2: each phase has its own 4-tap weight block
-        int s = 0, rem = k0;
-        while (rem >= p.seg_taps[s] * p.seg_kchunks[s]) {
-          rem -= p.seg_taps[s] * p.seg_kchunks[s];
-          ++s;
-        }
-        int tap = rem / p.seg_kchunks[s];
-        int c = rem - tap * p.seg_kchunks[s];
-        for (int kc = k0; kc < k1; ++kc) {
-          const int taps = p.seg_taps[s];
-          const int dy = (taps == 9) ? (tap / 3 - 1) : (taps == 4 ? (tap >> 1) + (phase >> 1) - 1 : 0);
-          const int dx = (taps == 9) ? (tap % 3 - 1) : (taps == 4 ? (tap & 1) + (phase & 1) - 1 : 0);
-          mbar_wait(&empty_bar[stage], ring_phase ^ 1);
-          uint8_t* sA = smem + stage * C::STAGE_BYTES;
-          uint8_t* sB = sA + A_STAGE_BYTES;
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          tma2_load_4d(sA, &p.tmA[s], &full_bar[stage], c * BK, x0 + dx, y0 + dy, n0);
-          tma2_load_3d(sB, &p.tmB, &full_bar[stage], (kb + kc) * BK, n_idx * BN + static_cast<int>(rank) * (BN / 2),
-                       p.w_batched ? n0 : 0);
-          if (++stage == C::STAGES) {
-            stage = 0;
-            ring_phase ^= 1;
-          }
-          if (++c == p.seg_kchunks[s]) {
-            c = 0;
-            if (++tap == taps) {
-              tap = 0;
-              ++s;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp_idx == 1) {
-    // ===================================== MMA issuer (leader CTA only) ======================
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_f16(256, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = pair; item < total_tiles; item += num_pairs) {
-        int tile, part, nparts, split, k0, k1;
-        if (!decode_item(item, tile, part, nparts, split, k0, k1)) continue;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * 256);
-        const int nk = k1 - k0;
-        for (int kc = 0; kc < nk; ++kc) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint64_t adesc = make_sw128_desc(a_addr);
-          const uint64_t bdesc = make_sw128_desc(a_addr + A_STAGE_BYTES);
+      const int nk = min(p.num_k_chunks, (split + 1) * p.k_per_split) - split * p.k_per_split;
+      float acc[NJ][NA];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma2_f16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc,
-                      (kc | k) != 0 ? 1u : 0u);
-          umma2_commit_mc(&empty_bar[stage], 0x3);  // the stage is free in BOTH CTAs once these MMAs retire
-          if (++stage == C::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma2_commit_mc(&tmem_full[acc], 0x3);  // each CTA's accumulator half is ready for its epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp_idx >= 4) {
-    // ===================================== epilogue (both CTAs, own TMEM) ====================
-    const int ew = (ES == 1) ? warp_idx - 4 : (warp_idx & 3);  // TMEM lane quarter
-    const int es = (ES == 1) ? 0 : ((warp_idx - 4) >> 2);       // epilogue warp set
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t leader_empty0 = mapa_u32(smem_u32(&tmem_empty[0]), 0);
-    const uint32_t leader_empty1 = mapa_u32(smem_u32(&tmem_empty[1]), 0);
-    for (int item = pair; item < total_tiles; item += num_pairs) {
-      int tile, part, nparts, split, k0, k1;
-      if (!decode_item(item, tile, part, nparts, split, k0, k1)) continue;
-      const int m_idx = (tile % m_pairs) * 2 + static_cast<int>(rank);
-      const int n_idx = (tile / m_pairs) % p.n_tiles;
-      int n0, y0, x0, phase;
-      decode_m_tile(p, m_idx, n0, y0, x0, phase);
-      // tail split: (tail_split - 1) hand-over slots per CTA half of a tail tile, one per K part >= 1
-      const int tail_role = (part < 0 || nparts == 1) ? 0 : (part > 0 ? 1 : 2);
-      const int tail_slot = (part < 0) ? 0 : ((tile - p.tail_first) * 2 + static_cast<int>(rank)) * (p.tail_split - 1) + max(part - 1, 0);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      epilogue_tile<BN, ES, TAIL>(p, tmem_base, acc * 256, ew, lane, n0, y0, x0, n_idx, split, m_idx, stat_smem, es, phase,
-                                  tail_role, tail_slot, nparts - 1);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(acc ? leader_empty1 : leader_empty0);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // the peer's smem / TMEM must outlive every MMA of the pair
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, C::TMEM_COLS);
-  }
-}
-
-template <int BN, int ES, bool TAIL>
-int launch_pair(const ConvGemmParams& p, cudaStream_t stream) {
-  using C = Cfg2<BN, ES>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm2_kernel<BN, ES, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set = true;
-  }
-  const int m_pairs = (p.m_tiles + 1) / 2;
-  const int total = m_pairs * p.n_tiles * p.splits;
-  const int max_pairs = num_sms() / 2;
-  const int pairs = (TAIL || total >= max_pairs) ? max_pairs : total;  // tail split: one K span per CTA pair of the device
-  K2_CHECK_CUDA(launch_k(conv_gemm2_kernel<BN, ES, TAIL>, dim3(2 * pairs), dim3(C::THREADS), C::SMEM_BYTES, stream, p));
-  return 0;
-}
-template <int BN>
-int launch_bn2(const ConvGemmParams& p, cudaStream_t stream) {
-  return p.tail_split > 1 ? launch_pair<BN, 1, true>(p, stream) : launch_pair<BN, 1, false>(p, stream);
-}
-// CTA-pair kernel with two epilogue warp sets (384 threads, one pipeline stage fewer); bit-identical to the one-set kernel
-// (tests/test_gpu_conv_gemm.py::test_two_epilogue_sets_bit_identical).
-template <int BN>
-int launch_bn2e(const ConvGemmParams& p, cudaStream_t stream) {
-  return p.tail_split > 1 ? launch_pair<BN, 2, true>(p, stream) : launch_pair<BN, 2, false>(p, stream);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Halo variant of the CTA-pair kernel for 3x3 convolutions: the 1-/2-CTA kernels above fetch the SAME activation
-// pixels nine times (one shifted 128-pixel box per tap), and L2->SM operand bandwidth (~64 B/clk/SM) is what bounds
-// them.  Here an M tile is 8 wide x 16 high and ONE (8+2) x (16+2) halo box per 64-channel chunk is staged in shared
-// memory; the nine taps are nine tcgen05 A descriptors into that box: a row of 8 output pixels is 8 consecutive 128 B
-// halo rows (one 8-row core group), the next output row starts `pitch` halo pixels later, so the stride between core
-// groups is pitch*128 B and tap (dy, dx) only moves the start address by ((1+dy)*pitch + 1+dx)*128 B.  Activation
-// traffic per chunk drops from 9 x 16 KB to one box; the weight tiles (one per tap) are unchanged.
-// ------------------------------------------------------------------------------------------------
-template <int BN>
-struct Cfg3 {
-  static constexpr int A_STAGE = 36864;                    // 18 rows x (up to) 16 pixels x 128 B
-  static constexpr int A_STAGES = 3;
-  static constexpr int B_STAGE = (BN / 2) * BK * 2;
-  static constexpr int B_STAGES = (BN >= 256) ? 4 : 5;
-  static constexpr int BAR_OFF = A_STAGES * A_STAGE + B_STAGES * B_STAGE;
-  static constexpr int STAT_OFF = BAR_OFF + 256;
-  static constexpr int SMEM_BYTES = STAT_OFF + EPI_BYTES + 1024;
-};
-
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
-conv_gemm3_kernel(const __grid_constant__ ConvGemmParams p) {
-  using C = Cfg3<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smemB = smem + C::A_STAGES * C::A_STAGE;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* a_empty = a_full + C::A_STAGES;
-  uint64_t* b_full = a_empty + C::A_STAGES;
-  uint64_t* b_empty = b_full + C::B_STAGES;
-  uint64_t* tmem_full = b_empty + C::B_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* stat_smem = reinterpret_cast<float*>(smem + C::STAT_OFF);
-
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-  const int pitch = p.halo_pitch;
-
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmB);
-    for (int s = 0; s < 3; ++s)
-      if (p.seg_taps[s]) tma_prefetch_desc(&p.tmA[s]);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    for (int i = 0; i < C::A_STAGES; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < C::B_STAGES; ++i) {
-      mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8);
-    }
-    fence_barrier_init();
-  }
-  if (warp_idx == 2) {
-    tmem_alloc2(tmem_ptr, 512);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  pdl_wait();
-  pdl_launch();
-
-  const int m_pairs = (p.m_tiles + 1) >> 1;
-  const int total_tiles = m_pairs * p.n_tiles;
-
-  if (warp_idx == 0) {
-    // ===================================== TMA producer (both CTAs) ==========================
-    if (elect_one()) {  // one lane, and ptxas KNOWS it is one: UTCHMMA / UTMALDG operands need no per-lane waterfall loop
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      const uint32_t halo_bytes = static_cast<uint32_t>(18 * pitch * 128);
-      for (int tile = pair; tile < total_tiles; tile += num_pairs) {
-        const int m_idx = (tile % m_pairs) * 2 + static_cast<int>(rank);
-        const int n_idx = tile / m_pairs;
-        int n0, y0, x0, phase_unused;
-        decode_m_tile(p, m_idx, n0, y0, x0, phase_unused);
-        int kc_base = 0;
-        for (int s = 0; s < 3; ++s) {
-          const int taps = p.seg_taps[s];
-          if (taps == 0) break;
-          const int kch = p.seg_kchunks[s];
-          for (int c = 0; c < kch; ++c) {
-            mbar_wait(&a_empty[as], aph ^ 1);
-            uint8_t* sA = smem + as * C::A_STAGE;
-            if (taps == 9) {
-              if (rank == 0) mbar_arrive_expect_tx(&a_full[as], 2u * halo_bytes);
-              tma2_load_4d(sA, &p.tmA[s], &a_full[as], c * BK, x0 - 1, y0 - 1, n0);
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < NA; ++i) acc[j][i] = 0.f;
+      int prev_stage = -1;
+      for (int kc = 0; kc < nk; ++kc) {
+        mbar_wait_lean(&full_bar[stage], phase);  // no printf call: wgmma stays pipelined across the wait
+        const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + g * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + A_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          // +32 bytes (2 x 16 B units) per 16-element K step inside the 128 B swizzle row
+          const uint64_t adesc = make_wgmma_desc(a_addr) + static_cast<uint64_t>(k * 2);
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) {
+            const uint64_t bdesc = make_wgmma_desc(b_addr + j * (64 * 128)) + static_cast<uint64_t>(k * 2);
+            if constexpr (BN >= 64) {
+              wgmma_m64n64k16(acc[j], adesc, bdesc, 1u);
             } else {
-              if (rank == 0) mbar_arrive_expect_tx(&a_full[as], 2u * A_STAGE_BYTES);
-              tma2_load_4d(sA, &p.tmA[s], &a_full[as], c * BK, x0, y0, n0);
-            }
-            if (++as == C::A_STAGES) {
-              as = 0;
-              aph ^= 1;
-            }
-            for (int tap = 0; tap < taps; ++tap) {
-              mbar_wait(&b_empty[bs], bph ^ 1);
-              if (rank == 0) mbar_arrive_expect_tx(&b_full[bs], 2u * C::B_STAGE);
-              tma2_load_3d(smemB + bs * C::B_STAGE, &p.tmB, &b_full[bs], (kc_base + tap * kch + c) * BK,
-                           n_idx * BN + static_cast<int>(rank) * (BN / 2), 0);
-              if (++bs == C::B_STAGES) {
-                bs = 0;
-                bph ^= 1;
-              }
+              wgmma_m64n16k16(acc[j], adesc, bdesc, 1u);
             }
           }
-          kc_base += taps * kch;
+        }
+        wgmma_commit();
+        // keep one K chunk in flight: the stage consumed by the previous chunk is free once only this one is pending
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == C::STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
       }
-    }
-  } else if (warp_idx == 1) {
-    // ===================================== MMA issuer (leader CTA only) ======================
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_f16(256, BN, 0, 0);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < total_tiles; tile += num_pairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * 256);
-        uint32_t first = 1;
-        for (int s = 0; s < 3; ++s) {
-          const int taps = p.seg_taps[s];
-          if (taps == 0) break;
-          const int kch = p.seg_kchunks[s];
-          for (int c = 0; c < kch; ++c) {
-            mbar_wait(&a_full[as], aph);
-            tc_fence_after();
-            const uint32_t a_base = smem_u32(smem + as * C::A_STAGE);
-            for (int tap = 0; tap < taps; ++tap) {
-              mbar_wait(&b_full[bs], bph);
-              tc_fence_after();
-              uint64_t adesc;
-              if (taps == 9) {
-                const uint32_t start = a_base + static_cast<uint32_t>(((tap / 3) * pitch + (tap % 3)) * 128);
-                adesc = make_sw128_desc_ex(start, static_cast<uint32_t>(pitch * 128), p.halo_bo ? (start >> 7) & 7u : 0u);
-              } else {
-                adesc = make_sw128_desc(a_base);
-              }
-              const uint64_t bdesc = make_sw128_desc(smem_u32(smemB + bs * C::B_STAGE));
+      wgmma_wait<0>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);  // an empty K range consumed no stage
+
+      int n0, y0, x0, mphase;
+      decode_m_tile(p, m_idx, n0, y0, x0, mphase);
+      const int r0 = 64 * g + 16 * w + (lane >> 2);
+      const int cq = 2 * (lane & 3);
 #pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                umma2_f16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc,
-                          (first && k == 0) ? 0u : 1u);
-              }
-              first = 0;
-              umma2_commit_mc(&b_empty[bs], 0x3);
-              if (++bs == C::B_STAGES) {
-                bs = 0;
-                bph ^= 1;
-              }
-            }
-            umma2_commit_mc(&a_empty[as], 0x3);
-            if (++as == C::A_STAGES) {
-              as = 0;
-              aph ^= 1;
-            }
+      for (int pass = 0; pass < BN / BNC; ++pass) {
+        named_bar_sync(3, 256);  // the staged tile of the previous pass / tile has been read
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          if (BN >= 64 && (j * 64) / BNC != pass) continue;
+#pragma unroll
+          for (int i = 0; i < NA; i += 2) {
+            const int row = r0 + 8 * ((i >> 1) & 1);
+            const int col = (BN >= 64 ? j * 64 - pass * BNC : 0) + 8 * (i >> 2) + cq;
+            *reinterpret_cast<float2*>(acc_smem + row * (BNC + ACC_PAD) + col) = make_float2(acc[j][i], acc[j][i + 1]);
           }
         }
-        umma2_commit_mc(&tmem_full[acc], 0x3);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
+        named_bar_sync(3, 256);  // staged tile complete
+        if (ES == 2 || g == 0)
+          epilogue_tile<BNC, ES>(p, acc_smem, w, lane, n0, y0, x0, n_idx * BN + pass * BNC, split, m_idx, stat_smem, g,
+                                 mphase);
       }
     }
-  } else if (warp_idx >= 4) {
-    // ===================================== epilogue (both CTAs, own TMEM) ====================
-    const int ew = warp_idx - 4;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t leader_empty0 = mapa_u32(smem_u32(&tmem_empty[0]), 0);
-    const uint32_t leader_empty1 = mapa_u32(smem_u32(&tmem_empty[1]), 0);
-    for (int tile = pair; tile < total_tiles; tile += num_pairs) {
-      const int m_idx = (tile % m_pairs) * 2 + static_cast<int>(rank);
-      const int n_idx = tile / m_pairs;
-      int n0, y0, x0, phase_unused;
-      decode_m_tile(p, m_idx, n0, y0, x0, phase_unused);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      epilogue_tile<BN>(p, tmem_base, acc * 256, ew, lane, n0, y0, x0, n_idx, 0, m_idx, stat_smem);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(acc ? leader_empty1 : leader_empty0);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, 512);
-  }
-}
-
-template <int BN>
-int launch_bn3(const ConvGemmParams& p, cudaStream_t stream) {
-  using C = Cfg3<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set = true;
-  }
-  const int m_pairs = (p.m_tiles + 1) / 2;
-  const int total = m_pairs * p.n_tiles;
-  const int max_pairs = num_sms() / 2;
-  const int pairs = total < max_pairs ? total : max_pairs;
-  K2_CHECK_CUDA(launch_k(conv_gemm3_kernel<BN>, dim3(2 * pairs), dim3(256), C::SMEM_BYTES, stream, p));
-  return 0;
 }
 
 // split-K second pass: out[m, n] = fp16( sum_s ws[s][m][n] (fixed order) + bias[n] + residual[m, n] ).
@@ -1162,18 +617,19 @@ __global__ void __launch_bounds__(256) splitk_finalize_kernel(const float* __res
   }
 }
 
-template <int BN>
+
+template <int BN, int ES>
 int launch_bn(const ConvGemmParams& p, cudaStream_t stream) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, ES>;
   static bool attr_set = false;
   if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, ES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        C::SMEM_BYTES));
     attr_set = true;
   }
   int total = p.m_tiles * p.n_tiles * p.splits;
   int grid = total < num_sms() ? total : num_sms();
-  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN>, dim3(grid), dim3(256), C::SMEM_BYTES, stream, p));
+  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN, ES>, dim3(grid), dim3(384), C::SMEM_BYTES, stream, p));
   return 0;
 }
 
@@ -1188,36 +644,19 @@ int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, c
 }
 
 int launch_conv_gemm(const ConvGemmParams& p, int BN, int epilogue_sets, cudaStream_t stream) {
-  if (p.halo_pitch) {
+  if (epilogue_sets == 2) {  // both consumer warpgroups drain the accumulator: short-K GEMMs are epilogue-paced
     switch (BN) {
-      case 128: return launch_bn3<128>(p, stream);
-      case 192: return launch_bn3<192>(p, stream);
-      case 256: return launch_bn3<256>(p, stream);
-      default: return fail("conv_gemm: unsupported BN for the halo kernel");
-    }
-  }
-  if (p.two_cta && epilogue_sets == 2) {  // two epilogue warp sets (384 threads): short-K GEMMs are epilogue-paced
-    switch (BN) {
-      case 128: return launch_bn2e<128>(p, stream);
-      case 192: return launch_bn2e<192>(p, stream);
-      case 256: return launch_bn2e<256>(p, stream);
-      default: return fail("conv_gemm: unsupported BN for the 2-CTA kernel");
-    }
-  }
-  if (p.two_cta) {
-    switch (BN) {
-      case 128: return launch_bn2<128>(p, stream);
-      case 192: return launch_bn2<192>(p, stream);
-      case 256: return launch_bn2<256>(p, stream);
-      default: return fail("conv_gemm: unsupported BN for the 2-CTA kernel");
+      case 128: return launch_bn<128, 2>(p, stream);
+      case 256: return launch_bn<256, 2>(p, stream);
+      default: break;  // N tile 192 stages 64 columns per pass: a second set would have nothing to drain
     }
   }
   switch (BN) {
-    case 16: return launch_bn<16>(p, stream);
-    case 64: return launch_bn<64>(p, stream);
-    case 128: return launch_bn<128>(p, stream);
-    case 192: return launch_bn<192>(p, stream);
-    case 256: return launch_bn<256>(p, stream);
+    case 16: return launch_bn<16, 1>(p, stream);
+    case 64: return launch_bn<64, 1>(p, stream);
+    case 128: return launch_bn<128, 1>(p, stream);
+    case 192: return launch_bn<192, 1>(p, stream);
+    case 256: return launch_bn<256, 1>(p, stream);
     default: return fail("conv_gemm: unsupported BN");
   }
 }

@@ -73,45 +73,31 @@ struct ConvGemmParams {
   int k_per_split;     // K chunks per split
   float* ws;           // [splits][M_total][Cout] fp32 partial sums (out_mode 2)
   long long M_total;
-  int two_cta;         // 1: CTA-pair kernel (cta_group::2, 256-row tiles)
   float2* gn_part;     // fused GroupNorm partials (sum, sumsq) of the fp16-rounded output, or null:
   int gn_mode;         //   1: [m_tiles][Cout], one per M tile (TN == 1); 2: [image][spatial tile][Cout] for 16-pixel x 8-image tiles
   int up2;             // 1: source 0 has taps == 4: 3x3 conv over the nearest-2x upsampled source as four 2x2 phase convs;
                        //    NB/H/W and the tile box are SOURCE geometry, outputs go to pixel (2y + a, 2x + b) of a 2H x 2W image
-  int m_tiles_phase;   // up2: tile slots per phase (m_tiles = 4 * m_tiles_phase; even in CTA-pair mode so a pair never
-                       //    straddles two phases -- its two boxes share one weight tile)
-  int halo_pitch;      // 0: per-tap boxes; 10 / 16: halo kernel, pixels per halo row in shared memory
-  int halo_bo;         // halo kernel: 1 = put (start >> 7) & 7 into the descriptor's base-offset field
-  // Tail split (CTA-pair kernel, splits == 1) = stream-K over the last, partial wave: the K loops of tiles [tail_first,
-  // tail_first + tail_count) laid end to end are cut into spans of tail_kps chunks, one per CTA pair; the part holding a tile's
-  // first chunk (the owner) adds the other parts' fp32 accumulator tiles, handed over through tail_buf / tail_flags, before its
-  // normal epilogue.  tail_split <= 1: off; else tail_split - 1 = hand-over slots per CTA half of a tile.
-  int tail_first, tail_count, tail_split, tail_kps;
-  float* tail_buf;            // [tile - tail_first][CTA rank][part - 1][128 x BN] fp32, accumulator (column-quad, row) order
-  unsigned int* tail_flags;   // [...same...][8 epilogue warps]: 1 = that warp's rows of the part are in tail_buf; zero between launches
+  int m_tiles_phase;   // up2: tile slots per phase (m_tiles = 4 * m_tiles_phase)
 };
 int launch_conv_gemm(const ConvGemmParams& p, int BN, int epilogue_sets, cudaStream_t stream);
 int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, const float* bias, const __half* residual,
                            int ldr, __half* out, int ldo, float2* gn_part, cudaStream_t stream);
 
-// ---- fused attention, head dim 64 (k2_attention.cu) ---------------------------------------------
-struct AttnParams {
-  CUtensorMap tmQKV;   // 3-D (channels, T, B) over the qkv rows, box (64, 128, 1)
-  CUtensorMap tmEnc;   // 3-D (channels, Tc, B) over the encoder kv rows, box (64, 128, 1)
+// ---- fused attention, head dim 64 / 512 (k2_attention.cu) ----------------------------------------
+struct FlashParams {
+  const __half* qkv;   // [B, T, ldq] rows; head h reads q / k / v at channels h*hs + {q,k,v}_off
+  long long ldq;
+  int hs, q_off, k_off, v_off;
+  const __half* enc;   // [B, Tc, lde] encoder rows (keys 0 .. Tc-1 come first), or null with Tc = 0
+  long long lde;
+  int ehs, ek_off, ev_off;
   int B, heads, T, Tc;
-  int hs, q_off, k_off, v_off;       // head h owns channels [h*hs, (h+1)*hs); q/k/v at these offsets
-  int ehs, ek_off, ev_off;           // same for the encoder kv rows
-  __half* out;         // [B, T, ldo], channel h*64+d
-  int ldo;
+  __half* out;         // [B, T, ldo], head h at channels h*ohs
+  int ldo, ohs;
   float scale_log2e;   // softmax scale * log2(e)
-  int stagger_cycles;  // tuning key 5 (default 0): delay of the second query tile's first score product; measured: no gain
-  unsigned long long* trace;  // diagnostics: 3 x 16 x 8 clock64 stamps of CTA (0,0,0), or null
 };
 int gn_apply_blocks_per_sm();  // tuning key 11: blocks per SM the GroupNorm apply kernels are sized for (0 = their occupancy)
-int attention_stagger();
-unsigned long long* attention_trace_buffer();
-int attention_half_rows();   // tuning key 9: 1 = 16 softmax warps with half a score row per thread, 0 = 8 warps, one row each
-int attention_poly_mode();  // eighths of the softmax exponentials evaluated without MUFU: 0, 2, 3, 4
-int launch_attention_d64(const AttnParams& p, cudaStream_t stream);
+int attention_half_rows();     // tuning key 9: 1 = 128 query rows per CTA (8 warps), 0 = 64 (4 warps)
+int launch_attention(const FlashParams& p, int head_dim, cudaStream_t stream);
 
 }  // namespace k2

@@ -5,10 +5,10 @@
 //       zq = interpolate(zq, size=f.shape[-2:], mode="nearest"); y = GroupNorm(f) * conv_y(zq) + conv_b(zq)   (+ swish, :21-23)
 //   AttnBlock's  v.reshape / permute before torch.bmm   movq_modules.py:216-219
 //
-// SpatialNorm is HBM-bound: one read and one write of the feature map (up to 604 MB per tensor at 768x768).  Round 1 ran it
-// through the generic gn_apply kernel, which re-derived the 2 x (4 -> C) modulation with 80 read-only loads per thread every
-// time the latent pixel under a thread changed: 1.16 TB/s, 38 % of the decode.  Here everything that does not depend on the
-// pixel is folded ONCE per thread into 10 coefficients per channel that live in registers:
+// SpatialNorm is HBM-bound: one read and one write of the feature map (up to 604 MB per tensor at 768x768).  The generic
+// gn_apply kernel would re-derive the 2 x (4 -> C) modulation with 80 read-only loads per thread every time the latent pixel
+// under a thread changes.  Here everything that does not depend on the pixel is folded ONCE per thread into 10 coefficients
+// per channel that live in registers:
 //       y = x * a(z) + b(z),   a(z) = A (wy.z + by),   b(z) = B (wy.z + by) + (wb.z + bb),   A = gamma rstd,  B = beta - mean A
 //   ->  a = a5[0..3].z + a5[4],  b = b5[0..3].z + b5[4], evaluated once per (latent pixel, channel) and reused for the run of
 //       pixels under it: ~2 FMA per element at the fine levels, the 4-float latent pixel z comes from L1.

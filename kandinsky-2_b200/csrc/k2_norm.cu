@@ -508,12 +508,12 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const ApplyParams p) {
 }
 
 // work pixels per block: `blocks_per_sm` blocks per SM in total, at least one pixel per lane.  For the apply kernels the
-// caller passes the kernel's real occupancy (3 blocks of 256 threads at 80 registers): ONE full wave.  Round 1 asked for 4 per
-// SM regardless, i.e. 592 blocks on 444 slots = a second wave with one block per SM (profiles/README.md, round 2).
+// caller passes the kernel's real occupancy (3 blocks of 256 threads at 80 registers): ONE full wave.  A fixed 4 per SM would
+// ask for more blocks than there are resident slots, i.e. a second wave with one block per SM.
 static int pick_chunk(int HW, int ctiles, int NB, int blocks_per_sm = 4) {
   const int target_blocks = blocks_per_sm * num_sms();
-  // rounded DOWN: the grid must not exceed the resident slots by a few blocks (a second wave of 36 blocks on 444 slots cost
-  // the level-1 applies ~40 % of their duration: sm__cycles_active 60 % of elapsed under ncu, profiles/README.md round 2)
+  // rounded DOWN: the grid must not exceed the resident slots by a few blocks (a short second wave leaves most SMs idle for
+  // the whole of its duration)
   int chunks = target_blocks / (ctiles * NB);
   int max_chunks = (HW + PY - 1) / PY;
   if (chunks > max_chunks) chunks = max_chunks;

@@ -158,7 +158,7 @@ int k2_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream) {
   K2_REQUIRE(x && y && n > 0 && n % 2 == 0, "gelu_f16: n must be a positive even element count");
   K2_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 3) == 0, "gelu_f16: 4-byte alignment");
   long long blocks = (n / 2 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   gelu_f16_kernel<<<static_cast<unsigned int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half2*>(x), reinterpret_cast<__half2*>(y), n / 2);
   K2_CHECK_CUDA(cudaGetLastError());

@@ -1,6 +1,6 @@
 """ctypes binding of libk2b200.so (the C ABI declared in include/k2b200.h).
 
-The library is the only compute path: if it is missing, or no sm_100 device is present, every op
+The library is the only compute path: if it is missing, or no sm_90 device is present, every op
 raises -- there is deliberately no PyTorch / CPU fallback (BASELINE.json north_star).
 """
 import ctypes
@@ -32,7 +32,6 @@ SIGNATURES = {
     "k2_version": (_I, []),
     "k2_launch_count": (_LL, []),
     "k2_reset_launch_count": (None, []),
-    "k2_conv_last_tail_split": (_I, []),
     "k2_set_tuning": (_I, [_I, _I]),
     "k2_conv_gemm": (_I, [ctypes.POINTER(K2ConvSrc), _I, _I, _I, _I, _P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _LL, _P,
                          ctypes.POINTER(ctypes.c_int), _P]),

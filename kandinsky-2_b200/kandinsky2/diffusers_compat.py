@@ -1,4 +1,4 @@
-"""A diffusers-`UNet2DConditionModel`-shaped front for the B200 UNet (SURVEY.md 8b, boundary B2).
+"""A diffusers-`UNet2DConditionModel`-shaped front for the H100 UNet (SURVEY.md 8b, boundary B2).
 
 The reference's Kandinsky 2.2 builds its decoder pipelines with `unet = UNet2DConditionModel.from_pretrained(..., subfolder='unet')`
 and hands that object to `KandinskyV22Pipeline(unet=...)` (kandinsky2/kandinsky2_2_model.py:26-42).  A user who keeps the

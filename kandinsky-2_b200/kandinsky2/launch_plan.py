@@ -9,17 +9,16 @@ import torch
 from . import ops
 
 # GroupNorm statistics are folded inside k2_gn_apply_fold when an image has at most this many partial row groups per source.
-# The per-block fold costs L2 latency x row groups; a separate k2_gn_finalize launch costs ~7 us.  Measured per GroupNorm
-# (profiles/README.md, round 2): 72 row groups (UNet level 0) finalize + apply 36-40 us vs fold 40-46 us; 18 (level 1) 23-27 vs
-# 21-23; <= 9 (levels 2-3) 18-21 vs 15-17 -> fold below level 0 only.
+# The per-block fold costs L2 latency x row groups; a separate k2_gn_finalize launch costs one more launch per GroupNorm, so the
+# fold pays where an image has few row groups (UNet levels 1-3, up to 18) and not at level 0 (72).  The threshold has not been
+# re-measured on the H100.
 FOLD_MAX_RG = int(os.environ.get("K2_GN_FOLD_MAX_RG", "18"))
 TUNE = os.environ.get("K2_AUTOTUNE", "1") != "0"
 FORK = os.environ.get("K2_FORK", "1") != "0"
-# Layers with at most this many output rows (UNet levels 2-3: 4608 / 1152 rows at cfg-2) also try the single-CTA kernel and
-# split-K factors 2..4: their tile counts leave a large part of the machine idle in the configuration the cycle model picks
-# (level 3: 60 work units on 74 CTA pairs; N tile 192 x 2-way split-K on single CTAs = 144 units on 148 SMs is 23-30 %
-# faster, profiles/conv_sustain.py).  A K split changes the fp32 summation order: deterministic per configuration, not
-# bit-identical across configurations (the choice is cached per process and shape).
+# Layers with at most this many output rows (UNet levels 2-3: 4608 / 1152 rows at cfg-2) also try split-K factors 2..4: their
+# tile counts leave a large part of the machine idle in the configuration the cycle model picks.  A K split changes the fp32
+# summation order: deterministic per configuration, not bit-identical across configurations (the choice is cached per process
+# and shape).
 TUNE_SMALL_M = int(os.environ.get("K2_TUNE_SMALL_M", "8192"))
 _tune_cache = {}
 
@@ -27,9 +26,9 @@ _tune_cache = {}
 def tune(key, run, m_rows=0):
     """Launch configuration of one conv / GEMM layer shape: (N tile, pair mode, splits, epilogue warp sets) for
     k2_conv_gemm_cfg, picked by timing candidates with CUDA events on the current stream: N tile x epilogue sets (bit-identical
-    results) everywhere, plus single-CTA / split-K variants for layers of at most TUNE_SMALL_M output rows (m_rows; see above).
-    Cached per shape and device; None = the library's own choice.  key = (kind, Cout, ...); run(cfg, info) must enqueue the
-    launch and report the configuration the library actually used in info."""
+    results) for layers of more than 64 output channels, plus split-K variants for layers of at most TUNE_SMALL_M output rows
+    (m_rows; see above).  Cached per shape and device; None = the library's own choice.  key = (kind, Cout, ...); run(cfg, info)
+    must enqueue the launch and report the configuration the library actually used in info."""
     if not TUNE:
         return None
     key = (torch.cuda.current_device(), TUNE_SMALL_M) + key
@@ -37,25 +36,25 @@ def tune(key, run, m_rows=0):
         return _tune_cache[key]
     info = [0] * 7
     run(None, info)
-    bn0, pair, splits = info[0], info[1], info[2]
+    bn0, splits = info[0], info[2]
+    cout = key[3]
     best = None
-    if pair:
-        cout = key[3]
+    if cout > 64:
         bns = [bn0] if splits > 1 else [bn for bn in (128, 192, 256) if bn - 64 < cout or bn == bn0]
-        cands = [(bn0, 0, splits, 1)] + [(bn, 0, splits, es) for bn in bns for es in (1, 2) if (bn, es) != (bn0, 1)]
+        cands = [(bn0, 0, splits, 1)] + [(bn, 0, splits, es) for bn in bns for es in ((1,) if bn == 192 else (1, 2))
+                                        if (bn, es) != (bn0, 1)]
         if 0 < m_rows <= TUNE_SMALL_M and splits == 1:
-            for pm in (2, 1):        # CTA pairs / single CTAs
-                for bn in (128, 192, 256):
-                    if bn - 64 >= cout:
+            for bn in (128, 192, 256):
+                if bn - 64 >= cout:
+                    continue
+                for sp in (2, 3, 4):
+                    probe = [0] * 7
+                    try:
+                        run((bn, 1, sp, 1), probe)
+                    except Exception:
                         continue
-                    for sp in ((2, 3, 4) if pm == 2 else (1, 2, 3, 4)):
-                        probe = [0] * 7
-                        try:
-                            run((bn, pm, sp, 1), probe)
-                        except Exception:
-                            continue
-                        if probe[0] == bn and probe[2] == sp and bool(probe[1]) == (pm == 2):  # else: the library refused
-                            cands.append((bn, pm, sp, 1))
+                    if probe[0] == bn and probe[2] == sp:  # else: the library refused
+                        cands.append((bn, 1, sp, 1))
 
         def timed(cfg, reps=6):
             run(cfg)

@@ -1,6 +1,6 @@
 """create_model / create_gaussian_diffusion with the reference's signatures (kandinsky2/model/model_creation.py:9-128).
 
-create_model(**CONFIG_2_1['model_config'], up=False, inpainting=...) returns the B200-native Text2ImUNet /
+create_model(**CONFIG_2_1['model_config'], up=False, inpainting=...) returns the H100-native Text2ImUNet /
 InpaintText2ImUNet; channel_mult / attention_resolutions strings are resolved exactly as the reference does
 (:33-48: attention 'resolutions' are image_size // res downsample rates).
 """
@@ -24,7 +24,7 @@ def create_model(image_size, num_channels, num_res_blocks, channel_mult, attenti
     if up:
         raise NotImplementedError("super-resolution UNet (SuperResText2ImUNet) is not on the hot path")
     cls = InpaintText2ImUNet if inpainting else Text2ImUNet
-    kwargs.pop("use_flash_attention", None)  # attention is always the fused tcgen05 kernel
+    kwargs.pop("use_flash_attention", None)  # attention is always the fused flash-attention kernel
     return cls(in_channels=in_channels, model_channels=num_channels, out_channels=out_channels,
                num_res_blocks=num_res_blocks, attention_resolutions=attention_ds, dropout=dropout,
                model_dim=model_dim, channel_mult=channel_mult, use_fp16=use_fp16, num_heads=num_heads,

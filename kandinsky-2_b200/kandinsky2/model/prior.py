@@ -6,7 +6,7 @@ oracle/prior_oracle.py, reproduces them exactly).  Not yet wired into the pipeli
 image embeddings) and not benchmarked.
 
 `PriorTransformer` keeps the reference's parameter names (prior.py:191-228), so `prior_fp16.ckpt` state dicts load as they
-are.  Compute: the Linear layers are flat-row tcgen05 GEMMs (`ops.gemm_rows`, fp16 storage / fp32 accumulate, bias and
+are.  Compute: the Linear layers are flat-row wgmma GEMMs (`ops.gemm_rows`, fp16 storage / fp32 accumulate, bias and
 the residual add in the epilogue), LayerNorm / GELU / the masked 81-token attention are the small kernels of
 csrc/k2_prior.cu, the four single-row projections are `ops.linear`.  The residual stream is fp16 like the reference's
 (`Kandinsky2_1.__init__` halves the prior when `use_fp16`).

@@ -1,4 +1,4 @@
-"""B200-native Text2ImUNet: the reference's module boundary, compute in libk2b200.so.
+"""H100-native Text2ImUNet: the reference's module boundary, compute in libk2b200.so.
 
 Drop-in for kandinsky2/model/text2im_model2_1.py:13-155 (Text2ImUNet / InpaintText2ImUNet) and its base
 kandinsky2/model/unet.py:343-611 (UNetModel): same constructor keywords, same state_dict keys and shapes
@@ -198,7 +198,7 @@ class Text2ImUNet(nn.Module):
         self.dtype = torch.float16
 
     def convert_to_fp32(self):
-        raise NotImplementedError("the sm_100a path stores activations in fp16 (BASELINE north_star); no fp32 torso")
+        raise NotImplementedError("the sm_90a path stores activations in fp16 (BASELINE north_star); no fp32 torso")
 
     def del_cache(self):
         self.cache = None
@@ -227,7 +227,7 @@ class Text2ImUNet(nn.Module):
         """Re-layout the weights for the kernels (fp16 [Cout][taps*Cin] K-major, fp32 biases / gains)."""
         dev = self._param("time_embed.0.weight").device
         if dev.type != "cuda":
-            raise K2Error("Text2ImUNet must live on a CUDA sm_100 device (module.to('cuda')); there is no CPU path")
+            raise K2Error("Text2ImUNet must live on a CUDA sm_90 device (module.to('cuda')); there is no CPU path")
         f32 = lambda k: self._param(k).detach().to(torch.float32).contiguous()
         pk = {"res": {}, "attn": {}}
         film_w, film_b, off = [], [], 0

@@ -91,8 +91,8 @@ def pad_rows(wp, rows):
 # ------------------------------------------------------------------------------------------------
 # conv / GEMM
 # ------------------------------------------------------------------------------------------------
-_CONV_WS_BYTES = 256 << 20  # split-K partial sums (lower half), tail-split hand-over tiles + flags (upper half); fixed size and
-# address (baked into captured CUDA graphs); conv launches that share it must be stream-ordered
+_CONV_WS_BYTES = 128 << 20  # split-K partial sums; fixed size and address (baked into captured CUDA graphs); conv launches that
+# share it must be stream-ordered
 _conv_ws = {}
 
 
@@ -100,7 +100,6 @@ def _workspace(dev):
     buf = _conv_ws.get(dev.index)
     if buf is None:
         buf = torch.empty(_CONV_WS_BYTES, dtype=torch.uint8, device=dev)
-        buf[-(64 << 10):].zero_()  # tail-split hand-over flags (k2b200.h: zero before the first launch, kept zero by the library)
         _conv_ws[dev.index] = buf
     return buf
 
@@ -145,12 +144,7 @@ def conv_gemm(srcs, w_packed, cout, bias=None, residual=None, out=None, out_mode
     return out
 
 
-def conv_last_tail_split():
-    """K parts of the tail split used by the most recent conv_gemm / conv_plan call of this thread (1 = none)."""
-    return nat.load().k2_conv_last_tail_split()
-
-
-def conv_plan(NB, H, W, taps, ktot, cout, out_mode=0, workspace_bytes=1 << 28, want_gn_partial=True):
+def conv_plan(NB, H, W, taps, ktot, cout, out_mode=0, workspace_bytes=_CONV_WS_BYTES, want_gn_partial=True):
     """What k2_conv_gemm would decide for this geometry (host arithmetic only, no GPU): dict of the info[7] fields."""
     lib = nat.load()
     info = (ctypes.c_int * 7)()

@@ -73,7 +73,7 @@ class _DecoderBase:
     def __init__(self, config, device, task_type="text2img", embedder=None, unet_state_dict=None, movq_state_dict=None,
                  seed=0):
         if not str(device).startswith("cuda"):
-            raise K2Error("k2b200 pipelines run on a CUDA sm_100 device only (no CPU fallback)")
+            raise K2Error("k2b200 pipelines run on a CUDA sm_90 device only (no CPU fallback)")
         self.config = config
         self.device = torch.device(device)
         self.task_type = task_type

@@ -1,4 +1,4 @@
-"""B200-native MOVQ: `decode` (latents -> image) through the C-ABI kernels; reference module boundary.
+"""H100-native MOVQ: `decode` (latents -> image) through the C-ABI kernels; reference module boundary.
 
 Drop-in for kandinsky2/vqgan/autoencoder.py:160-201 (class MOVQ; ctor (ddconfig, n_embed, embed_dim); decode :182-185)
 with the decoder of kandinsky2/vqgan/movq_modules.py:228-357.  state_dict keys/shapes equal the reference's for
@@ -27,7 +27,7 @@ from .._native import K2Error
 from ..launch_plan import LaunchPlan
 
 
-# MoVQ AttnBlock (one head, C = 512): fused tcgen05 flash kernel (k2_attention_d512) instead of two batched GEMMs around a
+# MoVQ AttnBlock (one head, C = 512): fused flash-attention kernel (k2_attention_d512) instead of two batched GEMMs around a
 # materialised [T, T] score matrix
 _FUSED_ATTN = os.environ.get("K2_MOVQ_FUSED_ATTN", "1") != "0"
 
@@ -200,7 +200,7 @@ class MOVQ(nn.Module):
     def finalize(self):
         dev = self._get("post_quant_conv.weight").device
         if dev.type != "cuda":
-            raise K2Error("MOVQ must live on a CUDA sm_100 device; there is no CPU path")
+            raise K2Error("MOVQ must live on a CUDA sm_90 device; there is no CPU path")
         f32 = lambda k: self._get(k).detach().to(torch.float32).contiguous()
         pk = {}
 

@@ -75,23 +75,24 @@ def test_product_never_imports_oracle():
 
 
 def test_conv_plan_host_logic():
-    """k2_conv_plan = the decisions k2_conv_gemm takes before touching a pointer (tile box, N tile, CTA pair, split-K,
-    GroupNorm-partial layout); pure host arithmetic, so the shapes of the 768x768 step are pinned here without a GPU."""
+    """k2_conv_plan = the decisions k2_conv_gemm takes before touching a pointer (tile box, N tile, split-K, GroupNorm-partial
+    layout); pure host arithmetic, so the shapes of the 768x768 step are pinned here without a GPU (132 SMs assumed when no
+    device is present, as on an H100 SXM)."""
     from kandinsky2 import ops
-    # level 0, 384 -> 384 3x3 at 96x96, UNet batch 8: (8 x 16)-pixel tiles, N tile 192 (divides 384), CTA pair, no split,
+    # level 0, 384 -> 384 3x3 at 96x96, UNet batch 8: (8 x 16)-pixel tiles, N tile 192 (divides 384), single CTA, no split,
     # one GroupNorm partial per M tile
     pl = ops.conv_plan(8, 96, 96, 9, 9 * 384, 384)
-    assert pl == dict(n_tile=192, cta_pair=1, splits=1, m_tiles=576, images_per_tile=1, gn_partial_mode=1, row_groups=576)
-    # level 1, 768 -> 768: widest tile
+    assert pl == dict(n_tile=192, cta_pair=0, splits=1, m_tiles=576, images_per_tile=1, gn_partial_mode=1, row_groups=576)
+    # level 1, 768 -> 768: 144 M tiles x 6 N tiles of 128 = 864 units fill 132 SMs better than 256-wide tiles
     pl = ops.conv_plan(8, 48, 48, 9, 9 * 768, 768)
-    assert (pl["n_tile"], pl["splits"], pl["m_tiles"]) == (256, 1, 144)
+    assert (pl["n_tile"], pl["splits"], pl["m_tiles"]) == (128, 1, 144)
     # level 2 (24 x 24): unsplit, N tile 192 (1152 = 6 x 192), 5-row tiles inside one image
     pl = ops.conv_plan(8, 24, 24, 9, 9 * 1152, 1152)
     assert (pl["n_tile"], pl["splits"], pl["m_tiles"], pl["images_per_tile"], pl["gn_partial_mode"]) == (192, 1, 40, 1, 1)
     # level 3 (12 x 12): (4 x 4 pixels x 8 images) tiles with every MMA row used, partials per (image, spatial tile)
     pl = ops.conv_plan(8, 12, 12, 9, 9 * 1536, 1536)
     assert (pl["m_tiles"], pl["images_per_tile"], pl["splits"], pl["gn_partial_mode"], pl["row_groups"]) == (9, 8, 1, 1, 72)
-    # attention qkv as a flat-row GEMM, and the 4-channel fp32 NCHW output head (single-CTA kernel, N tile 16)
+    # attention qkv as a flat-row GEMM, and the 4-channel fp32 NCHW output head (N tile 16)
     assert ops.conv_plan(1, 1, 18432, 1, 768, 2304, want_gn_partial=False)["n_tile"] == 256
     pl = ops.conv_plan(8, 96, 96, 9, 9 * 384, 8, out_mode=1, want_gn_partial=False)
     assert (pl["n_tile"], pl["cta_pair"], pl["gn_partial_mode"]) == (16, 0, 0)

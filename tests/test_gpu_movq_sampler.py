@@ -91,10 +91,10 @@ def test_movq_decode_full_size_vs_oracle():
     rel1 = ((y1 - y[1:]).norm() / y[1:].norm()).item()
     assert rel1 < 1e-3, rel1   # different tile shapes at batch 1 may change fp32 summation order, nothing more
     # decode_to_uint8 against the reference's process_images arithmetic on the very fp32 image it converted (the plan's static
-    # output buffer).  Until the end of round 2 this line compared with `y` from the replay further up; on two boxes, and only in
-    # full-suite order, that earlier image and this later replay differed by single fp32 roundings (a handful of uint8 values off
-    # by one) although the replays above are bit-identical and profiles/movq_repro_probe.py reproduces no difference in
-    # isolation -- recorded as an open item in DESIGN.md section 4; the bound below keeps the comparison meaningful.
+    # output buffer).  Comparing with `y` from the replay further up instead has shown, only in full-suite order, single fp32
+    # rounding differences between that earlier image and this later replay (a handful of uint8 values off by one) although the
+    # replays above are bit-identical -- recorded as an open item in DESIGN.md section 4; the bound below keeps the comparison
+    # meaningful.
     u8 = m.decode_to_uint8(z, crop_h=760, crop_w=768)
     y_now = m._plan("decode", 2, 96, 96).out.clone()
     assert torch.equal(u8, mo.process_images(y_now)[:, :760, :768])
@@ -161,7 +161,7 @@ def test_ddpm_v22_loop_vs_restated_diffusers(inpaint):
         ref = do.ddpm_v22_loop(lambda xx, tt: uo.unet_forward(sd, cfg, xx, tt, **kw), x_T, steps, 4.0, noise, **okw)
     err = (out.cpu() - ref).abs().max().item()
     rel = ((out.cpu() - ref).norm() / ref.norm()).item()
-    # measured on the B200: rel L2 6e-3, max-abs 8e-2 (guidance 4 x sqrt(1/ac - 1) ~ 5 at the first steps amplifies the UNet's
+    # guidance 4 x sqrt(1/ac - 1) ~ 5 at the first steps amplifies the UNet's
     # fp16 error; no dynamic-threshold renormalisation on this path, unlike the 2.1 trajectory test)
     assert err < 2e-1 and rel < 1e-2, (err, rel)
     if inpaint:  # the known region of the result IS the clean latent

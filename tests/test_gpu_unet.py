@@ -1,8 +1,8 @@
 """GPU parity of the full UNet forward (C-ABI kernels) against the reference's golden outputs and the oracle.
 
 Tolerance: activations are stored in fp16 (fp32 accumulate / GroupNorm / softmax), the reference output here is
-fp32.  Measured on the B200: relative L2 1.0-1.4e-3, max-abs 3-5e-3 on outputs of RMS ~0.58; asserted: relative L2 < 2e-3
-and max-abs < 1e-2 * RMS (about 2x what is measured).  The north_star's "1e-3 max-abs" is calibrated in
+fp32.  Asserted: relative L2 < 2e-3
+and max-abs < 1e-2 * RMS.  The north_star's "1e-3 max-abs" is calibrated in
 test_unet_full_size_fp16_calibration: the REFERENCE's own fp16 mode (use_fp16=True, the mode the pipelines run) deviates
 from its fp32 mode by MORE than this implementation does, so the bound asserted there is  k2 <= reference-fp16.
 """
