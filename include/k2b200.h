@@ -285,6 +285,18 @@ int k2_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream);
 int k2_attention_small(const void* qkv, int ldq, const unsigned char* keep_mask, int causal, void* out, int ldo, int B, int T,
                        int heads, float scale, k2_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
+ * fuse_lora): once per adapter load, never per step.
+ *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols
+ * base / out fp16 rows with strides ldb / ldo (elements, >= cols; columns >= cols are not touched; out may equal base);
+ * up fp32 [rows, rank], down fp32 [rank, cols], both contiguous.  The sum is fp32 in ascending j, one rounding to fp16
+ * (nearest-even); an element whose scaled sum is exactly zero keeps base's bits (scale 0 copies base).  The result does not
+ * depend on the launch configuration.
+ * ------------------------------------------------------------------------------------------- */
+int k2_lora_merge(const void* base, int ldb, const float* up, const float* down, int rows, int cols, int rank, float scale,
+                  void* out, int ldo, k2_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -69,6 +69,7 @@ SIGNATURES = {
     "k2_pointwise_nchw_f32": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "k2_nchw_to_nhwc_f32": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "k2_images_to_u8": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "k2_lora_merge": (_I, [_P, _I, _P, _P, _I, _I, _I, _F, _P, _I, _P]),
 }
 
 

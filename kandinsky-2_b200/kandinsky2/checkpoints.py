@@ -9,6 +9,9 @@
   head-interleaved `qkv` (and `encoder_kv`) Conv1d.  `diffusers_unet_to_k2` renames and re-packs such a state dict into
   the key layout of `Text2ImUNet(cond_version="2.2")`; `k2_to_diffusers_unet` is its inverse.
 
+* `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
+  qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
+
 **Parity unpinned:** diffusers is not part of /root/reference (`setup.py:27` lists it unpinned) and is not installed in the
 build container, so the diffusers-side key names below are restated from the published `UNet2DConditionModel` layout
 (`ResnetDownsampleBlock2D` / `SimpleCrossAttnDownBlock2D` / `UNetMidBlock2DSimpleCrossAttn` / `SimpleCrossAttnUpBlock2D` /
@@ -16,8 +19,11 @@ build container, so the diffusers-side key names below are restated from the pub
 are inverse bijections onto the package's exact key set, and the head-interleaved packing reproduces separate
 q / k / v projections numerically.
 """
+import re
+
 import torch
 
+from ._native import K2Error
 from .model.unet import _topology
 
 _RES = {"norm1": "in_layers.0", "conv1": "in_layers.2", "time_emb_proj": "emb_layers.1", "norm2": "out_layers.0",
@@ -105,6 +111,77 @@ def diffusers_unet_to_k2(sd, in_channels=4, model_channels=384, channel_mult=(1,
             out[f"{kp}.proj_out.weight"] = sd[f"{dp}.to_out.0.weight"].unsqueeze(-1)
             out[f"{kp}.proj_out.bias"] = sd[f"{dp}.to_out.0.bias"]
     return out
+
+
+_LORA_KEY = re.compile(r"^(.+)\.processor\.(to_q|to_k|to_v|to_out|add_k_proj|add_v_proj)_lora\.(down|up)\.weight$")
+# packed target -> the projections that feed it, in pack_heads order
+_LORA_TARGETS = {"qkv": ("to_q", "to_k", "to_v"), "encoder_kv": ("add_k_proj", "add_v_proj"), "proj_out": ("to_out",)}
+
+
+def lora_to_k2(lora, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3, attention_ds=(2, 4, 8),
+               model_dim=768, head_dim=64):
+    """A LoRA adapter of the decoder UNet in diffusers' attention-processor form -- the keys `AttnProcsLayers` /
+    `UNet2DConditionModel.save_attn_procs` write for `LoRAAttnAddedKVProcessor`:
+        {attention prefix}.processor.{to_q,to_k,to_v,to_out,add_k_proj,add_v_proj}_lora.{down,up}.weight
+    with the attention prefixes of unet_block_map (e.g. `mid_block.attentions.0`) -> {packed weight key: (up', down')}, fp32,
+    keyed like the output of diffusers_unet_to_k2 (`middle_block.1.qkv.weight`, `.encoder_kv.weight`, `.proj_out.weight`).
+
+    The delta of a projection is up @ down (diffusers' LoRALinearLayer without network_alpha), so
+    up' @ down' = diffusers_unet_to_k2 of the per-projection deltas: for qkv / encoder_kv, down' stacks the present projections'
+    down matrices and up' is block-diagonal (zeros elsewhere) with its rows head-interleaved by pack_heads -- the zero terms
+    add exact zeros, so each element's fp32 sum equals that of its own projection.  A missing projection has no delta.
+    Raises K2Error naming the first offending key for anything else: unknown keys, PEFT (lora_A / lora_B) or alpha entries,
+    a factor without its partner, rank or shape mismatches, non-floating tensors."""
+    inp, mid, out = _topology(in_channels, model_channels, channel_mult, num_res_blocks, attention_ds)
+    chans = [layer[1] for blk in inp + [mid] + out for layer in blk if layer[0] == "attn"]
+    prefixes = [(dp, kp) for dp, kp, kind in unet_block_map(in_channels, model_channels, channel_mult, num_res_blocks,
+                                                             attention_ds) if kind == "attn"]
+    blocks = {dp: (kp, c) for (dp, kp), c in zip(prefixes, chans)}  # both lists are in the reference's block order
+    found = {}  # (diffusers prefix, projection) -> {"down": fp32 tensor, "up": fp32 tensor}
+    for key, t in lora.items():
+        if "lora_A" in key or "lora_B" in key:
+            raise K2Error(f"LoRA key {key!r}: PEFT-format (lora_A / lora_B) adapters are not supported")
+        if "alpha" in key.rsplit(".", 1)[-1]:
+            raise K2Error(f"LoRA key {key!r}: alpha / network_alpha scaling is not supported")
+        m = _LORA_KEY.match(key)
+        if m is None or m.group(1) not in blocks:
+            raise K2Error(f"LoRA key {key!r} is not an attention-processor LoRA weight of this UNet")
+        if not torch.is_tensor(t) or t.dtype not in (torch.float16, torch.bfloat16, torch.float32) or t.dim() != 2:
+            raise K2Error(f"LoRA key {key!r}: expected a 2-D fp16, bf16 or fp32 tensor")
+        found.setdefault((m.group(1), m.group(2)), {})[m.group(3)] = t.detach().to("cpu", torch.float32)
+    for key in lora:
+        dp, proj, which = _LORA_KEY.match(key).groups()
+        pair = found[(dp, proj)]
+        other = "up" if which == "down" else "down"
+        if other not in pair:
+            raise K2Error(f"LoRA key {key!r} has no matching {other} weight")
+        down, up = pair["down"], pair["up"]
+        C = blocks[dp][1]
+        fan_in = model_dim if proj.startswith("add_") else C
+        if up.shape[1] != down.shape[0]:
+            raise K2Error(f"LoRA key {key!r}: rank mismatch between down {tuple(down.shape)} and up {tuple(up.shape)}")
+        if down.shape[1] != fan_in or up.shape[0] != C:
+            raise K2Error(f"LoRA key {key!r}: expected down [rank, {fan_in}] and up [{C}, rank], got down "
+                          f"{tuple(down.shape)} and up {tuple(up.shape)}")
+    packed = {}
+    for dp, (kp, C) in blocks.items():
+        for target, projs in _LORA_TARGETS.items():
+            present = [p for p in projs if (dp, p) in found]
+            if not present:
+                continue
+            downs = [found[(dp, p)]["down"] for p in present]
+            R = sum(d.shape[0] for d in downs)
+            ups, col = [], 0
+            for p in projs:
+                u = torch.zeros(C, R)
+                if (dp, p) in found:
+                    r = found[(dp, p)]["down"].shape[0]
+                    u[:, col:col + r] = found[(dp, p)]["up"]
+                    col += r
+                ups.append(u)
+            up = pack_heads(ups, head_dim) if len(projs) > 1 else ups[0]
+            packed[f"{kp}.{target}.weight"] = (up.contiguous(), torch.cat(downs, 0).contiguous())
+    return packed
 
 
 def k2_to_diffusers_unet(sd, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3,

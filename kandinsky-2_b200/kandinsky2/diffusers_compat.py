@@ -67,6 +67,16 @@ class K2UNet2DConditionModel(torch.nn.Module):
     def half(self):
         return self
 
+    def load_attn_procs(self, pretrained_model_name_or_path_or_dict):
+        """diffusers' loader for a LoRA of the attention processors (`save_attn_procs` / `AttnProcsLayers` keys, e.g. the
+        `pytorch_model.bin` of a decoder LoRA fine-tune), merged into the weights at scale 1.0 (Text2ImUNet.load_lora).  It
+        replaces diffusers' two steps `set_attn_processor(LoRAAttnAddedKVProcessor ...)` + `load_state_dict(..., strict=False)`.
+        A path is read with torch.load(map_location="cpu", weights_only=True)."""
+        sd = pretrained_model_name_or_path_or_dict
+        if not isinstance(sd, dict):
+            sd = torch.load(sd, map_location="cpu", weights_only=True)
+        self.unet.load_lora(sd)
+
     def to(self, *args, **kwargs):
         dev = [a for a in args if isinstance(a, (str, torch.device))]
         if dev or "device" in kwargs:

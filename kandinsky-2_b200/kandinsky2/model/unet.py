@@ -111,6 +111,8 @@ class Text2ImUNet(nn.Module):
         self.cache = None
         self._packed = None
         self._plans = {}
+        self._lora = None        # (factors from checkpoints.lora_to_k2, scale) of the loaded adapter
+        self._lora_base = None   # device copies of the unmerged packed attention weights while an adapter is merged
         self.use_cuda_graph = True
 
         mc = model_channels
@@ -213,6 +215,7 @@ class Text2ImUNet(nn.Module):
 
     def _invalidate(self):
         self._packed = None
+        self._lora_base = None
         self._plans = {}
         self.cache = None
 
@@ -291,10 +294,65 @@ class Text2ImUNet(nn.Module):
         self._packed = pk
         self._plans = {}
         self.cache = None
+        self._lora_base = None
+        if self._lora is not None:  # a loaded adapter survives re-packing (load_state_dict, .to)
+            self._merge_lora()
         if release_params:
             for prm in self.parameters():
                 prm.data = torch.empty(0, device=dev, dtype=prm.dtype)
         return self
+
+    # ---------------------------------------------------------------- LoRA adapters, merged into the packed weights
+    _LORA_WEIGHTS = (("wqkv", "qkv"), ("wenc", "encoder_kv"), ("wproj", "proj_out"))
+
+    @property
+    def lora_scale(self):
+        """Scale of the loaded LoRA adapter, None when there is none."""
+        return None if self._lora is None else self._lora[1]
+
+    def load_lora(self, state_dict, scale=1.0):
+        """Merge a LoRA adapter of the attention blocks -- diffusers' `LoRAAttnAddedKVProcessor` weights as
+        `save_attn_procs` / `AttnProcsLayers` write them (checkpoints.lora_to_k2) -- into the packed weights:
+        W = W_base + scale * up @ down, computed by k2_lora_merge in fp32 and rounded once to fp16 (diffusers' fuse_lora).
+        The merge writes the packed tensors in place, so captured launch plans and step graphs keep their addresses and
+        need no rebuild; the cached conditioning is dropped because the encoder K/V projections use the merged weights.
+        On first use the unmerged packed weights are copied on the device (restored by unload_lora).  Loading again
+        replaces the adapter (adapters do not stack; a new scale means loading again).  state_dict() never changes."""
+        from ..checkpoints import lora_to_k2
+        factors = lora_to_k2(state_dict, in_channels=self.in_channels, model_channels=self.model_channels,
+                             channel_mult=self.channel_mult, num_res_blocks=self.num_res_blocks,
+                             attention_ds=self.attention_resolutions, model_dim=self.model_dim,
+                             head_dim=self.num_head_channels)
+        if self._packed is None:
+            self.finalize()
+        self._lora = (factors, float(scale))
+        self._merge_lora()
+
+    def unload_lora(self):
+        """Restore the unmerged packed weights (bit-exact), free their copy and drop the cached conditioning."""
+        if self._lora_base is not None and self._packed is not None:
+            for p, a in self._packed["attn"].items():
+                for name, _ in self._LORA_WEIGHTS:
+                    a[name].copy_(self._lora_base[p][name])
+        self._lora = None
+        self._lora_base = None
+        self.cache = None
+
+    def _merge_lora(self):
+        factors, scale = self._lora
+        attn = self._packed["attn"]
+        if self._lora_base is None:
+            self._lora_base = {p: {name: a[name].clone() for name, _ in self._LORA_WEIGHTS} for p, a in attn.items()}
+        for p, a in attn.items():
+            for name, target in self._LORA_WEIGHTS:
+                base = self._lora_base[p][name]
+                f = factors.get(p + target + ".weight")
+                if f is None:
+                    a[name].copy_(base)
+                else:
+                    up, down = (t.to(base.device) for t in f)
+                    ops.lora_merge(base, up, down, scale, out=a[name])
+        self.cache = None
 
     def _skip_weight(self, d, c0, c1):
         """[W2 | Wskip] packed for the (conv3x3 of h, 1x1 of x0, 1x1 of x1) K segments."""

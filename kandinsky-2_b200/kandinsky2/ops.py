@@ -493,6 +493,23 @@ def images_to_u8(x, crop_h, crop_w, out=None):
     return out
 
 
+def lora_merge(base, up, down, scale, out=None):
+    """fp16 base [rows, >= cols] (row-strided) + scale * (fp32 up [rows, rank] @ fp32 down [rank, cols]) -> fp16 [rows, cols],
+    fp32 sum in ascending rank order, one rounding (k2_lora_merge).  out may be base itself, or another row-strided fp16
+    [rows, >= cols] tensor; its columns from cols on are left alone."""
+    lib = nat.load()
+    rows, rank = up.shape
+    cols = down.shape[1]
+    assert up.dtype == down.dtype == torch.float32 and up.is_contiguous() and down.is_contiguous() and down.shape[0] == rank
+    assert base.dtype == torch.float16 and base.stride(1) == 1 and base.shape[0] == rows and base.shape[1] >= cols
+    if out is None:
+        out = torch.empty((rows, cols), dtype=torch.float16, device=base.device)
+    assert out.dtype == torch.float16 and out.stride(1) == 1 and out.shape[0] == rows and out.shape[1] >= cols
+    check(lib.k2_lora_merge(ptr(base), base.stride(0), ptr(up), ptr(down), rows, cols, rank, float(scale), ptr(out),
+                            out.stride(0), stream_ptr()))
+    return out
+
+
 def set_tuning(key, value):
     """k2_set_tuning: key 0 = force conv N tile, key 1 = split-K (0 auto, 1 off, n forced)."""
     check(nat.load().k2_set_tuning(int(key), int(value)))
