@@ -15,8 +15,9 @@
 //     how ResBlock's  skip_connection(x) + conv(h)  (unet.py:220) becomes a single kernel.
 //   * Weights are pre-packed [Cout][K] fp16, K = concat over segments/taps/channels, loaded by 2-D TMA.
 //   * Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 = wgmma consumers, rows
-//     [0, 64) and [64, 128) of the M tile (m64nNk16, N = 64 per instruction -- 16 for the N = 16 output heads -- both operands
-//     K-major from the 128 B-swizzled TMA tiles).  Persistent over tiles, smem ring of STAGES (A 16 KB + B BN*128 B).
+//     [0, 64) and [64, 128) of the M tile: ONE m64nBNk16 per 16-element K step covers the whole N tile (BN = 16 ... 256), so
+//     each warpgroup reads its A slice from shared memory once per K step, not once per 64 columns.  Both operands are K-major
+//     in the 128 B-swizzled TMA tiles.  Persistent over tiles, smem ring of STAGES (A 16 KB + B BN*128 B).
 //   * Epilogue: the consumers park their register accumulators, BNC columns at a time, in a shared-memory tile with one fp32
 //     row per output pixel; the epilogue warps then read it one ROW per thread (warp ew of a set owns rows [32 ew, 32 ew + 32))
 //     -> + bias (+ residual) -> fp16 rows, fp32 split-K partials or fp32 NCHW, plus the fused GroupNorm partial statistics.
@@ -192,16 +193,18 @@ __device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, const flo
                 }
                 __syncwarp();
               }
-              uint32_t r[64];
-              acc_ld(arow + jp * 64, r);
               if constexpr (ES == 1) {
                 if (p.residual && jp + 1 < NP) load_res(jp + 1);
               }
 #pragma unroll
               for (int v = 0; v < 8; ++v) {  // 8 columns = one 16-byte piece of the staged row
+                // read per piece: the unread part of the register accumulator is still live while the first passes of a
+                // 256-column tile drain
+                uint32_t r[8];
+                acc_ld(arow + jp * 64 + v * 8, r);
                 float f[8];
 #pragma unroll
-                for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(r[v * 8 + e]);
+                for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(r[e]);
                 if (p.bias) {
                   const float4 b0 = *reinterpret_cast<const float4*>(bsm + jp * 64 + v * 8);
                   const float4 b1 = *reinterpret_cast<const float4*>(bsm + jp * 64 + v * 8 + 4);
@@ -389,8 +392,7 @@ template <int BN, int ES>
 __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   using C = Cfg<BN, ES>;
   constexpr int BNC = C::BNC;
-  constexpr int NJ = (BN >= 64) ? BN / 64 : 1;  // wgmma instructions per K step (N = 64 each, or one N = 16)
-  constexpr int NA = (BN >= 64) ? 32 : 8;       // accumulator registers per instruction
+  constexpr int NA = BN / 2;  // accumulator registers of the m64nBNk16 fragment
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -479,11 +481,9 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       const int n_idx = (tile / p.m_tiles) % p.n_tiles;
       const int split = tile / (p.m_tiles * p.n_tiles);
       const int nk = min(p.num_k_chunks, (split + 1) * p.k_per_split) - split * p.k_per_split;
-      float acc[NJ][NA];
+      float acc[NA];
 #pragma unroll
-      for (int j = 0; j < NJ; ++j)
-#pragma unroll
-        for (int i = 0; i < NA; ++i) acc[j][i] = 0.f;
+      for (int i = 0; i < NA; ++i) acc[i] = 0.f;
       int prev_stage = -1;
       for (int kc = 0; kc < nk; ++kc) {
         mbar_wait_lean(&full_bar[stage], phase);  // no printf call: wgmma stays pipelined across the wait
@@ -494,14 +494,18 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
         for (int k = 0; k < BK / 16; ++k) {
           // +32 bytes (2 x 16 B units) per 16-element K step inside the 128 B swizzle row
           const uint64_t adesc = make_wgmma_desc(a_addr) + static_cast<uint64_t>(k * 2);
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) {
-            const uint64_t bdesc = make_wgmma_desc(b_addr + j * (64 * 128)) + static_cast<uint64_t>(k * 2);
-            if constexpr (BN >= 64) {
-              wgmma_m64n64k16(acc[j], adesc, bdesc, 1u);
-            } else {
-              wgmma_m64n16k16(acc[j], adesc, bdesc, 1u);
-            }
+          const uint64_t bdesc = make_wgmma_desc(b_addr) + static_cast<uint64_t>(k * 2);
+          if constexpr (BN == 256) {
+            wgmma_m64n256k16(acc, adesc, bdesc, 1u);
+          } else if constexpr (BN == 192) {
+            wgmma_m64n192k16(acc, adesc, bdesc, 1u);
+          } else if constexpr (BN == 128) {
+            wgmma_m64n128k16(acc, adesc, bdesc, 1u);
+          } else if constexpr (BN == 64) {
+            wgmma_m64n64k16(acc, adesc, bdesc, 1u);
+          } else {
+            static_assert(BN == 16, "conv_gemm: N tile without a wgmma shape");
+            wgmma_m64n16k16(acc, adesc, bdesc, 1u);
           }
         }
         wgmma_commit();
@@ -525,14 +529,12 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       for (int pass = 0; pass < BN / BNC; ++pass) {
         named_bar_sync(3, 256);  // the staged tile of the previous pass / tile has been read
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) {
-          if (BN >= 64 && (j * 64) / BNC != pass) continue;
-#pragma unroll
-          for (int i = 0; i < NA; i += 2) {
-            const int row = r0 + 8 * ((i >> 1) & 1);
-            const int col = (BN >= 64 ? j * 64 - pass * BNC : 0) + 8 * (i >> 2) + cq;
-            *reinterpret_cast<float2*>(acc_smem + row * (BNC + ACC_PAD) + col) = make_float2(acc[j][i], acc[j][i + 1]);
-          }
+        for (int i = 0; i < NA; i += 2) {
+          // register i: row 16 w + l / 4 + 8 ((i / 2) & 1), column 8 (i / 4) + 2 (l & 3) + (i & 1) of the tile
+          if ((8 * (i >> 2)) / BNC != pass) continue;
+          const int row = r0 + 8 * ((i >> 1) & 1);
+          const int col = 8 * (i >> 2) - pass * BNC + cq;
+          *reinterpret_cast<float2*>(acc_smem + row * (BNC + ACC_PAD) + col) = make_float2(acc[i], acc[i + 1]);
         }
         named_bar_sync(3, 256);  // staged tile complete
         if (ES == 2 || g == 0)
