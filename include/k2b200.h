@@ -239,6 +239,24 @@ int k2_plms_step(const float* model_out, int C2, const float* x, float* out, con
                  const float* hist2, float* store, const float* coef, int B, int H, int W, float guidance, int cond_first,
                  k2_stream_t stream);
 
+/* DPM-Solver++(2M) step (Lu et al. 2022, "DPM-Solver++", Algorithm 2; multistep, one UNet evaluation per step), with the CFG
+ * closure fused.  Per element of x fp32 [B, 4, H, W] (in place):
+ *   eps  = uncond + g (cond - uncond) from model_out's first 4 channels (fp32 NCHW [2B, C2, H, W]; cond_first as in
+ *          k2_sampler_step; the variance channels are ignored);
+ *   x0   = coef[0] x - coef[1] eps   (no clamp, no threshold);
+ *   x0   = x0 (1 - mask) + init mask                         if inpaint_mask != NULL and inpaint_noise == NULL (2.1);
+ *   x'   = coef[2] x + coef[3] x0 + coef[4] hist   -- hist is NOT read when coef[4] == 0 (first-order steps), so its
+ *          contents (even NaN) cannot reach the result;
+ *   hist = x0   (hist fp32 [B, 4, H, W]: the previous step's x0 in, this step's out);
+ *   x'   = mask (coef[5] init + coef[6] inpaint_noise) + (1 - mask) x'   if inpaint_noise != NULL (2.2: the known region is
+ *          the clean latent noised to the next timestep with the run's initial noise; (1, 0) at the last step).
+ * coef is device fp32[8] = {1/alpha_k, sigma_k/alpha_k, c_x, c_D, c_P, alpha_{k+1}, sigma_{k+1}, 0}, one row of the host's
+ * schedule (kandinsky2/model/gaussian_diffusion.py: DPMSolverSchedule), so k2_step_begin can pick it by the step counter.
+ * Arguments are checked before any CUDA call. */
+int k2_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, int B, int H, int W,
+                       float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
+                       const float* inpaint_noise, k2_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * MoVQ helpers: nearest-codebook search (quntize.py:89-98; fp32, ties -> lowest index, int64 out),
  * fp32 NCHW -> NHWC transposes for the 4-channel latent, final image quantisation

@@ -404,6 +404,50 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const PlmsParams p) {
   p.out[i] = xn;
 }
 
+// DPM-Solver++(2M) update (Lu et al. 2022, Algorithm 2), linear in (x, D_k, D_{k-1}) with D the x0 prediction:
+//   eps = CFG(model_out)  (eps channels only);  x0 = coef[0] x - coef[1] eps  (no clamp, no threshold)
+//   x'  = coef[2] x + coef[3] x0 + coef[4] hist      (hist = D_{k-1}; not read when coef[4] == 0)
+//   hist = x0
+// coef = {1/a_k, s_k/a_k, c_x, c_D, c_P, a_{k+1}, s_{k+1}, 0}; the host builds the rows (DPMSolverSchedule).
+struct DpmParams {
+  const float* model_out;  // [2B, C2, H, W], eps = channels [0, 4)
+  float* x;                // [B, 4, H, W], in place
+  float* hist;             // [B, 4, H, W]: D of the previous step in, D of this step out
+  const float* coef;       // device [8]
+  int B, HW, C2;
+  float guidance;
+  int cond_first;
+  const float* init;       // [B,4,H,W] or null
+  const float* mask;       // [B,1,H,W] or null
+  const float* rnoise;     // [B,4,H,W] or null (2.2 inpainting: the known region is re-noised to the next timestep)
+};
+
+__global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  pdl_wait();
+  pdl_launch();
+  const long long total = static_cast<long long>(p.B) * 4 * p.HW;
+  if (i >= total) return;
+  const int sp = static_cast<int>(i % p.HW);
+  const int c = static_cast<int>((i / p.HW) % 4);
+  const int b = static_cast<int>(i / (4LL * p.HW));
+  const int bc = p.cond_first ? b : b + p.B;
+  const int bu = p.cond_first ? b + p.B : b;
+  const float ec = p.model_out[(static_cast<long long>(bc) * p.C2 + c) * p.HW + sp];
+  const float eu = p.model_out[(static_cast<long long>(bu) * p.C2 + c) * p.HW + sp];
+  const float eps = eu + p.guidance * (ec - eu);
+  const float xv = p.x[i];
+  float x0 = p.coef[0] * xv - p.coef[1] * eps;
+  const float m = p.mask ? p.mask[static_cast<long long>(b) * p.HW + sp] : 0.f;
+  if (p.mask && !p.rnoise) x0 = x0 * (1.f - m) + p.init[i] * m;  // Kandinsky 2.1: the known region replaces x0
+  float xn = p.coef[2] * xv + p.coef[3] * x0;
+  const float cp = p.coef[4];
+  if (cp != 0.f) xn += cp * p.hist[i];  // a first-order step never reads the history: it may hold anything, NaN included
+  p.hist[i] = x0;
+  if (p.mask && p.rnoise) xn = m * (p.coef[5] * p.init[i] + p.coef[6] * p.rnoise[i]) + (1.f - m) * xn;
+  p.x[i] = xn;
+}
+
 // ------------------------------------------------------------------------------------------------
 // MoVQ helpers
 // ------------------------------------------------------------------------------------------------
@@ -800,6 +844,24 @@ int k2_plms_step(const float* model_out, int C2, const float* x, float* out, con
   p.coef = coef; p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
   const long long total = static_cast<long long>(B) * 4 * H * W;
   K2_CHECK_CUDA(launch_k(plms_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p));
+  count_launch();
+  return 0;
+}
+
+int k2_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, int B, int H, int W,
+                       float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
+                       const float* inpaint_noise, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && hist && coef, "dpm_solver_step: null pointer");
+  K2_REQUIRE(B > 0 && H > 0 && W > 0 && C2 >= 4, "dpm_solver_step: B, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE((inpaint_init == nullptr) == (inpaint_mask == nullptr), "dpm_solver_step: init and mask go together");
+  K2_REQUIRE(inpaint_noise == nullptr || inpaint_init, "dpm_solver_step: inpaint_noise without init / mask");
+  DpmParams p;
+  p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
+  p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
+  p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
+  const long long total = static_cast<long long>(B) * 4 * H * W;
+  K2_CHECK_CUDA(launch_k(dpm_solver_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream),
+                         p));
   count_launch();
   return 0;
 }

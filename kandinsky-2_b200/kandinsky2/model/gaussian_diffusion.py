@@ -134,9 +134,104 @@ class SpacedDiffusion:
                               callback, sample_generators, inpaint_renoise=inpaint_renoise)
 
 
+class DPMSolverSchedule:
+    """DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models",
+    Algorithm 2) over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step, no noise.
+
+    N evaluations at tau_k = linspace(0, T-1, N+1).round()[::-1][k], k = 0..N-1; the UNet sees tau_k as a raw float timestep.
+    alpha_k = sqrt(ac[tau_k]), sigma_k = sqrt(1 - ac[tau_k]), lambda_k = log alpha_k - log sigma_k; the target after the last
+    evaluation is alpha_N = 1, sigma_N = 0.  With h_k = lambda_{k+1} - lambda_k and c = alpha_{k+1} (1 - exp(-h_k)):
+        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1},   c_x = sigma_{k+1} / sigma_k,
+        first order (the first step, the last step, which gives x_N = D_{N-1} exactly):  c_D = c, c_P = 0;
+        otherwise, r = h_{k-1} / h_k:  c_D = c (1 + 1/(2r)),  c_P = -c / (2r).
+    D is the x0 prediction (x - sigma eps) / alpha of the CFG-combined epsilon; k2_dpm_solver_step applies one row.
+    keep = s (img2img): only the last s evaluations run (k0 = N - s), from x = alpha_k0 latent + sigma_k0 noise
+    (start_latent); the history is empty at k0, so that step is first order.
+
+    Rows are stored in reverse step order (table index j = N-1-k) so that _sampling_loop, which walks the indices from the
+    top down like the DDPM schedules', runs k = k0 .. N-1."""
+
+    step_kind = "dpmpp_2m"
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None):
+        ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
+        n = int(num_steps)
+        if n < 1:
+            raise ValueError("DPM-Solver++: num_steps must be >= 1")
+        tau = np.linspace(0, len(ac) - 1, n + 1).round()[::-1][:n].astype(np.int64)
+        if np.any(np.diff(tau) >= 0):
+            raise ValueError(f"DPM-Solver++: {n} steps do not give distinct timesteps over {len(ac)} training steps")
+        keep = n if keep is None else int(keep)
+        if not 1 <= keep <= n:
+            raise ValueError(f"DPM-Solver++: keep must be in [1, {n}], got {keep}")
+        self.num_steps, self.k0 = n, n - keep
+        self.timesteps = tau
+        self.alphas = np.append(np.sqrt(ac[tau]), 1.0)    # alpha_0 .. alpha_N
+        self.sigmas = np.append(np.sqrt(1.0 - ac[tau]), 0.0)
+        self.num_timesteps = keep
+        self._dev_tables = {}
+
+    def coef_table(self):
+        """float32 [keep, 8]: the k2_dpm_solver_step rows, built in float64 and cast once."""
+        return self.coef_rows().astype(np.float32)
+
+    def coef_rows(self):
+        """float64 [keep, 8]: the rows of steps k = N-1 .. k0 (table order, see the class doc)."""
+        a, s, n, k0 = self.alphas, self.sigmas, self.num_steps, self.k0
+        with np.errstate(divide="ignore"):
+            lam = np.log(a) - np.log(s)                     # lambda_N = +inf
+        rows = np.zeros((n, 8), dtype=np.float64)
+        for k in range(k0, n):
+            rows[k, 0] = 1.0 / a[k]
+            rows[k, 1] = s[k] / a[k]
+            rows[k, 5], rows[k, 6] = a[k + 1], s[k + 1]
+            if k == n - 1:                                  # h = inf: x_N = D_{N-1}
+                rows[k, 3] = 1.0
+                continue
+            h = lam[k + 1] - lam[k]
+            c = -a[k + 1] * np.expm1(-h)
+            rows[k, 2] = s[k + 1] / s[k]
+            if k == k0:
+                rows[k, 3] = c
+            else:
+                r = (lam[k] - lam[k - 1]) / h
+                rows[k, 3] = c * (1.0 + 0.5 / r)
+                rows[k, 4] = -c * 0.5 / r
+        return np.ascontiguousarray(rows[k0:][::-1])
+
+    def model_timesteps(self):
+        """float32 [keep]: what the UNet sees, in table order."""
+        return self.timesteps[self.k0:][::-1].astype(np.float32)
+
+    def _tables(self, device):
+        key = str(device)
+        if key not in self._dev_tables:
+            self._dev_tables[key] = (torch.from_numpy(self.coef_table()).to(device),
+                                     torch.from_numpy(np.ascontiguousarray(self.model_timesteps())).to(device))
+        return self._dev_tables[key]
+
+    @staticmethod
+    def truncate(indices, init_step):
+        return indices  # `keep` already applied to the tables in __init__
+
+    def start_latent(self, latent, noise):
+        """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
+        return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
+
+    @torch.no_grad()
+    def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
+               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None):
+        """shape = (2*B, 4, h, w) (CFG doubled), noise = the start latent [2B or B, ...]; returns [2*B, 4, h, w] whose two halves
+        both hold the B samples, like p_sample_loop.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces x0),
+        True = Kandinsky 2.2 (the known region is re-noised to the next timestep with the start latent as the noise)."""
+        return _sampling_loop(self, model, shape, noise, model_kwargs, device, False, None, guidance_scale, cond_first, 1e30, 0,
+                              inpaint_init, inpaint_mask, None, callback, None, needs_noise=False,
+                              inpaint_renoise=inpaint_renoise, step_kind=self.step_kind)
+
+
 def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress, init_step, guidance_scale, cond_first,
                    clip_range, threshold_mode, inpaint_init, inpaint_mask, step_noise, callback, sample_generators,
-                   needs_noise=True, inpaint_renoise=False):
+                   needs_noise=True, inpaint_renoise=False, step_kind="ddpm"):
     """Shared host loop: `schedule` provides num_timesteps and _tables(device) -> (coef [n, 8], model timesteps [n])."""
     model_kwargs = dict(model_kwargs or {})
     if device is None:
@@ -157,7 +252,7 @@ def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress
         except ImportError:
             pass
     step = FusedStep(model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode, inpaint_init,
-                     inpaint_mask, inpaint_noise=x if inpaint_renoise else None)
+                     inpaint_mask, inpaint_noise=x if inpaint_renoise else None, step_kind=step_kind)
     order = [int(i) for i in indices]
     n = len(order)
     # the whole run's per-step noise is drawn up front (one stream per image when sample_generators are given, so an image's
@@ -312,10 +407,16 @@ class FusedStep:
     k2_step_begin (latent duplication for CFG, this step's t / coefficients / noise picked by a device-side counter), every
     launch of the UNet plan, k2_sampler_step and k2_step_end.  A 50-step call is 50 graph launches and nothing else (the
     reference syncs the device every step for np.percentile, gaussian_diffusion.py:288).
-    run(x, t, coef_row) is the step-at-a-time form (explicit timestep / coefficients; profiling scripts, PLMS)."""
+    run(x, t, coef_row) is the step-at-a-time form (explicit timestep / coefficients; profiling scripts, PLMS).
+    step_kind "ddpm" issues k2_sampler_step (DDPM, and DDIM through linear coefficients); "dpmpp_2m" issues
+    k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state."""
+
+    STEP_KINDS = ("ddpm", "dpmpp_2m")
 
     def __init__(self, model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode,
-                 inpaint_init=None, inpaint_mask=None, inpaint_noise=None):
+                 inpaint_init=None, inpaint_mask=None, inpaint_noise=None, step_kind="ddpm"):
+        if step_kind not in self.STEP_KINDS:
+            raise K2Error(f"FusedStep: unknown step kind {step_kind!r}")
         self.model = model
         if model._packed is None:
             model.finalize()
@@ -326,10 +427,12 @@ class FusedStep:
         dev = self.plan.dev
         self.B = B
         self.guidance, self.cond_first, self.clip, self.mode = guidance_scale, int(cond_first), clip_range, threshold_mode
+        self.step_kind = step_kind
+        dpm = step_kind == "dpmpp_2m"
         has_inpaint = inpaint_init is not None
         # buffers and the captured step graph live on the plan, keyed by everything the graph bakes in as a kernel argument
         renoise = inpaint_noise is not None
-        key = (float(guidance_scale), int(cond_first), float(clip_range), int(threshold_mode), has_inpaint, renoise)
+        key = (float(guidance_scale), int(cond_first), float(clip_range), int(threshold_mode), has_inpaint, renoise, step_kind)
         states = self.plan.__dict__.setdefault("_step_states", {})
         st = states.get(key)
         if st is None:
@@ -339,7 +442,8 @@ class FusedStep:
                       ts_seq=torch.zeros(4096, **f32), coef_seq=torch.zeros(4096, 8, **f32), noise_seq=None, graph=None,
                       init=torch.zeros(B, 4, H, W, **f32) if has_inpaint else None,
                       mask=torch.zeros(B, 1, H, W, **f32) if has_inpaint else None, x=torch.zeros(B, 4, H, W, **f32),
-                      rnoise=torch.zeros(B, 4, H, W, **f32) if renoise else None)
+                      rnoise=torch.zeros(B, 4, H, W, **f32) if renoise else None,
+                      hist=torch.zeros(B, 4, H, W, **f32) if dpm else None)
             states[key] = st
         self.st = st
         self.noise, self.coef, self.work = st["noise"], st["coef"], st["work"]
@@ -372,6 +476,13 @@ class FusedStep:
             st["noise_seq"][:n].copy_(noise_seq)
         self._use_noise_seq = noise_seq is not None
         st["counter"].copy_(torch.tensor([0, n], dtype=torch.int32))
+        if st["hist"] is not None:
+            st["hist"].zero_()
+
+    def _update(self, x):
+        """The DPM-Solver++ update of the step (the DDPM one is issued by _launch_step / run themselves)."""
+        ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init, self.mask,
+                            self.rnoise)
 
     def _launch_step(self, x, noise_seq, plan_graph=False):
         st, p = self.st, self.plan
@@ -381,7 +492,9 @@ class FusedStep:
         else:
             p.launch()
         args = (p.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip)
-        if self._sync_threshold():
+        if self.step_kind == "dpmpp_2m":
+            self._update(x)
+        elif self._sync_threshold():
             # Kandinsky 2.1 dynamic threshold under sharding: the reference clips the whole batch with the 99.5 % quantile of
             # GLOBAL sample 0 (gaussian_diffusion.py:288-292), which lives on rank 0 -> x0 (+ the quantile on rank 0), ONE
             # 4-byte broadcast, then the update
@@ -439,8 +552,11 @@ class FusedStep:
         p.t_in.copy_(t_scalar.expand_as(p.t_in))
         self.coef.copy_(coef_row)
         p.run(self.model.use_cuda_graph)
-        ops.sampler_step(p.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip, self.mode,
-                         self.init, self.mask, self.work, self.rnoise)
+        if self.step_kind == "dpmpp_2m":
+            self._update(x)
+        else:
+            ops.sampler_step(p.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip, self.mode,
+                             self.init, self.mask, self.work, self.rnoise)
         return x
 
 

@@ -17,7 +17,8 @@ import torch
 
 from . import ops, parallel
 from ._native import K2Error
-from .model.gaussian_diffusion import DDIMSampler, PLMSSampler, create_ddpm_v22, create_gaussian_diffusion
+from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, PLMSSampler, create_ddpm_v22,
+                                       create_gaussian_diffusion)
 from .model.model_creation import create_model
 from .utils import prepare_image, prepare_mask, q_sample, uint8_to_pil
 from .vqgan import MOVQ
@@ -65,6 +66,20 @@ class SyntheticEmbedder:
 
 def _new_h_w_latent_21(h, w):  # kandinsky2_1_model.py:106-113 (latent side, /8)
     return math.ceil(h / 64) * 8, math.ceil(w / 64) * 8
+
+
+SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler", "dpmpp_2m_sampler")
+SAMPLERS_22 = ("ddpm_sampler", "dpmpp_2m_sampler")
+
+
+def _check_sampler(sampler, allowed):
+    if sampler not in allowed:
+        raise ValueError(f"unknown sampler {sampler!r}: use one of {', '.join(allowed)}")
+
+
+def _dpm_keep(num_steps, strength):
+    """img2img with DPM-Solver++: the last int(N * strength) evaluations run (at least 1)."""
+    return max(min(int(num_steps * strength), num_steps), 1)
 
 
 class _DecoderBase:
@@ -135,9 +150,10 @@ class Kandinsky2_1(_DecoderBase):
     @torch.no_grad()
     def generate_img(self, prompt, img_prompt, batch_size=1, diffusion=None, guidance_scale=7, init_step=None,
                      noise=None, init_img=None, img_mask=None, h=512, w=512, sampler="ddim_sampler", num_steps=50):
-        """kandinsky2_1_model.py:184-292. img_prompt = cat([cond image emb, zero image emb]) [2B, 768]."""
-        if sampler not in ("p_sampler", "ddim_sampler", "plms_sampler"):
-            raise ValueError("Only ddim_sampler and plms_sampler is available")
+        """kandinsky2_1_model.py:184-292. img_prompt = cat([cond image emb, zero image emb]) [2B, 768].
+        sampler="dpmpp_2m_sampler" runs DPM-Solver++(2M) over `num_steps` evaluations of diffusion's base schedule; with
+        init_step = s only the last s of them run (img2img), starting from `noise`."""
+        _check_sampler(sampler, SAMPLERS_21)
         new_h, new_w = self.get_new_h_w(h, w)
         rank, ws, lo, hi = self._shard(batch_size)
         B = hi - lo
@@ -166,6 +182,10 @@ class Kandinsky2_1(_DecoderBase):
                                               progress=False, model_kwargs=kw, init_step=init_step,
                                               guidance_scale=guidance_scale, cond_first=True, clip_denoised=True,
                                               sample_generators=self._generators(lo, hi), **inpaint)[:B]
+        elif sampler == "dpmpp_2m_sampler":  # inpainting: the known region replaces x0 inside the step, as in p_sampler
+            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step)
+            samples = sched.sample(self.model, (2 * B, 4, new_h, new_w), noise=noise, model_kwargs=kw, device=self.device,
+                                   guidance_scale=guidance_scale, cond_first=True, **inpaint)[:B]
         else:  # kandinsky2_1_model.py:259-284: DDIM / PLMS over the un-respaced schedule, eta 0
             cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
             samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, new_h, new_w), conditioning=kw,
@@ -190,6 +210,7 @@ class Kandinsky2_1(_DecoderBase):
     def generate_text2img(self, prompt, num_steps=100, batch_size=1, guidance_scale=7, h=512, w=512,
                           sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25", negative_prior_prompt="",
                           negative_decoder_prompt=""):
+        _check_sampler(sampler, SAMPLERS_21)
         image_emb = self._image_embs(prompt, batch_size, negative_decoder_prompt)
         return self.generate_img(prompt=prompt, img_prompt=image_emb, batch_size=batch_size,
                                  guidance_scale=guidance_scale, h=h, w=w, sampler=sampler, num_steps=num_steps,
@@ -198,6 +219,7 @@ class Kandinsky2_1(_DecoderBase):
     def mix_images(self, images_texts, weights, num_steps=100, batch_size=1, guidance_scale=7, h=512, w=512,
                    sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25", negative_prior_prompt="",
                    negative_decoder_prompt=""):
+        _check_sampler(sampler, SAMPLERS_21)
         assert len(images_texts) == len(weights) and len(images_texts) > 0
         pos = self.embedder.interpolate(images_texts, weights, batch_size)
         image_emb = torch.cat([pos, self.embedder.zero_image_emb(batch_size)], 0)
@@ -208,15 +230,22 @@ class Kandinsky2_1(_DecoderBase):
 
     def generate_img2img(self, prompt, pil_img, strength=0.7, num_steps=100, batch_size=1, guidance_scale=7, h=512,
                          w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25"):
-        """kandinsky2_1_model.py:428-484: encode the image, noise it to step int(T*(1-strength)) and run the remaining steps."""
+        """kandinsky2_1_model.py:428-484: encode the image, noise it to step int(T*(1-strength)) and run the remaining steps.
+        With sampler="dpmpp_2m_sampler" the last int(num_steps*strength) solver evaluations run (at least 1), from the image
+        noised to the first of them."""
+        _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        start_step = int(diffusion.num_timesteps * (1 - strength))
         g = torch.Generator().manual_seed(self.base_seed)
         noise = torch.randn(image.shape, generator=g).to(self.device)
-        dc = self.config["diffusion_config"]
-        x = q_sample(image, diffusion.timestep_map[start_step - 1], schedule_name=dc["noise_schedule"],
-                     num_steps=dc["steps"], noise=noise)
+        if sampler == "dpmpp_2m_sampler":
+            start_step = _dpm_keep(num_steps, strength)
+            x = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=start_step).start_latent(image, noise)
+        else:
+            start_step = int(diffusion.num_timesteps * (1 - strength))
+            dc = self.config["diffusion_config"]
+            x = q_sample(image, diffusion.timestep_map[start_step - 1], schedule_name=dc["noise_schedule"],
+                         num_steps=dc["steps"], noise=noise)
         x = x.repeat(2 * batch_size, 1, 1, 1)
         image_emb = self._image_embs(prompt, batch_size)
         return self.generate_img(prompt=prompt, img_prompt=image_emb, batch_size=batch_size,
@@ -227,6 +256,7 @@ class Kandinsky2_1(_DecoderBase):
                             w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25",
                             negative_prior_prompt="", negative_decoder_prompt=""):
         """kandinsky2_1_model.py:487-548 (mask: 1 = keep, nearest-resized to the latent grid, then prepare_mask)."""
+        _check_sampler(sampler, SAMPLERS_21)
         image = self._encode_image(pil_img, h, w) * self.scale
         m = torch.as_tensor(img_mask).float()[None, None]
         m = torch.nn.functional.interpolate(m, tuple(image.shape[-2:]), mode="nearest")
@@ -246,9 +276,12 @@ class Kandinsky2_2(_DecoderBase):
 
     @torch.no_grad()
     def _decode_loop(self, image_embeds, negative_embeds, batch_size, steps, guidance, h, w, latents=None,
-                     inpaint_latent=None, inpaint_mask=None, init_step=None, hint=None):
+                     inpaint_latent=None, inpaint_mask=None, init_step=None, hint=None, sampler="ddpm_sampler"):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
-        106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold."""
+        106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
+        sampler="dpmpp_2m_sampler": DPM-Solver++(2M) over `steps` evaluations of the same base schedule instead (init_step =
+        the number of evaluations kept for img2img); inpainting re-noises the known region to the next timestep."""
+        _check_sampler(sampler, SAMPLERS_22)
         H, W = h // 8, w // 8
         rank, ws, lo, hi = self._shard(batch_size)
         B = hi - lo
@@ -274,9 +307,14 @@ class Kandinsky2_2(_DecoderBase):
                          inpaint_mask=inpaint_mask.repeat(B, 1, 1, 1).to(self.device), inpaint_renoise=True)
         diffusion = create_ddpm_v22(steps)
         self.model.del_cache()
-        out = diffusion.p_sample_loop(self.model, (2 * B, 4, H, W), device=self.device, noise=latents,
-                                      model_kwargs=kw, guidance_scale=guidance, cond_first=False, clip_denoised=False,
-                                      init_step=init_step, sample_generators=self._generators(lo, hi), **extra)[:B]
+        if sampler == "dpmpp_2m_sampler":
+            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, steps, keep=init_step)
+            out = sched.sample(self.model, (2 * B, 4, H, W), noise=latents, model_kwargs=kw, device=self.device,
+                               guidance_scale=guidance, cond_first=False, **extra)[:B]
+        else:
+            out = diffusion.p_sample_loop(self.model, (2 * B, 4, H, W), device=self.device, noise=latents,
+                                          model_kwargs=kw, guidance_scale=guidance, cond_first=False, clip_denoised=False,
+                                          init_step=init_step, sample_generators=self._generators(lo, hi), **extra)[:B]
         self.model.del_cache()
         return self._finish(out, h, w)
 
@@ -287,41 +325,50 @@ class Kandinsky2_2(_DecoderBase):
         return pos, neg
 
     def generate_text2img(self, prompt, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
-                          prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt=""):
+                          prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
+                          sampler="ddpm_sampler"):
+        _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
-        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w)
+        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, sampler=sampler)
 
     def mix_images(self, images_texts, weights, batch_size=1, decoder_steps=50, prior_steps=25,
                    decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
-                   negative_decoder_prompt=""):
+                   negative_decoder_prompt="", sampler="ddpm_sampler"):
+        _check_sampler(sampler, SAMPLERS_22)
         assert len(images_texts) == len(weights) and len(images_texts) > 0
         pos = self.embedder.interpolate(images_texts, weights, batch_size)
         _, neg = self._embeds("", batch_size, negative_decoder_prompt)
-        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w)
+        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, sampler=sampler)
 
     def generate_img2img(self, prompt, image, strength=0.4, batch_size=1, decoder_steps=100, prior_steps=25,
                          decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
-                         negative_decoder_prompt=""):
+                         negative_decoder_prompt="", sampler="ddpm_sampler"):
+        _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
         # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first of them
         start = max(min(int(decoder_steps * strength), decoder_steps), 1)
-        ac = float(diffusion.alphas_cumprod[start - 1])
         g = torch.Generator().manual_seed(self.base_seed)
         noise = torch.randn(lat.shape, generator=g).to(self.device)
-        x = ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * noise
+        if sampler == "dpmpp_2m_sampler":
+            x = DPMSolverSchedule(diffusion.base_alphas_cumprod, decoder_steps, keep=start).start_latent(lat, noise)
+        else:
+            ac = float(diffusion.alphas_cumprod[start - 1])
+            x = ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * noise
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
-                                 latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start)
+                                 latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, sampler=sampler)
 
     def generate_controlnet(self, prompt, hint, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
-                            prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt=""):
+                            prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
+                            sampler="ddpm_sampler"):
         """Kandinsky 2.2 ControlNet-depth (BASELINE configs[4]).  The reference package has no method for it -- its
         notebooks/kandinsky2_2_controlnet.ipynb calls diffusers' KandinskyV22ControlnetPipeline(image_embeds=...,
         negative_image_embeds=..., hint=hint, height=h, width=w) directly -- so this follows the sibling methods' signature.
         hint: depth map tensor [1, 3, h, w] in [0, 1] (the pipeline object must be built with task_type="controlnet")."""
+        _check_sampler(sampler, SAMPLERS_22)
         if self.task_type != "controlnet":
             raise ValueError("generate_controlnet needs a pipeline built with task_type='controlnet'")
         h, w = self.get_new_h_w(h, w)
@@ -331,15 +378,16 @@ class Kandinsky2_2(_DecoderBase):
             hint = hint[None]
         if tuple(hint.shape[-2:]) != (h, w):
             hint = torch.nn.functional.interpolate(hint, (h, w), mode="bilinear", align_corners=False)
-        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, hint=hint)
+        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, hint=hint, sampler=sampler)
 
     def generate_inpainting(self, prompt, pil_img, img_mask, batch_size=1, decoder_steps=50, prior_steps=25,
                             decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
-                            negative_decoder_prompt=""):
+                            negative_decoder_prompt="", sampler="ddpm_sampler"):
+        _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
         lat = self._encode_image(pil_img, h, w)
         m = torch.as_tensor(img_mask).float()[None, None]
         m = torch.nn.functional.interpolate(m, (h // 8, w // 8), mode="nearest").to(self.device)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
-                                 inpaint_latent=lat, inpaint_mask=m)
+                                 inpaint_latent=lat, inpaint_mask=m, sampler=sampler)

@@ -1,0 +1,158 @@
+"""Cost of the DPM-Solver++(2M) sampler against the default DDPM one at the cfg-2 geometry (Kandinsky 2.2 decoder, 768x768,
+4 images, guidance 4, the full-size UNet with random weights of the architecture).
+
+Measures, in one process on cuda:0, and prints one JSON line (also written to --out if given):
+  * whole-call images/s through Kandinsky2_2.generate_text2img (latent init, the denoising steps, MoVQ decode, uint8 + PIL) for
+    sampler="ddpm_sampler" x 50 steps and sampler="dpmpp_2m_sampler" x 20 and x 25: CUDA events, median of --calls
+    steady-state calls after one warm-up call per arm;
+  * graph-replayed steps/s of each sampler's step (k2_step_begin + UNet + k2_sampler_step or k2_dpm_solver_step +
+    k2_step_end, one graph launch per step), the two arms alternated --rounds times in this process;
+  * device time of one k2_dpm_solver_step and one k2_sampler_step launch (threshold mode 0, as the 2.2 step issues it) at this
+    geometry: CUDA events over --kernel-reps back-to-back launches.
+The card's name, power limit and maximum SM clock are read in the same run (nvidia-smi query only).  Needs a CUDA sm_90 device.
+
+    python profiles/sampler_steps.py [--out /tmp/sampler_steps.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "kandinsky-2_b200")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+import torch  # noqa: E402
+
+
+def _card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(0)
+
+
+def _events_ms(fn, reps):
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    s.record()
+    for _ in range(reps):
+        fn()
+    e.record()
+    torch.cuda.synchronize()
+    return s.elapsed_time(e)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50, help="timed graph replays per steps/s measurement")
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--calls", type=int, default=3)
+    ap.add_argument("--kernel-reps", type=int, default=2000)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("needs a CUDA sm_90 device")
+    from bench import _init_pipe_with_model, build_unet
+    from kandinsky2 import ops
+    from kandinsky2.configs import CONFIG_2_2
+    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, FusedStep, create_ddpm_v22
+    from kandinsky2.pipelines import Kandinsky2_2
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    ops.set_tuning(4, 1)  # programmatic dependent launch, as bench.py runs the step
+    B, H, W = 4, 96, 96
+    model = build_unet(dev)
+    res = {"card": _card(), "torch": torch.__version__, "geometry": f"{B} images, {H}x{W} latents (768x768), guidance 4"}
+
+    # ---- graph-replayed steps/s, the two step kinds alternated
+    g = torch.Generator(device=dev).manual_seed(1234)
+    image_emb = torch.randn(2 * B, 1280, device=dev, generator=g)
+    ddpm = create_ddpm_v22(50)
+    dpm = DPMSolverSchedule(ddpm.base_alphas_cumprod, 20)
+    x_start = torch.randn(B, 4, H, W, device=dev, generator=g)
+    noise = torch.randn(50, B, 4, H, W, device=dev, generator=g)
+    arms = {}
+    for name, sched, kind, nseq in (("ddpm_sampler", ddpm, "ddpm", noise), ("dpmpp_2m_sampler", dpm, "dpmpp_2m", None)):
+        coef, ts = sched._tables(dev)
+        order = torch.arange(sched.num_timesteps - 1, -1, -1, device=dev)
+        step = FusedStep(model, B, H, W, dict(image_emb=image_emb), guidance_scale=4.0, cond_first=False, clip_range=2.0,
+                         threshold_mode=0, step_kind=kind)
+        arms[name] = (step, ts[order], coef[order], nseq)
+    sps = {name: [] for name in arms}
+    for _ in range(args.rounds):
+        for name, (step, ts_seq, coef_seq, nseq) in arms.items():
+            step.set_schedule(ts_seq, coef_seq, nseq)
+            x = step.latent()
+            x.copy_(x_start)
+            for _ in range(args.warmup):
+                step.advance(x)
+            ms = _events_ms(lambda: step.advance(x), args.steps)
+            sps[name].append(round(1e3 * args.steps / ms, 3))
+    res["steps_per_s"] = sps
+    res["steps_per_s_note"] = (f"{args.steps} graph replays per run after {args.warmup} warm-up replays, arms alternated "
+                               f"{args.rounds} times; the DPM++ schedule wraps around its 20 rows")
+
+    # ---- step-kernel device time
+    mo = torch.randn(2 * B, 8, H, W, device=dev, generator=g)
+    xk = torch.randn(B, 4, H, W, device=dev, generator=g)
+    hist = torch.randn(B, 4, H, W, device=dev, generator=g)
+    nz = torch.randn(B, 4, H, W, device=dev, generator=g)
+    work = torch.empty(B * 4 * H * W + 4096, device=dev)
+    coef_ddpm = ddpm._tables(dev)[0][25].clone()
+    coef_dpm = dpm._tables(dev)[0][10].clone()
+    assert float(coef_dpm[4]) != 0.0   # a second-order row: the history is read
+    kern = {"k2_sampler_step": lambda: ops.sampler_step(mo, xk, nz, coef_ddpm, 4.0, False, 2.0, 0, work=work),
+            "k2_dpm_solver_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_dpm, 4.0, False)}
+    kt = {}
+    for name, fn in kern.items():
+        fn()
+        _events_ms(fn, 50)
+    for name, fn in kern.items():
+        kt[name] = {"us_per_launch": round(1e3 * _events_ms(fn, args.kernel_reps) / args.kernel_reps, 3)}
+    n = B * 4 * H * W
+    # fp32 words moved per latent element: DDPM reads cond + uncond eps, the variance, x (twice: one per kernel), the noise,
+    # writes and re-reads x0 through a scratch buffer and writes x = 9; DPM++ reads cond + uncond eps, x and hist and writes
+    # x and hist = 6
+    kt["k2_sampler_step"]["bytes"] = 4 * n * 9
+    kt["k2_dpm_solver_step"]["bytes"] = 4 * n * 6
+    for v in kt.values():
+        v["achieved_GBps"] = round(v["bytes"] / (v["us_per_launch"] * 1e-6) / 1e9, 1)
+    res["step_kernel"] = kt
+    res["step_kernel_note"] = f"CUDA events over {args.kernel_reps} back-to-back launches of each kernel, cfg-2 geometry"
+
+    # ---- whole-call images/s through the public pipeline
+    arms.clear()
+    model.del_cache()
+    pipe = Kandinsky2_2.__new__(Kandinsky2_2)
+    _init_pipe_with_model(pipe, CONFIG_2_2, dev, model)
+    calls = {}
+    for sampler, steps in (("ddpm_sampler", 50), ("dpmpp_2m_sampler", 20), ("dpmpp_2m_sampler", 25)):
+        ms_all = []
+        for it in range(args.calls + 1):   # call 0 builds plans / graphs
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            s.record()
+            pipe.generate_text2img("bench", batch_size=B, decoder_steps=steps, decoder_guidance_scale=4, h=768, w=768,
+                                   sampler=sampler)
+            e.record()
+            torch.cuda.synchronize()
+            if it > 0:
+                ms_all.append(s.elapsed_time(e))
+        med = sorted(ms_all)[len(ms_all) // 2]
+        calls[f"{sampler} x {steps}"] = {"images_per_s": round(B / (med * 1e-3), 3), "ms_per_call": round(med, 1),
+                                         "ms_per_call_all": [round(v, 1) for v in ms_all]}
+    res["images_per_s"] = calls
+    res["images_note"] = f"median of {args.calls} steady-state calls (CUDA events) after one warm-up call per arm"
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
