@@ -253,24 +253,38 @@ struct SamplerParams {
   float* sval;             // work scalar (dynamic threshold s)
 };
 
+// Element i of a [B, 4, HW] latent: its sample b, its pixel sp and the CFG epsilon eu + g (ec - eu) of its channel, read from the
+// eps channels of model_out [2B, C2, HW] (the conditional rows come first when cond_first; kandinsky2_1_model.py:222-233)
+struct CfgElem {
+  int b, sp;
+  float eps;
+};
+
+__device__ __forceinline__ CfgElem cfg_elem(const float* model_out, long long i, int B, int HW, int C2, float guidance,
+                                            int cond_first) {
+  CfgElem e;
+  e.sp = static_cast<int>(i % HW);
+  const int c = static_cast<int>((i / HW) % 4);
+  e.b = static_cast<int>(i / (4LL * HW));
+  const int bc = cond_first ? e.b : e.b + B;
+  const int bu = cond_first ? e.b + B : e.b;
+  const float ec = model_out[(static_cast<long long>(bc) * C2 + c) * HW + e.sp];
+  const float eu = model_out[(static_cast<long long>(bu) * C2 + c) * HW + e.sp];
+  e.eps = eu + guidance * (ec - eu);
+  return e;
+}
+
 __global__ void __launch_bounds__(256) sampler_x0_kernel(const SamplerParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
-  const int sp = static_cast<int>(i % p.HW);
-  const int c = static_cast<int>((i / p.HW) % 4);
-  const int b = static_cast<int>(i / (4LL * p.HW));
-  const int bc = p.cond_first ? b : b + p.B;
-  const int bu = p.cond_first ? b + p.B : b;
-  const float ec = p.model_out[(static_cast<long long>(bc) * 8 + c) * p.HW + sp];
-  const float eu = p.model_out[(static_cast<long long>(bu) * 8 + c) * p.HW + sp];
-  const float eps = eu + p.guidance * (ec - eu);
-  float x0 = p.coef[0] * p.x[i] - p.coef[1] * eps;
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, 8, p.guidance, p.cond_first);
+  float x0 = p.coef[0] * p.x[i] - p.coef[1] * e.eps;
   x0 = fminf(fmaxf(x0, -p.clip), p.clip);
   if (p.mask && !p.rnoise) {  // Kandinsky 2.1: the known region replaces x0 (denoised_fun, kandinsky2_1_model.py:237-243)
-    const float m = p.mask[static_cast<long long>(b) * p.HW + sp];
+    const float m = p.mask[static_cast<long long>(e.b) * p.HW + e.sp];
     x0 = x0 * (1.f - m) + p.init[i] * m;
   }
   p.x0[i] = x0;
@@ -386,14 +400,7 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const PlmsParams p) {
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
-  const int sp = static_cast<int>(i % p.HW);
-  const int c = static_cast<int>((i / p.HW) % 4);
-  const int b = static_cast<int>(i / (4LL * p.HW));
-  const int bc = p.cond_first ? b : b + p.B;
-  const int bu = p.cond_first ? b + p.B : b;
-  const float ec = p.model_out[(static_cast<long long>(bc) * p.C2 + c) * p.HW + sp];
-  const float eu = p.model_out[(static_cast<long long>(bu) * p.C2 + c) * p.HW + sp];
-  const float e_t = eu + p.guidance * (ec - eu);
+  const float e_t = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, p.guidance, p.cond_first).eps;
   float ep = p.coef[4] * e_t;
   if (p.hist[0]) ep = fmaf(p.coef[5], p.hist[0][i], ep);
   if (p.hist[1]) ep = fmaf(p.coef[6], p.hist[1][i], ep);
@@ -428,17 +435,10 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p)
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
-  const int sp = static_cast<int>(i % p.HW);
-  const int c = static_cast<int>((i / p.HW) % 4);
-  const int b = static_cast<int>(i / (4LL * p.HW));
-  const int bc = p.cond_first ? b : b + p.B;
-  const int bu = p.cond_first ? b + p.B : b;
-  const float ec = p.model_out[(static_cast<long long>(bc) * p.C2 + c) * p.HW + sp];
-  const float eu = p.model_out[(static_cast<long long>(bu) * p.C2 + c) * p.HW + sp];
-  const float eps = eu + p.guidance * (ec - eu);
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, p.guidance, p.cond_first);
   const float xv = p.x[i];
-  float x0 = p.coef[0] * xv - p.coef[1] * eps;
-  const float m = p.mask ? p.mask[static_cast<long long>(b) * p.HW + sp] : 0.f;
+  float x0 = p.coef[0] * xv - p.coef[1] * e.eps;
+  const float m = p.mask ? p.mask[static_cast<long long>(e.b) * p.HW + e.sp] : 0.f;
   if (p.mask && !p.rnoise) x0 = x0 * (1.f - m) + p.init[i] * m;  // Kandinsky 2.1: the known region replaces x0
   float xn = p.coef[2] * xv + p.coef[3] * x0;
   const float cp = p.coef[4];

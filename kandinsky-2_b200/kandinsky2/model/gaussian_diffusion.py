@@ -47,7 +47,24 @@ def space_timesteps(num_timesteps, section_counts):
     return set(steps)
 
 
-class SpacedDiffusion:
+class _Schedule:
+    """What _sampling_loop needs of a schedule: coef_table() (fp32 [n, 8] step-kernel rows) and model_timesteps() (what the UNet
+    sees, [n]) in the same index order; the loop runs the rows n-1 .. 0.  Each schedule also states whether its step draws
+    noise and which step kernel applies its rows ("ddpm": k2_sampler_step, "dpmpp_2m": k2_dpm_solver_step)."""
+
+    draws_noise = True
+    step_kind = "ddpm"
+
+    def _tables(self, device):
+        """-> (coef fp32 [n, 8], model timesteps fp32 [n]) on `device`, built once per device."""
+        key = str(device)
+        if key not in self._dev_tables:
+            self._dev_tables[key] = (torch.from_numpy(self.coef_table()).to(device),
+                                     torch.from_numpy(np.ascontiguousarray(self.model_timesteps(), dtype=np.float32)).to(device))
+        return self._dev_tables[key]
+
+
+class SpacedDiffusion(_Schedule):
     """Learned-range / epsilon diffusion over a subset of the base timesteps (respace.py:75-118)."""
 
     def __init__(self, use_timesteps, betas, rescale_timesteps=False):
@@ -76,15 +93,14 @@ class SpacedDiffusion:
         self.posterior_mean_coef2 = (1.0 - acp) * np.sqrt(alphas) / (1.0 - ac)
         self._dev_tables = {}
 
-    @staticmethod
-    def truncate(indices, init_step):
-        return indices[:init_step]
-
     # -- per-step scalars ----------------------------------------------------------------------
     def model_timestep(self, i):
         """What the UNet sees for step index i (respace.py:128-133)."""
         t = float(self.timestep_map[i])
         return t * (1000.0 / self.original_num_steps) if self.rescale_timesteps else t
+
+    def model_timesteps(self):
+        return [self.model_timestep(i) for i in range(self.num_timesteps)]
 
     def coef_table(self):
         """float32 [num_timesteps, 8]: the k2_sampler_step coefficient rows (include/k2b200.h)."""
@@ -99,15 +115,6 @@ class SpacedDiffusion:
         tab[:, 6] = (np.arange(n) != 0).astype(np.float64)
         tab[:, 7] = np.sqrt(self.alphas_cumprod_prev)  # 2.2 inpainting: the known region is re-noised to the NEXT timestep
         return tab.astype(np.float32)  # the reference casts each extracted scalar with .float() (:825-826)
-
-    def _tables(self, device):
-        key = str(device)
-        if key not in self._dev_tables:
-            coef = torch.from_numpy(self.coef_table()).to(device)
-            ts = torch.tensor([self.model_timestep(i) for i in range(self.num_timesteps)], dtype=torch.float32,
-                              device=device)
-            self._dev_tables[key] = (coef, ts)
-        return self._dev_tables[key]
 
     # -- the loop ------------------------------------------------------------------------------
     @torch.no_grad()
@@ -129,12 +136,14 @@ class SpacedDiffusion:
         run's INITIAL noise; the last step blends with the clean latent)."""
         if denoised_fn is not None:
             raise K2Error("denoised_fn closures are fused: pass clip_range / inpaint_init / inpaint_mask instead")
-        return _sampling_loop(self, model, shape, noise, model_kwargs, device, progress, init_step, guidance_scale,
-                              cond_first, clip_range, 1 if clip_denoised else 0, inpaint_init, inpaint_mask, step_noise,
-                              callback, sample_generators, inpaint_renoise=inpaint_renoise)
+        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device, progress=progress,
+                              init_step=init_step, guidance_scale=guidance_scale, cond_first=cond_first, clip_range=clip_range,
+                              threshold_mode=1 if clip_denoised else 0, inpaint_init=inpaint_init, inpaint_mask=inpaint_mask,
+                              inpaint_renoise=inpaint_renoise, step_noise=step_noise, sample_generators=sample_generators,
+                              callback=callback)
 
 
-class DPMSolverSchedule:
+class DPMSolverSchedule(_Schedule):
     """DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models",
     Algorithm 2) over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step, no noise.
 
@@ -151,6 +160,7 @@ class DPMSolverSchedule:
     Rows are stored in reverse step order (table index j = N-1-k) so that _sampling_loop, which walks the indices from the
     top down like the DDPM schedules', runs k = k0 .. N-1."""
 
+    draws_noise = False
     step_kind = "dpmpp_2m"
 
     def __init__(self, base_alphas_cumprod, num_steps, keep=None):
@@ -203,17 +213,6 @@ class DPMSolverSchedule:
         """float32 [keep]: what the UNet sees, in table order."""
         return self.timesteps[self.k0:][::-1].astype(np.float32)
 
-    def _tables(self, device):
-        key = str(device)
-        if key not in self._dev_tables:
-            self._dev_tables[key] = (torch.from_numpy(self.coef_table()).to(device),
-                                     torch.from_numpy(np.ascontiguousarray(self.model_timesteps())).to(device))
-        return self._dev_tables[key]
-
-    @staticmethod
-    def truncate(indices, init_step):
-        return indices  # `keep` already applied to the tables in __init__
-
     def start_latent(self, latent, noise):
         """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
         return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
@@ -224,15 +223,16 @@ class DPMSolverSchedule:
         """shape = (2*B, 4, h, w) (CFG doubled), noise = the start latent [2B or B, ...]; returns [2*B, 4, h, w] whose two halves
         both hold the B samples, like p_sample_loop.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces x0),
         True = Kandinsky 2.2 (the known region is re-noised to the next timestep with the start latent as the noise)."""
-        return _sampling_loop(self, model, shape, noise, model_kwargs, device, False, None, guidance_scale, cond_first, 1e30, 0,
-                              inpaint_init, inpaint_mask, None, callback, None, needs_noise=False,
-                              inpaint_renoise=inpaint_renoise, step_kind=self.step_kind)
+        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
+                              guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
+                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback)
 
 
-def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress, init_step, guidance_scale, cond_first,
-                   clip_range, threshold_mode, inpaint_init, inpaint_mask, step_noise, callback, sample_generators,
-                   needs_noise=True, inpaint_renoise=False, step_kind="ddpm"):
-    """Shared host loop: `schedule` provides num_timesteps and _tables(device) -> (coef [n, 8], model timesteps [n])."""
+def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,
+                   clip_range=1e30, threshold_mode=0, init_step=None, inpaint_init=None, inpaint_mask=None,
+                   inpaint_renoise=False, step_noise=None, sample_generators=None, callback=None, progress=False):
+    """Shared host loop over the rows n-1 .. 0 of a _Schedule, n = init_step when given (SpacedDiffusion img2img; the other
+    schedules cut their tables themselves), else num_timesteps."""
     model_kwargs = dict(model_kwargs or {})
     if device is None:
         device = next(model.parameters()).device
@@ -241,10 +241,10 @@ def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress
     x_full = noise.float().to(device) if noise is not None else torch.randn(*shape, device=device)
     x = x_full[:B].clone()  # the caller's noise tensor is left untouched, like the reference
     coef, ts = schedule._tables(device)
-    indices = list(range(schedule.num_timesteps))
+    order = list(range(schedule.num_timesteps))
     if init_step is not None:
-        indices = schedule.truncate(indices, init_step)
-    indices = indices[::-1]
+        order = order[:init_step]
+    order = order[::-1]
     tqdm = None
     if progress:
         try:
@@ -252,12 +252,11 @@ def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress
         except ImportError:
             pass
     step = FusedStep(model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode, inpaint_init,
-                     inpaint_mask, inpaint_noise=x if inpaint_renoise else None, step_kind=step_kind)
-    order = [int(i) for i in indices]
+                     inpaint_mask, inpaint_noise=x if inpaint_renoise else None, step_kind=schedule.step_kind)
     n = len(order)
     # the whole run's per-step noise is drawn up front (one stream per image when sample_generators are given, so an image's
     # noise does not depend on which rank / batch position it runs at) and indexed by the device-side step counter
-    if not needs_noise:
+    if not schedule.draws_noise:
         step.noise.zero_()
         noise_seq = None
     elif step_noise is not None:
@@ -281,7 +280,7 @@ def _sampling_loop(schedule, model, shape, noise, model_kwargs, device, progress
     return torch.cat([x, x], 0)
 
 
-class DDIMSampler:
+class DDIMSampler(_Schedule):
     """DDIM (eta = 0) over the un-respaced schedule, as the reference's default `sampler="ddim_sampler"` path uses it
     (kandinsky2/model/samplers.py:68-331; called from kandinsky2_1_model.py:259-275).
 
@@ -294,11 +293,12 @@ class DDIMSampler:
     reference's own DDIMSampler / PLMSSampler classes (tests/golden/ddim_tiny.pt, plms_tiny.pt; their hard-coded "cuda"
     device, :78-79,101,226, is remapped to the CPU by the generating script, oracle/make_golden.py)."""
 
+    draws_noise = False
+
     def __init__(self, model, old_diffusion, schedule="linear", **kwargs):
         self.model = model
         self.old_diffusion = old_diffusion
         self.ddpm_num_timesteps = old_diffusion.original_num_steps
-        self._dev_tables = {}
 
     def make_schedule(self, ddim_num_steps, ddim_eta=0.0, init_step=None):
         if ddim_eta != 0.0:
@@ -312,7 +312,7 @@ class DDIMSampler:
         self.ddim_alphas = acp[t]
         self.ddim_alphas_prev = np.asarray([acp[0]] + acp[t[:-1]].tolist())
         self.num_timesteps = len(t)
-        self._dev_tables = {}
+        self._dev_tables = {}  # the device tables of the previous schedule are stale
 
     def coef_table(self):
         a_t, a_p = self.ddim_alphas, self.ddim_alphas_prev
@@ -324,16 +324,8 @@ class DDIMSampler:
         tab[:, 3] = np.sqrt(1.0 - a_p) / s1
         return tab.astype(np.float32)  # columns 4-6 zero: log-variance terms unused, noise switched off
 
-    def _tables(self, device):
-        key = str(device)
-        if key not in self._dev_tables:
-            self._dev_tables[key] = (torch.from_numpy(self.coef_table()).to(device),
-                                     torch.tensor(self.ddim_timesteps.astype(np.float32), device=device))
-        return self._dev_tables[key]
-
-    @staticmethod
-    def truncate(indices, init_step):
-        return indices  # init_step already applied to the timestep list in make_schedule
+    def model_timesteps(self):
+        return self.ddim_timesteps
 
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, eta=0.0, x_T=None, init_step=None, *, guidance_scale=1.0,
@@ -341,8 +333,8 @@ class DDIMSampler:
         """-> (samples [batch_size, C, H, W], {}) like the reference (batch_size is the CFG-doubled batch)."""
         self.make_schedule(S, ddim_eta=eta, init_step=init_step)
         C, H, W = shape
-        out = _sampling_loop(self, self.model, (batch_size, C, H, W), x_T, conditioning, None, False, None, guidance_scale,
-                             cond_first, 1e30, 0, None, None, None, callback, None, needs_noise=False)
+        out = _sampling_loop(self, self.model, (batch_size, C, H, W), noise=x_T, model_kwargs=conditioning,
+                             guidance_scale=guidance_scale, cond_first=cond_first, callback=callback)
         return out, {}
 
 
@@ -364,7 +356,6 @@ class PLMSSampler(DDIMSampler):
         x_full = x_T.float().to(device) if x_T is not None else torch.randn(batch_size, C, H, W, device=device)
         x = x_full[:B].clone()  # the caller's noise tensor is left untouched, like the reference
         step = FusedStep(model, B, H, W, dict(conditioning or {}), guidance_scale, cond_first, 1e30, 0)
-        plan = step.plan
         a_t, a_p = self.ddim_alphas, self.ddim_alphas_prev
         ts = self.ddim_timesteps.astype(np.float32)
         n = self.num_timesteps
@@ -373,23 +364,16 @@ class PLMSSampler(DDIMSampler):
             row = [1.0 / np.sqrt(a_t[i]), np.sqrt(1.0 - a_t[i]) / np.sqrt(a_t[i]), np.sqrt(a_p[i]), np.sqrt(1.0 - a_p[i])] + list(w)
             return torch.tensor(row, dtype=torch.float32, device=device)
 
-        def forward(xin, t):
-            plan.x_in[:B].copy_(xin)
-            plan.x_in[B:].copy_(xin)
-            plan.t_in.fill_(float(t))
-            plan.run(model.use_cuda_graph)
-            return plan.out
-
         hist = []                                      # newest first
         ring = [torch.empty_like(x) for _ in range(4)]  # epsilon history slots (3 live + the one being written)
         x_tmp = torch.empty_like(x)
         for it, i in enumerate(range(n)[::-1]):
             slot = ring[it % 4]
-            mo = forward(x, ts[i])
+            mo = step.forward(x, float(ts[i]))
             if not hist:
                 # pseudo improved Euler: x' from e_t, second evaluation at t_next, then the step with (e_t + e_next) / 2
                 ops.plms_step(mo, x, x_tmp, [], slot, coef(i, (1.0, 0.0, 0.0, 0.0)), guidance_scale, cond_first)
-                mo2 = forward(x_tmp, ts[max(i - 1, 0)])
+                mo2 = step.forward(x_tmp, float(ts[max(i - 1, 0)]))
                 ops.plms_step(mo2, x, x, [slot], None, coef(i, (0.5, 0.5, 0.0, 0.0)), guidance_scale, cond_first)
             else:
                 ops.plms_step(mo, x, x, hist, slot, coef(i, self._AB[len(hist)]), guidance_scale, cond_first)
@@ -407,7 +391,8 @@ class FusedStep:
     k2_step_begin (latent duplication for CFG, this step's t / coefficients / noise picked by a device-side counter), every
     launch of the UNet plan, k2_sampler_step and k2_step_end.  A 50-step call is 50 graph launches and nothing else (the
     reference syncs the device every step for np.percentile, gaussian_diffusion.py:288).
-    run(x, t, coef_row) is the step-at-a-time form (explicit timestep / coefficients; profiling scripts, PLMS).
+    run(x, t, coef_row) is the step-at-a-time form (explicit timestep / coefficients); forward(x, t) is its UNet half alone
+    (PLMS, which applies its own update).
     step_kind "ddpm" issues k2_sampler_step (DDPM, and DDIM through linear coefficients); "dpmpp_2m" issues
     k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state."""
 
@@ -480,9 +465,26 @@ class FusedStep:
             st["hist"].zero_()
 
     def _update(self, x):
-        """The DPM-Solver++ update of the step (the DDPM one is issued by _launch_step / run themselves)."""
-        ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init, self.mask,
-                            self.rnoise)
+        """The scheduler update of x in place from the UNet output in plan.out, with the coefficient row in self.coef."""
+        if self.step_kind == "dpmpp_2m":
+            ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init,
+                                self.mask, self.rnoise)
+            return
+
+        def sampler_step(mode):
+            ops.sampler_step(self.plan.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip, mode,
+                             self.init, self.mask, self.work, self.rnoise)
+        if self._sync_threshold():
+            # Kandinsky 2.1 dynamic threshold under sharding: the reference clips the whole batch with the 99.5 % quantile of
+            # GLOBAL sample 0 (gaussian_diffusion.py:288-292), which lives on rank 0 -> x0 (+ the quantile on rank 0), ONE
+            # 4-byte broadcast, then the update
+            import torch.distributed as dist
+            sampler_step(2 if parallel.world()[0] == 0 else 4)
+            n = x.numel()
+            dist.broadcast(self.work[n:n + 1], src=0)
+            sampler_step(3)
+        else:
+            sampler_step(self.mode)
 
     def _launch_step(self, x, noise_seq, plan_graph=False):
         st, p = self.st, self.plan
@@ -491,20 +493,7 @@ class FusedStep:
             p.run(True)
         else:
             p.launch()
-        args = (p.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip)
-        if self.step_kind == "dpmpp_2m":
-            self._update(x)
-        elif self._sync_threshold():
-            # Kandinsky 2.1 dynamic threshold under sharding: the reference clips the whole batch with the 99.5 % quantile of
-            # GLOBAL sample 0 (gaussian_diffusion.py:288-292), which lives on rank 0 -> x0 (+ the quantile on rank 0), ONE
-            # 4-byte broadcast, then the update
-            import torch.distributed as dist
-            ops.sampler_step(*args, 2 if parallel.world()[0] == 0 else 4, self.init, self.mask, self.work, self.rnoise)
-            n = x.numel()
-            dist.broadcast(self.work[n:n + 1], src=0)
-            ops.sampler_step(*args, 3, self.init, self.mask, self.work, self.rnoise)
-        else:
-            ops.sampler_step(*args, self.mode, self.init, self.mask, self.work, self.rnoise)
+        self._update(x)
         ops.step_end(st["counter"])
 
     def _sync_threshold(self):
@@ -543,20 +532,20 @@ class FusedStep:
         return self.st["x"]
 
     # -- step-at-a-time mode ----------------------------------------------------------------------
-    def run(self, x, t_scalar, coef_row):
-        """x fp32 [B,4,H,W] is updated in place to x_{t-1}."""
-        p = self.plan
-        B = self.B
+    def forward(self, x, t):
+        """CFG-doubled UNet forward of x fp32 [B,4,H,W] at timestep t (a number, or a 0-d tensor on the device) -> plan.out."""
+        p, B = self.plan, self.B
         p.x_in[:B].copy_(x)
         p.x_in[B:].copy_(x)
-        p.t_in.copy_(t_scalar.expand_as(p.t_in))
-        self.coef.copy_(coef_row)
+        p.t_in.fill_(t)
         p.run(self.model.use_cuda_graph)
-        if self.step_kind == "dpmpp_2m":
-            self._update(x)
-        else:
-            ops.sampler_step(p.out, x, self.noise, self.coef, self.guidance, self.cond_first, self.clip, self.mode,
-                             self.init, self.mask, self.work, self.rnoise)
+        return p.out
+
+    def run(self, x, t_scalar, coef_row):
+        """x fp32 [B,4,H,W] is updated in place to x_{t-1}."""
+        self.coef.copy_(coef_row)
+        self.forward(x, t_scalar)
+        self._update(x)
         return x
 
 

@@ -6,7 +6,7 @@ image's latent, CFG twin, noise stream and MoVQ decode are independent.  Rank r 
 (NCCL over NVLink on GPUs, gloo in the CPU tests); nothing else crosses ranks.  RNG is seeded per GLOBAL
 sample index so results do not depend on the world size.  The 2.1 dynamic threshold uses GLOBAL sample 0's
 percentile for the whole batch (gaussian_diffusion.py:290): rank 0 owns that sample and broadcasts the one float
-per step (kandinsky2/model/gaussian_diffusion.py: FusedStep._launch_step) -- the 2.1 p_sampler path's second,
+per step (kandinsky2/model/gaussian_diffusion.py: FusedStep._update) -- the 2.1 p_sampler path's second,
 4-byte collective; Kandinsky 2.2 has no threshold and keeps exactly one broadcast per generation.
 """
 import torch

@@ -78,12 +78,17 @@ def _check_sampler(sampler, allowed):
 
 
 def _dpm_keep(num_steps, strength):
-    """img2img with DPM-Solver++: the last int(N * strength) evaluations run (at least 1)."""
+    """img2img with DPM-Solver++ (and the 2.2 DDPM sampler, as diffusers): the last int(N * strength) evaluations run (at
+    least 1)."""
     return max(min(int(num_steps * strength), num_steps), 1)
 
 
 class _DecoderBase:
     version = None
+    # how the versions' decoder steps differ: the order of the CFG-doubled rows, the reference's per-step dynamic threshold
+    # (the +-2 clamp alone when False), and the inpainting rule (False: the known region replaces x0; True: it is re-noised
+    # to the next timestep)
+    cond_first = dynamic_threshold = inpaint_renoise = None
 
     def __init__(self, config, device, task_type="text2img", embedder=None, unet_state_dict=None, movq_state_dict=None,
                  seed=0):
@@ -128,21 +133,74 @@ class _DecoderBase:
             return self.image_encoder.encode(image.to(self.device))
         return self.image_encoder.encode(prepare_image(image, w=w, h=h).to(self.device))
 
-    def _shard(self, batch_size):
-        rank, ws = parallel.world()
-        lo, hi = parallel.shard_range(batch_size, rank, ws)
-        return rank, ws, lo, hi
-
-    def _latents(self, lo, hi, shape):
-        return parallel.sample_noise(range(lo, hi), shape, base_seed=self.base_seed, device=self.device)
-
     def _generators(self, lo, hi):
         """One device RNG stream per GLOBAL sample index (step noise independent of world size / batch position)."""
         return [torch.Generator(device=self.device).manual_seed(self.base_seed * 7919 + gi) for gi in range(lo, hi)]
 
+    def _img2img_noise(self, latent):
+        """Seeded by base_seed alone: every img2img call on one image starts from the same noisy latent."""
+        return torch.randn(latent.shape, generator=torch.Generator().manual_seed(self.base_seed)).to(self.device)
+
+    def _dpm_img2img_start(self, latent, diffusion, num_steps, strength):
+        """DPM-Solver++ img2img -> (start latent, evaluations kept): the image latent noised to the first kept evaluation."""
+        keep = _dpm_keep(num_steps, strength)
+        sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=keep)
+        return sched.start_latent(latent, self._img2img_noise(latent)), keep
+
+    @torch.no_grad()
+    def _decode(self, cond, batch_size, latent_hw, image_hw, sampler, diffusion, num_steps, guidance_scale, *, noise=None,
+                init_step=None, inpaint=None, hint=None):
+        """The decoder call of both versions.  cond: the conditioning of the GLOBAL batch, [2 * batch_size, ...] per key, in
+        the version's row order; rank 0's copy is broadcast and this rank keeps its rows.  noise: the start latents
+        [2 * batch_size, 4, H, W], or None to draw them per global sample index.  inpaint: (clean latent [1, 4, H, W], mask
+        [1, 1, H, W]) for every sample, on the device.  hint: the ControlNet depth map [1, 3, h, w] for every row.  Runs
+        `sampler` over `diffusion` (`num_steps` evaluations for the DDIM, PLMS and DPM-Solver++ samplers) and decodes this
+        rank's samples to image_hw."""
+        rank, ws = parallel.world()
+        lo, hi = parallel.shard_range(batch_size, rank, ws)
+        B = hi - lo
+        H, W = latent_hw
+        parallel.broadcast_conditioning(cond, src=0)   # the path's only collective
+        rows = list(range(lo, hi)) + list(range(batch_size + lo, batch_size + hi))
+        kw = {k: v[rows].contiguous() for k, v in cond.items()}
+        if hint is not None:  # one depth map for the whole batch (cond and uncond rows alike, as the diffusers pipeline does)
+            kw["hint"] = hint.to(self.device).float().expand(2 * B, -1, -1, -1).contiguous()
+        blend = {}
+        if inpaint is not None:
+            init, mask = inpaint
+            kw["inpaint_image"] = (init * mask).repeat(2 * B, 1, 1, 1)
+            kw["inpaint_mask"] = mask.repeat(2 * B, 1, 1, 1)
+            blend = dict(inpaint_init=init.repeat(B, 1, 1, 1), inpaint_mask=mask.repeat(B, 1, 1, 1),
+                         inpaint_renoise=self.inpaint_renoise)
+        if noise is None:
+            x = parallel.sample_noise(range(lo, hi), (4, H, W), base_seed=self.base_seed, device=self.device)
+            noise = torch.cat([x, x], 0)
+        elif noise.shape[0] == 2 * batch_size and ws > 1:
+            noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
+        shape = (2 * B, 4, H, W)
+        self.model.del_cache()
+        if sampler == "dpmpp_2m_sampler":
+            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step)
+            samples = sched.sample(self.model, shape, noise=noise, model_kwargs=kw, device=self.device,
+                                   guidance_scale=guidance_scale, cond_first=self.cond_first, **blend)
+        elif sampler in ("ddim_sampler", "plms_sampler"):  # kandinsky2_1_model.py:259-284: un-respaced schedule, eta 0
+            cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
+            samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, H, W), conditioning=kw, x_T=noise,
+                                                           init_step=init_step, guidance_scale=guidance_scale,
+                                                           cond_first=self.cond_first)
+        else:  # "p_sampler" (2.1), "ddpm_sampler" (2.2)
+            samples = diffusion.p_sample_loop(self.model, shape, device=self.device, noise=noise, model_kwargs=kw,
+                                              init_step=init_step, guidance_scale=guidance_scale, cond_first=self.cond_first,
+                                              clip_denoised=self.dynamic_threshold,
+                                              sample_generators=self._generators(lo, hi), **blend)
+        self.model.del_cache()
+        return self._finish(samples[:B], *image_hw)
+
 
 class Kandinsky2_1(_DecoderBase):
     version = "2.1"
+    cond_first = dynamic_threshold = True
+    inpaint_renoise = False
 
     def get_new_h_w(self, h, w):
         return _new_h_w_latent_21(h, w)
@@ -152,48 +210,18 @@ class Kandinsky2_1(_DecoderBase):
                      noise=None, init_img=None, img_mask=None, h=512, w=512, sampler="ddim_sampler", num_steps=50):
         """kandinsky2_1_model.py:184-292. img_prompt = cat([cond image emb, zero image emb]) [2B, 768].
         sampler="dpmpp_2m_sampler" runs DPM-Solver++(2M) over `num_steps` evaluations of diffusion's base schedule; with
-        init_step = s only the last s of them run (img2img), starting from `noise`."""
+        init_step = s only the last s of them run (img2img), starting from `noise`.  Inpainting: the known region replaces
+        x0 inside the step (p_sampler and dpmpp_2m_sampler; the reference's DDIM / PLMS paths have no such blend)."""
         _check_sampler(sampler, SAMPLERS_21)
-        new_h, new_w = self.get_new_h_w(h, w)
-        rank, ws, lo, hi = self._shard(batch_size)
-        B = hi - lo
         full_emb, pooled_emb = self.embedder.text_emb(prompt, batch_size)
         cond = {"full_emb": full_emb.to(self.device), "pooled_emb": pooled_emb.to(self.device),
                 "image_emb": img_prompt.to(self.device).float()}
-        parallel.broadcast_conditioning(cond, src=0)   # the path's only collective
-        rows = list(range(lo, hi)) + list(range(batch_size + lo, batch_size + hi))
-        kw = {k: v[rows].contiguous() for k, v in cond.items()}
-        inpaint = {}
+        inpaint = None
         if self.task_type == "inpainting":
-            init = init_img.to(self.device).float()
-            mask = img_mask.to(self.device).float()
             # the reference repeats ONE image / mask for the cond and uncond rows (:536-537); same image for every sample here
-            kw["inpaint_image"] = (init * mask)[:1].repeat(2 * B, 1, 1, 1)
-            kw["inpaint_mask"] = mask[:1].repeat(2 * B, 1, 1, 1)
-            inpaint = dict(inpaint_init=init[:1].repeat(B, 1, 1, 1), inpaint_mask=mask[:1].repeat(B, 1, 1, 1))
-        if noise is None:
-            x = self._latents(lo, hi, (4, new_h, new_w))
-            noise = torch.cat([x, x], 0)
-        elif noise.shape[0] == 2 * batch_size and ws > 1:
-            noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
-        self.model.del_cache()
-        if sampler == "p_sampler":
-            samples = diffusion.p_sample_loop(self.model, (2 * B, 4, new_h, new_w), device=self.device, noise=noise,
-                                              progress=False, model_kwargs=kw, init_step=init_step,
-                                              guidance_scale=guidance_scale, cond_first=True, clip_denoised=True,
-                                              sample_generators=self._generators(lo, hi), **inpaint)[:B]
-        elif sampler == "dpmpp_2m_sampler":  # inpainting: the known region replaces x0 inside the step, as in p_sampler
-            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step)
-            samples = sched.sample(self.model, (2 * B, 4, new_h, new_w), noise=noise, model_kwargs=kw, device=self.device,
-                                   guidance_scale=guidance_scale, cond_first=True, **inpaint)[:B]
-        else:  # kandinsky2_1_model.py:259-284: DDIM / PLMS over the un-respaced schedule, eta 0
-            cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
-            samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, new_h, new_w), conditioning=kw,
-                                                                     x_T=noise, init_step=init_step,
-                                                                     guidance_scale=guidance_scale, cond_first=True)
-            samples = samples[:B]
-        self.model.del_cache()
-        return self._finish(samples, h, w)
+            inpaint = (init_img.to(self.device).float()[:1], img_mask.to(self.device).float()[:1])
+        return self._decode(cond, batch_size, self.get_new_h_w(h, w), (h, w), sampler, diffusion, num_steps, guidance_scale,
+                            noise=noise, init_step=init_step, inpaint=inpaint)
 
     def _diffusion(self, sampler, num_steps):
         dc = dict(self.config["diffusion_config"])
@@ -236,16 +264,13 @@ class Kandinsky2_1(_DecoderBase):
         _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        g = torch.Generator().manual_seed(self.base_seed)
-        noise = torch.randn(image.shape, generator=g).to(self.device)
         if sampler == "dpmpp_2m_sampler":
-            start_step = _dpm_keep(num_steps, strength)
-            x = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=start_step).start_latent(image, noise)
+            x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength)
         else:
             start_step = int(diffusion.num_timesteps * (1 - strength))
             dc = self.config["diffusion_config"]
             x = q_sample(image, diffusion.timestep_map[start_step - 1], schedule_name=dc["noise_schedule"],
-                         num_steps=dc["steps"], noise=noise)
+                         num_steps=dc["steps"], noise=self._img2img_noise(image))
         x = x.repeat(2 * batch_size, 1, 1, 1)
         image_emb = self._image_embs(prompt, batch_size)
         return self.generate_img(prompt=prompt, img_prompt=image_emb, batch_size=batch_size,
@@ -270,53 +295,25 @@ class Kandinsky2_1(_DecoderBase):
 
 class Kandinsky2_2(_DecoderBase):
     version = "2.2"
+    cond_first = dynamic_threshold = False
+    # diffusers KandinskyV22InpaintPipeline (the reference delegates to it, kandinsky2_2_model.py:143-173): after every
+    # scheduler step the known region (mask = 1) is the clean latent noised to the next timestep with the run's initial noise,
+    # and the result is blended with the clean latent at the end -- the step kernels' inpaint_noise mode
+    inpaint_renoise = True
 
     def get_new_h_w(self, h, w):  # kandinsky2_2_model.py:46-53 (pixels)
         return math.ceil(h / 64) * 64, math.ceil(w / 64) * 64
 
-    @torch.no_grad()
-    def _decode_loop(self, image_embeds, negative_embeds, batch_size, steps, guidance, h, w, latents=None,
-                     inpaint_latent=None, inpaint_mask=None, init_step=None, hint=None, sampler="ddpm_sampler"):
+    def _decode_loop(self, image_embeds, negative_embeds, batch_size, steps, guidance, h, w, latents=None, inpaint=None,
+                     init_step=None, hint=None, sampler="ddpm_sampler"):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
         106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
         sampler="dpmpp_2m_sampler": DPM-Solver++(2M) over `steps` evaluations of the same base schedule instead (init_step =
         the number of evaluations kept for img2img); inpainting re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
-        H, W = h // 8, w // 8
-        rank, ws, lo, hi = self._shard(batch_size)
-        B = hi - lo
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}
-        parallel.broadcast_conditioning(cond, src=0)
-        rows = list(range(lo, hi)) + list(range(batch_size + lo, batch_size + hi))
-        kw = {"image_emb": cond["image_emb"][rows].contiguous()}
-        if hint is not None:  # one depth map for the whole batch (cond and uncond rows alike, as the diffusers pipeline does)
-            kw["hint"] = hint.to(self.device).float().expand(2 * B, -1, -1, -1).contiguous()
-        if latents is None:
-            x = self._latents(lo, hi, (4, H, W))
-            latents = torch.cat([x, x], 0)
-        elif latents.shape[0] == 2 * batch_size and ws > 1:
-            latents = latents[rows].contiguous()   # caller-supplied start latents cover the GLOBAL batch
-        extra = {}
-        if inpaint_latent is not None:
-            kw["inpaint_image"] = (inpaint_latent * inpaint_mask).repeat(2 * B, 1, 1, 1).to(self.device)
-            kw["inpaint_mask"] = inpaint_mask.repeat(2 * B, 1, 1, 1).to(self.device)
-            # diffusers KandinskyV22InpaintPipeline (the reference delegates to it, kandinsky2_2_model.py:143-173): after every
-            # scheduler step the known region (mask = 1) is the clean latent noised to the next timestep with the run's initial
-            # noise, and the result is blended with the clean latent at the end -- k2_sampler_step's inpaint_noise mode
-            extra = dict(inpaint_init=inpaint_latent.repeat(B, 1, 1, 1).to(self.device),
-                         inpaint_mask=inpaint_mask.repeat(B, 1, 1, 1).to(self.device), inpaint_renoise=True)
-        diffusion = create_ddpm_v22(steps)
-        self.model.del_cache()
-        if sampler == "dpmpp_2m_sampler":
-            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, steps, keep=init_step)
-            out = sched.sample(self.model, (2 * B, 4, H, W), noise=latents, model_kwargs=kw, device=self.device,
-                               guidance_scale=guidance, cond_first=False, **extra)[:B]
-        else:
-            out = diffusion.p_sample_loop(self.model, (2 * B, 4, H, W), device=self.device, noise=latents,
-                                          model_kwargs=kw, guidance_scale=guidance, cond_first=False, clip_denoised=False,
-                                          init_step=init_step, sample_generators=self._generators(lo, hi), **extra)[:B]
-        self.model.del_cache()
-        return self._finish(out, h, w)
+        return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, create_ddpm_v22(steps), steps, guidance,
+                            noise=latents, init_step=init_step, inpaint=inpaint, hint=hint)
 
     def _embeds(self, prompt, batch_size, negative_decoder_prompt):
         pos = self.embedder.image_emb(prompt, batch_size)
@@ -349,15 +346,13 @@ class Kandinsky2_2(_DecoderBase):
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
-        # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first of them
-        start = max(min(int(decoder_steps * strength), decoder_steps), 1)
-        g = torch.Generator().manual_seed(self.base_seed)
-        noise = torch.randn(lat.shape, generator=g).to(self.device)
         if sampler == "dpmpp_2m_sampler":
-            x = DPMSolverSchedule(diffusion.base_alphas_cumprod, decoder_steps, keep=start).start_latent(lat, noise)
+            x, start = self._dpm_img2img_start(lat, diffusion, decoder_steps, strength)
         else:
+            # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first
+            start = _dpm_keep(decoder_steps, strength)
             ac = float(diffusion.alphas_cumprod[start - 1])
-            x = ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * noise
+            x = ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * self._img2img_noise(lat)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, sampler=sampler)
 
@@ -389,5 +384,5 @@ class Kandinsky2_2(_DecoderBase):
         lat = self._encode_image(pil_img, h, w)
         m = torch.as_tensor(img_mask).float()[None, None]
         m = torch.nn.functional.interpolate(m, (h // 8, w // 8), mode="nearest").to(self.device)
-        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
-                                 inpaint_latent=lat, inpaint_mask=m, sampler=sampler)
+        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, inpaint=(lat, m),
+                                 sampler=sampler)
