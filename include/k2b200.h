@@ -15,6 +15,8 @@
  *   - every launch is enqueued on the caller's stream (pass torch.cuda.current_stream().cuda_stream);
  *   - activations are NHWC fp16 ("rows" = pixels, row stride `ld*` in ELEMENTS so that a tensor may
  *     be a channel slice of a wider buffer); weights are pre-packed by the host (layout per function);
+ *   - kernels that move fp16 rows as 16-byte vectors need 16-byte aligned pointers, row strides that are multiples of 8
+ *     elements and >= the row width; such calls are refused (< 0) before anything is launched;
  *   - there is no CPU fallback: without an sm_90 device every call fails.
  */
 #ifndef K2B200_H_

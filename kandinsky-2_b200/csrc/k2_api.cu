@@ -308,6 +308,7 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
     K2_REQUIRE(cfg[1] != 2, "conv_gemm_cfg: no CTA-pair conv kernel on sm_90");
   }
   K2_REQUIRE(nsrc >= 1 && nsrc <= 3, "conv_gemm: 1..3 sources");
+  K2_REQUIRE((reinterpret_cast<uintptr_t>(gn_partial) & 7) == 0, "conv_gemm: gn_partial must be 8-byte aligned");
   K2_REQUIRE(NB > 0 && H > 0 && W > 0 && Cout > 0, "conv_gemm: bad geometry");
   K2_REQUIRE(w_rows >= Cout, "conv_gemm: w_rows < Cout");
   K2_REQUIRE(Ktot % 64 == 0, "conv_gemm: Ktot must be a multiple of 64");

@@ -23,6 +23,10 @@ int fail(const std::string& msg);  // records msg, returns -1
     if (!(cond)) return ::k2::fail(std::string("k2b200: ") + (msg)); \
   } while (0)
 
+// True when p may be accessed with 16-byte (uint4 / float4) vector loads and stores; null counts as aligned (optional
+// arguments are checked for presence separately).
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 int num_sms();
 bool pdl_enabled();
 

@@ -805,6 +805,8 @@ int k2_step_end(int* counter, k2_stream_t stream) {
 
 int k2_upsample2x_nhwc(const void* x, int ldx, void* y, int ldy, int NB, int H, int W, int C, k2_stream_t stream) {
   K2_REQUIRE(x && y && C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "upsample2x: channels / strides must be multiples of 8");
+  K2_REQUIRE(ldx >= C && ldy >= C, "upsample2x: row strides must be >= C");
+  K2_REQUIRE(aligned16(x) && aligned16(y), "upsample2x: x and y must be 16-byte aligned");
   const long long total = static_cast<long long>(NB) * H * W * (C / 8);
   upsample2x_kernel<<<blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, NB, H, W, C / 8);
@@ -817,6 +819,8 @@ int k2_subsample2_nhwc(const void* x, int ldx, void* y, int ldy, int NB, int H, 
                        k2_stream_t stream) {
   K2_REQUIRE(x && y && C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && H % 2 == 0 && W % 2 == 0 && (oy | 1) == 1 && (ox | 1) == 1,
              "subsample2: bad arguments");
+  K2_REQUIRE(ldx >= C && ldy >= C, "subsample2: row strides must be >= C");
+  K2_REQUIRE(aligned16(x) && aligned16(y), "subsample2: x and y must be 16-byte aligned");
   const long long total = static_cast<long long>(NB) * (H / 2) * (W / 2) * (C / 8);
   subsample2_kernel<<<blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, NB, H, W, C / 8, oy, ox);
@@ -828,6 +832,8 @@ int k2_subsample2_nhwc(const void* x, int ldx, void* y, int ldy, int NB, int H, 
 int k2_softmax_rows(const void* x, int ldx, void* y, int ldy, long long rows, int n, float scale, k2_stream_t stream) {
   K2_REQUIRE(x && y && rows > 0 && n > 0 && ldx % 8 == 0 && ldy % 8 == 0, "softmax_rows: bad arguments");
   K2_REQUIRE(rows < (1LL << 31), "softmax_rows: too many rows");
+  K2_REQUIRE(ldx >= n && ldy >= n, "softmax_rows: row strides must be >= n");
+  K2_REQUIRE(aligned16(x) && aligned16(y), "softmax_rows: x and y must be 16-byte aligned");
   softmax_rows_kernel<<<static_cast<unsigned int>(rows), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, n, scale * 1.4426950408889634f);
   K2_CHECK_CUDA(cudaGetLastError());
@@ -870,6 +876,7 @@ int k2_vq_argmin(const float* z, const float* codebook, long long* idx, int n, i
                  k2_stream_t stream) {
   K2_REQUIRE(z && codebook && idx && n > 0 && n_embed > 0, "vq_argmin: bad arguments");
   K2_REQUIRE(dim == 4, "vq_argmin: only embed_dim 4 (MoVQ) is implemented");
+  K2_REQUIRE(aligned16(z) && aligned16(codebook), "vq_argmin: z and codebook must be 16-byte aligned");
   vq_argmin_kernel<<<blocks_for(n, 256), 256, 2048 * sizeof(float4), static_cast<cudaStream_t>(stream)>>>(
       z, codebook, idx, n, n_embed);
   K2_CHECK_CUDA(cudaGetLastError());

@@ -189,6 +189,8 @@ int k2_sn_apply(const void* x, int C, int ldx, int NB, int H, int W, int groups,
   K2_REQUIRE(x && y && stats && gamma && beta && zq && sn_w, "sn_apply: null pointer");
   K2_REQUIRE(C % 8 == 0 && C % groups == 0 && ldx % 8 == 0 && ldy % 8 == 0, "sn_apply: bad channel counts / strides");
   K2_REQUIRE(NB > 0 && H > 0 && W > 0 && zh > 0 && zw > 0 && NB <= 65535, "sn_apply: bad geometry");
+  K2_REQUIRE(ldx >= C && ldy >= C, "sn_apply: row strides must be >= C");
+  K2_REQUIRE(aligned16(x) && aligned16(y) && aligned16(zq), "sn_apply: x, y and zq must be 16-byte aligned");
   SnParams p;
   p.x = reinterpret_cast<const __half*>(x);
   p.C = C; p.ldx = ldx; p.NB = NB; p.H = H; p.W = W; p.groups = groups;

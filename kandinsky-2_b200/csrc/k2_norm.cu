@@ -555,6 +555,10 @@ int k2_gn_stats(const void* src0, int C0, int ld0, const void* src1, int C1, int
   K2_REQUIRE(C % groups == 0, "gn_stats: C % groups != 0");
   K2_REQUIRE(src1 || C1 == 0, "gn_stats: src1 null with C1 > 0");
   K2_REQUIRE(NB <= 1024, "gn_stats: at most 1024 images per launch");
+  K2_REQUIRE(ld0 % 8 == 0 && ld0 >= C0 && (C1 == 0 || (ld1 % 8 == 0 && ld1 >= C1)),
+             "gn_stats: row strides must be multiples of 8 elements and >= the channels");
+  K2_REQUIRE(aligned16(src0) && aligned16(src1), "gn_stats: sources must be 16-byte aligned");
+  K2_REQUIRE(stats && scratch, "gn_stats: null pointer");
   const int ctiles = (C / 8 + VX - 1) / VX;
   const int chunk = pick_chunk(HW, ctiles, NB);
   const int chunks = (HW + chunk - 1) / chunk;
@@ -572,6 +576,8 @@ int k2_gn_finalize(const float* part0, int C0, int rg0, const float* part1, int 
                    float eps, float* stats, k2_stream_t stream) {
   K2_REQUIRE(part0 && stats && C0 > 0 && (part1 || C1 == 0) && (C0 + C1) % groups == 0 && rg0 > 0 && (C1 == 0 || rg1 > 0),
              "gn_finalize: bad arguments");
+  K2_REQUIRE(((reinterpret_cast<uintptr_t>(part0) | reinterpret_cast<uintptr_t>(part1)) & 7) == 0,
+             "gn_finalize: partial buffers must be 8-byte aligned");
   dim3 grid(groups, NB);
   K2_CHECK_CUDA(launch_k(gn_finalize_kernel, grid, dim3(FIN_T), 0, static_cast<cudaStream_t>(stream),
                          reinterpret_cast<const float2*>(part0), C0, rg0, reinterpret_cast<const float2*>(part1), C1, rg1, HW,
@@ -590,6 +596,12 @@ int k2_gn_apply(const void* src0, int C0, int ld0, const void* src1, int C1, int
   K2_REQUIRE(resample >= 0 && resample <= 2, "gn_apply: resample in {0,1,2}");
   K2_REQUIRE(resample != 1 || (H % 2 == 0 && W % 2 == 0), "gn_apply: avg-pool needs even H, W");
   K2_REQUIRE(!zq || sn_w, "gn_apply: zq without sn_w");
+  K2_REQUIRE(src1 || C1 == 0, "gn_apply: src1 null with C1 > 0");
+  K2_REQUIRE(ld0 % 8 == 0 && ld0 >= C0 && (C1 == 0 || (ld1 % 8 == 0 && ld1 >= C1)) && ldy % 8 == 0 && ldy >= C &&
+                 (!xres || (ldx % 8 == 0 && ldx >= C)),
+             "gn_apply: row strides must be multiples of 8 elements and >= the channels");
+  K2_REQUIRE(aligned16(src0) && aligned16(src1) && aligned16(y) && aligned16(xres) && aligned16(zq),
+             "gn_apply: x, y, xres and zq must be 16-byte aligned");
   ApplyParams p;
   p.s0 = reinterpret_cast<const __half*>(src0);
   p.s1 = reinterpret_cast<const __half*>(src1);
@@ -637,6 +649,13 @@ int k2_gn_apply_fold(const void* src0, int C0, int ld0, const void* src1, int C1
   K2_REQUIRE(resample >= 0 && resample <= 2, "gn_apply_fold: resample in {0,1,2}");
   K2_REQUIRE(resample != 1 || (H % 2 == 0 && W % 2 == 0), "gn_apply_fold: avg-pool needs even H, W");
   K2_REQUIRE(part0 && rg0 > 0 && (C1 == 0 || (src1 && part1 && rg1 > 0)), "gn_apply_fold: partial buffers");
+  K2_REQUIRE(ld0 % 8 == 0 && ld0 >= C0 && (C1 == 0 || (ld1 % 8 == 0 && ld1 >= C1)) && ldy % 8 == 0 && ldy >= C &&
+                 (!xres || (ldx % 8 == 0 && ldx >= C)),
+             "gn_apply_fold: row strides must be multiples of 8 elements and >= the channels");
+  K2_REQUIRE(aligned16(src0) && aligned16(src1) && aligned16(y) && aligned16(xres),
+             "gn_apply_fold: x, y and xres must be 16-byte aligned");
+  K2_REQUIRE(((reinterpret_cast<uintptr_t>(part0) | reinterpret_cast<uintptr_t>(part1)) & 7) == 0,
+             "gn_apply_fold: partial buffers must be 8-byte aligned");
   ApplyParams p;
   p.s0 = reinterpret_cast<const __half*>(src0);
   p.s1 = reinterpret_cast<const __half*>(src1);
