@@ -249,15 +249,21 @@ int k2_plms_step(const float* model_out, int C2, const float* x, float* out, con
  *   x0   = x0 (1 - mask) + init mask                         if inpaint_mask != NULL and inpaint_noise == NULL (2.1);
  *   x'   = coef[2] x + coef[3] x0 + coef[4] hist   -- hist is NOT read when coef[4] == 0 (first-order steps), so its
  *          contents (even NaN) cannot reach the result;
+ *   x'  += coef[7] noise   -- k2_dpm_solver_sde_step only; noise is NOT read when coef[7] == 0 (the SDE's last step);
  *   hist = x0   (hist fp32 [B, 4, H, W]: the previous step's x0 in, this step's out);
  *   x'   = mask (coef[5] init + coef[6] inpaint_noise) + (1 - mask) x'   if inpaint_noise != NULL (2.2: the known region is
  *          the clean latent noised to the next timestep with the run's initial noise; (1, 0) at the last step).
- * coef is device fp32[8] = {1/alpha_k, sigma_k/alpha_k, c_x, c_D, c_P, alpha_{k+1}, sigma_{k+1}, 0}, one row of the host's
+ * coef is device fp32[8] = {1/alpha_k, sigma_k/alpha_k, c_x, c_D, c_P, alpha_{k+1}, sigma_{k+1}, c_N}, one row of the host's
  * schedule (kandinsky2/model/gaussian_diffusion.py: DPMSolverSchedule), so k2_step_begin can pick it by the step counter.
- * Arguments are checked before any CUDA call. */
+ * k2_dpm_solver_step (the ODE solver) ignores c_N.  Arguments are checked before any CUDA call. */
 int k2_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, int B, int H, int W,
                        float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
                        const float* inpaint_noise, k2_stream_t stream);
+/* DPM-Solver++(2M) SDE step (Lu et al. 2022, the data-prediction SDE solver in its 2M form): the update above with this
+ * step's Gaussian noise z, noise fp32 [B, 4, H, W] (not NULL), added as coef[7] z.  Same kernel, same checks. */
+int k2_dpm_solver_sde_step(const float* model_out, int C2, float* x, float* hist, const float* noise, const float* coef,
+                           int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
+                           const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * MoVQ helpers: nearest-codebook search (quntize.py:89-98; fp32, ties -> lowest index, int64 out),

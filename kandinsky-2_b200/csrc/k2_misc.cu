@@ -411,11 +411,12 @@ __global__ void __launch_bounds__(256) plms_step_kernel(const PlmsParams p) {
   p.out[i] = xn;
 }
 
-// DPM-Solver++(2M) update (Lu et al. 2022, Algorithm 2), linear in (x, D_k, D_{k-1}) with D the x0 prediction:
+// DPM-Solver++(2M) update (Lu et al. 2022, Algorithm 2), linear in (x, D_k, D_{k-1}, z) with D the x0 prediction:
 //   eps = CFG(model_out)  (eps channels only);  x0 = coef[0] x - coef[1] eps  (no clamp, no threshold)
 //   x'  = coef[2] x + coef[3] x0 + coef[4] hist      (hist = D_{k-1}; not read when coef[4] == 0)
+//   x' += coef[7] noise                              (the SDE entry only: this step's noise z; not read when coef[7] == 0)
 //   hist = x0
-// coef = {1/a_k, s_k/a_k, c_x, c_D, c_P, a_{k+1}, s_{k+1}, 0}; the host builds the rows (DPMSolverSchedule).
+// coef = {1/a_k, s_k/a_k, c_x, c_D, c_P, a_{k+1}, s_{k+1}, c_N}; the host builds the rows (DPMSolverSchedule).
 struct DpmParams {
   const float* model_out;  // [2B, C2, H, W], eps = channels [0, 4)
   float* x;                // [B, 4, H, W], in place
@@ -427,8 +428,11 @@ struct DpmParams {
   const float* init;       // [B,4,H,W] or null
   const float* mask;       // [B,1,H,W] or null
   const float* rnoise;     // [B,4,H,W] or null (2.2 inpainting: the known region is re-noised to the next timestep)
+  const float* noise;      // [B,4,H,W] (the SDE entry) or null (the ODE entry): this step's Gaussian noise z
 };
 
+// kNoise: the SDE entry's instantiation; the ODE one has no noise term at all.
+template <bool kNoise>
 __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
@@ -443,6 +447,10 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p)
   float xn = p.coef[2] * xv + p.coef[3] * x0;
   const float cp = p.coef[4];
   if (cp != 0.f) xn += cp * p.hist[i];  // a first-order step never reads the history: it may hold anything, NaN included
+  if (kNoise) {
+    const float cn = p.coef[7];
+    if (cn != 0.f) xn += cn * p.noise[i];  // likewise the noise on a noise-free row (the SDE's last step)
+  }
   p.hist[i] = x0;
   if (p.mask && p.rnoise) xn = m * (p.coef[5] * p.init[i] + p.coef[6] * p.rnoise[i]) + (1.f - m) * xn;
   p.x[i] = xn;
@@ -854,22 +862,39 @@ int k2_plms_step(const float* model_out, int C2, const float* x, float* out, con
   return 0;
 }
 
-int k2_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, int B, int H, int W,
-                       float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
-                       const float* inpaint_noise, k2_stream_t stream) {
-  K2_REQUIRE(model_out && x && hist && coef, "dpm_solver_step: null pointer");
-  K2_REQUIRE(B > 0 && H > 0 && W > 0 && C2 >= 4, "dpm_solver_step: B, H, W must be >= 1 and C2 >= 4");
-  K2_REQUIRE((inpaint_init == nullptr) == (inpaint_mask == nullptr), "dpm_solver_step: init and mask go together");
-  K2_REQUIRE(inpaint_noise == nullptr || inpaint_init, "dpm_solver_step: inpaint_noise without init / mask");
+// The ODE and SDE entries share the kernel: `noise` is null for the ODE one (`name` prefixes the error messages).
+static int dpm_step(const char* name, const float* model_out, int C2, float* x, float* hist, const float* noise,
+                    const float* coef, int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
+                    const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream) {
+  const std::string who(name);
+  K2_REQUIRE(model_out && x && hist && coef, who + ": null pointer");
+  K2_REQUIRE(B > 0 && H > 0 && W > 0 && C2 >= 4, who + ": B, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE((inpaint_init == nullptr) == (inpaint_mask == nullptr), who + ": init and mask go together");
+  K2_REQUIRE(inpaint_noise == nullptr || inpaint_init, who + ": inpaint_noise without init / mask");
   DpmParams p;
   p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
   p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
-  p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
+  p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise; p.noise = noise;
   const long long total = static_cast<long long>(B) * 4 * H * W;
-  K2_CHECK_CUDA(launch_k(dpm_solver_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream),
-                         p));
+  K2_CHECK_CUDA(launch_k(noise ? dpm_solver_step_kernel<true> : dpm_solver_step_kernel<false>, dim3(blocks_for(total, 256)),
+                         dim3(256), 0, static_cast<cudaStream_t>(stream), p));
   count_launch();
   return 0;
+}
+
+int k2_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, int B, int H, int W,
+                       float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
+                       const float* inpaint_noise, k2_stream_t stream) {
+  return dpm_step("dpm_solver_step", model_out, C2, x, hist, nullptr, coef, B, H, W, guidance, cond_first, inpaint_init,
+                  inpaint_mask, inpaint_noise, stream);
+}
+
+int k2_dpm_solver_sde_step(const float* model_out, int C2, float* x, float* hist, const float* noise, const float* coef,
+                           int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
+                           const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream) {
+  K2_REQUIRE(noise, "dpm_solver_sde_step: null noise");
+  return dpm_step("dpm_solver_sde_step", model_out, C2, x, hist, noise, coef, B, H, W, guidance, cond_first, inpaint_init,
+                  inpaint_mask, inpaint_noise, stream);
 }
 
 int k2_vq_argmin(const float* z, const float* codebook, long long* idx, int n, int n_embed, int dim,

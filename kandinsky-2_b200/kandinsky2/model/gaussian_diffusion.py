@@ -50,7 +50,8 @@ def space_timesteps(num_timesteps, section_counts):
 class _Schedule:
     """What _sampling_loop needs of a schedule: coef_table() (fp32 [n, 8] step-kernel rows) and model_timesteps() (what the UNet
     sees, [n]) in the same index order; the loop runs the rows n-1 .. 0.  Each schedule also states whether its step draws
-    noise and which step kernel applies its rows ("ddpm": k2_sampler_step, "dpmpp_2m": k2_dpm_solver_step)."""
+    noise and which step kernel applies its rows ("ddpm": k2_sampler_step, "dpmpp_2m": k2_dpm_solver_step, "dpmpp_2m_sde":
+    k2_dpm_solver_sde_step)."""
 
     draws_noise = True
     step_kind = "ddpm"
@@ -145,7 +146,8 @@ class SpacedDiffusion(_Schedule):
 
 class DPMSolverSchedule(_Schedule):
     """DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models",
-    Algorithm 2) over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step, no noise.
+    Algorithm 2) over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step, no noise
+    (see sde below).
 
     N evaluations at tau_k = linspace(0, T-1, N+1).round()[::-1][k], k = 0..N-1; the UNet sees tau_k as a raw float timestep.
     alpha_k = sqrt(ac[tau_k]), sigma_k = sqrt(1 - ac[tau_k]), lambda_k = log alpha_k - log sigma_k; the target after the last
@@ -158,26 +160,47 @@ class DPMSolverSchedule(_Schedule):
     (start_latent); the history is empty at k0, so that step is first order.
 
     Rows are stored in reverse step order (table index j = N-1-k) so that _sampling_loop, which walks the indices from the
-    top down like the DDPM schedules', runs k = k0 .. N-1."""
+    top down like the DDPM schedules', runs k = k0 .. N-1.
 
-    draws_noise = False
-    step_kind = "dpmpp_2m"
+    spacing="karras" (Karras et al. 2022, eq. 5, rho = 7) places the N evaluations in the VE sigma s^(t) = sqrt((1 - ac_t) /
+    ac_t) of the base table instead: s^_i = (s^_max^(1/rho) + i/(N-1) (s^_min^(1/rho) - s^_max^(1/rho)))^rho with s^_max =
+    s^(T-1), s^_min = s^(0) (s^_max alone when N = 1), alpha_i = 1 / sqrt(1 + s^_i^2), sigma_i = s^_i alpha_i.  The UNet sees
+    the fractional timestep whose log s^ interpolates the table's log s^(t) linearly (k-diffusion's sigma_to_t, unrounded).
 
-    def __init__(self, base_alphas_cumprod, num_steps, keep=None):
+    sde=True: the data-prediction SDE solver of DPM-Solver++ in its 2M midpoint form (diffusers' "sde-dpmsolver++", k-diffusion's
+    sample_dpmpp_2m_sde with eta 1), one Gaussian draw z per step:
+        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1} + c_N z,   c_x = sigma_{k+1} / sigma_k e^{-h_k},
+        c = alpha_{k+1} (1 - e^{-2 h_k}) in place of c above (same first- / second-order split),  c_N = sigma_{k+1} sqrt(1 - e^{-2h_k});
+    the last step still lands on D_{N-1}, with no noise.  c_N is row column 7, which the ODE rows leave 0."""
+
+    SPACINGS = ("linspace", "karras")
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace", sde=False):
         ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
         n = int(num_steps)
         if n < 1:
             raise ValueError("DPM-Solver++: num_steps must be >= 1")
-        tau = np.linspace(0, len(ac) - 1, n + 1).round()[::-1][:n].astype(np.int64)
-        if np.any(np.diff(tau) >= 0):
-            raise ValueError(f"DPM-Solver++: {n} steps do not give distinct timesteps over {len(ac)} training steps")
+        if spacing not in self.SPACINGS:
+            raise ValueError(f"DPM-Solver++: spacing must be one of {self.SPACINGS}, got {spacing!r}")
         keep = n if keep is None else int(keep)
         if not 1 <= keep <= n:
             raise ValueError(f"DPM-Solver++: keep must be in [1, {n}], got {keep}")
+        if spacing == "linspace":
+            tau = np.linspace(0, len(ac) - 1, n + 1).round()[::-1][:n].astype(np.int64)
+            if np.any(np.diff(tau) >= 0):
+                raise ValueError(f"DPM-Solver++: {n} steps do not give distinct timesteps over {len(ac)} training steps")
+            alphas, sigmas = np.sqrt(ac[tau]), np.sqrt(1.0 - ac[tau])
+        else:
+            tau, s_hat = karras_timesteps(ac, n)
+            alphas = 1.0 / np.sqrt(1.0 + s_hat ** 2)
+            sigmas = s_hat * alphas
         self.num_steps, self.k0 = n, n - keep
+        self.spacing, self.sde = spacing, bool(sde)
+        self.draws_noise = self.sde
+        self.step_kind = "dpmpp_2m_sde" if self.sde else "dpmpp_2m"
         self.timesteps = tau
-        self.alphas = np.append(np.sqrt(ac[tau]), 1.0)    # alpha_0 .. alpha_N
-        self.sigmas = np.append(np.sqrt(1.0 - ac[tau]), 0.0)
+        self.alphas = np.append(alphas, 1.0)    # alpha_0 .. alpha_N
+        self.sigmas = np.append(sigmas, 0.0)
         self.num_timesteps = keep
         self._dev_tables = {}
 
@@ -199,8 +222,13 @@ class DPMSolverSchedule(_Schedule):
                 rows[k, 3] = 1.0
                 continue
             h = lam[k + 1] - lam[k]
-            c = -a[k + 1] * np.expm1(-h)
-            rows[k, 2] = s[k + 1] / s[k]
+            if self.sde:
+                rows[k, 2] = s[k + 1] / s[k] * np.exp(-h)
+                c = -a[k + 1] * np.expm1(-2.0 * h)
+                rows[k, 7] = s[k + 1] * np.sqrt(-np.expm1(-2.0 * h))
+            else:
+                c = -a[k + 1] * np.expm1(-h)
+                rows[k, 2] = s[k + 1] / s[k]
             if k == k0:
                 rows[k, 3] = c
             else:
@@ -219,13 +247,33 @@ class DPMSolverSchedule(_Schedule):
 
     @torch.no_grad()
     def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
-               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None):
+               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None, step_noise=None,
+               sample_generators=None):
         """shape = (2*B, 4, h, w) (CFG doubled), noise = the start latent [2B or B, ...]; returns [2*B, 4, h, w] whose two halves
         both hold the B samples, like p_sample_loop.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces x0),
-        True = Kandinsky 2.2 (the known region is re-noised to the next timestep with the start latent as the noise)."""
+        True = Kandinsky 2.2 (the known region is re-noised to the next timestep with the start latent as the noise).
+        The SDE's per-step noise is drawn like p_sample_loop's: step_noise fp32 [keep, B, 4, h, w] injects it, sample_generators
+        (one per sample) draw it per image; both are ignored by the ODE solver."""
         return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
                               guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
-                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback)
+                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback,
+                              step_noise=step_noise, sample_generators=sample_generators)
+
+
+def karras_timesteps(base_alphas_cumprod, n, rho=7.0):
+    """Karras et al. 2022, eq. 5 over a base table: -> (fractional model timesteps [n], VE sigmas s^ [n]), both decreasing,
+    from s^_max = s^(T-1) at t = T-1 to s^_min = s^(0) at t = 0 (endpoints exact)."""
+    ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
+    s_table = np.sqrt((1.0 - ac) / ac)                     # increasing in t
+    log_table = np.log(s_table)
+    s_max, s_min = s_table[-1], s_table[0]
+    ramp = np.arange(n, dtype=np.float64) / max(n - 1, 1)
+    s_hat = (s_max ** (1.0 / rho) + ramp * (s_min ** (1.0 / rho) - s_max ** (1.0 / rho))) ** rho
+    s_hat[0] = s_max
+    if n > 1:
+        s_hat[-1] = s_min
+    t = np.interp(np.log(s_hat), log_table, np.arange(len(ac), dtype=np.float64))
+    return t, s_hat
 
 
 def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,
@@ -281,7 +329,7 @@ def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=
 
 
 class DDIMSampler(_Schedule):
-    """DDIM (eta = 0) over the un-respaced schedule, as the reference's default `sampler="ddim_sampler"` path uses it
+    """DDIM over the un-respaced schedule, eta = 0 as the reference's default `sampler="ddim_sampler"` path uses it
     (kandinsky2/model/samplers.py:68-331; called from kandinsky2_1_model.py:259-275).
 
     make_ddim_timesteps('uniform') (:34-55): t = range(0, 1000, 1000 // S) + 1;  alphas = acp[t], alphas_prev = [acp[0]] + acp[t[:-1]]
@@ -291,7 +339,12 @@ class DDIMSampler(_Schedule):
     kernel with coefficients  c2 = sqrt(a_prev) - sqrt(1-a_prev) sqrt(a_t) / sqrt(1-a_t),  c3 = sqrt(1-a_prev) / sqrt(1-a_t).
     Pinned: the schedule helpers against tests/golden/schedule_kat.pt, the whole loop against the final latents of the
     reference's own DDIMSampler / PLMSSampler classes (tests/golden/ddim_tiny.pt, plms_tiny.pt; their hard-coded "cuda"
-    device, :78-79,101,226, is remapped to the CPU by the generating script, oracle/make_golden.py)."""
+    device, :78-79,101,226, is remapped to the CPU by the generating script, oracle/make_golden.py).
+
+    eta > 0 (make_ddim_sampling_parameters, :21-31): sigma = eta sqrt((1-a_prev)/(1-a_t) (1 - a_t/a_prev)) and
+    x' = sqrt(a_prev) x0 + sqrt(1-a_prev-sigma^2) e + sigma z with fresh Gaussian noise z every step -- still linear in (x0, x),
+    so the same kernel applies it with sqrt(1-a_prev-sigma^2) in place of sqrt(1-a_prev) in c2, c3 and the noise term as its
+    learned-range variance with both log-variance bounds = log sigma^2 (pinned against tests/golden/ddim_eta_tiny.pt)."""
 
     draws_noise = False
 
@@ -301,8 +354,8 @@ class DDIMSampler(_Schedule):
         self.ddpm_num_timesteps = old_diffusion.original_num_steps
 
     def make_schedule(self, ddim_num_steps, ddim_eta=0.0, init_step=None):
-        if ddim_eta != 0.0:
-            raise NotImplementedError("DDIM with eta > 0")
+        if not ddim_eta >= 0.0:
+            raise ValueError(f"DDIM: eta must be >= 0, got {ddim_eta}")
         c = self.ddpm_num_timesteps // ddim_num_steps
         t = np.asarray(list(range(0, self.ddpm_num_timesteps, c))) + 1
         if init_step is not None:
@@ -311,30 +364,40 @@ class DDIMSampler(_Schedule):
         self.ddim_timesteps = t
         self.ddim_alphas = acp[t]
         self.ddim_alphas_prev = np.asarray([acp[0]] + acp[t[:-1]].tolist())
+        a_t, a_p = self.ddim_alphas, self.ddim_alphas_prev
+        self.ddim_sigmas = ddim_eta * np.sqrt((1 - a_p) / (1 - a_t) * (1 - a_t / a_p))
+        if np.any(self.ddim_sigmas ** 2 > 1.0 - a_p):
+            raise ValueError(f"DDIM: eta = {ddim_eta} makes sigma^2 exceed 1 - alpha_prev (the direction term's square root)")
+        self.draws_noise = bool(ddim_eta > 0.0)
         self.num_timesteps = len(t)
         self._dev_tables = {}  # the device tables of the previous schedule are stale
 
     def coef_table(self):
-        a_t, a_p = self.ddim_alphas, self.ddim_alphas_prev
+        a_t, a_p, sg = self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas
         s1 = np.sqrt(1.0 - a_t)
+        d = np.sqrt(1.0 - a_p - sg ** 2)   # sqrt(1 - a_prev) exactly when eta = 0
         tab = np.zeros((self.num_timesteps, 8), dtype=np.float64)
         tab[:, 0] = 1.0 / np.sqrt(a_t)
         tab[:, 1] = s1 / np.sqrt(a_t)
-        tab[:, 2] = np.sqrt(a_p) - np.sqrt(1.0 - a_p) * np.sqrt(a_t) / s1
-        tab[:, 3] = np.sqrt(1.0 - a_p) / s1
-        return tab.astype(np.float32)  # columns 4-6 zero: log-variance terms unused, noise switched off
+        tab[:, 2] = np.sqrt(a_p) - d * np.sqrt(a_t) / s1
+        tab[:, 3] = d / s1
+        noisy = sg > 0.0                   # eta = 0: columns 4-6 stay zero, the noise is switched off
+        tab[noisy, 4] = tab[noisy, 5] = np.log(sg[noisy] ** 2)
+        tab[noisy, 6] = 1.0
+        return tab.astype(np.float32)
 
     def model_timesteps(self):
         return self.ddim_timesteps
 
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, eta=0.0, x_T=None, init_step=None, *, guidance_scale=1.0,
-               cond_first=True, callback=None, **unused):
-        """-> (samples [batch_size, C, H, W], {}) like the reference (batch_size is the CFG-doubled batch)."""
+               cond_first=True, callback=None, step_noise=None, **unused):
+        """-> (samples [batch_size, C, H, W], {}) like the reference (batch_size is the CFG-doubled batch).
+        step_noise: optional fp32 [num_steps, batch_size // 2, C, H, W] injected as the eta > 0 noise (parity tests)."""
         self.make_schedule(S, ddim_eta=eta, init_step=init_step)
         C, H, W = shape
         out = _sampling_loop(self, self.model, (batch_size, C, H, W), noise=x_T, model_kwargs=conditioning,
-                             guidance_scale=guidance_scale, cond_first=cond_first, callback=callback)
+                             guidance_scale=guidance_scale, cond_first=cond_first, callback=callback, step_noise=step_noise)
         return out, {}
 
 
@@ -344,6 +407,11 @@ class PLMSSampler(DDIMSampler):
     (Adams-Bashforth 2/3/4) and apply the DDIM (eta 0) update with the combined epsilon -- k2_plms_step."""
 
     _AB = {1: (1.5, -0.5, 0.0, 0.0), 2: (23 / 12, -16 / 12, 5 / 12, 0.0), 3: (55 / 24, -59 / 24, 37 / 24, -9 / 24)}
+
+    def make_schedule(self, ddim_num_steps, ddim_eta=0.0, init_step=None):
+        if ddim_eta != 0.0:  # as the reference (samplers.py:356): the multistep epsilon has no noise term
+            raise NotImplementedError("PLMS: ddim_eta must be 0")
+        super().make_schedule(ddim_num_steps, ddim_eta, init_step)
 
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, eta=0.0, x_T=None, init_step=None, *, guidance_scale=1.0,
@@ -394,9 +462,10 @@ class FusedStep:
     run(x, t, coef_row) is the step-at-a-time form (explicit timestep / coefficients); forward(x, t) is its UNet half alone
     (PLMS, which applies its own update).
     step_kind "ddpm" issues k2_sampler_step (DDPM, and DDIM through linear coefficients); "dpmpp_2m" issues
-    k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state."""
+    k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state;
+    "dpmpp_2m_sde" issues k2_dpm_solver_sde_step the same way, with this step's noise."""
 
-    STEP_KINDS = ("ddpm", "dpmpp_2m")
+    STEP_KINDS = ("ddpm", "dpmpp_2m", "dpmpp_2m_sde")
 
     def __init__(self, model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode,
                  inpaint_init=None, inpaint_mask=None, inpaint_noise=None, step_kind="ddpm"):
@@ -413,7 +482,7 @@ class FusedStep:
         self.B = B
         self.guidance, self.cond_first, self.clip, self.mode = guidance_scale, int(cond_first), clip_range, threshold_mode
         self.step_kind = step_kind
-        dpm = step_kind == "dpmpp_2m"
+        dpm = step_kind != "ddpm"
         has_inpaint = inpaint_init is not None
         # buffers and the captured step graph live on the plan, keyed by everything the graph bakes in as a kernel argument
         renoise = inpaint_noise is not None
@@ -466,9 +535,9 @@ class FusedStep:
 
     def _update(self, x):
         """The scheduler update of x in place from the UNet output in plan.out, with the coefficient row in self.coef."""
-        if self.step_kind == "dpmpp_2m":
+        if self.step_kind != "ddpm":
             ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init,
-                                self.mask, self.rnoise)
+                                self.mask, self.rnoise, noise=self.noise if self.step_kind == "dpmpp_2m_sde" else None)
             return
 
         def sampler_step(mode):

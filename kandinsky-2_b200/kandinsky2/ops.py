@@ -406,16 +406,22 @@ def plms_step(model_out, x, out, hist, store, coef, guidance, cond_first):
     return out
 
 
-def dpm_solver_step(model_out, x, hist, coef, guidance, cond_first, inpaint_init=None, inpaint_mask=None, inpaint_noise=None):
+def dpm_solver_step(model_out, x, hist, coef, guidance, cond_first, inpaint_init=None, inpaint_mask=None, inpaint_noise=None,
+                    noise=None):
     """k2_dpm_solver_step: x fp32 [B,4,H,W] -> the next DPM-Solver++(2M) iterate in place; hist fp32 [B,4,H,W] -> this step's
-    x0 (read only when coef[4] != 0); coef = device fp32 [8] row of DPMSolverSchedule; see k2b200.h."""
-    tensors = (model_out, x, hist, coef, inpaint_init, inpaint_mask, inpaint_noise)
+    x0 (read only when coef[4] != 0); coef = device fp32 [8] row of DPMSolverSchedule; see k2b200.h.
+    noise fp32 [B,4,H,W] selects the SDE step, k2_dpm_solver_sde_step: x' += coef[7] noise (read only when coef[7] != 0)."""
+    tensors = (model_out, x, hist, coef, inpaint_init, inpaint_mask, inpaint_noise, noise)
     if not all(t is None or t.is_cuda for t in tensors):
         raise nat.K2Error("dpm_solver_step: tensors must live on a CUDA sm_90 device (no CPU fallback)")
     lib = nat.load()
     B, _, H, W = x.shape
-    check(lib.k2_dpm_solver_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef), B, H, W, float(guidance),
-                                 int(cond_first), ptr(inpaint_init), ptr(inpaint_mask), ptr(inpaint_noise), stream_ptr()))
+    tail = (ptr(coef), B, H, W, float(guidance), int(cond_first), ptr(inpaint_init), ptr(inpaint_mask), ptr(inpaint_noise),
+            stream_ptr())
+    if noise is None:
+        check(lib.k2_dpm_solver_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), *tail))
+    else:
+        check(lib.k2_dpm_solver_sde_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(noise), *tail))
     return x
 
 

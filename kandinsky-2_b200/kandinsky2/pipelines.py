@@ -68,8 +68,11 @@ def _new_h_w_latent_21(h, w):  # kandinsky2_1_model.py:106-113 (latent side, /8)
     return math.ceil(h / 64) * 8, math.ceil(w / 64) * 8
 
 
-SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler", "dpmpp_2m_sampler")
-SAMPLERS_22 = ("ddpm_sampler", "dpmpp_2m_sampler")
+# DPM-Solver++(2M) sampler name -> (timestep spacing, SDE variant) of its DPMSolverSchedule
+DPM_SAMPLERS = {"dpmpp_2m_sampler": ("linspace", False), "dpmpp_2m_karras_sampler": ("karras", False),
+                "dpmpp_2m_sde_sampler": ("linspace", True), "dpmpp_2m_sde_karras_sampler": ("karras", True)}
+SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(DPM_SAMPLERS)
+SAMPLERS_22 = ("ddpm_sampler",) + tuple(DPM_SAMPLERS)
 
 
 def _check_sampler(sampler, allowed):
@@ -141,10 +144,11 @@ class _DecoderBase:
         """Seeded by base_seed alone: every img2img call on one image starts from the same noisy latent."""
         return torch.randn(latent.shape, generator=torch.Generator().manual_seed(self.base_seed)).to(self.device)
 
-    def _dpm_img2img_start(self, latent, diffusion, num_steps, strength):
+    def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler):
         """DPM-Solver++ img2img -> (start latent, evaluations kept): the image latent noised to the first kept evaluation."""
         keep = _dpm_keep(num_steps, strength)
-        sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=keep)
+        spacing, sde = DPM_SAMPLERS[sampler]
+        sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=keep, spacing=spacing, sde=sde)
         return sched.start_latent(latent, self._img2img_noise(latent)), keep
 
     @torch.no_grad()
@@ -179,10 +183,12 @@ class _DecoderBase:
             noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
         shape = (2 * B, 4, H, W)
         self.model.del_cache()
-        if sampler == "dpmpp_2m_sampler":
-            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step)
+        if sampler in DPM_SAMPLERS:
+            spacing, sde = DPM_SAMPLERS[sampler]
+            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step, spacing=spacing, sde=sde)
             samples = sched.sample(self.model, shape, noise=noise, model_kwargs=kw, device=self.device,
-                                   guidance_scale=guidance_scale, cond_first=self.cond_first, **blend)
+                                   guidance_scale=guidance_scale, cond_first=self.cond_first,
+                                   sample_generators=self._generators(lo, hi) if sde else None, **blend)
         elif sampler in ("ddim_sampler", "plms_sampler"):  # kandinsky2_1_model.py:259-284: un-respaced schedule, eta 0
             cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
             samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, H, W), conditioning=kw, x_T=noise,
@@ -210,8 +216,10 @@ class Kandinsky2_1(_DecoderBase):
                      noise=None, init_img=None, img_mask=None, h=512, w=512, sampler="ddim_sampler", num_steps=50):
         """kandinsky2_1_model.py:184-292. img_prompt = cat([cond image emb, zero image emb]) [2B, 768].
         sampler="dpmpp_2m_sampler" runs DPM-Solver++(2M) over `num_steps` evaluations of diffusion's base schedule; with
-        init_step = s only the last s of them run (img2img), starting from `noise`.  Inpainting: the known region replaces
-        x0 inside the step (p_sampler and dpmpp_2m_sampler; the reference's DDIM / PLMS paths have no such blend)."""
+        init_step = s only the last s of them run (img2img), starting from `noise`.  "dpmpp_2m_karras_sampler" places the
+        evaluations with Karras sigma spacing, "dpmpp_2m_sde_sampler" / "dpmpp_2m_sde_karras_sampler" run the SDE variant
+        (fresh noise every step, drawn per global sample index like p_sampler's).  Inpainting: the known region replaces x0
+        inside the step (p_sampler and the dpmpp_2m samplers; the reference's DDIM / PLMS paths have no such blend)."""
         _check_sampler(sampler, SAMPLERS_21)
         full_emb, pooled_emb = self.embedder.text_emb(prompt, batch_size)
         cond = {"full_emb": full_emb.to(self.device), "pooled_emb": pooled_emb.to(self.device),
@@ -259,13 +267,13 @@ class Kandinsky2_1(_DecoderBase):
     def generate_img2img(self, prompt, pil_img, strength=0.7, num_steps=100, batch_size=1, guidance_scale=7, h=512,
                          w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25"):
         """kandinsky2_1_model.py:428-484: encode the image, noise it to step int(T*(1-strength)) and run the remaining steps.
-        With sampler="dpmpp_2m_sampler" the last int(num_steps*strength) solver evaluations run (at least 1), from the image
+        With a dpmpp_2m sampler the last int(num_steps*strength) solver evaluations run (at least 1), from the image
         noised to the first of them."""
         _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        if sampler == "dpmpp_2m_sampler":
-            x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength)
+        if sampler in DPM_SAMPLERS:
+            x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength, sampler)
         else:
             start_step = int(diffusion.num_timesteps * (1 - strength))
             dc = self.config["diffusion_config"]
@@ -308,7 +316,8 @@ class Kandinsky2_2(_DecoderBase):
                      init_step=None, hint=None, sampler="ddpm_sampler"):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
         106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
-        sampler="dpmpp_2m_sampler": DPM-Solver++(2M) over `steps` evaluations of the same base schedule instead (init_step =
+        sampler="dpmpp_2m_sampler" (or its Karras / SDE variants, DPM_SAMPLERS): DPM-Solver++(2M) over `steps` evaluations of
+        the same base schedule instead (init_step =
         the number of evaluations kept for img2img); inpainting re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}
@@ -346,8 +355,8 @@ class Kandinsky2_2(_DecoderBase):
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
-        if sampler == "dpmpp_2m_sampler":
-            x, start = self._dpm_img2img_start(lat, diffusion, decoder_steps, strength)
+        if sampler in DPM_SAMPLERS:
+            x, start = self._dpm_img2img_start(lat, diffusion, decoder_steps, strength, sampler)
         else:
             # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first
             start = _dpm_keep(decoder_steps, strength)

@@ -1,14 +1,14 @@
-"""Cost of the DPM-Solver++(2M) sampler against the default DDPM one at the cfg-2 geometry (Kandinsky 2.2 decoder, 768x768,
-4 images, guidance 4, the full-size UNet with random weights of the architecture).
+"""Cost of the DPM-Solver++(2M) samplers (ODE and SDE, linspace and Karras spacing) against the default DDPM one at the cfg-2
+geometry (Kandinsky 2.2 decoder, 768x768, 4 images, guidance 4, the full-size UNet with random weights of the architecture).
 
 Measures, in one process on cuda:0, and prints one JSON line (also written to --out if given):
   * whole-call images/s through Kandinsky2_2.generate_text2img (latent init, the denoising steps, MoVQ decode, uint8 + PIL) for
-    sampler="ddpm_sampler" x 50 steps and sampler="dpmpp_2m_sampler" x 20 and x 25: CUDA events, median of --calls
-    steady-state calls after one warm-up call per arm;
-  * graph-replayed steps/s of each sampler's step (k2_step_begin + UNet + k2_sampler_step or k2_dpm_solver_step +
-    k2_step_end, one graph launch per step), the two arms alternated --rounds times in this process;
-  * device time of one k2_dpm_solver_step and one k2_sampler_step launch (threshold mode 0, as the 2.2 step issues it) at this
-    geometry: CUDA events over --kernel-reps back-to-back launches.
+    sampler="ddpm_sampler" x 50 steps, "dpmpp_2m_sampler" x 20 and x 25, "dpmpp_2m_sde_sampler" x 20 and
+    "dpmpp_2m_karras_sampler" x 20: CUDA events, median of --calls steady-state calls after one warm-up call per arm;
+  * graph-replayed steps/s of each step kind (k2_step_begin + UNet + k2_sampler_step, k2_dpm_solver_step or
+    k2_dpm_solver_sde_step + k2_step_end, one graph launch per step), the three arms alternated --rounds times in this process;
+  * device time of one k2_dpm_solver_step, k2_dpm_solver_sde_step and k2_sampler_step launch (threshold mode 0, as the 2.2
+    step issues it) at this geometry: CUDA events over --kernel-reps back-to-back launches.
 The card's name, power limit and maximum SM clock are read in the same run (nvidia-smi query only).  Needs a CUDA sm_90 device.
 
     python profiles/sampler_steps.py [--out /tmp/sampler_steps.json]
@@ -72,10 +72,12 @@ def main():
     image_emb = torch.randn(2 * B, 1280, device=dev, generator=g)
     ddpm = create_ddpm_v22(50)
     dpm = DPMSolverSchedule(ddpm.base_alphas_cumprod, 20)
+    sde = DPMSolverSchedule(ddpm.base_alphas_cumprod, 20, sde=True)
     x_start = torch.randn(B, 4, H, W, device=dev, generator=g)
     noise = torch.randn(50, B, 4, H, W, device=dev, generator=g)
     arms = {}
-    for name, sched, kind, nseq in (("ddpm_sampler", ddpm, "ddpm", noise), ("dpmpp_2m_sampler", dpm, "dpmpp_2m", None)):
+    for name, sched, kind, nseq in (("ddpm_sampler", ddpm, "ddpm", noise), ("dpmpp_2m_sampler", dpm, "dpmpp_2m", None),
+                                    ("dpmpp_2m_sde_sampler", sde, "dpmpp_2m_sde", noise[:20])):
         coef, ts = sched._tables(dev)
         order = torch.arange(sched.num_timesteps - 1, -1, -1, device=dev)
         step = FusedStep(model, B, H, W, dict(image_emb=image_emb), guidance_scale=4.0, cond_first=False, clip_range=2.0,
@@ -93,7 +95,7 @@ def main():
             sps[name].append(round(1e3 * args.steps / ms, 3))
     res["steps_per_s"] = sps
     res["steps_per_s_note"] = (f"{args.steps} graph replays per run after {args.warmup} warm-up replays, arms alternated "
-                               f"{args.rounds} times; the DPM++ schedule wraps around its 20 rows")
+                               f"{args.rounds} times; the DPM++ schedules wrap around their 20 rows")
 
     # ---- step-kernel device time
     mo = torch.randn(2 * B, 8, H, W, device=dev, generator=g)
@@ -103,9 +105,11 @@ def main():
     work = torch.empty(B * 4 * H * W + 4096, device=dev)
     coef_ddpm = ddpm._tables(dev)[0][25].clone()
     coef_dpm = dpm._tables(dev)[0][10].clone()
-    assert float(coef_dpm[4]) != 0.0   # a second-order row: the history is read
+    coef_sde = sde._tables(dev)[0][10].clone()
+    assert float(coef_dpm[4]) != 0.0 and float(coef_sde[4]) != 0.0 and float(coef_sde[7]) != 0.0  # history and noise are read
     kern = {"k2_sampler_step": lambda: ops.sampler_step(mo, xk, nz, coef_ddpm, 4.0, False, 2.0, 0, work=work),
-            "k2_dpm_solver_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_dpm, 4.0, False)}
+            "k2_dpm_solver_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_dpm, 4.0, False),
+            "k2_dpm_solver_sde_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_sde, 4.0, False, noise=nz)}
     kt = {}
     for name, fn in kern.items():
         fn()
@@ -115,9 +119,10 @@ def main():
     n = B * 4 * H * W
     # fp32 words moved per latent element: DDPM reads cond + uncond eps, the variance, x (twice: one per kernel), the noise,
     # writes and re-reads x0 through a scratch buffer and writes x = 9; DPM++ reads cond + uncond eps, x and hist and writes
-    # x and hist = 6
+    # x and hist = 6; the SDE step also reads the noise = 7
     kt["k2_sampler_step"]["bytes"] = 4 * n * 9
     kt["k2_dpm_solver_step"]["bytes"] = 4 * n * 6
+    kt["k2_dpm_solver_sde_step"]["bytes"] = 4 * n * 7
     for v in kt.values():
         v["achieved_GBps"] = round(v["bytes"] / (v["us_per_launch"] * 1e-6) / 1e9, 1)
     res["step_kernel"] = kt
@@ -129,7 +134,8 @@ def main():
     pipe = Kandinsky2_2.__new__(Kandinsky2_2)
     _init_pipe_with_model(pipe, CONFIG_2_2, dev, model)
     calls = {}
-    for sampler, steps in (("ddpm_sampler", 50), ("dpmpp_2m_sampler", 20), ("dpmpp_2m_sampler", 25)):
+    for sampler, steps in (("ddpm_sampler", 50), ("dpmpp_2m_sampler", 20), ("dpmpp_2m_sampler", 25), ("dpmpp_2m_sde_sampler", 20),
+                           ("dpmpp_2m_karras_sampler", 20)):
         ms_all = []
         for it in range(args.calls + 1):   # call 0 builds plans / graphs
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
