@@ -37,8 +37,8 @@ long long k2_launch_count(void);
 void k2_reset_launch_count(void);
 /* Tuning knobs: key 0 = force conv/GEMM N tile (0 = auto); key 1 = split-K (0 auto, 1 off, n>1 forced);
  * key 2 = CTA-pair conv kernel (0 auto, 1 off; 2 = on is refused: sm_90 has no CTA-pair MMA);
- * key 4 = programmatic dependent launch (0/1); key 9 = attention query rows per CTA (1 = 128, 8 warps, default; 0 = 64,
- * 4 warps; bit-identical results); key 10 = default number of epilogue warp sets of the conv kernel (1 = the first
+ * key 4 = programmatic dependent launch (0/1); key 9 = accepted for compatibility and ignored (it chose between two CTA
+ * layouts of an earlier head-width-64 attention kernel; the current one has one); key 10 = default number of epilogue warp sets of the conv kernel (1 = the first
  * consumer warpgroup; 2 = both consumer warpgroups, each draining half of the 64-column pairs, for N tiles 128 and 256 -- N tile
  * 192 runs with one set: bit-identical results, faster where the K loop is short).  Keys 0, 1, 2 and 10 are process-wide defaults; k2_conv_gemm_cfg overrides them per call.
  * key 11 = blocks per SM the GroupNorm apply grids are sized for (0 = each kernel's real occupancy, i.e. one full wave). */
@@ -148,7 +148,7 @@ int k2_gn_apply_fold(const void* src0, int C0, int ld0, const void* src1, int C1
                      int ldx, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Attention, head dim 64, online softmax, on mma.sync tensor cores (QK^T and PV) with encoder K/V prepended.
+ * Attention, head dim 64, online softmax, on wgmma tensor cores (QK^T and PV) with encoder K/V prepended.
  * Replaces QKVAttention.forward (unet.py:286-340) incl. the optional flash-attn path (:303-332).
  *   qkv   fp16 [B, T, ldq] rows; head h owns channels [h*hs, (h+1)*hs) with q at +q_off, k at +k_off,
  *         v at +v_off (reference layout: hs=192, 0/64/128 -- unet.py:296).

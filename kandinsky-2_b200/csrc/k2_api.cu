@@ -31,8 +31,6 @@ bool pdl_enabled() { return g_pdl != 0; }
 static int g_conv_epi_sets = 1;
 static int g_gn_bps = 0;
 int gn_apply_blocks_per_sm() { return g_gn_bps; }
-static int g_attn_half = 1;
-int attention_half_rows() { return g_attn_half; }
 
 int num_sms() {
   static int n = 0;
@@ -278,8 +276,7 @@ int k2_set_tuning(int key, int value) {
     g_gn_bps = value;
     return 0;
   }
-  if (key == 9) {  // attention query rows per CTA: 1 = 128 (8 warps), 0 = 64 (4 warps)
-    g_attn_half = value ? 1 : 0;
+  if (key == 9) {  // accepted and ignored: the head-width-64 attention kernel has a single CTA layout (128 query rows)
     return 0;
   }
 

@@ -1,15 +1,19 @@
-// k2_attention.cu -- fused softmax(Q K^T * scale) V on sm_90 tensor cores (mma.sync m16n8k16, fp16 in / fp32 accumulate),
-// flash-style: no [T, Tkv] score matrix in HBM.  One kernel template serves both attention shapes of the model:
-//   head dim 64  (k2_attention_d64): QKVAttention.forward (kandinsky2/model/unet.py:286-340): the two torch.einsum calls
-//                (:335,:339), the fp32 softmax (:338), the torch.cat that prepends the encoder K/V (:300-302) and the optional
-//                flash-attn path (:303-332).  Keys / values are read from TWO buffers -- encoder tokens first, then the
-//                spatial tokens -- so the concat never exists.
-//   head dim 512 (k2_attention_d512): the single-head MoVQ AttnBlock (kandinsky2/vqgan/movq_modules.py:201-225; encoder twin
-//                vqgan_blocks.py:186-240).  Its output channels are split over two CTAs (DV = 256 each): an fp32 O row of 256
-//                channels is 128 registers per thread, the full 512 would not fit next to the scores.  8 warps = 128 queries
-//                per CTA, 16-key blocks.
+// k2_attention.cu -- fused softmax(Q K^T * scale) V on sm_90a tensor cores (fp16 in / fp32 accumulate), flash-style: no
+// [T, Tkv] score matrix in HBM.  Two kernels serve the two attention shapes of the model:
+//   head dim 64  (k2_attention_d64, attention_d64_kernel): QKVAttention.forward (kandinsky2/model/unet.py:286-340): the two
+//                torch.einsum calls (:335,:339), the fp32 softmax (:338), the torch.cat that prepends the encoder K/V (:300-302)
+//                and the optional flash-attn path (:303-332).  Keys / values are read from TWO tensor maps -- encoder tokens
+//                first, then the spatial tokens -- so the concat never exists.  Warp-specialised TMA -> wgmma kernel with the
+//                structure of FlashAttention-3 (Shah et al. 2024), described above the kernel.
+//   head dim 512 (k2_attention_d512, flash_attention_kernel): the single-head MoVQ AttnBlock (kandinsky2/vqgan/movq_modules.py:
+//                201-225; encoder twin vqgan_blocks.py:186-240) on mma.sync m16n8k16.  Its output channels are split over two
+//                CTAs (DV = 256 each): an fp32 O row of 256 channels is 128 registers per thread, the full 512 would not fit
+//                next to the scores.  8 warps = 128 queries per CTA, 16-key blocks.
+// Both follow one numerical recipe: fp32 scores, scale * log2(e) folded into ex2, row sums from the unrounded fp32 P, P rounded
+// to fp16 before PV (as in the reference's fp16 mode, unet.py:338), O / l rounded once to fp16.  Every key block they process
+// holds at least one valid key, so the running maximum is finite from the first block on.
 //
-// CTA = NW warps, 16 query rows per warp; per key block of BKV keys:
+// flash_attention_kernel: CTA = NW warps, 16 query rows per warp; per key block of BKV keys:
 //     S = Q K^T            Q fragments (ldmatrix) x K fragments (ldmatrix) from shared memory, fp32 in registers
 //     m = max(m, rowmax S * c), P = exp2(S * c - m), l = l * alpha + rowsum P, O = O * alpha + fp16(P) V
 //   P goes from the score accumulators straight into the A fragments of the PV product (same register layout), V is read
@@ -228,14 +232,273 @@ int launch_flash(const FlashParams& p, cudaStream_t stream) {
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------------------------
+// Head width 64.  At this width a score costs 256 tensor FLOPs (QK^T + PV) and one ex2: an H100 SM does 16 scores' worth of MMA
+// per clock and 16 ex2 per clock, so a warp that runs its MMAs and its softmax one after the other leaves the tensor cores idle
+// half the time.  The kernel overlaps the two (FlashAttention-3, Shah et al. 2024, sections 3.1-3.2):
+//   CTA = 3 warpgroups, 128 query rows.  Warpgroup 0 is the producer: one thread issues the TMA loads (Q once, then K / V blocks
+//   of 128 keys into a STAGES-deep mbarrier ring); the warpgroup gives its registers to the two consumer warpgroups, each of which
+//   owns 64 query rows.  Per key block j a consumer
+//     issues  S_j = Q K_j^T         wgmma m64n128k16, both operands in shared memory (K stored [key][channel] is K-major)
+//     issues  O += P_{j-1} V_{j-1}  wgmma m64n64k16, P in registers, V read MN-major ([key][channel]) with the transpose flag
+//     waits for S_j, runs the online softmax of block j while PV_{j-1} is still on the tensor cores (intra-warpgroup overlap),
+//     waits for PV_{j-1}, frees its stage, and rescales O by the new maximum before it issues PV_j.
+//   Named barriers make the two consumers take turns at issuing (inter-warpgroup ping-pong), so one's softmax runs while the
+//   other's products run.
+// Keys: ceil(Tc / 128) blocks from the encoder tensor map, then ceil(T / 128) blocks from qkv.  The tensor maps are [B][T][width]
+// with the width the heads span, so a box never reaches another image's rows or a strided view's gap columns; rows past Tc / T
+// arrive zero-filled and only the last block of each source masks its tail.
+// ------------------------------------------------------------------------------------------------------------------------------
+namespace d64 {
+constexpr int BQ = 128;                     // query rows per CTA (two consumer warpgroups of 64)
+constexpr int BKV = 128;                    // keys per block
+constexpr int STAGES = 4;                   // K / V ring depth: a stage stays busy until the PV of the next block is issued
+constexpr int TILE = 128 * 128;             // one 128-row x 64-channel fp16 tile, 128-byte swizzled rows
+constexpr int BAR_BYTES = 8 * (2 * STAGES + 1);
+constexpr int SMEM_BYTES = 1024 + TILE * (1 + 2 * STAGES) + BAR_BYTES;  // + slack to align the tiles to 1024 B
+constexpr int TURN_BAR = 1;                 // named barriers 1, 2: the issuing turn of consumer warpgroup 0, 1
+}  // namespace d64
+
+struct AttnD64Params {
+  CUtensorMap tm_qkv;  // [B][T][width of the heads' q | k | v], box 64 x 128 x 1
+  CUtensorMap tm_enc;  // [B][Tc][width of the heads' k | v] (unused when Tc = 0)
+  __half* out;         // [B, T, ldo], head h at channels 64 h
+  long long ldo;
+  int hs, q_off, k_off, v_off;
+  int ehs, ek_off, ev_off;
+  int T, Tc;
+  float scale_log2e;
+};
+
+// Online softmax of one 64 x 128 block held as an m64n128 accumulator: this thread's rows r0 = l / 4 and r0 + 8 of its warp's
+// 16 (h = (i / 2) & 1), key 8 (i / 4) + 2 (l & 3) + (i & 1) of the block.  s becomes the unrounded fp32 P; m / l are the running
+// maximum (scaled units) and this thread's partial row sums; alpha is the factor O must be rescaled by before P V is added.
+template <bool MASK>
+__device__ __forceinline__ void softmax_block(float (&s)[64], float (&m)[2], float (&l)[2], float (&alpha)[2], float c, int valid) {
+  const int kq = 2 * (threadIdx.x & 3);
+  if (MASK) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i)
+      if (8 * (i >> 2) + kq + (i & 1) >= valid) s[i] = -INFINITY;
+  }
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    const float m_new = fmaxf(m[h], mx[h] * c);  // finite: the block holds at least one valid key
+    alpha[h] = ex2(m[h] - m_new);                // 0 for the first block
+    m[h] = m_new;
+  }
+  float ls[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // two partial sums per row: shorter dependency chains
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int h = (i >> 1) & 1;
+    s[i] = ex2(fmaf(s[i], c, -m[h]));
+    ls[h][(i >> 2) & 1] += s[i];
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) l[h] = l[h] * alpha[h] + (ls[h][0] + ls[h][1]);
+}
+
+// grid: (query tiles, heads, B)
+__global__ void __launch_bounds__(384, 1) attention_d64_kernel(const __grid_constant__ AttnD64Params p) {
+  using namespace d64;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sK = smem + TILE;                   // [STAGES] tiles
+  uint8_t* sV = sK + STAGES * TILE;            // [STAGES] tiles
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sV + STAGES * TILE);
+  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* q_bar = empty_bar + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const int q0 = blockIdx.x * BQ;
+  const int head = blockIdx.y;
+  const int b = blockIdx.z;
+  const int nenc = (p.Tc + BKV - 1) / BKV;
+  const int nblk = nenc + (p.T + BKV - 1) / BKV;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&p.tm_qkv);
+    if (nenc) tma_prefetch_desc(&p.tm_enc);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp, after its wgmma.wait_group
+    }
+    mbar_init(q_bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_launch();
+
+  if (wg == 0) {
+    // ===================================== TMA producer =====================================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      mbar_arrive_expect_tx(q_bar, TILE);
+      tma_load_3d(sQ, &p.tm_qkv, q_bar, head * p.hs + p.q_off, q0, b);
+      for (int j = 0; j < nblk; ++j) {
+        const int st = j % STAGES;
+        if (j >= STAGES) mbar_wait_lean(&empty_bar[st], (j / STAGES - 1) & 1);
+        mbar_arrive_expect_tx(&full_bar[st], 2 * TILE);  // zero-filled rows count: the box is always written whole
+        if (j < nenc) {
+          tma_load_3d(sK + st * TILE, &p.tm_enc, &full_bar[st], head * p.ehs + p.ek_off, j * BKV, b);
+          tma_load_3d(sV + st * TILE, &p.tm_enc, &full_bar[st], head * p.ehs + p.ev_off, j * BKV, b);
+        } else {
+          tma_load_3d(sK + st * TILE, &p.tm_qkv, &full_bar[st], head * p.hs + p.k_off, (j - nenc) * BKV, b);
+          tma_load_3d(sV + st * TILE, &p.tm_qkv, &full_bar[st], head * p.hs + p.v_off, (j - nenc) * BKV, b);
+        }
+      }
+    }
+    return;
+  }
+
+  // ====================================== consumers ======================================
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;  // query rows [64 cw, 64 cw + 64) of the tile
+  const float c = p.scale_log2e;
+  const uint64_t qdesc = make_wgmma_desc(smem_u32(sQ) + cw * 64 * 128);
+  const uint32_t k_base = smem_u32(sK), v_base = smem_u32(sV);
+
+  float o[32], s[64], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2] = {0.f, 0.f};
+  uint32_t pa[32];  // fp16 P of the previous block: the A fragments of its 8 PV steps of 16 keys
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+
+  auto issue_pv = [&](int st) {
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+      wgmma_m64n64k16_rs_tb(o, a, make_wgmma_desc_mn(v_base + st * TILE) + static_cast<uint64_t>(kk * (2048 >> 4)));
+    }
+    wgmma_commit();
+  };
+  auto rescale_o = [&]() {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+  };
+
+  // S_j = Q K_j^T after this warpgroup's turn has come; hands the turn over once the block's products are issued
+  auto issue_s = [&](int j) {
+    const int st = j % STAGES;
+    mbar_wait_lean(&full_bar[st], (j / STAGES) & 1);
+    named_bar_sync(TURN_BAR + cw, 256);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)  // +32 B per 16 channels inside the 128 B swizzle row
+      wgmma_m64n128k16(s, qdesc + static_cast<uint64_t>(kk * 2), make_wgmma_desc(k_base + st * TILE) + static_cast<uint64_t>(kk * 2),
+                       kk > 0);
+    wgmma_commit();
+  };
+  // warpgroup 1 skips its last hand-over, so that every arrival at a turn barrier meets a wait
+  auto pass_turn = [&](int j) {
+    if (cw == 0 || j + 1 < nblk) named_bar_arrive(TURN_BAR + 1 - cw, 256);
+  };
+  auto softmax = [&](int j) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) reg_fence(s[i]);
+    const int valid = j < nenc ? p.Tc - j * BKV : p.T - (j - nenc) * BKV;
+    if (valid < BKV) softmax_block<true>(s, m, l, alpha, c, valid);
+    else softmax_block<false>(s, m, l, alpha, c, valid);
+  };
+  auto to_p = [&]() {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) pa[i] = pack_h2(s[2 * i], s[2 * i + 1]);
+  };
+
+  if (cw == 1) named_bar_arrive(TURN_BAR, 256);  // warpgroup 0 takes the first turn
+  mbar_wait_lean(q_bar, 0);
+  issue_s(0);
+  pass_turn(0);
+  wgmma_wait<0>();
+  softmax(0);
+  to_p();
+  for (int j = 1; j < nblk; ++j) {
+    const int pst = (j - 1) % STAGES;
+    rescale_o();  // by the maximum of block j - 1, before P_{j-1} V_{j-1} is added
+    issue_s(j);
+    issue_pv(pst);
+    pass_turn(j);
+    wgmma_wait<1>();  // S_j; P_{j-1} V_{j-1} stays on the tensor cores during the softmax
+    softmax(j);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(o[i]);
+    if (lane == 0) mbar_arrive(&empty_bar[pst]);
+    to_p();
+  }
+  rescale_o();
+  wgmma_fence();
+  issue_pv((nblk - 1) % STAGES);
+  wgmma_wait<0>();
+#pragma unroll
+  for (int i = 0; i < 32; ++i) reg_fence(o[i]);
+
+  // out = O / l
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+  }
+  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int q = q0 + 64 * cw + 16 * (warp & 3) + (lane >> 2) + 8 * h;
+    if (q >= p.T) continue;
+    __half* orow = p.out + (static_cast<long long>(b) * p.T + q) * p.ldo + head * 64 + 2 * (lane & 3);
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_h2(o[4 * n + 2 * h] * inv[h], o[4 * n + 2 * h + 1] * inv[h]);
+  }
+}
+
+int launch_attention_d64(const FlashParams& f, cudaStream_t stream) {
+  using namespace d64;
+  AttnD64Params p;
+  memset(&p, 0, sizeof p);
+  const uint32_t box[3] = {64, BKV, 1};  // BQ = BKV: Q, K and V tiles share the box
+  {
+    const uint64_t width = static_cast<uint64_t>(f.heads - 1) * f.hs + std::max(std::max(f.q_off, f.k_off), f.v_off) + 64;
+    const uint64_t dims[3] = {width, static_cast<uint64_t>(f.T), static_cast<uint64_t>(f.B)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(f.ldq) * 2, static_cast<uint64_t>(f.ldq) * 2 * f.T};
+    if (encode_tmap_f16(&p.tm_qkv, f.qkv, 3, dims, strides, box)) return -1;
+  }
+  if (f.Tc > 0) {
+    const uint64_t width = static_cast<uint64_t>(f.heads - 1) * f.ehs + std::max(f.ek_off, f.ev_off) + 64;
+    const uint64_t dims[3] = {width, static_cast<uint64_t>(f.Tc), static_cast<uint64_t>(f.B)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(f.lde) * 2, static_cast<uint64_t>(f.lde) * 2 * f.Tc};
+    if (encode_tmap_f16(&p.tm_enc, f.enc, 3, dims, strides, box)) return -1;
+  }
+  p.out = f.out;
+  p.ldo = f.ldo;
+  p.hs = f.hs; p.q_off = f.q_off; p.k_off = f.k_off; p.v_off = f.v_off;
+  p.ehs = f.ehs; p.ek_off = f.ek_off; p.ev_off = f.ev_off;
+  p.T = f.T; p.Tc = f.Tc;
+  p.scale_log2e = f.scale_log2e;
+  static bool attr_set = false;
+  if (!attr_set) {
+    K2_CHECK_CUDA(cudaFuncSetAttribute(attention_d64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    attr_set = true;
+  }
+  dim3 grid((f.T + BQ - 1) / BQ, f.heads, f.B);
+  K2_CHECK_CUDA(launch_k(attention_d64_kernel, grid, dim3(384), SMEM_BYTES, stream, p));
+  return 0;
+}
+
 }  // namespace
 
 int launch_attention(const FlashParams& p, int head_dim, cudaStream_t stream) {
   // head width 512: 8 warps x 16-key blocks (Q 130 KB + two K / V stages 49 KB of shared memory) -- 7.5 ms at the MoVQ 768 x 768
   // geometry on an H100 SXM at 700 W, against 12.0 ms with 4 warps x 32-key blocks (one CTA of 4 warps per SM)
   if (head_dim == 512) return launch_flash<512, 256, 8, 16>(p, stream);
-  // tuning key 9: query rows per CTA, 128 (8 warps, default) or 64 (4 warps); every warp computes its rows the same way
-  return attention_half_rows() ? launch_flash<64, 64, 8, 64>(p, stream) : launch_flash<64, 64, 4, 64>(p, stream);
+  return launch_attention_d64(p, stream);
 }
 
 }  // namespace k2

@@ -229,8 +229,42 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
       : K2_WGMMA_D32(0), K2_WGMMA_D32(32), K2_WGMMA_D32(64), K2_WGMMA_D32(96)
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// Descriptor of an MN-major B operand (wgmma with the transpose-B flag), 128-byte swizzle: each 128 B row holds 64 consecutive N
+// elements (fp16) of one K index, rows of consecutive K at a 128 B pitch -- a [K][N] tile as a TMA box with a 64 x fp16 inner
+// dimension and CU_TENSOR_MAP_SWIZZLE_128B writes it.  Canonical layout in 16 B units ((8,n),(8,k)) : ((1,LBO),(8,SBO)): unlike
+// the K-major form, SBO is the distance between 8-row groups along K and LBO the distance between 64-element swizzle atoms along
+// N.  An N = 64 operand is a single atom, so LBO is not used; SBO = 1024 B.  A K step of 16 rows advances the start address by
+// 2048 B (+128 in the address field).
+__device__ __forceinline__ uint64_t make_wgmma_desc_mn(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;          // LBO (one swizzle atom along N)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;  // SBO = 1024 B between 8-row groups along K
+  d |= static_cast<uint64_t>(1) << 62;          // SWIZZLE_128B
+  return d;
+}
+
+// D[64 x 64] (+)= A[64 x 16, registers] * B[16 x 64, smem, MN-major]: the A fragment of warp w (rows 16 w .. 16 w + 15 of the
+// warpgroup's 64), lane l is the mma.sync m16n8k16 one -- a[0] row l / 4, columns 2 (l & 3) + {0, 1}; a[1] row + 8; a[2]
+// columns + 8; a[3] both -- i.e. the places the m64nN accumulator layout above gives those elements, so an fp32 accumulator
+// converts into the next product's A operand in registers.  B is read with the transpose flag (allowed for 16-bit types).
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, {%32, %33, %34, %35}, %36, 1, 1, 1, 1;\n"
+      "}\n"
+      : K2_WGMMA_D32(0)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
+}
 #undef K2_WGMMA_D32
 #undef K2_WGMMA_D8
+
+// Ties a register to the position of this statement: keeps the compiler from moving reads or writes of a wgmma accumulator
+// across the wgmma.wait_group that completes it.
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // register budget of a warp-specialised kernel: the producer warpgroup gives registers back, the MMA warpgroups take them
 template <int R>
@@ -288,6 +322,10 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {
 // named barrier among `count` threads (count % 32 == 0); id 0 is __syncthreads'
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// arrive at a named barrier without waiting for it (the other `count` - 32 k threads wait with named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 // Programmatic dependent launch: every kernel of the step waits here (before its first global-memory access) for the
 // previous kernel in the stream to complete, and immediately lets the next kernel's CTAs be scheduled, so their

@@ -101,7 +101,6 @@ struct FlashParams {
   float scale_log2e;   // softmax scale * log2(e)
 };
 int gn_apply_blocks_per_sm();  // tuning key 11: blocks per SM the GroupNorm apply kernels are sized for (0 = their occupancy)
-int attention_half_rows();     // tuning key 9: 1 = 128 query rows per CTA (8 warps), 0 = 64 (4 warps)
 int launch_attention(const FlashParams& p, int head_dim, cudaStream_t stream);
 
 }  // namespace k2
