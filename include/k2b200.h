@@ -265,6 +265,24 @@ int k2_dpm_solver_sde_step(const float* model_out, int C2, float* x, float* hist
                            int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
                            const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream);
 
+/* UniPC step (Zhao et al. 2023, "UniPC"; data prediction, B(h) = bh2, order 2): the corrector UniC of the previous interval
+ * and the predictor UniP of the next one in one pass, one UNet evaluation per step, CFG closure fused.  Per element of x fp32
+ * [B, 4, H, W] (in place), with r = the step's row of 16 floats:
+ *   eps  = uncond + g (cond - uncond) as in k2_dpm_solver_step;
+ *   D    = r[0] x - r[1] eps;   D = D (1 - mask) + init mask   if inpaint_mask != NULL and inpaint_noise == NULL (2.1);
+ *   xc   = r[2] x + r[3] last + r[4] D + r[5] hist1 + r[6] hist2     (the corrected sample);
+ *   x'   = r[7] xc + r[8] D + r[9] hist1;
+ *   x'   = mask (r[10] init + r[11] inpaint_noise) + (1 - mask) x'   if inpaint_noise != NULL (2.2; `last` is not blended);
+ *   last = xc;  hist2 = hist1;  hist1 = D.
+ * last, hist1 and hist2 (fp32 [B, 4, H, W]) enter a sum only under a non-zero coefficient, so whatever they hold (even NaN)
+ * cannot reach the result of a row that does not use them.  r = {1/alpha_k, sigma_k/alpha_k, a_x, a_L, a_0, a_1, a_2, b_c,
+ * b_0, b_1, alpha_{k+1}, sigma_{k+1}, 0, 0, 0, 0} (kandinsky2/model/gaussian_diffusion.py: unipc_rows).  coef is device fp32:
+ * with counter == NULL it is the row itself; otherwise it is a table [steps][16] and the row is counter[0] % counter[1] of the
+ * device int32 counter k2_step_begin / k2_step_end maintain.  Arguments are checked before any CUDA call. */
+int k2_unipc_step(const float* model_out, int C2, float* x, float* last, float* hist1, float* hist2, const float* coef,
+                  const int* counter, int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
+                  const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * MoVQ helpers: nearest-codebook search (quntize.py:89-98; fp32, ties -> lowest index, int64 out),
  * fp32 NCHW -> NHWC transposes for the 4-channel latent, final image quantisation

@@ -456,6 +456,58 @@ __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p)
   p.x[i] = xn;
 }
 
+// UniPC update (Zhao et al. 2023; data prediction, B(h) = bh2, order 2), linear in (x, eps, last, D_{k-1}, D_{k-2}):
+//   D   = r[0] x - r[1] eps                                              (the x0 prediction of the CFG epsilon)
+//   xc  = r[2] x + r[3] last + r[4] D + r[5] h1 + r[6] h2                 (UniC; r[2] = 1, r[3..6] = 0 without it)
+//   x'  = r[7] xc + r[8] D + r[9] h1                                     (UniP)
+//   last = xc;  h2 = h1;  h1 = D                                         (h1 = D_{k-1}, h2 = D_{k-2})
+// last, h1 and h2 are read only under a non-zero coefficient.  The row (16 floats, UniPCSchedule) is row counter[0] of the
+// staged table when counter is given (the step graph), else coef itself.
+struct UniPCParams {
+  const float* model_out;  // [2B, C2, H, W], eps = channels [0, 4)
+  float* x;                // [B, 4, H, W], in place
+  float* last;             // [B, 4, H, W]: the previous corrected sample in, this step's out
+  float* h1;               // [B, 4, H, W]: D_{k-1} in, D_k out
+  float* h2;               // [B, 4, H, W]: D_{k-2} in, D_{k-1} out
+  const float* coef;       // device fp32 [rows][16]
+  const int* counter;      // device (step, steps) or null
+  int B, HW, C2;
+  float guidance;
+  int cond_first;
+  const float* init;       // [B,4,H,W] or null
+  const float* mask;       // [B,1,H,W] or null
+  const float* rnoise;     // [B,4,H,W] or null (2.2 inpainting: the known region of x' is re-noised to the next timestep)
+};
+
+__global__ void __launch_bounds__(256) unipc_step_kernel(const UniPCParams p) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  pdl_wait();
+  pdl_launch();
+  const long long total = static_cast<long long>(p.B) * 4 * p.HW;
+  if (i >= total) return;
+  const float* r = p.coef;
+  if (p.counter) r += 16LL * (p.counter[0] % max(p.counter[1], 1));
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, p.guidance, p.cond_first);
+  const float xv = p.x[i];
+  float d = r[0] * xv - r[1] * e.eps;
+  const float m = p.mask ? p.mask[static_cast<long long>(e.b) * p.HW + e.sp] : 0.f;
+  if (p.mask && !p.rnoise) d = d * (1.f - m) + p.init[i] * m;  // Kandinsky 2.1: the known region replaces D
+  const float a_x = r[2], a_l = r[3], a_1 = r[5], a_2 = r[6], b_1 = r[9];
+  const float h1 = p.h1[i];  // always loaded (it moves to h2), used only under a non-zero coefficient
+  float xc = r[4] * d;
+  if (a_x != 0.f) xc += a_x * xv;
+  if (a_l != 0.f) xc += a_l * p.last[i];
+  if (a_1 != 0.f) xc += a_1 * h1;
+  if (a_2 != 0.f) xc += a_2 * p.h2[i];
+  float xn = r[7] * xc + r[8] * d;
+  if (b_1 != 0.f) xn += b_1 * h1;
+  if (p.mask && p.rnoise) xn = m * (r[10] * p.init[i] + r[11] * p.rnoise[i]) + (1.f - m) * xn;
+  p.h2[i] = h1;
+  p.h1[i] = d;
+  p.last[i] = xc;
+  p.x[i] = xn;
+}
+
 // ------------------------------------------------------------------------------------------------
 // MoVQ helpers
 // ------------------------------------------------------------------------------------------------
@@ -895,6 +947,23 @@ int k2_dpm_solver_sde_step(const float* model_out, int C2, float* x, float* hist
   K2_REQUIRE(noise, "dpm_solver_sde_step: null noise");
   return dpm_step("dpm_solver_sde_step", model_out, C2, x, hist, noise, coef, B, H, W, guidance, cond_first, inpaint_init,
                   inpaint_mask, inpaint_noise, stream);
+}
+
+int k2_unipc_step(const float* model_out, int C2, float* x, float* last, float* hist1, float* hist2, const float* coef,
+                  const int* counter, int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
+                  const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && last && hist1 && hist2 && coef, "unipc_step: null pointer");
+  K2_REQUIRE(B > 0 && H > 0 && W > 0 && C2 >= 4, "unipc_step: B, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE((inpaint_init == nullptr) == (inpaint_mask == nullptr), "unipc_step: init and mask go together");
+  K2_REQUIRE(inpaint_noise == nullptr || inpaint_init, "unipc_step: inpaint_noise without init / mask");
+  UniPCParams p;
+  p.model_out = model_out; p.x = x; p.last = last; p.h1 = hist1; p.h2 = hist2; p.coef = coef; p.counter = counter;
+  p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
+  p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
+  const long long total = static_cast<long long>(B) * 4 * H * W;
+  K2_CHECK_CUDA(launch_k(unipc_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p));
+  count_launch();
+  return 0;
 }
 
 int k2_vq_argmin(const float* z, const float* codebook, long long* idx, int n, int n_embed, int dim,

@@ -51,13 +51,13 @@ class _Schedule:
     """What _sampling_loop needs of a schedule: coef_table() (fp32 [n, 8] step-kernel rows) and model_timesteps() (what the UNet
     sees, [n]) in the same index order; the loop runs the rows n-1 .. 0.  Each schedule also states whether its step draws
     noise and which step kernel applies its rows ("ddpm": k2_sampler_step, "dpmpp_2m": k2_dpm_solver_step, "dpmpp_2m_sde":
-    k2_dpm_solver_sde_step)."""
+    k2_dpm_solver_sde_step, "unipc": k2_unipc_step, whose rows are 16 floats wide)."""
 
     draws_noise = True
     step_kind = "ddpm"
 
     def _tables(self, device):
-        """-> (coef fp32 [n, 8], model timesteps fp32 [n]) on `device`, built once per device."""
+        """-> (coef fp32 [n, 8] or [n, 16], model timesteps fp32 [n]) on `device`, built once per device."""
         key = str(device)
         if key not in self._dev_tables:
             self._dev_tables[key] = (torch.from_numpy(self.coef_table()).to(device),
@@ -185,15 +185,7 @@ class DPMSolverSchedule(_Schedule):
         keep = n if keep is None else int(keep)
         if not 1 <= keep <= n:
             raise ValueError(f"DPM-Solver++: keep must be in [1, {n}], got {keep}")
-        if spacing == "linspace":
-            tau = np.linspace(0, len(ac) - 1, n + 1).round()[::-1][:n].astype(np.int64)
-            if np.any(np.diff(tau) >= 0):
-                raise ValueError(f"DPM-Solver++: {n} steps do not give distinct timesteps over {len(ac)} training steps")
-            alphas, sigmas = np.sqrt(ac[tau]), np.sqrt(1.0 - ac[tau])
-        else:
-            tau, s_hat = karras_timesteps(ac, n)
-            alphas = 1.0 / np.sqrt(1.0 + s_hat ** 2)
-            sigmas = s_hat * alphas
+        tau, alphas, sigmas = _solver_grid("DPM-Solver++", ac, n, spacing)
         self.num_steps, self.k0 = n, n - keep
         self.spacing, self.sde = spacing, bool(sde)
         self.draws_noise = self.sde
@@ -274,6 +266,152 @@ def karras_timesteps(base_alphas_cumprod, n, rho=7.0):
         s_hat[-1] = s_min
     t = np.interp(np.log(s_hat), log_table, np.arange(len(ac), dtype=np.float64))
     return t, s_hat
+
+
+def _solver_grid(kind, ac, n, spacing):
+    """(model timesteps [n], alpha [n], sigma [n]) of an n-evaluation multistep-solver run over the base table ac."""
+    if spacing == "linspace":
+        tau = np.linspace(0, len(ac) - 1, n + 1).round()[::-1][:n].astype(np.int64)
+        if np.any(np.diff(tau) >= 0):
+            raise ValueError(f"{kind}: {n} steps do not give distinct timesteps over {len(ac)} training steps")
+        return tau, np.sqrt(ac[tau]), np.sqrt(1.0 - ac[tau])
+    tau, s_hat = karras_timesteps(ac, n)
+    alphas = 1.0 / np.sqrt(1.0 + s_hat ** 2)
+    return tau, alphas, s_hat * alphas
+
+
+UNIPC_ROW = 16   # floats per k2_unipc_step row
+
+
+def unipc_rows(alphas, sigmas, first=0, order=2, corrector=True, lower_order_final=True):
+    """float64 [n - first, 16]: the k2_unipc_step rows of steps k = first .. n-1 (step order) on any grid alphas / sigmas [n+1]
+    (the target sigma_n may be 0, the sampler's, or interior).  UniPC with data prediction and B(h) = bh2 = e^{-h} - 1 (see
+    UniPCSchedule); a step's update is linear in (x_k, eps_k, last, D_{k-1}, D_{k-2}):
+        D_k   = c0 x_k - c1 eps_k,                                       c0 = 1 / alpha_k,  c1 = sigma_k / alpha_k
+        x_k^c = a_x x_k + a_L last + a_0 D_k + a_1 D_{k-1} + a_2 D_{k-2}   (UniC; a_x = 1 and the rest 0 without it)
+        x_k+1 = b_c x_k^c + b_0 D_k + b_1 D_{k-1}                         (UniP)
+    row = {c0, c1, a_x, a_L, a_0, a_1, a_2, b_c, b_0, b_1, alpha_{k+1}, sigma_{k+1}, 0, 0, 0, 0}.
+    With phi(h) = e^{-h} - 1 and r = (lambda of the older point - lambda of the interval's start) / h (r < 0):
+        UniP order 1:  b_c = sigma_{k+1} / sigma_k,  b_0 = -alpha_{k+1} phi;  order 2: b_0 = -alpha_{k+1} phi (1 - 1/(2r)),
+            b_1 = -alpha_{k+1} phi / (2r)  -- DPM-Solver++(2M);  sigma_{k+1} = 0: b_c = 0, b_0 = alpha_{k+1} (x' = D_k)
+        UniC over [k-1, k] with the order p of step k-1's predictor, h = lambda_k - lambda_{k-1}:  a_L = sigma_k / sigma_{k-1};
+            p = 1:  rho = 1/2;  p = 2: (rho_1, rho_2) solves [[1, 1], [r, 1]] rho = (g_1, g_2) with g_1 = (phi/(-h) - 1) / phi,
+            g_2 = 2 ((phi/(-h) - 1)/(-h) - 1/2) / phi;
+            a_0 = -alpha_k phi rho_p,  a_1 = -alpha_k phi (1 - rho_p - rho_1 / r),  a_2 = -alpha_k phi rho_1 / r.
+    The predictor's order ramps up from the first step, min(order, k - first + 1), and is 1 at the last step when
+    lower_order_final; the corrector runs at every step after the first.  order: 1 or 2."""
+    if order not in (1, 2):
+        raise ValueError(f"UniPC: order must be 1 or 2, got {order}")
+    a, s = np.asarray(alphas, dtype=np.float64), np.asarray(sigmas, dtype=np.float64)
+    n = len(a) - 1
+    with np.errstate(divide="ignore"):
+        lam = np.log(a) - np.log(s)
+    rows = np.zeros((n, UNIPC_ROW), dtype=np.float64)
+    prev_p = None
+    for k in range(first, n):
+        row = rows[k]
+        row[0], row[1], row[10], row[11] = 1.0 / a[k], s[k] / a[k], a[k + 1], s[k + 1]
+        row[2] = 1.0
+        if corrector and k > first:
+            h = lam[k] - lam[k - 1]
+            phi = np.expm1(-h)
+            if prev_p == 1:
+                rho_1, rho_p, r = 0.0, 0.5, 1.0
+            else:
+                r = (lam[k - 2] - lam[k - 1]) / h
+                g1 = (phi / -h - 1.0) / phi
+                g2 = 2.0 * ((phi / -h - 1.0) / -h - 0.5) / phi
+                rho_1 = (g1 - g2) / (1.0 - r)
+                rho_p = g1 - rho_1
+            row[2], row[3] = 0.0, s[k] / s[k - 1]
+            row[4] = -a[k] * phi * rho_p
+            row[5] = -a[k] * phi * (1.0 - rho_p - rho_1 / r)
+            row[6] = -a[k] * phi * rho_1 / r
+        p = min(order, k - first + 1)
+        if lower_order_final:
+            p = min(p, n - k)
+        if s[k + 1] == 0.0:                               # h = inf: x_{k+1} = alpha_{k+1} D_k
+            if p != 1:
+                raise ValueError("UniPC: a step to sigma = 0 must be first order (lower_order_final)")
+            row[8] = a[k + 1]
+        else:
+            h = lam[k + 1] - lam[k]
+            c = -a[k + 1] * np.expm1(-h)
+            row[7] = s[k + 1] / s[k]
+            if p == 1:
+                row[8] = c
+            else:
+                r = (lam[k - 1] - lam[k]) / h
+                row[8], row[9] = c * (1.0 - 0.5 / r), c * 0.5 / r
+        prev_p = p
+    return np.ascontiguousarray(rows[first:])
+
+
+class UniPCSchedule(_Schedule):
+    """UniPC (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework for Fast Sampling of Diffusion Models") with
+    data prediction, B(h) = bh2 and solver order 2, over the model's own base table alphas_cumprod (float64), in the step order of
+    diffusers' UniPCMultistepScheduler: one CFG-doubled UNet evaluation per step, no noise.
+
+    The N evaluations are DPMSolverSchedule's (spacing "linspace" or "karras", the same grid and model timesteps), and its
+    predictor UniP-2 with bh2 is DPM-Solver++(2M) exactly.  What UniPC adds is the corrector UniC: once the UNet has run at x_k,
+    the previous interval is solved again from the previous corrected sample with the new D_k, which raises the order by one at
+    no extra evaluation.  The predictor then continues from the corrected x_k^c; the history keeps D_k of the uncorrected x_k.
+    The predictor is first order at the first step (also the first step after an img2img truncation) and at the last one, which
+    lands on D_{N-1} exactly; unipc_rows holds the formulas.  keep = s (img2img): only the last s evaluations run, from
+    start_latent.
+
+    Rows are 16 floats (unipc_rows), stored in reverse step order like DPMSolverSchedule's; k2_unipc_step reads its row from the
+    staged table by the device-side step counter."""
+
+    SPACINGS = ("linspace", "karras")
+    draws_noise = False
+    step_kind = "unipc"
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace"):
+        ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
+        n = int(num_steps)
+        if n < 1:
+            raise ValueError("UniPC: num_steps must be >= 1")
+        if spacing not in self.SPACINGS:
+            raise ValueError(f"UniPC: spacing must be one of {self.SPACINGS}, got {spacing!r}")
+        keep = n if keep is None else int(keep)
+        if not 1 <= keep <= n:
+            raise ValueError(f"UniPC: keep must be in [1, {n}], got {keep}")
+        tau, alphas, sigmas = _solver_grid("UniPC", ac, n, spacing)
+        self.num_steps, self.k0, self.spacing = n, n - keep, spacing
+        self.timesteps = tau
+        self.alphas = np.append(alphas, 1.0)    # alpha_0 .. alpha_N
+        self.sigmas = np.append(sigmas, 0.0)
+        self.num_timesteps = keep
+        self._dev_tables = {}
+
+    def coef_rows(self):
+        """float64 [keep, 16]: the rows of steps k = N-1 .. k0 (table order)."""
+        return np.ascontiguousarray(unipc_rows(self.alphas, self.sigmas, first=self.k0)[::-1])
+
+    def coef_table(self):
+        """float32 [keep, 16]: the k2_unipc_step rows, built in float64 and cast once."""
+        return self.coef_rows().astype(np.float32)
+
+    def model_timesteps(self):
+        """float32 [keep]: what the UNet sees, in table order."""
+        return self.timesteps[self.k0:][::-1].astype(np.float32)
+
+    def start_latent(self, latent, noise):
+        """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
+        return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
+
+    @torch.no_grad()
+    def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
+               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None, sample_generators=None):
+        """DPMSolverSchedule.sample's call surface: shape = (2*B, 4, h, w), noise = the start latent; returns [2*B, 4, h, w]
+        whose two halves both hold the B samples.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces D), True =
+        Kandinsky 2.2 (the known region of x is re-noised to the next timestep with the start latent as the noise; the
+        corrector's previous sample is not blended, as in diffusers).  The step draws no noise, so sample_generators (the
+        solver samplers' common call surface) is ignored."""
+        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
+                              guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
+                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback)
 
 
 def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,
@@ -463,9 +601,11 @@ class FusedStep:
     (PLMS, which applies its own update).
     step_kind "ddpm" issues k2_sampler_step (DDPM, and DDIM through linear coefficients); "dpmpp_2m" issues
     k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state;
-    "dpmpp_2m_sde" issues k2_dpm_solver_sde_step the same way, with this step's noise."""
+    "dpmpp_2m_sde" issues k2_dpm_solver_sde_step the same way, with this step's noise; "unipc" issues k2_unipc_step with
+    UniPCSchedule's 16-float rows, which it reads from its own staged table by the step counter, on the last-sample and two-deep
+    D history buffers of the step state."""
 
-    STEP_KINDS = ("ddpm", "dpmpp_2m", "dpmpp_2m_sde")
+    STEP_KINDS = ("ddpm", "dpmpp_2m", "dpmpp_2m_sde", "unipc")
 
     def __init__(self, model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode,
                  inpaint_init=None, inpaint_mask=None, inpaint_noise=None, step_kind="ddpm"):
@@ -498,6 +638,9 @@ class FusedStep:
                       mask=torch.zeros(B, 1, H, W, **f32) if has_inpaint else None, x=torch.zeros(B, 4, H, W, **f32),
                       rnoise=torch.zeros(B, 4, H, W, **f32) if renoise else None,
                       hist=torch.zeros(B, 4, H, W, **f32) if dpm else None)
+            if step_kind == "unipc":
+                st.update(last=torch.zeros(B, 4, H, W, **f32), hist2=torch.zeros(B, 4, H, W, **f32),
+                          coef16=torch.zeros(UNIPC_ROW, **f32), coef16_seq=torch.zeros(4096, UNIPC_ROW, **f32))
             states[key] = st
         self.st = st
         self.noise, self.coef, self.work = st["noise"], st["coef"], st["work"]
@@ -515,14 +658,17 @@ class FusedStep:
 
     # -- scheduled mode ---------------------------------------------------------------------------
     def set_schedule(self, ts_seq, coef_seq, noise_seq=None):
-        """ts_seq fp32 [n], coef_seq fp32 [n, 8] in LOOP order; noise_seq fp32 [n, B, 4, H, W] or None (then the caller
-        fills self.noise before every advance()).  Resets the device-side step counter."""
+        """ts_seq fp32 [n], coef_seq fp32 [n, 8] ([n, 16] for "unipc") in LOOP order; noise_seq fp32 [n, B, 4, H, W] or None
+        (then the caller fills self.noise before every advance()).  Resets the device-side step counter and the history."""
         st = self.st
         n = ts_seq.shape[0]
         if n > st["ts_seq"].shape[0]:
             raise K2Error("FusedStep: more than 4096 sampling steps")
         st["ts_seq"][:n].copy_(ts_seq)
-        st["coef_seq"][:n].copy_(coef_seq)
+        if self.step_kind == "unipc":
+            st["coef16_seq"][:n].copy_(coef_seq)   # k2_step_begin stages the (unused) zero rows of coef_seq
+        else:
+            st["coef_seq"][:n].copy_(coef_seq)
         if noise_seq is not None:
             if st["noise_seq"] is None or st["noise_seq"].shape[0] < n:
                 st["noise_seq"] = torch.empty((n,) + tuple(self.noise.shape), device=self.noise.device, dtype=torch.float32)
@@ -530,11 +676,19 @@ class FusedStep:
             st["noise_seq"][:n].copy_(noise_seq)
         self._use_noise_seq = noise_seq is not None
         st["counter"].copy_(torch.tensor([0, n], dtype=torch.int32))
-        if st["hist"] is not None:
-            st["hist"].zero_()
+        for name in ("hist", "last", "hist2"):
+            if st.get(name) is not None:
+                st[name].zero_()
 
-    def _update(self, x):
-        """The scheduler update of x in place from the UNet output in plan.out, with the coefficient row in self.coef."""
+    def _update(self, x, scheduled=False):
+        """The scheduler update of x in place from the UNet output in plan.out, with the coefficient row in self.coef (UniPC:
+        the staged row of the step counter when scheduled, else self.st["coef16"])."""
+        if self.step_kind == "unipc":
+            st = self.st
+            ops.unipc_step(self.plan.out, x, st["last"], st["hist"], st["hist2"], st["coef16_seq"] if scheduled else st["coef16"],
+                           self.guidance, self.cond_first, counter=st["counter"] if scheduled else None,
+                           inpaint_init=self.init, inpaint_mask=self.mask, inpaint_noise=self.rnoise)
+            return
         if self.step_kind != "ddpm":
             ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init,
                                 self.mask, self.rnoise, noise=self.noise if self.step_kind == "dpmpp_2m_sde" else None)
@@ -562,7 +716,7 @@ class FusedStep:
             p.run(True)
         else:
             p.launch()
-        self._update(x)
+        self._update(x, scheduled=True)
         ops.step_end(st["counter"])
 
     def _sync_threshold(self):
@@ -611,8 +765,8 @@ class FusedStep:
         return p.out
 
     def run(self, x, t_scalar, coef_row):
-        """x fp32 [B,4,H,W] is updated in place to x_{t-1}."""
-        self.coef.copy_(coef_row)
+        """x fp32 [B,4,H,W] is updated in place to x_{t-1} (coef_row: 16 floats for "unipc", else 8)."""
+        (self.st["coef16"] if self.step_kind == "unipc" else self.coef).copy_(coef_row)
         self.forward(x, t_scalar)
         self._update(x)
         return x

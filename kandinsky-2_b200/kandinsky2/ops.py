@@ -425,6 +425,22 @@ def dpm_solver_step(model_out, x, hist, coef, guidance, cond_first, inpaint_init
     return x
 
 
+def unipc_step(model_out, x, last, hist1, hist2, coef, guidance, cond_first, counter=None, inpaint_init=None, inpaint_mask=None,
+               inpaint_noise=None):
+    """k2_unipc_step: x fp32 [B,4,H,W] -> the next UniPC iterate in place; last -> this step's corrected sample, (hist1, hist2)
+    -> (D_k, D_{k-1}).  coef: a device fp32 [16] row of UniPCSchedule, or with counter (device int32 [2] = (k, steps)) the
+    staged table [steps, 16] whose row k applies; see k2b200.h."""
+    tensors = (model_out, x, last, hist1, hist2, coef, counter, inpaint_init, inpaint_mask, inpaint_noise)
+    if not all(t is None or t.is_cuda for t in tensors):
+        raise nat.K2Error("unipc_step: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    lib = nat.load()
+    B, _, H, W = x.shape
+    check(lib.k2_unipc_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(last), ptr(hist1), ptr(hist2), ptr(coef),
+                            ptr(counter), B, H, W, float(guidance), int(cond_first), ptr(inpaint_init), ptr(inpaint_mask),
+                            ptr(inpaint_noise), stream_ptr()))
+    return x
+
+
 def vq_argmin(z, codebook):
     """z fp32 [n, dim], codebook fp32 [n_embed, dim] -> int64 [n] (ties -> lowest index)."""
     lib = nat.load()

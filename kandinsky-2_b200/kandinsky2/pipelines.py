@@ -17,7 +17,7 @@ import torch
 
 from . import ops, parallel
 from ._native import K2Error
-from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, PLMSSampler, create_ddpm_v22,
+from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, PLMSSampler, UniPCSchedule, create_ddpm_v22,
                                        create_gaussian_diffusion)
 from .model.model_creation import create_model
 from .utils import prepare_image, prepare_mask, q_sample, uint8_to_pil
@@ -71,8 +71,13 @@ def _new_h_w_latent_21(h, w):  # kandinsky2_1_model.py:106-113 (latent side, /8)
 # DPM-Solver++(2M) sampler name -> (timestep spacing, SDE variant) of its DPMSolverSchedule
 DPM_SAMPLERS = {"dpmpp_2m_sampler": ("linspace", False), "dpmpp_2m_karras_sampler": ("karras", False),
                 "dpmpp_2m_sde_sampler": ("linspace", True), "dpmpp_2m_sde_karras_sampler": ("karras", True)}
-SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(DPM_SAMPLERS)
-SAMPLERS_22 = ("ddpm_sampler",) + tuple(DPM_SAMPLERS)
+# UniPC sampler name -> timestep spacing of its UniPCSchedule
+UNIPC_SAMPLERS = {"unipc_sampler": "linspace", "unipc_karras_sampler": "karras"}
+# every multistep-solver sampler name -> (schedule class, its keyword arguments): the one table _decode and the img2img start use
+SOLVER_SAMPLERS = {**{name: (DPMSolverSchedule, dict(spacing=sp, sde=sde)) for name, (sp, sde) in DPM_SAMPLERS.items()},
+                   **{name: (UniPCSchedule, dict(spacing=sp)) for name, sp in UNIPC_SAMPLERS.items()}}
+SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(SOLVER_SAMPLERS)
+SAMPLERS_22 = ("ddpm_sampler",) + tuple(SOLVER_SAMPLERS)
 
 
 def _check_sampler(sampler, allowed):
@@ -81,9 +86,15 @@ def _check_sampler(sampler, allowed):
 
 
 def _dpm_keep(num_steps, strength):
-    """img2img with DPM-Solver++ (and the 2.2 DDPM sampler, as diffusers): the last int(N * strength) evaluations run (at
-    least 1)."""
+    """img2img with DPM-Solver++ or UniPC (and the 2.2 DDPM sampler, as diffusers): the last int(N * strength) evaluations run
+    (at least 1)."""
     return max(min(int(num_steps * strength), num_steps), 1)
+
+
+def _solver_schedule(sampler, diffusion, num_steps, keep=None):
+    """The DPMSolverSchedule / UniPCSchedule of a SOLVER_SAMPLERS name over diffusion's base table."""
+    cls, kw = SOLVER_SAMPLERS[sampler]
+    return cls(diffusion.base_alphas_cumprod, num_steps, keep=keep, **kw)
 
 
 class _DecoderBase:
@@ -145,10 +156,10 @@ class _DecoderBase:
         return torch.randn(latent.shape, generator=torch.Generator().manual_seed(self.base_seed)).to(self.device)
 
     def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler):
-        """DPM-Solver++ img2img -> (start latent, evaluations kept): the image latent noised to the first kept evaluation."""
+        """DPM-Solver++ / UniPC img2img -> (start latent, evaluations kept): the image latent noised to the first kept
+        evaluation."""
         keep = _dpm_keep(num_steps, strength)
-        spacing, sde = DPM_SAMPLERS[sampler]
-        sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=keep, spacing=spacing, sde=sde)
+        sched = _solver_schedule(sampler, diffusion, num_steps, keep)
         return sched.start_latent(latent, self._img2img_noise(latent)), keep
 
     @torch.no_grad()
@@ -158,7 +169,7 @@ class _DecoderBase:
         the version's row order; rank 0's copy is broadcast and this rank keeps its rows.  noise: the start latents
         [2 * batch_size, 4, H, W], or None to draw them per global sample index.  inpaint: (clean latent [1, 4, H, W], mask
         [1, 1, H, W]) for every sample, on the device.  hint: the ControlNet depth map [1, 3, h, w] for every row.  Runs
-        `sampler` over `diffusion` (`num_steps` evaluations for the DDIM, PLMS and DPM-Solver++ samplers) and decodes this
+        `sampler` over `diffusion` (`num_steps` evaluations for the DDIM, PLMS, DPM-Solver++ and UniPC samplers) and decodes this
         rank's samples to image_hw."""
         rank, ws = parallel.world()
         lo, hi = parallel.shard_range(batch_size, rank, ws)
@@ -183,12 +194,11 @@ class _DecoderBase:
             noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
         shape = (2 * B, 4, H, W)
         self.model.del_cache()
-        if sampler in DPM_SAMPLERS:
-            spacing, sde = DPM_SAMPLERS[sampler]
-            sched = DPMSolverSchedule(diffusion.base_alphas_cumprod, num_steps, keep=init_step, spacing=spacing, sde=sde)
+        if sampler in SOLVER_SAMPLERS:
+            sched = _solver_schedule(sampler, diffusion, num_steps, init_step)
             samples = sched.sample(self.model, shape, noise=noise, model_kwargs=kw, device=self.device,
                                    guidance_scale=guidance_scale, cond_first=self.cond_first,
-                                   sample_generators=self._generators(lo, hi) if sde else None, **blend)
+                                   sample_generators=self._generators(lo, hi) if sched.draws_noise else None, **blend)
         elif sampler in ("ddim_sampler", "plms_sampler"):  # kandinsky2_1_model.py:259-284: un-respaced schedule, eta 0
             cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
             samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, H, W), conditioning=kw, x_T=noise,
@@ -218,8 +228,9 @@ class Kandinsky2_1(_DecoderBase):
         sampler="dpmpp_2m_sampler" runs DPM-Solver++(2M) over `num_steps` evaluations of diffusion's base schedule; with
         init_step = s only the last s of them run (img2img), starting from `noise`.  "dpmpp_2m_karras_sampler" places the
         evaluations with Karras sigma spacing, "dpmpp_2m_sde_sampler" / "dpmpp_2m_sde_karras_sampler" run the SDE variant
-        (fresh noise every step, drawn per global sample index like p_sampler's).  Inpainting: the known region replaces x0
-        inside the step (p_sampler and the dpmpp_2m samplers; the reference's DDIM / PLMS paths have no such blend)."""
+        (fresh noise every step, drawn per global sample index like p_sampler's).  "unipc_sampler" / "unipc_karras_sampler" run
+        UniPC (DPM-Solver++(2M) plus the UniC corrector, UniPCSchedule) over the same evaluations.  Inpainting: the known region
+        replaces x0 inside the step (p_sampler and the solver samplers; the reference's DDIM / PLMS paths have no such blend)."""
         _check_sampler(sampler, SAMPLERS_21)
         full_emb, pooled_emb = self.embedder.text_emb(prompt, batch_size)
         cond = {"full_emb": full_emb.to(self.device), "pooled_emb": pooled_emb.to(self.device),
@@ -267,12 +278,12 @@ class Kandinsky2_1(_DecoderBase):
     def generate_img2img(self, prompt, pil_img, strength=0.7, num_steps=100, batch_size=1, guidance_scale=7, h=512,
                          w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25"):
         """kandinsky2_1_model.py:428-484: encode the image, noise it to step int(T*(1-strength)) and run the remaining steps.
-        With a dpmpp_2m sampler the last int(num_steps*strength) solver evaluations run (at least 1), from the image
+        With a dpmpp_2m or unipc sampler the last int(num_steps*strength) solver evaluations run (at least 1), from the image
         noised to the first of them."""
         _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        if sampler in DPM_SAMPLERS:
+        if sampler in SOLVER_SAMPLERS:
             x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength, sampler)
         else:
             start_step = int(diffusion.num_timesteps * (1 - strength))
@@ -317,8 +328,8 @@ class Kandinsky2_2(_DecoderBase):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
         106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
         sampler="dpmpp_2m_sampler" (or its Karras / SDE variants, DPM_SAMPLERS): DPM-Solver++(2M) over `steps` evaluations of
-        the same base schedule instead (init_step =
-        the number of evaluations kept for img2img); inpainting re-noises the known region to the next timestep."""
+        the same base schedule instead, "unipc_sampler" / "unipc_karras_sampler" UniPC (init_step = the number of evaluations
+        kept for img2img); inpainting re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}
         return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, create_ddpm_v22(steps), steps, guidance,
@@ -355,7 +366,7 @@ class Kandinsky2_2(_DecoderBase):
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
-        if sampler in DPM_SAMPLERS:
+        if sampler in SOLVER_SAMPLERS:
             x, start = self._dpm_img2img_start(lat, diffusion, decoder_steps, strength, sampler)
         else:
             # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first

@@ -1,17 +1,20 @@
-"""Cost of the DPM-Solver++(2M) samplers (ODE and SDE, linspace and Karras spacing) against the default DDPM one at the cfg-2
-geometry (Kandinsky 2.2 decoder, 768x768, 4 images, guidance 4, the full-size UNet with random weights of the architecture).
+"""Cost of the DPM-Solver++(2M) samplers (ODE and SDE, linspace and Karras spacing) and of UniPC against the default DDPM one at
+the cfg-2 geometry (Kandinsky 2.2 decoder, 768x768, 4 images, guidance 4, the full-size UNet with random weights of the architecture).
 
 Measures, in one process on cuda:0, and prints one JSON line (also written to --out if given):
   * whole-call images/s through Kandinsky2_2.generate_text2img (latent init, the denoising steps, MoVQ decode, uint8 + PIL) for
     sampler="ddpm_sampler" x 50 steps, "dpmpp_2m_sampler" x 20 and x 25, "dpmpp_2m_sde_sampler" x 20 and
-    "dpmpp_2m_karras_sampler" x 20: CUDA events, median of --calls steady-state calls after one warm-up call per arm;
-  * graph-replayed steps/s of each step kind (k2_step_begin + UNet + k2_sampler_step, k2_dpm_solver_step or
-    k2_dpm_solver_sde_step + k2_step_end, one graph launch per step), the three arms alternated --rounds times in this process;
-  * device time of one k2_dpm_solver_step, k2_dpm_solver_sde_step and k2_sampler_step launch (threshold mode 0, as the 2.2
-    step issues it) at this geometry: CUDA events over --kernel-reps back-to-back launches.
+    "dpmpp_2m_karras_sampler" x 20, "unipc_sampler" x 10, 15 and 20: CUDA events, median of --calls steady-state calls after
+    one warm-up call per arm;
+  * graph-replayed steps/s of each step kind (k2_step_begin + UNet + k2_sampler_step, k2_dpm_solver_step,
+    k2_dpm_solver_sde_step or k2_unipc_step + k2_step_end, one graph launch per step), the arms alternated --rounds times in
+    this process;
+  * device time of one k2_dpm_solver_step, k2_dpm_solver_sde_step, k2_unipc_step and k2_sampler_step launch (threshold mode 0,
+    as the 2.2 step issues it) at this geometry: CUDA events over --kernel-reps back-to-back launches.
+--arms unipc keeps only the UniPC arms and DPM++(2M), its baseline (dpmpp_2m_sampler x 20 for the whole call).
 The card's name, power limit and maximum SM clock are read in the same run (nvidia-smi query only).  Needs a CUDA sm_90 device.
 
-    python profiles/sampler_steps.py [--out /tmp/sampler_steps.json]
+    python profiles/sampler_steps.py [--arms all|unipc] [--out /tmp/sampler_steps.json]
 """
 import argparse
 import json
@@ -51,6 +54,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--calls", type=int, default=3)
     ap.add_argument("--kernel-reps", type=int, default=2000)
+    ap.add_argument("--arms", default="all", choices=["all", "unipc"])
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -58,7 +62,7 @@ def main():
     from bench import _init_pipe_with_model, build_unet
     from kandinsky2 import ops
     from kandinsky2.configs import CONFIG_2_2
-    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, FusedStep, create_ddpm_v22
+    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, FusedStep, UniPCSchedule, create_ddpm_v22
     from kandinsky2.pipelines import Kandinsky2_2
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
@@ -73,11 +77,15 @@ def main():
     ddpm = create_ddpm_v22(50)
     dpm = DPMSolverSchedule(ddpm.base_alphas_cumprod, 20)
     sde = DPMSolverSchedule(ddpm.base_alphas_cumprod, 20, sde=True)
+    unipc = UniPCSchedule(ddpm.base_alphas_cumprod, 20)
+    only = None if args.arms == "all" else ("dpmpp_2m", "unipc")
     x_start = torch.randn(B, 4, H, W, device=dev, generator=g)
     noise = torch.randn(50, B, 4, H, W, device=dev, generator=g)
     arms = {}
     for name, sched, kind, nseq in (("ddpm_sampler", ddpm, "ddpm", noise), ("dpmpp_2m_sampler", dpm, "dpmpp_2m", None),
-                                    ("dpmpp_2m_sde_sampler", sde, "dpmpp_2m_sde", noise[:20])):
+                                    ("dpmpp_2m_sde_sampler", sde, "dpmpp_2m_sde", noise[:20]), ("unipc_sampler", unipc, "unipc", None)):
+        if only and kind not in only:
+            continue
         coef, ts = sched._tables(dev)
         order = torch.arange(sched.num_timesteps - 1, -1, -1, device=dev)
         step = FusedStep(model, B, H, W, dict(image_emb=image_emb), guidance_scale=4.0, cond_first=False, clip_range=2.0,
@@ -95,21 +103,27 @@ def main():
             sps[name].append(round(1e3 * args.steps / ms, 3))
     res["steps_per_s"] = sps
     res["steps_per_s_note"] = (f"{args.steps} graph replays per run after {args.warmup} warm-up replays, arms alternated "
-                               f"{args.rounds} times; the DPM++ schedules wrap around their 20 rows")
+                               f"{args.rounds} times; the DPM++ and UniPC schedules wrap around their 20 rows")
 
     # ---- step-kernel device time
     mo = torch.randn(2 * B, 8, H, W, device=dev, generator=g)
     xk = torch.randn(B, 4, H, W, device=dev, generator=g)
     hist = torch.randn(B, 4, H, W, device=dev, generator=g)
+    last, hist2 = torch.randn(B, 4, H, W, device=dev, generator=g), torch.randn(B, 4, H, W, device=dev, generator=g)
     nz = torch.randn(B, 4, H, W, device=dev, generator=g)
     work = torch.empty(B * 4 * H * W + 4096, device=dev)
     coef_ddpm = ddpm._tables(dev)[0][25].clone()
     coef_dpm = dpm._tables(dev)[0][10].clone()
     coef_sde = sde._tables(dev)[0][10].clone()
+    coef_unipc = unipc._tables(dev)[0][10].clone()
     assert float(coef_dpm[4]) != 0.0 and float(coef_sde[4]) != 0.0 and float(coef_sde[7]) != 0.0  # history and noise are read
+    assert all(float(coef_unipc[i]) != 0.0 for i in (3, 5, 6, 9))                                 # last, D_{k-1}, D_{k-2} too
     kern = {"k2_sampler_step": lambda: ops.sampler_step(mo, xk, nz, coef_ddpm, 4.0, False, 2.0, 0, work=work),
             "k2_dpm_solver_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_dpm, 4.0, False),
-            "k2_dpm_solver_sde_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_sde, 4.0, False, noise=nz)}
+            "k2_dpm_solver_sde_step": lambda: ops.dpm_solver_step(mo, xk, hist, coef_sde, 4.0, False, noise=nz),
+            "k2_unipc_step": lambda: ops.unipc_step(mo, xk, last, hist, hist2, coef_unipc, 4.0, False)}
+    if only:
+        kern = {k: v for k, v in kern.items() if k in ("k2_dpm_solver_step", "k2_unipc_step")}
     kt = {}
     for name, fn in kern.items():
         fn()
@@ -119,10 +133,11 @@ def main():
     n = B * 4 * H * W
     # fp32 words moved per latent element: DDPM reads cond + uncond eps, the variance, x (twice: one per kernel), the noise,
     # writes and re-reads x0 through a scratch buffer and writes x = 9; DPM++ reads cond + uncond eps, x and hist and writes
-    # x and hist = 6; the SDE step also reads the noise = 7
-    kt["k2_sampler_step"]["bytes"] = 4 * n * 9
-    kt["k2_dpm_solver_step"]["bytes"] = 4 * n * 6
-    kt["k2_dpm_solver_sde_step"]["bytes"] = 4 * n * 7
+    # x and hist = 6; the SDE step also reads the noise = 7; UniPC reads cond + uncond eps, x, last, D_{k-1} and D_{k-2} and writes
+    # x, last and both history slots = 10
+    words = {"k2_sampler_step": 9, "k2_dpm_solver_step": 6, "k2_dpm_solver_sde_step": 7, "k2_unipc_step": 10}
+    for name in kt:
+        kt[name]["bytes"] = 4 * n * words[name]
     for v in kt.values():
         v["achieved_GBps"] = round(v["bytes"] / (v["us_per_launch"] * 1e-6) / 1e9, 1)
     res["step_kernel"] = kt
@@ -134,8 +149,11 @@ def main():
     pipe = Kandinsky2_2.__new__(Kandinsky2_2)
     _init_pipe_with_model(pipe, CONFIG_2_2, dev, model)
     calls = {}
-    for sampler, steps in (("ddpm_sampler", 50), ("dpmpp_2m_sampler", 20), ("dpmpp_2m_sampler", 25), ("dpmpp_2m_sde_sampler", 20),
-                           ("dpmpp_2m_karras_sampler", 20)):
+    call_arms = (("ddpm_sampler", 50), ("dpmpp_2m_sampler", 20), ("dpmpp_2m_sampler", 25), ("dpmpp_2m_sde_sampler", 20),
+                 ("dpmpp_2m_karras_sampler", 20), ("unipc_sampler", 10), ("unipc_sampler", 15), ("unipc_sampler", 20))
+    if only:
+        call_arms = (("dpmpp_2m_sampler", 20), ("unipc_sampler", 10), ("unipc_sampler", 15), ("unipc_sampler", 20))
+    for sampler, steps in call_arms:
         ms_all = []
         for it in range(args.calls + 1):   # call 0 builds plans / graphs
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
