@@ -317,11 +317,12 @@ int k2_transpose_f16(const void* x, int ldx, void* y, int B, int T, int C, k2_st
 /* ---------------------------------------------------------------------------------------------
  * Diffusion prior (SURVEY.md 8f rank 3; kandinsky2/model/prior.py:46-127), not on the measured denoising path and not
  * tuned.  The transformer's Linear layers are k2_conv_gemm flat-row GEMMs; these are the rest:
- *   k2_layernorm_f16   LayerNorm over the last dim of fp16 rows, fp32 statistics / gain / bias (prior.py:46-53)
+ *   k2_layernorm_f16   LayerNorm over the last dim of fp16 rows, float64 statistics, fp32 gain / bias (prior.py:46-53)
  *   k2_gelu_f16        nn.GELU (exact erf) on n fp16 elements, may run in place (prior.py:74-83)
  *   k2_attention_small QKVMultiheadAttention for T <= 128 tokens, head dim 64 (prior.py:86-103): qkv rows
  *                      [B, T, >= heads*192] with per-head [q | k | v]; additive mask = causal (if set) AND key keep-mask
- *                      (uint8 [B, T], may be NULL); fp32 softmax; out rows [B, T, >= heads*64].
+ *                      (uint8 [B, T], nonzero = kept, may be NULL); fp32 softmax; out rows [B, T, >= heads*64].  A query
+ *                      row that reaches no key is NaN, like torch's softmax over an all -inf row.
  * ------------------------------------------------------------------------------------------- */
 int k2_layernorm_f16(const void* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int M, int N, float eps,
                      k2_stream_t stream);

@@ -2,8 +2,17 @@
 // on top of the GEMM (k2_conv_gemm as a flat-row GEMM): LayerNorm on fp16 rows, exact GELU, and a masked multi-head
 // attention over a SHORT sequence (81 tokens, head dim 64).
 //
-// Parity: tests/test_gpu_zz_prior.py (each kernel against torch fp32, the whole prior against tests/golden/prior_tiny.pt = the
-// reference's own classes).  Nothing on the measured denoising path calls these entry points; they are not tuned.
+// Parity: tests/test_gpu_prior_kernels.py checks each kernel against float64 of the same fp16 inputs, bounds in fp16 ulps
+// of the float64 value.  Measured on an H100 (400 W):
+//   attention_small  T = 1..128 across every 32-key chunk edge, 1 / 3 / 32 heads, B = 1 / 2 / 8, causal and CLIP prefix or
+//                    holed keep masks, scores of +-60, strided views: within 1 ulp plus the first-order fp32 error of the
+//                    scores and weights; the largest error is 0.46 of that bound (the fp16 output rounding).
+//   layernorm_f16    N = 1..2049, rows offset by up to 1000 std, constant rows (exactly fp16(beta)), a 3e4 channel, variance
+//                    below eps: within 1 ulp plus 2^-20 (|gamma x_hat| + |beta|); worst 1.34 ulp, on outputs that cancel.
+//   gelu_f16         all 65536 fp16 inputs: within 1 ulp of 0.5 x erfc(-x / sqrt 2); worst 0.50 ulp (all correctly rounded).
+// tests/test_gpu_zz_prior.py pins the whole prior to tests/golden/prior_tiny.pt (the reference's own classes), and
+// tests/test_gpu_zz_prior_full.py runs the full 2.1 prior against the fp32 oracle.  Nothing on the measured denoising path
+// calls these entry points; they are not tuned.
 #include <math.h>
 
 #include "../../include/k2b200.h"
@@ -13,58 +22,64 @@
 namespace k2 {
 namespace {
 
-// LayerNorm over the last dimension of fp16 rows, fp32 statistics and affine (prior.py:46-53: "supports fp16 inputs but
-// fp32 gains/biases"), fp16 out.  One block per row.
+// Sum over the 256 threads of a block in a fixed order; every thread gets the total.
+__device__ __forceinline__ double block_sum_256(double v, double* sred) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = 0.0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) v += sred[w];
+  __syncthreads();  // sred is reused by the next call
+  return v;
+}
+
+// LayerNorm over the last dimension of fp16 rows, fp32 gain / bias (prior.py:46-53: "supports fp16 inputs but fp32
+// gains/biases"), fp16 out.  One block per row.  The statistics are two passes in double: a sum of up to 8192 fp16 values
+// is exact in double (2^-24 .. 2^16 spans 40 bits), so the mean is correctly rounded, and the variance is the centred sum
+// of squares.  A
+// one-pass q/N - mean^2 in fp32 cancels once |mean| >> std: it misses the one-ulp bound on rows offset by 100 std or more,
+// and on rows whose variance is below eps.  The row is at most a few KB and the second and third passes read it from L1.
 __global__ void __launch_bounds__(256) layernorm_f16_kernel(const __half* __restrict__ x, int ldx,
                                                             const float* __restrict__ g, const float* __restrict__ b,
                                                             __half* __restrict__ y, int ldy, int N, float eps) {
-  __shared__ float sred[2][8];
+  __shared__ double sred[8];
   const __half* xr = x + static_cast<long long>(blockIdx.x) * ldx;
-  float s = 0.f, q = 0.f;
+  double s = 0.0;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) s += static_cast<double>(__half2float(xr[i]));
+  const double mean = block_sum_256(s, sred) / N;
+  double q = 0.0;
   for (int i = threadIdx.x; i < N; i += blockDim.x) {
-    const float v = __half2float(xr[i]);
-    s += v;
-    q = fmaf(v, v, q);
+    const double d = static_cast<double>(__half2float(xr[i])) - mean;
+    q = fma(d, d, q);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s += __shfl_xor_sync(0xffffffffu, s, o);
-    q += __shfl_xor_sync(0xffffffffu, q, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    sred[0][threadIdx.x >> 5] = s;
-    sred[1][threadIdx.x >> 5] = q;
-  }
-  __syncthreads();
-  s = 0.f;
-  q = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) {  // fixed order
-    s += sred[0][w];
-    q += sred[1][w];
-  }
-  const float mean = s / N;
-  const float var = fmaxf(q / N - mean * mean, 0.f);
-  const float rstd = rsqrtf(var + eps);
+  const double rstd = 1.0 / sqrt(block_sum_256(q, sred) / N + static_cast<double>(eps));
   __half* yr = y + static_cast<long long>(blockIdx.x) * ldy;
-  for (int i = threadIdx.x; i < N; i += blockDim.x)
-    yr[i] = __float2half_rn((__half2float(xr[i]) - mean) * rstd * g[i] + b[i]);
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const float xh = static_cast<float>((static_cast<double>(__half2float(xr[i])) - mean) * rstd);
+    yr[i] = __float2half_rn(fmaf(xh, g[i], b[i]));
+  }
 }
 
-// nn.GELU() (exact, erf) on fp16, in place or out of place (prior.py:74-83)
+// nn.GELU() (exact, erf) on fp16, in place or out of place (prior.py:74-83), as 0.5 x erfc(-x / sqrt 2).  torch's
+// 0.5 x (1 + erf(x / sqrt 2)) cancels for x < -3 (1 + erf is the difference of two numbers near 1) and misses by up to 2.2
+// fp16 ulps there on an H100; erfc keeps its relative accuracy, and every fp16 input comes out within one ulp of the float64
+// value.  +-inf and NaN map as in torch's fp32 GELU: +inf, NaN (-inf * 0), NaN.
 __global__ void __launch_bounds__(256) gelu_f16_kernel(const __half2* __restrict__ x, __half2* __restrict__ y, long long n2) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n2;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float2 v = __half22float2(x[i]);
-    const float a = 0.5f * v.x * (1.f + erff(v.x * 0.70710678118654752f));
-    const float c = 0.5f * v.y * (1.f + erff(v.y * 0.70710678118654752f));
+    const float a = 0.5f * v.x * erfcf(v.x * -0.70710678118654752f);
+    const float c = 0.5f * v.y * erfcf(v.y * -0.70710678118654752f);
     y[i] = __floats2half2_rn(a, c);
   }
 }
 
 // QKVMultiheadAttention (prior.py:86-103) for a short sequence: qkv rows [B, T, heads*192] with per-head [q | k | v]
 // (64 each), additive mask = causal AND key-padding (prior.py:251-252: where(mask, 0, -inf)[:, None, :] + triu(-inf, 1)),
-// softmax in fp32, out [B, T, heads*64].  One block per (batch, head); K and V of the head in shared memory (rows padded
+// softmax in fp32, out [B, T, heads*64].  A query row with no reachable key has sum = 0 and comes out 0 * inf = NaN, as
+// torch's softmax of an all -inf row does; that is the contract, not an accident.  One block per (batch, head); K and V of the head in shared memory (rows padded
 // to 66 halfs against bank conflicts), one warp per query row, lanes over keys for the scores and over channels for PV.
 constexpr int SA_MAXT = 128;
 constexpr int SA_PITCH = 66;

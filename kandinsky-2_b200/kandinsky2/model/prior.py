@@ -2,8 +2,12 @@
 
 Parity: tests/test_gpu_zz_prior.py compares the transformer forward and the guided x0-prediction sampling loop with the
 outputs of the reference's own PriorTransformer / PriorDiffusionModel classes (tests/golden/prior_tiny.pt; the oracle,
-oracle/prior_oracle.py, reproduces them exactly).  Not yet wired into the pipelines (they take synthetic / user-supplied
-image embeddings) and not benchmarked.
+oracle/prior_oracle.py, reproduces them exactly).  tests/test_gpu_zz_prior_full.py runs the full 2.1 prior (20 layers,
+width 2048, 32 heads, 81 tokens) on synthetic weights against the fp32 oracle; on an H100 (400 W), at B = 1 / 4, the forward
+deviates by rel-L2 1.38e-3 / 1.31e-3 and max-abs 4.5e-3 / 5.6e-3, less than the reference's own fp16 mode does (1.67e-3 /
+1.53e-3, 5.3e-3 / 5.7e-3), the fp16 residual stream stays finite (peak |h| 26), and 25-step guided sampling deviates by
+rel-L2 1.7e-3.  tests/test_gpu_prior_kernels.py bounds
+the three kernels against float64.  Not benchmarked.
 
 `PriorTransformer` keeps the reference's parameter names (prior.py:191-228), so `prior_fp16.ckpt` state dicts load as they
 are.  Compute: the Linear layers are flat-row wgmma GEMMs (`ops.gemm_rows`, fp16 storage / fp32 accumulate, bias and

@@ -583,11 +583,19 @@ def gelu_f16_(x):
 
 
 def attention_small(qkv, heads, keep_mask=None, causal=True, scale=0.125, out=None):
-    """qkv fp16 [B, T, heads*192] (per head [q|k|v]), keep_mask uint8 [B, T] or None -> fp16 [B, T, heads*64]; T <= 128."""
-    lib = nat.load()
+    """qkv fp16 [B, T, heads*192] (per head [q|k|v]), keep_mask uint8 or bool [B, T] (nonzero = key kept) or None -> fp16
+    [B, T, heads*64]; T <= 128.  A query row that can reach no key (every key masked, or causal with key 0 masked) is NaN,
+    as torch's softmax over an all -inf row is."""
     B, T = qkv.shape[:2]
+    assert qkv.dtype == torch.float16 and qkv.dim() == 3 and qkv.shape[2] == heads * 192, (qkv.dtype, qkv.shape, heads)
+    if keep_mask is not None:
+        assert keep_mask.dtype in (torch.uint8, torch.bool), keep_mask.dtype
+        assert tuple(keep_mask.shape) == (B, T) and keep_mask.is_contiguous(), (keep_mask.shape, keep_mask.stride(), B, T)
+        assert keep_mask.device == qkv.device, (keep_mask.device, qkv.device)
+    lib = nat.load()
     if out is None:
         out = torch.empty((B, T, heads * 64), dtype=torch.float16, device=qkv.device)
+    assert out.dtype == torch.float16 and tuple(out.shape) == (B, T, heads * 64), (out.dtype, out.shape)
     check(lib.k2_attention_small(ptr(qkv), _row_stride(qkv), ptr(keep_mask), int(causal), ptr(out), _row_stride(out), B, T,
                                  heads, scale, stream_ptr()))
     return out

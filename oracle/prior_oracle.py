@@ -44,43 +44,51 @@ def prior_param_spec(cfg):
 
 def _timestep_embedding(t, dim, max_period=10000):  # prior.py:15-35 (cos first, like model/nn.py)
     half = dim // 2
-    freqs = torch.exp(-math.log(max_period) * torch.arange(half, dtype=torch.float32) / half)
+    freqs = torch.exp(-math.log(max_period) * torch.arange(half, dtype=torch.float32, device=t.device) / half)
     args = t[:, None].float() * freqs[None]
     return torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
 
 
-def prior_forward(sd, cfg, x, timesteps, text_emb, text_enc, mask):
+def prior_forward(sd, cfg, x, timesteps, text_emb, text_enc, mask, fp16=False):
     """x [N, clip_dim] noisy image embedding, text_emb [N, clip_dim], text_enc [N, text_ctx, clip_xf_width], mask [N, text_ctx]
-    bool (True = real token) -> predicted x0 [N, clip_dim] (the last position of the causal transformer)."""
+    bool (True = real token) -> predicted x0 [N, clip_dim] (the last position of the causal transformer).  Runs on the
+    device of the inputs.
+
+    fp16=True: the reference's fp16 mode (Kandinsky2_1.__init__ calls prior.half() under use_fp16): sd holds fp16 tensors,
+    every Linear and einsum is fp16, LayerNorm computes in fp32 and returns fp16 (prior.py:48-54 on a CUDA fp16 tensor),
+    the fp32 additive mask promotes the scores to fp32 for the softmax, whose result is cast back to fp16 (prior.py:102)."""
     W, H = cfg["xf_width"], cfg["xf_heads"]
     N = x.shape[0]
+    dt = torch.float16 if fp16 else torch.float32
+    x, text_emb, text_enc = x.to(dt), text_emb.to(dt), text_enc.to(dt)
     lin = lambda name, v: F.linear(v, sd[name + ".weight"], sd[name + ".bias"])  # noqa: E731
+    ln = lambda v, name: F.layer_norm(v.float(), (W,), sd[name + ".weight"].float(), sd[name + ".bias"].float()).to(dt)  # noqa: E731
     mask = F.pad(mask, (0, 4), value=True)                                       # ext_len = 4 extra positions
-    t_emb = lin("time_embed.2", F.silu(lin("time_embed.0", _timestep_embedding(timesteps, W))))
+    t_emb = lin("time_embed.2", F.silu(lin("time_embed.0", _timestep_embedding(timesteps, W).to(dt))))
     seq = torch.cat([lin("text_enc_proj", text_enc), lin("text_emb_proj", text_emb)[:, None], t_emb[:, None],
                      lin("clip_img_proj", x)[:, None], sd["prd_emb"].expand(N, -1, -1)], dim=1)
     seq = seq + sd["positional_embedding"]
     if cfg["xf_padding"]:
         seq = torch.where(mask[..., None], seq, sd["padding_embedding"][None])
     n = seq.shape[1]
-    causal = torch.full((n, n), float("-inf")).triu_(1)
-    add = torch.where(mask, 0.0, float("-inf"))[:, None, :] + causal[None]       # [N, n, n]
+    causal = torch.full((n, n), float("-inf"), device=seq.device).triu_(1)
+    add = torch.where(mask, 0.0, float("-inf"))[:, None, :] + causal[None]       # [N, n, n] fp32
     d = W // H
     scale = 1 / math.sqrt(math.sqrt(d))
     h = seq
     for i in range(cfg["xf_layers"]):
         p = f"transformer.resblocks.{i}."
-        y = F.layer_norm(h, (W,), sd[p + "ln_1.weight"], sd[p + "ln_1.bias"])
+        y = ln(h, p + "ln_1")
         qkv = lin(p + "attn.c_qkv", y).view(N, n, H, 3 * d)                      # per head [q | k | v]  (prior.py:92-95)
         q, k, v = torch.split(qkv, d, dim=-1)
         w = torch.einsum("bthc,bshc->bhts", q * scale, k * scale) + add[:, None]
-        a = torch.einsum("bhts,bshc->bthc", torch.softmax(w, dim=-1), v).reshape(N, n, W)
+        a = torch.einsum("bhts,bshc->bthc", torch.softmax(w, dim=-1).to(dt), v).reshape(N, n, W)
         h = h + lin(p + "attn.c_proj", a)
-        y = F.layer_norm(h, (W,), sd[p + "ln_2.weight"], sd[p + "ln_2.bias"])
+        y = ln(h, p + "ln_2")
         h = h + lin(p + "mlp.c_proj", F.gelu(lin(p + "mlp.c_fc", y)))
     if cfg["xf_final_ln"]:
-        h = F.layer_norm(h, (W,), sd["final_ln.weight"], sd["final_ln.bias"])
-    return lin("out_proj", h[:, -1])
+        h = ln(h, "final_ln")
+    return lin("out_proj", h[:, -1]).float()
 
 
 def cosine_betas(steps=1000, max_beta=0.999):
@@ -109,7 +117,7 @@ def prior_sample(model_fn, x_T, step_noise, use_steps, guidance, clip_mean, clip
     B = x_T.shape[0]
     x = x_T
     for n, i in enumerate(range(len(use_steps))[::-1]):
-        t = torch.full((2 * B,), float(use_steps[i]))      # _WrappedModel: timestep_map[i], rescale_timesteps False
+        t = torch.full((2 * B,), float(use_steps[i]), device=x.device)  # _WrappedModel: timestep_map[i], no rescaling
         out = model_fn(torch.cat([x, x]), t)
         cond, uncond = out[:B], out[B:]
         x0 = (uncond + guidance * (cond - uncond)).clamp(-10, 10)

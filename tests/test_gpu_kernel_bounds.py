@@ -229,8 +229,8 @@ def test_silu_gelu_f16_in_place_bounds():
     from kandinsky2 import ops
     x = torch.cat([_rand(998, scale=4.0, seed=8), torch.tensor([-65504.0, 65504.0], device="cuda").half()])
     # one fp16 rounding (half an ulp = 2^-11 relative) of an fp32 evaluation.  SiLU is 0.5 x (1 + tanh.approx(x / 2)) (the
-    # UNet's activation, k2_common.cuh): tanh.approx's ~2^-11 error scaled by 0.5 |x|.  GELU is exact-erf fp32: its
-    # 1 + erf(x / sqrt 2) cancels for x < -3, leaving ~1e-7 absolute error on values of ~1e-6.
+    # UNet's activation, k2_common.cuh): tanh.approx's ~2^-11 error scaled by 0.5 |x|.  GELU is 0.5 x erfc(-x / sqrt 2) in
+    # fp32 (tests/test_gpu_prior_kernels.py bounds it by one ulp over every fp16 input).
     xd = x.double()
     for name, fn, ref, tol in (("silu", ops.silu_f16_, xd * torch.sigmoid(xd), 2 ** -10 * xd.abs() + 6e-8),
                                ("gelu", ops.gelu_f16_, F.gelu(xd), torch.full_like(xd, 5e-7))):
