@@ -203,6 +203,9 @@ int k2_stem_im2col(const float* x, int Cx, const float* x2, int C2, const float*
  *   model_out fp32 NCHW [2B, 8, H, W]; x fp32 [B, 4, H, W] (in place -> x_{t-1}); noise fp32 [B,4,H,W].
  *   coef (device, fp32[8]): sqrt_recip_ac, sqrt_recipm1_ac, post_coef1, post_coef2, min_log, max_log,
  *   nonzero, sqrt(alphas_cumprod[next timestep]) (2.2 inpainting only).  cond_first: 1 = rows [0,B) conditional (2.1), 0 = unconditional first (2.2).
+ *   noise is not read when nonzero == 0 (the last step), so its contents (even NaN) cannot reach the result.
+ *   The Kandinsky 2.2 prior's UnCLIP step runs here too (kandinsky2/model/prior.py: UnCLIPSchedule): H = 1, W = 320, the
+ *   prediction in channels 0-3 and zeros in 4-7, rows {0, -1, c_x0, c_x, log var, log var, t > 0, 0}, clip 10.
  *   threshold_mode 0: x0 = clamp(x0, -clip, clip); 1: additionally the reference's dynamic threshold
  *   s = max(percentile_99.5(|x0[sample 0]|), 1); x0 = clip(x0, -s, s)/s   (gaussian_diffusion.py:284-294).
  *   Split step for sharded runs (the reference's "sample 0" is GLOBAL sample 0): 2 = x0 + percentile of local sample 0 -> s in
@@ -316,7 +319,7 @@ int k2_transpose_f16(const void* x, int ldx, void* y, int B, int T, int C, k2_st
 
 /* ---------------------------------------------------------------------------------------------
  * Diffusion prior (SURVEY.md 8f rank 3; kandinsky2/model/prior.py:46-127), not on the measured denoising path and not
- * tuned.  The transformer's Linear layers are k2_conv_gemm flat-row GEMMs; these are the rest:
+ * tuned (the Kandinsky 2.2 prior replays its step as one CUDA graph: kandinsky2/model/prior.py _PriorStepPlan).  The transformer's Linear layers are k2_conv_gemm flat-row GEMMs; these are the rest:
  *   k2_layernorm_f16   LayerNorm over the last dim of fp16 rows, float64 statistics, fp32 gain / bias (prior.py:46-53)
  *   k2_gelu_f16        nn.GELU (exact erf) on n fp16 elements, may run in place (prior.py:74-83)
  *   k2_attention_small QKVMultiheadAttention for T <= 128 tokens, head dim 64 (prior.py:86-103): qkv rows
@@ -329,6 +332,15 @@ int k2_layernorm_f16(const void* x, int ldx, const float* gamma, const float* be
 int k2_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream);
 int k2_attention_small(const void* qkv, int ldq, const unsigned char* keep_mask, int causal, void* out, int ldo, int B, int T,
                        int heads, float scale, k2_stream_t stream);
+/* Token rows of the prior's sequence, bit-identical to the eager forward's `seq[:, j] = v.half()` followed by the fp16
+ * `seq + positional_embedding.half()`:
+ *   y[m, c] = fp16_rn( float(fp16_rn(x[m * ldx + c])) + float(pos[m * ldp + c]) )      m < M, c < N
+ * x fp32, pos and y fp16; ldx = 0 / ldp = 0 repeat one source / positional row for every m.  Strides are in elements
+ * (ldx, ldp: 0 or >= N; ldy >= N); x 4-byte and pos / y 2-byte aligned.  Arguments are checked before any CUDA call. */
+int k2_prior_tokens(const float* x, int ldx, const void* pos, int ldp, void* y, int ldy, int M, int N, k2_stream_t stream);
+/* y[m, c] = float(x[m * ldx + c]), exact: fp16 rows (ldx >= N) -> fp32 rows (ldy >= N), the `.float()` in front of the prior's
+ * fp32 out_proj.  x 2-byte and y 4-byte aligned.  Arguments are checked before any CUDA call. */
+int k2_f16_to_f32(const void* x, int ldx, float* y, int ldy, int M, int N, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'

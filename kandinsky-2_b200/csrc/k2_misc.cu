@@ -363,7 +363,9 @@ __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p
   const float v = p.model_out[(static_cast<long long>(bc) * 8 + 4 + c) * p.HW + sp];
   const float frac = (v + 1.f) * 0.5f;
   const float logvar = frac * p.coef[5] + (1.f - frac) * p.coef[4];
-  float xp = mean + p.coef[6] * expf(0.5f * logvar) * p.noise[i];
+  // noise is not read at a step without noise (coef[6] = 0): whatever it holds, even NaN, cannot reach the result
+  float xp = mean;
+  if (p.coef[6] != 0.f) xp = mean + p.coef[6] * expf(0.5f * logvar) * p.noise[i];
   if (p.mask && p.rnoise) {
     // Kandinsky 2.2 (diffusers KandinskyV22InpaintPipeline): after the scheduler step the known region is replaced by the
     // clean latent noised to the NEXT timestep with the run's initial noise; coef[7] = sqrt(alphas_cumprod[t_next]), 1 at

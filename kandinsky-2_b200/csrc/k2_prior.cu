@@ -1,6 +1,8 @@
 // k2_prior.cu -- the three small kernels the diffusion prior (SURVEY.md 8f rank 3, kandinsky2/model/prior.py:46-127) needs
 // on top of the GEMM (k2_conv_gemm as a flat-row GEMM): LayerNorm on fp16 rows, exact GELU, and a masked multi-head
-// attention over a SHORT sequence (81 tokens, head dim 64).
+// attention over a SHORT sequence (81 tokens, head dim 64).  Two copies keep torch off the graph-replayed prior step
+// (PriorTransformer._step_plan): the token rows written into the sequence with their positional embedding, and the fp16 ->
+// fp32 widening in front of out_proj.  Both reproduce the eager forward's roundings bit for bit.
 //
 // Parity: tests/test_gpu_prior_kernels.py checks each kernel against float64 of the same fp16 inputs, bounds in fp16 ulps
 // of the float64 value.  Measured on an H100 (400 W):
@@ -152,6 +154,30 @@ __global__ void __launch_bounds__(256) attention_small_kernel(const __half* __re
   }
 }
 
+// Token rows of the prior's sequence, as the eager forward builds them (kandinsky2/model/prior.py PriorTransformer.forward):
+// the fp32 projection is rounded to fp16 (`v.half()`), then the fp16 positional row is added in fp32 and rounded again
+// (torch's fp16 `seq + pos.half()`).  Two roundings, both round-to-nearest-even, so the rows are bit-identical to the eager
+// forward's.  One block per row; ldx = 0 / ldp = 0 broadcast one source / positional row to every output row.
+__global__ void __launch_bounds__(256) prior_tokens_kernel(const float* __restrict__ x, long long ldx,
+                                                           const __half* __restrict__ pos, long long ldp,
+                                                           __half* __restrict__ y, long long ldy, int N) {
+  const float* xr = x + blockIdx.x * ldx;
+  const __half* pr = pos + blockIdx.x * ldp;
+  __half* yr = y + blockIdx.x * ldy;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) {
+    const float v = __half2float(__float2half_rn(xr[c]));
+    yr[c] = __float2half_rn(v + __half2float(pr[c]));
+  }
+}
+
+// Exact fp16 -> fp32 widening of strided rows (the eager forward's `.float()` in front of the fp32 out_proj).
+__global__ void __launch_bounds__(256) f16_to_f32_rows_kernel(const __half* __restrict__ x, long long ldx,
+                                                              float* __restrict__ y, long long ldy, int N) {
+  const __half* xr = x + blockIdx.x * ldx;
+  float* yr = y + blockIdx.x * ldy;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) yr[c] = __half2float(xr[c]);
+}
+
 }  // namespace
 }  // namespace k2
 
@@ -189,6 +215,30 @@ int k2_attention_small(const void* qkv, int ldq, const unsigned char* keep_mask,
   K2_REQUIRE(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) & 3) == 0, "attention_small: alignment");
   attention_small_kernel<<<B * heads, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half*>(qkv), ldq, keep_mask, causal, reinterpret_cast<__half*>(out), ldo, T, heads, scale);
+  K2_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int k2_prior_tokens(const float* x, int ldx, const void* pos, int ldp, void* y, int ldy, int M, int N, k2_stream_t stream) {
+  K2_REQUIRE(x && pos && y && M > 0 && N > 0, "prior_tokens: bad arguments");
+  K2_REQUIRE((ldx == 0 || ldx >= N) && (ldp == 0 || ldp >= N) && ldy >= N, "prior_tokens: row strides");
+  K2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 3) == 0 &&
+                 ((reinterpret_cast<uintptr_t>(pos) | reinterpret_cast<uintptr_t>(y)) & 1) == 0,
+             "prior_tokens: alignment");
+  prior_tokens_kernel<<<M, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, ldx, reinterpret_cast<const __half*>(pos), ldp, reinterpret_cast<__half*>(y), ldy, N);
+  K2_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int k2_f16_to_f32(const void* x, int ldx, float* y, int ldy, int M, int N, k2_stream_t stream) {
+  K2_REQUIRE(x && y && M > 0 && N > 0, "f16_to_f32: bad arguments");
+  K2_REQUIRE(ldx >= N && ldy >= N, "f16_to_f32: row strides");
+  K2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 1) == 0 && (reinterpret_cast<uintptr_t>(y) & 3) == 0, "f16_to_f32: alignment");
+  f16_to_f32_rows_kernel<<<M, 256, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const __half*>(x), ldx, y, ldy,
+                                                                          N);
   K2_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;

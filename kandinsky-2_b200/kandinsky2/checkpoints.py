@@ -9,6 +9,11 @@
   head-interleaved `qkv` (and `encoder_kv`) Conv1d.  `diffusers_unet_to_k2` renames and re-packs such a state dict into
   the key layout of `Text2ImUNet(cond_version="2.2")`; `k2_to_diffusers_unet` is its inverse.
 
+* Kandinsky 2.2 ships its prior as a diffusers `PriorTransformer` (`kandinsky-community/kandinsky-2-2-prior`, subfolder
+  `prior`): the 2.1 prior network with separate q / k / v.  `diffusers_prior_to_k2` renames and re-packs it into
+  `model.prior.PriorTransformer` names and returns clip_mean / clip_std beside it (tests/test_cpu_prior22.py pins it through the
+  network: the reference's forward on the remapped weights equals the diffusers-form forward).
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -184,7 +189,53 @@ def lora_to_k2(lora, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4
     return packed
 
 
-def k2_to_diffusers_unet(sd, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3,
+_PRIOR_TOP = {"time_embedding.linear_1": "time_embed.0", "time_embedding.linear_2": "time_embed.2", "proj_in": "clip_img_proj",
+              "embedding_proj": "text_emb_proj", "encoder_hidden_states_proj": "text_enc_proj", "norm_out": "final_ln",
+              "proj_to_clip_embeddings": "out_proj"}
+_PRIOR_BLOCK = {"norm1": "ln_1", "norm3": "ln_2", "attn1.to_out.0": "attn.c_proj", "ff.net.0.proj": "mlp.c_fc",
+                "ff.net.2": "mlp.c_proj"}
+
+
+def diffusers_prior_keys(layers):
+    """Every key of a diffusers Kandinsky 2.2 `PriorTransformer` state dict with `layers` transformer blocks."""
+    keys = ["positional_embedding", "prd_embedding", "clip_mean", "clip_std"]
+    keys += [f"{d}.{s}" for d in _PRIOR_TOP for s in ("weight", "bias")]
+    for i in range(layers):
+        keys += [f"transformer_blocks.{i}.{d}.{s}" for d in (*_PRIOR_BLOCK, "attn1.to_q", "attn1.to_k", "attn1.to_v")
+                 for s in ("weight", "bias")]
+    return keys
+
+
+def diffusers_prior_to_k2(sd, head_dim=64):
+    """diffusers `PriorTransformer` state dict (Kandinsky 2.2, `kandinsky-community/kandinsky-2-2-prior`, subfolder `prior`) ->
+    (state dict in `kandinsky2.model.prior.PriorTransformer` names, clip_mean [clip_dim], clip_std [clip_dim]).
+
+    The network is the 2.1 prior's (token order, causal attention, exact GELU, final LayerNorm); only the names differ, and
+    attn1.to_q / to_k / to_v become one c_qkv whose rows are interleaved per head [q_h | k_h | v_h] (pack_heads).  The
+    `causal_attention_mask` buffer is dropped: the attention kernel builds the causal mask itself.  Raises K2Error naming
+    the unknown and the missing keys.  Restated from diffusers' published layout (diffusers is not a dependency)."""
+    sd = {k: v for k, v in sd.items() if k != "causal_attention_mask"}
+    blocks = {int(m.group(1)) for m in (re.match(r"^transformer_blocks\.(\d+)\.", k) for k in sd) if m}
+    expected = diffusers_prior_keys(max(blocks) + 1 if blocks else 0)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"diffusers prior state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {"positional_embedding": sd["positional_embedding"], "prd_emb": sd["prd_embedding"]}
+    for d, k in _PRIOR_TOP.items():
+        for s in ("weight", "bias"):
+            out[f"{k}.{s}"] = sd[f"{d}.{s}"]
+    for i in sorted(blocks):
+        dp, kp = f"transformer_blocks.{i}.", f"transformer.resblocks.{i}."
+        for d, k in _PRIOR_BLOCK.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.c_qkv.{s}"] = pack_heads([sd[f"{dp}attn1.to_{n}.{s}"] for n in "qkv"], head_dim)
+    return out, sd["clip_mean"].reshape(-1), sd["clip_std"].reshape(-1)
+
+
+def k2_to_diffusers_unet(sd,in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3,
                          attention_ds=(2, 4, 8), head_dim=64):
     """Inverse of diffusers_unet_to_k2 (export, and the round-trip test)."""
     out = {k: v for k, v in sd.items() if k.startswith("add_embedding.input_hint_block.")}

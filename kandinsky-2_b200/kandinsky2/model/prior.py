@@ -14,6 +14,11 @@ are.  Compute: the Linear layers are flat-row wgmma GEMMs (`ops.gemm_rows`, fp16
 the residual add in the epilogue), LayerNorm / GELU / the masked 81-token attention are the small kernels of
 csrc/k2_prior.cu, the four single-row projections are `ops.linear`.  The residual stream is fp16 like the reference's
 (`Kandinsky2_1.__init__` halves the prior when `use_fp16`).
+
+Kandinsky 2.2 runs the same network at CLIP-bigG width (clip_dim = clip_xf_width = 1280) from a diffusers state dict
+(checkpoints.diffusers_prior_to_k2).  Its sampler is diffusers' UnCLIPScheduler (UnCLIPSchedule, restated), and each sampling
+step is one CUDA graph replay of _PriorStepPlan, whose model output equals `forward` bit for bit under the same GEMM
+configurations; PriorEmbedder22 puts it behind the embedder protocol (tests/test_gpu_zz_prior22.py, DESIGN.md section 7).
 """
 import math
 
@@ -23,6 +28,7 @@ import torch.nn as nn
 
 from .. import ops
 from .._native import K2Error
+from ..launch_plan import LaunchPlan
 
 
 class _Node(nn.Module):
@@ -77,6 +83,7 @@ class PriorTransformer(nn.Module):
         else:
             self.final_ln = None
         self._packed = None
+        self._step_plans = {}
 
     def finalize(self):
         """Pack the GEMM weights (fp16 [N, K], K padded to 64) once per checkpoint."""
@@ -86,7 +93,16 @@ class PriorTransformer(nn.Module):
                 pk[(i, name)] = (ops.pack_conv_weight(m.weight), m.bias.float().contiguous())
         pk["text_enc"] = (ops.pack_conv_weight(self.text_enc_proj.weight), self.text_enc_proj.bias.float().contiguous())
         self._packed = pk
+        self._step_plans = {}
         return self
+
+    def _step_plan(self, B):
+        """The UnCLIP sampling step at B samples (2B CFG rows) as a static launch list (_PriorStepPlan), built once per B."""
+        if self._packed is None:
+            self.finalize()
+        if B not in self._step_plans:
+            self._step_plans[B] = _PriorStepPlan(self, B)
+        return self._step_plans[B]
 
     @torch.no_grad()
     def forward(self, x, timesteps, text_emb=None, text_enc=None, mask=None, causal_mask=None):
@@ -236,3 +252,272 @@ def _space_timesteps(num_timesteps, count):
         out.add(round(cur))
         cur += stride
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# Kandinsky 2.2 prior: diffusers' UnCLIPScheduler, the graph-replayed sampling step, and the embedder
+# ------------------------------------------------------------------------------------------------------------------------------
+class UnCLIPSchedule:
+    """diffusers' `UnCLIPScheduler` as `kandinsky-2-2-prior` configures it (1000 training steps, squaredcos_cap_v2,
+    prediction_type="sample", variance_type="fixed_small_log", clip_sample at +-10), restated (diffusers is not a dependency).
+
+    Timesteps for N >= 2 steps: (arange(N) * 999 / (N - 1)).round() in descending order (999, 957, ..., 0 for N = 25).  Step k
+    at t with t' = the next timestep (t - 1 after the last), a = acp[t], a' = acp[t'] (1 if t' < 0), beta = betas[t] if
+    t' = t - 1 else 1 - a / a', alpha = 1 - beta:
+        x' = (sqrt(a') beta / (1 - a)) clamp(pred, +-10) + (sqrt(alpha) (1 - a') / (1 - a)) x + sigma z,
+        sigma^2 = max((1 - a') / (1 - a) beta, 1e-20), and no noise at t = 0.
+    As a k2_sampler_step row (include/k2b200.h): {0, -1, c_x0, c_x, log sigma^2, log sigma^2, t > 0, 0}, so x0 = 0 x + pred
+    and both variance bounds are equal.  Built in float64, cast to fp32 once."""
+
+    def __init__(self, num_steps, num_train_timesteps=1000, clip_range=10.0):
+        num_steps = int(num_steps)
+        if num_steps < 2:
+            raise ValueError(f"UnCLIPSchedule: at least 2 steps (diffusers' UnCLIPScheduler divides by N - 1), got {num_steps}")
+        T = num_train_timesteps
+        self.num_steps, self.clip_range = num_steps, float(clip_range)
+        self.betas = cosine_betas(T)
+        self.alphas_cumprod = np.cumprod(1.0 - self.betas)
+        self.timesteps = (np.arange(num_steps) * ((T - 1) / (num_steps - 1))).round()[::-1].astype(np.int64)
+
+    def rows(self):
+        """float64 [N, 8]: the k2_sampler_step row of every step, in loop order."""
+        ts, acp, out = self.timesteps, self.alphas_cumprod, []
+        for k, t in enumerate(ts):
+            tp = int(ts[k + 1]) if k + 1 < len(ts) else int(t) - 1
+            a = acp[t]
+            ap = acp[tp] if tp >= 0 else 1.0
+            beta = self.betas[t] if tp == t - 1 else 1.0 - a / ap
+            logvar = math.log(max((1.0 - ap) / (1.0 - a) * beta, 1e-20))
+            out.append([0.0, -1.0, math.sqrt(ap) * beta / (1.0 - a), math.sqrt(1.0 - beta) * (1.0 - ap) / (1.0 - a), logvar, logvar,
+                        1.0 if t > 0 else 0.0, 0.0])
+        return np.array(out, dtype=np.float64)
+
+    def coef_table(self):
+        return self.rows().astype(np.float32)
+
+
+class _PriorStepPlan(LaunchPlan):
+    """One UnCLIP sampling step of the prior at B samples, on static buffers, as ONE launch list (replayed as one CUDA graph):
+    k2_step_begin (x duplicated for the 2B CFG rows, this step's t / row / noise picked by the device-side counter), the time
+    embedding and its two linears, clip_img_proj, the token rows 78 and 79 written into the sequence, 20 x (LayerNorm, qkv
+    GEMM, attention, proj GEMM + residual, LayerNorm, fc GEMM, GELU, proj GEMM + residual), the final LayerNorm of the last
+    token (a strided view), out_proj, k2_sampler_step and k2_step_end.  What does not change from step to step -- the text
+    token rows, the text_emb_proj and prd_emb rows with their positional embedding, the keep mask -- is written once per call
+    by bind().  Layer 0 reads the sequence buffer as its residual input.
+
+    Every launch has the eager forward's arguments, so the model output (self.model_out[:, :clip_dim]) equals
+    PriorTransformer.forward bit for bit under the same GEMM configurations (the per-shape tuner may pick split-K, which
+    reorders fp32 sums; with launch_plan.TUNE_SMALL_M = 0 it only picks among bit-identical configurations)."""
+
+    def __init__(self, model, B):
+        dev = model._packed["text_enc"][0].device
+        super().__init__(dev, 2 * B)
+        self.m, self.B = model, B
+        N, W, D, n, ctx = 2 * B, model.xf_width, model.clip_dim, model.text_ctx + model.ext_len, model.text_ctx
+        if D % 4:
+            raise K2Error("k2b200 prior: clip_dim must be a multiple of 4 (the sampler step sees it as [4, 1, clip_dim / 4])")
+        self.N, self.n = N, n
+        f32 = dict(device=dev, dtype=torch.float32)
+        self.x = torch.zeros(B, D, **f32)                   # the sample, updated in place every step
+        self.x_in = torch.zeros(N, D, **f32)
+        self.t_in = torch.zeros(N, **f32)
+        self.coef = torch.zeros(8, **f32)
+        self.noise = torch.zeros(B, D, **f32)
+        self.work = torch.empty(B * D + 4096, **f32)
+        self.counter = torch.zeros(2, device=dev, dtype=torch.int32)
+        self.ts_seq = torch.zeros(1000, **f32)
+        self.coef_seq = torch.zeros(1000, 8, **f32)
+        self.noise_seq = torch.zeros(1000, B, D, **f32)
+        self.guidance = 4.0
+        # model_out [2B, 2 * clip_dim]: out_proj writes the first clip_dim columns of each row, the variance half stays zero
+        self.model_out = torch.zeros(N, 2 * D, **f32)
+        self.seq = torch.zeros(N, n, W, device=dev, dtype=torch.float16)
+        self.keep = torch.ones(N, n, device=dev, dtype=torch.uint8)
+        self.pos16 = model.positional_embedding[0].half().contiguous()
+        self._te32 = torch.empty(N * ctx, W, **f32)
+        self._row32 = torch.empty(N, W, **f32)
+        self._build()
+
+    def _build(self):
+        m, pk, N, n, W, B = self.m, self.m._packed, self.N, self.n, self.m.xf_width, self.B
+        D, ctx, H = m.clip_dim, m.text_ctx, m.xf_heads
+        S = self._add
+        f32 = dict(device=self.dev, dtype=torch.float32)
+        lw = lambda mod: (mod.weight.float().contiguous(), mod.bias.float())  # noqa: E731  (as forward's `lin` passes them)
+        te0, te2, img, outp = (lw(getattr(m.time_embed, "0")), lw(getattr(m.time_embed, "2")), lw(m.clip_img_proj),
+                               lw(m.out_proj))
+        e0, e1, tok_t, tok_x = (torch.empty(N, W, **f32) for _ in range(4))
+        S(lambda: ops.step_begin(self.x, self.x_in, self.t_in, self.coef, self.ts_seq, self.coef_seq, self.noise_seq, self.noise,
+                                 self.counter), "step")
+        S(lambda: ops.timestep_embedding(self.t_in, W, out=e0), "timestep_embedding")
+        S(lambda: ops.linear(e0, *te0, out=e1), "linear", 2 * N * W * W)
+        S(lambda: ops.linear(e1, *te2, silu_in=True, out=tok_t), "linear", 2 * N * W * W)
+        S(lambda: ops.prior_tokens(tok_t, self.pos16[ctx + 1:ctx + 2].expand(N, W), self.seq[:, ctx + 1]), "tokens")
+        S(lambda: ops.linear(self.x_in, *img, out=tok_x), "linear", 2 * N * W * D)
+        S(lambda: ops.prior_tokens(tok_x, self.pos16[ctx + 2:ctx + 3].expand(N, W), self.seq[:, ctx + 2]), "tokens")
+        M = N * n
+        # [N, n, C] views: the tuner counts M = N * n output rows (split-K candidates for small M, launch_plan.tune)
+        y, att = self._new(N, n, W), self._new(N, n, W)
+        qkv, f = self._new(N, n, 3 * W), self._new(N, n, 4 * W)
+        hA, hB = self._new(N, n, W), self._new(N, n, W)
+        h = self.seq
+        self._norms = []   # fp32 gains / biases the launches point at
+        for i, blk in enumerate(m.transformer.resblocks):
+            g1, b1, g2, b2 = (blk.ln_1.weight.float(), blk.ln_1.bias.float(), blk.ln_2.weight.float(), blk.ln_2.bias.float())
+            self._norms += [g1, b1, g2, b2]
+            S(lambda h=h, g=g1, b=b1: ops.layernorm_f16(h, g, b, out=y), "layernorm")
+            w, b = pk[(i, "qkv")]
+            self._gemm(y, w, 3 * W, qkv, 2 * M * 3 * W * W, bias=b)
+            S(lambda: ops.attention_small(qkv, H, keep_mask=self.keep, causal=True, scale=1.0 / math.sqrt(64.0), out=att), "attention",
+              4 * N * H * n * n * 64)
+            w, b = pk[(i, "proj")]
+            self._gemm(att, w, W, hA, 2 * M * W * W, bias=b, residual=h)
+            S(lambda g=g2, b=b2: ops.layernorm_f16(hA, g, b, out=y), "layernorm")
+            w, b = pk[(i, "fc")]
+            self._gemm(y, w, 4 * W, f, 2 * M * 4 * W * W, bias=b)
+            S(lambda: ops.gelu_f16_(f), "gelu")
+            w, b = pk[(i, "proj2")]
+            self._gemm(f, w, W, hB, 2 * M * 4 * W * W, bias=b, residual=hA)
+            h = hB
+        last = h[:, -1]
+        last32 = torch.empty(N, W, **f32)
+        if m.final_ln is not None:
+            lnf = self._new(N, W)
+            gf, bf = m.final_ln.weight.float(), m.final_ln.bias.float()
+            self._norms += [gf, bf]
+            S(lambda: ops.layernorm_f16(last, gf, bf, out=lnf), "layernorm")
+            S(lambda: ops.f16_to_f32(lnf, out=last32), "widen")
+        else:
+            S(lambda: ops.f16_to_f32(last, out=last32), "widen")
+        S(lambda: ops.linear(last32, *outp, out=self.model_out[:, :D]), "linear", 2 * N * W * D)
+        x4, n4, mo8 = self.x.view(B, 4, 1, D // 4), self.noise.view(B, 4, 1, D // 4), self.model_out.view(N, 8, 1, D // 4)
+        S(lambda: ops.sampler_step(mo8, x4, n4, self.coef, self.guidance, 0, clip=10.0, threshold_mode=0, work=self.work),
+          "sampler_step")
+        S(lambda: ops.step_end(self.counter), "step")
+
+    def bind(self, text_emb, text_enc, mask):
+        """This call's conditioning (2B rows, [uncond | cond]) -> the sequence rows that stay fixed for every step and the keep
+        mask, with the eager forward's arithmetic (text_enc_proj GEMM, text_emb_proj linear, prd_emb, + positional rows)."""
+        m, N, n, W, ctx = self.m, self.N, self.n, self.m.xf_width, self.m.text_ctx
+        self.keep.copy_(torch.nn.functional.pad(mask.bool(), (0, m.ext_len), value=True).to(torch.uint8))
+        wte, bte = m._packed["text_enc"]
+        te16 = ops.f32_to_f16(text_enc.float().contiguous()).reshape(N * ctx, m.clip_xf_width)
+        ops.f16_to_f32(ops.gemm_rows(te16, wte, W, bias=bte), out=self._te32)
+        for b in range(N):
+            ops.prior_tokens(self._te32[b * ctx:(b + 1) * ctx], self.pos16[:ctx], self.seq[b, :ctx])
+        ops.linear(text_emb.float().contiguous(), m.text_emb_proj.weight.float().contiguous(), m.text_emb_proj.bias.float(),
+                   out=self._row32)
+        ops.prior_tokens(self._row32, self.pos16[ctx:ctx + 1].expand(N, W), self.seq[:, ctx])
+        ops.prior_tokens(m.prd_emb[0].float().expand(N, W), self.pos16[ctx + 3:ctx + 4].expand(N, W), self.seq[:, ctx + 3])
+
+    def set_schedule(self, sched, x_T, step_noise, guidance, use_graph=True):
+        """Stage a run: the schedule's timesteps and rows, x_T [B, clip_dim], step_noise [N, B, clip_dim]; resets the counter.
+        A new guidance scale drops the captured graph (the scale is a kernel argument baked into it); with use_graph the
+        graph is captured here, before the state is staged, because its warm-up and first replay advance that state."""
+        k = sched.num_steps
+        if k > self.ts_seq.shape[0]:
+            raise K2Error(f"k2b200 prior: at most {self.ts_seq.shape[0]} sampling steps")
+        if float(guidance) != self.guidance:
+            self.guidance, self.graph = float(guidance), None
+        if use_graph and self.graph is None:
+            self.run(True)
+        self.ts_seq[:k].copy_(torch.from_numpy(sched.timesteps.astype(np.float32)))
+        self.coef_seq[:k].copy_(torch.from_numpy(sched.coef_table()))
+        self.noise_seq[:k].copy_(step_noise)
+        self.x.copy_(x_T)
+        self.counter.copy_(torch.tensor([0, k], dtype=torch.int32))
+
+
+@torch.no_grad()
+def sample_prior22(model, text_emb, text_enc, mask, num_steps, guidance, clip_mean, clip_std, x_T, step_noise, use_graph=True):
+    """KandinskyV22PriorPipeline.__call__'s loop (diffusers, restated) with injected noise: text_* hold 2B rows [uncond | cond],
+    x_T [B, clip_dim], step_noise [num_steps, B, clip_dim] (the last step draws none).  Every step is one replay of the
+    prior's step graph (use_graph=False: the same launches, issued one by one).  Returns x * clip_std + clip_mean [B, clip_dim].
+    CFG is uncond + g (cond - uncond); a caller without guidance passes the conditional rows twice, which makes it the
+    conditional prediction exactly."""
+    sched = UnCLIPSchedule(num_steps)
+    plan = model._step_plan(x_T.shape[0])
+    plan.bind(text_emb, text_enc, mask)
+    plan.set_schedule(sched, x_T.float(), step_noise.float(), guidance, use_graph)
+    for _ in range(int(num_steps)):
+        plan.run(use_graph)
+    return plan.x * clip_std + clip_mean
+
+
+class PriorEmbedder22:
+    """The Kandinsky 2.2 diffusion prior behind the pipelines' `embedder` protocol: what diffusers'
+    `KandinskyV22PriorPipeline.__call__` does for the reference's Kandinsky2_2 methods (kandinsky2_2_model.py:69-80,
+    99-111, 130-141, 160-172) -- CLIP text features of [negative prior prompt x B | prompt x B] -> UnCLIP sampling with
+    classifier-free guidance (sample_prior22, one CUDA graph replay per step) -> CLIP image embedding [B, clip_dim].
+
+    clip_text(list[str]) -> (text_embeds [n, clip_dim], last_hidden_state [n, text_ctx, clip_dim], mask [n, text_ctx] bool) and
+    clip_image(PIL.Image) -> [1, clip_dim] are callables, as for the 2.1 PriorEmbedder.  `runs_prior` tells the 2.2 pipeline
+    methods to pass their prior_steps / prior_guidance_scale / negative_prior_prompt to image_emb and interpolate; the
+    constructor's values are the defaults.  With a guidance scale <= 1 the prior runs unguided on the prompt alone, as
+    diffusers does.  x_T and the step noise come from a generator keyed by the seed and the prompt."""
+
+    runs_prior = True
+
+    def __init__(self, prior, clip_text, clip_mean, clip_std, zero_image_emb=None, clip_image=None, prior_steps=25,
+                 prior_guidance_scale=4, negative_prior_prompt="", seed=0, use_cuda_graph=True):
+        self.prior, self.clip_text, self.clip_image = prior, clip_text, clip_image
+        self.clip_mean, self.clip_std = clip_mean, clip_std
+        self.prior_steps, self.prior_guidance_scale = int(prior_steps), float(prior_guidance_scale)
+        self.negative_prior_prompt, self.seed, self.use_cuda_graph = negative_prior_prompt, seed, use_cuda_graph
+        self._zero = zero_image_emb
+
+    @classmethod
+    def from_diffusers(cls, state_dict, clip_text, device="cuda", **kwargs):
+        """Build from a diffusers `PriorTransformer` state dict (kandinsky-community/kandinsky-2-2-prior, subfolder `prior`)
+        via checkpoints.diffusers_prior_to_k2; the configuration is read from the tensor shapes."""
+        from ..checkpoints import diffusers_prior_to_k2
+        sd, mean, std = diffusers_prior_to_k2(state_dict)
+        W = sd["positional_embedding"].shape[-1]
+        layers = sum(1 for k in sd if k.endswith(".attn.c_qkv.weight"))
+        prior = PriorTransformer(text_ctx=sd["positional_embedding"].shape[1] - 4, xf_width=W, xf_layers=layers, xf_heads=W // 64,
+                                 xf_final_ln=True, xf_padding=False, clip_dim=sd["out_proj.weight"].shape[0],
+                                 clip_xf_width=sd["text_enc_proj.weight"].shape[1], device=device)
+        prior.load_state_dict(sd, strict=True)
+        return cls(prior.finalize(), clip_text, mean.to(device).float(), std.to(device).float(), **kwargs)
+
+    @torch.no_grad()
+    def image_emb(self, prompt, batch_size, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None):
+        steps = self.prior_steps if prior_steps is None else int(prior_steps)
+        g = self.prior_guidance_scale if prior_guidance_scale is None else float(prior_guidance_scale)
+        neg = self.negative_prior_prompt if negative_prior_prompt is None else negative_prior_prompt
+        dev, B = self.clip_mean.device, batch_size
+        if g > 1.0:
+            feat, seq, mask = self.clip_text([neg] * B + [prompt] * B)
+        else:  # no guidance (diffusers' do_classifier_free_guidance is False): the conditional rows twice, see sample_prior22
+            feat, seq, mask = (torch.cat([t, t]) for t in self.clip_text([prompt] * B))
+        import hashlib
+        gen = torch.Generator(device=dev).manual_seed(
+            int.from_bytes(hashlib.sha256(f"{self.seed}:{prompt}".encode()).digest()[:7], "little"))
+        D = self.prior.clip_dim
+        x_T = torch.randn(B, D, device=dev, generator=gen)
+        noise = torch.randn(steps, B, D, device=dev, generator=gen)
+        return sample_prior22(self.prior, feat.to(dev), seq.to(dev), mask.to(dev), steps, g, self.clip_mean, self.clip_std, x_T,
+                              noise, use_graph=self.use_cuda_graph).float().cpu()
+
+    def zero_image_emb(self, batch_size):
+        """CLIP embedding of a black image (diffusers' KandinskyV22PriorPipeline.get_zero_embed): supplied by the deployment
+        (it needs the CLIP vision tower); zeros when absent."""
+        z = self._zero if self._zero is not None else torch.zeros(1, self.prior.clip_dim)
+        return z.reshape(1, -1).float().cpu().repeat(batch_size, 1)
+
+    def text_emb(self, prompt, batch_size):
+        raise K2Error("PriorEmbedder22: the Kandinsky 2.2 decoder takes no text input (image embeddings only)")
+
+    def interpolate(self, items, weights, batch_size, **prior_kwargs):
+        """diffusers' KandinskyV22PriorPipeline.interpolate: a text item runs the prior for batch_size rows, an image item is
+        clip_image(img) repeated batch_size times; the result is the weighted sum."""
+        acc = None
+        for it, w in zip(items, weights):
+            if isinstance(it, str):
+                e = self.image_emb(it, batch_size, **prior_kwargs)
+            else:
+                if self.clip_image is None:
+                    raise K2Error("PriorEmbedder22.interpolate: image items need clip_image=")
+                e = self.clip_image(it).float().cpu().reshape(1, -1).repeat(batch_size, 1)
+            acc = e * w if acc is None else acc + e * w
+        return acc

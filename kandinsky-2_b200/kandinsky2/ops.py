@@ -599,3 +599,36 @@ def attention_small(qkv, heads, keep_mask=None, causal=True, scale=0.125, out=No
     check(lib.k2_attention_small(ptr(qkv), _row_stride(qkv), ptr(keep_mask), int(causal), ptr(out), _row_stride(out), B, T,
                                  heads, scale, stream_ptr()))
     return out
+
+
+def _rows_2d(t, dtype, name):
+    """(row stride, rows, columns) of a 2-D view with unit column stride; a row stride of 0 (an expanded row) is kept."""
+    assert t.dtype == dtype and t.dim() == 2 and t.stride(1) == 1, (name, t.dtype, tuple(t.shape), t.stride())
+    return t.stride(0) if t.shape[0] > 1 else t.shape[1], t.shape[0], t.shape[1]
+
+
+def prior_tokens(x, pos, out):
+    """k2_prior_tokens: out fp16 [M, N] (row-strided view) = fp16(fp16(x) + pos) with the eager forward's two roundings.
+    x fp32 [M, N] or [1, N] expanded to M rows (row stride 0), pos fp16 likewise."""
+    tensors = (x, pos, out)
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error("prior_tokens: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    ldy, M, N = _rows_2d(out, torch.float16, "out")
+    ldx, mx, nx = _rows_2d(x, torch.float32, "x")
+    ldp, mp, np_ = _rows_2d(pos, torch.float16, "pos")
+    assert nx == N and np_ == N and mx == M and mp == M, (tuple(x.shape), tuple(pos.shape), tuple(out.shape))
+    check(nat.load().k2_prior_tokens(ptr(x), ldx, ptr(pos), ldp, ptr(out), ldy, M, N, stream_ptr()))
+    return out
+
+
+def f16_to_f32(x, out=None):
+    """k2_f16_to_f32: exact widening of fp16 rows [M, N] (row-strided view) -> fp32 [M, N] (out may be row-strided)."""
+    if not x.is_cuda or (out is not None and not out.is_cuda):
+        raise nat.K2Error("f16_to_f32: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    ldx, M, N = _rows_2d(x, torch.float16, "x")
+    if out is None:
+        out = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    ldy, my, ny = _rows_2d(out, torch.float32, "out")
+    assert (my, ny) == (M, N), (tuple(x.shape), tuple(out.shape))
+    check(nat.load().k2_f16_to_f32(ptr(x), ldx, ptr(out), ldy, M, N, stream_ptr()))
+    return out

@@ -335,18 +335,34 @@ class Kandinsky2_2(_DecoderBase):
         return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, create_ddpm_v22(steps), steps, guidance,
                             noise=latents, init_step=init_step, inpaint=inpaint, hint=hint)
 
-    def _embeds(self, prompt, batch_size, negative_decoder_prompt):
-        pos = self.embedder.image_emb(prompt, batch_size)
-        neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == ""
-               else self.embedder.image_emb(negative_decoder_prompt, batch_size))
-        return pos, neg
+    def _prior_kwargs(self, prior_steps, prior_guidance_scale, negative_prior_prompt):
+        """The call's prior keywords for an embedder that runs the prior (`runs_prior`, e.g. model.prior.PriorEmbedder22); None
+        for every other embedder, which sees exactly the calls it always saw."""
+        if not getattr(self.embedder, "runs_prior", False):
+            return None
+        return dict(prior_steps=prior_steps, prior_guidance_scale=prior_guidance_scale,
+                    negative_prior_prompt=negative_prior_prompt)
+
+    def _embeds(self, prompt, batch_size, negative_decoder_prompt, prior_kw=None):
+        """(image embedding of prompt, decoder negative): the negative is zero_image_emb when negative_decoder_prompt is "",
+        else the prior's embedding of negative_decoder_prompt guided against "" (kandinsky2_2_model.py:72-76)."""
+        pos = self.embedder.image_emb(prompt, batch_size, **(prior_kw or {}))
+        return pos, self._negative(batch_size, negative_decoder_prompt, prior_kw)
+
+    def _negative(self, batch_size, negative_decoder_prompt, prior_kw):
+        if negative_decoder_prompt == "":
+            return self.embedder.zero_image_emb(batch_size)
+        if prior_kw is None:
+            return self.embedder.image_emb(negative_decoder_prompt, batch_size)
+        return self.embedder.image_emb(negative_decoder_prompt, batch_size, **{**prior_kw, "negative_prior_prompt": ""})
 
     def generate_text2img(self, prompt, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                           prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
                           sampler="ddpm_sampler"):
         _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
-        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, sampler=sampler)
 
     def mix_images(self, images_texts, weights, batch_size=1, decoder_steps=50, prior_steps=25,
@@ -354,8 +370,13 @@ class Kandinsky2_2(_DecoderBase):
                    negative_decoder_prompt="", sampler="ddpm_sampler"):
         _check_sampler(sampler, SAMPLERS_22)
         assert len(images_texts) == len(weights) and len(images_texts) > 0
-        pos = self.embedder.interpolate(images_texts, weights, batch_size)
-        _, neg = self._embeds("", batch_size, negative_decoder_prompt)
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        if pk is None:
+            pos = self.embedder.interpolate(images_texts, weights, batch_size)
+            _, neg = self._embeds("", batch_size, negative_decoder_prompt)
+        else:  # no prior run for the unused embedding of ""
+            pos = self.embedder.interpolate(images_texts, weights, batch_size, **pk)
+            neg = self._negative(batch_size, negative_decoder_prompt, pk)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, sampler=sampler)
 
     def generate_img2img(self, prompt, image, strength=0.4, batch_size=1, decoder_steps=100, prior_steps=25,
@@ -363,7 +384,8 @@ class Kandinsky2_2(_DecoderBase):
                          negative_decoder_prompt="", sampler="ddpm_sampler"):
         _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
-        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
         if sampler in SOLVER_SAMPLERS:
@@ -387,7 +409,8 @@ class Kandinsky2_2(_DecoderBase):
         if self.task_type != "controlnet":
             raise ValueError("generate_controlnet needs a pipeline built with task_type='controlnet'")
         h, w = self.get_new_h_w(h, w)
-        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         hint = torch.as_tensor(hint).float()
         if hint.dim() == 3:
             hint = hint[None]
@@ -400,7 +423,8 @@ class Kandinsky2_2(_DecoderBase):
                             negative_decoder_prompt="", sampler="ddpm_sampler"):
         _check_sampler(sampler, SAMPLERS_22)
         h, w = self.get_new_h_w(h, w)
-        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt)
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         lat = self._encode_image(pil_img, h, w)
         m = torch.as_tensor(img_mask).float()[None, None]
         m = torch.nn.functional.interpolate(m, (h // 8, w // 8), mode="nearest").to(self.device)
