@@ -2,6 +2,7 @@
 running it eagerly (so data-dependent decisions -- did a conv emit GroupNorm partials? which tile shape is fastest? -- are
 known when the next launch is recorded) and then replayed eagerly or as ONE CUDA graph.  Shared by the UNet
 (kandinsky2/model/unet.py) and the MoVQ encoder / decoder (kandinsky2/vqgan/autoencoder.py)."""
+import gc
 import os
 
 import torch
@@ -252,8 +253,21 @@ class LaunchPlan:
         if self.graph is None:
             self.launch()  # warm-up: one-time cudaFuncSetAttribute calls are not capturable
             torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.launch()
-            self.graph = g
+            self.graph = capture_graph(self.launch)
         self.graph.replay()
+
+
+def capture_graph(launch):
+    """launch() recorded into a new CUDA graph, with Python's cyclic garbage collector paused for the capture.  A launch plan
+    is a reference cycle (its launch closures hold it), so the CUDA graph of a plan nobody holds any more is destroyed whenever
+    the collector next runs; if that happens while a stream captures, the destruction invalidates the capture."""
+    g = torch.cuda.CUDAGraph()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(g):
+            launch()
+    finally:
+        if enabled:
+            gc.enable()
+    return g

@@ -17,6 +17,7 @@ import torch
 
 from .. import ops, parallel
 from .._native import K2Error
+from ..launch_plan import capture_graph
 
 
 def get_named_beta_schedule(schedule_name, num_diffusion_timesteps, linear_start=0.0001, linear_end=0.02):
@@ -739,10 +740,7 @@ class FusedStep:
             k0, x0 = st["counter"].clone(), xs.clone()
             self._launch_step(xs, nseq)  # warm-up: one-time cudaFuncSetAttribute calls are not capturable
             torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._launch_step(xs, nseq)
-            st[gkey] = g
+            st[gkey] = capture_graph(lambda: self._launch_step(xs, nseq))
             st["counter"].copy_(k0)  # the warm-up advanced the schedule and the latent: put both back
             xs.copy_(x0)
         st[gkey].replay()

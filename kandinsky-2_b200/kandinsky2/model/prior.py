@@ -267,22 +267,37 @@ class UnCLIPSchedule:
         x' = (sqrt(a') beta / (1 - a)) clamp(pred, +-10) + (sqrt(alpha) (1 - a') / (1 - a)) x + sigma z,
         sigma^2 = max((1 - a') / (1 - a) beta, 1e-20), and no noise at t = 0.
     As a k2_sampler_step row (include/k2b200.h): {0, -1, c_x0, c_x, log sigma^2, log sigma^2, t > 0, 0}, so x0 = 0 x + pred
-    and both variance bounds are equal.  Built in float64, cast to fp32 once."""
+    and both variance bounds are equal.  Built in float64, cast to fp32 once.
 
-    def __init__(self, num_steps, num_train_timesteps=1000, clip_range=10.0):
+    keep = s (KandinskyV22PriorEmb2EmbPipeline's strength): only the last s of the N steps run, `timesteps` and `rows()` are
+    the tail of the full schedule's (a row's next timestep is still the full list's, as diffusers passes
+    prev_timestep = timesteps[i + 1]), and the run starts from start_latent(emb, noise) at the first kept timestep."""
+
+    def __init__(self, num_steps, num_train_timesteps=1000, clip_range=10.0, keep=None):
         num_steps = int(num_steps)
         if num_steps < 2:
             raise ValueError(f"UnCLIPSchedule: at least 2 steps (diffusers' UnCLIPScheduler divides by N - 1), got {num_steps}")
+        keep = num_steps if keep is None else int(keep)
+        if not 1 <= keep <= num_steps:
+            raise ValueError(f"UnCLIPSchedule: keep must be in [1, {num_steps}], got {keep}")
         T = num_train_timesteps
-        self.num_steps, self.clip_range = num_steps, float(clip_range)
+        self.num_steps, self.keep, self.clip_range = num_steps, keep, float(clip_range)
         self.betas = cosine_betas(T)
         self.alphas_cumprod = np.cumprod(1.0 - self.betas)
-        self.timesteps = (np.arange(num_steps) * ((T - 1) / (num_steps - 1))).round()[::-1].astype(np.int64)
+        self._all = (np.arange(num_steps) * ((T - 1) / (num_steps - 1))).round()[::-1].astype(np.int64)
+        self.timesteps = self._all[num_steps - keep:]
+
+    def start_latent(self, emb, noise):
+        """UnCLIPScheduler.add_noise at the first kept timestep t: sqrt(acp[t]) emb + sqrt(1 - acp[t]) noise, the coefficients
+        in float64."""
+        a = float(self.alphas_cumprod[int(self.timesteps[0])])
+        return math.sqrt(a) * emb + math.sqrt(1.0 - a) * noise
 
     def rows(self):
-        """float64 [N, 8]: the k2_sampler_step row of every step, in loop order."""
-        ts, acp, out = self.timesteps, self.alphas_cumprod, []
-        for k, t in enumerate(ts):
+        """float64 [keep, 8]: the k2_sampler_step row of every kept step, in loop order."""
+        ts, acp, out = self._all, self.alphas_cumprod, []
+        for k in range(self.num_steps - self.keep, self.num_steps):
+            t = ts[k]
             tp = int(ts[k + 1]) if k + 1 < len(ts) else int(t) - 1
             a = acp[t]
             ap = acp[tp] if tp >= 0 else 1.0
@@ -411,10 +426,10 @@ class _PriorStepPlan(LaunchPlan):
         ops.prior_tokens(m.prd_emb[0].float().expand(N, W), self.pos16[ctx + 3:ctx + 4].expand(N, W), self.seq[:, ctx + 3])
 
     def set_schedule(self, sched, x_T, step_noise, guidance, use_graph=True):
-        """Stage a run: the schedule's timesteps and rows, x_T [B, clip_dim], step_noise [N, B, clip_dim]; resets the counter.
-        A new guidance scale drops the captured graph (the scale is a kernel argument baked into it); with use_graph the
-        graph is captured here, before the state is staged, because its warm-up and first replay advance that state."""
-        k = sched.num_steps
+        """Stage a run: the schedule's kept timesteps and rows, x_T [B, clip_dim], step_noise [keep, B, clip_dim]; resets the
+        counter.  A new guidance scale drops the captured graph (the scale is a kernel argument baked into it); with use_graph
+        the graph is captured here, before the state is staged, because its warm-up and first replay advance that state."""
+        k = sched.keep
         if k > self.ts_seq.shape[0]:
             raise K2Error(f"k2b200 prior: at most {self.ts_seq.shape[0]} sampling steps")
         if float(guidance) != self.guidance:
@@ -429,17 +444,19 @@ class _PriorStepPlan(LaunchPlan):
 
 
 @torch.no_grad()
-def sample_prior22(model, text_emb, text_enc, mask, num_steps, guidance, clip_mean, clip_std, x_T, step_noise, use_graph=True):
+def sample_prior22(model, text_emb, text_enc, mask, num_steps, guidance, clip_mean, clip_std, x_T, step_noise, use_graph=True,
+                   keep=None):
     """KandinskyV22PriorPipeline.__call__'s loop (diffusers, restated) with injected noise: text_* hold 2B rows [uncond | cond],
     x_T [B, clip_dim], step_noise [num_steps, B, clip_dim] (the last step draws none).  Every step is one replay of the
     prior's step graph (use_graph=False: the same launches, issued one by one).  Returns x * clip_std + clip_mean [B, clip_dim].
     CFG is uncond + g (cond - uncond); a caller without guidance passes the conditional rows twice, which makes it the
-    conditional prediction exactly."""
-    sched = UnCLIPSchedule(num_steps)
+    conditional prediction exactly.  keep = s runs only the last s of the num_steps UnCLIP steps from x_T (the emb2emb
+    pipeline's truncation, UnCLIPSchedule); step_noise then has s rows."""
+    sched = UnCLIPSchedule(num_steps, keep=keep)
     plan = model._step_plan(x_T.shape[0])
     plan.bind(text_emb, text_enc, mask)
     plan.set_schedule(sched, x_T.float(), step_noise.float(), guidance, use_graph)
-    for _ in range(int(num_steps)):
+    for _ in range(sched.keep):
         plan.run(use_graph)
     return plan.x * clip_std + clip_mean
 
@@ -452,8 +469,9 @@ class PriorEmbedder22:
 
     clip_text(list[str]) -> (text_embeds [n, clip_dim], last_hidden_state [n, text_ctx, clip_dim], mask [n, text_ctx] bool) and
     clip_image(PIL.Image) -> [1, clip_dim] are callables, as for the 2.1 PriorEmbedder.  `runs_prior` tells the 2.2 pipeline
-    methods to pass their prior_steps / prior_guidance_scale / negative_prior_prompt to image_emb and interpolate; the
-    constructor's values are the defaults.  With a guidance scale <= 1 the prior runs unguided on the prompt alone, as
+    methods to pass their prior_steps / prior_guidance_scale / negative_prior_prompt to image_emb, interpolate and emb2emb; the
+    constructor's values are the defaults.  emb2emb is KandinskyV22PriorEmb2EmbPipeline: the prior started from a noised
+    image embedding.  With a guidance scale <= 1 the prior runs unguided on the prompt alone, as
     diffusers does.  x_T and the step noise come from a generator keyed by the seed and the prompt."""
 
     runs_prior = True
@@ -480,24 +498,66 @@ class PriorEmbedder22:
         prior.load_state_dict(sd, strict=True)
         return cls(prior.finalize(), clip_text, mean.to(device).float(), std.to(device).float(), **kwargs)
 
-    @torch.no_grad()
-    def image_emb(self, prompt, batch_size, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None):
+    def _call_args(self, prompt, B, prior_steps, prior_guidance_scale, negative_prior_prompt):
+        """(steps, guidance, CFG rows [text_embeds, hidden states, mask] on the device, the call's generator): the rows are
+        [negative prior prompt x B | prompt x B], or the prompt's rows twice when guidance <= 1 (diffusers'
+        do_classifier_free_guidance is False, see sample_prior22); the generator is keyed by the seed and the prompt."""
         steps = self.prior_steps if prior_steps is None else int(prior_steps)
         g = self.prior_guidance_scale if prior_guidance_scale is None else float(prior_guidance_scale)
         neg = self.negative_prior_prompt if negative_prior_prompt is None else negative_prior_prompt
-        dev, B = self.clip_mean.device, batch_size
+        dev = self.clip_mean.device
         if g > 1.0:
             feat, seq, mask = self.clip_text([neg] * B + [prompt] * B)
-        else:  # no guidance (diffusers' do_classifier_free_guidance is False): the conditional rows twice, see sample_prior22
+        else:
             feat, seq, mask = (torch.cat([t, t]) for t in self.clip_text([prompt] * B))
         import hashlib
         gen = torch.Generator(device=dev).manual_seed(
             int.from_bytes(hashlib.sha256(f"{self.seed}:{prompt}".encode()).digest()[:7], "little"))
-        D = self.prior.clip_dim
+        return steps, g, (feat.to(dev), seq.to(dev), mask.to(dev)), gen
+
+    @torch.no_grad()
+    def image_emb(self, prompt, batch_size, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None):
+        dev, B, D = self.clip_mean.device, batch_size, self.prior.clip_dim
+        steps, g, rows, gen = self._call_args(prompt, B, prior_steps, prior_guidance_scale, negative_prior_prompt)
         x_T = torch.randn(B, D, device=dev, generator=gen)
         noise = torch.randn(steps, B, D, device=dev, generator=gen)
-        return sample_prior22(self.prior, feat.to(dev), seq.to(dev), mask.to(dev), steps, g, self.clip_mean, self.clip_std, x_T,
-                              noise, use_graph=self.use_cuda_graph).float().cpu()
+        return sample_prior22(self.prior, *rows, steps, g, self.clip_mean, self.clip_std, x_T, noise,
+                              use_graph=self.use_cuda_graph).float().cpu()
+
+    @torch.no_grad()
+    def emb2emb(self, prompt, image, batch_size, strength=0.3, prior_steps=None, prior_guidance_scale=None,
+                negative_prior_prompt=None):
+        """diffusers' KandinskyV22PriorEmb2EmbPipeline.__call__ (restated, unpinned): the prior started from a noised image
+        embedding instead of pure noise.  image: a CLIP image embedding [1, clip_dim] (repeated to batch_size rows) or
+        [batch_size, clip_dim], or a PIL image, which goes through clip_image.  Of the N = prior_steps UnCLIP steps the last
+        keep = min(int(N * strength), N) run (get_timesteps), from x = UnCLIPScheduler.add_noise(image embedding, z) at the first
+        kept timestep (prepare_latents: the embedding is NOT normalised by clip_mean / clip_std on the way in); the result is
+        x * clip_std + clip_mean (post_process_latents), as for image_emb.  Rows, guidance and the negative prior prompt are
+        image_emb's; the generator draws z [B, clip_dim] first, then the step noise [keep, B, clip_dim]."""
+        steps = self.prior_steps if prior_steps is None else int(prior_steps)
+        strength = float(strength)
+        if not 0.0 <= strength <= 1.0:
+            raise ValueError(f"PriorEmbedder22.emb2emb: strength must be in [0, 1], got {strength}")
+        keep = min(int(steps * strength), steps)
+        if keep == 0:
+            raise ValueError(f"PriorEmbedder22.emb2emb: strength {strength} keeps no step of {steps} (int(N * strength) = 0)")
+        sched = UnCLIPSchedule(steps, keep=keep)
+        dev, B, D = self.clip_mean.device, batch_size, self.prior.clip_dim
+        if torch.is_tensor(image):
+            emb = image.float().reshape(-1, D) if image.dim() == 1 else image.float()
+            if emb.dim() != 2 or emb.shape[1] != D or emb.shape[0] not in (1, B):
+                raise ValueError(f"PriorEmbedder22.emb2emb: an image embedding must be [1, {D}] or [{B}, {D}], got "
+                                 f"{list(image.shape)}")
+        else:
+            if self.clip_image is None:
+                raise K2Error("PriorEmbedder22.emb2emb: a PIL image needs clip_image=")
+            emb = self.clip_image(image).float().reshape(1, D)
+        emb = emb.to(dev).expand(B, D)
+        steps, g, rows, gen = self._call_args(prompt, B, steps, prior_guidance_scale, negative_prior_prompt)
+        z = torch.randn(B, D, device=dev, generator=gen)
+        noise = torch.randn(keep, B, D, device=dev, generator=gen)
+        return sample_prior22(self.prior, *rows, steps, g, self.clip_mean, self.clip_std, sched.start_latent(emb, z), noise,
+                              use_graph=self.use_cuda_graph, keep=keep).float().cpu()
 
     def zero_image_emb(self, batch_size):
         """CLIP embedding of a black image (diffusers' KandinskyV22PriorPipeline.get_zero_embed): supplied by the deployment

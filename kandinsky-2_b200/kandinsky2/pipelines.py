@@ -388,15 +388,30 @@ class Kandinsky2_2(_DecoderBase):
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         lat = self._encode_image(image, h, w)
         diffusion = create_ddpm_v22(decoder_steps)
-        if sampler in SOLVER_SAMPLERS:
-            x, start = self._dpm_img2img_start(lat, diffusion, decoder_steps, strength, sampler)
-        else:
-            # diffusers KandinskyV22Img2ImgPipeline: the last int(steps*strength) timesteps, scheduler.add_noise at the first
-            start = _dpm_keep(decoder_steps, strength)
-            ac = float(diffusion.alphas_cumprod[start - 1])
-            x = ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * self._img2img_noise(lat)
+        x, start = self._img2img_start(lat, diffusion, decoder_steps, strength, sampler)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, sampler=sampler)
+
+    def _img2img_start(self, lat, diffusion, steps, strength, sampler):
+        """img2img of the 2.2 methods -> (start latent [1, 4, h, w], the init_step of _decode_loop): the solver samplers'
+        _dpm_img2img_start, else diffusers' KandinskyV22Img2ImgPipeline rule -- the last int(steps * strength) DDPM timesteps
+        (at least 1) run, from scheduler.add_noise of the image latent at the first of them."""
+        if sampler in SOLVER_SAMPLERS:
+            return self._dpm_img2img_start(lat, diffusion, steps, strength, sampler)
+        start = _dpm_keep(steps, strength)
+        ac = float(diffusion.alphas_cumprod[start - 1])
+        return ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * self._img2img_noise(lat), start
+
+    @staticmethod
+    def _hint(hint, h, w):
+        """The ControlNet depth map as a float tensor [1, 3, h, w] (a [3, H, W] map gains the batch axis; another size is
+        resized bilinearly)."""
+        hint = torch.as_tensor(hint).float()
+        if hint.dim() == 3:
+            hint = hint[None]
+        if tuple(hint.shape[-2:]) != (h, w):
+            hint = torch.nn.functional.interpolate(hint, (h, w), mode="bilinear", align_corners=False)
+        return hint
 
     def generate_controlnet(self, prompt, hint, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                             prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
@@ -411,12 +426,45 @@ class Kandinsky2_2(_DecoderBase):
         h, w = self.get_new_h_w(h, w)
         pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
-        hint = torch.as_tensor(hint).float()
-        if hint.dim() == 3:
-            hint = hint[None]
-        if tuple(hint.shape[-2:]) != (h, w):
-            hint = torch.nn.functional.interpolate(hint, (h, w), mode="bilinear", align_corners=False)
+        hint = self._hint(hint, h, w)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, hint=hint, sampler=sampler)
+
+    def generate_controlnet_img2img(self, prompt, image, hint, strength=0.5, batch_size=1, decoder_steps=50, prior_steps=25,
+                                    decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
+                                    negative_decoder_prompt="", sampler="ddpm_sampler", prior_strength=None):
+        """Kandinsky 2.2 ControlNet-depth image-to-image: what notebooks/kandinsky2_2_controlnet.ipynb, the reference's one use
+        of the ControlNet model, runs with diffusers' KandinskyV22ControlnetImg2ImgPipeline (the reference package has no
+        method for it; the signature follows generate_controlnet's, the defaults are the notebook's).  image (PIL image, image
+        tensor or encoded latent, as generate_img2img takes it) is encoded by the MoVQ encoder and noised to the first of the
+        last int(decoder_steps * strength) evaluations (generate_img2img's start, for every sampler name), and those run with
+        the depth hint (as generate_controlnet takes it).
+
+        prior_strength=None: the image embeddings come from the prompt alone, as in generate_controlnet.  A number runs the
+        prior from the image's CLIP embedding instead (KandinskyV22PriorEmb2EmbPipeline, PriorEmbedder22.emb2emb; image must
+        then be a PIL image, which the embedder's clip_image embeds): the positive embedding is emb2emb(prompt, image,
+        strength=prior_strength), the decoder negative is zero_image_emb for negative_decoder_prompt == "", else
+        emb2emb(negative_decoder_prompt, image, strength=1, guided against "") -- the notebook's second prior call.  That
+        needs an embedder with `runs_prior` and `emb2emb`."""
+        _check_sampler(sampler, SAMPLERS_22)
+        if self.task_type != "controlnet":
+            raise ValueError("generate_controlnet_img2img needs a pipeline built with task_type='controlnet'")
+        pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        if prior_strength is not None and (pk is None or not hasattr(self.embedder, "emb2emb")):
+            raise ValueError("prior_strength needs an embedder that runs the prior from an image embedding "
+                             "(runs_prior and emb2emb, e.g. model.prior.PriorEmbedder22)")
+        h, w = self.get_new_h_w(h, w)
+        if prior_strength is None:
+            pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
+        else:
+            pos = self.embedder.emb2emb(prompt, image, batch_size, strength=prior_strength, **pk)
+            neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == "" else
+                   self.embedder.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
+                                         **{**pk, "negative_prior_prompt": ""}))
+        lat = self._encode_image(image, h, w)
+        x, start = self._img2img_start(lat, create_ddpm_v22(decoder_steps), decoder_steps, strength, sampler)
+        return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
+                                 latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, hint=self._hint(hint, h, w),
+                                 sampler=sampler)
 
     def generate_inpainting(self, prompt, pil_img, img_mask, batch_size=1, decoder_steps=50, prior_steps=25,
                             decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
