@@ -419,6 +419,12 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
   pdl_wait();
   pdl_launch();
 
+  // Tile order: N tile fastest.  The CTAs running at one time then cover SM count / n_tiles M tiles, all of whose N tiles, so
+  // the source rows they re-read for every tap stay in L2.  With the M tile fastest they covered up to SM count M tiles:
+  // for the 1536- and 1920-channel 48 x 48 convolutions that is 52-65 MB of source, more than the 50 MB L2, and every
+  // tap's pass over the channel chunks came from HBM again.  In exchange the weights of all N tiles are live at once instead
+  // of one N tile's (profiles/conv_layers.md lists the shapes that gain and lose).  Each tile computes exactly what it did,
+  // so results are bit-identical.
   const int total_tiles = p.m_tiles * p.n_tiles * p.splits;
 
   if (wg == 0) {
@@ -429,8 +435,8 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       uint32_t ring_phase = 0;
       const uint32_t tx_bytes = p.a_box_bytes + C::B_STAGE_BYTES;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m_idx = tile % p.m_tiles;
-        const int n_idx = (tile / p.m_tiles) % p.n_tiles;
+        const int n_idx = tile % p.n_tiles;
+        const int m_idx = (tile / p.n_tiles) % p.m_tiles;
         const int split = tile / (p.m_tiles * p.n_tiles);
         int n0, y0, x0, phase;
         decode_m_tile(p, m_idx, n0, y0, x0, phase);
@@ -477,8 +483,8 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_idx = tile % p.m_tiles;
-      const int n_idx = (tile / p.m_tiles) % p.n_tiles;
+      const int n_idx = tile % p.n_tiles;
+      const int m_idx = (tile / p.n_tiles) % p.m_tiles;
       const int split = tile / (p.m_tiles * p.n_tiles);
       const int nk = min(p.num_k_chunks, (split + 1) * p.k_per_split) - split * p.k_per_split;
       float acc[NA];
