@@ -343,6 +343,28 @@ int k2_prior_tokens(const float* x, int ldx, const void* pos, int ldp, void* y, 
 int k2_f16_to_f32(const void* x, int ldx, float* y, int ldy, int M, int N, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * CLIP image tower (diffusers' KandinskyV22PriorPipeline image_encoder, a transformers CLIPVisionModelWithProjection; the
+ * reference builds it at kandinsky2_2_model.py:24; kandinsky2/model/clip_vision.py).  Its Linear layers are k2_conv_gemm
+ * flat-row GEMMs and its LayerNorm / GELU / widening are the prior's entry points above; these two are the rest.
+ *
+ * k2_clip_patchify: x fp32 NCHW [B, 3, S, S] (4-byte aligned) -> out fp16 rows [B * (G^2 + 1), ldo], G = S / P, for ONE GEMM
+ *   with the weight [hidden, Kp] = (patch conv weight flattened as c P^2 + ky P + kx | class_embedding | zeros) and the
+ *   position embedding as the residual:
+ *     row b (G^2 + 1):            1 in column 3 P^2 (the CLS slot), 0 elsewhere;
+ *     row b (G^2 + 1) + 1 + t:    column c P^2 + ky P + kx = fp16_rn(x[b, c, P (t / G) + ky, P (t % G) + kx]), t < G^2;
+ *   columns [3 P^2 (+1), Kp) are zero; columns >= Kp are not touched.  Needs S % P == 0, Kp >= 3 P^2 + 1, ldo >= Kp.
+ * k2_attention_heads: softmax(scale q k^T) v per head, no mask, over T tokens, head width head_dim (104 only, the ViT-bigG/14
+ *   geometry; anything else is refused).  qkv fp16 rows [B, T, ldq], head h reads q / k / v at h hs + q_off / k_off / v_off;
+ *   out fp16 rows [B, T, ldo], head h at h ohs (only its head_dim columns are written).  Strides and offsets are multiples of 8
+ *   elements, pointers 16-byte aligned, (heads - 1) hs + max offset + head_dim <= ldq, ohs >= head_dim and
+ *   (heads - 1) ohs + head_dim <= ldo.  fp32 scores and softmax, P rounded to fp16 before PV (the k2_attention_d512 recipe).
+ * Both check their arguments before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+int k2_clip_patchify(const float* x, int B, int S, int P, void* out, int ldo, int Kp, k2_stream_t stream);
+int k2_attention_heads(const void* qkv, int ldq, int hs, int q_off, int k_off, int v_off, int B, int heads, int T, int head_dim,
+                       float scale, void* out, int ldo, int ohs, k2_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
  * fuse_lora): once per adapter load, never per step.
  *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols

@@ -9,11 +9,17 @@
 //                201-225; encoder twin vqgan_blocks.py:186-240) on mma.sync m16n8k16.  Its output channels are split over two
 //                CTAs (DV = 256 each): an fp32 O row of 256 channels is 128 registers per thread, the full 512 would not fit
 //                next to the scores.  8 warps = 128 queries per CTA, 16-key blocks.
+//   head dim 104 (k2_attention_heads, flash_attention_kernel with DR = 104): the CLIP ViT-bigG/14 image tower's 16 heads
+//                (kandinsky2/model/clip_vision.py).  The tiles are D = 112 wide (seven k16 steps); the 8 columns past the real
+//                width arrive zero-filled and the matching output columns are not stored, so the arithmetic is the unpadded one.
 // Both follow one numerical recipe: fp32 scores, scale * log2(e) folded into ex2, row sums from the unrounded fp32 P, P rounded
 // to fp16 before PV (as in the reference's fp16 mode, unet.py:338), O / l rounded once to fp16.  Every key block they process
 // holds at least one valid key, so the running maximum is finite from the first block on.
 //
 // flash_attention_kernel: CTA = NW warps, 16 query rows per warp; per key block of BKV keys:
+//   (DR = the real head width, <= D, a multiple of 8: q / k / v columns [DR, D) of the tiles are zero-filled by cp.async with
+//   src-size 0 -- zero q and k columns add exact zeros to the fp32 scores -- and output columns [DR, D) are never stored.
+//   With DR = D every such test is a compile-time constant and the kernel is the unpadded one.)
 //     S = Q K^T            Q fragments (ldmatrix) x K fragments (ldmatrix) from shared memory, fp32 in registers
 //     m = max(m, rowmax S * c), P = exp2(S * c - m), l = l * alpha + rowsum P, O = O * alpha + fp16(P) V
 //   P goes from the score accumulators straight into the A fragments of the PV product (same register layout), V is read
@@ -53,10 +59,11 @@ struct FlashCfg {
 };
 
 // grid: (query tiles, heads * D / DV, B); blockIdx.y = head * (D / DV) + output-channel split
-template <int D, int DV, int NW, int BKV>
+template <int D, int DV, int NW, int BKV, int DR>
 __global__ void __launch_bounds__(NW * 32, 1) flash_attention_kernel(const FlashParams p) {
   using C = FlashCfg<D, DV, NW, BKV>;
   constexpr int NSPLIT = D / DV;
+  static_assert(DR % 8 == 0 && DR <= D && (DR == D || NSPLIT == 1), "a padded head keeps its output channels in one CTA");
   extern __shared__ __align__(16) uint8_t smem[];
   __half* sQ = reinterpret_cast<__half*>(smem);
   __half* sK = reinterpret_cast<__half*>(smem + C::Q_BYTES);                  // [2][BKV][QP]
@@ -80,8 +87,10 @@ __global__ void __launch_bounds__(NW * 32, 1) flash_attention_kernel(const Flash
     for (int i = tid; i < C::BQ * CPR; i += NW * 32) {
       const int r = i / CPR, c = i - r * CPR;
       const int q = q0 + r;
-      const __half* src = p.qkv + (static_cast<long long>(b) * p.T + (q < p.T ? q : 0)) * p.ldq + head * p.hs + p.q_off + c * 8;
-      cp_async_16(smem_u32(sQ + r * C::QP + c * 8), src, q < p.T ? 16 : 0);
+      const bool real = DR == D || c < DR / 8;
+      const __half* src = p.qkv + (static_cast<long long>(b) * p.T + (q < p.T ? q : 0)) * p.ldq + head * p.hs + p.q_off +
+                          (real ? c * 8 : 0);
+      cp_async_16(smem_u32(sQ + r * C::QP + c * 8), src, q < p.T && real ? 16 : 0);
     }
   }
   auto load_kv = [&](int jb, int st) {
@@ -89,7 +98,7 @@ __global__ void __launch_bounds__(NW * 32, 1) flash_attention_kernel(const Flash
     for (int i = tid; i < BKV * (KC + VC); i += NW * 32) {
       const int r = i / (KC + VC), c = i - r * (KC + VC);
       const int key = jb * BKV + r;
-      const bool ok = key < Tkv;
+      const bool ok = key < Tkv && (DR == D || (c < KC ? c : c - KC) < DR / 8);
       const bool from_enc = key < p.Tc;
       const __half* row = from_enc ? p.enc + (static_cast<long long>(b) * p.Tc + key) * p.lde + head * p.ehs
                                    : p.qkv + (static_cast<long long>(b) * p.T + (ok ? key - p.Tc : 0)) * p.ldq + head * p.hs;
@@ -214,21 +223,22 @@ __global__ void __launch_bounds__(NW * 32, 1) flash_attention_kernel(const Flash
     __half* orow = p.out + (static_cast<long long>(b) * p.T + q) * p.ldo + head * p.ohs + dsplit * DV + 2 * (lane & 3);
 #pragma unroll
     for (int n = 0; n < DV / 8; ++n)
-      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_h2(o[n][2 * h] * inv[h], o[n][2 * h + 1] * inv[h]);
+      if (DR == D || n < DR / 8)
+        *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_h2(o[n][2 * h] * inv[h], o[n][2 * h + 1] * inv[h]);
   }
 }
 
-template <int D, int DV, int NW, int BKV>
+template <int D, int DV, int NW, int BKV, int DR = D>
 int launch_flash(const FlashParams& p, cudaStream_t stream) {
   using C = FlashCfg<D, DV, NW, BKV>;
   static bool attr_set = false;
   if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(flash_attention_kernel<D, DV, NW, BKV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    K2_CHECK_CUDA(cudaFuncSetAttribute(flash_attention_kernel<D, DV, NW, BKV, DR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        C::SMEM_BYTES));
     attr_set = true;
   }
   dim3 grid((p.T + C::BQ - 1) / C::BQ, p.heads * (D / DV), p.B);
-  K2_CHECK_CUDA(launch_k(flash_attention_kernel<D, DV, NW, BKV>, grid, dim3(NW * 32), C::SMEM_BYTES, stream, p));
+  K2_CHECK_CUDA(launch_k(flash_attention_kernel<D, DV, NW, BKV, DR>, grid, dim3(NW * 32), C::SMEM_BYTES, stream, p));
   return 0;
 }
 
@@ -498,6 +508,12 @@ int launch_attention(const FlashParams& p, int head_dim, cudaStream_t stream) {
   // head width 512: 8 warps x 16-key blocks (Q 130 KB + two K / V stages 49 KB of shared memory) -- 7.5 ms at the MoVQ 768 x 768
   // geometry on an H100 SXM at 700 W, against 12.0 ms with 4 warps x 32-key blocks (one CTA of 4 warps per SM)
   if (head_dim == 512) return launch_flash<512, 256, 8, 16>(p, stream);
+  // head width 104 (CLIP ViT-bigG/14: T = 257, 16 heads): 4 warps = 64 queries per CTA and 64-key blocks.  An image is then
+  // 5 query tiles x 16 heads = 80 CTAs, and a B >= 2 batch fills the 132 SMs; each CTA keeps O (14 x 4 fp32), the scores
+  // (8 x 4) and a 64-key block's K / V stages (Q 15 KB + 2 x 30 KB of shared memory) resident, so two CTAs fit per SM.
+  // Smaller query tiles would cut the padding of the last tile (257 = 4 x 64 + 1) but re-read every key from L2 for half as
+  // many queries.  Not tuned: the attention is 2.2 % of the tower's FLOPs.
+  if (head_dim == 104) return launch_flash<112, 112, 4, 64, 104>(p, stream);
   return launch_attention_d64(p, stream);
 }
 

@@ -87,7 +87,7 @@ int launch_conv_gemm(const ConvGemmParams& p, int BN, int epilogue_sets, cudaStr
 int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, const float* bias, const __half* residual,
                            int ldr, __half* out, int ldo, float2* gn_part, cudaStream_t stream);
 
-// ---- fused attention, head dim 64 / 512 (k2_attention.cu) ----------------------------------------
+// ---- fused attention, head dim 64 / 104 / 512 (k2_attention.cu) ----------------------------------
 struct FlashParams {
   const __half* qkv;   // [B, T, ldq] rows; head h reads q / k / v at channels h*hs + {q,k,v}_off
   long long ldq;

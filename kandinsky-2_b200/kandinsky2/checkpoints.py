@@ -14,6 +14,11 @@
   `model.prior.PriorTransformer` names and returns clip_mean / clip_std beside it (tests/test_cpu_prior22.py pins it through the
   network: the reference's forward on the remapped weights equals the diffusers-form forward).
 
+* Kandinsky 2.2's prior pipeline carries a CLIP image tower, a transformers `CLIPVisionModelWithProjection`
+  (`kandinsky2_2_model.py:24`, subfolder `image_encoder`).  `transformers_clip_vision_to_k2` renames it into
+  `model.clip_vision.CLIPVisionTower` names and packs q / k / v per head (tests/test_cpu_clip_vision.py pins it through the
+  network against the transformers-name forward and transformers' own outputs).
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -261,4 +266,53 @@ def k2_to_diffusers_unet(sd,in_channels=4, model_channels=384, channel_mult=(1, 
                 out[f"{dp}.{n}.weight"], out[f"{dp}.{n}.bias"] = w, b
             out[f"{dp}.to_out.0.weight"] = sd[f"{kp}.proj_out.weight"].squeeze(-1)
             out[f"{dp}.to_out.0.bias"] = sd[f"{kp}.proj_out.bias"]
+    return out
+
+
+_CLIP_V_LAYER = {"layer_norm1": "ln_1", "layer_norm2": "ln_2", "self_attn.out_proj": "attn.proj", "mlp.fc1": "mlp.fc1",
+                 "mlp.fc2": "mlp.fc2"}
+
+
+def transformers_clip_vision_keys(layers):
+    """Every key of a transformers `CLIPVisionModelWithProjection` state dict with `layers` encoder layers (without the
+    non-persistent `position_ids` buffer)."""
+    p = "vision_model."
+    keys = [p + "embeddings.class_embedding", p + "embeddings.patch_embedding.weight", p + "embeddings.position_embedding.weight"]
+    keys += [f"{p}{n}.{s}" for n in ("pre_layrnorm", "post_layernorm") for s in ("weight", "bias")]
+    for i in range(layers):
+        lp = f"{p}encoder.layers.{i}."
+        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_V_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
+                 for s in ("weight", "bias")]
+    return keys + ["visual_projection.weight"]
+
+
+def transformers_clip_vision_to_k2(sd, head_dim=104):
+    """transformers `CLIPVisionModelWithProjection` state dict (the Kandinsky 2.2 prior's `image_encoder`) ->
+    `model.clip_vision.CLIPVisionTower` names:
+        class_embedding [H], patch_embedding.weight [H, 3, P, P], position_embedding [T, H], pre_ln.*, post_ln.*, proj.weight,
+        layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}
+    where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads with the tower's head width).  A
+    `position_ids` buffer is ignored; unknown and missing keys raise K2Error naming them."""
+    p = "vision_model."
+    sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
+    layers = {int(m.group(1)) for m in (re.match(r"^vision_model\.encoder\.layers\.(\d+)\.", k) for k in sd) if m}
+    expected = transformers_clip_vision_keys(max(layers) + 1 if layers else 0)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"transformers CLIP vision state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {"class_embedding": sd[p + "embeddings.class_embedding"],
+           "patch_embedding.weight": sd[p + "embeddings.patch_embedding.weight"],
+           "position_embedding": sd[p + "embeddings.position_embedding.weight"],
+           "proj.weight": sd["visual_projection.weight"]}
+    for d, k in (("pre_layrnorm", "pre_ln"), ("post_layernorm", "post_ln")):
+        for s in ("weight", "bias"):
+            out[f"{k}.{s}"] = sd[f"{p}{d}.{s}"]
+    for i in sorted(layers):
+        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
+        for d, k in _CLIP_V_LAYER.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], head_dim)
     return out

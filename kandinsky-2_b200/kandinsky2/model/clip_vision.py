@@ -1,0 +1,258 @@
+"""The CLIP image tower of the Kandinsky 2.2 prior pipeline: a transformers `CLIPVisionModelWithProjection` (ViT-bigG/14 in
+`kandinsky-2-2-prior/image_encoder`), which the reference builds at `kandinsky2_2_model.py:24` and diffusers runs for the
+default decoder negative (`get_zero_embed`), the image items of `interpolate` and the PIL images of the emb2emb prior.
+
+The tower is read from the checkpoint's `config.json` (hidden 1664, 48 layers, 16 heads of 104, MLP 8192, patch 14, image 224,
+projection 1280, exact GELU for ViT-bigG/14); what is not implemented is refused with K2Error: any `hidden_act` but "gelu", any
+head width but 104.  Compute, per batch size one LaunchPlan replayed as one CUDA graph:
+    k2_clip_patchify -> ONE GEMM: patch conv + class embedding (K column 3 P^2) + position embedding (the epilogue residual),
+    pre_layrnorm, then per layer  LayerNorm -> qkv GEMM (q / k / v packed per head) -> k2_attention_heads -> out_proj GEMM +
+    residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual,
+    post_layernorm on the CLS rows (a strided view), fp16 -> fp32, and the bias-free visual_projection in fp32 (ops.linear).
+fp16 storage, fp32 accumulation, fp32 softmax with P rounded to fp16 before PV, the prior's LayerNorm statistics.
+
+Parity: tests/test_cpu_clip_vision.py pins the oracle (tests/clip_vision_oracle.py) and `preprocess` to transformers
+(tests/golden/clip_vision_tiny.pt); tests/test_gpu_zz_clip_vision.py runs the tower against the golden and, at full size on
+synthetic weights, against the fp32 oracle.
+"""
+import math
+
+import numpy as np
+import torch
+
+from .. import ops
+from .._native import K2Error
+from ..launch_plan import LaunchPlan
+
+OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
+OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+# CLIPImageProcessor as kandinsky-2-2-prior's image_processor configures it (transformers' defaults for CLIP)
+DEFAULT_PREPROCESSOR = dict(do_convert_rgb=True, do_resize=True, size={"shortest_edge": 224}, resample=3, do_center_crop=True,
+                            crop_size={"height": 224, "width": 224}, do_rescale=True, rescale_factor=1 / 255, do_normalize=True,
+                            image_mean=list(OPENAI_CLIP_MEAN), image_std=list(OPENAI_CLIP_STD))
+_REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "image_size", "patch_size",
+             "projection_dim")
+
+
+def tower_config(config):
+    """The transformers CLIPVisionConfig dict -> the geometry this module implements; K2Error for anything else.  A key that
+    is absent takes transformers' default (hidden_act "quick_gelu", layer_norm_eps 1e-5, num_channels 3)."""
+    missing = [k for k in _REQUIRED if k not in config]
+    if missing:
+        raise K2Error(f"CLIP vision config: missing {missing}")
+    c = {k: int(config[k]) for k in _REQUIRED}
+    c["hidden_act"] = config.get("hidden_act", "quick_gelu")
+    c["layer_norm_eps"] = float(config.get("layer_norm_eps", 1e-5))
+    if c["hidden_act"] != "gelu":
+        raise K2Error(f"CLIP vision tower: hidden_act {c['hidden_act']!r} is not implemented (only the exact 'gelu' of "
+                      "ViT-bigG/14; the 2.1 tower's quick_gelu is not)")
+    if int(config.get("num_channels", 3)) != 3:
+        raise K2Error("CLIP vision tower: only 3-channel images are implemented")
+    H, heads = c["hidden_size"], c["num_attention_heads"]
+    if H % heads or H // heads != 104:
+        raise K2Error(f"CLIP vision tower: head width {H / heads:g} is not implemented (only 104, ViT-bigG/14)")
+    if c["image_size"] % c["patch_size"]:
+        raise K2Error("CLIP vision tower: image_size must be a multiple of patch_size")
+    c["head_dim"] = 104
+    c["tokens"] = (c["image_size"] // c["patch_size"]) ** 2 + 1
+    c["kp"] = (3 * c["patch_size"] ** 2 + 1 + 63) // 64 * 64
+    return c
+
+
+def preprocess_images(images, config=None):
+    """CLIPImageProcessor (transformers' PIL backend, restated) -> fp32 [B, 3, crop, crop] on the CPU.  Per image: convert to
+    RGB (RGBA drops alpha, L is replicated), resize the shortest edge to size["shortest_edge"] with the long edge
+    int(S * long / short) (PIL, `resample`), center-crop at ((h - ch) // 2, (w - cw) // 2) (zero-padded if smaller), then
+    float32(uint8 * rescale_factor in float64), then (x - mean) / std in float32.  config: a preprocessor_config.json dict
+    (defaults: DEFAULT_PREPROCESSOR)."""
+    from PIL import Image
+    cfg = dict(DEFAULT_PREPROCESSOR)
+    cfg.update(config or {})
+    if isinstance(images, Image.Image):
+        images = [images]
+    out = []
+    for img in images:
+        if cfg["do_convert_rgb"] and img.mode != "RGB":
+            img = img.convert("RGB")
+        if cfg["do_resize"]:
+            S = int(cfg["size"]["shortest_edge"])
+            w, h = img.size
+            short, long = (w, h) if w <= h else (h, w)
+            new_long = int(S * long / short)
+            nh, nw = (new_long, S) if w <= h else (S, new_long)
+            img = img.resize((nw, nh), resample=int(cfg["resample"]))
+        a = np.array(img)
+        if a.ndim == 2:
+            a = a[:, :, None]
+        a = a.transpose(2, 0, 1)
+        if cfg["do_center_crop"]:
+            ch, cw = int(cfg["crop_size"]["height"]), int(cfg["crop_size"]["width"])
+            a = _center_crop(a, ch, cw)
+        x = a
+        if cfg["do_rescale"]:
+            x = (x.astype(np.float64) * cfg["rescale_factor"]).astype(np.float32)
+        if cfg["do_normalize"]:
+            x = x.astype(np.float32) if not np.issubdtype(x.dtype, np.floating) else x
+            mean = np.array(cfg["image_mean"], dtype=x.dtype)
+            std = np.array(cfg["image_std"], dtype=x.dtype)
+            x = ((x.T - mean) / std).T
+        out.append(torch.from_numpy(np.ascontiguousarray(x)).float())
+    return torch.stack(out)
+
+
+def _center_crop(a, ch, cw):
+    """transformers' image_transforms.center_crop on a CHW array."""
+    h, w = a.shape[1:]
+    top, left = (h - ch) // 2, (w - cw) // 2
+    if top >= 0 and left >= 0 and top + ch <= h and left + cw <= w:
+        return a[:, top:top + ch, left:left + cw]
+    nh, nw = max(ch, h), max(cw, w)
+    big = np.zeros((a.shape[0], nh, nw), dtype=a.dtype)
+    tp, lp = math.ceil((nh - h) / 2), math.ceil((nw - w) / 2)
+    big[:, tp:tp + h, lp:lp + w] = a
+    top, left = top + tp, left + lp
+    return big[:, max(0, top):min(nh, top + ch), max(0, left):min(nw, left + cw)]
+
+
+class CLIPVisionTower:
+    """CLIPVisionModelWithProjection on this package's kernels.  sd: state dict in this module's names
+    (checkpoints.transformers_clip_vision_to_k2); config: the transformers config.json dict; preprocessor_config: the
+    image processor's dict (None = DEFAULT_PREPROCESSOR)."""
+
+    def __init__(self, sd, config, device="cuda", preprocessor_config=None):
+        c = tower_config(config)
+        self.cfg, self.device = c, torch.device(device)
+        self.preprocessor_config = preprocessor_config
+        H, I, P, T, L = c["hidden_size"], c["intermediate_size"], c["patch_size"], c["tokens"], c["num_hidden_layers"]
+        want = {"class_embedding": (H,), "patch_embedding.weight": (H, 3, P, P), "position_embedding": (T, H),
+                "pre_ln.weight": (H,), "pre_ln.bias": (H,), "post_ln.weight": (H,), "post_ln.bias": (H,),
+                "proj.weight": (c["projection_dim"], H)}
+        for i in range(L):
+            for name, shape in (("ln_1.weight", (H,)), ("ln_1.bias", (H,)), ("ln_2.weight", (H,)), ("ln_2.bias", (H,)),
+                                ("attn.qkv.weight", (3 * H, H)), ("attn.qkv.bias", (3 * H,)), ("attn.proj.weight", (H, H)),
+                                ("attn.proj.bias", (H,)), ("mlp.fc1.weight", (I, H)), ("mlp.fc1.bias", (I,)),
+                                ("mlp.fc2.weight", (H, I)), ("mlp.fc2.bias", (H,))):
+                want[f"layers.{i}.{name}"] = shape
+        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
+        extra = sorted(set(sd) - set(want))
+        if bad or extra:
+            raise K2Error(f"CLIP vision tower: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
+        self.sd = sd
+        self._packed = None
+        self._plans = {}
+
+    @classmethod
+    def from_transformers(cls, state_dict, config, device="cuda", preprocessor_config=None):
+        """From a transformers CLIPVisionModelWithProjection state dict and its config.json dict; packs the weights."""
+        from ..checkpoints import transformers_clip_vision_to_k2
+        c = tower_config(config)
+        sd = transformers_clip_vision_to_k2(state_dict, head_dim=c["head_dim"])
+        return cls(sd, config, device, preprocessor_config).finalize()
+
+    def finalize(self):
+        """Pack the weights on the device once: fp16 GEMM weights [N, K] (the patch embedding as [H, Kp] with the class
+        embedding in column 3 P^2), fp32 biases / LayerNorm parameters / projection, the fp16 position embedding."""
+        c, dev, sd = self.cfg, self.device, self.sd
+        H, P, kp = c["hidden_size"], c["patch_size"], c["kp"]
+        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+        K = 3 * P * P
+        we = torch.zeros(H, kp, dtype=torch.float16, device=dev)
+        we[:, :K] = sd["patch_embedding.weight"].detach().to(dev).reshape(H, K).half()
+        we[:, K] = sd["class_embedding"].detach().to(dev).half()
+        pk = {"embed": we, "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
+              "pre_ln": (f32(sd["pre_ln.weight"]), f32(sd["pre_ln.bias"])),
+              "post_ln": (f32(sd["post_ln.weight"]), f32(sd["post_ln.bias"])), "proj": f32(sd["proj.weight"])}
+        for i in range(c["num_hidden_layers"]):
+            p = f"layers.{i}."
+            pk[i] = {"ln_1": (f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])),
+                     "ln_2": (f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"]))}
+            for name in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2"):
+                pk[i][name] = (ops.pack_conv_weight(sd[p + name + ".weight"].detach().to(dev)), f32(sd[p + name + ".bias"]))
+        self._packed = pk
+        self._plans = {}
+        return self
+
+    def _plan(self, B):
+        if self._packed is None:
+            self.finalize()
+        if B not in self._plans:
+            self._plans[B] = _TowerPlan(self, B)
+        return self._plans[B]
+
+    def preprocess(self, images):
+        """PIL image(s) -> fp32 pixel_values [B, 3, S, S] on the CPU (preprocess_images with this tower's processor config)."""
+        return preprocess_images(images, self.preprocessor_config)
+
+    @torch.no_grad()
+    def forward(self, pixel_values, use_graph=True):
+        """pixel_values fp32 [B, 3, S, S] -> (last_hidden_state fp16 [B, T, hidden], image_embeds fp32 [B, projection_dim]), on
+        the device.  One CUDA graph replay of the batch size's launch plan (use_graph=False: the same launches one by one)."""
+        S = self.cfg["image_size"]
+        if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
+            raise K2Error(f"CLIP vision tower: pixel_values must be [B, 3, {S}, {S}], got {list(pixel_values.shape)}")
+        plan = self._plan(pixel_values.shape[0])
+        plan.pix.copy_(pixel_values)
+        plan.run(use_graph)
+        return plan.hidden.clone(), plan.out.clone()
+
+    def image_embeds(self, pixel_values, use_graph=True):
+        """pixel_values fp32 [B, 3, S, S] -> image_embeds fp32 [B, projection_dim] on the device."""
+        return self.forward(pixel_values, use_graph)[1]
+
+    def __call__(self, image):
+        """The embedders' clip_image protocol: a PIL image -> fp32 [1, projection_dim] on the CPU."""
+        return self.image_embeds(self.preprocess(image).to(self.device)).float().cpu()
+
+    def zero_embed(self):
+        """diffusers' get_zero_embed: the tower on an all-zero pixel_values tensor [1, 3, S, S] (zeros after normalisation,
+        not a black image) -> fp32 [1, projection_dim] on the device."""
+        S = self.cfg["image_size"]
+        return self.image_embeds(torch.zeros(1, 3, S, S, device=self.device))
+
+
+class _TowerPlan(LaunchPlan):
+    """The tower at B images as one static launch list over fixed buffers (replayed as one CUDA graph): pix -> patchify ->
+    embedding GEMM (+ position embedding, tiled over the batch once here) -> pre LayerNorm -> L layers -> post LayerNorm of the
+    CLS rows -> fp32 -> projection.  self.hidden is the last layer's output (transformers' last_hidden_state), self.out the
+    image embeddings."""
+
+    def __init__(self, tower, B):
+        super().__init__(tower.device, B)
+        self.t, self.B = tower, B
+        c = tower.cfg
+        S, T, H = c["image_size"], c["tokens"], c["hidden_size"]
+        self.pix = torch.zeros(B, 3, S, S, device=self.dev, dtype=torch.float32)
+        self.pos = tower._packed["pos"].expand(B, T, H).contiguous()
+        self.out = torch.zeros(B, c["projection_dim"], device=self.dev, dtype=torch.float32)
+        self._build()
+
+    def _build(self):
+        c, pk, B, S = self.t.cfg, self.t._packed, self.B, self._add
+        T, H, I, hd, heads, eps = (c["tokens"], c["hidden_size"], c["intermediate_size"], c["head_dim"], c["num_attention_heads"],
+                                   c["layer_norm_eps"])
+        M = B * T
+        rows = self._new(B, T, c["kp"])
+        S(lambda: ops.clip_patchify(self.pix, c["patch_size"], c["kp"], out=rows), "patchify")
+        emb, x = self._new(B, T, H), self._new(B, T, H)
+        self._gemm(rows, pk["embed"], H, emb, 2 * M * c["kp"] * H, residual=self.pos)
+        S(lambda: ops.layernorm_f16(emb, *pk["pre_ln"], eps=eps, out=x), "layernorm")
+        y, att, hA, hB = (self._new(B, T, H) for _ in range(4))
+        qkv, f = self._new(B, T, 3 * H), self._new(B, T, I)
+        scale = hd ** -0.5
+        h = x
+        for i in range(c["num_hidden_layers"]):
+            L = pk[i]
+            S(lambda h=h, L=L: ops.layernorm_f16(h, *L["ln_1"], eps=eps, out=y), "layernorm")
+            self._gemm(y, L["attn.qkv"][0], 3 * H, qkv, 2 * M * H * 3 * H, bias=L["attn.qkv"][1])
+            S(lambda: ops.attention_heads(qkv, heads, hd, scale, out=att), "attention", 4 * B * heads * T * T * hd)
+            self._gemm(att, L["attn.proj"][0], H, hA, 2 * M * H * H, bias=L["attn.proj"][1], residual=h)
+            S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
+            self._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * H * I, bias=L["mlp.fc1"][1])
+            S(lambda: ops.gelu_f16_(f), "gelu")
+            self._gemm(f, L["mlp.fc2"][0], H, hB, 2 * M * I * H, bias=L["mlp.fc2"][1], residual=hA)
+            h = hB
+        self.hidden = h
+        cls, cls32 = self._new(B, H), torch.empty(B, H, device=self.dev, dtype=torch.float32)
+        S(lambda: ops.layernorm_f16(h[:, 0], *pk["post_ln"], eps=eps, out=cls), "layernorm")
+        S(lambda: ops.f16_to_f32(cls, out=cls32), "widen")
+        S(lambda: ops.linear(cls32, pk["proj"], out=self.out), "linear", 2 * B * H * c["projection_dim"])

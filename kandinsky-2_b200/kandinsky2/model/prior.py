@@ -485,9 +485,17 @@ class PriorEmbedder22:
         self._zero = zero_image_emb
 
     @classmethod
-    def from_diffusers(cls, state_dict, clip_text, device="cuda", **kwargs):
+    def from_diffusers(cls, state_dict, clip_text, device="cuda", image_encoder=None, **kwargs):
         """Build from a diffusers `PriorTransformer` state dict (kandinsky-community/kandinsky-2-2-prior, subfolder `prior`)
-        via checkpoints.diffusers_prior_to_k2; the configuration is read from the tensor shapes."""
+        via checkpoints.diffusers_prior_to_k2; the configuration is read from the tensor shapes.  image_encoder: the pipeline's
+        CLIP image tower (model.clip_vision.CLIPVisionTower) or None.  A tower becomes clip_image and, unless zero_image_emb is
+        passed, supplies it as the tower on all-zero pixel_values, computed here once (diffusers' get_zero_embed)."""
+        if image_encoder is not None:
+            if kwargs.get("clip_image") is not None:
+                raise ValueError("PriorEmbedder22.from_diffusers: pass image_encoder= or clip_image=, not both")
+            kwargs["clip_image"] = image_encoder
+            if kwargs.get("zero_image_emb") is None:
+                kwargs["zero_image_emb"] = image_encoder.zero_embed().float().cpu()
         from ..checkpoints import diffusers_prior_to_k2
         sd, mean, std = diffusers_prior_to_k2(state_dict)
         W = sd["positional_embedding"].shape[-1]
@@ -560,8 +568,8 @@ class PriorEmbedder22:
                               use_graph=self.use_cuda_graph, keep=keep).float().cpu()
 
     def zero_image_emb(self, batch_size):
-        """CLIP embedding of a black image (diffusers' KandinskyV22PriorPipeline.get_zero_embed): supplied by the deployment
-        (it needs the CLIP vision tower); zeros when absent."""
+        """diffusers' KandinskyV22PriorPipeline.get_zero_embed: the CLIP image tower on all-zero pixel_values, supplied by the
+        deployment or by from_diffusers(image_encoder=...); zeros when absent."""
         z = self._zero if self._zero is not None else torch.zeros(1, self.prior.clip_dim)
         return z.reshape(1, -1).float().cpu().repeat(batch_size, 1)
 

@@ -632,3 +632,40 @@ def f16_to_f32(x, out=None):
     assert (my, ny) == (M, N), (tuple(x.shape), tuple(out.shape))
     check(nat.load().k2_f16_to_f32(ptr(x), ldx, ptr(out), ldy, M, N, stream_ptr()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# CLIP image tower (kandinsky2/model/clip_vision.py, see k2b200.h)
+# ------------------------------------------------------------------------------------------------
+def clip_patchify(x, patch, kp, out=None):
+    """k2_clip_patchify: fp32 NCHW pixels [B, 3, S, S] -> fp16 GEMM rows [B, (S / patch)^2 + 1, kp] (out may be row-strided):
+    the one-hot CLS row, then each patch's pixels in (c, ky, kx) order, zero-padded to kp columns."""
+    if not x.is_cuda or (out is not None and not out.is_cuda):
+        raise nat.K2Error("clip_patchify: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3 and x.shape[2] == x.shape[3] and x.is_contiguous(), \
+        (x.dtype, tuple(x.shape))
+    B, S = x.shape[0], x.shape[2]
+    T = (S // patch) ** 2 + 1
+    if out is None:
+        out = torch.empty((B, T, kp), dtype=torch.float16, device=x.device)
+    assert out.dtype == torch.float16 and tuple(out.shape) == (B, T, kp), (out.dtype, tuple(out.shape))
+    check(nat.load().k2_clip_patchify(ptr(x), B, S, patch, ptr(out), _row_stride(out), kp, stream_ptr()))
+    return out
+
+
+def attention_heads(qkv, heads, head_dim, scale, out=None, hs=None, q_off=0, k_off=None, v_off=None, ohs=None):
+    """k2_attention_heads: qkv fp16 [B, T, >= heads * hs] with per-head [q | k | v] (hs = 3 head_dim, offsets 0 / head_dim /
+    2 head_dim by default: checkpoints.pack_heads) -> fp16 [B, T, heads * head_dim] (out may be a row-strided view whose heads
+    are ohs apart).  head_dim 104 only (the library refuses anything else)."""
+    hs = 3 * head_dim if hs is None else hs
+    k_off = head_dim if k_off is None else k_off
+    v_off = 2 * head_dim if v_off is None else v_off
+    ohs = head_dim if ohs is None else ohs
+    assert qkv.dtype == torch.float16 and qkv.dim() == 3, (qkv.dtype, tuple(qkv.shape))
+    B, T = qkv.shape[:2]
+    if out is None:
+        out = torch.empty((B, T, heads * ohs), dtype=torch.float16, device=qkv.device)
+    assert out.dtype == torch.float16 and out.dim() == 3 and tuple(out.shape[:2]) == (B, T), (out.dtype, tuple(out.shape))
+    check(nat.load().k2_attention_heads(ptr(qkv), _row_stride(qkv), hs, q_off, k_off, v_off, B, heads, T, head_dim,
+                                        float(scale), ptr(out), _row_stride(out), ohs, stream_ptr()))
+    return out
