@@ -365,6 +365,28 @@ int k2_attention_heads(const void* qkv, int ldq, int hs, int q_off, int k_off, i
                        float scale, void* out, int ldo, int ohs, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * CLIP text tower (diffusers' KandinskyV22PriorPipeline text_encoder, a transformers CLIPTextModelWithProjection;
+ * kandinsky2/model/clip_text.py).  Its Linear layers are k2_conv_gemm flat-row GEMMs, its attention is k2_attention_small
+ * (causal, no keep mask), its LayerNorm / GELU are the prior's entry points above; these two are the rest.
+ *
+ * k2_clip_text_embed: ids int32 [B, ldi] (T used per row), tok fp16 [V, H], pos fp16 [>= T, H] (both contiguous) ->
+ *   out fp16 rows [B * T, ldo]:  out[b T + t, c] = fp16_rn( float(tok[ids[b, t], c]) + float(pos[t, c]) ),  c < H
+ *   (the fp16 model's inputs_embeds + position_embeds, one rounding).  An id outside [0, V) writes a NaN row and reads no
+ *   table.  H % 8 == 0, ldo >= H and a multiple of 8, tok / pos / out 16-byte aligned, ids 4-byte aligned; columns >= H are
+ *   not touched.
+ * k2_clip_text_pool: per sequence b the pooled position p_b, from the ids on the device:
+ *     eos_id < 0:   the first t with ids[b, t] == max_t ids[b, t]   (transformers' eos_token_id == 2 rule, argmax)
+ *     eos_id >= 0:  the first t with ids[b, t] == eos_id, or 0 if there is none
+ *   then out[b, c] = float(hidden[(b T + p_b) ldh + c]) exactly (c < H), fp32 rows with stride ldo; index_out int32 [B] (may be
+ *   NULL) receives p_b.  ldi >= T, ldh >= H, ldo >= H; ids / out / index_out 4-byte and hidden 2-byte aligned.
+ * Both check their arguments before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+int k2_clip_text_embed(const int* ids, int ldi, int B, int T, const void* tok, int V, const void* pos, int H, void* out, int ldo,
+                       k2_stream_t stream);
+int k2_clip_text_pool(const int* ids, int ldi, int B, int T, int eos_id, const void* hidden, int ldh, int H, float* out, int ldo,
+                      int* index_out, k2_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
  * fuse_lora): once per adapter load, never per step.
  *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols

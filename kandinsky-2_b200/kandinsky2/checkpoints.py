@@ -17,7 +17,9 @@
 * Kandinsky 2.2's prior pipeline carries a CLIP image tower, a transformers `CLIPVisionModelWithProjection`
   (`kandinsky2_2_model.py:24`, subfolder `image_encoder`).  `transformers_clip_vision_to_k2` renames it into
   `model.clip_vision.CLIPVisionTower` names and packs q / k / v per head (tests/test_cpu_clip_vision.py pins it through the
-  network against the transformers-name forward and transformers' own outputs).
+  network against the transformers-name forward and transformers' own outputs).  Its text tower, a transformers
+  `CLIPTextModelWithProjection` (subfolder `text_encoder`), goes the same way through `transformers_clip_text_to_k2` into
+  `model.clip_text.CLIPTextTower` names (tests/test_cpu_clip_text.py).
 
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
@@ -315,4 +317,45 @@ def transformers_clip_vision_to_k2(sd, head_dim=104):
                 out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
         for s in ("weight", "bias"):
             out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], head_dim)
+    return out
+
+
+def transformers_clip_text_keys(layers):
+    """Every key of a transformers `CLIPTextModelWithProjection` state dict with `layers` encoder layers (without the
+    `position_ids` buffer)."""
+    p = "text_model."
+    keys = [p + "embeddings.token_embedding.weight", p + "embeddings.position_embedding.weight"]
+    for i in range(layers):
+        lp = f"{p}encoder.layers.{i}."
+        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_V_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
+                 for s in ("weight", "bias")]
+    return keys + [f"{p}final_layer_norm.{s}" for s in ("weight", "bias")] + ["text_projection.weight"]
+
+
+def transformers_clip_text_to_k2(sd):
+    """transformers `CLIPTextModelWithProjection` state dict (the Kandinsky 2.2 prior's `text_encoder`) ->
+    `model.clip_text.CLIPTextTower` names:
+        token_embedding [V, H], position_embedding [T, H], final_ln.*, proj.weight,
+        layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}
+    where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads, head width 64).  A `position_ids`
+    buffer (older checkpoints carry it) is ignored; unknown and missing keys raise K2Error naming them."""
+    p = "text_model."
+    sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
+    layers = {int(m.group(1)) for m in (re.match(r"^text_model\.encoder\.layers\.(\d+)\.", k) for k in sd) if m}
+    expected = transformers_clip_text_keys(max(layers) + 1 if layers else 0)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"transformers CLIP text state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {"token_embedding": sd[p + "embeddings.token_embedding.weight"],
+           "position_embedding": sd[p + "embeddings.position_embedding.weight"],
+           "final_ln.weight": sd[p + "final_layer_norm.weight"], "final_ln.bias": sd[p + "final_layer_norm.bias"],
+           "proj.weight": sd["text_projection.weight"]}
+    for i in sorted(layers):
+        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
+        for d, k in _CLIP_V_LAYER.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], 64)
     return out

@@ -1,0 +1,429 @@
+"""The CLIP text side of the Kandinsky 2.2 prior pipeline: the tokenizer and the transformers `CLIPTextModelWithProjection`
+(ViT-bigG/14 text in `kandinsky-2-2-prior/text_encoder`) that diffusers' `KandinskyV22PriorPipeline._encode_prompt` runs for
+every prompt of every 2.2 method.
+
+The tower is read from the checkpoint's `config.json` (hidden 1280, 32 layers, 20 heads of 64, MLP 5120, 77 positions,
+vocabulary 49408, projection 1280, exact GELU expected for ViT-bigG/14); what is not implemented is refused with K2Error: any
+`hidden_act` but "gelu", any head width but 64 (so the hidden size is a multiple of 8), more than 128 positions.  Compute, per
+(row count, length) one LaunchPlan replayed as one CUDA graph:
+    k2_clip_text_embed (token + position embedding, one fp16 rounding), then per layer  LayerNorm -> qkv GEMM (q / k / v
+    packed per head) -> k2_attention_small (causal, no key mask: diffusers calls the encoder without attention_mask) ->
+    out_proj GEMM + residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual,
+    final_layer_norm over every row (last_hidden_state), k2_clip_text_pool (the pooled row, chosen on the device from the ids
+    by the config's eos_token_id rule, widened to fp32) and the bias-free text_projection in fp32 (ops.linear).
+fp16 storage, fp32 accumulation, the prior's LayerNorm statistics and attention.
+
+CLIPTokenizer restates transformers 5's CLIPTokenizer (the `tokenizers` backend) in the standard library only.
+
+Parity: tests/test_cpu_clip_text.py pins the oracle (tests/clip_text_oracle.py) and the tokenizer to transformers
+(tests/golden/clip_text_tiny.pt); tests/test_gpu_zz_clip_text.py runs the tower against the golden and, at full size on
+synthetic weights, against the fp32 oracle.
+"""
+import json
+import os
+import unicodedata
+
+import torch
+
+from .. import ops
+from .._native import K2Error
+from ..launch_plan import LaunchPlan
+
+_REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "max_position_embeddings",
+             "vocab_size", "projection_dim")
+MAX_TOKENS = 128   # k2_attention_small's sequence limit
+
+
+def text_tower_config(config):
+    """The transformers CLIPTextConfig dict -> the geometry this module implements; K2Error for anything else.  A key that is
+    absent takes transformers' default (hidden_act "quick_gelu", layer_norm_eps 1e-5, eos_token_id 49407).  "pool_eos" is the
+    pooling rule: -1 for eos_token_id == 2 (the first argmax of the ids, pre-#24773 configs), else the eos id."""
+    missing = [k for k in _REQUIRED if k not in config]
+    if missing:
+        raise K2Error(f"CLIP text config: missing {missing}")
+    c = {k: int(config[k]) for k in _REQUIRED}
+    c["hidden_act"] = config.get("hidden_act", "quick_gelu")
+    c["layer_norm_eps"] = float(config.get("layer_norm_eps", 1e-5))
+    c["eos_token_id"] = int(config.get("eos_token_id", 49407))
+    if c["hidden_act"] != "gelu":
+        raise K2Error(f"CLIP text tower: hidden_act {c['hidden_act']!r} is not implemented (only the exact 'gelu' of "
+                      "ViT-bigG/14; the 2.1 tower's quick_gelu is not)")
+    H, heads = c["hidden_size"], c["num_attention_heads"]
+    if H % heads or H // heads != 64:
+        raise K2Error(f"CLIP text tower: head width {H / heads:g} is not implemented (only 64)")
+    # heads of 64 make hidden_size a multiple of 8, which k2_clip_text_embed's 16-byte rows need
+    if not 0 < c["max_position_embeddings"] <= MAX_TOKENS:
+        raise K2Error(f"CLIP text tower: max_position_embeddings {c['max_position_embeddings']} is not implemented "
+                      f"(at most {MAX_TOKENS} tokens)")
+    c["head_dim"] = 64
+    c["pool_eos"] = -1 if c["eos_token_id"] == 2 else c["eos_token_id"]
+    return c
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# tokenizer
+# ---------------------------------------------------------------------------------------------------------------------------
+# Unicode White_Space (what the tokenizers regex engine's \s matches; Python's str.isspace adds U+001C..U+001F)
+_WS = frozenset("\t\n\x0b\x0c\r \x85\xa0\u1680\u2000\u2001\u2002\u2003\u2004\u2005\u2006\u2007\u2008\u2009"
+                "\u200a\u2028\u2029\u202f\u205f\u3000")
+_CONTRACTIONS = ("'s", "'t", "'re", "'ve", "'m", "'ll", "'d")
+_CLIP_SPECIALS = ("<|startoftext|>", "<|endoftext|>")
+
+
+def bytes_to_unicode():
+    """GPT-2's reversible byte -> printable character map (the ByteLevel pre-tokenizer's alphabet)."""
+    bs = list(range(ord("!"), ord("~") + 1)) + list(range(ord("¡"), ord("¬") + 1)) + list(range(ord("®"), ord("ÿ") + 1))
+    cs = bs[:]
+    n = 0
+    for b in range(256):
+        if b not in bs:
+            bs.append(b)
+            cs.append(256 + n)
+            n += 1
+    return dict(zip(bs, map(chr, cs)))
+
+
+def _is_letter(ch):
+    return unicodedata.category(ch)[0] == "L"
+
+
+def _is_number(ch):
+    return unicodedata.category(ch)[0] == "N"
+
+
+def _clip_split(text):
+    """The CLIP pre-tokenizer's Split (matches kept, the rest removed):
+    <|startoftext|>|<|endoftext|>|'s|'t|'re|'ve|'m|'ll|'d|[\\p{L}]+|[\\p{N}]|[^\\s\\p{L}\\p{N}]+  (leftmost-first)."""
+    out, i, n = [], 0, len(text)
+    while i < n:
+        m = next((s for s in _CLIP_SPECIALS + _CONTRACTIONS if text.startswith(s, i)), None)
+        if m is not None:
+            out.append(m)
+            i += len(m)
+            continue
+        ch = text[i]
+        if _is_letter(ch):
+            j = i + 1
+            while j < n and _is_letter(text[j]):
+                j += 1
+        elif _is_number(ch):
+            j = i + 1
+        elif ch not in _WS:
+            j = i + 1
+            while j < n and not (text[j] in _WS or _is_letter(text[j]) or _is_number(text[j])):
+                j += 1
+        else:
+            i += 1
+            continue
+        out.append(text[i:j])
+        i = j
+    return out
+
+
+def _byte_level_split(piece):
+    """The ByteLevel pre-tokenizer's own GPT-2 split of one CLIP piece (no whitespace inside):
+    's|'t|'re|'ve|'m|'ll|'d| ?\\p{L}+| ?\\p{N}+| ?[^\\s\\p{L}\\p{N}]+.  It only changes the special-token pieces:
+    "<|endoftext|>" -> "<|", "endoftext", "|>"."""
+    out, i, n = [], 0, len(piece)
+    while i < n:
+        m = next((s for s in _CONTRACTIONS if piece.startswith(s, i)), None)
+        if m is not None:
+            out.append(m)
+            i += len(m)
+            continue
+        cls = _is_letter if _is_letter(piece[i]) else _is_number if _is_number(piece[i]) else None
+        j = i + 1
+        if cls is not None:
+            while j < n and cls(piece[j]):
+                j += 1
+        else:
+            while j < n and not (piece[j] in _WS or _is_letter(piece[j]) or _is_number(piece[j])):
+                j += 1
+        out.append(piece[i:j])
+        i = j
+    return out
+
+
+class CLIPTokenizer:
+    """transformers 5's CLIPTokenizer (the `tokenizers` backend: tokenization_clip.py), restated with the standard library:
+      1. added (special) tokens are matched in the raw text first, leftmost-longest, case-sensitively;
+      2. the rest is normalised: NFC, runs of Unicode White_Space -> " ", then each character lowercased on its own (no
+         final-sigma rule);
+      3. split by the CLIP pattern, then by ByteLevel's GPT-2 pattern; each piece's UTF-8 bytes are mapped to
+         bytes_to_unicode characters;
+      4. BPE per piece with "</w>" on its last symbol, merging the lowest-ranked adjacent pair (leftmost first) until none
+         is left; a symbol missing from the vocabulary becomes unk;
+      5. [bos] + tokens[:max_length - 2] + [eos], right-padded with pad to max_length, and the attention mask.
+    vocab: {token: id}; merges: [(a, b)] in rank order."""
+
+    def __init__(self, vocab, merges, bos_token="<|startoftext|>", eos_token="<|endoftext|>", unk_token="<|endoftext|>",
+                 pad_token="<|endoftext|>", model_max_length=77, added_tokens=()):
+        self.vocab = dict(vocab)
+        self.ranks = {tuple(m): r for r, m in enumerate(merges)}
+        self.model_max_length = int(model_max_length)
+        for name, tok in (("bos", bos_token), ("eos", eos_token), ("unk", unk_token), ("pad", pad_token)):
+            if tok not in self.vocab:
+                raise K2Error(f"CLIPTokenizer: the {name} token {tok!r} is not in the vocabulary")
+        self.bos_token_id, self.eos_token_id = self.vocab[bos_token], self.vocab[eos_token]
+        self.unk_token_id, self.pad_token_id = self.vocab[unk_token], self.vocab[pad_token]
+        self.special = sorted({bos_token, eos_token, unk_token, pad_token, *added_tokens}, key=len, reverse=True)
+        self.byte_map = bytes_to_unicode()
+        self._cache = {}
+
+    @classmethod
+    def from_dir(cls, path):
+        """A transformers tokenizer folder: vocab.json, merges.txt, and special_tokens_map.json / tokenizer_config.json when
+        present (special tokens, the pad token, model_max_length; without one, model_max_length is 77)."""
+        def read_json(name, required):
+            f = os.path.join(path, name)
+            if not os.path.exists(f):
+                if required:
+                    raise K2Error(f"CLIPTokenizer: {f} not found")
+                return {}
+            with open(f, encoding="utf-8") as fh:
+                return json.load(fh)
+
+        vocab = read_json("vocab.json", True)
+        mf = os.path.join(path, "merges.txt")
+        if not os.path.exists(mf):
+            raise K2Error(f"CLIPTokenizer: {mf} not found")
+        with open(mf, encoding="utf-8") as fh:
+            lines = fh.read().split("\n")
+        merges = [tuple(ln.split(" ")) for ln in lines if ln and not ln.startswith("#version")]
+        kw = {}
+        cfg = read_json("tokenizer_config.json", False)
+        cfg.update(read_json("special_tokens_map.json", False))
+        for k in ("bos_token", "eos_token", "unk_token", "pad_token"):
+            v = cfg.get(k)
+            if v is not None:
+                kw[k] = v["content"] if isinstance(v, dict) else v
+        if cfg.get("model_max_length") is not None and int(cfg["model_max_length"]) <= 1 << 20:
+            kw["model_max_length"] = int(cfg["model_max_length"])
+        added = [v["content"] for v in cfg.get("added_tokens_decoder", {}).values() if isinstance(v, dict) and "content" in v]
+        return cls(vocab, merges, added_tokens=added, **kw)
+
+    # -- steps ------------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def normalize(text):
+        text = unicodedata.normalize("NFC", text)
+        out, prev_ws = [], False
+        for ch in text:
+            if ch in _WS:
+                if not prev_ws:
+                    out.append(" ")
+                prev_ws = True
+            else:
+                out.append(ch.lower())
+                prev_ws = False
+        return "".join(out)
+
+    def _bpe(self, word):
+        """One pre-token (byte-level characters) -> vocabulary ids."""
+        hit = self._cache.get(word)
+        if hit is not None:
+            return hit
+        syms = list(word)
+        syms[-1] += "</w>"
+        while len(syms) > 1:
+            best, at = None, -1
+            for i in range(len(syms) - 1):
+                r = self.ranks.get((syms[i], syms[i + 1]))
+                if r is not None and (best is None or r < best):
+                    best, at = r, i
+            if best is None:
+                break
+            syms[at:at + 2] = [syms[at] + syms[at + 1]]
+        ids = [self.vocab.get(s, self.unk_token_id) for s in syms]
+        self._cache[word] = ids
+        return ids
+
+    def _split_special(self, text):
+        """[(segment, is_special)] with the added tokens matched leftmost-longest in the raw text."""
+        out, i, start, n = [], 0, 0, len(text)
+        while i < n:
+            m = next((s for s in self.special if text.startswith(s, i)), None)
+            if m is None:
+                i += 1
+                continue
+            if i > start:
+                out.append((text[start:i], False))
+            out.append((m, True))
+            i += len(m)
+            start = i
+        if start < n:
+            out.append((text[start:], False))
+        return out
+
+    def tokenize_ids(self, text):
+        """The token ids of one text, without bos / eos."""
+        ids = []
+        for seg, special in self._split_special(text):
+            if special:
+                ids.append(self.vocab[seg])
+                continue
+            for piece in _clip_split(self.normalize(seg)):
+                for word in _byte_level_split(piece):
+                    ids += self._bpe("".join(self.byte_map[b] for b in word.encode("utf-8")))
+        return ids
+
+    def __call__(self, texts, max_length=None):
+        """texts: str or list[str] -> dict(input_ids int64 [n, L], attention_mask int64 [n, L]) on the CPU, L = max_length
+        (default model_max_length): padding="max_length", truncation=True."""
+        if isinstance(texts, str):
+            texts = [texts]
+        L = self.model_max_length if max_length is None else int(max_length)
+        if L < 2:
+            raise K2Error(f"CLIPTokenizer: max_length {L} leaves no room for bos and eos")
+        ids = torch.full((len(texts), L), self.pad_token_id, dtype=torch.int64)
+        mask = torch.zeros(len(texts), L, dtype=torch.int64)
+        for r, t in enumerate(texts):
+            row = [self.bos_token_id] + self.tokenize_ids(t)[:L - 2] + [self.eos_token_id]
+            ids[r, :len(row)] = torch.tensor(row)
+            mask[r, :len(row)] = 1
+        return {"input_ids": ids, "attention_mask": mask}
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# tower
+# ---------------------------------------------------------------------------------------------------------------------------
+class CLIPTextTower:
+    """CLIPTextModelWithProjection on this package's kernels.  sd: state dict in this module's names
+    (checkpoints.transformers_clip_text_to_k2); config: the transformers config.json dict; tokenizer: a CLIPTokenizer (needed
+    by __call__ only).  `tokens` is the sequence length __call__ produces: the tokenizer's model_max_length, or
+    max_position_embeddings without a tokenizer."""
+
+    def __init__(self, sd, config, device="cuda", tokenizer=None):
+        c = text_tower_config(config)
+        self.cfg, self.device, self.tokenizer = c, torch.device(device), tokenizer
+        self.tokens = tokenizer.model_max_length if tokenizer is not None else c["max_position_embeddings"]
+        if not 2 <= self.tokens <= c["max_position_embeddings"]:
+            raise K2Error(f"CLIP text tower: the tokenizer's model_max_length {self.tokens} does not fit the "
+                          f"{c['max_position_embeddings']} positions")
+        if tokenizer is not None and max(tokenizer.vocab.values()) >= c["vocab_size"]:
+            raise K2Error(f"CLIP text tower: the tokenizer's ids reach {max(tokenizer.vocab.values())}, beyond the "
+                          f"vocabulary of {c['vocab_size']}")
+        H, I, L = c["hidden_size"], c["intermediate_size"], c["num_hidden_layers"]
+        want = {"token_embedding": (c["vocab_size"], H), "position_embedding": (c["max_position_embeddings"], H),
+                "final_ln.weight": (H,), "final_ln.bias": (H,), "proj.weight": (c["projection_dim"], H)}
+        for i in range(L):
+            for name, shape in (("ln_1.weight", (H,)), ("ln_1.bias", (H,)), ("ln_2.weight", (H,)), ("ln_2.bias", (H,)),
+                                ("attn.qkv.weight", (3 * H, H)), ("attn.qkv.bias", (3 * H,)), ("attn.proj.weight", (H, H)),
+                                ("attn.proj.bias", (H,)), ("mlp.fc1.weight", (I, H)), ("mlp.fc1.bias", (I,)),
+                                ("mlp.fc2.weight", (H, I)), ("mlp.fc2.bias", (H,))):
+                want[f"layers.{i}.{name}"] = shape
+        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
+        extra = sorted(set(sd) - set(want))
+        if bad or extra:
+            raise K2Error(f"CLIP text tower: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
+        self.sd = sd
+        self._packed = None
+        self._plans = {}
+
+    @classmethod
+    def from_transformers(cls, state_dict, config, device="cuda", tokenizer=None):
+        """From a transformers CLIPTextModelWithProjection state dict and its config.json dict; packs the weights."""
+        from ..checkpoints import transformers_clip_text_to_k2
+        text_tower_config(config)
+        return cls(transformers_clip_text_to_k2(state_dict), config, device, tokenizer).finalize()
+
+    def finalize(self):
+        """Pack the weights on the device once: fp16 GEMM weights [N, K], fp32 biases / LayerNorm parameters / projection, the
+        fp16 token and position tables."""
+        c, dev, sd = self.cfg, self.device, self.sd
+        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+        pk = {"tok": sd["token_embedding"].detach().to(dev).half().contiguous(),
+              "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
+              "final_ln": (f32(sd["final_ln.weight"]), f32(sd["final_ln.bias"])), "proj": f32(sd["proj.weight"])}
+        for i in range(c["num_hidden_layers"]):
+            p = f"layers.{i}."
+            pk[i] = {"ln_1": (f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])),
+                     "ln_2": (f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"]))}
+            for name in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2"):
+                pk[i][name] = (ops.pack_conv_weight(sd[p + name + ".weight"].detach().to(dev)), f32(sd[p + name + ".bias"]))
+        self._packed = pk
+        self._plans = {}
+        return self
+
+    def _plan(self, n, T=None):
+        if self._packed is None:
+            self.finalize()
+        key = (n, self.cfg["max_position_embeddings"] if T is None else T)
+        if key not in self._plans:
+            self._plans[key] = _TextPlan(self, *key)
+        return self._plans[key]
+
+    @torch.no_grad()
+    def forward(self, input_ids, use_graph=True):
+        """input_ids integer [n, T] (T <= max_position_embeddings) -> (last_hidden_state fp16 [n, T, hidden], text_embeds fp32
+        [n, projection_dim]), on the device.  One CUDA graph replay of the (n, T) launch plan (use_graph=False: the same
+        launches one by one).  Ids outside [0, vocab_size) are refused before anything is copied."""
+        c = self.cfg
+        if input_ids.dim() != 2 or not 0 < input_ids.shape[1] <= c["max_position_embeddings"] or input_ids.shape[0] == 0:
+            raise K2Error(f"CLIP text tower: input_ids must be [n, T] with 0 < T <= {c['max_position_embeddings']}, got "
+                          f"{list(input_ids.shape)}")
+        if input_ids.is_floating_point() or input_ids.is_complex() or input_ids.dtype == torch.bool:
+            raise K2Error(f"CLIP text tower: input_ids must be integers, got {input_ids.dtype}")
+        lo, hi = int(input_ids.min()), int(input_ids.max())
+        if lo < 0 or hi >= c["vocab_size"]:
+            raise K2Error(f"CLIP text tower: token ids must lie in [0, {c['vocab_size']}), got [{lo}, {hi}]")
+        plan = self._plan(*input_ids.shape)
+        plan.ids.copy_(input_ids)
+        plan.run(use_graph)
+        return plan.hidden.clone(), plan.out.clone()
+
+    def __call__(self, prompts):
+        """The embedders' clip_text protocol: list[str] -> (text_embeds fp32 [n, projection_dim], last_hidden_state fp16
+        [n, tokens, hidden], mask bool [n, tokens]), on the device.  Each distinct prompt is tokenized and encoded once and its
+        rows are gathered back (diffusers encodes a prompt once and repeats its rows)."""
+        if self.tokenizer is None:
+            raise K2Error("CLIP text tower: calling it with prompts needs tokenizer=")
+        if isinstance(prompts, str):
+            prompts = [prompts]
+        distinct = list(dict.fromkeys(prompts))
+        tok = self.tokenizer(distinct, max_length=self.tokens)
+        hid, emb = self.forward(tok["input_ids"])
+        idx = torch.tensor([distinct.index(p) for p in prompts], device=self.device)
+        mask = tok["attention_mask"].to(self.device).bool()
+        return emb[idx], hid[idx], mask[idx]
+
+
+class _TextPlan(LaunchPlan):
+    """The tower on n sequences of T tokens as one static launch list over fixed buffers (replayed as one CUDA graph): ids ->
+    embed -> L layers -> final LayerNorm (self.hidden, transformers' last_hidden_state) -> pool (fp32) -> projection (self.out).
+    self.index holds the pooled positions of the last run."""
+
+    def __init__(self, tower, n, T):
+        super().__init__(tower.device, n)
+        self.t, self.n, self.T = tower, n, T
+        self.ids = torch.zeros(n, T, device=self.dev, dtype=torch.int32)
+        self.index = torch.zeros(n, device=self.dev, dtype=torch.int32)
+        self.out = torch.zeros(n, tower.cfg["projection_dim"], device=self.dev, dtype=torch.float32)
+        self._build()
+
+    def _build(self):
+        c, pk, n, T, S = self.t.cfg, self.t._packed, self.n, self.T, self._add
+        H, I, heads, eps = c["hidden_size"], c["intermediate_size"], c["num_attention_heads"], c["layer_norm_eps"]
+        M = n * T
+        x = self._new(n, T, H)
+        S(lambda: ops.clip_text_embed(self.ids, pk["tok"], pk["pos"], out=x), "embed")
+        y, att, hA, hB = (self._new(n, T, H) for _ in range(4))
+        qkv, f = self._new(n, T, 3 * H), self._new(n, T, I)
+        scale = c["head_dim"] ** -0.5
+        h = x
+        for i in range(c["num_hidden_layers"]):
+            L = pk[i]
+            S(lambda h=h, L=L: ops.layernorm_f16(h, *L["ln_1"], eps=eps, out=y), "layernorm")
+            self._gemm(y, L["attn.qkv"][0], 3 * H, qkv, 2 * M * H * 3 * H, bias=L["attn.qkv"][1])
+            S(lambda: ops.attention_small(qkv, heads, keep_mask=None, causal=True, scale=scale, out=att), "attention",
+              4 * n * heads * T * T * c["head_dim"])
+            self._gemm(att, L["attn.proj"][0], H, hA, 2 * M * H * H, bias=L["attn.proj"][1], residual=h)
+            S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
+            self._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * H * I, bias=L["mlp.fc1"][1])
+            S(lambda: ops.gelu_f16_(f), "gelu")
+            self._gemm(f, L["mlp.fc2"][0], H, hB, 2 * M * I * H, bias=L["mlp.fc2"][1], residual=hA)
+            h = hB
+        self.hidden = self._new(n, T, H)
+        S(lambda: ops.layernorm_f16(h, *pk["final_ln"], eps=eps, out=self.hidden), "layernorm")
+        pooled = torch.empty(n, H, device=self.dev, dtype=torch.float32)
+        S(lambda: ops.clip_text_pool(self.ids, self.hidden, c["pool_eos"], out=pooled, index_out=self.index), "pool")
+        S(lambda: ops.linear(pooled, pk["proj"], out=self.out), "linear", 2 * n * H * c["projection_dim"])

@@ -21,6 +21,7 @@ step is one CUDA graph replay of _PriorStepPlan, whose model output equals `forw
 configurations; PriorEmbedder22 puts it behind the embedder protocol (tests/test_gpu_zz_prior22.py, DESIGN.md section 7).
 """
 import math
+import os
 
 import numpy as np
 import torch
@@ -461,6 +462,23 @@ def sample_prior22(model, text_emb, text_enc, mask, num_steps, guidance, clip_me
     return plan.x * clip_std + clip_mean
 
 
+def _load_weights(folder, stem):
+    """A diffusers / transformers component's state dict on the CPU: folder/stem.safetensors when the safetensors package
+    imports and the file exists, else folder/stem.bin (torch.load, weights_only).  K2Error names the file when neither is
+    there."""
+    try:
+        from safetensors.torch import load_file
+    except ImportError:
+        load_file = None
+    st, bin_ = os.path.join(folder, stem + ".safetensors"), os.path.join(folder, stem + ".bin")
+    if load_file is not None and os.path.exists(st):
+        return load_file(st)
+    if os.path.exists(bin_):
+        return torch.load(bin_, map_location="cpu", weights_only=True)
+    want = f"{st} or {bin_}" if load_file is not None else f"{bin_} (safetensors is not installed)"
+    raise K2Error(f"PriorEmbedder22.from_pretrained: {want} not found")
+
+
 class PriorEmbedder22:
     """The Kandinsky 2.2 diffusion prior behind the pipelines' `embedder` protocol: what diffusers'
     `KandinskyV22PriorPipeline.__call__` does for the reference's Kandinsky2_2 methods (kandinsky2_2_model.py:69-80,
@@ -485,11 +503,16 @@ class PriorEmbedder22:
         self._zero = zero_image_emb
 
     @classmethod
-    def from_diffusers(cls, state_dict, clip_text, device="cuda", image_encoder=None, **kwargs):
+    def from_diffusers(cls, state_dict, clip_text=None, device="cuda", image_encoder=None, text_encoder=None, **kwargs):
         """Build from a diffusers `PriorTransformer` state dict (kandinsky-community/kandinsky-2-2-prior, subfolder `prior`)
         via checkpoints.diffusers_prior_to_k2; the configuration is read from the tensor shapes.  image_encoder: the pipeline's
         CLIP image tower (model.clip_vision.CLIPVisionTower) or None.  A tower becomes clip_image and, unless zero_image_emb is
-        passed, supplies it as the tower on all-zero pixel_values, computed here once (diffusers' get_zero_embed)."""
+        passed, supplies it as the tower on all-zero pixel_values, computed here once (diffusers' get_zero_embed).
+        text_encoder: the pipeline's CLIP text tower with its tokenizer (model.clip_text.CLIPTextTower), which becomes
+        clip_text; exactly one of clip_text / text_encoder is given (ValueError otherwise), and a tower whose sequence length,
+        hidden size or projection width does not fit the prior raises K2Error."""
+        if (clip_text is None) == (text_encoder is None):
+            raise ValueError("PriorEmbedder22.from_diffusers: pass exactly one of clip_text= and text_encoder=")
         if image_encoder is not None:
             if kwargs.get("clip_image") is not None:
                 raise ValueError("PriorEmbedder22.from_diffusers: pass image_encoder= or clip_image=, not both")
@@ -503,8 +526,50 @@ class PriorEmbedder22:
         prior = PriorTransformer(text_ctx=sd["positional_embedding"].shape[1] - 4, xf_width=W, xf_layers=layers, xf_heads=W // 64,
                                  xf_final_ln=True, xf_padding=False, clip_dim=sd["out_proj.weight"].shape[0],
                                  clip_xf_width=sd["text_enc_proj.weight"].shape[1], device=device)
+        if text_encoder is not None:
+            c = text_encoder.cfg
+            got = (text_encoder.tokens, c["hidden_size"], c["projection_dim"])
+            want = (prior.text_ctx, prior.clip_xf_width, prior.clip_dim)
+            if got != want:
+                raise K2Error(f"PriorEmbedder22.from_diffusers: the text encoder gives (tokens, hidden, projection) {got}, "
+                              f"the prior takes (text_ctx, clip_xf_width, clip_dim) {want}")
+            clip_text = text_encoder
         prior.load_state_dict(sd, strict=True)
         return cls(prior.finalize(), clip_text, mean.to(device).float(), std.to(device).float(), **kwargs)
+
+    @classmethod
+    def from_pretrained(cls, path, device="cuda", **kwargs):
+        """A local `kandinsky-2-2-prior` folder (the diffusers layout) -> the embedder with its own CLIP text tower and
+        tokenizer, and its CLIP image tower when the folder has one:
+            prior/           diffusion_pytorch_model.{safetensors,bin}
+            text_encoder/    config.json, model.{safetensors,bin}
+            tokenizer/       vocab.json, merges.txt (+ special_tokens_map.json, tokenizer_config.json)
+            image_encoder/   config.json, model.{safetensors,bin}           (optional)
+            image_processor/ preprocessor_config.json                       (optional)
+        *.safetensors are read when the safetensors package imports, else the .bin files (torch.load, weights_only).  A
+        missing file raises K2Error naming it.  kwargs go to from_diffusers (prior_steps, seed, ...)."""
+        import json
+
+        from .clip_text import CLIPTextTower, CLIPTokenizer
+
+        def read_config(sub, name="config.json"):
+            f = os.path.join(path, sub, name)
+            if not os.path.exists(f):
+                raise K2Error(f"PriorEmbedder22.from_pretrained: {f} not found")
+            with open(f, encoding="utf-8") as fh:
+                return json.load(fh)
+
+        tok_dir = os.path.join(path, "tokenizer")
+        tower = CLIPTextTower.from_transformers(_load_weights(os.path.join(path, "text_encoder"), "model"),
+                                                read_config("text_encoder"), device, CLIPTokenizer.from_dir(tok_dir))
+        if os.path.isdir(os.path.join(path, "image_encoder")) and kwargs.get("image_encoder") is None:
+            from .clip_vision import CLIPVisionTower
+            proc = (read_config("image_processor", "preprocessor_config.json")
+                    if os.path.isdir(os.path.join(path, "image_processor")) else None)
+            kwargs["image_encoder"] = CLIPVisionTower.from_transformers(
+                _load_weights(os.path.join(path, "image_encoder"), "model"), read_config("image_encoder"), device, proc)
+        return cls.from_diffusers(_load_weights(os.path.join(path, "prior"), "diffusion_pytorch_model"), device=device,
+                                  text_encoder=tower, **kwargs)
 
     def _call_args(self, prompt, B, prior_steps, prior_guidance_scale, negative_prior_prompt):
         """(steps, guidance, CFG rows [text_embeds, hidden states, mask] on the device, the call's generator): the rows are

@@ -669,3 +669,47 @@ def attention_heads(qkv, heads, head_dim, scale, out=None, hs=None, q_off=0, k_o
     check(nat.load().k2_attention_heads(ptr(qkv), _row_stride(qkv), hs, q_off, k_off, v_off, B, heads, T, head_dim,
                                         float(scale), ptr(out), _row_stride(out), ohs, stream_ptr()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# CLIP text tower (kandinsky2/model/clip_text.py, see k2b200.h)
+# ------------------------------------------------------------------------------------------------
+def clip_text_embed(ids, tok, pos, out=None):
+    """k2_clip_text_embed: int32 ids [B, T] (row-strided view), fp16 tables tok [V, H] and pos [>= T, H] -> fp16 rows
+    [B, T, H] (out may be row-strided) = fp16(float(tok[id]) + float(pos[t])); an id outside [0, V) gives a NaN row."""
+    tensors = (ids, tok, pos) + ((out,) if out is not None else ())
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error("clip_text_embed: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    ldi, B, T = _rows_2d(ids, torch.int32, "ids")
+    assert tok.dtype == torch.float16 and pos.dtype == torch.float16 and tok.is_contiguous() and pos.is_contiguous(), \
+        (tok.dtype, pos.dtype)
+    V, H = tok.shape
+    assert pos.dim() == 2 and pos.shape[1] == H and pos.shape[0] >= T, (tuple(pos.shape), H, T)
+    if out is None:
+        out = torch.empty((B, T, H), dtype=torch.float16, device=ids.device)
+    assert out.dtype == torch.float16 and tuple(out.shape) == (B, T, H), (out.dtype, tuple(out.shape))
+    check(nat.load().k2_clip_text_embed(ptr(ids), ldi, B, T, ptr(tok), V, ptr(pos), H, ptr(out), _row_stride(out),
+                                        stream_ptr()))
+    return out
+
+
+def clip_text_pool(ids, hidden, eos_id, out=None, index_out=None):
+    """k2_clip_text_pool: int32 ids [B, T] (row-strided view), fp16 hidden [B, T, H] (row-strided) -> fp32 [B, H] = the
+    hidden row at each sequence's pooled position (eos_id < 0: the first argmax of the ids; else the first position equal to
+    eos_id, 0 if none), widened exactly.  index_out: int32 [B] receives the positions."""
+    tensors = (ids, hidden) + tuple(t for t in (out, index_out) if t is not None)
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error("clip_text_pool: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    ldi, B, T = _rows_2d(ids, torch.int32, "ids")
+    assert hidden.dtype == torch.float16 and hidden.dim() == 3 and tuple(hidden.shape[:2]) == (B, T), \
+        (hidden.dtype, tuple(hidden.shape))
+    H = hidden.shape[2]
+    if out is None:
+        out = torch.empty((B, H), dtype=torch.float32, device=ids.device)
+    ldo, mo, no = _rows_2d(out, torch.float32, "out")
+    assert (mo, no) == (B, H), (tuple(out.shape), B, H)
+    if index_out is not None:
+        assert index_out.dtype == torch.int32 and tuple(index_out.shape) == (B,) and index_out.is_contiguous()
+    check(nat.load().k2_clip_text_pool(ptr(ids), ldi, B, T, int(eos_id), ptr(hidden), _row_stride(hidden), H, ptr(out), ldo,
+                                       ptr(index_out), stream_ptr()))
+    return out
