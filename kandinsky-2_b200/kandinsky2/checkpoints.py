@@ -271,21 +271,57 @@ def k2_to_diffusers_unet(sd,in_channels=4, model_channels=384, channel_mult=(1, 
     return out
 
 
-_CLIP_V_LAYER = {"layer_norm1": "ln_1", "layer_norm2": "ln_2", "self_attn.out_proj": "attn.proj", "mlp.fc1": "mlp.fc1",
-                 "mlp.fc2": "mlp.fc2"}
+_CLIP_LAYER = {"layer_norm1": "ln_1", "layer_norm2": "ln_2", "self_attn.out_proj": "attn.proj", "mlp.fc1": "mlp.fc1",
+               "mlp.fc2": "mlp.fc2"}
+# the keys outside the encoder layers: this package's name -> transformers' name
+_CLIP_TOP = {
+    "vision": {"class_embedding": "vision_model.embeddings.class_embedding",
+               "patch_embedding.weight": "vision_model.embeddings.patch_embedding.weight",
+               "position_embedding": "vision_model.embeddings.position_embedding.weight",
+               "pre_ln.weight": "vision_model.pre_layrnorm.weight", "pre_ln.bias": "vision_model.pre_layrnorm.bias",
+               "post_ln.weight": "vision_model.post_layernorm.weight", "post_ln.bias": "vision_model.post_layernorm.bias",
+               "proj.weight": "visual_projection.weight"},
+    "text": {"token_embedding": "text_model.embeddings.token_embedding.weight",
+             "position_embedding": "text_model.embeddings.position_embedding.weight",
+             "final_ln.weight": "text_model.final_layer_norm.weight", "final_ln.bias": "text_model.final_layer_norm.bias",
+             "proj.weight": "text_projection.weight"},
+}
+
+
+def _clip_keys(tower, layers):
+    keys = list(_CLIP_TOP[tower].values())
+    for i in range(layers):
+        lp = f"{tower}_model.encoder.layers.{i}."
+        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
+                 for s in ("weight", "bias")]
+    return keys
+
+
+def _clip_to_k2(sd, tower, head_dim):
+    """transformers CLIP `tower` ("text" / "vision") state dict -> this package's names, q / k / v packed per head_dim head."""
+    p = f"{tower}_model."
+    sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
+    layers = {int(m.group(1)) for m in (re.match(rf"^{re.escape(p)}encoder\.layers\.(\d+)\.", k) for k in sd) if m}
+    expected = _clip_keys(tower, max(layers) + 1 if layers else 0)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"transformers CLIP {tower} state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {k: sd[d] for k, d in _CLIP_TOP[tower].items()}
+    for i in sorted(layers):
+        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
+        for d, k in _CLIP_LAYER.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], head_dim)
+    return out
 
 
 def transformers_clip_vision_keys(layers):
     """Every key of a transformers `CLIPVisionModelWithProjection` state dict with `layers` encoder layers (without the
     non-persistent `position_ids` buffer)."""
-    p = "vision_model."
-    keys = [p + "embeddings.class_embedding", p + "embeddings.patch_embedding.weight", p + "embeddings.position_embedding.weight"]
-    keys += [f"{p}{n}.{s}" for n in ("pre_layrnorm", "post_layernorm") for s in ("weight", "bias")]
-    for i in range(layers):
-        lp = f"{p}encoder.layers.{i}."
-        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_V_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
-                 for s in ("weight", "bias")]
-    return keys + ["visual_projection.weight"]
+    return _clip_keys("vision", layers)
 
 
 def transformers_clip_vision_to_k2(sd, head_dim=104):
@@ -295,41 +331,13 @@ def transformers_clip_vision_to_k2(sd, head_dim=104):
         layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}
     where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads with the tower's head width).  A
     `position_ids` buffer is ignored; unknown and missing keys raise K2Error naming them."""
-    p = "vision_model."
-    sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
-    layers = {int(m.group(1)) for m in (re.match(r"^vision_model\.encoder\.layers\.(\d+)\.", k) for k in sd) if m}
-    expected = transformers_clip_vision_keys(max(layers) + 1 if layers else 0)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"transformers CLIP vision state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {"class_embedding": sd[p + "embeddings.class_embedding"],
-           "patch_embedding.weight": sd[p + "embeddings.patch_embedding.weight"],
-           "position_embedding": sd[p + "embeddings.position_embedding.weight"],
-           "proj.weight": sd["visual_projection.weight"]}
-    for d, k in (("pre_layrnorm", "pre_ln"), ("post_layernorm", "post_ln")):
-        for s in ("weight", "bias"):
-            out[f"{k}.{s}"] = sd[f"{p}{d}.{s}"]
-    for i in sorted(layers):
-        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
-        for d, k in _CLIP_V_LAYER.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], head_dim)
-    return out
+    return _clip_to_k2(sd, "vision", head_dim)
 
 
 def transformers_clip_text_keys(layers):
     """Every key of a transformers `CLIPTextModelWithProjection` state dict with `layers` encoder layers (without the
     `position_ids` buffer)."""
-    p = "text_model."
-    keys = [p + "embeddings.token_embedding.weight", p + "embeddings.position_embedding.weight"]
-    for i in range(layers):
-        lp = f"{p}encoder.layers.{i}."
-        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_V_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
-                 for s in ("weight", "bias")]
-    return keys + [f"{p}final_layer_norm.{s}" for s in ("weight", "bias")] + ["text_projection.weight"]
+    return _clip_keys("text", layers)
 
 
 def transformers_clip_text_to_k2(sd):
@@ -339,23 +347,4 @@ def transformers_clip_text_to_k2(sd):
         layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}
     where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads, head width 64).  A `position_ids`
     buffer (older checkpoints carry it) is ignored; unknown and missing keys raise K2Error naming them."""
-    p = "text_model."
-    sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
-    layers = {int(m.group(1)) for m in (re.match(r"^text_model\.encoder\.layers\.(\d+)\.", k) for k in sd) if m}
-    expected = transformers_clip_text_keys(max(layers) + 1 if layers else 0)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"transformers CLIP text state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {"token_embedding": sd[p + "embeddings.token_embedding.weight"],
-           "position_embedding": sd[p + "embeddings.position_embedding.weight"],
-           "final_ln.weight": sd[p + "final_layer_norm.weight"], "final_ln.bias": sd[p + "final_layer_norm.bias"],
-           "proj.weight": sd["text_projection.weight"]}
-    for i in sorted(layers):
-        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
-        for d, k in _CLIP_V_LAYER.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], 64)
-    return out
+    return _clip_to_k2(sd, "text", 64)

@@ -6,9 +6,9 @@ The tower is read from the checkpoint's `config.json` (hidden 1280, 32 layers, 2
 vocabulary 49408, projection 1280, exact GELU expected for ViT-bigG/14); what is not implemented is refused with K2Error: any
 `hidden_act` but "gelu", any head width but 64 (so the hidden size is a multiple of 8), more than 128 positions.  Compute, per
 (row count, length) one LaunchPlan replayed as one CUDA graph:
-    k2_clip_text_embed (token + position embedding, one fp16 rounding), then per layer  LayerNorm -> qkv GEMM (q / k / v
-    packed per head) -> k2_attention_small (causal, no key mask: diffusers calls the encoder without attention_mask) ->
-    out_proj GEMM + residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual,
+    k2_clip_text_embed (token + position embedding, one fp16 rounding), then the pre-LayerNorm layers of model/encoder.py
+    (q / k / v packed per head) with k2_attention_small as the attention (causal, no key mask: diffusers calls the encoder
+    without attention_mask),
     final_layer_norm over every row (last_hidden_state), k2_clip_text_pool (the pooled row, chosen on the device from the ids
     by the config's eos_token_id rule, widened to fp32) and the bias-free text_projection in fp32 (ops.linear).
 fp16 storage, fp32 accumulation, the prior's LayerNorm statistics and attention.
@@ -28,6 +28,7 @@ import torch
 from .. import ops
 from .._native import K2Error
 from ..launch_plan import LaunchPlan
+from .encoder import clip_config, layer_shapes, pack_layers, record_layers
 
 _REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "max_position_embeddings",
              "vocab_size", "projection_dim")
@@ -38,24 +39,12 @@ def text_tower_config(config):
     """The transformers CLIPTextConfig dict -> the geometry this module implements; K2Error for anything else.  A key that is
     absent takes transformers' default (hidden_act "quick_gelu", layer_norm_eps 1e-5, eos_token_id 49407).  "pool_eos" is the
     pooling rule: -1 for eos_token_id == 2 (the first argmax of the ids, pre-#24773 configs), else the eos id."""
-    missing = [k for k in _REQUIRED if k not in config]
-    if missing:
-        raise K2Error(f"CLIP text config: missing {missing}")
-    c = {k: int(config[k]) for k in _REQUIRED}
-    c["hidden_act"] = config.get("hidden_act", "quick_gelu")
-    c["layer_norm_eps"] = float(config.get("layer_norm_eps", 1e-5))
-    c["eos_token_id"] = int(config.get("eos_token_id", 49407))
-    if c["hidden_act"] != "gelu":
-        raise K2Error(f"CLIP text tower: hidden_act {c['hidden_act']!r} is not implemented (only the exact 'gelu' of "
-                      "ViT-bigG/14; the 2.1 tower's quick_gelu is not)")
-    H, heads = c["hidden_size"], c["num_attention_heads"]
-    if H % heads or H // heads != 64:
-        raise K2Error(f"CLIP text tower: head width {H / heads:g} is not implemented (only 64)")
     # heads of 64 make hidden_size a multiple of 8, which k2_clip_text_embed's 16-byte rows need
+    c = clip_config(config, _REQUIRED, "text", 64)
     if not 0 < c["max_position_embeddings"] <= MAX_TOKENS:
         raise K2Error(f"CLIP text tower: max_position_embeddings {c['max_position_embeddings']} is not implemented "
                       f"(at most {MAX_TOKENS} tokens)")
-    c["head_dim"] = 64
+    c["eos_token_id"] = int(config.get("eos_token_id", 49407))
     c["pool_eos"] = -1 if c["eos_token_id"] == 2 else c["eos_token_id"]
     return c
 
@@ -305,12 +294,7 @@ class CLIPTextTower:
         H, I, L = c["hidden_size"], c["intermediate_size"], c["num_hidden_layers"]
         want = {"token_embedding": (c["vocab_size"], H), "position_embedding": (c["max_position_embeddings"], H),
                 "final_ln.weight": (H,), "final_ln.bias": (H,), "proj.weight": (c["projection_dim"], H)}
-        for i in range(L):
-            for name, shape in (("ln_1.weight", (H,)), ("ln_1.bias", (H,)), ("ln_2.weight", (H,)), ("ln_2.bias", (H,)),
-                                ("attn.qkv.weight", (3 * H, H)), ("attn.qkv.bias", (3 * H,)), ("attn.proj.weight", (H, H)),
-                                ("attn.proj.bias", (H,)), ("mlp.fc1.weight", (I, H)), ("mlp.fc1.bias", (I,)),
-                                ("mlp.fc2.weight", (H, I)), ("mlp.fc2.bias", (H,))):
-                want[f"layers.{i}.{name}"] = shape
+        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, I).items()})
         bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
         extra = sorted(set(sd) - set(want))
         if bad or extra:
@@ -333,13 +317,8 @@ class CLIPTextTower:
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
         pk = {"tok": sd["token_embedding"].detach().to(dev).half().contiguous(),
               "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
-              "final_ln": (f32(sd["final_ln.weight"]), f32(sd["final_ln.bias"])), "proj": f32(sd["proj.weight"])}
-        for i in range(c["num_hidden_layers"]):
-            p = f"layers.{i}."
-            pk[i] = {"ln_1": (f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])),
-                     "ln_2": (f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"]))}
-            for name in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2"):
-                pk[i][name] = (ops.pack_conv_weight(sd[p + name + ".weight"].detach().to(dev)), f32(sd[p + name + ".bias"]))
+              "final_ln": (f32(sd["final_ln.weight"]), f32(sd["final_ln.bias"])), "proj": f32(sd["proj.weight"]),
+              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
         self._packed = pk
         self._plans = {}
         return self
@@ -402,26 +381,13 @@ class _TextPlan(LaunchPlan):
 
     def _build(self):
         c, pk, n, T, S = self.t.cfg, self.t._packed, self.n, self.T, self._add
-        H, I, heads, eps = c["hidden_size"], c["intermediate_size"], c["num_attention_heads"], c["layer_norm_eps"]
-        M = n * T
+        H, heads, eps = c["hidden_size"], c["num_attention_heads"], c["layer_norm_eps"]
         x = self._new(n, T, H)
         S(lambda: ops.clip_text_embed(self.ids, pk["tok"], pk["pos"], out=x), "embed")
-        y, att, hA, hB = (self._new(n, T, H) for _ in range(4))
-        qkv, f = self._new(n, T, 3 * H), self._new(n, T, I)
         scale = c["head_dim"] ** -0.5
-        h = x
-        for i in range(c["num_hidden_layers"]):
-            L = pk[i]
-            S(lambda h=h, L=L: ops.layernorm_f16(h, *L["ln_1"], eps=eps, out=y), "layernorm")
-            self._gemm(y, L["attn.qkv"][0], 3 * H, qkv, 2 * M * H * 3 * H, bias=L["attn.qkv"][1])
-            S(lambda: ops.attention_small(qkv, heads, keep_mask=None, causal=True, scale=scale, out=att), "attention",
-              4 * n * heads * T * T * c["head_dim"])
-            self._gemm(att, L["attn.proj"][0], H, hA, 2 * M * H * H, bias=L["attn.proj"][1], residual=h)
-            S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
-            self._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * H * I, bias=L["mlp.fc1"][1])
-            S(lambda: ops.gelu_f16_(f), "gelu")
-            self._gemm(f, L["mlp.fc2"][0], H, hB, 2 * M * I * H, bias=L["mlp.fc2"][1], residual=hA)
-            h = hB
+        h = record_layers(self, x, pk["layers"],
+                          lambda qkv, out: ops.attention_small(qkv, heads, keep_mask=None, causal=True, scale=scale, out=out),
+                          4 * n * heads * T * T * c["head_dim"], eps)
         self.hidden = self._new(n, T, H)
         S(lambda: ops.layernorm_f16(h, *pk["final_ln"], eps=eps, out=self.hidden), "layernorm")
         pooled = torch.empty(n, H, device=self.dev, dtype=torch.float32)

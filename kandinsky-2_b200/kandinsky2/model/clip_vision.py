@@ -6,8 +6,8 @@ The tower is read from the checkpoint's `config.json` (hidden 1664, 48 layers, 1
 projection 1280, exact GELU for ViT-bigG/14); what is not implemented is refused with K2Error: any `hidden_act` but "gelu", any
 head width but 104.  Compute, per batch size one LaunchPlan replayed as one CUDA graph:
     k2_clip_patchify -> ONE GEMM: patch conv + class embedding (K column 3 P^2) + position embedding (the epilogue residual),
-    pre_layrnorm, then per layer  LayerNorm -> qkv GEMM (q / k / v packed per head) -> k2_attention_heads -> out_proj GEMM +
-    residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual,
+    pre_layrnorm, then the pre-LayerNorm layers of model/encoder.py (q / k / v packed per head) with k2_attention_heads as the
+    attention,
     post_layernorm on the CLS rows (a strided view), fp16 -> fp32, and the bias-free visual_projection in fp32 (ops.linear).
 fp16 storage, fp32 accumulation, fp32 softmax with P rounded to fp16 before PV, the prior's LayerNorm statistics.
 
@@ -23,6 +23,7 @@ import torch
 from .. import ops
 from .._native import K2Error
 from ..launch_plan import LaunchPlan
+from .encoder import clip_config, layer_shapes, pack_layers, record_layers
 
 OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -37,23 +38,11 @@ _REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_atten
 def tower_config(config):
     """The transformers CLIPVisionConfig dict -> the geometry this module implements; K2Error for anything else.  A key that
     is absent takes transformers' default (hidden_act "quick_gelu", layer_norm_eps 1e-5, num_channels 3)."""
-    missing = [k for k in _REQUIRED if k not in config]
-    if missing:
-        raise K2Error(f"CLIP vision config: missing {missing}")
-    c = {k: int(config[k]) for k in _REQUIRED}
-    c["hidden_act"] = config.get("hidden_act", "quick_gelu")
-    c["layer_norm_eps"] = float(config.get("layer_norm_eps", 1e-5))
-    if c["hidden_act"] != "gelu":
-        raise K2Error(f"CLIP vision tower: hidden_act {c['hidden_act']!r} is not implemented (only the exact 'gelu' of "
-                      "ViT-bigG/14; the 2.1 tower's quick_gelu is not)")
+    c = clip_config(config, _REQUIRED, "vision", 104)
     if int(config.get("num_channels", 3)) != 3:
         raise K2Error("CLIP vision tower: only 3-channel images are implemented")
-    H, heads = c["hidden_size"], c["num_attention_heads"]
-    if H % heads or H // heads != 104:
-        raise K2Error(f"CLIP vision tower: head width {H / heads:g} is not implemented (only 104, ViT-bigG/14)")
     if c["image_size"] % c["patch_size"]:
         raise K2Error("CLIP vision tower: image_size must be a multiple of patch_size")
-    c["head_dim"] = 104
     c["tokens"] = (c["image_size"] // c["patch_size"]) ** 2 + 1
     c["kp"] = (3 * c["patch_size"] ** 2 + 1 + 63) // 64 * 64
     return c
@@ -127,12 +116,7 @@ class CLIPVisionTower:
         want = {"class_embedding": (H,), "patch_embedding.weight": (H, 3, P, P), "position_embedding": (T, H),
                 "pre_ln.weight": (H,), "pre_ln.bias": (H,), "post_ln.weight": (H,), "post_ln.bias": (H,),
                 "proj.weight": (c["projection_dim"], H)}
-        for i in range(L):
-            for name, shape in (("ln_1.weight", (H,)), ("ln_1.bias", (H,)), ("ln_2.weight", (H,)), ("ln_2.bias", (H,)),
-                                ("attn.qkv.weight", (3 * H, H)), ("attn.qkv.bias", (3 * H,)), ("attn.proj.weight", (H, H)),
-                                ("attn.proj.bias", (H,)), ("mlp.fc1.weight", (I, H)), ("mlp.fc1.bias", (I,)),
-                                ("mlp.fc2.weight", (H, I)), ("mlp.fc2.bias", (H,))):
-                want[f"layers.{i}.{name}"] = shape
+        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, I).items()})
         bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
         extra = sorted(set(sd) - set(want))
         if bad or extra:
@@ -161,13 +145,8 @@ class CLIPVisionTower:
         we[:, K] = sd["class_embedding"].detach().to(dev).half()
         pk = {"embed": we, "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
               "pre_ln": (f32(sd["pre_ln.weight"]), f32(sd["pre_ln.bias"])),
-              "post_ln": (f32(sd["post_ln.weight"]), f32(sd["post_ln.bias"])), "proj": f32(sd["proj.weight"])}
-        for i in range(c["num_hidden_layers"]):
-            p = f"layers.{i}."
-            pk[i] = {"ln_1": (f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])),
-                     "ln_2": (f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"]))}
-            for name in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2"):
-                pk[i][name] = (ops.pack_conv_weight(sd[p + name + ".weight"].detach().to(dev)), f32(sd[p + name + ".bias"]))
+              "post_ln": (f32(sd["post_ln.weight"]), f32(sd["post_ln.bias"])), "proj": f32(sd["proj.weight"]),
+              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
         self._packed = pk
         self._plans = {}
         return self
@@ -228,29 +207,15 @@ class _TowerPlan(LaunchPlan):
 
     def _build(self):
         c, pk, B, S = self.t.cfg, self.t._packed, self.B, self._add
-        T, H, I, hd, heads, eps = (c["tokens"], c["hidden_size"], c["intermediate_size"], c["head_dim"], c["num_attention_heads"],
-                                   c["layer_norm_eps"])
-        M = B * T
+        T, H, hd, heads, eps = c["tokens"], c["hidden_size"], c["head_dim"], c["num_attention_heads"], c["layer_norm_eps"]
         rows = self._new(B, T, c["kp"])
         S(lambda: ops.clip_patchify(self.pix, c["patch_size"], c["kp"], out=rows), "patchify")
         emb, x = self._new(B, T, H), self._new(B, T, H)
-        self._gemm(rows, pk["embed"], H, emb, 2 * M * c["kp"] * H, residual=self.pos)
+        self._gemm(rows, pk["embed"], H, emb, 2 * B * T * c["kp"] * H, residual=self.pos)
         S(lambda: ops.layernorm_f16(emb, *pk["pre_ln"], eps=eps, out=x), "layernorm")
-        y, att, hA, hB = (self._new(B, T, H) for _ in range(4))
-        qkv, f = self._new(B, T, 3 * H), self._new(B, T, I)
         scale = hd ** -0.5
-        h = x
-        for i in range(c["num_hidden_layers"]):
-            L = pk[i]
-            S(lambda h=h, L=L: ops.layernorm_f16(h, *L["ln_1"], eps=eps, out=y), "layernorm")
-            self._gemm(y, L["attn.qkv"][0], 3 * H, qkv, 2 * M * H * 3 * H, bias=L["attn.qkv"][1])
-            S(lambda: ops.attention_heads(qkv, heads, hd, scale, out=att), "attention", 4 * B * heads * T * T * hd)
-            self._gemm(att, L["attn.proj"][0], H, hA, 2 * M * H * H, bias=L["attn.proj"][1], residual=h)
-            S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
-            self._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * H * I, bias=L["mlp.fc1"][1])
-            S(lambda: ops.gelu_f16_(f), "gelu")
-            self._gemm(f, L["mlp.fc2"][0], H, hB, 2 * M * I * H, bias=L["mlp.fc2"][1], residual=hA)
-            h = hB
+        h = record_layers(self, x, pk["layers"], lambda qkv, out: ops.attention_heads(qkv, heads, hd, scale, out=out),
+                          4 * B * heads * T * T * hd, eps)
         self.hidden = h
         cls, cls32 = self._new(B, H), torch.empty(B, H, device=self.dev, dtype=torch.float32)
         S(lambda: ops.layernorm_f16(h[:, 0], *pk["post_ln"], eps=eps, out=cls), "layernorm")

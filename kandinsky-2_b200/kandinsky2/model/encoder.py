@@ -1,0 +1,78 @@
+"""The pre-LayerNorm transformer layer stack shared by the diffusion prior (model/prior.py) and the two CLIP towers
+(model/clip_text.py, model/clip_vision.py): how one layer's weights are named, checked and packed, and the launches one layer
+records in a LaunchPlan:
+    LayerNorm -> qkv GEMM -> attention -> out-proj GEMM + residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual.
+The attention launch is the caller's; everything else is the same for all three models.  Also the part of the transformers
+CLIP config both towers read."""
+import torch
+
+from .. import ops
+from .._native import K2Error
+
+_NORMS = ("ln_1", "ln_2")
+_GEMMS = ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")
+
+
+def layer_shapes(H, I):
+    """{name: shape} of one layer's parameters in this package's names, at width H and MLP width I."""
+    return {"ln_1.weight": (H,), "ln_1.bias": (H,), "ln_2.weight": (H,), "ln_2.bias": (H,),
+            "attn.qkv.weight": (3 * H, H), "attn.qkv.bias": (3 * H,), "attn.proj.weight": (H, H), "attn.proj.bias": (H,),
+            "mlp.fc1.weight": (I, H), "mlp.fc1.bias": (I,), "mlp.fc2.weight": (H, I), "mlp.fc2.bias": (H,)}
+
+
+def pack_layers(get, L, dev):
+    """L layers packed on `dev` once: a list of dicts with "ln_1" / "ln_2" -> (fp32 gain, fp32 bias) and "attn.qkv",
+    "attn.proj", "mlp.fc1", "mlp.fc2" -> (fp16 [N, K] GEMM weight, ops.pack_conv_weight; fp32 bias).  get(i, name) returns
+    layer i's parameter `name` (a layer_shapes key)."""
+    f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+    layers = []
+    for i in range(L):
+        p = {n: (f32(get(i, n + ".weight")), f32(get(i, n + ".bias"))) for n in _NORMS}
+        for n in _GEMMS:
+            p[n] = (ops.pack_conv_weight(get(i, n + ".weight").detach().to(dev)), f32(get(i, n + ".bias")))
+        layers.append(p)
+    return layers
+
+
+def record_layers(plan, h, layers, attend, attn_flops, eps):
+    """Record the layers (pack_layers) into `plan` over h fp16 [rows, tokens, C]; returns the last layer's output.  The
+    buffers are [rows, tokens, C] views so that the GEMM tuner counts rows * tokens output rows.  attend(qkv, out) launches
+    the attention of qkv [rows, tokens, 3C] into out [rows, tokens, C]; attn_flops is what one such launch computes.  The
+    first layer reads h as its residual input; the stream then alternates between two buffers."""
+    rows, tokens, C = h.shape
+    if not layers:
+        return h
+    I, M, S = layers[0]["mlp.fc1"][0].shape[0], rows * tokens, plan._add
+    y, att, hA, hB = (plan._new(rows, tokens, C) for _ in range(4))
+    qkv, f = plan._new(rows, tokens, 3 * C), plan._new(rows, tokens, I)
+    for L in layers:
+        S(lambda h=h, L=L: ops.layernorm_f16(h, *L["ln_1"], eps=eps, out=y), "layernorm")
+        plan._gemm(y, L["attn.qkv"][0], 3 * C, qkv, 2 * M * C * 3 * C, bias=L["attn.qkv"][1])
+        S(lambda: attend(qkv, att), "attention", attn_flops)
+        plan._gemm(att, L["attn.proj"][0], C, hA, 2 * M * C * C, bias=L["attn.proj"][1], residual=h)
+        S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
+        plan._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * C * I, bias=L["mlp.fc1"][1])
+        S(lambda: ops.gelu_f16_(f), "gelu")
+        plan._gemm(f, L["mlp.fc2"][0], C, hB, 2 * M * I * C, bias=L["mlp.fc2"][1], residual=hA)
+        h = hB
+    return h
+
+
+def clip_config(config, required, what, head_dim):
+    """The part of a transformers CLIP{Text,Vision}Config dict both towers read: the `required` integer keys, hidden_act and
+    layer_norm_eps (transformers' defaults "quick_gelu" and 1e-5 when absent), checked against what this package implements
+    (exact GELU, heads of head_dim); K2Error naming the `what` tower otherwise."""
+    missing = [k for k in required if k not in config]
+    if missing:
+        raise K2Error(f"CLIP {what} config: missing {missing}")
+    c = {k: int(config[k]) for k in required}
+    c["hidden_act"] = config.get("hidden_act", "quick_gelu")
+    c["layer_norm_eps"] = float(config.get("layer_norm_eps", 1e-5))
+    if c["hidden_act"] != "gelu":
+        raise K2Error(f"CLIP {what} tower: hidden_act {c['hidden_act']!r} is not implemented (only the exact 'gelu' of "
+                      "ViT-bigG/14; the 2.1 tower's quick_gelu is not)")
+    H, heads = c["hidden_size"], c["num_attention_heads"]
+    if H % heads or H // heads != head_dim:
+        raise K2Error(f"CLIP {what} tower: head width {H / heads:g} is not implemented (only {head_dim})")
+    c["head_dim"] = head_dim
+    return c

@@ -30,6 +30,11 @@ import torch.nn as nn
 from .. import ops
 from .._native import K2Error
 from ..launch_plan import LaunchPlan
+from .encoder import pack_layers, record_layers
+
+# encoder.layer_shapes names -> the reference's names inside transformer.resblocks[i]
+_BLOCK_NAMES = {"ln_1": "ln_1", "ln_2": "ln_2", "attn.qkv": "attn.c_qkv", "attn.proj": "attn.c_proj", "mlp.fc1": "mlp.c_fc",
+                "mlp.fc2": "mlp.c_proj"}
 
 
 class _Node(nn.Module):
@@ -87,13 +92,15 @@ class PriorTransformer(nn.Module):
         self._step_plans = {}
 
     def finalize(self):
-        """Pack the GEMM weights (fp16 [N, K], K padded to 64) once per checkpoint."""
-        pk = {}
-        for i, blk in enumerate(self.transformer.resblocks):
-            for name, m in (("qkv", blk.attn.c_qkv), ("proj", blk.attn.c_proj), ("fc", blk.mlp.c_fc), ("proj2", blk.mlp.c_proj)):
-                pk[(i, name)] = (ops.pack_conv_weight(m.weight), m.bias.float().contiguous())
-        pk["text_enc"] = (ops.pack_conv_weight(self.text_enc_proj.weight), self.text_enc_proj.bias.float().contiguous())
-        self._packed = pk
+        """Pack the GEMM weights (fp16 [N, K], K padded to 64) once per checkpoint, the blocks' with their LayerNorm parameters
+        (encoder.pack_layers)."""
+        def get(i, name):
+            mod, leaf = name.rsplit(".", 1)
+            return self.get_parameter(f"transformer.resblocks.{i}.{_BLOCK_NAMES[mod]}.{leaf}")
+
+        te = self.text_enc_proj
+        self._packed = {"layers": pack_layers(get, self.xf_layers, te.weight.device),
+                        "text_enc": (ops.pack_conv_weight(te.weight), te.bias.float().contiguous())}
         self._step_plans = {}
         return self
 
@@ -129,17 +136,17 @@ class PriorTransformer(nn.Module):
         seq[:, self.text_ctx + 2] = lin(self.clip_img_proj, x).half()
         seq[:, self.text_ctx + 3] = self.prd_emb[0].half()
         h = (seq + self.positional_embedding.half()).reshape(N * n, W).contiguous()
-        for i, blk in enumerate(self.transformer.resblocks):
-            y = ops.layernorm_f16(h, blk.ln_1.weight.float(), blk.ln_1.bias.float())
-            w, b = self._packed[(i, "qkv")]
+        for L in self._packed["layers"]:
+            y = ops.layernorm_f16(h, *L["ln_1"])
+            w, b = L["attn.qkv"]
             qkv = ops.gemm_rows(y, w, 3 * W, bias=b).reshape(N, n, 3 * W)
             a = ops.attention_small(qkv, H, keep_mask=keep, causal=True, scale=1.0 / math.sqrt(64.0)).reshape(N * n, W)
-            w, b = self._packed[(i, "proj")]
+            w, b = L["attn.proj"]
             h = ops.gemm_rows(a, w, W, bias=b, residual=h)
-            y = ops.layernorm_f16(h, blk.ln_2.weight.float(), blk.ln_2.bias.float())
-            w, b = self._packed[(i, "fc")]
+            y = ops.layernorm_f16(h, *L["ln_2"])
+            w, b = L["mlp.fc1"]
             f = ops.gelu_f16_(ops.gemm_rows(y, w, 4 * W, bias=b))
-            w, b = self._packed[(i, "proj2")]
+            w, b = L["mlp.fc2"]
             h = ops.gemm_rows(f, w, W, bias=b, residual=h)
         last = h.reshape(N, n, W)[:, -1].contiguous()
         if self.final_ln is not None:
@@ -315,8 +322,8 @@ class UnCLIPSchedule:
 class _PriorStepPlan(LaunchPlan):
     """One UnCLIP sampling step of the prior at B samples, on static buffers, as ONE launch list (replayed as one CUDA graph):
     k2_step_begin (x duplicated for the 2B CFG rows, this step's t / row / noise picked by the device-side counter), the time
-    embedding and its two linears, clip_img_proj, the token rows 78 and 79 written into the sequence, 20 x (LayerNorm, qkv
-    GEMM, attention, proj GEMM + residual, LayerNorm, fc GEMM, GELU, proj GEMM + residual), the final LayerNorm of the last
+    embedding and its two linears, clip_img_proj, the token rows 78 and 79 written into the sequence, the 20 pre-LayerNorm
+    layers of model/encoder.py with the masked k2_attention_small as the attention, the final LayerNorm of the last
     token (a strided view), out_proj, k2_sampler_step and k2_step_end.  What does not change from step to step -- the text
     token rows, the text_emb_proj and prd_emb rows with their positional embedding, the keep mask -- is written once per call
     by bind().  Layer 0 reads the sequence buffer as its residual input.
@@ -371,36 +378,15 @@ class _PriorStepPlan(LaunchPlan):
         S(lambda: ops.prior_tokens(tok_t, self.pos16[ctx + 1:ctx + 2].expand(N, W), self.seq[:, ctx + 1]), "tokens")
         S(lambda: ops.linear(self.x_in, *img, out=tok_x), "linear", 2 * N * W * D)
         S(lambda: ops.prior_tokens(tok_x, self.pos16[ctx + 2:ctx + 3].expand(N, W), self.seq[:, ctx + 2]), "tokens")
-        M = N * n
-        # [N, n, C] views: the tuner counts M = N * n output rows (split-K candidates for small M, launch_plan.tune)
-        y, att = self._new(N, n, W), self._new(N, n, W)
-        qkv, f = self._new(N, n, 3 * W), self._new(N, n, 4 * W)
-        hA, hB = self._new(N, n, W), self._new(N, n, W)
-        h = self.seq
-        self._norms = []   # fp32 gains / biases the launches point at
-        for i, blk in enumerate(m.transformer.resblocks):
-            g1, b1, g2, b2 = (blk.ln_1.weight.float(), blk.ln_1.bias.float(), blk.ln_2.weight.float(), blk.ln_2.bias.float())
-            self._norms += [g1, b1, g2, b2]
-            S(lambda h=h, g=g1, b=b1: ops.layernorm_f16(h, g, b, out=y), "layernorm")
-            w, b = pk[(i, "qkv")]
-            self._gemm(y, w, 3 * W, qkv, 2 * M * 3 * W * W, bias=b)
-            S(lambda: ops.attention_small(qkv, H, keep_mask=self.keep, causal=True, scale=1.0 / math.sqrt(64.0), out=att), "attention",
-              4 * N * H * n * n * 64)
-            w, b = pk[(i, "proj")]
-            self._gemm(att, w, W, hA, 2 * M * W * W, bias=b, residual=h)
-            S(lambda g=g2, b=b2: ops.layernorm_f16(hA, g, b, out=y), "layernorm")
-            w, b = pk[(i, "fc")]
-            self._gemm(y, w, 4 * W, f, 2 * M * 4 * W * W, bias=b)
-            S(lambda: ops.gelu_f16_(f), "gelu")
-            w, b = pk[(i, "proj2")]
-            self._gemm(f, w, W, hB, 2 * M * 4 * W * W, bias=b, residual=hA)
-            h = hB
+        attend = lambda qkv, out: ops.attention_small(qkv, H, keep_mask=self.keep, causal=True,  # noqa: E731
+                                                      scale=1.0 / math.sqrt(64.0), out=out)
+        # eps 1e-5: ops.layernorm_f16's default, which forward uses
+        h = record_layers(self, self.seq, pk["layers"], attend, 4 * N * H * n * n * 64, 1e-5)
         last = h[:, -1]
         last32 = torch.empty(N, W, **f32)
         if m.final_ln is not None:
             lnf = self._new(N, W)
             gf, bf = m.final_ln.weight.float(), m.final_ln.bias.float()
-            self._norms += [gf, bf]
             S(lambda: ops.layernorm_f16(last, gf, bf, out=lnf), "layernorm")
             S(lambda: ops.f16_to_f32(lnf, out=last32), "widen")
         else:

@@ -61,8 +61,8 @@ def main():
     tok = CLIPTokenizer(cto.synthetic_vocab(fx["merges"]), [tuple(m) for m in fx["merges"]], model_max_length=77)
     sd16 = {k: v.cuda().half() for k, v in cto.synth_weights(cfg, 1).items()}
     tower = CLIPTextTower(transformers_clip_text_to_k2(sd16), cfg, device="cuda", tokenizer=tok).finalize()
-    wbytes = sum(t.numel() * t.element_size() for L in range(cfg["num_hidden_layers"])
-                 for t, _ in (tower._packed[L][n] for n in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")))
+    wbytes = sum(t.numel() * t.element_size() for L in tower._packed["layers"]
+                 for t, _ in (L[n] for n in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")))
     res = dict(card=_card(), reps=args.reps, flops_per_sequence=total, attention_flops_per_sequence=attn,
                layer_weight_bytes=wbytes, tower={})
     for n in [int(x) for x in args.ns.split(",")]:

@@ -68,8 +68,8 @@ def main():
     total, attn = flops_per_image(cfg)
     sd16 = {k: v.cuda().half() for k, v in cvo.synth_weights(cfg, 1).items()}
     tower = CLIPVisionTower(transformers_clip_vision_to_k2(sd16), cfg, device="cuda").finalize()
-    wbytes = sum(t.numel() * t.element_size() for L in range(cfg["num_hidden_layers"])
-                 for t, _ in (tower._packed[L][n] for n in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")))
+    wbytes = sum(t.numel() * t.element_size() for L in tower._packed["layers"]
+                 for t, _ in (L[n] for n in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")))
     wbytes += tower._packed["embed"].numel() * 2 + tower._packed["proj"].numel() * 4
     res = dict(card=_card(), reps=args.reps, flops_per_image=total, attention_flops_per_image=attn, weight_bytes=wbytes,
                tower={})

@@ -57,7 +57,8 @@ def _prior(cfg, seed):
 def _step_weight_bytes(m):
     """Bytes of weights one step reads: the fp16 packed GEMM matrices of the 20 blocks, and the fp32 time_embed, clip_img_proj
     and out_proj matrices (text_enc_proj and text_emb_proj run once per call)."""
-    n = sum(w.numel() * w.element_size() for key, (w, _) in m._packed.items() if key != "text_enc")
+    n = sum(L[k][0].numel() * L[k][0].element_size() for L in m._packed["layers"]
+            for k in ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2"))
     for mod in (getattr(m.time_embed, "0"), getattr(m.time_embed, "2"), m.clip_img_proj, m.out_proj):
         n += mod.weight.numel() * mod.weight.element_size()
     return n
