@@ -51,8 +51,7 @@ def space_timesteps(num_timesteps, section_counts):
 class _Schedule:
     """What _sampling_loop needs of a schedule: coef_table() (fp32 [n, 8] step-kernel rows) and model_timesteps() (what the UNet
     sees, [n]) in the same index order; the loop runs the rows n-1 .. 0.  Each schedule also states whether its step draws
-    noise and which step kernel applies its rows ("ddpm": k2_sampler_step, "dpmpp_2m": k2_dpm_solver_step, "dpmpp_2m_sde":
-    k2_dpm_solver_sde_step, "unipc": k2_unipc_step, whose rows are 16 floats wide)."""
+    noise and which step kernel applies its rows (step_kind, one of FusedStep.STEP_KINDS; FusedStep's doc lists them)."""
 
     draws_noise = True
     step_kind = "ddpm"
@@ -145,52 +144,39 @@ class SpacedDiffusion(_Schedule):
                               callback=callback)
 
 
-class DPMSolverSchedule(_Schedule):
-    """DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models",
-    Algorithm 2) over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step, no noise
-    (see sde below).
+class _SolverSchedule(_Schedule):
+    """A multistep solver over the model's own base table alphas_cumprod (float64): one CFG-doubled UNet evaluation per step.
 
     N evaluations at tau_k = linspace(0, T-1, N+1).round()[::-1][k], k = 0..N-1; the UNet sees tau_k as a raw float timestep.
-    alpha_k = sqrt(ac[tau_k]), sigma_k = sqrt(1 - ac[tau_k]), lambda_k = log alpha_k - log sigma_k; the target after the last
-    evaluation is alpha_N = 1, sigma_N = 0.  With h_k = lambda_{k+1} - lambda_k and c = alpha_{k+1} (1 - exp(-h_k)):
-        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1},   c_x = sigma_{k+1} / sigma_k,
-        first order (the first step, the last step, which gives x_N = D_{N-1} exactly):  c_D = c, c_P = 0;
-        otherwise, r = h_{k-1} / h_k:  c_D = c (1 + 1/(2r)),  c_P = -c / (2r).
-    D is the x0 prediction (x - sigma eps) / alpha of the CFG-combined epsilon; k2_dpm_solver_step applies one row.
-    keep = s (img2img): only the last s evaluations run (k0 = N - s), from x = alpha_k0 latent + sigma_k0 noise
-    (start_latent); the history is empty at k0, so that step is first order.
-
-    Rows are stored in reverse step order (table index j = N-1-k) so that _sampling_loop, which walks the indices from the
-    top down like the DDPM schedules', runs k = k0 .. N-1.
+    alpha_k = sqrt(ac[tau_k]), sigma_k = sqrt(1 - ac[tau_k]); the target after the last evaluation is alpha_N = 1, sigma_N = 0.
 
     spacing="karras" (Karras et al. 2022, eq. 5, rho = 7) places the N evaluations in the VE sigma s^(t) = sqrt((1 - ac_t) /
     ac_t) of the base table instead: s^_i = (s^_max^(1/rho) + i/(N-1) (s^_min^(1/rho) - s^_max^(1/rho)))^rho with s^_max =
     s^(T-1), s^_min = s^(0) (s^_max alone when N = 1), alpha_i = 1 / sqrt(1 + s^_i^2), sigma_i = s^_i alpha_i.  The UNet sees
     the fractional timestep whose log s^ interpolates the table's log s^(t) linearly (k-diffusion's sigma_to_t, unrounded).
 
-    sde=True: the data-prediction SDE solver of DPM-Solver++ in its 2M midpoint form (diffusers' "sde-dpmsolver++", k-diffusion's
-    sample_dpmpp_2m_sde with eta 1), one Gaussian draw z per step:
-        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1} + c_N z,   c_x = sigma_{k+1} / sigma_k e^{-h_k},
-        c = alpha_{k+1} (1 - e^{-2 h_k}) in place of c above (same first- / second-order split),  c_N = sigma_{k+1} sqrt(1 - e^{-2h_k});
-    the last step still lands on D_{N-1}, with no noise.  c_N is row column 7, which the ODE rows leave 0."""
+    keep = s (img2img): only the last s evaluations run (k0 = N - s), from x = alpha_k0 latent + sigma_k0 noise
+    (start_latent); the history is empty at k0, so that step is first order.
+
+    A subclass names itself (SOLVER, the prefix of the error messages), states step_kind and draws_noise, and gives
+    coef_rows(): float64 [keep, row width], the rows of steps k = N-1 .. k0.  Rows are stored in this reverse step order (table
+    index j = N-1-k) so that _sampling_loop, which walks the indices from the top down like the DDPM schedules', runs
+    k = k0 .. N-1."""
 
     SPACINGS = ("linspace", "karras")
 
-    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace", sde=False):
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace"):
         ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
         n = int(num_steps)
         if n < 1:
-            raise ValueError("DPM-Solver++: num_steps must be >= 1")
+            raise ValueError(f"{self.SOLVER}: num_steps must be >= 1")
         if spacing not in self.SPACINGS:
-            raise ValueError(f"DPM-Solver++: spacing must be one of {self.SPACINGS}, got {spacing!r}")
+            raise ValueError(f"{self.SOLVER}: spacing must be one of {self.SPACINGS}, got {spacing!r}")
         keep = n if keep is None else int(keep)
         if not 1 <= keep <= n:
-            raise ValueError(f"DPM-Solver++: keep must be in [1, {n}], got {keep}")
-        tau, alphas, sigmas = _solver_grid("DPM-Solver++", ac, n, spacing)
-        self.num_steps, self.k0 = n, n - keep
-        self.spacing, self.sde = spacing, bool(sde)
-        self.draws_noise = self.sde
-        self.step_kind = "dpmpp_2m_sde" if self.sde else "dpmpp_2m"
+            raise ValueError(f"{self.SOLVER}: keep must be in [1, {n}], got {keep}")
+        tau, alphas, sigmas = _solver_grid(self.SOLVER, ac, n, spacing)
+        self.num_steps, self.k0, self.spacing = n, n - keep, spacing
         self.timesteps = tau
         self.alphas = np.append(alphas, 1.0)    # alpha_0 .. alpha_N
         self.sigmas = np.append(sigmas, 0.0)
@@ -198,11 +184,58 @@ class DPMSolverSchedule(_Schedule):
         self._dev_tables = {}
 
     def coef_table(self):
-        """float32 [keep, 8]: the k2_dpm_solver_step rows, built in float64 and cast once."""
+        """float32 [keep, row width]: the step kernel's rows, built in float64 (coef_rows) and cast once."""
         return self.coef_rows().astype(np.float32)
 
+    def model_timesteps(self):
+        """float32 [keep]: what the UNet sees, in table order."""
+        return self.timesteps[self.k0:][::-1].astype(np.float32)
+
+    def start_latent(self, latent, noise):
+        """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
+        return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
+
+    @torch.no_grad()
+    def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
+               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None, step_noise=None,
+               sample_generators=None):
+        """shape = (2*B, 4, h, w) (CFG doubled), noise = the start latent [2B or B, ...]; returns [2*B, 4, h, w] whose two halves
+        both hold the B samples, like p_sample_loop.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces the x0
+        prediction), True = Kandinsky 2.2 (the known region of x is re-noised to the next timestep with the start latent as the
+        noise; UniPC's previous corrected sample is not blended, as in diffusers).
+        A schedule that draws noise (DPMSolverSchedule(sde=True)) draws it like p_sample_loop: step_noise fp32 [keep, B, 4, h, w]
+        injects it, sample_generators (one per sample) draw it per image; a schedule with draws_noise = False ignores both."""
+        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
+                              guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
+                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback,
+                              step_noise=step_noise, sample_generators=sample_generators)
+
+
+class DPMSolverSchedule(_SolverSchedule):
+    """DPM-Solver++(2M) (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models",
+    Algorithm 2) on _SolverSchedule's grid, no noise (see sde below).
+
+    With lambda_k = log alpha_k - log sigma_k, h_k = lambda_{k+1} - lambda_k and c = alpha_{k+1} (1 - exp(-h_k)):
+        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1},   c_x = sigma_{k+1} / sigma_k,
+        first order (the first step, the last step, which gives x_N = D_{N-1} exactly):  c_D = c, c_P = 0;
+        otherwise, r = h_{k-1} / h_k:  c_D = c (1 + 1/(2r)),  c_P = -c / (2r).
+    D is the x0 prediction (x - sigma eps) / alpha of the CFG-combined epsilon; k2_dpm_solver_step applies one row.
+
+    sde=True: the data-prediction SDE solver of DPM-Solver++ in its 2M midpoint form (diffusers' "sde-dpmsolver++", k-diffusion's
+    sample_dpmpp_2m_sde with eta 1), one Gaussian draw z per step:
+        x_{k+1} = c_x x_k + c_D D_k + c_P D_{k-1} + c_N z,   c_x = sigma_{k+1} / sigma_k e^{-h_k},
+        c = alpha_{k+1} (1 - e^{-2 h_k}) in place of c above (same first- / second-order split),  c_N = sigma_{k+1} sqrt(1 - e^{-2h_k});
+    the last step still lands on D_{N-1}, with no noise.  c_N is row column 7, which the ODE rows leave 0."""
+
+    SOLVER = "DPM-Solver++"
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace", sde=False):
+        super().__init__(base_alphas_cumprod, num_steps, keep=keep, spacing=spacing)
+        self.sde = self.draws_noise = bool(sde)
+        self.step_kind = "dpmpp_2m_sde" if self.sde else "dpmpp_2m"
+
     def coef_rows(self):
-        """float64 [keep, 8]: the rows of steps k = N-1 .. k0 (table order, see the class doc)."""
+        """float64 [keep, 8]: the rows of steps k = N-1 .. k0 (table order, see _SolverSchedule)."""
         a, s, n, k0 = self.alphas, self.sigmas, self.num_steps, self.k0
         with np.errstate(divide="ignore"):
             lam = np.log(a) - np.log(s)                     # lambda_N = +inf
@@ -229,28 +262,6 @@ class DPMSolverSchedule(_Schedule):
                 rows[k, 3] = c * (1.0 + 0.5 / r)
                 rows[k, 4] = -c * 0.5 / r
         return np.ascontiguousarray(rows[k0:][::-1])
-
-    def model_timesteps(self):
-        """float32 [keep]: what the UNet sees, in table order."""
-        return self.timesteps[self.k0:][::-1].astype(np.float32)
-
-    def start_latent(self, latent, noise):
-        """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
-        return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
-
-    @torch.no_grad()
-    def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
-               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None, step_noise=None,
-               sample_generators=None):
-        """shape = (2*B, 4, h, w) (CFG doubled), noise = the start latent [2B or B, ...]; returns [2*B, 4, h, w] whose two halves
-        both hold the B samples, like p_sample_loop.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces x0),
-        True = Kandinsky 2.2 (the known region is re-noised to the next timestep with the start latent as the noise).
-        The SDE's per-step noise is drawn like p_sample_loop's: step_noise fp32 [keep, B, 4, h, w] injects it, sample_generators
-        (one per sample) draw it per image; both are ignored by the ODE solver."""
-        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
-                              guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
-                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback,
-                              step_noise=step_noise, sample_generators=sample_generators)
 
 
 def karras_timesteps(base_alphas_cumprod, n, rho=7.0):
@@ -348,71 +359,27 @@ def unipc_rows(alphas, sigmas, first=0, order=2, corrector=True, lower_order_fin
     return np.ascontiguousarray(rows[first:])
 
 
-class UniPCSchedule(_Schedule):
+class UniPCSchedule(_SolverSchedule):
     """UniPC (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework for Fast Sampling of Diffusion Models") with
-    data prediction, B(h) = bh2 and solver order 2, over the model's own base table alphas_cumprod (float64), in the step order of
-    diffusers' UniPCMultistepScheduler: one CFG-doubled UNet evaluation per step, no noise.
+    data prediction, B(h) = bh2 and solver order 2 on _SolverSchedule's grid, in the step order of diffusers'
+    UniPCMultistepScheduler, no noise.
 
-    The N evaluations are DPMSolverSchedule's (spacing "linspace" or "karras", the same grid and model timesteps), and its
+    The N evaluations are DPMSolverSchedule's (the same grid and model timesteps), and its
     predictor UniP-2 with bh2 is DPM-Solver++(2M) exactly.  What UniPC adds is the corrector UniC: once the UNet has run at x_k,
     the previous interval is solved again from the previous corrected sample with the new D_k, which raises the order by one at
     no extra evaluation.  The predictor then continues from the corrected x_k^c; the history keeps D_k of the uncorrected x_k.
     The predictor is first order at the first step (also the first step after an img2img truncation) and at the last one, which
-    lands on D_{N-1} exactly; unipc_rows holds the formulas.  keep = s (img2img): only the last s evaluations run, from
-    start_latent.
+    lands on D_{N-1} exactly; unipc_rows holds the formulas.
 
-    Rows are 16 floats (unipc_rows), stored in reverse step order like DPMSolverSchedule's; k2_unipc_step reads its row from the
-    staged table by the device-side step counter."""
+    Rows are 16 floats (unipc_rows); k2_unipc_step reads its row from the staged table by the device-side step counter."""
 
-    SPACINGS = ("linspace", "karras")
+    SOLVER = "UniPC"
     draws_noise = False
     step_kind = "unipc"
-
-    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace"):
-        ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
-        n = int(num_steps)
-        if n < 1:
-            raise ValueError("UniPC: num_steps must be >= 1")
-        if spacing not in self.SPACINGS:
-            raise ValueError(f"UniPC: spacing must be one of {self.SPACINGS}, got {spacing!r}")
-        keep = n if keep is None else int(keep)
-        if not 1 <= keep <= n:
-            raise ValueError(f"UniPC: keep must be in [1, {n}], got {keep}")
-        tau, alphas, sigmas = _solver_grid("UniPC", ac, n, spacing)
-        self.num_steps, self.k0, self.spacing = n, n - keep, spacing
-        self.timesteps = tau
-        self.alphas = np.append(alphas, 1.0)    # alpha_0 .. alpha_N
-        self.sigmas = np.append(sigmas, 0.0)
-        self.num_timesteps = keep
-        self._dev_tables = {}
 
     def coef_rows(self):
         """float64 [keep, 16]: the rows of steps k = N-1 .. k0 (table order)."""
         return np.ascontiguousarray(unipc_rows(self.alphas, self.sigmas, first=self.k0)[::-1])
-
-    def coef_table(self):
-        """float32 [keep, 16]: the k2_unipc_step rows, built in float64 and cast once."""
-        return self.coef_rows().astype(np.float32)
-
-    def model_timesteps(self):
-        """float32 [keep]: what the UNet sees, in table order."""
-        return self.timesteps[self.k0:][::-1].astype(np.float32)
-
-    def start_latent(self, latent, noise):
-        """img2img start: alpha_k0 latent + sigma_k0 noise (the clean latent noised to the first kept evaluation)."""
-        return float(self.alphas[self.k0]) * latent + float(self.sigmas[self.k0]) * noise
-
-    @torch.no_grad()
-    def sample(self, model, shape, noise=None, model_kwargs=None, device=None, *, guidance_scale=1.0, cond_first=True,
-               inpaint_init=None, inpaint_mask=None, inpaint_renoise=False, callback=None, sample_generators=None):
-        """DPMSolverSchedule.sample's call surface: shape = (2*B, 4, h, w), noise = the start latent; returns [2*B, 4, h, w]
-        whose two halves both hold the B samples.  inpaint_renoise: False = Kandinsky 2.1 (the known region replaces D), True =
-        Kandinsky 2.2 (the known region of x is re-noised to the next timestep with the start latent as the noise; the
-        corrector's previous sample is not blended, as in diffusers).  The step draws no noise, so sample_generators (the
-        solver samplers' common call surface) is ignored."""
-        return _sampling_loop(self, model, shape, noise=noise, model_kwargs=model_kwargs, device=device,
-                              guidance_scale=guidance_scale, cond_first=cond_first, inpaint_init=inpaint_init,
-                              inpaint_mask=inpaint_mask, inpaint_renoise=inpaint_renoise, callback=callback)
 
 
 def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,

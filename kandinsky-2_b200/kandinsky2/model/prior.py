@@ -31,6 +31,7 @@ from .. import ops
 from .._native import K2Error
 from ..launch_plan import LaunchPlan
 from .encoder import pack_layers, record_layers
+from .gaussian_diffusion import SpacedDiffusion, space_timesteps
 
 # encoder.layer_shapes names -> the reference's names inside transformer.resblocks[i]
 _BLOCK_NAMES = {"ln_1": "ln_1", "ln_2": "ln_2", "attn.qkv": "attn.c_qkv", "attn.proj": "attn.c_proj", "mlp.fc1": "mlp.c_fc",
@@ -165,19 +166,11 @@ def sample_prior(model, text_emb, text_enc, mask, use_steps, guidance, clip_mean
     """PriorDiffusionModel.forward (prior.py:336-384) with injected noise: x0-prediction, cosine schedule respaced to
     `use_steps`, fixed small variance, x0 clamped to +-10, classifier-free guidance with the conditional rows first.
     text_* hold 2B rows (cond | uncond); x_T [B, D]; step_noise [steps, B, D].  The per-step update acts on a [B, 768]
-    tensor and is left to torch."""
-    acp_full = np.cumprod(1.0 - cosine_betas(1000))
-    last, betas = 1.0, []
-    for i in use_steps:
-        betas.append(1 - acp_full[i] / last)
-        last = acp_full[i]
-    betas = np.array(betas)
-    acp = np.cumprod(1.0 - betas)
-    acp_prev = np.append(1.0, acp[:-1])
-    post_var = betas * (1.0 - acp_prev) / (1.0 - acp)
-    post_logvar = np.log(np.append(post_var[1], post_var[1:]))
-    c1 = betas * np.sqrt(acp_prev) / (1.0 - acp)
-    c2 = (1.0 - acp_prev) * np.sqrt(1.0 - betas) / (1.0 - acp)
+    tensor and is left to torch.  use_steps: base timesteps in strictly increasing order (ValueError otherwise)."""
+    if any(b <= a for a, b in zip(use_steps, use_steps[1:])):
+        raise ValueError("sample_prior: use_steps must be strictly increasing")
+    d = SpacedDiffusion(set(use_steps), cosine_betas(1000))
+    c1, c2, post_logvar = d.posterior_mean_coef1, d.posterior_mean_coef2, d.posterior_log_variance_clipped
     B = x_T.shape[0]
     x = x_T.float()
     for n, i in enumerate(range(len(use_steps))[::-1]):
@@ -216,7 +209,7 @@ class PriorEmbedder:
     def image_emb(self, prompt, batch_size):
         dev = self.clip_mean.device
         feat, seq, mask = self.clip_text([prompt] * batch_size + [self.negative_prior_prompt] * batch_size)
-        use_steps = sorted(_space_timesteps(1000, self.prior_steps))
+        use_steps = sorted(space_timesteps(1000, [self.prior_steps]))
         import hashlib
         g = torch.Generator(device=dev).manual_seed(
             int.from_bytes(hashlib.sha256(f"{self.seed}:{prompt}".encode()).digest()[:7], "little"))
@@ -250,16 +243,6 @@ class PriorEmbedder:
                 e = self.clip_image(it).float().cpu()
             acc = e * w if acc is None else acc + e * w
         return acc.repeat(batch_size, 1)
-
-
-def _space_timesteps(num_timesteps, count):
-    """respace.py:24-72 with one section (the prior's timestep_respacing=str(prior_steps))."""
-    stride = 1 if count <= 1 else (num_timesteps - 1) / (count - 1)
-    cur, out = 0.0, set()
-    for _ in range(count):
-        out.add(round(cur))
-        cur += stride
-    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

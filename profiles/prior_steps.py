@@ -74,7 +74,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("prior_steps.py needs a CUDA sm_90 device")
     from kandinsky2 import ops
-    from kandinsky2.model.prior import UnCLIPSchedule, _space_timesteps, sample_prior, sample_prior22
+    from kandinsky2.model.gaussian_diffusion import space_timesteps
+    from kandinsky2.model.prior import UnCLIPSchedule, sample_prior, sample_prior22
     from oracle import prior_oracle as po
     from tests import prior22_oracle as p22
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -86,7 +87,7 @@ def main():
     res["weight_bytes_per_step"] = wbytes
     sched = UnCLIPSchedule(N)
     table = torch.from_numpy(sched.coef_table()).cuda()
-    use21 = sorted(_space_timesteps(1000, N))
+    use21 = sorted(space_timesteps(1000, [N]))
     for B in [int(b) for b in args.batches.split(",")]:
         g = torch.Generator(device="cuda").manual_seed(B)
 

@@ -90,12 +90,13 @@ def test_prior_full_size_fp16_calibration(full, B, prompt_len, monkeypatch):
 def test_prior_full_size_sampling(full):
     """PriorDiffusionModel's 25-step guided sampling (guidance 4) with the same x_T and per-step noise, the product's forward
     against the fp32 oracle's."""
-    from kandinsky2.model.prior import _space_timesteps, sample_prior
+    from kandinsky2.model.gaussian_diffusion import space_timesteps
+    from kandinsky2.model.prior import sample_prior
     from oracle import prior_oracle as po
     cfg, m, sd32 = full["cfg"], full["m"], full["sd32"]
     B = 2
     text_emb, text_enc, mask, g = _inputs(B, 12, seed=9)
-    use_steps = sorted(_space_timesteps(1000, 25))
+    use_steps = sorted(space_timesteps(1000, [25]))
     assert len(use_steps) == 25
     x_T = torch.randn(B, 768, device="cuda", generator=g)
     noise = torch.randn(25, B, 768, device="cuda", generator=g)
