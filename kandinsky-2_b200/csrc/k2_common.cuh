@@ -334,13 +334,16 @@ __device__ __forceinline__ void named_bar_arrive(int id, int count) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// x * sigmoid(x) as h + h*tanh(h), h = x/2: ONE MUFU.TANH (rel. error 2^-11, below the fp16 rounding of the stored result)
-// instead of ex2 + rcp -- GroupNorm+SiLU touches 1.3 G elements per step and the MUFU pipe is the narrow one.
+// x * sigmoid(x) = x / (1 + e), e = 2^(-x log2 e): no cancellation for either sign (the tanh form h + h tanh(h), h = x / 2,
+// loses every bit of 1 + tanh(h) for x <~ -4).  Two MUFU ops (ex2, rcp; relative errors ~2^-22 and ~2^-23) and three on the
+// FMA pipe: a Newton reciprocal instead of rcp measured slower in the GroupNorm apply.  Relative error <= 2^-20 + 2^-23 |x|
+// (|x| from the rounding of -x log2 e); 0 for x in (-103, -87), where 1 + e leaves rcp.approx.ftz's range though silu is a
+// normal fp32 number; NaN for NaN and -inf, as torch's.
 __device__ __forceinline__ float silu_f(float x) {
-  const float h = 0.5f * x;
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
-  return fmaf(h, t, h);
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-1.44269504088896341f * x));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.f + e));
+  return x * r;
 }
 
 }  // namespace k2

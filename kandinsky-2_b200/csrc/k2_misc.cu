@@ -118,6 +118,10 @@ __global__ void __launch_bounds__(256) linear_kernel(const float* __restrict__ x
         }
       }
     }
+    // the xor butterfly leaves the same bits in every lane: lane cb * LIN_MT + i keeps output (i, cb), so the bias / SiLU / add
+    // epilogue is evaluated once per lane instead of 32 times in lane 0
+    static_assert(LIN_CB * LIN_MT == 32, "one output per lane");
+    float mine = 0.f;
 #pragma unroll
     for (int cb = 0; cb < LIN_CB; ++cb) {
 #pragma unroll
@@ -125,13 +129,17 @@ __global__ void __launch_bounds__(256) linear_kernel(const float* __restrict__ x
         float v = acc[cb][i];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        const int n = n0 + cb;
-        if (lane == 0 && i < mt && n < N) {
-          if (b) v += b[n];
-          if (silu_out) v = silu_f(v);
-          if (add) v += add[static_cast<long long>(m0 + i) * ldadd + n];
-          y[static_cast<long long>(m0 + i) * ldy + n] = v;
-        }
+        if (lane == cb * LIN_MT + i) mine = v;
+      }
+    }
+    {
+      const int i = lane % LIN_MT, n = n0 + lane / LIN_MT;
+      if (i < mt && n < N) {
+        float v = mine;
+        if (b) v += b[n];
+        if (silu_out) v = silu_f(v);
+        if (add) v += add[static_cast<long long>(m0 + i) * ldadd + n];
+        y[static_cast<long long>(m0 + i) * ldy + n] = v;
       }
     }
   }

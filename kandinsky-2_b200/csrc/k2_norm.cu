@@ -52,7 +52,8 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 // statistics: grid (chunks, channel tiles, images); per-channel partial sums -> last block of an image
 // folds them into per-group mean / rstd in fp64, fixed order.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict__ s0, int C0, int ld0,
+// 4 resident blocks per SM: the wave pick_chunk sizes (the default register budget spills the fp64 fold)
+__global__ void __launch_bounds__(256, 4) gn_stats_kernel(const __half* __restrict__ s0, int C0, int ld0,
                                                        const __half* __restrict__ s1, int C1, int ld1, int HW,
                                                        int groups, float eps, int chunk, float* __restrict__ stats,
                                                        float* __restrict__ partial, unsigned int* __restrict__ counters) {
@@ -69,6 +70,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
   const int p1 = min(HW, p0 + chunk);
   pdl_wait();
   pdl_launch();
+  // sums of d = x - pivot, pivot = the channel's value at the image's first pixel (every chunk reads the same one): d is of
+  // the order of the channel's spread (exact in fp32 unless x and the pivot are more than ~12 binades apart), so the fp32 sums
+  // of d and d^2 keep their precision whatever the mean
   float a[16];
 #pragma unroll
   for (int e = 0; e < 16; ++e) a[e] = 0.f;
@@ -77,6 +81,8 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
     const __half* base = (c < C0) ? (s0 + c) : (s1 + (c - C0));
     const int ld = (c < C0) ? ld0 : ld1;
     const long long row0 = static_cast<long long>(n) * HW;
+    float piv[8];
+    unpack8(ldg16(base + row0 * ld), piv);
     int p = p0 + py;
     for (; p + (UNR - 1) * PY < p1; p += UNR * PY) {
       uint4 raw[UNR];
@@ -88,8 +94,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
         unpack8(raw[u], f);
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          a[e] += f[e];
-          a[8 + e] = fmaf(f[e], f[e], a[8 + e]);
+          const float d = f[e] - piv[e];
+          a[e] += d;
+          a[8 + e] = fmaf(d, d, a[8 + e]);
         }
       }
     }
@@ -98,8 +105,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
       unpack8(ldg16(base + (row0 + p) * ld), f);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        a[e] += f[e];
-        a[8 + e] = fmaf(f[e], f[e], a[8 + e]);
+        const float d = f[e] - piv[e];
+        a[e] += d;
+        a[8 + e] = fmaf(d, d, a[8 + e]);
       }
     }
   }
@@ -126,36 +134,48 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  // fold: thread t -> group t/8, slice t%8 of that group's (chunk, channel) pairs; then a fixed-order shuffle sum
+  // fold: thread t -> group t/8, slice t%8 of that group's (chunk, channel) pairs; then a fixed-order shuffle sum.  In fp64,
+  // every channel's sums are moved from its own pivot p_c to the group's K = p of its first channel:
+  //   sum (x - K) = sum d + HW (p_c - K),   sum (x - K)^2 = sum d^2 + 2 (p_c - K) sum d + HW (p_c - K)^2
   const int cpg = C / groups;
   const double cnt = static_cast<double>(HW) * cpg;
   const float* pn = partial + static_cast<long long>(n) * chunks * C * 2;
+  const long long row0 = static_cast<long long>(n) * HW;
   for (int g0 = 0; g0 < groups; g0 += 32) {
     const int g = g0 + threadIdx.x / 8;
     const int sub = threadIdx.x % 8;
-    double s = 0.0, q = 0.0;
+    double s = 0.0, q = 0.0, K = 0.0;
     if (g < groups) {
+      auto pivot = [&](int c) { return __half2float(*src_ptr(s0, C0, ld0, s1, ld1, row0, c)); };
+      K = pivot(g * cpg);
+      for (int j = sub; j < cpg; j += 8) {
+        const double dk = static_cast<double>(pivot(g * cpg + j)) - K;
+        s += HW * dk;
+        q += HW * dk * dk;
+      }
       const int items = chunks * cpg;
       int i = sub;
       for (; i + 56 < items; i += 64) {  // 8 independent loads in flight
         float2 t[8];
+        float pc[8];
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
           const int ii = i + 8 * u;
           const int ch = ii / cpg, c = g * cpg + (ii - ch * cpg);
           t[u] = __ldcg(reinterpret_cast<const float2*>(pn + (static_cast<long long>(ch) * C + c) * 2));
+          pc[u] = pivot(c);
         }
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
           s += static_cast<double>(t[u].x);
-          q += static_cast<double>(t[u].y);
+          q += static_cast<double>(t[u].y) + 2.0 * (pc[u] - K) * t[u].x;
         }
       }
       for (; i < items; i += 8) {
         const int ch = i / cpg, c = g * cpg + (i - ch * cpg);
         const float2 t = __ldcg(reinterpret_cast<const float2*>(pn + (static_cast<long long>(ch) * C + c) * 2));
         s += static_cast<double>(t.x);
-        q += static_cast<double>(t.y);
+        q += static_cast<double>(t.y) + 2.0 * (static_cast<double>(pivot(c)) - K) * t.x;
       }
     }
 #pragma unroll
@@ -164,8 +184,9 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const __half* __restrict_
       q += __shfl_down_sync(0xffffffffu, q, o, 8);
     }
     if (g < groups && sub == 0) {
-      const double mean = s / cnt;
-      double var = q / cnt - mean * mean;
+      const double ms = s / cnt;
+      const double mean = K + ms;
+      double var = q / cnt - ms * ms;
       if (var < 0.0) var = 0.0;
       stats[(static_cast<long long>(n) * groups + g) * 2] = static_cast<float>(mean);
       stats[(static_cast<long long>(n) * groups + g) * 2 + 1] =
@@ -190,8 +211,9 @@ __global__ void __launch_bounds__(FIN_T) gn_finalize_kernel(const float2* __rest
   const int cpg = C / groups;
   pdl_wait();
   pdl_launch();
-  // 4 independent fp32 accumulator pairs per thread (loads in flight), folded in fp64 in a fixed order
-  float fs[4] = {0.f, 0.f, 0.f, 0.f}, fq[4] = {0.f, 0.f, 0.f, 0.f};
+  // 4 independent accumulator pairs per thread (loads in flight), fp64 from the first partial on: the partials are raw
+  // (sum, sumsq) of x, so the variance q / cnt - mean^2 cancels, and fp32 accumulation error would be multiplied by (mean / std)^2
+  double fs[4] = {0.0, 0.0, 0.0, 0.0}, fq[4] = {0.0, 0.0, 0.0, 0.0};
   // the group's channels [c_lo, c_hi) restricted to one source: part[(n*rgs + rg)][c - base]
   auto fold = [&](const float2* part, int Cs, int base, int rgs) {
     const int c_lo = max(g * cpg, base), c_hi = min((g + 1) * cpg, base + Cs);
@@ -222,8 +244,8 @@ __global__ void __launch_bounds__(FIN_T) gn_finalize_kernel(const float2* __rest
   };
   fold(part0, C0, 0, rg0);
   if (C1 > 0) fold(part1, C1, C0, rg1);
-  double s = (static_cast<double>(fs[0]) + fs[1]) + (static_cast<double>(fs[2]) + fs[3]);
-  double q = (static_cast<double>(fq[0]) + fq[1]) + (static_cast<double>(fq[2]) + fq[3]);
+  double s = (fs[0] + fs[1]) + (fs[2] + fs[3]);
+  double q = (fq[0] + fq[1]) + (fq[2] + fq[3]);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     s += __shfl_down_sync(0xffffffffu, s, o);
@@ -319,7 +341,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const ApplyParams p) {
     const int g_hi = (c_hi - 1) / cpg;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int g = g_lo + warp; g <= g_hi; g += 8) {
-      float fs = 0.f, fq = 0.f;
+      double fs = 0.0, fq = 0.0;  // fp64 from the first partial on, as in gn_finalize_kernel
       auto fold = [&](const float2* part, int Cs, int base, int rgs) {
         const int lo = max(g * cpg, base), hi = min((g + 1) * cpg, base + Cs);
         const int w = hi - lo;
