@@ -387,6 +387,33 @@ int k2_clip_text_pool(const int* ids, int ldi, int B, int T, int eos_id, const v
                       int* index_out, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Kandinsky 2.1 text encoder (the reference's MultilingualCLIP: XLM-RoBERTa-large and a Linear, text_encoders.py:108-122;
+ * kandinsky2/model/text_encoders.py).  Its Linear layers are k2_conv_gemm flat-row GEMMs, its attention is k2_attention_small
+ * (not causal, the attention mask as the key keep-mask), its LayerNorm / GELU are the prior's entry points above; these two
+ * are the rest.
+ *
+ * k2_xlmr_embed: ids int32 [B, ldi] (T used per row) -> out fp16 rows [B * T, ldo]; for row m = b T + t
+ *     p = pad_id                                        if ids[b, t] == pad_id
+ *       = pad_id + #{s <= t : ids[b, s] != pad_id}      otherwise   (transformers' create_position_ids_from_input_ids)
+ *     x[c] = (float(word[ids[b, t], c]) + float(type_row[c])) + float(pos[p, c])      fp32, c < H
+ *     out[m, c] = fp16_rn( fmaf(float((x[c] - mean) * rstd), gamma[c], beta[c]) )
+ *   with mean and rstd = 1 / sqrt(var + eps) of x in float64 (two passes, as k2_layernorm_f16).  An id outside [0, V) or a
+ *   position p >= P writes a NaN row and reads no table.  word fp16 [V, H], pos fp16 [P, H], type_row fp16 [H] (contiguous),
+ *   gamma / beta fp32 [H].  H <= 8192, pad_id >= 0, eps > 0, ldi >= T, ldo >= H; ids / gamma / beta 4-byte and word / pos /
+ *   type_row / out 2-byte aligned; columns >= H are not touched.
+ * k2_masked_mean_f16: hidden fp16 rows [B * T, ldh], mask uint8 [B, ldm] (nonzero = kept) ->
+ *     out[b, c] = (sum over kept t, ascending, of float(hidden[(b T + t) ldh + c]) in fp32) / count_b      fp32 [B, ldo]
+ *   one division; a row with no kept token is NaN (0 / 0, as torch).  ldh >= H, ldm >= T, ldo >= H, B <= 65535; hidden
+ *   2-byte and out 4-byte aligned.
+ * Both check their arguments before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+int k2_xlmr_embed(const int* ids, int ldi, int B, int T, int pad_id, const void* word, int V, const void* pos, int P,
+                  const void* type_row, const float* gamma, const float* beta, float eps, void* out, int ldo, int H,
+                  k2_stream_t stream);
+int k2_masked_mean_f16(const void* hidden, int ldh, const unsigned char* mask, int ldm, int B, int T, int H, float* out,
+                       int ldo, k2_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
  * fuse_lora): once per adapter load, never per step.
  *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols

@@ -52,6 +52,8 @@ SIGNATURES = {
     "k2_attention_heads": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P, _I, _I, _P]),
     "k2_clip_text_embed": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _P, _I, _P]),
     "k2_clip_text_pool": (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _P, _I, _P, _P]),
+    "k2_xlmr_embed": (_I, [_P, _I, _I, _I, _I, _P, _I, _P, _I, _P, _P, _P, _F, _P, _I, _I, _P]),
+    "k2_masked_mean_f16": (_I, [_P, _I, _P, _I, _I, _I, _I, _P, _I, _P]),
     "k2_conv_plan": (_I, [_I, _I, _I, _I, _I, _I, _I, _LL, _I, _P]),
     "k2_gn_scratch_floats": (_LL, [_I, _I, _I]),
     "k2_gn_stats": (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _F, _P, _P, _P]),

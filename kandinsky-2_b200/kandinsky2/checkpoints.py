@@ -21,6 +21,10 @@
   `CLIPTextModelWithProjection` (subfolder `text_encoder`), goes the same way through `transformers_clip_text_to_k2` into
   `model.clip_text.CLIPTextTower` names (tests/test_cpu_clip_text.py).
 
+* Kandinsky 2.1's text encoder (`2_1/text_encoder/pytorch_model.bin`, the reference's `MultilingualCLIP`:
+  XLM-RoBERTa-large and a Linear, `model/text_encoders.py:108-122`) goes through `mclip_to_k2` into
+  `model.text_encoders.MultilingualCLIP` names (tests/test_cpu_text_encoder.py).
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -348,3 +352,52 @@ def transformers_clip_text_to_k2(sd):
     where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads, head width 64).  A `position_ids`
     buffer (older checkpoints carry it) is ignored; unknown and missing keys raise K2Error naming them."""
     return _clip_to_k2(sd, "text", 64)
+
+
+# the M-CLIP text encoder (Kandinsky 2.1's text_encoder/pytorch_model.bin): this package's name -> the checkpoint's name
+_MCLIP_TOP = {"word_embedding": "transformer.embeddings.word_embeddings.weight",
+              "position_embedding": "transformer.embeddings.position_embeddings.weight",
+              "token_type_embedding": "transformer.embeddings.token_type_embeddings.weight",
+              "emb_ln.weight": "transformer.embeddings.LayerNorm.weight", "emb_ln.bias": "transformer.embeddings.LayerNorm.bias",
+              "proj.weight": "LinearTransformation.weight", "proj.bias": "LinearTransformation.bias"}
+_MCLIP_LAYER = {"attention.output.dense": "attn.proj", "attention.output.LayerNorm": "ln_1", "intermediate.dense": "mlp.fc1",
+                "output.dense": "mlp.fc2", "output.LayerNorm": "ln_2"}
+
+
+def mclip_keys(layers):
+    """Every key of the reference's MultilingualCLIP state dict with `layers` XLM-R layers, without the ones mclip_to_k2
+    ignores (transformer.pooler.*, transformer.embeddings.position_ids)."""
+    keys = list(_MCLIP_TOP.values())
+    for i in range(layers):
+        lp = f"transformer.encoder.layer.{i}."
+        keys += [f"{lp}{d}.{s}" for d in (*_MCLIP_LAYER, "attention.self.query", "attention.self.key", "attention.self.value")
+                 for s in ("weight", "bias")]
+    return keys
+
+
+def mclip_to_k2(sd, layers, head_dim=64):
+    """The reference's MultilingualCLIP state dict (text_encoders.py:108-122: `transformer` an XLMRobertaModel,
+    `LinearTransformation` the 1024 -> 768 Linear) -> `model.text_encoders.MultilingualCLIP` names:
+        word_embedding [V, H], position_embedding [P, H], token_type_embedding [types, H], emb_ln.*, proj.{weight, bias},
+        layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}
+    with ln_1 = attention.output.LayerNorm, ln_2 = output.LayerNorm and attn.qkv stacking attention.self.{query,key,value}
+    per head [q_h | k_h | v_h] (pack_heads).  transformer.pooler.* (unused by the reference's forward) and the
+    embeddings.position_ids buffer are ignored.  Any other unknown key, and any missing one, raises K2Error naming it: the
+    reference loads with strict=False, which would silently keep random weights there."""
+    sd = {k: v for k, v in sd.items()
+          if not k.startswith("transformer.pooler.") and k != "transformer.embeddings.position_ids"}
+    expected = mclip_keys(layers)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"M-CLIP text encoder state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {k: sd[d] for k, d in _MCLIP_TOP.items()}
+    for i in range(layers):
+        dp, kp = f"transformer.encoder.layer.{i}.", f"layers.{i}."
+        for d, k in _MCLIP_LAYER.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}attention.self.{n}.{s}"] for n in ("query", "key", "value")],
+                                                   head_dim)
+    return out

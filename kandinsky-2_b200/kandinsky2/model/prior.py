@@ -194,6 +194,7 @@ class PriorEmbedder:
     deterministic stand-ins:
         clip_text(list[str])  -> (txt_feat [n, clip_dim], txt_feat_seq [n, text_ctx, clip_xf_width], mask [n, text_ctx] bool)
         text_encoder(prompt, batch_size) -> (full_emb [2B, L, D1], pooled_emb [2B, D2])           (2.1 decoder only)
+    The 2.1 text_encoder comes with this package: model.text_encoders.MultilingualCLIP.from_pretrained(dir).
         clip_image(PIL.Image) -> [1, clip_dim]                                                    (mix_images with images)
     """
 

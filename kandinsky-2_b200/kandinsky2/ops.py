@@ -713,3 +713,52 @@ def clip_text_pool(ids, hidden, eos_id, out=None, index_out=None):
     check(nat.load().k2_clip_text_pool(ptr(ids), ldi, B, T, int(eos_id), ptr(hidden), _row_stride(hidden), H, ptr(out), ldo,
                                        ptr(index_out), stream_ptr()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Kandinsky 2.1 text encoder (kandinsky2/model/text_encoders.py, see k2b200.h)
+# ------------------------------------------------------------------------------------------------
+def xlmr_embed(ids, pad_id, word, pos, type_row, gamma, beta, eps, out=None):
+    """k2_xlmr_embed: int32 ids [B, T] (row-strided view) -> fp16 rows [B, T, H] (out may be row-strided) =
+    LayerNorm(word[id] + type_row + pos[p]) with the position p computed from the row's ids (pad_id + the count of non-pad
+    ids up to t; pad_id on a pad id), fp32 sum, float64 statistics, one rounding.  An id outside [0, V) or a position beyond
+    the table gives a NaN row."""
+    tensors = (ids, word, pos, type_row, gamma, beta) + ((out,) if out is not None else ())
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error("xlmr_embed: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    ldi, B, T = _rows_2d(ids, torch.int32, "ids")
+    assert word.dtype == pos.dtype == type_row.dtype == torch.float16, (word.dtype, pos.dtype, type_row.dtype)
+    assert word.is_contiguous() and pos.is_contiguous() and type_row.is_contiguous()
+    V, H = word.shape
+    P = pos.shape[0]
+    assert pos.dim() == 2 and pos.shape[1] == H and type_row.numel() == H, (tuple(pos.shape), tuple(type_row.shape), H)
+    for t in (gamma, beta):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == H, (t.dtype, tuple(t.shape), H)
+    if out is None:
+        out = torch.empty((B, T, H), dtype=torch.float16, device=ids.device)
+    assert out.dtype == torch.float16 and tuple(out.shape) == (B, T, H), (out.dtype, tuple(out.shape))
+    check(nat.load().k2_xlmr_embed(ptr(ids), ldi, B, T, int(pad_id), ptr(word), V, ptr(pos), P, ptr(type_row), ptr(gamma),
+                                   ptr(beta), float(eps), ptr(out), _row_stride(out), H, stream_ptr()))
+    return out
+
+
+def masked_mean_f16(hidden, mask, out=None):
+    """k2_masked_mean_f16: fp16 hidden [B, T, H] (row-strided), uint8 / bool mask [B, T] (row-strided, nonzero = kept) -> fp32
+    [B, H] (out may be row-strided): the kept rows' fp32 sum in ascending t divided once by their count; NaN for a row with
+    no kept token."""
+    tensors = (hidden, mask) + ((out,) if out is not None else ())
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error("masked_mean_f16: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    if mask.dtype == torch.bool:
+        mask = mask.view(torch.uint8)
+    ldm, B, T = _rows_2d(mask, torch.uint8, "mask")
+    assert hidden.dtype == torch.float16 and hidden.dim() == 3 and tuple(hidden.shape[:2]) == (B, T), \
+        (hidden.dtype, tuple(hidden.shape))
+    H = hidden.shape[2]
+    if out is None:
+        out = torch.empty((B, H), dtype=torch.float32, device=hidden.device)
+    ldo, mo, no = _rows_2d(out, torch.float32, "out")
+    assert (mo, no) == (B, H), (tuple(out.shape), B, H)
+    check(nat.load().k2_masked_mean_f16(ptr(hidden), _row_stride(hidden), ptr(mask), ldm, B, T, H, ptr(out), ldo,
+                                        stream_ptr()))
+    return out
