@@ -55,7 +55,8 @@ int k2_set_tuning(int key, int value);
  * same output; source s has `taps` = 9 (3x3, zero padding 1) or 1 (1x1).  Packed weights Wp are fp16
  * [w_rows >= Cout][Ktot], K contiguous, k ordered source-major, then tap (ky*3+kx), then channel, each
  * source's channel count padded to a multiple of 64 (zero weights for the padding).
- * out_mode 0: fp16 rows [M, ldo]; out_mode 1: fp32 NCHW [NB, Cout, H, W] (output heads).
+ * out_mode 0: fp16 rows [M, ldo]; out_mode 1: fp32 NCHW [NB, Cout, H, W] (output heads), which takes no residual
+ * (residual must be NULL); any other out_mode is refused.  Both checks happen before any CUDA call.
  * ldw is the row stride of Wp in elements (0 = Ktot); a strided Wp lets an ACTIVATION matrix be the B operand
  * (MoVQ attention: scores = q k^T with k rows as "weights").
  * workspace (may be NULL): caller-owned scratch for split-K.  Where a cycle model of the launch (waves of work units x

@@ -296,6 +296,9 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
                      int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
                      const int* cfg, long long w_batch_stride, k2_stream_t stream) {
   K2_REQUIRE(w_batch_stride >= 0 && w_batch_stride % 8 == 0, "conv_gemm_cfg: w_batch_stride must be a multiple of 8 elements");
+  // out_mode 2 (raw fp32 split-K partials into the workspace) is internal: the split-K plan sets it and adds the finalize pass
+  K2_REQUIRE(out_mode == 0 || out_mode == 1, "conv_gemm: out_mode must be 0 (fp16 rows) or 1 (fp32 NCHW)");
+  K2_REQUIRE(out_mode == 0 || residual == nullptr, "conv_gemm: out_mode 1 (fp32 NCHW) takes no residual");
   const bool w_batched = w_batch_stride > 0;
   if (cfg) {
     K2_REQUIRE(cfg[0] == 0 || cfg[0] == 16 || cfg[0] == 64 || cfg[0] == 128 || cfg[0] == 192 || cfg[0] == 256,

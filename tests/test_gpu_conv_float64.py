@@ -49,12 +49,14 @@ def _up2_conv64(x_nhwc, wp, cin, cout):
     return out, wabs
 
 
-def _check(y, ref, absum, k_terms):
-    """|y - ref| <= fp16 rounding of the output + fp32 accumulation error over k_terms products (+ subnormal step)."""
-    bound = EPS16 * ref.abs() + 1.01 * k_terms * EPS32 * absum + TINY
+def _check(y, ref, absum, k_terms, eps_out=EPS16):
+    """|y - ref| <= rounding of the output (eps_out relative: fp16 by default, 0 for fp32 outputs) + fp32 accumulation error
+    over k_terms products (+ subnormal step).  Returns the worst share of the bound."""
+    bound = eps_out * ref.abs() + 1.01 * k_terms * EPS32 * absum + TINY
     err = (y.double() - ref).abs()
     worst = (err / bound).max().item()
     assert worst <= 1.0, f"error exceeds the fp32-accumulation bound by {worst:.3f}x (max abs err {err.max().item():.3e})"
+    return worst
 
 
 def _case(g, NB, H, W, C, Cout, *, taps=9, strided=False, residual=False, skips=None, split=0, gn=False):
