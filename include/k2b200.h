@@ -331,6 +331,12 @@ int k2_transpose_f16(const void* x, int ldx, void* y, int B, int T, int C, k2_st
 int k2_layernorm_f16(const void* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int M, int N, float eps,
                      k2_stream_t stream);
 int k2_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream);
+/* OpenAI CLIP's QuickGELU (the Kandinsky 2.1 ViT-L/14 text and image towers, kandinsky2/model/clip_vitl14.py) on n fp16
+ * elements, may run in place (x == y):
+ *   y[i] = fp16_rn( x / (1 + exp(-1.702 x)) )   in fp32, x = float(x[i]); within one fp16 ulp of x sigmoid(1.702 x) in float64
+ * +inf -> +inf, -inf -> NaN, NaN -> NaN (torch's fp32 x * sigmoid(1.702 x)).  n positive and even, x / y 4-byte aligned;
+ * arguments are checked before any CUDA call. */
+int k2_quick_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream);
 int k2_attention_small(const void* qkv, int ldq, const unsigned char* keep_mask, int causal, void* out, int ldo, int B, int T,
                        int heads, float scale, k2_stream_t stream);
 /* Token rows of the prior's sequence, bit-identical to the eager forward's `seq[:, j] = v.half()` followed by the fp16

@@ -12,6 +12,8 @@
 //   layernorm_f16    N = 1..2049, rows offset by up to 1000 std, constant rows (exactly fp16(beta)), a 3e4 channel, variance
 //                    below eps: within 1 ulp plus 2^-20 (|gamma x_hat| + |beta|); worst 1.34 ulp, on outputs that cancel.
 //   gelu_f16         all 65536 fp16 inputs: within 1 ulp of 0.5 x erfc(-x / sqrt 2); worst 0.50 ulp (all correctly rounded).
+//   quick_gelu_f16   (the 2.1 ViT-L/14 towers' QuickGELU; tests/test_gpu_clip_vitl14_kernels.py) all 65536 fp16 inputs:
+//                    within 1 ulp of x sigmoid(1.702 x); worst 0.500 ulp, 99.995 % correctly rounded.
 // tests/test_gpu_zz_prior.py pins the whole prior to tests/golden/prior_tiny.pt (the reference's own classes), and
 // tests/test_gpu_zz_prior_full.py runs the full 2.1 prior against the fp32 oracle.  Nothing on the measured denoising path
 // calls these entry points; they are not tuned.
@@ -74,6 +76,22 @@ __global__ void __launch_bounds__(256) gelu_f16_kernel(const __half2* __restrict
     const float2 v = __half22float2(x[i]);
     const float a = 0.5f * v.x * erfcf(v.x * -0.70710678118654752f);
     const float c = 0.5f * v.y * erfcf(v.y * -0.70710678118654752f);
+    y[i] = __floats2half2_rn(a, c);
+  }
+}
+
+// OpenAI CLIP's QuickGELU, x sigmoid(1.702 x), on fp16, in place or out of place (the Kandinsky 2.1 ViT-L/14 towers,
+// kandinsky2/model/clip_vitl14.py), as x / (1 + exp(-1.702 x)) in fp32 with one final rounding.  The form keeps its relative
+// accuracy everywhere: for x >> 0 the denominator is 1 + (tiny), for x << 0 it is exp(...) with no cancellation, and once
+// exp overflows (x < -52) the quotient is -0, which is also the correctly rounded fp16 value.  Over all fp16 inputs it is within
+// 0.51 ulp of the float64 value.  +-inf and NaN map as in torch's fp32 x * sigmoid(1.702 x): +inf, NaN (-inf / inf), NaN.
+__global__ void __launch_bounds__(256) quick_gelu_f16_kernel(const __half2* __restrict__ x, __half2* __restrict__ y,
+                                                             long long n2) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n2;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float2 v = __half22float2(x[i]);
+    const float a = v.x / (1.f + expf(-1.702f * v.x));
+    const float c = v.y / (1.f + expf(-1.702f * v.y));
     y[i] = __floats2half2_rn(a, c);
   }
 }
@@ -201,6 +219,19 @@ int k2_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream) {
   long long blocks = (n / 2 + 255) / 256;
   if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   gelu_f16_kernel<<<static_cast<unsigned int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __half2*>(x), reinterpret_cast<__half2*>(y), n / 2);
+  K2_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int k2_quick_gelu_f16(const void* x, void* y, long long n, k2_stream_t stream) {
+  K2_REQUIRE(x && y && n > 0 && n % 2 == 0, "quick_gelu_f16: n must be a positive even element count");
+  K2_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 3) == 0,
+             "quick_gelu_f16: 4-byte alignment");
+  long long blocks = (n / 2 + 255) / 256;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+  quick_gelu_f16_kernel<<<static_cast<unsigned int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __half2*>(x), reinterpret_cast<__half2*>(y), n / 2);
   K2_CHECK_CUDA(cudaGetLastError());
   count_launch();

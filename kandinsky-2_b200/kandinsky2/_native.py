@@ -45,6 +45,7 @@ SIGNATURES = {
     "k2_softmax_rows": (_I, [_P, _I, _P, _I, _LL, _I, _F, _P]),
     "k2_layernorm_f16": (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _F, _P]),
     "k2_gelu_f16": (_I, [_P, _P, _LL, _P]),
+    "k2_quick_gelu_f16": (_I, [_P, _P, _LL, _P]),
     "k2_attention_small": (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _F, _P]),
     "k2_prior_tokens": (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _P]),
     "k2_f16_to_f32": (_I, [_P, _I, _P, _I, _I, _I, _P]),

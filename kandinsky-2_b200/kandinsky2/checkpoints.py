@@ -25,6 +25,9 @@
   XLM-RoBERTa-large and a Linear, `model/text_encoders.py:108-122`) goes through `mclip_to_k2` into
   `model.text_encoders.MultilingualCLIP` names (tests/test_cpu_text_encoder.py).
 
+* Kandinsky 2.1's CLIP ViT-L/14 (`ViT-L-14.pt`, an OpenAI `clip` checkpoint) goes through `openai_clip_to_k2` into the
+  text and image tower names above, with the geometry read from the shapes (tests/test_cpu_clip_vitl14.py).
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -35,6 +38,8 @@ build container, so the diffusers-side key names below are restated from the pub
 are inverse bijections onto the package's exact key set, and the head-interleaved packing reproduces separate
 q / k / v projections numerically.
 """
+import math
+import os
 import re
 
 import torch
@@ -401,3 +406,119 @@ def mclip_to_k2(sd, layers, head_dim=64):
             out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}attention.self.{n}.{s}"] for n in ("query", "key", "value")],
                                                    head_dim)
     return out
+
+
+# the OpenAI `clip` checkpoint (Kandinsky 2.1's ViT-L-14.pt; clip/model.py build_model reads it): one resblock's names
+_OPENAI_LAYER = {"ln_1": "ln_1", "ln_2": "ln_2", "attn.out_proj": "attn.proj", "mlp.c_fc": "mlp.fc1", "mlp.c_proj": "mlp.fc2"}
+# the entries build_model deletes before loading, and the contrastive temperature neither tower uses
+_OPENAI_IGNORED = ("input_resolution", "context_length", "vocab_size", "logit_scale")
+
+
+def openai_clip_keys(text_layers, vision_layers):
+    """Every key of an OpenAI CLIP (ViT) state dict with the given resblock counts, without the ones openai_clip_to_k2
+    ignores."""
+    keys = ["token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection",
+            "visual.class_embedding", "visual.positional_embedding", "visual.conv1.weight", "visual.ln_pre.weight",
+            "visual.ln_pre.bias", "visual.ln_post.weight", "visual.ln_post.bias", "visual.proj"]
+    for prefix, n in (("transformer.", text_layers), ("visual.transformer.", vision_layers)):
+        for i in range(n):
+            lp = f"{prefix}resblocks.{i}."
+            keys += [f"{lp}{d}.{s}" for d in _OPENAI_LAYER for s in ("weight", "bias")]
+            keys += [f"{lp}attn.in_proj_weight", f"{lp}attn.in_proj_bias"]
+    return keys
+
+
+def openai_clip_geometry(sd):
+    """The geometry of an OpenAI CLIP (ViT) state dict, read from the tensor shapes as clip/model.py build_model does (there
+    is no config): {"text": dict(width, layers, heads, mlp, context, vocab, embed_dim), "vision": dict(width, layers, heads,
+    mlp, patch, grid, tokens, image_size, embed_dim)}; heads are of width 64.  K2Error names a key the geometry needs and
+    the dict lacks."""
+    need = ("ln_final.weight", "visual.conv1.weight", "positional_embedding", "visual.positional_embedding",
+            "token_embedding.weight", "text_projection", "visual.proj")
+    missing = [k for k in need if k not in sd]
+    if missing:
+        raise K2Error(f"OpenAI CLIP state dict: missing keys {missing}")
+
+    def layers(prefix):
+        return sum(1 for k in sd if re.fullmatch(rf"{re.escape(prefix)}resblocks\.\d+\.attn\.in_proj_weight", k))
+
+    tw, vw = sd["ln_final.weight"].shape[0], sd["visual.conv1.weight"].shape[0]
+    P, T = sd["visual.conv1.weight"].shape[-1], sd["visual.positional_embedding"].shape[0]
+    G = math.isqrt(T - 1)
+    for name, w in (("text", tw), ("vision", vw)):
+        if w % 64:
+            raise K2Error(f"OpenAI CLIP {name} tower: width {w} is not a multiple of the head width 64")
+    if G * G != T - 1:
+        raise K2Error(f"OpenAI CLIP vision tower: {T} positions are not a square grid plus the class token")
+    text = dict(width=tw, layers=layers("transformer."), heads=tw // 64, mlp=4 * tw,
+                context=sd["positional_embedding"].shape[0], vocab=sd["token_embedding.weight"].shape[0],
+                embed_dim=sd["text_projection"].shape[1])
+    vision = dict(width=vw, layers=layers("visual.transformer."), heads=vw // 64, mlp=4 * vw, patch=P, grid=G, tokens=T,
+                  image_size=P * G, embed_dim=sd["visual.proj"].shape[1])
+    return {"text": text, "vision": vision}
+
+
+def openai_clip_to_k2(sd):
+    """OpenAI CLIP (ViT) state dict (`clip.load(..., jit=False)` builds its model from it; Kandinsky 2.1's ViT-L-14.pt) ->
+    (text, vision, geometry): the two towers' state dicts in this package's names (those of model/clip_text.py and
+    model/clip_vision.py) and openai_clip_geometry(sd).
+        text:    token_embedding, position_embedding, final_ln.*, proj.weight, layers.{i}.*
+        vision:  class_embedding, patch_embedding.weight, position_embedding, pre_ln.*, post_ln.*, proj.weight, layers.{i}.*
+    with layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias}: attn.in_proj_{weight,bias} ([q; k; v])
+    re-packed per 64-wide head [q_h | k_h | v_h] (pack_heads), attn.out_proj -> attn.proj, mlp.c_fc -> mlp.fc1, mlp.c_proj ->
+    mlp.fc2.  text_projection and visual.proj are applied as x @ P there and become the Linear weights P^T here.
+    input_resolution / context_length / vocab_size (the entries build_model deletes) and logit_scale are ignored; any other
+    unknown key, and any missing one, raises K2Error naming it."""
+    sd = {k: v for k, v in sd.items() if k not in _OPENAI_IGNORED}
+    geo = openai_clip_geometry(sd)
+    expected = openai_clip_keys(geo["text"]["layers"], geo["vision"]["layers"])
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"OpenAI CLIP state dict: unknown keys {unknown}, missing keys {missing}")
+
+    def layers(prefix, n, width):
+        out = {}
+        for i in range(n):
+            dp, kp = f"{prefix}resblocks.{i}.", f"layers.{i}."
+            for d, k in _OPENAI_LAYER.items():
+                for s in ("weight", "bias"):
+                    out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+            for s in ("weight", "bias"):
+                w = sd[f"{dp}attn.in_proj_{s}"]
+                if w.shape[0] != 3 * width:
+                    raise K2Error(f"OpenAI CLIP state dict: {dp}attn.in_proj_{s} has {w.shape[0]} rows, not 3 x {width}")
+                out[f"{kp}attn.qkv.{s}"] = pack_heads(list(w.split(width, 0)), 64)
+        return out
+
+    t, v = geo["text"], geo["vision"]
+    text = {"token_embedding": sd["token_embedding.weight"], "position_embedding": sd["positional_embedding"],
+            "final_ln.weight": sd["ln_final.weight"], "final_ln.bias": sd["ln_final.bias"],
+            "proj.weight": sd["text_projection"].t().contiguous()}
+    text.update(layers("transformer.", t["layers"], t["width"]))
+    vision = {"class_embedding": sd["visual.class_embedding"], "patch_embedding.weight": sd["visual.conv1.weight"],
+              "position_embedding": sd["visual.positional_embedding"], "pre_ln.weight": sd["visual.ln_pre.weight"],
+              "pre_ln.bias": sd["visual.ln_pre.bias"], "post_ln.weight": sd["visual.ln_post.weight"],
+              "post_ln.bias": sd["visual.ln_post.bias"], "proj.weight": sd["visual.proj"].t().contiguous()}
+    vision.update(layers("visual.transformer.", v["layers"], v["width"]))
+    return text, vision, geo
+
+
+def load_openai_clip(path_or_sd):
+    """An OpenAI CLIP state dict from a path or as given: a TorchScript archive (what the `clip` package downloads, e.g.
+    ViT-L-14.pt: torch.jit.load(...).state_dict()) or a plain torch.save'd state dict.  K2Error names a missing file."""
+    if isinstance(path_or_sd, dict):
+        return dict(path_or_sd)
+    path = os.fspath(path_or_sd)
+    if not os.path.exists(path):
+        raise K2Error(f"OpenAI CLIP checkpoint {path} not found")
+    try:
+        m = torch.jit.load(path, map_location="cpu")
+    except RuntimeError:
+        m = None
+    if m is not None:
+        return {k: v for k, v in m.state_dict().items()}
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    if not isinstance(sd, dict):
+        raise K2Error(f"OpenAI CLIP checkpoint {path}: neither a TorchScript archive nor a state dict")
+    return sd

@@ -281,6 +281,8 @@ class CLIPTextTower:
     by __call__ only).  `tokens` is the sequence length __call__ produces: the tokenizer's model_max_length, or
     max_position_embeddings without a tokenizer."""
 
+    act = "gelu"   # the layers' MLP activation (encoder.ACTIVATIONS)
+
     def __init__(self, sd, config, device="cuda", tokenizer=None):
         c = text_tower_config(config)
         self.cfg, self.device, self.tokenizer = c, torch.device(device), tokenizer
@@ -387,7 +389,7 @@ class _TextPlan(LaunchPlan):
         scale = c["head_dim"] ** -0.5
         h = record_layers(self, x, pk["layers"],
                           lambda qkv, out: ops.attention_small(qkv, heads, keep_mask=None, causal=True, scale=scale, out=out),
-                          4 * n * heads * T * T * c["head_dim"], eps)
+                          4 * n * heads * T * T * c["head_dim"], eps, act=self.t.act)
         self.hidden = self._new(n, T, H)
         S(lambda: ops.layernorm_f16(h, *pk["final_ln"], eps=eps, out=self.hidden), "layernorm")
         pooled = torch.empty(n, H, device=self.dev, dtype=torch.float32)

@@ -108,6 +108,8 @@ class CLIPVisionTower:
     (checkpoints.transformers_clip_vision_to_k2); config: the transformers config.json dict; preprocessor_config: the
     image processor's dict (None = DEFAULT_PREPROCESSOR)."""
 
+    act = "gelu"   # the layers' MLP activation (encoder.ACTIVATIONS)
+
     def __init__(self, sd, config, device="cuda", preprocessor_config=None):
         c = tower_config(config)
         self.cfg, self.device = c, torch.device(device)
@@ -157,6 +159,11 @@ class CLIPVisionTower:
         if B not in self._plans:
             self._plans[B] = _TowerPlan(self, B)
         return self._plans[B]
+
+    def attend(self, qkv, out):
+        """The layers' attention: qkv fp16 [B, T, heads * 3 head_dim] (per head [q | k | v]) -> out fp16 [B, T, hidden]."""
+        c = self.cfg
+        return ops.attention_heads(qkv, c["num_attention_heads"], c["head_dim"], c["head_dim"] ** -0.5, out=out)
 
     def preprocess(self, images):
         """PIL image(s) -> fp32 pixel_values [B, 3, S, S] on the CPU (preprocess_images with this tower's processor config)."""
@@ -213,9 +220,7 @@ class _TowerPlan(LaunchPlan):
         emb, x = self._new(B, T, H), self._new(B, T, H)
         self._gemm(rows, pk["embed"], H, emb, 2 * B * T * c["kp"] * H, residual=self.pos)
         S(lambda: ops.layernorm_f16(emb, *pk["pre_ln"], eps=eps, out=x), "layernorm")
-        scale = hd ** -0.5
-        h = record_layers(self, x, pk["layers"], lambda qkv, out: ops.attention_heads(qkv, heads, hd, scale, out=out),
-                          4 * B * heads * T * T * hd, eps)
+        h = record_layers(self, x, pk["layers"], self.t.attend, 4 * B * heads * T * T * hd, eps, act=self.t.act)
         self.hidden = h
         cls, cls32 = self._new(B, H), torch.empty(B, H, device=self.dev, dtype=torch.float32)
         S(lambda: ops.layernorm_f16(h[:, 0], *pk["post_ln"], eps=eps, out=cls), "layernorm")

@@ -2,7 +2,8 @@
 (model/clip_text.py, model/clip_vision.py): how one layer's weights are named, checked and packed, and the launches one layer
 records in a LaunchPlan:
     LayerNorm -> qkv GEMM -> attention -> out-proj GEMM + residual -> LayerNorm -> fc1 GEMM -> GELU -> fc2 GEMM + residual.
-The attention launch is the caller's; everything else is the same for all three models.  record_layers(post_ln=True)
+The attention launch is the caller's; everything else is the same for all the models (the 2.1 ViT-L/14 towers of
+model/clip_vitl14.py record QuickGELU instead of GELU: record_layers(act="quick_gelu")).  record_layers(post_ln=True)
 records the post-LayerNorm layer of the 2.1 text encoder (model/text_encoders.py, XLM-RoBERTa) over the same packed names.
 Also the part of the transformers CLIP config both towers read."""
 import torch
@@ -12,6 +13,9 @@ from .._native import K2Error
 
 _NORMS = ("ln_1", "ln_2")
 _GEMMS = ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")
+# the MLP activations a layer can record, by name (the name is also the launch's kind): the exact GELU of the prior, the bigG
+# towers and XLM-R, and OpenAI CLIP's QuickGELU x * sigmoid(1.702 x) of the Kandinsky 2.1 ViT-L/14 towers
+ACTIVATIONS = {"gelu": ops.gelu_f16_, "quick_gelu": ops.quick_gelu_f16_}
 
 
 def layer_shapes(H, I):
@@ -35,17 +39,20 @@ def pack_layers(get, L, dev):
     return layers
 
 
-def record_layers(plan, h, layers, attend, attn_flops, eps, post_ln=False):
+def record_layers(plan, h, layers, attend, attn_flops, eps, post_ln=False, act="gelu"):
     """Record the layers (pack_layers) into `plan` over h fp16 [rows, tokens, C]; returns the last layer's output.  The
     buffers are [rows, tokens, C] views so that the GEMM tuner counts rows * tokens output rows.  attend(qkv, out) launches
     the attention of qkv [rows, tokens, 3C] into out [rows, tokens, C]; attn_flops is what one such launch computes.  The
     first layer reads h as its residual input; the stream then alternates between two buffers.  post_ln=True records the
-    post-LayerNorm layer of BERT / XLM-RoBERTa instead (_record_post_ln)."""
+    post-LayerNorm layer of BERT / XLM-RoBERTa instead (_record_post_ln).  act: the MLP activation, an ACTIVATIONS name."""
     rows, tokens, C = h.shape
+    if act not in ACTIVATIONS:
+        raise K2Error(f"encoder layers: activation {act!r} is not implemented (only {sorted(ACTIVATIONS)})")
     if not layers:
         return h
     if post_ln:
-        return _record_post_ln(plan, h, layers, attend, attn_flops, eps)
+        return _record_post_ln(plan, h, layers, attend, attn_flops, eps, act)
+    gelu = ACTIVATIONS[act]
     I, M, S = layers[0]["mlp.fc1"][0].shape[0], rows * tokens, plan._add
     y, att, hA, hB = (plan._new(rows, tokens, C) for _ in range(4))
     qkv, f = plan._new(rows, tokens, 3 * C), plan._new(rows, tokens, I)
@@ -56,19 +63,20 @@ def record_layers(plan, h, layers, attend, attn_flops, eps, post_ln=False):
         plan._gemm(att, L["attn.proj"][0], C, hA, 2 * M * C * C, bias=L["attn.proj"][1], residual=h)
         S(lambda L=L: ops.layernorm_f16(hA, *L["ln_2"], eps=eps, out=y), "layernorm")
         plan._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * C * I, bias=L["mlp.fc1"][1])
-        S(lambda: ops.gelu_f16_(f), "gelu")
+        S(lambda: gelu(f), act)
         plan._gemm(f, L["mlp.fc2"][0], C, hB, 2 * M * I * C, bias=L["mlp.fc2"][1], residual=hA)
         h = hB
     return h
 
 
-def _record_post_ln(plan, h, layers, attend, attn_flops, eps):
+def _record_post_ln(plan, h, layers, attend, attn_flops, eps, act):
     """The post-LayerNorm layer (transformers' XLMRobertaLayer), eight launches:
         qkv GEMM -> attention -> out-proj GEMM + residual -> LayerNorm ln_1 (attention.output.LayerNorm) -> fc1 GEMM -> GELU
         -> fc2 GEMM + residual (ln_1's output) -> LayerNorm ln_2 (output.LayerNorm), whose output is the next layer's input.
     The first layer reads h; the stream then lives in one buffer that every layer overwrites last."""
     rows, tokens, C = h.shape
     I, M, S = layers[0]["mlp.fc1"][0].shape[0], rows * tokens, plan._add
+    gelu = ACTIVATIONS[act]
     att, hA, y, hB, out = (plan._new(rows, tokens, C) for _ in range(5))
     qkv, f = plan._new(rows, tokens, 3 * C), plan._new(rows, tokens, I)
     for L in layers:
@@ -77,7 +85,7 @@ def _record_post_ln(plan, h, layers, attend, attn_flops, eps):
         plan._gemm(att, L["attn.proj"][0], C, hA, 2 * M * C * C, bias=L["attn.proj"][1], residual=h)
         S(lambda L=L: ops.layernorm_f16(hA, *L["ln_1"], eps=eps, out=y), "layernorm")
         plan._gemm(y, L["mlp.fc1"][0], I, f, 2 * M * C * I, bias=L["mlp.fc1"][1])
-        S(lambda: ops.gelu_f16_(f), "gelu")
+        S(lambda: gelu(f), act)
         plan._gemm(f, L["mlp.fc2"][0], C, hB, 2 * M * I * C, bias=L["mlp.fc2"][1], residual=y)
         S(lambda L=L: ops.layernorm_f16(hB, *L["ln_2"], eps=eps, out=out), "layernorm")
         h = out

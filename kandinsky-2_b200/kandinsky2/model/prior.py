@@ -22,6 +22,7 @@ configurations; PriorEmbedder22 puts it behind the embedder protocol (tests/test
 """
 import math
 import os
+import re
 
 import numpy as np
 import torch
@@ -155,6 +156,29 @@ class PriorTransformer(nn.Module):
         return ops.linear(last.float(), self.out_proj.weight.float().contiguous(), self.out_proj.bias.float())
 
 
+def prior_from_state_dict(sd, device="cuda"):
+    """A 2.1 PriorTransformer from its state dict (the reference's names, `prior_fp16.ckpt` without the "model." prefix), the
+    geometry read from the shapes (text_ctx, width, layers, heads of 64, final LayerNorm, clip_dim, clip_xf_width); packed.
+    Unknown and missing keys raise K2Error naming them (the reference loads with strict=False)."""
+    need = ("positional_embedding", "out_proj.weight", "text_enc_proj.weight")
+    if any(k not in sd for k in need):
+        raise K2Error(f"2.1 prior state dict: missing keys {[k for k in need if k not in sd]}")
+    W = sd["positional_embedding"].shape[-1]
+    prior = PriorTransformer(text_ctx=sd["positional_embedding"].shape[1] - 4, xf_width=W,
+                             xf_layers=sum(1 for k in sd if re.fullmatch(r"transformer\.resblocks\.\d+\.attn\.c_qkv\.weight", k)),
+                             xf_heads=W // 64, xf_final_ln="final_ln.weight" in sd, xf_padding="padding_embedding" in sd,
+                             clip_dim=sd["out_proj.weight"].shape[0], clip_xf_width=sd["text_enc_proj.weight"].shape[1],
+                             device=device)
+    want = prior.state_dict()
+    unknown = sorted(set(sd) - set(want))
+    missing = [k for k in want if k not in sd]
+    bad = [k for k in want if k in sd and tuple(sd[k].shape) != tuple(want[k].shape)]
+    if unknown or missing or bad:
+        raise K2Error(f"2.1 prior state dict: unknown keys {unknown}, missing keys {missing}, wrong shapes {bad}")
+    prior.load_state_dict(sd, strict=True)
+    return prior.finalize()
+
+
 def cosine_betas(steps=1000, max_beta=0.999):
     """get_named_beta_schedule('cosine') of the reference (model/utils.py)."""
     f = lambda t: math.cos((t + 0.008) / 1.008 * math.pi / 2) ** 2  # noqa: E731
@@ -205,6 +229,45 @@ class PriorEmbedder:
         self.prior_steps, self.prior_cf_scale, self.negative_prior_prompt = int(prior_steps), float(prior_cf_scale), negative_prior_prompt
         self._zero = zero_image_emb
         self.seed = seed
+
+    @classmethod
+    def from_pretrained(cls, path, clip_path=None, bpe_path=None, device="cuda", **kwargs):
+        """The reference's 2.1 cache folder (`get_kandinsky2` writes it to <cache_dir>/2_1) -> the embedder with every
+        conditioning producer on this package's kernels:
+            prior_fp16.ckpt       the PriorDiffusionModel state dict ("model." stripped; the geometry is read from the shapes)
+            ViT-L-14_stats.th     (clip_mean, clip_std)
+            text_encoder/         the M-CLIP text encoder (text_encoders.MultilingualCLIP.from_pretrained) -> text_encoder
+            ViT-L-14.pt           the OpenAI CLIP checkpoint (clip_path; clip_vitl14.load_openai_clip) -> clip_text,
+                                  clip_image and zero_image_emb (the image tower's zero_embed, computed here once)
+            bpe_simple_vocab_16e6.txt.gz   clip's BPE vocabulary (bpe_path) for the CLIP tokenizer
+        A missing file raises K2Error naming it, and so does a CLIP tower that does not fit the prior (its width, embedding
+        width or context against the prior's clip_xf_width, clip_dim, text_ctx).  kwargs go to the constructor
+        (prior_steps, prior_cf_scale, negative_prior_prompt, seed)."""
+        from .clip_vitl14 import load_openai_clip
+        from .text_encoders import MultilingualCLIP
+        clip_path = os.path.join(path, "ViT-L-14.pt") if clip_path is None else clip_path
+        bpe_path = os.path.join(path, "bpe_simple_vocab_16e6.txt.gz") if bpe_path is None else bpe_path
+        files = [os.path.join(path, "prior_fp16.ckpt"), os.path.join(path, "ViT-L-14_stats.th"),
+                 os.path.join(path, "text_encoder"), clip_path, bpe_path]
+        for f in files:
+            if not os.path.exists(f):
+                raise K2Error(f"PriorEmbedder.from_pretrained: {f} not found")
+        sd = torch.load(files[0], map_location="cpu", weights_only=True)
+        prior = prior_from_state_dict({k[len("model."):] if k.startswith("model.") else k: v for k, v in sd.items()}, device)
+        clip_mean, clip_std = torch.load(files[1], map_location="cpu", weights_only=True)
+        text, image = load_openai_clip(clip_path, device, bpe_path)
+        got = (text.cfg["hidden_size"], text.cfg["projection_dim"], text.tokens)
+        want = (prior.clip_xf_width, prior.clip_dim, prior.text_ctx)
+        if got != want:
+            raise K2Error(f"PriorEmbedder.from_pretrained: the CLIP text tower gives (width, embedding width, context) {got}, "
+                          f"the prior takes (clip_xf_width, clip_dim, text_ctx) {want}")
+        if image.cfg["projection_dim"] != prior.clip_dim:
+            raise K2Error(f"PriorEmbedder.from_pretrained: the CLIP image tower's embedding width "
+                          f"{image.cfg['projection_dim']} is not the prior's clip_dim {prior.clip_dim}")
+        encoder = MultilingualCLIP.from_pretrained(files[2], device=device)
+        dev = torch.device(device)
+        return cls(prior, text, clip_mean.reshape(-1).to(dev, torch.float32), clip_std.reshape(-1).to(dev, torch.float32),
+                   zero_image_emb=image.zero_embed().float().cpu(), text_encoder=encoder, clip_image=image, **kwargs)
 
     @torch.no_grad()
     def image_emb(self, prompt, batch_size):

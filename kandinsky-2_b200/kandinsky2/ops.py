@@ -582,6 +582,18 @@ def gelu_f16_(x):
     return x
 
 
+def quick_gelu_f16_(x, out=None):
+    """OpenAI CLIP's QuickGELU, x * sigmoid(1.702 x), on a contiguous fp16 tensor: in place, or into `out` (contiguous fp16
+    of the same shape)."""
+    if not x.is_cuda or (out is not None and not out.is_cuda):
+        raise nat.K2Error("quick_gelu_f16: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    assert x.dtype == torch.float16 and x.is_contiguous(), (x.dtype, x.stride())
+    out = x if out is None else out
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.shape == x.shape, (out.dtype, tuple(out.shape))
+    check(nat.load().k2_quick_gelu_f16(ptr(x), ptr(out), x.numel(), stream_ptr()))
+    return out
+
+
 def attention_small(qkv, heads, keep_mask=None, causal=True, scale=0.125, out=None):
     """qkv fp16 [B, T, heads*192] (per head [q|k|v]), keep_mask uint8 or bool [B, T] (nonzero = key kept) or None -> fp16
     [B, T, heads*64]; T <= 128.  A query row that can reach no key (every key masked, or causal with key 0 masked) is NaN,
