@@ -316,8 +316,13 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const ApplyParams p) {
   const int v = blockIdx.y * VX + vx;
   const int n = blockIdx.z;
   // Everything that the PREVIOUS kernel of the stream does not produce is fetched before griddepcontrol.wait, i.e. while that
-  // kernel is still draining: gamma / beta are weights, the FiLM rows come from the step's first launches (every kernel waits
-  // for its predecessor before it lets its successor start, so launches <= N-2 are complete when launch N begins).
+  // kernel is still draining: gamma / beta are weights; launches <= N-2 of the stream are complete when launch N begins (every
+  // kernel waits for its predecessor before it lets its successor start).  The FiLM rows come from a branch forked onto a side
+  // stream (model/unet.py) and joined in by an event wait right before the first ResBlock's out-norm, which may be this kernel
+  // (the folded variant).  That join acts as a full dependency, eagerly and as a captured graph, also when the launch after it
+  // is a PDL launch: tests/test_gpu_pdl_plans.py holds the branch back and NaN-fills the FiLM rows before every run and
+  // replay, and the output stays bit-identical to the serialised run (without the join, the same harness reads the NaN).
+  // Reading the rows here relies on that.
   float ga8[8], be8[8], sc8[8], sh8[8];
   {
     const int cc = min(v, CV - 1) * 8;
