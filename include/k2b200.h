@@ -421,6 +421,37 @@ int k2_masked_mean_f16(const void* hidden, int ldh, const unsigned char* mask, i
                        int ldo, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * DPT depth estimator (transformers' DPTForDepthEstimation with a plain ViT backbone, the default model of the
+ * depth-estimation pipeline that builds the Kandinsky 2.2 ControlNet-depth hint; kandinsky2/model/depth.py).  Its Linear
+ * layers and convolutions are k2_conv_gemm launches (ConvTranspose2d(kernel = stride = s) is one GEMM [M, C] x [C, s^2 C]
+ * with the bias tiled s^2 times, followed by k2_depth_to_space_f16), its LayerNorm / GELU / attention are the ViT towers'
+ * entry points above; these are the rest.  Strides are in elements; every argument is checked before any CUDA call.
+ *
+ * k2_relu_f16: y[m, c] = relu(x[m, c]) on fp16 rows (M rows, N columns, strides ldx / ldy >= N), bit for bit torch.relu on
+ *   the GPU: a NaN keeps its bits, anything else is fp16(fmaxf(x, 0)).  x == y (in place) is allowed, other overlap is not.
+ *   2-byte alignment; rows of a multiple of 8 with 16-byte aligned pointers move as 16-byte vectors.
+ * k2_relu_f32: the same on fp32 rows (4-byte alignment).
+ * k2_bilinear_f16: x fp16 NHWC [NB, Hi, Wi, C] rows (pixel stride ldx) -> y fp16 NHWC [NB, Ho, Wo, C] (pixel stride ldy),
+ *   torch's upsample_bilinear2d without a scale factor:
+ *     r = align_corners ? (out > 1 ? (in - 1) / (out - 1) : 0) : in / out                       fp32
+ *     src = align_corners ? r d : max(r (d + 0.5) - 0.5, 0),  i0 = (int) src,  i1 = i0 + (i0 < in - 1),  l1 = src - i0,
+ *     l0 = 1 - l1,  y = fp16_rn( l0y (l0x x[i0y, i0x] + l1x x[i0y, i1x]) + l1y (l0x x[i1y, i0x] + l1x x[i1y, i1x]) )   fp32
+ *   C, ldx, ldy multiples of 8, strides >= C, 16-byte aligned pointers; columns >= C are not touched.
+ * k2_depth_to_space_f16: g fp16 rows [NB H W, ldg] (ldg >= s^2 C) -> y fp16 NHWC [NB, s H, s W, C] (pixel stride ldy):
+ *     y[n, s y + a, s x + b, c] = g[(n H + y) W + x, (a s + b) C + c]          a copy; a, b < s
+ *   C, ldg, ldy multiples of 8, ldy >= C, 16-byte aligned pointers.
+ * k2_readout_rows_f16: h fp16 rows [B T, ldh] (token 0 of each image is the CLS token) -> y fp16 rows [B (T - 1), ldy]:
+ *     y[n (T - 1) + t - 1, :] = [ h[n T + t, 0:H] | h[n T, 0:H] ]               t = 1 .. T - 1, a copy
+ *   (DPT's readout "project" input, cat(token, CLS)).  H, ldh, ldy multiples of 8, ldh >= H, ldy >= 2 H, 16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+int k2_relu_f16(const void* x, int ldx, void* y, int ldy, int M, int N, k2_stream_t stream);
+int k2_relu_f32(const float* x, int ldx, float* y, int ldy, int M, int N, k2_stream_t stream);
+int k2_bilinear_f16(const void* x, int ldx, int NB, int Hi, int Wi, int C, void* y, int ldy, int Ho, int Wo, int align_corners,
+                    k2_stream_t stream);
+int k2_depth_to_space_f16(const void* g, int ldg, int NB, int H, int W, int C, int s, void* y, int ldy, k2_stream_t stream);
+int k2_readout_rows_f16(const void* h, int ldh, int B, int T, int H, void* y, int ldy, k2_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
  * fuse_lora): once per adapter load, never per step.
  *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols

@@ -82,6 +82,11 @@ SIGNATURES = {
     "k2_nchw_to_nhwc_f32": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "k2_images_to_u8": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "k2_lora_merge": (_I, [_P, _I, _P, _P, _I, _I, _I, _F, _P, _I, _P]),
+    "k2_relu_f16": (_I, [_P, _I, _P, _I, _I, _I, _P]),
+    "k2_relu_f32": (_I, [_P, _I, _P, _I, _I, _I, _P]),
+    "k2_bilinear_f16": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _P]),
+    "k2_depth_to_space_f16": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "k2_readout_rows_f16": (_I, [_P, _I, _I, _I, _I, _P, _I, _P]),
 }
 
 

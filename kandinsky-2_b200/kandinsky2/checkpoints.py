@@ -28,6 +28,10 @@
 * Kandinsky 2.1's CLIP ViT-L/14 (`ViT-L-14.pt`, an OpenAI `clip` checkpoint) goes through `openai_clip_to_k2` into the
   text and image tower names above, with the geometry read from the shapes (tests/test_cpu_clip_vitl14.py).
 
+* The depth estimator of the Kandinsky 2.2 ControlNet-depth hint, a transformers `DPTForDepthEstimation` with a plain ViT
+  backbone (`Intel/dpt-large`), goes through `transformers_dpt_to_k2` into `model.depth.DPTDepthEstimator` names
+  (tests/test_cpu_dpt.py).
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -357,6 +361,61 @@ def transformers_clip_text_to_k2(sd):
     where attn.qkv stacks self_attn.{q,k,v}_proj per head [q_h | k_h | v_h] (pack_heads, head width 64).  A `position_ids`
     buffer (older checkpoints carry it) is ignored; unknown and missing keys raise K2Error naming them."""
     return _clip_to_k2(sd, "text", 64)
+
+
+# DPTForDepthEstimation: the ViT layer's names -> model/encoder.py's
+_DPT_LAYER = {"layernorm_before": "ln_1", "layernorm_after": "ln_2", "attention.output.dense": "attn.proj",
+              "intermediate.dense": "mlp.fc1", "output.dense": "mlp.fc2"}
+_DPT_TOP = {"cls_token": "dpt.embeddings.cls_token", "position_embedding": "dpt.embeddings.position_embeddings",
+            "patch_embedding.weight": "dpt.embeddings.patch_embeddings.projection.weight",
+            "patch_embedding.bias": "dpt.embeddings.patch_embeddings.projection.bias"}
+
+
+def transformers_dpt_keys(config):
+    """Every key of a transformers `DPTForDepthEstimation` state dict (plain ViT) for a config.json dict, including the
+    ones transformers_dpt_to_k2 drops."""
+    from .model.depth import dpt_config, k2_shapes
+    c = dpt_config(config)
+    keys = list(_DPT_TOP.values()) + ["dpt.layernorm.weight", "dpt.layernorm.bias"]
+    for i in range(c["num_hidden_layers"]):
+        lp = f"dpt.encoder.layer.{i}."
+        keys += [f"{lp}{d}.{s}" for d in (*_DPT_LAYER, "attention.attention.query", "attention.attention.key",
+                                            "attention.attention.value") for s in ("weight", "bias")]
+    keys += [k for k in k2_shapes(c) if k.startswith(("neck.", "head."))]
+    return keys + [f"neck.fusion_stage.layers.0.residual_layer1.{conv}.{s}" for conv in ("convolution1", "convolution2")
+                   for s in ("weight", "bias")]
+
+
+def transformers_dpt_to_k2(sd, config):
+    """transformers `DPTForDepthEstimation` state dict (plain ViT backbone, e.g. Intel/dpt-large) and its config.json dict ->
+    `model.depth.DPTDepthEstimator` names:
+        cls_token [H], position_embedding [T, H], patch_embedding.{weight, bias},
+        layers.{i}.{ln_1, ln_2, attn.qkv, attn.proj, mlp.fc1, mlp.fc2}.{weight, bias},
+        neck.* and head.* as transformers names them
+    where attn.qkv stacks attention.attention.{query,key,value} per 64-wide head [q_h | k_h | v_h] (pack_heads).  Dropped on
+    purpose, because transformers never runs them: dpt.layernorm.* (the neck reads the raw per-layer hidden states) and
+    neck.fusion_stage.layers.0.residual_layer1.* (the first fusion layer gets no residual).  Unknown and missing keys raise
+    K2Error naming them."""
+    expected = transformers_dpt_keys(config)
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"transformers DPT state dict: unknown keys {unknown}, missing keys {missing}")
+    out = {k: sd[d] for k, d in _DPT_TOP.items()}
+    out["cls_token"] = out["cls_token"].reshape(-1)                    # [1, 1, H] -> [H]
+    out["position_embedding"] = out["position_embedding"][0]           # [1, T, H] -> [T, H]
+    layers = {int(m.group(1)) for m in (re.match(r"^dpt\.encoder\.layer\.(\d+)\.", k) for k in sd) if m}
+    for i in sorted(layers):
+        dp, kp = f"dpt.encoder.layer.{i}.", f"layers.{i}."
+        for d, k in _DPT_LAYER.items():
+            for s in ("weight", "bias"):
+                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
+        for s in ("weight", "bias"):
+            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}attention.attention.{n}.{s}"] for n in ("query", "key", "value")],
+                                                  64)
+    out.update({k: v for k, v in sd.items() if k.startswith(("neck.", "head."))
+                and not k.startswith("neck.fusion_stage.layers.0.residual_layer1.")})
+    return out
 
 
 # the M-CLIP text encoder (Kandinsky 2.1's text_encoder/pytorch_model.bin): this package's name -> the checkpoint's name

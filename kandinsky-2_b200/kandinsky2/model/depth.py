@@ -1,0 +1,443 @@
+"""The depth estimator behind the Kandinsky 2.2 ControlNet-depth hint: transformers' `DPTForDepthEstimation` with a plain ViT
+backbone (`is_hybrid` false, no `backbone_config`; `Intel/dpt-large` is the default model of transformers' depth-estimation
+pipeline, which diffusers' kandinsky-2-2-controlnet-depth documentation uses to build the hint).
+
+The network is read from the checkpoint's `config.json` (for Intel/dpt-large: hidden 1024, 24 layers, 16 heads of 64, MLP
+4096, patch 16, image 384, backbone_out_indices [5, 11, 17, 23], neck sizes [256, 512, 1024, 1024], fusion 256); what is
+not implemented is refused with K2Error naming the key (dpt_config).  Compute, per batch size one LaunchPlan replayed as
+one CUDA graph:
+    backbone  k2_clip_patchify -> ONE GEMM: patch conv + CLS column + (position embedding + conv bias on the patch rows) as
+              the residual, then the pre-LayerNorm layers of model/encoder.py with k2_attention_d64, recorded in segments
+              that end at each backbone_out_indices layer, so each kept hidden state has a buffer of its own;
+    neck      per stage: k2_readout_rows_f16 ([token | CLS] rows) -> Linear(2H -> H) GEMM -> GELU -> 1x1 projection GEMM ->
+              resize (factor 4 / 2: ConvTranspose2d as one GEMM with the bias tiled, then k2_depth_to_space_f16; 1: none;
+              0.5: the stride-1 3x3 convolution, then every second pixel: k2_subsample2_nhwc for an even grid, or for an odd
+              grid k2_bilinear_f16 with align_corners, whose source index is then exactly 2i) -> bias-free 3x3 conv;
+    fusion    from the deepest stage up: [bilinear resize of the stage to the running map (align_corners=False; only where
+              the sizes differ, i.e. odd patch grids) -> running + unit1(stage)], unit2, bilinear x2 (align_corners=True),
+              1x1 projection; unit(x) = conv3x3(relu(conv3x3(relu(x)))) + x with k2_relu_f16.  The sum running + unit1
+              is the last convolution's epilogue: the running map is a second, 1x1 source of that GEMM with an identity
+              weight block (exact products, one fp32 sum, one rounding);
+    head      conv3x3 -> bilinear x2 (align_corners=True) -> conv3x3 -> ReLU -> 1x1 conv to one channel, fp32 NCHW out
+              (k2_conv_gemm out_mode 1) -> k2_relu_f32.
+fp16 storage, fp32 accumulation, the prior's LayerNorm statistics.  Not run, as in transformers: the final LayerNorm
+(`dpt.layernorm`: the neck reads the raw per-layer hidden states) and the first fusion layer's residual_layer1 (it gets no
+residual); their keys are accepted and dropped by checkpoints.transformers_dpt_to_k2.
+
+Host side: preprocess restates transformers' DPTImageProcessorPil (RGB, PIL resize with the configured resample, rescale,
+normalise; only a square output that is a multiple of the patch size is accepted); depth restates the depth-estimation
+pipeline's postprocess (bicubic resize to the image's size, min-max to [0, 255], uint8) except that a constant map gives
+zeros where transformers divides by zero; make_hint restates the hint builder of diffusers' kandinsky-2-2-controlnet-depth
+documentation.
+
+Parity: tests/test_cpu_dpt.py pins the oracle (tests/dpt_oracle.py), preprocess and postprocess to transformers
+(tests/golden/dpt_tiny.pt); tests/test_gpu_zz_depth.py runs the estimator against the golden and, at the Intel/dpt-large
+geometry on synthetic weights, against the fp32 oracle.
+"""
+import json
+import math
+import os
+
+import numpy as np
+import torch
+
+from .. import ops
+from .._native import K2Error
+from ..launch_plan import LaunchPlan
+from .encoder import layer_shapes, pack_layers, record_layers
+
+# transformers' DPTConfig defaults, for keys a config.json leaves out
+_CONFIG_DEFAULTS = dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
+                        hidden_act="gelu", layer_norm_eps=1e-12, image_size=384, patch_size=16, num_channels=3, is_hybrid=False,
+                        qkv_bias=True, backbone_out_indices=[2, 5, 8, 11], readout_type="project",
+                        reassemble_factors=[4, 2, 1, 0.5], neck_hidden_sizes=[96, 192, 384, 768], fusion_hidden_size=256,
+                        head_in_index=-1, use_batch_norm_in_fusion_residual=False, use_bias_in_fusion_residual=None,
+                        add_projection=False, backbone_config=None, backbone=None)
+# DPTImageProcessorPil's defaults (resample 3 = PIL BICUBIC; mean / std are IMAGENET_STANDARD_*)
+DEFAULT_PREPROCESSOR = dict(do_resize=True, size={"height": 384, "width": 384}, resample=3, do_rescale=True,
+                            rescale_factor=1 / 255, do_normalize=True, image_mean=[0.5, 0.5, 0.5], image_std=[0.5, 0.5, 0.5],
+                            keep_aspect_ratio=False, ensure_multiple_of=1, do_pad=False)
+
+
+def dpt_config(config):
+    """The transformers DPTConfig dict -> the geometry this module implements; K2Error naming the key for anything else."""
+    c = dict(_CONFIG_DEFAULTS)
+    c.update({k: v for k, v in config.items() if k in _CONFIG_DEFAULTS})
+    refuse = [("is_hybrid", c["is_hybrid"], "the hybrid (BiT) DPT"),
+              ("backbone_config", c["backbone_config"] is not None, "a separate backbone"),
+              ("backbone", c["backbone"] is not None, "a separate backbone"),
+              ("readout_type", c["readout_type"] != "project", f"readout_type {c['readout_type']!r}"),
+              ("hidden_act", c["hidden_act"] != "gelu", f"hidden_act {c['hidden_act']!r}"),
+              ("use_batch_norm_in_fusion_residual", c["use_batch_norm_in_fusion_residual"], "batch norm in the fusion units"),
+              ("use_bias_in_fusion_residual", c["use_bias_in_fusion_residual"] is False, "bias-free fusion units"),
+              ("add_projection", c["add_projection"], "the head's extra projection"),
+              ("head_in_index", c["head_in_index"] != -1, f"head_in_index {c['head_in_index']}"),
+              ("qkv_bias", not c["qkv_bias"], "bias-free q / k / v"),
+              ("num_channels", c["num_channels"] != 3, f"{c['num_channels']}-channel images")]
+    for key, bad, what in refuse:
+        if bad:
+            raise K2Error(f"DPT config: {key}: {what} is not implemented (only the plain-ViT DPT of Intel/dpt-large)")
+    for k in ("hidden_size", "num_hidden_layers", "num_attention_heads", "intermediate_size", "image_size", "patch_size",
+              "fusion_hidden_size"):
+        if not isinstance(c[k], int) or isinstance(c[k], bool) or c[k] <= 0:
+            raise K2Error(f"DPT config: {k} must be a positive integer, got {c[k]!r}")
+    H, heads = c["hidden_size"], c["num_attention_heads"]
+    if H % heads or H // heads != 64:
+        raise K2Error(f"DPT config: num_attention_heads: head width {H / heads:g} is not implemented (only 64)")
+    factors = [float(f) for f in c["reassemble_factors"]]
+    if any(f not in (4.0, 2.0, 1.0, 0.5) for f in factors):
+        raise K2Error(f"DPT config: reassemble_factors {c['reassemble_factors']}: only 4, 2, 1 and 0.5 are implemented")
+    idx, sizes = [int(i) for i in c["backbone_out_indices"]], [int(s) for s in c["neck_hidden_sizes"]]
+    if not (len(idx) == len(sizes) == len(factors)) or not idx:
+        raise K2Error("DPT config: backbone_out_indices, neck_hidden_sizes and reassemble_factors must have one entry per "
+                      "neck stage")
+    if idx != sorted(set(idx)) or idx[0] < 0 or idx[-1] >= c["num_hidden_layers"]:
+        raise K2Error(f"DPT config: backbone_out_indices {idx} must be increasing layer indices below num_hidden_layers")
+    if c["image_size"] % c["patch_size"]:
+        raise K2Error("DPT config: image_size must be a multiple of patch_size")
+    if any(s % 8 for s in sizes) or c["fusion_hidden_size"] % 16 or H % 8:
+        raise K2Error("DPT config: neck_hidden_sizes and hidden_size must be multiples of 8, fusion_hidden_size of 16")
+    c.update(reassemble_factors=factors, backbone_out_indices=idx, neck_hidden_sizes=sizes, head_dim=64,
+             layer_norm_eps=float(c["layer_norm_eps"]), kp=(3 * c["patch_size"] ** 2 + 1 + 63) // 64 * 64)
+    return c
+
+
+def k2_shapes(c):
+    """{name: shape} of the state dict DPTDepthEstimator takes (checkpoints.transformers_dpt_to_k2's output) for config c."""
+    H, P, F = c["hidden_size"], c["patch_size"], c["fusion_hidden_size"]
+    T0 = (c["image_size"] // P) ** 2 + 1
+    want = {"cls_token": (H,), "position_embedding": (T0, H), "patch_embedding.weight": (H, 3, P, P),
+            "patch_embedding.bias": (H,)}
+    want.update({f"layers.{i}.{k}": s for i in range(c["num_hidden_layers"])
+                 for k, s in layer_shapes(H, c["intermediate_size"]).items()})
+    rs = "neck.reassemble_stage."
+    for i, (C, f) in enumerate(zip(c["neck_hidden_sizes"], c["reassemble_factors"])):
+        want.update({f"{rs}readout_projects.{i}.0.weight": (H, 2 * H), f"{rs}readout_projects.{i}.0.bias": (H,),
+                     f"{rs}layers.{i}.projection.weight": (C, H, 1, 1), f"{rs}layers.{i}.projection.bias": (C,),
+                     f"neck.convs.{i}.weight": (F, C, 3, 3)})
+        if f != 1:
+            k = int(f) if f > 1 else 3
+            want.update({f"{rs}layers.{i}.resize.weight": (C, C, k, k), f"{rs}layers.{i}.resize.bias": (C,)})
+        fp = f"neck.fusion_stage.layers.{i}."
+        want.update({fp + "projection.weight": (F, F, 1, 1), fp + "projection.bias": (F,)})
+        for unit in (("residual_layer1", "residual_layer2") if i else ("residual_layer2",)):
+            for conv in ("convolution1", "convolution2"):
+                want.update({f"{fp}{unit}.{conv}.weight": (F, F, 3, 3), f"{fp}{unit}.{conv}.bias": (F,)})
+    want.update({"head.head.0.weight": (F // 2, F, 3, 3), "head.head.0.bias": (F // 2,), "head.head.2.weight": (32, F // 2, 3, 3),
+                 "head.head.2.bias": (32,), "head.head.4.weight": (1, 32, 1, 1), "head.head.4.bias": (1,)})
+    return want
+
+
+def preprocessor_settings(preprocessor_config, image_size):
+    """DPTImageProcessorPil's settings: DEFAULT_PREPROCESSOR updated with a preprocessor_config.json dict (None: the defaults at
+    the model's image_size).  An integer `size` means a square of that side."""
+    cfg = dict(DEFAULT_PREPROCESSOR, size={"height": image_size, "width": image_size})
+    cfg.update(preprocessor_config or {})
+    if isinstance(cfg["size"], int):
+        cfg["size"] = {"height": cfg["size"], "width": cfg["size"]}
+    if cfg.get("do_pad"):
+        raise K2Error("DPT preprocessing: do_pad is not implemented")
+    return cfg
+
+
+def _constrain_to_multiple_of(val, multiple):
+    x = round(val / multiple) * multiple
+    return math.ceil(val / multiple) * multiple if x < 0 else x
+
+
+def resize_output_size(h, w, cfg):
+    """DPTImageProcessorPil's get_resize_output_image_size -> (height, width)."""
+    oh, ow = int(cfg["size"]["height"]), int(cfg["size"]["width"])
+    sh, sw = oh / h, ow / w
+    if cfg["keep_aspect_ratio"]:
+        if abs(1 - sw) < abs(1 - sh):
+            sh = sw
+        else:
+            sw = sh
+    m = int(cfg["ensure_multiple_of"])
+    return _constrain_to_multiple_of(sh * h, m), _constrain_to_multiple_of(sw * w, m)
+
+
+def preprocess_images(images, cfg, size):
+    """DPTImageProcessorPil (restated) -> fp32 [B, 3, size, size] on the CPU.  Per image: convert to RGB, resize with PIL
+    (`resample`) to resize_output_size, float32(uint8 * rescale_factor in float64), (x - mean) / std in float32.  An image whose
+    processed size is not size x size raises K2Error (the ViT DPT runs square patch grids only)."""
+    from PIL import Image
+    if isinstance(images, Image.Image):
+        images = [images]
+    out = []
+    for img in images:
+        if img.mode != "RGB":
+            img = img.convert("RGB")
+        if cfg["do_resize"]:
+            nh, nw = resize_output_size(img.size[1], img.size[0], cfg)
+            img = img.resize((nw, nh), resample=int(cfg["resample"]))
+        if img.size != (size, size):
+            raise K2Error(f"DPT preprocessing: the image is processed to {img.size[1]} x {img.size[0]}; only the square "
+                          f"{size} x {size} input of this estimator is implemented")
+        x = np.array(img).transpose(2, 0, 1)
+        if cfg["do_rescale"]:
+            x = (x.astype(np.float64) * cfg["rescale_factor"]).astype(np.float32)
+        if cfg["do_normalize"]:
+            x = x.astype(np.float32) if not np.issubdtype(x.dtype, np.floating) else x
+            mean = np.array(cfg["image_mean"], dtype=x.dtype)
+            std = np.array(cfg["image_std"], dtype=x.dtype)
+            x = ((x.T - mean) / std).T
+        out.append(torch.from_numpy(np.ascontiguousarray(x)).float())
+    return torch.stack(out)
+
+
+def depth_image(predicted, height, width):
+    """The depth-estimation pipeline's postprocess of one map: fp32 predicted depth [S', S'] -> PIL "L" image of height x width:
+    bicubic resize (align_corners=False), (d - min) / (max - min), * 255, uint8 (truncation), in float32.  A constant map
+    gives all zeros (transformers divides by zero there)."""
+    from PIL import Image
+    d = torch.nn.functional.interpolate(predicted.float().cpu()[None, None], size=(height, width), mode="bicubic",
+                                        align_corners=False).squeeze().numpy()
+    lo, hi = d.min(), d.max()
+    d = np.zeros_like(d) if hi == lo else (d - lo) / (hi - lo)
+    return Image.fromarray((d * 255).astype("uint8"))
+
+
+def make_hint(image, estimator):
+    """diffusers' make_hint for kandinsky-2-2-controlnet-depth: the estimator's uint8 depth image of `image`, repeated over three
+    channels, / 255 -> float32 [3, H, W] in [0, 1] on the CPU."""
+    d = np.array(estimator.depth([image])[0])[:, :, None]
+    d = np.concatenate([d, d, d], axis=2)
+    return (torch.from_numpy(d).float() / 255.0).permute(2, 0, 1)
+
+
+def resize_pos_embed(pos, grid):
+    """DPTViTEmbeddings._resize_pos_embed in fp32 on the host: pos [1 + G0^2, H] -> [1 + grid^2, H], the grid part resized
+    bilinearly (align_corners=False)."""
+    g0 = int(math.sqrt(pos.shape[0] - 1))
+    p = pos[1:].float().reshape(1, g0, g0, -1).permute(0, 3, 1, 2)
+    p = torch.nn.functional.interpolate(p, size=(grid, grid), mode="bilinear")
+    return torch.cat([pos[:1].float(), p.permute(0, 2, 3, 1).reshape(grid * grid, -1)])
+
+
+class DPTDepthEstimator:
+    """DPTForDepthEstimation (plain ViT) on this package's kernels.  sd: state dict in this module's names
+    (checkpoints.transformers_dpt_to_k2); config: the transformers config.json dict; preprocessor_config: the image
+    processor's preprocessor_config.json dict (None: DPTImageProcessorPil's defaults at the model's image_size).  The input
+    size is the processor's; the position embedding is resized to its patch grid once, on the host."""
+
+    def __init__(self, sd, config, device="cuda", preprocessor_config=None):
+        c = dpt_config(config)
+        self.cfg, self.device = c, torch.device(device)
+        self.proc = preprocessor_settings(preprocessor_config, c["image_size"])
+        S = int(self.proc["size"]["height"])
+        if int(self.proc["size"]["width"]) != S or S % c["patch_size"] or S <= 0:
+            raise K2Error(f"DPT preprocessing: size {self.proc['size']}: only a square input that is a multiple of the patch "
+                          f"size {c['patch_size']} is implemented")
+        self.size, self.grid = S, S // c["patch_size"]
+        want = k2_shapes(c)
+        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
+        extra = sorted(set(sd) - set(want))
+        if bad or extra:
+            raise K2Error(f"DPT: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
+        self.sd, self._packed, self._plans = sd, None, {}
+
+    @classmethod
+    def from_transformers(cls, state_dict, config, preprocessor_config=None, device="cuda"):
+        """From a transformers DPTForDepthEstimation state dict and its config.json dict; packs the weights."""
+        from ..checkpoints import transformers_dpt_to_k2
+        return cls(transformers_dpt_to_k2(state_dict, config), config, device, preprocessor_config).finalize()
+
+    @classmethod
+    def from_pretrained(cls, path, device="cuda"):
+        """A local transformers model folder (e.g. a download of Intel/dpt-large): config.json, preprocessor_config.json
+        (optional) and model.safetensors or pytorch_model.bin.  A missing file raises K2Error naming it."""
+        from .prior import _load_weights
+
+        def read(name, required=True):
+            f = os.path.join(path, name)
+            if not os.path.exists(f):
+                if required:
+                    raise K2Error(f"DPTDepthEstimator.from_pretrained: {f} not found")
+                return None
+            with open(f, encoding="utf-8") as fh:
+                return json.load(fh)
+
+        config = read("config.json")
+        stem = "pytorch_model" if os.path.exists(os.path.join(path, "pytorch_model.bin")) else "model"
+        return cls.from_transformers(_load_weights(path, stem), config, read("preprocessor_config.json", False), device)
+
+    def finalize(self):
+        """Pack the weights on the device once (fp16 GEMM weights, fp32 biases and LayerNorm parameters)."""
+        c, dev, sd = self.cfg, self.device, self.sd
+        H, P, kp, F = c["hidden_size"], c["patch_size"], c["kp"], c["fusion_hidden_size"]
+        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+        w = lambda name: ops.pack_conv_weight(sd[name].detach().to(dev))  # noqa: E731
+        K = 3 * P * P
+        we = torch.zeros(H, kp, dtype=torch.float16, device=dev)
+        we[:, :K] = sd["patch_embedding.weight"].detach().to(dev).reshape(H, K).half()
+        we[:, K] = sd["cls_token"].detach().to(dev).half()
+        pos = resize_pos_embed(sd["position_embedding"].detach().cpu(), self.grid)
+        pos[1:] += sd["patch_embedding.bias"].detach().cpu().float()   # the patch conv's bias, on the patch rows only
+        pk = {"embed": we, "pos": pos.to(dev).half().contiguous(),
+              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["backbone_out_indices"][-1] + 1, dev)}
+        rs = "neck.reassemble_stage."
+        for i, (C, f) in enumerate(zip(c["neck_hidden_sizes"], c["reassemble_factors"])):
+            pk[f"readout.{i}"] = (w(f"{rs}readout_projects.{i}.0.weight"), f32(sd[f"{rs}readout_projects.{i}.0.bias"]))
+            pk[f"proj.{i}"] = (w(f"{rs}layers.{i}.projection.weight"), f32(sd[f"{rs}layers.{i}.projection.bias"]))
+            rw, rb = sd.get(f"{rs}layers.{i}.resize.weight"), sd.get(f"{rs}layers.{i}.resize.bias")
+            if f > 1:   # ConvTranspose2d weight [in, out, a, b] -> GEMM rows (a s + b) C + out over K = in
+                s = int(f)
+                g = rw.detach().to(dev).permute(2, 3, 1, 0).reshape(s * s * C, C)
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(g), f32(rb).repeat(s * s))
+            elif f < 1:
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(rw.detach().to(dev)), f32(rb))
+            pk[f"neck_conv.{i}"] = w(f"neck.convs.{i}.weight")
+            fp = f"neck.fusion_stage.layers.{i}."
+            pk[f"fusion_proj.{i}"] = (w(fp + "projection.weight"), f32(sd[fp + "projection.bias"]))
+            for u in ((1, 2) if i else (2,)):
+                p = f"{fp}residual_layer{u}."
+                c2 = w(p + "convolution2.weight")
+                if u == 1:   # + the running map as a 1x1 source with an identity block: running + unit1(stage) in one epilogue
+                    eye = torch.zeros(F, c2.shape[1] // 9, dtype=torch.float16, device=dev)
+                    eye[:, :F] = torch.eye(F, dtype=torch.float16, device=dev)
+                    c2 = torch.cat([c2, eye], 1).contiguous()
+                pk[f"unit{u}.{i}"] = ((w(p + "convolution1.weight"), f32(sd[p + "convolution1.bias"])),
+                                      (c2, f32(sd[p + "convolution2.bias"])))
+        pk["head"] = [(w("head.head.0.weight"), f32(sd["head.head.0.bias"])),
+                      (w("head.head.2.weight"), f32(sd["head.head.2.bias"])),
+                      (ops.pad_rows(w("head.head.4.weight"), 16), f32(sd["head.head.4.bias"]))]
+        self._packed, self._plans = pk, {}
+        return self
+
+    def _plan(self, B):
+        if self._packed is None:
+            self.finalize()
+        if B not in self._plans:
+            self._plans[B] = _DepthPlan(self, B)
+        return self._plans[B]
+
+    def attend(self, qkv, out):
+        """The layers' attention: k2_attention_d64 over the tokens (per-head [q | k | v], scale 1/8)."""
+        return ops.attention_d64(qkv, self.cfg["num_attention_heads"], scale=0.125, out=out)
+
+    def preprocess(self, images):
+        """PIL image(s) -> fp32 pixel_values [B, 3, S, S] on the CPU (preprocess_images with this estimator's settings)."""
+        return preprocess_images(images, self.proc, self.size)
+
+    @torch.no_grad()
+    def predicted_depth(self, pixel_values, use_graph=True):
+        """pixel_values fp32 [B, 3, S, S] -> DPTForDepthEstimation's predicted_depth, fp32 [B, S', S'] on the device (S' = S for
+        an even patch grid).  One CUDA graph replay of the batch size's launch plan (use_graph=False: the same launches one
+        by one)."""
+        S = self.size
+        if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
+            raise K2Error(f"DPT: pixel_values must be [B, 3, {S}, {S}], got {list(pixel_values.shape)}")
+        plan = self._plan(pixel_values.shape[0])
+        plan.pix.copy_(pixel_values)
+        plan.run(use_graph)
+        return plan.out.clone()
+
+    def depth(self, images):
+        """PIL image(s) -> a list of PIL "L" depth images, each of its image's size (depth_image of predicted_depth)."""
+        from PIL import Image
+        if isinstance(images, Image.Image):
+            images = [images]
+        pred = self.predicted_depth(self.preprocess(images).to(self.device)).cpu()
+        return [depth_image(p, img.size[1], img.size[0]) for p, img in zip(pred, images)]
+
+
+class _DepthPlan(LaunchPlan):
+    """The estimator at B images as one static launch list over fixed buffers (replayed as one CUDA graph); see the module
+    docstring.  self.out is predicted_depth, fp32 [B, S', S']."""
+
+    def __init__(self, est, B):
+        super().__init__(est.device, B)
+        self.e, self.B = est, B
+        self.pix = torch.zeros(B, 3, est.size, est.size, device=self.dev, dtype=torch.float32)
+        self.pos = est._packed["pos"].expand(B, *est._packed["pos"].shape).contiguous()
+        self._build()
+
+    def _conv3(self, x, wb, cout, residual=None, extra=None):
+        """3x3 convolution (+ bias) (+ residual) of x fp16 NHWC; extra: a second source read as a 1x1 term."""
+        B, Hs, Ws, C = x.shape
+        out = self._new(B, Hs, Ws, cout)
+        srcs = [(x, 9)] + ([(extra, 1)] if extra is not None else [])
+        K = 9 * C + (extra.shape[-1] if extra is not None else 0)
+        w, b = wb if isinstance(wb, tuple) else (wb, None)
+        self._conv(srcs, w, cout, out, 2 * B * Hs * Ws * K * cout, bias=b, residual=residual, want_stats=False, kind="conv")
+        return out
+
+    def _relu(self, x):
+        y = self._new(*x.shape)
+        self._add(lambda: ops.relu_f16(x, out=y), "relu")
+        return y
+
+    def _bilinear(self, x, size, align):
+        y = self._new(x.shape[0], size[0], size[1], x.shape[-1])
+        self._add(lambda: ops.bilinear_f16(x, size, align, out=y), "bilinear")
+        return y
+
+    def _unit(self, x, units, extra=None):
+        """DPTPreActResidualLayer: conv3x3(relu(conv3x3(relu(x)))) + x (+ extra through the identity block)."""
+        (w1, b1), (w2, b2) = units
+        F = w1.shape[0]
+        a = self._conv3(self._relu(x), (w1, b1), F)
+        self._add(lambda: ops.relu_f16(a), "relu")
+        return self._conv3(a, (w2, b2), F, residual=x, extra=extra)
+
+    def _build(self):
+        e, pk, B, A = self.e, self.e._packed, self.B, self._add
+        c = e.cfg
+        G, H, P, F = e.grid, c["hidden_size"], c["patch_size"], c["fusion_hidden_size"]
+        T, heads, eps = G * G + 1, c["num_attention_heads"], c["layer_norm_eps"]
+        rows = self._new(B, T, c["kp"])
+        A(lambda: ops.clip_patchify(self.pix, P, c["kp"], out=rows), "patchify")
+        h = self._new(B, T, H)
+        self._gemm(rows, pk["embed"], H, h, 2 * B * T * c["kp"] * H, residual=self.pos)
+        hidden, start = [], 0
+        for idx in c["backbone_out_indices"]:
+            h = record_layers(self, h, pk["layers"][start:idx + 1], e.attend, 4 * B * heads * T * T * 64, eps)
+            hidden.append(h)
+            start = idx + 1
+        feats, M = [], B * G * G
+        for i, (hs, C, f) in enumerate(zip(hidden, c["neck_hidden_sizes"], c["reassemble_factors"])):
+            ro, r, p = self._new(B, G, G, 2 * H), self._new(B, G, G, H), self._new(B, G, G, C)
+            A(lambda hs=hs, ro=ro: ops.readout_rows_f16(hs, out=ro.view(B, G * G, 2 * H)), "readout")
+            self._gemm(ro, pk[f"readout.{i}"][0], H, r, 2 * M * 2 * H * H, bias=pk[f"readout.{i}"][1])
+            A(lambda r=r: ops.gelu_f16_(r), "gelu")
+            self._gemm(r, pk[f"proj.{i}"][0], C, p, 2 * M * H * C, bias=pk[f"proj.{i}"][1])
+            if f > 1:
+                s = int(f)
+                g, y = self._new(B, G, G, s * s * C), self._new(B, s * G, s * G, C)
+                self._gemm(p, pk[f"resize.{i}"][0], s * s * C, g, 2 * M * C * s * s * C, bias=pk[f"resize.{i}"][1])
+                A(lambda g=g, y=y, s=s, C=C: ops.depth_to_space_f16(g, s, C, out=y), "depth_to_space")
+            elif f < 1:
+                full, Go = self._conv3(p, pk[f"resize.{i}"], C), (G + 1) // 2
+                if G % 2 == 0:
+                    y = self._new(B, Go, Go, C)
+                    A(lambda full=full, y=y: ops.subsample2(full, 0, 0, out=y), "subsample")
+                else:   # align_corners from G to (G + 1) / 2 samples: source index 2i exactly, weights 1 and 0
+                    y = self._bilinear(full, (Go, Go), True)
+            else:
+                y = p
+            feats.append(self._conv3(y, pk[f"neck_conv.{i}"], F))
+        run = None
+        for j, fe in enumerate(reversed(feats)):   # fusion layer j (its packed weights' key) takes the stage from the deep end
+            if run is None:
+                x = fe
+            else:
+                if fe.shape[1:3] != run.shape[1:3]:
+                    fe = self._bilinear(fe, tuple(run.shape[1:3]), False)
+                x = self._unit(fe, pk[f"unit1.{j}"], extra=run)
+            x = self._unit(x, pk[f"unit2.{j}"])
+            up = self._bilinear(x, (2 * x.shape[1], 2 * x.shape[2]), True)
+            run = self._new(*up.shape)
+            wp, bp = pk[f"fusion_proj.{j}"]
+            self._gemm(up, wp, F, run, 2 * up.numel() * F, bias=bp)
+        (w0, b0), (w2, b2), (w4, b4) = pk["head"]
+        a = self._conv3(run, (w0, b0), F // 2)
+        a = self._bilinear(a, (2 * a.shape[1], 2 * a.shape[2]), True)
+        a = self._conv3(a, (w2, b2), 32)
+        A(lambda: ops.relu_f16(a), "relu")
+        So = a.shape[1]
+        out = torch.empty(B, 1, So, So, device=self.dev, dtype=torch.float32)
+        self._conv([(a, 1)], w4, 1, out, 2 * B * So * So * 32, bias=b4, want_stats=False, out_mode=1, kind="conv")
+        A(lambda: ops.relu_f32(out), "relu")
+        self.out = out.view(B, So, So)

@@ -774,3 +774,74 @@ def masked_mean_f16(hidden, mask, out=None):
     check(nat.load().k2_masked_mean_f16(ptr(hidden), _row_stride(hidden), ptr(mask), ldm, B, T, H, ptr(out), ldo,
                                         stream_ptr()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# DPT depth estimator (kandinsky2/model/depth.py, see k2b200.h)
+# ------------------------------------------------------------------------------------------------
+def _on_device(name, *tensors):
+    if not all(t.is_cuda for t in tensors if t is not None):
+        raise nat.K2Error(f"{name}: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+
+
+def _rows(t, dtype, name):
+    """(rows, columns, row stride) of a tensor whose last dimension is contiguous and whose leading dimensions are row-strided
+    (_row_stride)."""
+    assert t.dtype == dtype and t.dim() >= 2 and t.stride(-1) == 1, (name, t.dtype, tuple(t.shape), t.stride())
+    return t.numel() // t.shape[-1] if t.numel() else 0, t.shape[-1], _row_stride(t)
+
+
+def relu_f16(x, out=None):
+    """k2_relu_f16: torch.relu of fp16 rows [..., N] (row-strided views) into out (default: in place)."""
+    out = x if out is None else out
+    _on_device("relu_f16", x, out)
+    M, N, ldx = _rows(x, torch.float16, "x")
+    assert tuple(out.shape) == tuple(x.shape), (tuple(out.shape), tuple(x.shape))
+    check(nat.load().k2_relu_f16(ptr(x), ldx, ptr(out), _rows(out, torch.float16, "out")[2], M, N, stream_ptr()))
+    return out
+
+
+def relu_f32(x, out=None):
+    """k2_relu_f32: torch.relu of fp32 rows [..., N] (row-strided views) into out (default: in place)."""
+    out = x if out is None else out
+    _on_device("relu_f32", x, out)
+    M, N, ldx = _rows(x, torch.float32, "x")
+    assert tuple(out.shape) == tuple(x.shape), (tuple(out.shape), tuple(x.shape))
+    check(nat.load().k2_relu_f32(ptr(x), ldx, ptr(out), _rows(out, torch.float32, "out")[2], M, N, stream_ptr()))
+    return out
+
+
+def bilinear_f16(x, size, align_corners, out=None):
+    """k2_bilinear_f16: fp16 NHWC [NB, Hi, Wi, C] (row-strided) -> [NB, Ho, Wo, C], size = (Ho, Wo); torch's
+    interpolate(mode="bilinear", size=size, align_corners=align_corners) on the NCHW view, one rounding per output."""
+    NB, Hi, Wi, C = x.shape
+    Ho, Wo = size
+    if out is None:
+        out = torch.empty((NB, Ho, Wo, C), dtype=torch.float16, device=x.device)
+    _on_device("bilinear_f16", x, out)
+    assert x.dtype == out.dtype == torch.float16 and tuple(out.shape) == (NB, Ho, Wo, C), (x.dtype, out.dtype, tuple(out.shape))
+    check(nat.load().k2_bilinear_f16(ptr(x), _row_stride(x), NB, Hi, Wi, C, ptr(out), _row_stride(out), Ho, Wo,
+                                     int(bool(align_corners)), stream_ptr()))
+    return out
+
+
+def depth_to_space_f16(g, s, C, out=None):
+    """k2_depth_to_space_f16: GEMM rows g fp16 [NB, H, W, >= s^2 C] (column (a s + b) C + c) -> fp16 NHWC [NB, s H, s W, C]."""
+    NB, H, W = g.shape[:3]
+    if out is None:
+        out = torch.empty((NB, s * H, s * W, C), dtype=torch.float16, device=g.device)
+    _on_device("depth_to_space_f16", g, out)
+    assert g.dtype == out.dtype == torch.float16 and tuple(out.shape) == (NB, s * H, s * W, C), (g.dtype, tuple(out.shape))
+    check(nat.load().k2_depth_to_space_f16(ptr(g), _row_stride(g), NB, H, W, C, s, ptr(out), _row_stride(out), stream_ptr()))
+    return out
+
+
+def readout_rows_f16(h, out=None):
+    """k2_readout_rows_f16: fp16 [B, T, H] (token 0 = CLS, row-strided) -> fp16 [B, T - 1, 2 H] = cat(token, CLS) rows."""
+    B, T, H = h.shape
+    if out is None:
+        out = torch.empty((B, T - 1, 2 * H), dtype=torch.float16, device=h.device)
+    _on_device("readout_rows_f16", h, out)
+    assert h.dtype == out.dtype == torch.float16 and tuple(out.shape) == (B, T - 1, 2 * H), (h.dtype, tuple(out.shape))
+    check(nat.load().k2_readout_rows_f16(ptr(h), _row_stride(h), B, T, H, ptr(out), _row_stride(out), stream_ptr()))
+    return out

@@ -320,6 +320,12 @@ class Kandinsky2_2(_DecoderBase):
     # and the result is blended with the clean latent at the end -- the step kernels' inpaint_noise mode
     inpaint_renoise = True
 
+    def __init__(self, *args, depth_estimator=None, **kwargs):
+        """depth_estimator: a model.depth.DPTDepthEstimator (or anything with its depth(images) method); with one set,
+        generate_controlnet and generate_controlnet_img2img also take a PIL image as hint and build the depth map from it."""
+        super().__init__(*args, **kwargs)
+        self.depth_estimator = depth_estimator
+
     def get_new_h_w(self, h, w):  # kandinsky2_2_model.py:46-53 (pixels)
         return math.ceil(h / 64) * 64, math.ceil(w / 64) * 64
 
@@ -413,20 +419,32 @@ class Kandinsky2_2(_DecoderBase):
             hint = torch.nn.functional.interpolate(hint, (h, w), mode="bilinear", align_corners=False)
         return hint
 
+    def _depth_hint(self, hint):
+        """A PIL image -> model.depth.make_hint(hint, self.depth_estimator), [3, H, W] in [0, 1]; any other hint unchanged."""
+        from PIL import Image
+        if not isinstance(hint, Image.Image):
+            return hint
+        if self.depth_estimator is None:
+            raise ValueError("a PIL image as hint needs a pipeline built with depth_estimator= (e.g. a "
+                             "model.depth.DPTDepthEstimator); without one, pass the depth map as a [1, 3, h, w] tensor")
+        from .model.depth import make_hint
+        return make_hint(hint, self.depth_estimator)
+
     def generate_controlnet(self, prompt, hint, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                             prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
                             sampler="ddpm_sampler"):
         """Kandinsky 2.2 ControlNet-depth (BASELINE configs[4]).  The reference package has no method for it -- its
         notebooks/kandinsky2_2_controlnet.ipynb calls diffusers' KandinskyV22ControlnetPipeline(image_embeds=...,
         negative_image_embeds=..., hint=hint, height=h, width=w) directly -- so this follows the sibling methods' signature.
-        hint: depth map tensor [1, 3, h, w] in [0, 1] (the pipeline object must be built with task_type="controlnet")."""
+        hint: depth map tensor [1, 3, h, w] in [0, 1] (the pipeline object must be built with task_type="controlnet"), or, with
+        a depth_estimator, a PIL image whose depth map make_hint builds."""
         _check_sampler(sampler, SAMPLERS_22)
         if self.task_type != "controlnet":
             raise ValueError("generate_controlnet needs a pipeline built with task_type='controlnet'")
         h, w = self.get_new_h_w(h, w)
         pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
-        hint = self._hint(hint, h, w)
+        hint = self._hint(self._depth_hint(hint), h, w)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w, hint=hint, sampler=sampler)
 
     def generate_controlnet_img2img(self, prompt, image, hint, strength=0.5, batch_size=1, decoder_steps=50, prior_steps=25,
@@ -463,7 +481,8 @@ class Kandinsky2_2(_DecoderBase):
         lat = self._encode_image(image, h, w)
         x, start = self._img2img_start(lat, create_ddpm_v22(decoder_steps), decoder_steps, strength, sampler)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
-                                 latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, hint=self._hint(hint, h, w),
+                                 latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start,
+                                 hint=self._hint(self._depth_hint(hint), h, w),
                                  sampler=sampler)
 
     def generate_inpainting(self, prompt, pil_img, img_mask, batch_size=1, decoder_steps=50, prior_steps=25,
