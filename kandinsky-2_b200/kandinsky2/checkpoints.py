@@ -32,6 +32,11 @@
   backbone (`Intel/dpt-large`), goes through `transformers_dpt_to_k2` into `model.depth.DPTDepthEstimator` names
   (tests/test_cpu_dpt.py).
 
+* The transformer remaps above (diffusers prior, both transformers CLIP towers, M-CLIP, OpenAI CLIP, DPT) are tables over one
+  recipe: `_stack_keys` lists a checkpoint's keys, `_require_keys` refuses unknown and missing ones, `_stack_to_k2` renames
+  the top-level and per-layer names and packs q / k / v per head.  Each format's own cases (dropped keys, reshapes,
+  transposes) stay at its call site.  `read_json` and `load_weights` read the component folders the towers load from.
+
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
@@ -42,6 +47,7 @@ build container, so the diffusers-side key names below are restated from the pub
 are inverse bijections onto the package's exact key set, and the head-interleaved packing reproduces separate
 q / k / v projections numerically.
 """
+import json
 import math
 import os
 import re
@@ -106,6 +112,51 @@ def unpack_heads(w, n, head_dim=64):
     heads = C // head_dim
     v = w.reshape(heads, n, head_dim, *w.shape[1:])
     return [v[:, i].reshape(C, *w.shape[1:]) for i in range(n)]
+
+
+_WB = ("weight", "bias")
+
+
+def _stack_keys(top, prefix, layer, qkv, layers):
+    """The keys of a transformer checkpoint: `top` (the keys outside the layers), then for each of the `layers` layers,
+    under prefix.format(i), the names of `layer` ({source name: this package's name}) and the q / k / v projections, each
+    with its weight and bias.  qkv: the three projections' names up to the weight / bias suffix (e.g. "self_attn.q_proj."),
+    or one name of a fused [q; k; v] projection (OpenAI's "attn.in_proj_")."""
+    keys = list(top)
+    for i in range(layers):
+        lp = prefix.format(i)
+        keys += [f"{lp}{d}.{s}" for d in layer for s in _WB] + [f"{lp}{n}{s}" for n in qkv for s in _WB]
+    return keys
+
+
+def _stack_to_k2(sd, top, prefix, layer, qkv, layers, dst, dst_qkv, head_dim):
+    """A transformer checkpoint laid out as _stack_keys describes -> this package's names: top ({this package's name: source
+    key}) copied, and layer i's `layer` names renamed under dst.format(i), its q / k / v packed per head_dim head into
+    dst.format(i) + dst_qkv (pack_heads; a fused projection is split into thirds first)."""
+    out = {k: sd[d] for k, d in top.items()}
+    for i in range(layers):
+        sp, dp = prefix.format(i), dst.format(i)
+        for d, k in layer.items():
+            for s in _WB:
+                out[f"{dp}{k}.{s}"] = sd[f"{sp}{d}.{s}"]
+        for s in _WB:
+            parts = [sd[f"{sp}{n}{s}"] for n in qkv]
+            out[f"{dp}{dst_qkv}.{s}"] = pack_heads(parts if len(parts) == 3 else list(parts[0].chunk(3)), head_dim)
+    return out
+
+
+def _count_layers(sd, prefix):
+    """1 + the largest i with a key starting prefix.format(i), or 0."""
+    rx = re.compile(re.escape(prefix).replace(r"\{\}", r"(\d+)"))
+    return max((int(m.group(1)) + 1 for m in map(rx.match, sd) if m), default=0)
+
+
+def _require_keys(sd, expected, what):
+    """K2Error naming the keys of sd that are not expected and the expected keys sd lacks."""
+    unknown = sorted(set(sd) - set(expected))
+    missing = [k for k in expected if k not in sd]
+    if unknown or missing:
+        raise K2Error(f"{what} state dict: unknown keys {unknown}, missing keys {missing}")
 
 
 def diffusers_unet_to_k2(sd, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3,
@@ -214,16 +265,13 @@ _PRIOR_TOP = {"time_embedding.linear_1": "time_embed.0", "time_embedding.linear_
               "proj_to_clip_embeddings": "out_proj"}
 _PRIOR_BLOCK = {"norm1": "ln_1", "norm3": "ln_2", "attn1.to_out.0": "attn.c_proj", "ff.net.0.proj": "mlp.c_fc",
                 "ff.net.2": "mlp.c_proj"}
+_PRIOR_QKV = ("attn1.to_q.", "attn1.to_k.", "attn1.to_v.")
 
 
 def diffusers_prior_keys(layers):
     """Every key of a diffusers Kandinsky 2.2 `PriorTransformer` state dict with `layers` transformer blocks."""
-    keys = ["positional_embedding", "prd_embedding", "clip_mean", "clip_std"]
-    keys += [f"{d}.{s}" for d in _PRIOR_TOP for s in ("weight", "bias")]
-    for i in range(layers):
-        keys += [f"transformer_blocks.{i}.{d}.{s}" for d in (*_PRIOR_BLOCK, "attn1.to_q", "attn1.to_k", "attn1.to_v")
-                 for s in ("weight", "bias")]
-    return keys
+    top = ["positional_embedding", "prd_embedding", "clip_mean", "clip_std", *(f"{d}.{s}" for d in _PRIOR_TOP for s in _WB)]
+    return _stack_keys(top, "transformer_blocks.{}.", _PRIOR_BLOCK, _PRIOR_QKV, layers)
 
 
 def diffusers_prior_to_k2(sd, head_dim=64):
@@ -235,23 +283,12 @@ def diffusers_prior_to_k2(sd, head_dim=64):
     `causal_attention_mask` buffer is dropped: the attention kernel builds the causal mask itself.  Raises K2Error naming
     the unknown and the missing keys.  Restated from diffusers' published layout (diffusers is not a dependency)."""
     sd = {k: v for k, v in sd.items() if k != "causal_attention_mask"}
-    blocks = {int(m.group(1)) for m in (re.match(r"^transformer_blocks\.(\d+)\.", k) for k in sd) if m}
-    expected = diffusers_prior_keys(max(blocks) + 1 if blocks else 0)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"diffusers prior state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {"positional_embedding": sd["positional_embedding"], "prd_emb": sd["prd_embedding"]}
-    for d, k in _PRIOR_TOP.items():
-        for s in ("weight", "bias"):
-            out[f"{k}.{s}"] = sd[f"{d}.{s}"]
-    for i in sorted(blocks):
-        dp, kp = f"transformer_blocks.{i}.", f"transformer.resblocks.{i}."
-        for d, k in _PRIOR_BLOCK.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.c_qkv.{s}"] = pack_heads([sd[f"{dp}attn1.to_{n}.{s}"] for n in "qkv"], head_dim)
+    layers = _count_layers(sd, "transformer_blocks.{}.")
+    _require_keys(sd, diffusers_prior_keys(layers), "diffusers prior")
+    top = {"positional_embedding": "positional_embedding", "prd_emb": "prd_embedding",
+           **{f"{k}.{s}": f"{d}.{s}" for d, k in _PRIOR_TOP.items() for s in _WB}}
+    out = _stack_to_k2(sd, top, "transformer_blocks.{}.", _PRIOR_BLOCK, _PRIOR_QKV, layers, "transformer.resblocks.{}.",
+                       "attn.c_qkv", head_dim)
     return out, sd["clip_mean"].reshape(-1), sd["clip_std"].reshape(-1)
 
 
@@ -286,6 +323,7 @@ def k2_to_diffusers_unet(sd,in_channels=4, model_channels=384, channel_mult=(1, 
 
 _CLIP_LAYER = {"layer_norm1": "ln_1", "layer_norm2": "ln_2", "self_attn.out_proj": "attn.proj", "mlp.fc1": "mlp.fc1",
                "mlp.fc2": "mlp.fc2"}
+_CLIP_QKV = ("self_attn.q_proj.", "self_attn.k_proj.", "self_attn.v_proj.")
 # the keys outside the encoder layers: this package's name -> transformers' name
 _CLIP_TOP = {
     "vision": {"class_embedding": "vision_model.embeddings.class_embedding",
@@ -302,33 +340,17 @@ _CLIP_TOP = {
 
 
 def _clip_keys(tower, layers):
-    keys = list(_CLIP_TOP[tower].values())
-    for i in range(layers):
-        lp = f"{tower}_model.encoder.layers.{i}."
-        keys += [f"{lp}{d}.{s}" for d in (*_CLIP_LAYER, "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")
-                 for s in ("weight", "bias")]
-    return keys
+    return _stack_keys(_CLIP_TOP[tower].values(), f"{tower}_model.encoder.layers.{{}}.", _CLIP_LAYER, _CLIP_QKV, layers)
 
 
 def _clip_to_k2(sd, tower, head_dim):
     """transformers CLIP `tower` ("text" / "vision") state dict -> this package's names, q / k / v packed per head_dim head."""
     p = f"{tower}_model."
     sd = {k: v for k, v in sd.items() if k != p + "embeddings.position_ids"}
-    layers = {int(m.group(1)) for m in (re.match(rf"^{re.escape(p)}encoder\.layers\.(\d+)\.", k) for k in sd) if m}
-    expected = _clip_keys(tower, max(layers) + 1 if layers else 0)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"transformers CLIP {tower} state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {k: sd[d] for k, d in _CLIP_TOP[tower].items()}
-    for i in sorted(layers):
-        dp, kp = f"{p}encoder.layers.{i}.", f"layers.{i}."
-        for d, k in _CLIP_LAYER.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}self_attn.{n}_proj.{s}"] for n in "qkv"], head_dim)
-    return out
+    layers = _count_layers(sd, p + "encoder.layers.{}.")
+    _require_keys(sd, _clip_keys(tower, layers), f"transformers CLIP {tower}")
+    return _stack_to_k2(sd, _CLIP_TOP[tower], p + "encoder.layers.{}.", _CLIP_LAYER, _CLIP_QKV, layers, "layers.{}.",
+                        "attn.qkv", head_dim)
 
 
 def transformers_clip_vision_keys(layers):
@@ -369,6 +391,7 @@ _DPT_LAYER = {"layernorm_before": "ln_1", "layernorm_after": "ln_2", "attention.
 _DPT_TOP = {"cls_token": "dpt.embeddings.cls_token", "position_embedding": "dpt.embeddings.position_embeddings",
             "patch_embedding.weight": "dpt.embeddings.patch_embeddings.projection.weight",
             "patch_embedding.bias": "dpt.embeddings.patch_embeddings.projection.bias"}
+_DPT_QKV = ("attention.attention.query.", "attention.attention.key.", "attention.attention.value.")
 
 
 def transformers_dpt_keys(config):
@@ -376,14 +399,11 @@ def transformers_dpt_keys(config):
     ones transformers_dpt_to_k2 drops."""
     from .model.depth import dpt_config, k2_shapes
     c = dpt_config(config)
-    keys = list(_DPT_TOP.values()) + ["dpt.layernorm.weight", "dpt.layernorm.bias"]
-    for i in range(c["num_hidden_layers"]):
-        lp = f"dpt.encoder.layer.{i}."
-        keys += [f"{lp}{d}.{s}" for d in (*_DPT_LAYER, "attention.attention.query", "attention.attention.key",
-                                            "attention.attention.value") for s in ("weight", "bias")]
+    keys = _stack_keys([*_DPT_TOP.values(), "dpt.layernorm.weight", "dpt.layernorm.bias"], "dpt.encoder.layer.{}.", _DPT_LAYER,
+                       _DPT_QKV, c["num_hidden_layers"])
     keys += [k for k in k2_shapes(c) if k.startswith(("neck.", "head."))]
     return keys + [f"neck.fusion_stage.layers.0.residual_layer1.{conv}.{s}" for conv in ("convolution1", "convolution2")
-                   for s in ("weight", "bias")]
+                   for s in _WB]
 
 
 def transformers_dpt_to_k2(sd, config):
@@ -396,23 +416,12 @@ def transformers_dpt_to_k2(sd, config):
     purpose, because transformers never runs them: dpt.layernorm.* (the neck reads the raw per-layer hidden states) and
     neck.fusion_stage.layers.0.residual_layer1.* (the first fusion layer gets no residual).  Unknown and missing keys raise
     K2Error naming them."""
-    expected = transformers_dpt_keys(config)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"transformers DPT state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {k: sd[d] for k, d in _DPT_TOP.items()}
+    from .model.depth import dpt_config
+    _require_keys(sd, transformers_dpt_keys(config), "transformers DPT")
+    out = _stack_to_k2(sd, _DPT_TOP, "dpt.encoder.layer.{}.", _DPT_LAYER, _DPT_QKV, dpt_config(config)["num_hidden_layers"],
+                       "layers.{}.", "attn.qkv", 64)
     out["cls_token"] = out["cls_token"].reshape(-1)                    # [1, 1, H] -> [H]
     out["position_embedding"] = out["position_embedding"][0]           # [1, T, H] -> [T, H]
-    layers = {int(m.group(1)) for m in (re.match(r"^dpt\.encoder\.layer\.(\d+)\.", k) for k in sd) if m}
-    for i in sorted(layers):
-        dp, kp = f"dpt.encoder.layer.{i}.", f"layers.{i}."
-        for d, k in _DPT_LAYER.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}attention.attention.{n}.{s}"] for n in ("query", "key", "value")],
-                                                  64)
     out.update({k: v for k, v in sd.items() if k.startswith(("neck.", "head."))
                 and not k.startswith("neck.fusion_stage.layers.0.residual_layer1.")})
     return out
@@ -426,17 +435,13 @@ _MCLIP_TOP = {"word_embedding": "transformer.embeddings.word_embeddings.weight",
               "proj.weight": "LinearTransformation.weight", "proj.bias": "LinearTransformation.bias"}
 _MCLIP_LAYER = {"attention.output.dense": "attn.proj", "attention.output.LayerNorm": "ln_1", "intermediate.dense": "mlp.fc1",
                 "output.dense": "mlp.fc2", "output.LayerNorm": "ln_2"}
+_MCLIP_QKV = ("attention.self.query.", "attention.self.key.", "attention.self.value.")
 
 
 def mclip_keys(layers):
     """Every key of the reference's MultilingualCLIP state dict with `layers` XLM-R layers, without the ones mclip_to_k2
     ignores (transformer.pooler.*, transformer.embeddings.position_ids)."""
-    keys = list(_MCLIP_TOP.values())
-    for i in range(layers):
-        lp = f"transformer.encoder.layer.{i}."
-        keys += [f"{lp}{d}.{s}" for d in (*_MCLIP_LAYER, "attention.self.query", "attention.self.key", "attention.self.value")
-                 for s in ("weight", "bias")]
-    return keys
+    return _stack_keys(_MCLIP_TOP.values(), "transformer.encoder.layer.{}.", _MCLIP_LAYER, _MCLIP_QKV, layers)
 
 
 def mclip_to_k2(sd, layers, head_dim=64):
@@ -450,25 +455,21 @@ def mclip_to_k2(sd, layers, head_dim=64):
     reference loads with strict=False, which would silently keep random weights there."""
     sd = {k: v for k, v in sd.items()
           if not k.startswith("transformer.pooler.") and k != "transformer.embeddings.position_ids"}
-    expected = mclip_keys(layers)
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"M-CLIP text encoder state dict: unknown keys {unknown}, missing keys {missing}")
-    out = {k: sd[d] for k, d in _MCLIP_TOP.items()}
-    for i in range(layers):
-        dp, kp = f"transformer.encoder.layer.{i}.", f"layers.{i}."
-        for d, k in _MCLIP_LAYER.items():
-            for s in ("weight", "bias"):
-                out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-        for s in ("weight", "bias"):
-            out[f"{kp}attn.qkv.{s}"] = pack_heads([sd[f"{dp}attention.self.{n}.{s}"] for n in ("query", "key", "value")],
-                                                   head_dim)
-    return out
+    _require_keys(sd, mclip_keys(layers), "M-CLIP text encoder")
+    return _stack_to_k2(sd, _MCLIP_TOP, "transformer.encoder.layer.{}.", _MCLIP_LAYER, _MCLIP_QKV, layers, "layers.{}.",
+                        "attn.qkv", head_dim)
 
 
 # the OpenAI `clip` checkpoint (Kandinsky 2.1's ViT-L-14.pt; clip/model.py build_model reads it): one resblock's names
 _OPENAI_LAYER = {"ln_1": "ln_1", "ln_2": "ln_2", "attn.out_proj": "attn.proj", "mlp.c_fc": "mlp.fc1", "mlp.c_proj": "mlp.fc2"}
+_OPENAI_QKV = ("attn.in_proj_",)
+# the keys outside the resblocks: this package's name -> the checkpoint's name, per tower
+_OPENAI_TEXT_TOP = {"token_embedding": "token_embedding.weight", "position_embedding": "positional_embedding",
+                    "final_ln.weight": "ln_final.weight", "final_ln.bias": "ln_final.bias", "proj.weight": "text_projection"}
+_OPENAI_VISION_TOP = {"class_embedding": "visual.class_embedding", "position_embedding": "visual.positional_embedding",
+                      "patch_embedding.weight": "visual.conv1.weight", "pre_ln.weight": "visual.ln_pre.weight",
+                      "pre_ln.bias": "visual.ln_pre.bias", "post_ln.weight": "visual.ln_post.weight",
+                      "post_ln.bias": "visual.ln_post.bias", "proj.weight": "visual.proj"}
 # the entries build_model deletes before loading, and the contrastive temperature neither tower uses
 _OPENAI_IGNORED = ("input_resolution", "context_length", "vocab_size", "logit_scale")
 
@@ -476,15 +477,9 @@ _OPENAI_IGNORED = ("input_resolution", "context_length", "vocab_size", "logit_sc
 def openai_clip_keys(text_layers, vision_layers):
     """Every key of an OpenAI CLIP (ViT) state dict with the given resblock counts, without the ones openai_clip_to_k2
     ignores."""
-    keys = ["token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection",
-            "visual.class_embedding", "visual.positional_embedding", "visual.conv1.weight", "visual.ln_pre.weight",
-            "visual.ln_pre.bias", "visual.ln_post.weight", "visual.ln_post.bias", "visual.proj"]
-    for prefix, n in (("transformer.", text_layers), ("visual.transformer.", vision_layers)):
-        for i in range(n):
-            lp = f"{prefix}resblocks.{i}."
-            keys += [f"{lp}{d}.{s}" for d in _OPENAI_LAYER for s in ("weight", "bias")]
-            keys += [f"{lp}attn.in_proj_weight", f"{lp}attn.in_proj_bias"]
-    return keys
+    keys = _stack_keys([*_OPENAI_TEXT_TOP.values(), *_OPENAI_VISION_TOP.values()], "transformer.resblocks.{}.", _OPENAI_LAYER,
+                       _OPENAI_QKV, text_layers)
+    return keys + _stack_keys((), "visual.transformer.resblocks.{}.", _OPENAI_LAYER, _OPENAI_QKV, vision_layers)
 
 
 def openai_clip_geometry(sd):
@@ -530,37 +525,19 @@ def openai_clip_to_k2(sd):
     unknown key, and any missing one, raises K2Error naming it."""
     sd = {k: v for k, v in sd.items() if k not in _OPENAI_IGNORED}
     geo = openai_clip_geometry(sd)
-    expected = openai_clip_keys(geo["text"]["layers"], geo["vision"]["layers"])
-    unknown = sorted(set(sd) - set(expected))
-    missing = [k for k in expected if k not in sd]
-    if unknown or missing:
-        raise K2Error(f"OpenAI CLIP state dict: unknown keys {unknown}, missing keys {missing}")
-
-    def layers(prefix, n, width):
-        out = {}
-        for i in range(n):
-            dp, kp = f"{prefix}resblocks.{i}.", f"layers.{i}."
-            for d, k in _OPENAI_LAYER.items():
-                for s in ("weight", "bias"):
-                    out[f"{kp}{k}.{s}"] = sd[f"{dp}{d}.{s}"]
-            for s in ("weight", "bias"):
-                w = sd[f"{dp}attn.in_proj_{s}"]
-                if w.shape[0] != 3 * width:
-                    raise K2Error(f"OpenAI CLIP state dict: {dp}attn.in_proj_{s} has {w.shape[0]} rows, not 3 x {width}")
-                out[f"{kp}attn.qkv.{s}"] = pack_heads(list(w.split(width, 0)), 64)
-        return out
-
-    t, v = geo["text"], geo["vision"]
-    text = {"token_embedding": sd["token_embedding.weight"], "position_embedding": sd["positional_embedding"],
-            "final_ln.weight": sd["ln_final.weight"], "final_ln.bias": sd["ln_final.bias"],
-            "proj.weight": sd["text_projection"].t().contiguous()}
-    text.update(layers("transformer.", t["layers"], t["width"]))
-    vision = {"class_embedding": sd["visual.class_embedding"], "patch_embedding.weight": sd["visual.conv1.weight"],
-              "position_embedding": sd["visual.positional_embedding"], "pre_ln.weight": sd["visual.ln_pre.weight"],
-              "pre_ln.bias": sd["visual.ln_pre.bias"], "post_ln.weight": sd["visual.ln_post.weight"],
-              "post_ln.bias": sd["visual.ln_post.bias"], "proj.weight": sd["visual.proj"].t().contiguous()}
-    vision.update(layers("visual.transformer.", v["layers"], v["width"]))
-    return text, vision, geo
+    _require_keys(sd, openai_clip_keys(geo["text"]["layers"], geo["vision"]["layers"]), "OpenAI CLIP")
+    towers = []
+    for top, prefix, g in ((_OPENAI_TEXT_TOP, "transformer.resblocks.{}.", geo["text"]),
+                           (_OPENAI_VISION_TOP, "visual.transformer.resblocks.{}.", geo["vision"])):
+        for i in range(g["layers"]):
+            for s in _WB:
+                k = f"{prefix.format(i)}attn.in_proj_{s}"
+                if sd[k].shape[0] != 3 * g["width"]:
+                    raise K2Error(f"OpenAI CLIP state dict: {k} has {sd[k].shape[0]} rows, not 3 x {g['width']}")
+        out = _stack_to_k2(sd, top, prefix, _OPENAI_LAYER, _OPENAI_QKV, g["layers"], "layers.{}.", "attn.qkv", 64)
+        out["proj.weight"] = out["proj.weight"].t().contiguous()    # applied as x @ P in clip/model.py
+        towers.append(out)
+    return towers[0], towers[1], geo
 
 
 def load_openai_clip(path_or_sd):
@@ -581,3 +558,36 @@ def load_openai_clip(path_or_sd):
     if not isinstance(sd, dict):
         raise K2Error(f"OpenAI CLIP checkpoint {path}: neither a TorchScript archive nor a state dict")
     return sd
+
+
+def read_json(folder, name, what, required=True):
+    """folder/name parsed as JSON.  A missing file raises K2Error naming it (`what` says who asked), or gives None when the
+    file is not required."""
+    f = os.path.join(folder, name)
+    if not os.path.exists(f):
+        if required:
+            raise K2Error(f"{what}: {f} not found")
+        return None
+    with open(f, encoding="utf-8") as fh:
+        return json.load(fh)
+
+
+def load_weights(folder, candidates, what):
+    """A component's state dict on the CPU from the first of `candidates` (file names in folder, most preferred first) that
+    exists: a *.safetensors file through the safetensors package, skipped when that does not import; any other file with
+    torch.load (weights_only).  K2Error names the files when none can be read."""
+    try:
+        from safetensors.torch import load_file
+    except ImportError:
+        load_file = None
+    for name in candidates:
+        f = os.path.join(folder, name)
+        if not os.path.exists(f):
+            continue
+        if not name.endswith(".safetensors"):
+            return torch.load(f, map_location="cpu", weights_only=True)
+        if load_file is not None:
+            return load_file(f)
+    skipped = load_file is None and any(n.endswith(".safetensors") for n in candidates)
+    note = " (safetensors is not installed)" if skipped else ""
+    raise K2Error(f"{what}: {' or '.join(os.path.join(folder, n) for n in candidates)} not found{note}")

@@ -19,7 +19,6 @@ Parity: tests/test_cpu_clip_text.py pins the oracle (tests/clip_text_oracle.py) 
 (tests/golden/clip_text_tiny.pt); tests/test_gpu_zz_clip_text.py runs the tower against the golden and, at full size on
 synthetic weights, against the fp32 oracle.
 """
-import json
 import os
 import unicodedata
 
@@ -27,8 +26,9 @@ import torch
 
 from .. import ops
 from .._native import K2Error
+from ..checkpoints import read_json
 from ..launch_plan import LaunchPlan
-from .encoder import clip_config, layer_shapes, pack_layers, record_layers
+from .encoder import Tower, clip_config, f16, f32, layer_shapes, pack_layers, record_layers
 
 _REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "max_position_embeddings",
              "vocab_size", "projection_dim")
@@ -163,16 +163,7 @@ class CLIPTokenizer:
     def from_dir(cls, path):
         """A transformers tokenizer folder: vocab.json, merges.txt, and special_tokens_map.json / tokenizer_config.json when
         present (special tokens, the pad token, model_max_length; without one, model_max_length is 77)."""
-        def read_json(name, required):
-            f = os.path.join(path, name)
-            if not os.path.exists(f):
-                if required:
-                    raise K2Error(f"CLIPTokenizer: {f} not found")
-                return {}
-            with open(f, encoding="utf-8") as fh:
-                return json.load(fh)
-
-        vocab = read_json("vocab.json", True)
+        vocab = read_json(path, "vocab.json", "CLIPTokenizer")
         mf = os.path.join(path, "merges.txt")
         if not os.path.exists(mf):
             raise K2Error(f"CLIPTokenizer: {mf} not found")
@@ -180,8 +171,8 @@ class CLIPTokenizer:
             lines = fh.read().split("\n")
         merges = [tuple(ln.split(" ")) for ln in lines if ln and not ln.startswith("#version")]
         kw = {}
-        cfg = read_json("tokenizer_config.json", False)
-        cfg.update(read_json("special_tokens_map.json", False))
+        cfg = read_json(path, "tokenizer_config.json", "CLIPTokenizer", False) or {}
+        cfg.update(read_json(path, "special_tokens_map.json", "CLIPTokenizer", False) or {})
         for k in ("bos_token", "eos_token", "unk_token", "pad_token"):
             v = cfg.get(k)
             if v is not None:
@@ -275,12 +266,13 @@ class CLIPTokenizer:
 # ---------------------------------------------------------------------------------------------------------------------------
 # tower
 # ---------------------------------------------------------------------------------------------------------------------------
-class CLIPTextTower:
+class CLIPTextTower(Tower):
     """CLIPTextModelWithProjection on this package's kernels.  sd: state dict in this module's names
     (checkpoints.transformers_clip_text_to_k2); config: the transformers config.json dict; tokenizer: a CLIPTokenizer (needed
     by __call__ only).  `tokens` is the sequence length __call__ produces: the tokenizer's model_max_length, or
     max_position_embeddings without a tokenizer."""
 
+    what = "CLIP text tower"
     act = "gelu"   # the layers' MLP activation (encoder.ACTIVATIONS)
 
     def __init__(self, sd, config, device="cuda", tokenizer=None):
@@ -293,17 +285,17 @@ class CLIPTextTower:
         if tokenizer is not None and max(tokenizer.vocab.values()) >= c["vocab_size"]:
             raise K2Error(f"CLIP text tower: the tokenizer's ids reach {max(tokenizer.vocab.values())}, beyond the "
                           f"vocabulary of {c['vocab_size']}")
-        H, I, L = c["hidden_size"], c["intermediate_size"], c["num_hidden_layers"]
+        self._take(sd, self._want())
+
+    def _want(self):
+        """{name: shape} of the state dict this tower takes."""
+        c = self.cfg
+        H = c["hidden_size"]
         want = {"token_embedding": (c["vocab_size"], H), "position_embedding": (c["max_position_embeddings"], H),
                 "final_ln.weight": (H,), "final_ln.bias": (H,), "proj.weight": (c["projection_dim"], H)}
-        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, I).items()})
-        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
-        extra = sorted(set(sd) - set(want))
-        if bad or extra:
-            raise K2Error(f"CLIP text tower: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
-        self.sd = sd
-        self._packed = None
-        self._plans = {}
+        want.update({f"layers.{i}.{k}": s for i in range(c["num_hidden_layers"])
+                     for k, s in layer_shapes(H, c["intermediate_size"]).items()})
+        return want
 
     @classmethod
     def from_transformers(cls, state_dict, config, device="cuda", tokenizer=None):
@@ -312,41 +304,26 @@ class CLIPTextTower:
         text_tower_config(config)
         return cls(transformers_clip_text_to_k2(state_dict), config, device, tokenizer).finalize()
 
-    def finalize(self):
-        """Pack the weights on the device once: fp16 GEMM weights [N, K], fp32 biases / LayerNorm parameters / projection, the
-        fp16 token and position tables."""
+    def _pack(self):
+        """fp16 GEMM weights [N, K], fp32 biases / LayerNorm parameters / projection, the fp16 token and position tables."""
         c, dev, sd = self.cfg, self.device, self.sd
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
-        pk = {"tok": sd["token_embedding"].detach().to(dev).half().contiguous(),
-              "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
-              "final_ln": (f32(sd["final_ln.weight"]), f32(sd["final_ln.bias"])), "proj": f32(sd["proj.weight"]),
-              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
-        self._packed = pk
-        self._plans = {}
-        return self
+        return {"tok": f16(sd["token_embedding"], dev), "pos": f16(sd["position_embedding"], dev),
+                "final_ln": (f32(sd["final_ln.weight"], dev), f32(sd["final_ln.bias"], dev)),
+                "proj": f32(sd["proj.weight"], dev),
+                "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
 
     def _plan(self, n, T=None):
-        if self._packed is None:
-            self.finalize()
-        key = (n, self.cfg["max_position_embeddings"] if T is None else T)
-        if key not in self._plans:
-            self._plans[key] = _TextPlan(self, *key)
-        return self._plans[key]
+        return super()._plan(n, self.cfg["max_position_embeddings"] if T is None else T)
+
+    def _new_plan(self, n, T):
+        return _TextPlan(self, n, T)
 
     @torch.no_grad()
     def forward(self, input_ids, use_graph=True):
         """input_ids integer [n, T] (T <= max_position_embeddings) -> (last_hidden_state fp16 [n, T, hidden], text_embeds fp32
         [n, projection_dim]), on the device.  One CUDA graph replay of the (n, T) launch plan (use_graph=False: the same
         launches one by one).  Ids outside [0, vocab_size) are refused before anything is copied."""
-        c = self.cfg
-        if input_ids.dim() != 2 or not 0 < input_ids.shape[1] <= c["max_position_embeddings"] or input_ids.shape[0] == 0:
-            raise K2Error(f"CLIP text tower: input_ids must be [n, T] with 0 < T <= {c['max_position_embeddings']}, got "
-                          f"{list(input_ids.shape)}")
-        if input_ids.is_floating_point() or input_ids.is_complex() or input_ids.dtype == torch.bool:
-            raise K2Error(f"CLIP text tower: input_ids must be integers, got {input_ids.dtype}")
-        lo, hi = int(input_ids.min()), int(input_ids.max())
-        if lo < 0 or hi >= c["vocab_size"]:
-            raise K2Error(f"CLIP text tower: token ids must lie in [0, {c['vocab_size']}), got [{lo}, {hi}]")
+        self._check_ids(input_ids, self.cfg["max_position_embeddings"])
         plan = self._plan(*input_ids.shape)
         plan.ids.copy_(input_ids)
         plan.run(use_graph)
@@ -360,12 +337,12 @@ class CLIPTextTower:
             raise K2Error("CLIP text tower: calling it with prompts needs tokenizer=")
         if isinstance(prompts, str):
             prompts = [prompts]
-        distinct = list(dict.fromkeys(prompts))
-        tok = self.tokenizer(distinct, max_length=self.tokens)
-        hid, emb = self.forward(tok["input_ids"])
-        idx = torch.tensor([distinct.index(p) for p in prompts], device=self.device)
-        mask = tok["attention_mask"].to(self.device).bool()
-        return emb[idx], hid[idx], mask[idx]
+
+        def encode(distinct):
+            tok = self.tokenizer(distinct, max_length=self.tokens)
+            hid, emb = self.forward(tok["input_ids"])
+            return emb, hid, tok["attention_mask"].to(self.device).bool()
+        return self._encode_distinct(prompts, encode)
 
 
 class _TextPlan(LaunchPlan):

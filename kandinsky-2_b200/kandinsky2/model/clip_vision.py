@@ -23,7 +23,8 @@ import torch
 from .. import ops
 from .._native import K2Error
 from ..launch_plan import LaunchPlan
-from .encoder import clip_config, layer_shapes, pack_layers, record_layers
+from .encoder import (Tower, clip_config, f16, f32, layer_shapes, pack_layers, pack_patch_embed, record_layers,
+                      record_patch_embed)
 
 OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -77,16 +78,22 @@ def preprocess_images(images, config=None):
         if cfg["do_center_crop"]:
             ch, cw = int(cfg["crop_size"]["height"]), int(cfg["crop_size"]["width"])
             a = _center_crop(a, ch, cw)
-        x = a
-        if cfg["do_rescale"]:
-            x = (x.astype(np.float64) * cfg["rescale_factor"]).astype(np.float32)
-        if cfg["do_normalize"]:
-            x = x.astype(np.float32) if not np.issubdtype(x.dtype, np.floating) else x
-            mean = np.array(cfg["image_mean"], dtype=x.dtype)
-            std = np.array(cfg["image_std"], dtype=x.dtype)
-            x = ((x.T - mean) / std).T
-        out.append(torch.from_numpy(np.ascontiguousarray(x)).float())
+        out.append(rescale_normalize(a, cfg))
     return torch.stack(out)
+
+
+def rescale_normalize(x, cfg):
+    """The end of transformers' image processors on a uint8 CHW array -> fp32 CHW tensor: float32(x * rescale_factor in
+    float64) when do_rescale, then (x - image_mean) / image_std in float32 when do_normalize (model/depth.py's
+    DPTImageProcessorPil ends the same way)."""
+    if cfg["do_rescale"]:
+        x = (x.astype(np.float64) * cfg["rescale_factor"]).astype(np.float32)
+    if cfg["do_normalize"]:
+        x = x.astype(np.float32) if not np.issubdtype(x.dtype, np.floating) else x
+        mean = np.array(cfg["image_mean"], dtype=x.dtype)
+        std = np.array(cfg["image_std"], dtype=x.dtype)
+        x = ((x.T - mean) / std).T
+    return torch.from_numpy(np.ascontiguousarray(x)).float()
 
 
 def _center_crop(a, ch, cw):
@@ -103,29 +110,29 @@ def _center_crop(a, ch, cw):
     return big[:, max(0, top):min(nh, top + ch), max(0, left):min(nw, left + cw)]
 
 
-class CLIPVisionTower:
+class CLIPVisionTower(Tower):
     """CLIPVisionModelWithProjection on this package's kernels.  sd: state dict in this module's names
     (checkpoints.transformers_clip_vision_to_k2); config: the transformers config.json dict; preprocessor_config: the
     image processor's dict (None = DEFAULT_PREPROCESSOR)."""
 
+    what = "CLIP vision tower"
     act = "gelu"   # the layers' MLP activation (encoder.ACTIVATIONS)
 
     def __init__(self, sd, config, device="cuda", preprocessor_config=None):
-        c = tower_config(config)
-        self.cfg, self.device = c, torch.device(device)
+        self.cfg, self.device = tower_config(config), torch.device(device)
         self.preprocessor_config = preprocessor_config
-        H, I, P, T, L = c["hidden_size"], c["intermediate_size"], c["patch_size"], c["tokens"], c["num_hidden_layers"]
+        self._take(sd, self._want())
+
+    def _want(self):
+        """{name: shape} of the state dict this tower takes."""
+        c = self.cfg
+        H, P, T = c["hidden_size"], c["patch_size"], c["tokens"]
         want = {"class_embedding": (H,), "patch_embedding.weight": (H, 3, P, P), "position_embedding": (T, H),
                 "pre_ln.weight": (H,), "pre_ln.bias": (H,), "post_ln.weight": (H,), "post_ln.bias": (H,),
                 "proj.weight": (c["projection_dim"], H)}
-        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, I).items()})
-        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
-        extra = sorted(set(sd) - set(want))
-        if bad or extra:
-            raise K2Error(f"CLIP vision tower: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
-        self.sd = sd
-        self._packed = None
-        self._plans = {}
+        want.update({f"layers.{i}.{k}": s for i in range(c["num_hidden_layers"])
+                     for k, s in layer_shapes(H, c["intermediate_size"]).items()})
+        return want
 
     @classmethod
     def from_transformers(cls, state_dict, config, device="cuda", preprocessor_config=None):
@@ -135,30 +142,19 @@ class CLIPVisionTower:
         sd = transformers_clip_vision_to_k2(state_dict, head_dim=c["head_dim"])
         return cls(sd, config, device, preprocessor_config).finalize()
 
-    def finalize(self):
-        """Pack the weights on the device once: fp16 GEMM weights [N, K] (the patch embedding as [H, Kp] with the class
-        embedding in column 3 P^2), fp32 biases / LayerNorm parameters / projection, the fp16 position embedding."""
+    def _pack(self):
+        """fp16 GEMM weights [N, K] (the patch embedding as [H, Kp] with the class embedding in column 3 P^2,
+        pack_patch_embed), fp32 biases / LayerNorm parameters / projection, the fp16 position embedding."""
         c, dev, sd = self.cfg, self.device, self.sd
-        H, P, kp = c["hidden_size"], c["patch_size"], c["kp"]
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
-        K = 3 * P * P
-        we = torch.zeros(H, kp, dtype=torch.float16, device=dev)
-        we[:, :K] = sd["patch_embedding.weight"].detach().to(dev).reshape(H, K).half()
-        we[:, K] = sd["class_embedding"].detach().to(dev).half()
-        pk = {"embed": we, "pos": sd["position_embedding"].detach().to(dev).half().contiguous(),
-              "pre_ln": (f32(sd["pre_ln.weight"]), f32(sd["pre_ln.bias"])),
-              "post_ln": (f32(sd["post_ln.weight"]), f32(sd["post_ln.bias"])), "proj": f32(sd["proj.weight"]),
-              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
-        self._packed = pk
-        self._plans = {}
-        return self
+        return {"embed": pack_patch_embed(sd["patch_embedding.weight"], sd["class_embedding"], c["kp"], dev),
+                "pos": f16(sd["position_embedding"], dev),
+                "pre_ln": (f32(sd["pre_ln.weight"], dev), f32(sd["pre_ln.bias"], dev)),
+                "post_ln": (f32(sd["post_ln.weight"], dev), f32(sd["post_ln.bias"], dev)),
+                "proj": f32(sd["proj.weight"], dev),
+                "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
 
-    def _plan(self, B):
-        if self._packed is None:
-            self.finalize()
-        if B not in self._plans:
-            self._plans[B] = _TowerPlan(self, B)
-        return self._plans[B]
+    def _new_plan(self, B):
+        return _TowerPlan(self, B)
 
     def attend(self, qkv, out):
         """The layers' attention: qkv fp16 [B, T, heads * 3 head_dim] (per head [q | k | v]) -> out fp16 [B, T, hidden]."""
@@ -175,7 +171,7 @@ class CLIPVisionTower:
         the device.  One CUDA graph replay of the batch size's launch plan (use_graph=False: the same launches one by one)."""
         S = self.cfg["image_size"]
         if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
-            raise K2Error(f"CLIP vision tower: pixel_values must be [B, 3, {S}, {S}], got {list(pixel_values.shape)}")
+            raise K2Error(f"{self.what}: pixel_values must be [B, 3, {S}, {S}], got {list(pixel_values.shape)}")
         plan = self._plan(pixel_values.shape[0])
         plan.pix.copy_(pixel_values)
         plan.run(use_graph)
@@ -215,10 +211,8 @@ class _TowerPlan(LaunchPlan):
     def _build(self):
         c, pk, B, S = self.t.cfg, self.t._packed, self.B, self._add
         T, H, hd, heads, eps = c["tokens"], c["hidden_size"], c["head_dim"], c["num_attention_heads"], c["layer_norm_eps"]
-        rows = self._new(B, T, c["kp"])
-        S(lambda: ops.clip_patchify(self.pix, c["patch_size"], c["kp"], out=rows), "patchify")
-        emb, x = self._new(B, T, H), self._new(B, T, H)
-        self._gemm(rows, pk["embed"], H, emb, 2 * B * T * c["kp"] * H, residual=self.pos)
+        emb = record_patch_embed(self, self.pix, pk["embed"], self.pos, c["patch_size"], c["kp"])
+        x = self._new(B, T, H)
         S(lambda: ops.layernorm_f16(emb, *pk["pre_ln"], eps=eps, out=x), "layernorm")
         h = record_layers(self, x, pk["layers"], self.t.attend, 4 * B * heads * T * T * hd, eps, act=self.t.act)
         self.hidden = h

@@ -43,7 +43,6 @@ from .. import ops
 from .._native import K2Error
 from .clip_text import CLIPTextTower, CLIPTokenizer, _clip_split, bytes_to_unicode
 from .clip_vision import OPENAI_CLIP_MEAN, OPENAI_CLIP_STD, CLIPVisionTower
-from .encoder import layer_shapes
 
 IMAGE_SIZE = 224
 
@@ -207,18 +206,12 @@ def preprocess_openai(images, size=IMAGE_SIZE):
 # ---------------------------------------------------------------------------------------------------------------------------
 # towers
 # ---------------------------------------------------------------------------------------------------------------------------
-def _check_keys(sd, want, what):
-    bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
-    extra = sorted(set(sd) - set(want))
-    if bad or extra:
-        raise K2Error(f"OpenAI CLIP {what} tower: keys missing or of the wrong shape {bad}, unknown keys {extra}")
-
-
 class OpenAICLIPTextTower(CLIPTextTower):
     """The text side of OpenAI CLIP (`generate_clip_emb`'s tower lines) on the 2.2 text tower's launch plan with QuickGELU.
     sd: the text state dict of checkpoints.openai_clip_to_k2; geo: its geometry["text"]; tokenizer: an OpenAICLIPTokenizer
     (needed by __call__ only)."""
 
+    what = "OpenAI CLIP text tower"
     act = "quick_gelu"
 
     def __init__(self, sd, geo, device="cuda", tokenizer=None):
@@ -232,11 +225,7 @@ class OpenAICLIPTextTower(CLIPTextTower):
         if tokenizer is not None and max(tokenizer.vocab.values()) >= geo["vocab"]:
             raise K2Error(f"OpenAI CLIP text tower: the tokenizer's ids reach {max(tokenizer.vocab.values())}, beyond the "
                           f"vocabulary of {geo['vocab']}")
-        want = {"token_embedding": (geo["vocab"], H), "position_embedding": (T, H), "final_ln.weight": (H,),
-                "final_ln.bias": (H,), "proj.weight": (geo["embed_dim"], H)}
-        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, geo["mlp"]).items()})
-        _check_keys(sd, want, "text")
-        self.sd, self._packed, self._plans = sd, None, {}
+        self._take(sd, self._want())
 
     def __call__(self, prompts):
         """The 2.1 PriorEmbedder's clip_text protocol, with generate_clip_emb's semantics: list[str] -> (txt_feat fp32
@@ -246,11 +235,12 @@ class OpenAICLIPTextTower(CLIPTextTower):
             raise K2Error("OpenAI CLIP text tower: calling it with prompts needs tokenizer=")
         if isinstance(prompts, str):
             prompts = [prompts]
-        distinct = list(dict.fromkeys(prompts))
-        tok, mask = self.tokenizer.padded_tokens_and_mask(distinct, self.tokens)
-        hid, emb = self.forward(tok)
-        idx = torch.tensor([distinct.index(p) for p in prompts], device=self.device)
-        return emb[idx], hid.float()[idx], mask.to(self.device)[idx]
+
+        def encode(distinct):
+            tok, mask = self.tokenizer.padded_tokens_and_mask(distinct, self.tokens)
+            hid, emb = self.forward(tok)
+            return emb, hid.float(), mask.to(self.device)
+        return self._encode_distinct(prompts, encode)
 
 
 class OpenAICLIPVisionTower(CLIPVisionTower):
@@ -259,20 +249,17 @@ class OpenAICLIPVisionTower(CLIPVisionTower):
     geometry["vision"].  zero_embed() (the 2.2 tower's: the tower on an all-zero [1, 3, S, S] tensor, not preprocessed) is
     the reference's create_zero_img_emb."""
 
+    what = "OpenAI CLIP vision tower"
     act = "quick_gelu"
 
     def __init__(self, sd, geo, device="cuda"):
-        H, L, P, T = geo["width"], geo["layers"], geo["patch"], geo["tokens"]
-        self.cfg = dict(hidden_size=H, intermediate_size=geo["mlp"], num_hidden_layers=L, num_attention_heads=geo["heads"],
-                        head_dim=64, image_size=geo["image_size"], patch_size=P, projection_dim=geo["embed_dim"],
-                        layer_norm_eps=1e-5, tokens=T, kp=(3 * P * P + 1 + 63) // 64 * 64)
+        P = geo["patch"]
+        self.cfg = dict(hidden_size=geo["width"], intermediate_size=geo["mlp"], num_hidden_layers=geo["layers"],
+                        num_attention_heads=geo["heads"], head_dim=64, image_size=geo["image_size"], patch_size=P,
+                        projection_dim=geo["embed_dim"], layer_norm_eps=1e-5, tokens=geo["tokens"],
+                        kp=(3 * P * P + 1 + 63) // 64 * 64)
         self.device, self.preprocessor_config = torch.device(device), None
-        want = {"class_embedding": (H,), "patch_embedding.weight": (H, 3, P, P), "position_embedding": (T, H),
-                "pre_ln.weight": (H,), "pre_ln.bias": (H,), "post_ln.weight": (H,), "post_ln.bias": (H,),
-                "proj.weight": (geo["embed_dim"], H)}
-        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, geo["mlp"]).items()})
-        _check_keys(sd, want, "vision")
-        self.sd, self._packed, self._plans = sd, None, {}
+        self._take(sd, self._want())
 
     def attend(self, qkv, out):
         """k2_attention_d64 over the image tokens (no encoder tokens; per-head [q | k | v], scale 1/8)."""

@@ -34,7 +34,6 @@ Parity: tests/test_cpu_dpt.py pins the oracle (tests/dpt_oracle.py), preprocess 
 (tests/golden/dpt_tiny.pt); tests/test_gpu_zz_depth.py runs the estimator against the golden and, at the Intel/dpt-large
 geometry on synthetic weights, against the fp32 oracle.
 """
-import json
 import math
 import os
 
@@ -43,8 +42,10 @@ import torch
 
 from .. import ops
 from .._native import K2Error
+from ..checkpoints import load_weights, read_json
 from ..launch_plan import LaunchPlan
-from .encoder import layer_shapes, pack_layers, record_layers
+from .clip_vision import rescale_normalize
+from .encoder import Tower, f32, layer_shapes, pack_layers, pack_patch_embed, record_layers, record_patch_embed
 
 # transformers' DPTConfig defaults, for keys a config.json leaves out
 _CONFIG_DEFAULTS = dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
@@ -175,15 +176,7 @@ def preprocess_images(images, cfg, size):
         if img.size != (size, size):
             raise K2Error(f"DPT preprocessing: the image is processed to {img.size[1]} x {img.size[0]}; only the square "
                           f"{size} x {size} input of this estimator is implemented")
-        x = np.array(img).transpose(2, 0, 1)
-        if cfg["do_rescale"]:
-            x = (x.astype(np.float64) * cfg["rescale_factor"]).astype(np.float32)
-        if cfg["do_normalize"]:
-            x = x.astype(np.float32) if not np.issubdtype(x.dtype, np.floating) else x
-            mean = np.array(cfg["image_mean"], dtype=x.dtype)
-            std = np.array(cfg["image_std"], dtype=x.dtype)
-            x = ((x.T - mean) / std).T
-        out.append(torch.from_numpy(np.ascontiguousarray(x)).float())
+        out.append(rescale_normalize(np.array(img).transpose(2, 0, 1), cfg))
     return torch.stack(out)
 
 
@@ -216,11 +209,13 @@ def resize_pos_embed(pos, grid):
     return torch.cat([pos[:1].float(), p.permute(0, 2, 3, 1).reshape(grid * grid, -1)])
 
 
-class DPTDepthEstimator:
+class DPTDepthEstimator(Tower):
     """DPTForDepthEstimation (plain ViT) on this package's kernels.  sd: state dict in this module's names
     (checkpoints.transformers_dpt_to_k2); config: the transformers config.json dict; preprocessor_config: the image
     processor's preprocessor_config.json dict (None: DPTImageProcessorPil's defaults at the model's image_size).  The input
     size is the processor's; the position embedding is resized to its patch grid once, on the host."""
+
+    what = "DPT"
 
     def __init__(self, sd, config, device="cuda", preprocessor_config=None):
         c = dpt_config(config)
@@ -231,12 +226,7 @@ class DPTDepthEstimator:
             raise K2Error(f"DPT preprocessing: size {self.proc['size']}: only a square input that is a multiple of the patch "
                           f"size {c['patch_size']} is implemented")
         self.size, self.grid = S, S // c["patch_size"]
-        want = k2_shapes(c)
-        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
-        extra = sorted(set(sd) - set(want))
-        if bad or extra:
-            raise K2Error(f"DPT: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
-        self.sd, self._packed, self._plans = sd, None, {}
+        self._take(sd, k2_shapes(c))
 
     @classmethod
     def from_transformers(cls, state_dict, config, preprocessor_config=None, device="cuda"):
@@ -248,49 +238,37 @@ class DPTDepthEstimator:
     def from_pretrained(cls, path, device="cuda"):
         """A local transformers model folder (e.g. a download of Intel/dpt-large): config.json, preprocessor_config.json
         (optional) and model.safetensors or pytorch_model.bin.  A missing file raises K2Error naming it."""
-        from .prior import _load_weights
-
-        def read(name, required=True):
-            f = os.path.join(path, name)
-            if not os.path.exists(f):
-                if required:
-                    raise K2Error(f"DPTDepthEstimator.from_pretrained: {f} not found")
-                return None
-            with open(f, encoding="utf-8") as fh:
-                return json.load(fh)
-
-        config = read("config.json")
+        what = "DPTDepthEstimator.from_pretrained"
         stem = "pytorch_model" if os.path.exists(os.path.join(path, "pytorch_model.bin")) else "model"
-        return cls.from_transformers(_load_weights(path, stem), config, read("preprocessor_config.json", False), device)
+        return cls.from_transformers(load_weights(path, (f"{stem}.safetensors", f"{stem}.bin"), what),
+                                     read_json(path, "config.json", what),
+                                     read_json(path, "preprocessor_config.json", what, required=False), device)
 
-    def finalize(self):
-        """Pack the weights on the device once (fp16 GEMM weights, fp32 biases and LayerNorm parameters)."""
+    def _pack(self):
+        """fp16 GEMM weights (the patch embedding as pack_patch_embed's [H, Kp]), fp32 biases and LayerNorm parameters, the
+        fp16 position embedding at the input's patch grid with the patch convolution's bias folded into the patch rows."""
         c, dev, sd = self.cfg, self.device, self.sd
-        H, P, kp, F = c["hidden_size"], c["patch_size"], c["kp"], c["fusion_hidden_size"]
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+        F = c["fusion_hidden_size"]
         w = lambda name: ops.pack_conv_weight(sd[name].detach().to(dev))  # noqa: E731
-        K = 3 * P * P
-        we = torch.zeros(H, kp, dtype=torch.float16, device=dev)
-        we[:, :K] = sd["patch_embedding.weight"].detach().to(dev).reshape(H, K).half()
-        we[:, K] = sd["cls_token"].detach().to(dev).half()
         pos = resize_pos_embed(sd["position_embedding"].detach().cpu(), self.grid)
         pos[1:] += sd["patch_embedding.bias"].detach().cpu().float()   # the patch conv's bias, on the patch rows only
-        pk = {"embed": we, "pos": pos.to(dev).half().contiguous(),
+        pk = {"embed": pack_patch_embed(sd["patch_embedding.weight"], sd["cls_token"], c["kp"], dev),
+              "pos": pos.to(dev).half().contiguous(),
               "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["backbone_out_indices"][-1] + 1, dev)}
         rs = "neck.reassemble_stage."
         for i, (C, f) in enumerate(zip(c["neck_hidden_sizes"], c["reassemble_factors"])):
-            pk[f"readout.{i}"] = (w(f"{rs}readout_projects.{i}.0.weight"), f32(sd[f"{rs}readout_projects.{i}.0.bias"]))
-            pk[f"proj.{i}"] = (w(f"{rs}layers.{i}.projection.weight"), f32(sd[f"{rs}layers.{i}.projection.bias"]))
+            pk[f"readout.{i}"] = (w(f"{rs}readout_projects.{i}.0.weight"), f32(sd[f"{rs}readout_projects.{i}.0.bias"], dev))
+            pk[f"proj.{i}"] = (w(f"{rs}layers.{i}.projection.weight"), f32(sd[f"{rs}layers.{i}.projection.bias"], dev))
             rw, rb = sd.get(f"{rs}layers.{i}.resize.weight"), sd.get(f"{rs}layers.{i}.resize.bias")
             if f > 1:   # ConvTranspose2d weight [in, out, a, b] -> GEMM rows (a s + b) C + out over K = in
                 s = int(f)
                 g = rw.detach().to(dev).permute(2, 3, 1, 0).reshape(s * s * C, C)
-                pk[f"resize.{i}"] = (ops.pack_conv_weight(g), f32(rb).repeat(s * s))
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(g), f32(rb, dev).repeat(s * s))
             elif f < 1:
-                pk[f"resize.{i}"] = (ops.pack_conv_weight(rw.detach().to(dev)), f32(rb))
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(rw.detach().to(dev)), f32(rb, dev))
             pk[f"neck_conv.{i}"] = w(f"neck.convs.{i}.weight")
             fp = f"neck.fusion_stage.layers.{i}."
-            pk[f"fusion_proj.{i}"] = (w(fp + "projection.weight"), f32(sd[fp + "projection.bias"]))
+            pk[f"fusion_proj.{i}"] = (w(fp + "projection.weight"), f32(sd[fp + "projection.bias"], dev))
             for u in ((1, 2) if i else (2,)):
                 p = f"{fp}residual_layer{u}."
                 c2 = w(p + "convolution2.weight")
@@ -298,20 +276,15 @@ class DPTDepthEstimator:
                     eye = torch.zeros(F, c2.shape[1] // 9, dtype=torch.float16, device=dev)
                     eye[:, :F] = torch.eye(F, dtype=torch.float16, device=dev)
                     c2 = torch.cat([c2, eye], 1).contiguous()
-                pk[f"unit{u}.{i}"] = ((w(p + "convolution1.weight"), f32(sd[p + "convolution1.bias"])),
-                                      (c2, f32(sd[p + "convolution2.bias"])))
-        pk["head"] = [(w("head.head.0.weight"), f32(sd["head.head.0.bias"])),
-                      (w("head.head.2.weight"), f32(sd["head.head.2.bias"])),
-                      (ops.pad_rows(w("head.head.4.weight"), 16), f32(sd["head.head.4.bias"]))]
-        self._packed, self._plans = pk, {}
-        return self
+                pk[f"unit{u}.{i}"] = ((w(p + "convolution1.weight"), f32(sd[p + "convolution1.bias"], dev)),
+                                      (c2, f32(sd[p + "convolution2.bias"], dev)))
+        pk["head"] = [(w("head.head.0.weight"), f32(sd["head.head.0.bias"], dev)),
+                      (w("head.head.2.weight"), f32(sd["head.head.2.bias"], dev)),
+                      (ops.pad_rows(w("head.head.4.weight"), 16), f32(sd["head.head.4.bias"], dev))]
+        return pk
 
-    def _plan(self, B):
-        if self._packed is None:
-            self.finalize()
-        if B not in self._plans:
-            self._plans[B] = _DepthPlan(self, B)
-        return self._plans[B]
+    def _new_plan(self, B):
+        return _DepthPlan(self, B)
 
     def attend(self, qkv, out):
         """The layers' attention: k2_attention_d64 over the tokens (per-head [q | k | v], scale 1/8)."""
@@ -387,10 +360,7 @@ class _DepthPlan(LaunchPlan):
         c = e.cfg
         G, H, P, F = e.grid, c["hidden_size"], c["patch_size"], c["fusion_hidden_size"]
         T, heads, eps = G * G + 1, c["num_attention_heads"], c["layer_norm_eps"]
-        rows = self._new(B, T, c["kp"])
-        A(lambda: ops.clip_patchify(self.pix, P, c["kp"], out=rows), "patchify")
-        h = self._new(B, T, H)
-        self._gemm(rows, pk["embed"], H, h, 2 * B * T * c["kp"] * H, residual=self.pos)
+        h = record_patch_embed(self, self.pix, pk["embed"], self.pos, P, c["kp"])
         hidden, start = [], 0
         for idx in c["backbone_out_indices"]:
             h = record_layers(self, h, pk["layers"][start:idx + 1], e.attend, 4 * B * heads * T * T * 64, eps)

@@ -5,7 +5,11 @@ records in a LaunchPlan:
 The attention launch is the caller's; everything else is the same for all the models (the 2.1 ViT-L/14 towers of
 model/clip_vitl14.py record QuickGELU instead of GELU: record_layers(act="quick_gelu")).  record_layers(post_ln=True)
 records the post-LayerNorm layer of the 2.1 text encoder (model/text_encoders.py, XLM-RoBERTa) over the same packed names.
-Also the part of the transformers CLIP config both towers read."""
+
+Around the stack: Tower, the shell of every tower that runs as graph-replayed launch plans (the CLIP towers, XLM-R, DPT):
+the state-dict check, the packed weights, the plan cache, the token-id check and the distinct-prompt encode; the ViT patch
+embedding the image towers share (pack_patch_embed, record_patch_embed); the f32 / f16 device packers; and the part of the
+transformers CLIP config both CLIP towers read."""
 import torch
 
 from .. import ops
@@ -25,16 +29,25 @@ def layer_shapes(H, I):
             "mlp.fc1.weight": (I, H), "mlp.fc1.bias": (I,), "mlp.fc2.weight": (H, I), "mlp.fc2.bias": (H,)}
 
 
+def f32(t, dev):
+    """t as a contiguous fp32 tensor on dev."""
+    return t.detach().to(dev, torch.float32).contiguous()
+
+
+def f16(t, dev):
+    """t as a contiguous fp16 tensor on dev."""
+    return t.detach().to(dev, torch.float16).contiguous()
+
+
 def pack_layers(get, L, dev):
     """L layers packed on `dev` once: a list of dicts with "ln_1" / "ln_2" -> (fp32 gain, fp32 bias) and "attn.qkv",
     "attn.proj", "mlp.fc1", "mlp.fc2" -> (fp16 [N, K] GEMM weight, ops.pack_conv_weight; fp32 bias).  get(i, name) returns
     layer i's parameter `name` (a layer_shapes key)."""
-    f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
     layers = []
     for i in range(L):
-        p = {n: (f32(get(i, n + ".weight")), f32(get(i, n + ".bias"))) for n in _NORMS}
+        p = {n: (f32(get(i, n + ".weight"), dev), f32(get(i, n + ".bias"), dev)) for n in _NORMS}
         for n in _GEMMS:
-            p[n] = (ops.pack_conv_weight(get(i, n + ".weight").detach().to(dev)), f32(get(i, n + ".bias")))
+            p[n] = (ops.pack_conv_weight(get(i, n + ".weight").detach().to(dev)), f32(get(i, n + ".bias"), dev))
         layers.append(p)
     return layers
 
@@ -90,6 +103,78 @@ def _record_post_ln(plan, h, layers, attend, attn_flops, eps, act):
         S(lambda L=L: ops.layernorm_f16(hB, *L["ln_2"], eps=eps, out=out), "layernorm")
         h = out
     return h
+
+
+def pack_patch_embed(weight, cls, kp, dev):
+    """The ViT patch embedding as one fp16 GEMM weight [H, kp] on dev: the patch convolution's weight [H, 3, P, P] in columns
+    [0, 3 P^2), the class embedding [H] in column 3 P^2 (k2_clip_patchify's CLS row holds a 1 there), zeros after."""
+    H, K = weight.shape[0], weight[0].numel()
+    we = torch.zeros(H, kp, dtype=torch.float16, device=dev)
+    we[:, :K] = weight.detach().to(dev).reshape(H, K).half()
+    we[:, K] = cls.detach().to(dev).half()
+    return we
+
+
+def record_patch_embed(plan, pix, embed, pos, patch, kp):
+    """Record the ViT embedding into `plan`: k2_clip_patchify of pix fp32 [B, 3, S, S] into [CLS | patch] rows of width kp,
+    then ONE GEMM with pack_patch_embed's weight and pos fp16 [B, T, H] as the epilogue residual.  Returns the fp16
+    embeddings [B, T, H]."""
+    B, T, H = pos.shape
+    rows = plan._new(B, T, kp)
+    plan._add(lambda: ops.clip_patchify(pix, patch, kp, out=rows), "patchify")
+    emb = plan._new(B, T, H)
+    plan._gemm(rows, embed, H, emb, 2 * B * T * kp * H, residual=pos)
+    return emb
+
+
+class Tower:
+    """The shell of a tower that runs as graph-replayed launch plans: the state-dict check, the weights packed on the device
+    once, one plan per input geometry built on demand, the token-id check and the distinct-prompt encode.  A subclass sets
+    `what` (the name its K2Error messages start with) and `device`, calls _take(sd, want) from its constructor, and
+    implements _pack() (the packed dict, read by its plans as tower._packed) and _new_plan(*key) (its LaunchPlan)."""
+
+    what = "tower"
+
+    def _take(self, sd, want):
+        """Keep the state dict sd after checking it against want {name: shape}: K2Error names the keys missing or of another
+        shape and the unknown keys.  Nothing is packed yet: finalize() does that, or the first _plan()."""
+        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
+        extra = sorted(set(sd) - set(want))
+        if bad or extra:
+            raise K2Error(f"{self.what}: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
+        self.sd, self._packed, self._plans = sd, None, {}
+
+    def finalize(self):
+        """Pack the weights on the device once (_pack); plans built on earlier weights are dropped."""
+        self._packed, self._plans = self._pack(), {}
+        return self
+
+    def _plan(self, *key):
+        """The launch plan for `key`, built (and the weights packed) on first use."""
+        if self._packed is None:
+            self.finalize()
+        if key not in self._plans:
+            self._plans[key] = self._new_plan(*key)
+        return self._plans[key]
+
+    def _check_ids(self, input_ids, max_tokens):
+        """K2Error unless input_ids is an integer [n, T] tensor with n > 0, 0 < T <= max_tokens and every id in
+        [0, cfg["vocab_size"]); checked before anything is copied to the device."""
+        if input_ids.dim() != 2 or not 0 < input_ids.shape[1] <= max_tokens or input_ids.shape[0] == 0:
+            raise K2Error(f"{self.what}: input_ids must be [n, T] with 0 < T <= {max_tokens}, got {list(input_ids.shape)}")
+        if input_ids.is_floating_point() or input_ids.is_complex() or input_ids.dtype == torch.bool:
+            raise K2Error(f"{self.what}: input_ids must be integers, got {input_ids.dtype}")
+        lo, hi, V = int(input_ids.min()), int(input_ids.max()), self.cfg["vocab_size"]
+        if lo < 0 or hi >= V:
+            raise K2Error(f"{self.what}: token ids must lie in [0, {V}), got [{lo}, {hi}]")
+
+    def _encode_distinct(self, prompts, encode):
+        """encode(distinct prompts) -> device tensors with one row per distinct prompt, in order; returns them with the rows
+        gathered back to one per prompt, so that each distinct prompt is tokenized and encoded once."""
+        distinct = list(dict.fromkeys(prompts))
+        outs = encode(distinct)
+        idx = torch.tensor([distinct.index(p) for p in prompts], device=self.device)
+        return tuple(t[idx] for t in outs)
 
 
 def clip_config(config, required, what, head_dim):

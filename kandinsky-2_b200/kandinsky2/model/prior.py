@@ -495,23 +495,6 @@ def sample_prior22(model, text_emb, text_enc, mask, num_steps, guidance, clip_me
     return plan.x * clip_std + clip_mean
 
 
-def _load_weights(folder, stem):
-    """A diffusers / transformers component's state dict on the CPU: folder/stem.safetensors when the safetensors package
-    imports and the file exists, else folder/stem.bin (torch.load, weights_only).  K2Error names the file when neither is
-    there."""
-    try:
-        from safetensors.torch import load_file
-    except ImportError:
-        load_file = None
-    st, bin_ = os.path.join(folder, stem + ".safetensors"), os.path.join(folder, stem + ".bin")
-    if load_file is not None and os.path.exists(st):
-        return load_file(st)
-    if os.path.exists(bin_):
-        return torch.load(bin_, map_location="cpu", weights_only=True)
-    want = f"{st} or {bin_}" if load_file is not None else f"{bin_} (safetensors is not installed)"
-    raise K2Error(f"PriorEmbedder22.from_pretrained: {want} not found")
-
-
 class PriorEmbedder22:
     """The Kandinsky 2.2 diffusion prior behind the pipelines' `embedder` protocol: what diffusers'
     `KandinskyV22PriorPipeline.__call__` does for the reference's Kandinsky2_2 methods (kandinsky2_2_model.py:69-80,
@@ -581,28 +564,24 @@ class PriorEmbedder22:
             image_processor/ preprocessor_config.json                       (optional)
         *.safetensors are read when the safetensors package imports, else the .bin files (torch.load, weights_only).  A
         missing file raises K2Error naming it.  kwargs go to from_diffusers (prior_steps, seed, ...)."""
-        import json
-
+        from ..checkpoints import load_weights, read_json
         from .clip_text import CLIPTextTower, CLIPTokenizer
+        what = "PriorEmbedder22.from_pretrained"
 
-        def read_config(sub, name="config.json"):
-            f = os.path.join(path, sub, name)
-            if not os.path.exists(f):
-                raise K2Error(f"PriorEmbedder22.from_pretrained: {f} not found")
-            with open(f, encoding="utf-8") as fh:
-                return json.load(fh)
+        def weights(sub, stem):
+            return load_weights(os.path.join(path, sub), (f"{stem}.safetensors", f"{stem}.bin"), what)
 
-        tok_dir = os.path.join(path, "tokenizer")
-        tower = CLIPTextTower.from_transformers(_load_weights(os.path.join(path, "text_encoder"), "model"),
-                                                read_config("text_encoder"), device, CLIPTokenizer.from_dir(tok_dir))
+        tower = CLIPTextTower.from_transformers(weights("text_encoder", "model"),
+                                                read_json(os.path.join(path, "text_encoder"), "config.json", what), device,
+                                                CLIPTokenizer.from_dir(os.path.join(path, "tokenizer")))
         if os.path.isdir(os.path.join(path, "image_encoder")) and kwargs.get("image_encoder") is None:
             from .clip_vision import CLIPVisionTower
-            proc = (read_config("image_processor", "preprocessor_config.json")
+            proc = (read_json(os.path.join(path, "image_processor"), "preprocessor_config.json", what)
                     if os.path.isdir(os.path.join(path, "image_processor")) else None)
             kwargs["image_encoder"] = CLIPVisionTower.from_transformers(
-                _load_weights(os.path.join(path, "image_encoder"), "model"), read_config("image_encoder"), device, proc)
-        return cls.from_diffusers(_load_weights(os.path.join(path, "prior"), "diffusion_pytorch_model"), device=device,
-                                  text_encoder=tower, **kwargs)
+                weights("image_encoder", "model"), read_json(os.path.join(path, "image_encoder"), "config.json", what), device,
+                proc)
+        return cls.from_diffusers(weights("prior", "diffusion_pytorch_model"), device=device, text_encoder=tower, **kwargs)
 
     def _call_args(self, prompt, B, prior_steps, prior_guidance_scale, negative_prior_prompt):
         """(steps, guidance, CFG rows [text_embeds, hidden states, mask] on the device, the call's generator): the rows are

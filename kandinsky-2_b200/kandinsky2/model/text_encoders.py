@@ -24,8 +24,6 @@ Parity: tests/test_cpu_text_encoder.py pins the tokenizer and the oracle (tests/
 synthetic weights, against the fp32 oracle.
 """
 import base64
-import json
-import os
 import re
 import struct
 import unicodedata
@@ -34,8 +32,9 @@ import torch
 
 from .. import ops
 from .._native import K2Error
+from ..checkpoints import load_weights, read_json
 from ..launch_plan import LaunchPlan
-from .encoder import layer_shapes, pack_layers, record_layers
+from .encoder import Tower, f16, f32, layer_shapes, pack_layers, record_layers
 
 _REQUIRED = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "max_position_embeddings",
              "vocab_size")
@@ -459,17 +458,10 @@ class XLMRobertaTokenizer:
     def from_dir(cls, path, model_max_length=77):
         """A transformers tokenizer folder: tokenizer.json, and special_tokens_map.json / tokenizer_config.json when present
         (the pad token; default "<pad>").  model_max_length is the row length (encode_text's max_length=77)."""
-        f = os.path.join(path, "tokenizer.json")
-        if not os.path.exists(f):
-            raise K2Error(f"XLM-R tokenizer: {f} not found")
-        with open(f, encoding="utf-8") as fh:
-            spec = json.load(fh)
+        spec = read_json(path, "tokenizer.json", "XLM-R tokenizer")
         cfg = {}
         for name in ("tokenizer_config.json", "special_tokens_map.json"):
-            p = os.path.join(path, name)
-            if os.path.exists(p):
-                with open(p, encoding="utf-8") as fh:
-                    cfg.update(json.load(fh))
+            cfg.update(read_json(path, name, "XLM-R tokenizer", False) or {})
         pad = cfg.get("pad_token", "<pad>")
         pad = pad["content"] if isinstance(pad, dict) else pad
         return cls(spec, pad_token=pad, model_max_length=model_max_length)
@@ -530,21 +522,12 @@ class XLMRobertaTokenizer:
 # ---------------------------------------------------------------------------------------------------------------------------
 # tower
 # ---------------------------------------------------------------------------------------------------------------------------
-def _load_state_dict(path):
-    for name in ("pytorch_model.bin", "model.safetensors"):
-        f = os.path.join(path, name)
-        if os.path.exists(f):
-            if name.endswith(".safetensors"):
-                from safetensors.torch import load_file
-                return load_file(f)
-            return torch.load(f, map_location="cpu", weights_only=True)
-    raise K2Error(f"M-CLIP text encoder: neither pytorch_model.bin nor model.safetensors in {path}")
-
-
-class MultilingualCLIP:
+class MultilingualCLIP(Tower):
     """The reference's MultilingualCLIP on this package's kernels.  sd: state dict in this module's names
     (checkpoints.mclip_to_k2); config: the transformers config.json dict; tokenizer: an XLMRobertaTokenizer (needed by
     __call__ only).  `tokens` is the row length __call__ produces: the tokenizer's model_max_length (77), or 77 without one."""
+
+    what = "M-CLIP text encoder"
 
     def __init__(self, sd, config, device="cuda", tokenizer=None):
         c = xlmr_config(config)
@@ -559,20 +542,16 @@ class MultilingualCLIP:
         if tokenizer is not None and tokenizer.pad_token_id != c["pad_token_id"]:
             raise K2Error(f"M-CLIP text encoder: the tokenizer pads with {tokenizer.pad_token_id}, the config's pad_token_id "
                           f"is {c['pad_token_id']}")
-        H, I, L = c["hidden_size"], c["intermediate_size"], c["num_hidden_layers"]
+        H = c["hidden_size"]
         proj = sd.get("proj.weight")
-        self.out_features = int(proj.shape[0]) if proj is not None and proj.dim() == 2 else -1
+        # the output width is the projection's; one that is missing, not 2-D or empty is refused below as (-1, H)
+        self.out_features = int(proj.shape[0]) if proj is not None and proj.dim() == 2 and proj.shape[0] > 0 else -1
         want = {"word_embedding": (c["vocab_size"], H), "position_embedding": (c["max_position_embeddings"], H),
                 "token_type_embedding": (1, H), "emb_ln.weight": (H,), "emb_ln.bias": (H,),
                 "proj.weight": (self.out_features, H), "proj.bias": (self.out_features,)}
-        want.update({f"layers.{i}.{k}": s for i in range(L) for k, s in layer_shapes(H, I).items()})
-        bad = [k for k, s in want.items() if k not in sd or tuple(sd[k].shape) != s]
-        extra = sorted(set(sd) - set(want))
-        if bad or extra or self.out_features <= 0:
-            raise K2Error(f"M-CLIP text encoder: keys missing or of the wrong shape for the config {bad}, unknown keys {extra}")
-        self.sd = sd
-        self._packed = None
-        self._plans = {}
+        want.update({f"layers.{i}.{k}": s for i in range(c["num_hidden_layers"])
+                     for k, s in layer_shapes(H, c["intermediate_size"]).items()})
+        self._take(sd, want)
 
     @classmethod
     def from_state_dict(cls, state_dict, config, tokenizer=None, device="cuda"):
@@ -586,34 +565,25 @@ class MultilingualCLIP:
     def from_pretrained(cls, path, device="cuda"):
         """The reference's `2_1/text_encoder/` folder: config.json, pytorch_model.bin (or model.safetensors) and the
         tokenizer's tokenizer.json (+ special_tokens_map.json / tokenizer_config.json)."""
-        f = os.path.join(path, "config.json")
-        if not os.path.exists(f):
-            raise K2Error(f"M-CLIP text encoder: {f} not found")
-        with open(f, encoding="utf-8") as fh:
-            config = json.load(fh)
+        config = read_json(path, "config.json", cls.what)
         tok = XLMRobertaTokenizer.from_dir(path)
-        return cls.from_state_dict(_load_state_dict(path), config, tokenizer=tok, device=device)
+        sd = load_weights(path, ("pytorch_model.bin", "model.safetensors"), cls.what)
+        return cls.from_state_dict(sd, config, tokenizer=tok, device=device)
 
-    def finalize(self):
-        """Pack the weights on the device once: fp16 GEMM weights [N, K] and tables, fp32 biases / LayerNorm parameters /
-        Linear."""
+    def _pack(self):
+        """fp16 GEMM weights [N, K] and tables, fp32 biases / LayerNorm parameters / Linear."""
         c, dev, sd = self.cfg, self.device, self.sd
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
-        f16 = lambda t: t.detach().to(dev, torch.float16).contiguous()  # noqa: E731
-        self._packed = {"word": f16(sd["word_embedding"]), "pos": f16(sd["position_embedding"]),
-                        "type": f16(sd["token_type_embedding"][0]), "emb_ln": (f32(sd["emb_ln.weight"]), f32(sd["emb_ln.bias"])),
-                        "proj": (f32(sd["proj.weight"]), f32(sd["proj.bias"])),
-                        "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
-        self._plans = {}
-        return self
+        return {"word": f16(sd["word_embedding"], dev), "pos": f16(sd["position_embedding"], dev),
+                "type": f16(sd["token_type_embedding"][0], dev),
+                "emb_ln": (f32(sd["emb_ln.weight"], dev), f32(sd["emb_ln.bias"], dev)),
+                "proj": (f32(sd["proj.weight"], dev), f32(sd["proj.bias"], dev)),
+                "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["num_hidden_layers"], dev)}
 
     def _plan(self, n, T=None):
-        if self._packed is None:
-            self.finalize()
-        key = (n, self.tokens if T is None else T)
-        if key not in self._plans:
-            self._plans[key] = _XLMRPlan(self, *key)
-        return self._plans[key]
+        return super()._plan(n, self.tokens if T is None else T)
+
+    def _new_plan(self, n, T):
+        return _XLMRPlan(self, n, T)
 
     @torch.no_grad()
     def forward(self, input_ids, attention_mask, use_graph=True):
@@ -621,18 +591,10 @@ class MultilingualCLIP:
         [n, T, hidden], pooled fp32 [n, out_features]) on the device: MultilingualCLIP.forward's (embs, LinearTransformation
         of the masked mean).  One CUDA graph replay of the (n, T) launch plan (use_graph=False: the same launches one by
         one).  Ids outside [0, vocab_size) are refused before anything is copied."""
-        c = self.cfg
-        if input_ids.dim() != 2 or not 0 < input_ids.shape[1] <= c["max_tokens"] or input_ids.shape[0] == 0:
-            raise K2Error(f"M-CLIP text encoder: input_ids must be [n, T] with 0 < T <= {c['max_tokens']}, got "
-                          f"{list(input_ids.shape)}")
-        if input_ids.is_floating_point() or input_ids.is_complex() or input_ids.dtype == torch.bool:
-            raise K2Error(f"M-CLIP text encoder: input_ids must be integers, got {input_ids.dtype}")
+        self._check_ids(input_ids, self.cfg["max_tokens"])
         if tuple(attention_mask.shape) != tuple(input_ids.shape) or attention_mask.is_floating_point():
             raise K2Error(f"M-CLIP text encoder: attention_mask must be an integer or bool [n, T] like input_ids, got "
                           f"{attention_mask.dtype} {list(attention_mask.shape)}")
-        lo, hi = int(input_ids.min()), int(input_ids.max())
-        if lo < 0 or hi >= c["vocab_size"]:
-            raise K2Error(f"M-CLIP text encoder: token ids must lie in [0, {c['vocab_size']}), got [{lo}, {hi}]")
         plan = self._plan(*input_ids.shape)
         plan.ids.copy_(input_ids)
         plan.mask.copy_(attention_mask != 0)
@@ -645,12 +607,11 @@ class MultilingualCLIP:
         prompt is tokenized and encoded once and its rows are gathered back."""
         if self.tokenizer is None:
             raise K2Error("M-CLIP text encoder: calling it with a prompt needs tokenizer=")
-        prompts = [prompt] * batch_size + [""] * batch_size
-        distinct = list(dict.fromkeys(prompts))
-        tok = self.tokenizer(distinct, max_length=self.tokens)
-        full, pooled = self.forward(tok["input_ids"], tok["attention_mask"])
-        idx = torch.tensor([distinct.index(p) for p in prompts], device=self.device)
-        return full[idx], pooled[idx]
+
+        def encode(distinct):
+            tok = self.tokenizer(distinct, max_length=self.tokens)
+            return self.forward(tok["input_ids"], tok["attention_mask"])
+        return self._encode_distinct([prompt] * batch_size + [""] * batch_size, encode)
 
 
 class _XLMRPlan(LaunchPlan):
