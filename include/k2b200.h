@@ -452,6 +452,39 @@ int k2_depth_to_space_f16(const void* g, int ldg, int NB, int H, int W, int C, i
 int k2_readout_rows_f16(const void* h, int ldh, int B, int T, int H, void* y, int ldy, k2_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * BiT ResNet backbone of the hybrid DPT (MiDaS v3 DPT-Hybrid, transformers' Intel/dpt-hybrid-midas; kandinsky2/model/depth.py).
+ * Its 1x1 and 3x3 convolutions (weights standardised on the host) are k2_conv_gemm launches with fused GroupNorm partials,
+ * a stride-2 convolution runs at stride 1 followed by k2_subsample2_nhwc; these are the rest.  Every argument is checked
+ * before any CUDA call; nothing outside the output view is written.
+ *
+ * k2_im2col_f16: x fp32 NCHW [NB, C, H, W] (contiguous) -> y fp16 rows [NB Ho Wo, ldy] (ldy >= Kp), the k x k stride-s
+ *   window of output pixel (oy, ox) with pad_top / pad_left zero rows / columns before the image (and zeros after it):
+ *     y[(n Ho + oy) Wo + ox, (c k + ky) k + kx] = fp16_rn(x[n, c, oy s - pad_top + ky, ox s - pad_left + kx])
+ *   columns k^2 C <= j < Kp are 0; columns >= Kp are not touched.  The column order is weight.reshape(Cout, -1)'s, so a
+ *   k2_conv_gemm flat GEMM with that weight (padded to Kp) is the convolution.  Pads in [0, k).
+ * k2_maxpool_f16: x fp16 NHWC [NB, H, W, C] (pixel stride ldx) -> y [NB, Ho, Wo, C] (pixel stride ldy), 3x3 window, stride 2,
+ *   pad_top / pad_left (in [0, 3)) before the image and whatever Ho / Wo implies after it.  The pad value is +0, not -inf
+ *   (BiT's BitMaxPool2d pads with DynamicPad2d(value=0) before max_pool2d).  Scan order ky, kx; a value replaces the running
+ *   maximum when it is greater or NaN (torch's rule), so of equal values the first wins.  C, strides multiples of 8,
+ *   16-byte aligned.
+ * k2_gn_act_f16: y = [relu]( (x - mean) rstd gamma + beta + r ) per image and channel, groups of C / groups channels:
+ *     r = 0                                                            r == NULL
+ *     r = r_src                                                        r_stats == NULL
+ *     r = (r_src - r_mean) r_rstd r_gamma + r_beta                     r_stats != NULL (a second GroupNorm)
+ *   stats / r_stats fp32 [NB, groups, 2] (mean, rstd) as k2_gn_stats and k2_gn_finalize write them; gamma / beta fp32 [C].
+ *   fp32 arithmetic (x a + b with a = gamma rstd, b = beta - mean a), one rounding.  x / r pixel strides ldx / ldr, images
+ *   contiguous; y pixel stride ldy and image stride ldy_img (elements, >= (H W - 1) ldy + C), so y may be the patch rows of a
+ *   wider token buffer.  C, strides multiples of 8, 16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+int k2_im2col_f16(const float* x, int NB, int C, int H, int W, int k, int s, int pad_top, int pad_left, int Ho, int Wo,
+                  void* y, int ldy, int Kp, k2_stream_t stream);
+int k2_maxpool_f16(const void* x, int ldx, int NB, int H, int W, int C, int pad_top, int pad_left, int Ho, int Wo, void* y,
+                   int ldy, k2_stream_t stream);
+int k2_gn_act_f16(const void* x, int ldx, const float* stats, const float* gamma, const float* beta, const void* r, int ldr,
+                  const float* r_stats, const float* r_gamma, const float* r_beta, int NB, int H, int W, int C, int groups,
+                  int relu, void* y, int ldy, long long ldy_img, k2_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LoRA adapter merge (diffusers LoRAAttnAddedKVProcessor weights folded into a packed weight, the arithmetic of diffusers'
  * fuse_lora): once per adapter load, never per step.
  *   out[n, k] = fp16_rn( float(base[n, k]) + scale * sum_j up[n, j] * down[j, k] )   n < rows, k < cols

@@ -87,6 +87,9 @@ SIGNATURES = {
     "k2_bilinear_f16": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _P]),
     "k2_depth_to_space_f16": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
     "k2_readout_rows_f16": (_I, [_P, _I, _I, _I, _I, _P, _I, _P]),
+    "k2_im2col_f16": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _P]),
+    "k2_maxpool_f16": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "k2_gn_act_f16": (_I, [_P, _I, _P, _P, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _I, _LL, _P]),
 }
 
 

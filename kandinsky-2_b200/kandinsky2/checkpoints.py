@@ -591,3 +591,42 @@ def load_weights(folder, candidates, what):
     skipped = load_file is None and any(n.endswith(".safetensors") for n in candidates)
     note = " (safetensors is not installed)" if skipped else ""
     raise K2Error(f"{what}: {' or '.join(os.path.join(folder, n) for n in candidates)} not found{note}")
+
+
+_DPT_HYBRID_TOP = {"cls_token": "dpt.embeddings.cls_token", "position_embedding": "dpt.embeddings.position_embeddings",
+                   "projection.weight": "dpt.embeddings.projection.weight",
+                   "projection.bias": "dpt.embeddings.projection.bias"}
+_BIT_PREFIX = "dpt.embeddings.backbone."
+
+
+def transformers_dpt_hybrid_keys(config):
+    """Every key of a transformers `DPTForDepthEstimation` state dict with the hybrid (BiT) backbone for a config.json dict,
+    including the ones transformers_dpt_hybrid_to_k2 drops."""
+    from .model.depth import _bit_layer_shapes, dpt_hybrid_config, k2_hybrid_shapes
+    c = dpt_hybrid_config(config)
+    keys = _stack_keys([*_DPT_HYBRID_TOP.values(), "dpt.layernorm.weight", "dpt.layernorm.bias"], "dpt.encoder.layer.{}.",
+                       _DPT_LAYER, _DPT_QKV, c["num_hidden_layers"])
+    keys += [_BIT_PREFIX + k for k in _bit_layer_shapes(c["bit"])]
+    keys += [k for k in k2_hybrid_shapes(c) if k.startswith(("neck.", "head."))]
+    return keys + [f"neck.fusion_stage.layers.0.residual_layer1.{conv}.{s}" for conv in ("convolution1", "convolution2")
+                   for s in _WB]
+
+
+def transformers_dpt_hybrid_to_k2(sd, config):
+    """transformers `DPTForDepthEstimation` state dict with the hybrid backbone (MiDaS v3 DPT-Hybrid, Intel/dpt-hybrid-midas)
+    and its config.json dict -> `model.depth.DPTDepthEstimator` names:
+        cls_token [H], position_embedding [T, H], projection.{weight, bias} (the 1x1 token projection of the stage-3 map),
+        bit.* (dpt.embeddings.backbone.bit.*: the BiT stem and stages, weights not yet standardised),
+        layers.{i}.* as transformers_dpt_to_k2 packs them, neck.* (reassemble stages 2 and 3 only) and head.*.
+    Dropped on purpose, as in transformers_dpt_to_k2: dpt.layernorm.* and neck.fusion_stage.layers.0.residual_layer1.*.
+    Unknown and missing keys raise K2Error naming them."""
+    from .model.depth import dpt_hybrid_config
+    _require_keys(sd, transformers_dpt_hybrid_keys(config), "transformers DPT-Hybrid")
+    out = _stack_to_k2(sd, _DPT_HYBRID_TOP, "dpt.encoder.layer.{}.", _DPT_LAYER, _DPT_QKV,
+                       dpt_hybrid_config(config)["num_hidden_layers"], "layers.{}.", "attn.qkv", 64)
+    out["cls_token"] = out["cls_token"].reshape(-1)
+    out["position_embedding"] = out["position_embedding"][0]
+    out.update({k[len(_BIT_PREFIX):]: v for k, v in sd.items() if k.startswith(_BIT_PREFIX)})
+    out.update({k: v for k, v in sd.items() if k.startswith(("neck.", "head."))
+                and not k.startswith("neck.fusion_stage.layers.0.residual_layer1.")})
+    return out

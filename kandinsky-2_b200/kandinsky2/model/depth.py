@@ -30,6 +30,11 @@ pipeline's postprocess (bicubic resize to the image's size, min-max to [0, 255],
 zeros where transformers divides by zero; make_hint restates the hint builder of diffusers' kandinsky-2-2-controlnet-depth
 documentation.
 
+The hybrid (is_hybrid: MiDaS v3 DPT-Hybrid, Intel/dpt-hybrid-midas, the estimator of ControlNet's MidasDetector) replaces the
+patch embedding with a BiT ResNet backbone (_HybridPlan) and takes any input size that is a multiple of 16; midas_hint
+restates the ControlNet notebook's make_hint(img, MidasDetector()).  Parity: tests/test_cpu_dpt_hybrid.py,
+tests/test_gpu_zz_dpt_hybrid.py.
+
 Parity: tests/test_cpu_dpt.py pins the oracle (tests/dpt_oracle.py), preprocess and postprocess to transformers
 (tests/golden/dpt_tiny.pt); tests/test_gpu_zz_depth.py runs the estimator against the golden and, at the Intel/dpt-large
 geometry on synthetic weights, against the fp32 oracle.
@@ -101,6 +106,124 @@ def dpt_config(config):
     c.update(reassemble_factors=factors, backbone_out_indices=idx, neck_hidden_sizes=sizes, head_dim=64,
              layer_norm_eps=float(c["layer_norm_eps"]), kp=(3 * c["patch_size"] ** 2 + 1 + 63) // 64 * 64)
     return c
+
+
+# transformers' BitConfig defaults as DPTConfig fills them in for a hybrid model without a backbone_config
+_BIT_DEFAULTS = dict(num_channels=3, embedding_size=64, hidden_sizes=[256, 512, 1024, 2048], depths=[3, 4, 9],
+                     layer_type="bottleneck", hidden_act="relu", global_padding="same", num_groups=32,
+                     embedding_dynamic_padding=True, output_stride=32, width_factor=1,
+                     out_features=["stage1", "stage2", "stage3"])
+BIT_GN_EPS = 1e-5   # BitGroupNormActivation
+BIT_WS_EPS = 1e-8   # WeightStandardizedConv2d in every BiT layer
+
+
+def _make_div(v, divisor=8):
+    """transformers' modeling_bit.make_div."""
+    n = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return n + divisor if n < 0.9 * v else n
+
+
+def dpt_hybrid_config(config):
+    """The transformers DPTConfig dict of a hybrid DPT (MiDaS v3 DPT-Hybrid: BiT ResNet + ViT, Intel/dpt-hybrid-midas) -> the
+    geometry this module implements; K2Error naming the key for anything else.  The ViT, neck and head follow dpt_config's
+    rules; c["bit"] holds the backbone: stem width, three stages' channels, bottleneck widths and depths."""
+    if not config.get("is_hybrid"):
+        raise K2Error("DPT-Hybrid config: is_hybrid: the config is not a hybrid DPT")
+    plain = {k: v for k, v in config.items() if k not in ("is_hybrid", "backbone_config", "backbone")}
+    c = dpt_config(plain)
+    bc = dict(_BIT_DEFAULTS)
+    bc.update({k: v for k, v in (config.get("backbone_config") or {}).items() if k in _BIT_DEFAULTS})
+
+    def refuse(key, what):
+        raise K2Error(f"DPT-Hybrid config: {key}: {what} is not implemented (only the BiT bottleneck backbone of "
+                      f"Intel/dpt-hybrid-midas)")
+    if config.get("backbone") is not None:
+        refuse("backbone", "a named backbone")
+    mt = (config.get("backbone_config") or {}).get("model_type", "bit")
+    if mt != "bit":
+        refuse("backbone_config.model_type", repr(mt))
+    checks = [("layer_type", bc["layer_type"] == "bottleneck"),
+              ("global_padding", str(bc["global_padding"]).lower() == "same"),
+              ("embedding_dynamic_padding", bc["embedding_dynamic_padding"] is True),
+              ("out_features", list(bc["out_features"]) == ["stage1", "stage2", "stage3"]),
+              ("depths", len(bc["depths"]) == 3 and all(isinstance(d, int) and d > 0 for d in bc["depths"])),
+              ("width_factor", bc["width_factor"] == 1),
+              ("hidden_act", bc["hidden_act"] == "relu"),
+              ("num_groups", bc["num_groups"] == 32),
+              ("output_stride", bc["output_stride"] >= 16),
+              ("num_channels", bc["num_channels"] == 3),
+              ("hidden_sizes", len(bc["hidden_sizes"]) >= 3)]
+    for key, ok in checks:
+        if not ok:
+            refuse(f"backbone_config.{key}", f"{key} {bc[key]!r}")
+    chans = [_make_div(h) for h in bc["hidden_sizes"][:3]]
+    mids = [_make_div(ch * 0.25) for ch in chans]
+    stem = int(bc["embedding_size"])
+    if any(ch % 64 for ch in chans + mids + [stem]):
+        refuse("backbone_config.hidden_sizes", "stage or stem widths that are not multiples of 64")
+    if c["patch_size"] != 16:
+        refuse("patch_size", f"patch_size {c['patch_size']} (the BiT stage-3 map is at 1/16)")
+    if len(c["neck_hidden_sizes"]) != 4:
+        refuse("neck_hidden_sizes", "a neck without four stages")
+    if c["neck_hidden_sizes"][:2] != chans[:2]:
+        refuse("neck_hidden_sizes", f"neck_hidden_sizes[0:2] {c['neck_hidden_sizes'][:2]} other than the BiT stage-1 / "
+               f"stage-2 channels {chans[:2]}")
+    fm = config.get("backbone_featmap_shape", [1, 1024, 24, 24])
+    if fm is None or len(fm) < 2 or fm[1] != chans[2]:
+        refuse("backbone_featmap_shape", f"backbone_featmap_shape {fm} whose channels are not the BiT stage-3 channels "
+               f"{chans[2]}")
+    if list(config.get("neck_ignore_stages", [0, 1])) != [0, 1]:
+        refuse("neck_ignore_stages", f"neck_ignore_stages {config.get('neck_ignore_stages')}")
+    c.update(is_hybrid=True, bit=dict(stem=stem, channels=chans, mids=mids, depths=[int(d) for d in bc["depths"]]),
+             kp=_pad64(chans[2] + 1))
+    return c
+
+
+def _pad64(n):
+    return (n + 63) // 64 * 64
+
+
+def _bit_layer_shapes(b):
+    """{name: shape} of the BiT backbone under this module's names (bit.*, transformers' names below
+    dpt.embeddings.backbone.bit)."""
+    want = {"bit.embedder.convolution.weight": (b["stem"], 3, 7, 7), "bit.embedder.norm.weight": (b["stem"],),
+            "bit.embedder.norm.bias": (b["stem"],)}
+    cin = b["stem"]
+    for s, (ch, mid, depth) in enumerate(zip(b["channels"], b["mids"], b["depths"])):
+        for l in range(depth):
+            lp = f"bit.encoder.stages.{s}.layers.{l}."
+            for conv, shape in (("1", (mid, cin, 1, 1)), ("2", (mid, mid, 3, 3)), ("3", (ch, mid, 1, 1))):
+                want[f"{lp}conv{conv}.weight"] = shape
+                want.update({f"{lp}norm{conv}.{k}": (shape[0],) for k in ("weight", "bias")})
+            if l == 0:
+                want.update({f"{lp}downsample.conv.weight": (ch, cin, 1, 1), f"{lp}downsample.norm.weight": (ch,),
+                             f"{lp}downsample.norm.bias": (ch,)})
+            cin = ch
+    return want
+
+
+def k2_hybrid_shapes(c):
+    """{name: shape} of the state dict a hybrid DPTDepthEstimator takes (checkpoints.transformers_dpt_hybrid_to_k2's output):
+    the plain DPT's ViT, neck stages 2 and 3, neck convolutions, fusion and head, the BiT backbone (bit.*) and the token
+    projection over the stage-3 map (projection.*) in place of the patch embedding."""
+    H = c["hidden_size"]
+    rs = "neck.reassemble_stage."
+    want = {k: s for k, s in k2_shapes(c).items()
+            if not k.startswith(("patch_embedding.", f"{rs}readout_projects.0.", f"{rs}readout_projects.1.",
+                                 f"{rs}layers.0.", f"{rs}layers.1."))}
+    want.update({"projection.weight": (H, c["bit"]["channels"][2], 1, 1), "projection.bias": (H,)})
+    want.update(_bit_layer_shapes(c["bit"]))
+    return want
+
+
+def standardize_weight(w, eps=BIT_WS_EPS):
+    """WeightStandardizedConv2d's weight in float64: per output channel over in * kh * kw, (w - mean) / sqrt(biased var +
+    eps)."""
+    w = w.detach().double()
+    flat = w.reshape(w.shape[0], -1)
+    mean = flat.mean(1, keepdim=True)
+    var = ((flat - mean) ** 2).mean(1, keepdim=True)
+    return ((flat - mean) / torch.sqrt(var + eps)).reshape(w.shape)
 
 
 def k2_shapes(c):
@@ -200,13 +323,84 @@ def make_hint(image, estimator):
     return (torch.from_numpy(d).float() / 255.0).permute(2, 0, 1)
 
 
+def hwc3(x):
+    """ControlNet's annotator.util.HWC3: uint8 [H, W] / [H, W, 1 | 3 | 4] -> uint8 [H, W, 3]; grey is repeated, RGBA is
+    composited over white in float32, clipped and truncated."""
+    if x.dtype != np.uint8:
+        raise K2Error(f"midas_hint: images must be uint8, got {x.dtype}")
+    if x.ndim == 2:
+        x = x[:, :, None]
+    C = x.shape[2]
+    if C == 3:
+        return x
+    if C == 1:
+        return np.concatenate([x, x, x], axis=2)
+    if C == 4:
+        color = x[:, :, 0:3].astype(np.float32)
+        alpha = x[:, :, 3:4].astype(np.float32) / 255.0
+        return (color * alpha + 255.0 * (1.0 - alpha)).clip(0, 255).astype(np.uint8)
+    raise K2Error(f"midas_hint: {C}-channel images are not implemented")
+
+
+def resize_image_size(h, w, resolution):
+    """ControlNet's annotator.util.resize_image target size -> (height, width, k): k = resolution / min(h, w), both sides
+    scaled by k and rounded to multiples of 64."""
+    k = float(resolution) / min(float(h), float(w))
+    return int(np.round(h * k / 64.0)) * 64, int(np.round(w * k / 64.0)) * 64, k
+
+
+def resize_image(img, resolution):
+    """ControlNet's annotator.util.resize_image: cv2.resize to resize_image_size with INTER_LANCZOS4 when enlarging (k > 1),
+    else INTER_AREA.  An image already at its target size is returned as it is (cv2.resize returns such an image unchanged
+    with either flag), and cv2 is imported only when the size changes; a resize without cv2 installed raises K2Error."""
+    H, W, k = resize_image_size(img.shape[0], img.shape[1], resolution)
+    if (H, W) == img.shape[:2]:
+        return img
+    try:
+        import cv2
+    except ImportError as e:
+        raise K2Error(f"midas_hint: resizing {img.shape[1]} x {img.shape[0]} to {W} x {H} needs cv2 (opencv-python), which "
+                      "is not installed") from e
+    return cv2.resize(img, (W, H), interpolation=cv2.INTER_LANCZOS4 if k > 1 else cv2.INTER_AREA)
+
+
+def midas_pixels(img):
+    """MidasDetector's input: uint8 HWC -> fp32 [1, 3, H, W] = float32(u8) / 127.5 - 1 (no resize, no image processor)."""
+    return torch.from_numpy(img.astype(np.float32) / np.float32(127.5) - np.float32(1.0)).permute(2, 0, 1)[None].contiguous()
+
+
+def midas_depth_u8(d):
+    """MidasDetector's depth image: fp32 depth [H, W] (numpy) -> d - min, / max, * 255, clip to [0, 255], uint8 (truncation),
+    in float32.  A constant map gives zeros (MidasDetector divides by zero there)."""
+    d = d.astype(np.float32) - d.min()
+    mx = d.max()
+    d = np.zeros_like(d) if mx == 0 else d / mx
+    return (d * np.float32(255.0)).clip(0, 255).astype(np.uint8)
+
+
+def midas_hint(image, estimator):
+    """The ControlNet notebook's make_hint(img, MidasDetector()), restated from ControlNet's annotator/util.py (HWC3,
+    resize_image) and annotator/midas/__init__.py; this restatement is not pinned to that code by a test:
+        img = resize_image(HWC3(uint8 image), resolution = its width); depth = estimator's predicted depth of
+        float32(img) / 127.5 - 1 at img's size; hint = HWC3(midas_depth_u8(depth)) / 255 -> fp32 [3, H, W] on the CPU.
+    image: a PIL image or a uint8 numpy array (HW, HWC).  estimator: a hybrid DPTDepthEstimator (any input size that is a
+    multiple of 16; resize_image's multiples of 64 always are).  MidasDetector's normal map is not computed (make_hint
+    discards it)."""
+    x = np.array(image)
+    img = resize_image(hwc3(x), x.shape[1])
+    pred = estimator.predicted_depth(midas_pixels(img).to(estimator.device))[0].cpu().numpy()
+    d = hwc3(midas_depth_u8(pred))
+    return torch.from_numpy(d.copy()).float().div(255.0).permute(2, 0, 1)
+
+
 def resize_pos_embed(pos, grid):
-    """DPTViTEmbeddings._resize_pos_embed in fp32 on the host: pos [1 + G0^2, H] -> [1 + grid^2, H], the grid part resized
-    bilinearly (align_corners=False)."""
+    """DPTViTEmbeddings._resize_pos_embed in fp32 on the host: pos [1 + G0^2, H] -> [1 + gh gw, H], the grid part resized
+    bilinearly (align_corners=False) to grid = (gh, gw), or to a square grid x grid for an integer."""
+    gh, gw = (grid, grid) if isinstance(grid, int) else grid
     g0 = int(math.sqrt(pos.shape[0] - 1))
     p = pos[1:].float().reshape(1, g0, g0, -1).permute(0, 3, 1, 2)
-    p = torch.nn.functional.interpolate(p, size=(grid, grid), mode="bilinear")
-    return torch.cat([pos[:1].float(), p.permute(0, 2, 3, 1).reshape(grid * grid, -1)])
+    p = torch.nn.functional.interpolate(p, size=(gh, gw), mode="bilinear")
+    return torch.cat([pos[:1].float(), p.permute(0, 2, 3, 1).reshape(gh * gw, -1)])
 
 
 class DPTDepthEstimator(Tower):
@@ -218,7 +412,8 @@ class DPTDepthEstimator(Tower):
     what = "DPT"
 
     def __init__(self, sd, config, device="cuda", preprocessor_config=None):
-        c = dpt_config(config)
+        self.hybrid = bool(config.get("is_hybrid"))
+        c = dpt_hybrid_config(config) if self.hybrid else dpt_config(config)
         self.cfg, self.device = c, torch.device(device)
         self.proc = preprocessor_settings(preprocessor_config, c["image_size"])
         S = int(self.proc["size"]["height"])
@@ -226,17 +421,19 @@ class DPTDepthEstimator(Tower):
             raise K2Error(f"DPT preprocessing: size {self.proc['size']}: only a square input that is a multiple of the patch "
                           f"size {c['patch_size']} is implemented")
         self.size, self.grid = S, S // c["patch_size"]
-        self._take(sd, k2_shapes(c))
+        self._take(sd, k2_hybrid_shapes(c) if self.hybrid else k2_shapes(c))
 
     @classmethod
     def from_transformers(cls, state_dict, config, preprocessor_config=None, device="cuda"):
-        """From a transformers DPTForDepthEstimation state dict and its config.json dict; packs the weights."""
-        from ..checkpoints import transformers_dpt_to_k2
-        return cls(transformers_dpt_to_k2(state_dict, config), config, device, preprocessor_config).finalize()
+        """From a transformers DPTForDepthEstimation state dict and its config.json dict (plain or hybrid, after
+        `is_hybrid`); packs the weights."""
+        from ..checkpoints import transformers_dpt_hybrid_to_k2, transformers_dpt_to_k2
+        remap = transformers_dpt_hybrid_to_k2 if config.get("is_hybrid") else transformers_dpt_to_k2
+        return cls(remap(state_dict, config), config, device, preprocessor_config).finalize()
 
     @classmethod
     def from_pretrained(cls, path, device="cuda"):
-        """A local transformers model folder (e.g. a download of Intel/dpt-large): config.json, preprocessor_config.json
+        """A local transformers model folder (e.g. a download of Intel/dpt-large or Intel/dpt-hybrid-midas): config.json, preprocessor_config.json
         (optional) and model.safetensors or pytorch_model.bin.  A missing file raises K2Error naming it."""
         what = "DPTDepthEstimator.from_pretrained"
         stem = "pytorch_model" if os.path.exists(os.path.join(path, "pytorch_model.bin")) else "model"
@@ -250,22 +447,16 @@ class DPTDepthEstimator(Tower):
         c, dev, sd = self.cfg, self.device, self.sd
         F = c["fusion_hidden_size"]
         w = lambda name: ops.pack_conv_weight(sd[name].detach().to(dev))  # noqa: E731
-        pos = resize_pos_embed(sd["position_embedding"].detach().cpu(), self.grid)
-        pos[1:] += sd["patch_embedding.bias"].detach().cpu().float()   # the patch conv's bias, on the patch rows only
-        pk = {"embed": pack_patch_embed(sd["patch_embedding.weight"], sd["cls_token"], c["kp"], dev),
-              "pos": pos.to(dev).half().contiguous(),
-              "layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["backbone_out_indices"][-1] + 1, dev)}
+        pk = {"layers": pack_layers(lambda i, name: sd[f"layers.{i}.{name}"], c["backbone_out_indices"][-1] + 1, dev)}
+        if self.hybrid:
+            pk.update(self._pack_bit())
+        else:
+            pos = resize_pos_embed(sd["position_embedding"].detach().cpu(), self.grid)
+            pos[1:] += sd["patch_embedding.bias"].detach().cpu().float()   # the patch conv's bias, on the patch rows only
+            pk.update(embed=pack_patch_embed(sd["patch_embedding.weight"], sd["cls_token"], c["kp"], dev),
+                      pos=pos.to(dev).half().contiguous())
         rs = "neck.reassemble_stage."
         for i, (C, f) in enumerate(zip(c["neck_hidden_sizes"], c["reassemble_factors"])):
-            pk[f"readout.{i}"] = (w(f"{rs}readout_projects.{i}.0.weight"), f32(sd[f"{rs}readout_projects.{i}.0.bias"], dev))
-            pk[f"proj.{i}"] = (w(f"{rs}layers.{i}.projection.weight"), f32(sd[f"{rs}layers.{i}.projection.bias"], dev))
-            rw, rb = sd.get(f"{rs}layers.{i}.resize.weight"), sd.get(f"{rs}layers.{i}.resize.bias")
-            if f > 1:   # ConvTranspose2d weight [in, out, a, b] -> GEMM rows (a s + b) C + out over K = in
-                s = int(f)
-                g = rw.detach().to(dev).permute(2, 3, 1, 0).reshape(s * s * C, C)
-                pk[f"resize.{i}"] = (ops.pack_conv_weight(g), f32(rb, dev).repeat(s * s))
-            elif f < 1:
-                pk[f"resize.{i}"] = (ops.pack_conv_weight(rw.detach().to(dev)), f32(rb, dev))
             pk[f"neck_conv.{i}"] = w(f"neck.convs.{i}.weight")
             fp = f"neck.fusion_stage.layers.{i}."
             pk[f"fusion_proj.{i}"] = (w(fp + "projection.weight"), f32(sd[fp + "projection.bias"], dev))
@@ -278,13 +469,54 @@ class DPTDepthEstimator(Tower):
                     c2 = torch.cat([c2, eye], 1).contiguous()
                 pk[f"unit{u}.{i}"] = ((w(p + "convolution1.weight"), f32(sd[p + "convolution1.bias"], dev)),
                                       (c2, f32(sd[p + "convolution2.bias"], dev)))
+            if self.hybrid and i < 2:   # the BiT stage maps go straight into neck.convs.0 / 1
+                continue
+            pk[f"readout.{i}"] = (w(f"{rs}readout_projects.{i}.0.weight"), f32(sd[f"{rs}readout_projects.{i}.0.bias"], dev))
+            pk[f"proj.{i}"] = (w(f"{rs}layers.{i}.projection.weight"), f32(sd[f"{rs}layers.{i}.projection.bias"], dev))
+            rw, rb = sd.get(f"{rs}layers.{i}.resize.weight"), sd.get(f"{rs}layers.{i}.resize.bias")
+            if f > 1:   # ConvTranspose2d weight [in, out, a, b] -> GEMM rows (a s + b) C + out over K = in
+                s = int(f)
+                g = rw.detach().to(dev).permute(2, 3, 1, 0).reshape(s * s * C, C)
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(g), f32(rb, dev).repeat(s * s))
+            elif f < 1:
+                pk[f"resize.{i}"] = (ops.pack_conv_weight(rw.detach().to(dev)), f32(rb, dev))
         pk["head"] = [(w("head.head.0.weight"), f32(sd["head.head.0.bias"], dev)),
                       (w("head.head.2.weight"), f32(sd["head.head.2.bias"], dev)),
                       (ops.pad_rows(w("head.head.4.weight"), 16), f32(sd["head.head.4.bias"], dev))]
         return pk
 
-    def _new_plan(self, B):
-        return _DepthPlan(self, B)
+    def _pack_bit(self):
+        """The hybrid's backbone: each BiT convolution's weight standardised in float64 and rounded once (the stem's
+        [64, 3 * 49] padded to 192 columns for k2_im2col_f16's rows), GroupNorm gamma / beta fp32; the token projection as one
+        GEMM weight [H, kp]: the 1x1 projection in columns [0, C3), the CLS token in column C3 (the token rows hold a 1
+        there on the CLS row); the position embedding stays on the host (fp32, projection bias on the patch rows) and is
+        resized per input size by the plan."""
+        c, dev, sd = self.cfg, self.device, self.sd
+        b, H = c["bit"], c["hidden_size"]
+        ws = lambda name: ops.pack_conv_weight(standardize_weight(sd[name]).to(dev))  # noqa: E731
+        gn = lambda name: (f32(sd[name + ".weight"], dev), f32(sd[name + ".bias"], dev))  # noqa: E731
+        stem = standardize_weight(sd["bit.embedder.convolution.weight"]).reshape(b["stem"], -1)
+        pk = {"stem": (ops.pack_conv_weight(stem.to(dev)), *gn("bit.embedder.norm")), "stages": []}
+        for s, depth in enumerate(b["depths"]):
+            blocks = []
+            for l in range(depth):
+                lp = f"bit.encoder.stages.{s}.layers.{l}."
+                blk = {f"conv{k}": (ws(f"{lp}conv{k}.weight"), *gn(f"{lp}norm{k}")) for k in (1, 2, 3)}
+                if l == 0:
+                    blk["down"] = (ws(f"{lp}downsample.conv.weight"), *gn(f"{lp}downsample.norm"))
+                blocks.append(blk)
+            pk["stages"].append(blocks)
+        C3 = b["channels"][2]
+        we = torch.zeros(H, c["kp"], dtype=torch.float16, device=dev)
+        we[:, :C3] = sd["projection.weight"].detach().to(dev).reshape(H, C3).half()
+        we[:, C3] = sd["cls_token"].detach().to(dev).half()
+        pk["embed"] = we
+        pk["pos_host"] = sd["position_embedding"].detach().cpu().float()
+        pk["proj_bias_host"] = sd["projection.bias"].detach().cpu().float()
+        return pk
+
+    def _new_plan(self, B, h=None, w=None):
+        return _HybridPlan(self, B, h, w) if self.hybrid else _DepthPlan(self, B)
 
     def attend(self, qkv, out):
         """The layers' attention: k2_attention_d64 over the tokens (per-head [q | k | v], scale 1/8)."""
@@ -297,12 +529,21 @@ class DPTDepthEstimator(Tower):
     @torch.no_grad()
     def predicted_depth(self, pixel_values, use_graph=True):
         """pixel_values fp32 [B, 3, S, S] -> DPTForDepthEstimation's predicted_depth, fp32 [B, S', S'] on the device (S' = S for
-        an even patch grid).  One CUDA graph replay of the batch size's launch plan (use_graph=False: the same launches one
+        an even patch grid).  The hybrid takes any [B, 3, H, W] with H and W multiples of 16 (one plan per (B, H, W)).  One CUDA graph replay of the batch size's launch plan (use_graph=False: the same launches one
         by one)."""
         S = self.size
-        if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
+        if self.hybrid:
+            shp = tuple(pixel_values.shape)
+            if pixel_values.dim() != 4 or shp[1] != 3 or shp[2] % 16 or shp[3] % 16 or min(shp[2:]) <= 0:
+                raise K2Error(f"DPT-Hybrid: pixel_values must be [B, 3, H, W] with H and W multiples of 16, got {list(shp)}")
+            if (shp[2] // 16) % 2 != (shp[3] // 16) % 2:
+                raise K2Error(f"DPT-Hybrid: pixel_values {list(shp)}: patch grids with one odd and one even side are not "
+                              "implemented")
+            plan = self._plan(shp[0], shp[2], shp[3])
+        elif pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, S, S):
             raise K2Error(f"DPT: pixel_values must be [B, 3, {S}, {S}], got {list(pixel_values.shape)}")
-        plan = self._plan(pixel_values.shape[0])
+        else:
+            plan = self._plan(pixel_values.shape[0])
         plan.pix.copy_(pixel_values)
         plan.run(use_graph)
         return plan.out.clone()
@@ -356,9 +597,9 @@ class _DepthPlan(LaunchPlan):
         return self._conv3(a, (w2, b2), F, residual=x, extra=extra)
 
     def _build(self):
-        e, pk, B, A = self.e, self.e._packed, self.B, self._add
+        e, pk, B = self.e, self.e._packed, self.B
         c = e.cfg
-        G, H, P, F = e.grid, c["hidden_size"], c["patch_size"], c["fusion_hidden_size"]
+        G, H, P = e.grid, c["hidden_size"], c["patch_size"]
         T, heads, eps = G * G + 1, c["num_attention_heads"], c["layer_norm_eps"]
         h = record_patch_embed(self, self.pix, pk["embed"], self.pos, P, c["kp"])
         hidden, start = [], 0
@@ -366,28 +607,38 @@ class _DepthPlan(LaunchPlan):
             h = record_layers(self, h, pk["layers"][start:idx + 1], e.attend, 4 * B * heads * T * T * 64, eps)
             hidden.append(h)
             start = idx + 1
-        feats, M = [], B * G * G
-        for i, (hs, C, f) in enumerate(zip(hidden, c["neck_hidden_sizes"], c["reassemble_factors"])):
-            ro, r, p = self._new(B, G, G, 2 * H), self._new(B, G, G, H), self._new(B, G, G, C)
-            A(lambda hs=hs, ro=ro: ops.readout_rows_f16(hs, out=ro.view(B, G * G, 2 * H)), "readout")
-            self._gemm(ro, pk[f"readout.{i}"][0], H, r, 2 * M * 2 * H * H, bias=pk[f"readout.{i}"][1])
-            A(lambda r=r: ops.gelu_f16_(r), "gelu")
-            self._gemm(r, pk[f"proj.{i}"][0], C, p, 2 * M * H * C, bias=pk[f"proj.{i}"][1])
-            if f > 1:
-                s = int(f)
-                g, y = self._new(B, G, G, s * s * C), self._new(B, s * G, s * G, C)
-                self._gemm(p, pk[f"resize.{i}"][0], s * s * C, g, 2 * M * C * s * s * C, bias=pk[f"resize.{i}"][1])
-                A(lambda g=g, y=y, s=s, C=C: ops.depth_to_space_f16(g, s, C, out=y), "depth_to_space")
-            elif f < 1:
-                full, Go = self._conv3(p, pk[f"resize.{i}"], C), (G + 1) // 2
-                if G % 2 == 0:
-                    y = self._new(B, Go, Go, C)
-                    A(lambda full=full, y=y: ops.subsample2(full, 0, 0, out=y), "subsample")
-                else:   # align_corners from G to (G + 1) / 2 samples: source index 2i exactly, weights 1 and 0
-                    y = self._bilinear(full, (Go, Go), True)
-            else:
-                y = p
-            feats.append(self._conv3(y, pk[f"neck_conv.{i}"], F))
+        self._fuse_head([self._reassemble(i, hs, (G, G)) for i, hs in enumerate(hidden)])
+
+    def _reassemble(self, i, hs, grid):
+        """Neck stage i of the hidden state hs [B, 1 + gh gw, H]: readout, projection, resize, then neck.convs.i."""
+        e, pk, B, A = self.e, self.e._packed, self.B, self._add
+        c = e.cfg
+        (gh, gw), H, F = grid, c["hidden_size"], c["fusion_hidden_size"]
+        C, f, M = c["neck_hidden_sizes"][i], c["reassemble_factors"][i], B * gh * gw
+        ro, r, p = self._new(B, gh, gw, 2 * H), self._new(B, gh, gw, H), self._new(B, gh, gw, C)
+        A(lambda: ops.readout_rows_f16(hs, out=ro.view(B, gh * gw, 2 * H)), "readout")
+        self._gemm(ro, pk[f"readout.{i}"][0], H, r, 2 * M * 2 * H * H, bias=pk[f"readout.{i}"][1])
+        A(lambda: ops.gelu_f16_(r), "gelu")
+        self._gemm(r, pk[f"proj.{i}"][0], C, p, 2 * M * H * C, bias=pk[f"proj.{i}"][1])
+        if f > 1:
+            s = int(f)
+            g, y = self._new(B, gh, gw, s * s * C), self._new(B, s * gh, s * gw, C)
+            self._gemm(p, pk[f"resize.{i}"][0], s * s * C, g, 2 * M * C * s * s * C, bias=pk[f"resize.{i}"][1])
+            A(lambda: ops.depth_to_space_f16(g, s, C, out=y), "depth_to_space")
+        elif f < 1:
+            full, Go = self._conv3(p, pk[f"resize.{i}"], C), ((gh + 1) // 2, (gw + 1) // 2)
+            if gh % 2 == 0 and gw % 2 == 0:
+                y = self._new(B, *Go, C)
+                A(lambda: ops.subsample2(full, 0, 0, out=y), "subsample")
+            else:   # align_corners from G to (G + 1) / 2 samples: source index 2i exactly, weights 1 and 0
+                y = self._bilinear(full, Go, True)
+        else:
+            y = p
+        return self._conv3(y, pk[f"neck_conv.{i}"], F)
+
+    def _fuse_head(self, feats):
+        """The fusion stage over the neck maps feats (shallow to deep), then the head -> self.out fp32 [B, S'h, S'w]."""
+        pk, B, A, F = self.e._packed, self.B, self._add, self.e.cfg["fusion_hidden_size"]
         run = None
         for j, fe in enumerate(reversed(feats)):   # fusion layer j (its packed weights' key) takes the stage from the deep end
             if run is None:
@@ -406,8 +657,105 @@ class _DepthPlan(LaunchPlan):
         a = self._bilinear(a, (2 * a.shape[1], 2 * a.shape[2]), True)
         a = self._conv3(a, (w2, b2), 32)
         A(lambda: ops.relu_f16(a), "relu")
-        So = a.shape[1]
-        out = torch.empty(B, 1, So, So, device=self.dev, dtype=torch.float32)
-        self._conv([(a, 1)], w4, 1, out, 2 * B * So * So * 32, bias=b4, want_stats=False, out_mode=1, kind="conv")
+        Sh, Sw = a.shape[1:3]
+        out = torch.empty(B, 1, Sh, Sw, device=self.dev, dtype=torch.float32)
+        self._conv([(a, 1)], w4, 1, out, 2 * B * Sh * Sw * 32, bias=b4, want_stats=False, out_mode=1, kind="conv")
         A(lambda: ops.relu_f32(out), "relu")
-        self.out = out.view(B, So, So)
+        self.out = out.view(B, Sh, Sw)
+
+
+class _HybridPlan(_DepthPlan):
+    """The hybrid estimator at B images of h x w (multiples of 16) as one static launch list; the neck stages 2 / 3, fusion
+    and head are _DepthPlan's.  The BiT backbone:
+        stem      k2_im2col_f16 (7x7 stride 2, TF-SAME: 2 before, 3 after on an even side) -> ONE k2_conv_gemm over the
+                  [B, h/2, w/2, 192] rows with fused GroupNorm partials -> k2_gn_act_f16 (GN + ReLU) -> k2_maxpool_f16
+                  (3x3 stride 2, pads 0 before, 1 after, pad value 0);
+        stages    bottlenecks: 1x1 conv -> GN + ReLU -> 3x3 conv -> GN + ReLU -> 1x1 conv -> k2_gn_act_f16(GN + shortcut,
+                  ReLU), the shortcut the input or, in a stage's first block, GN(1x1 conv(input)) normalised inside the same
+                  launch.  Stride 2 (the first block of stages 2 and 3): the 3x3 convolution at stride 1, pad 1, then
+                  k2_subsample2_nhwc(1, 1) (TF-SAME pads 0 before, 1 after on an even side); the 1x1 downsample
+                  subsamples (0, 0) first.  GroupNorm statistics come from the convolutions' fused partials
+                  (k2_gn_finalize) or a k2_gn_stats pass, as LaunchPlan._stats picks.
+    The last stage-3 block writes straight into the token rows [B, 1 + gh gw, kp] (CLS row: a 1 in column C3), and ONE GEMM
+    with the [projection | CLS] weight and the resized position embedding (+ projection bias on the patch rows) as its
+    residual gives the tokens; then the ViT layers in segments ending at backbone_out_indices[2] and [3]."""
+
+    def __init__(self, est, B, h, w):
+        LaunchPlan.__init__(self, est.device, B)
+        self.e, self.B, self.h, self.w = est, B, h, w
+        self.pix = torch.zeros(B, 3, h, w, device=self.dev, dtype=torch.float32)
+        pk, gh, gw = est._packed, h // 16, w // 16
+        pos = resize_pos_embed(pk["pos_host"], (gh, gw))
+        pos[1:] += pk["proj_bias_host"]
+        self.pos = pos.to(self.dev).half().expand(B, *pos.shape).contiguous()
+        self._build()
+
+    def _conv1(self, x, wb, cout):
+        out = self._new(*x.shape[:3], cout)
+        self._conv([(x, 1)], wb[0], cout, out, 2 * x.shape[0] * x.shape[1] * x.shape[2] * x.shape[-1] * cout)
+        return out
+
+    def _gn_act(self, x, wb, relu=True, r=None, r_norm=None, out=None):
+        st = self._stats(x, None, BIT_GN_EPS)
+        y = self._new(*x.shape) if out is None else out
+        self._add(lambda: ops.gn_act_f16(x, st, wb[1], wb[2], r=r, r_norm=r_norm, relu=relu, out=y), "gn_act")
+        return y
+
+    def _bottleneck(self, x, blk, stride2, out=None):
+        mid, cout = blk["conv1"][0].shape[0], blk["conv3"][0].shape[0]
+        r, r_norm = x, None
+        if "down" in blk:
+            xs = x
+            if stride2:
+                xs = self._new(x.shape[0], x.shape[1] // 2, x.shape[2] // 2, x.shape[3])
+                self._add(lambda: ops.subsample2(x, 0, 0, out=xs), "subsample")
+            r = self._conv1(xs, blk["down"], cout)
+            r_norm = (self._stats(r, None, BIT_GN_EPS), blk["down"][1], blk["down"][2])
+        a = self._gn_act(self._conv1(x, blk["conv1"], mid), blk["conv1"])
+        B, Hs, Ws, _ = a.shape
+        c2 = self._new(B, Hs, Ws, mid)
+        self._conv([(a, 9)], blk["conv2"][0], mid, c2, 2 * B * Hs * Ws * 9 * mid * mid, want_stats=not stride2,
+                   kind="conv_stride2_at_1" if stride2 else "conv_gemm")
+        if stride2:
+            full, c2 = c2, self._new(B, Hs // 2, Ws // 2, mid)
+            self._add(lambda: ops.subsample2(full, 1, 1, out=c2), "subsample")
+        a = self._gn_act(c2, blk["conv2"])
+        return self._gn_act(self._conv1(a, blk["conv3"], cout), blk["conv3"], r=r, r_norm=r_norm, out=out)
+
+    def _build(self):
+        e, pk, B, A = self.e, self.e._packed, self.B, self._add
+        c = e.cfg
+        b, H, h, w = c["bit"], c["hidden_size"], self.h, self.w
+        gh, gw = h // 16, w // 16
+        T, heads, eps = gh * gw + 1, c["num_attention_heads"], c["layer_norm_eps"]
+        kst = pk["stem"][0].shape[1]
+        rows = self._new(B, h // 2, w // 2, kst)
+        A(lambda: ops.im2col_f16(self.pix, 7, 2, (2, 2), (h // 2, w // 2), kst, out=rows), "im2col")
+        s0 = self._new(B, h // 2, w // 2, b["stem"])
+        self._conv([(rows, 1)], pk["stem"][0], b["stem"], s0, 2 * B * (h // 2) * (w // 2) * 147 * b["stem"], kind="conv")
+        a0 = self._gn_act(s0, pk["stem"])
+        pooled = self._new(B, h // 4, w // 4, b["stem"])
+        A(lambda: ops.maxpool_f16(a0, (0, 0), (h // 4, w // 4), out=pooled), "maxpool")
+        # the token rows: the CLS row holds a 1 in column C3, the patch rows' columns >= C3 stay 0; set once here
+        C3 = b["channels"][2]
+        self.tok_rows = self._new(B, T, c["kp"])
+        self.tok_rows.zero_()
+        self.tok_rows[:, 0, C3] = 1
+        patch_view = self.tok_rows.as_strided((B, gh, gw, C3), (T * c["kp"], gw * c["kp"], c["kp"], 1), c["kp"])
+        maps, x = [], pooled
+        for s, blocks in enumerate(pk["stages"]):
+            for l, blk in enumerate(blocks):
+                last = s == 2 and l == len(blocks) - 1
+                x = self._bottleneck(x, blk, stride2=(s > 0 and l == 0), out=patch_view if last else None)
+            maps.append(x)
+        self.bit_maps = maps
+        emb = self._new(B, T, H)
+        self._gemm(self.tok_rows, pk["embed"], H, emb, 2 * B * T * c["kp"] * H, residual=self.pos)
+        idx = c["backbone_out_indices"]
+        h1 = record_layers(self, emb, pk["layers"][:idx[2] + 1], e.attend, 4 * B * heads * T * T * 64, eps)
+        h2 = record_layers(self, h1, pk["layers"][idx[2] + 1:idx[3] + 1], e.attend, 4 * B * heads * T * T * 64, eps)
+        self.vit_hidden = (h1, h2)
+        F = c["fusion_hidden_size"]
+        feats = [self._conv3(maps[0], pk["neck_conv.0"], F), self._conv3(maps[1], pk["neck_conv.1"], F),
+                 self._reassemble(2, h1, (gh, gw)), self._reassemble(3, h2, (gh, gw))]
+        self._fuse_head(feats)

@@ -845,3 +845,56 @@ def readout_rows_f16(h, out=None):
     assert h.dtype == out.dtype == torch.float16 and tuple(out.shape) == (B, T - 1, 2 * H), (h.dtype, tuple(out.shape))
     check(nat.load().k2_readout_rows_f16(ptr(h), _row_stride(h), B, T, H, ptr(out), _row_stride(out), stream_ptr()))
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# BiT backbone of the hybrid DPT (kandinsky2/model/depth.py, see k2b200.h)
+# ------------------------------------------------------------------------------------------------
+def im2col_f16(x, k, s, pad, size, kp, out=None):
+    """k2_im2col_f16: fp32 NCHW x [NB, C, H, W] -> fp16 rows [NB, Ho, Wo, kp] (out may be row-strided): the k x k stride-s
+    windows with pad = (top, left) zero padding, columns in (c, ky, kx) order, zeros from k^2 C to kp.  size = (Ho, Wo)."""
+    NB, C, H, W = x.shape
+    Ho, Wo = size
+    if out is None:
+        out = torch.empty((NB, Ho, Wo, kp), dtype=torch.float16, device=x.device)
+    _on_device("im2col_f16", x, out)
+    assert x.dtype == torch.float32 and x.is_contiguous(), (x.dtype, x.stride())
+    assert out.dtype == torch.float16 and tuple(out.shape) == (NB, Ho, Wo, kp), (out.dtype, tuple(out.shape))
+    check(nat.load().k2_im2col_f16(ptr(x), NB, C, H, W, k, s, pad[0], pad[1], Ho, Wo, ptr(out), _row_stride(out), kp,
+                                   stream_ptr()))
+    return out
+
+
+def maxpool_f16(x, pad, size, out=None):
+    """k2_maxpool_f16: fp16 NHWC [NB, H, W, C] (row-strided) -> [NB, Ho, Wo, C], 3x3 stride 2, pad = (top, left), pad value 0
+    (BitMaxPool2d's).  size = (Ho, Wo)."""
+    NB, H, W, C = x.shape
+    Ho, Wo = size
+    if out is None:
+        out = torch.empty((NB, Ho, Wo, C), dtype=torch.float16, device=x.device)
+    _on_device("maxpool_f16", x, out)
+    assert x.dtype == out.dtype == torch.float16 and tuple(out.shape) == (NB, Ho, Wo, C), (x.dtype, tuple(out.shape))
+    check(nat.load().k2_maxpool_f16(ptr(x), _row_stride(x), NB, H, W, C, pad[0], pad[1], Ho, Wo, ptr(out), _row_stride(out),
+                                    stream_ptr()))
+    return out
+
+
+def gn_act_f16(x, stats, gamma, beta, r=None, r_norm=None, relu=True, groups=32, out=None):
+    """k2_gn_act_f16: fp16 NHWC x [NB, H, W, C] (row-strided) -> [relu](GroupNorm(x) + r) fp16, stats fp32 [NB, groups, 2].
+    r: None, an fp16 source of x's shape, or with r_norm = (r_stats, r_gamma, r_beta) a second GroupNorm's input.  out may be
+    any [NB, H, W, C] view whose pixels are row-strided within an image (its image stride is read from out.stride(0))."""
+    NB, H, W, C = x.shape
+    if out is None:
+        out = torch.empty_like(x, memory_format=torch.contiguous_format)
+    rs, rg, rb = r_norm if r_norm is not None else (None, None, None)
+    _on_device("gn_act_f16", x, out, r, stats, gamma, beta, rs, rg, rb)
+    assert x.dtype == out.dtype == torch.float16 and tuple(out.shape) == (NB, H, W, C), (x.dtype, tuple(out.shape))
+    assert r is None or (r.dtype == torch.float16 and tuple(r.shape) == tuple(x.shape)), tuple(r.shape)
+    assert out.stride(-1) == 1 and out.stride(1) == W * out.stride(2), (tuple(out.shape), out.stride())
+    for t in (stats, gamma, beta, rs, rg, rb):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous()), (t.dtype, t.stride())
+    check(nat.load().k2_gn_act_f16(ptr(x), _row_stride(x), ptr(stats), ptr(gamma), ptr(beta), ptr(r),
+                                   _row_stride(r) if r is not None else 0, ptr(rs), ptr(rg), ptr(rb), NB, H, W, C, groups,
+                                   int(bool(relu)), ptr(out), out.stride(2), out.stride(0) if NB > 1 else H * W * out.stride(2),
+                                   stream_ptr()))
+    return out
