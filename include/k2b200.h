@@ -38,9 +38,9 @@ void k2_reset_launch_count(void);
 /* Tuning knobs: key 0 = force conv/GEMM N tile (0 = auto); key 1 = split-K (0 auto, 1 off, n>1 forced);
  * key 2 = CTA-pair conv kernel (0 auto, 1 off; 2 = on is refused: sm_90 has no CTA-pair MMA);
  * key 4 = programmatic dependent launch (0/1); key 9 = accepted for compatibility and ignored (it chose between two CTA
- * layouts of an earlier head-width-64 attention kernel; the current one has one); key 10 = default number of epilogue warp sets of the conv kernel (1 = the first
- * consumer warpgroup; 2 = both consumer warpgroups, each draining half of the 64-column pairs, for N tiles 128 and 256 -- N tile
- * 192 runs with one set: bit-identical results, faster where the K loop is short).  Keys 0, 1, 2 and 10 are process-wide defaults; k2_conv_gemm_cfg overrides them per call.
+ * layouts of an earlier head-width-64 attention kernel; the current one has one); key 10 = accepted for compatibility and
+ * ignored (it chose how many consumer warpgroups drained the conv kernel's accumulators; every consumer warp now drains its
+ * own rows).  Keys 0, 1 and 2 are process-wide defaults; k2_conv_gemm_cfg overrides them per call.
  * key 11 = blocks per SM the GroupNorm apply grids are sized for (0 = each kernel's real occupancy, i.e. one full wave). */
 int k2_set_tuning(int key, int value);
 
@@ -92,8 +92,9 @@ int k2_conv_gemm(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const vo
 
 /* k2_conv_gemm with the launch configuration chosen by the caller instead of the library's cycle model:
  * cfg (HOST pointer, may be NULL = k2_conv_gemm) = int[4] {N tile (16/64/128/192/256), CTA-pair kernel (1 off; 2 is refused
- * on sm_90), split-K factor (1 = off), epilogue warp sets (1 or 2)}; a 0 entry keeps the automatic choice.
- * N tile and epilogue sets never change a result bit (same K order per output element); the split factor does.
+ * on sm_90), split-K factor (1 = off), epilogue warp sets}; a 0 entry keeps the automatic choice.  The epilogue-sets
+ * entry is checked (0, 1 or 2) and otherwise ignored: both consumer warpgroups always drain their own accumulator rows, so
+ * 1 and 2 run the same kernel.  The N tile never changes a result bit (same K order per output element); the split factor does.
  * The UNet / MoVQ launch plans time the candidates once per distinct layer shape and bake the winner into their CUDA graph.
  * w_batch_stride (elements, multiple of 8; 0 = one weight matrix): > 0 makes the call a BATCHED GEMM -- image n of the NB
  * images multiplies Wp + n * w_batch_stride.  This is how the MoVQ AttnBlock (movq_modules.py:201-225) runs without a loop

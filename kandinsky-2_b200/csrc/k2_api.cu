@@ -28,7 +28,6 @@ int fail(const std::string& msg) {
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 bool pdl_enabled() { return g_pdl != 0; }
-static int g_conv_epi_sets = 1;
 static int g_gn_bps = 0;
 int gn_apply_blocks_per_sm() { return g_gn_bps; }
 
@@ -142,18 +141,16 @@ struct ConvPlan {
   int m_tiles_phase;  // up2: tile slots per output phase
   int BN, splits;
   int fuse_stats, row_groups;
-  int es;  // epilogue warp sets (1 or 2)
 };
 
 // cfg (may be null): per-call overrides {N tile, CTA-pair mode (0 / 1 = single CTA, the only kernel on sm_90), split-K factor,
-// epilogue warp sets}; 0 = the process-wide tuning knob, else automatic.  The caller's launch plan bakes its choice per launch (kandinsky2/model/unet.py).
+// epilogue warp sets (ignored: every consumer warp drains its own rows)}; 0 = the process-wide tuning knob, else automatic.  The caller's launch plan bakes its choice per launch (kandinsky2/model/unet.py).
 static void plan_conv(int NB, int H, int W, bool any9, int kchunks, int Cout, int out_mode, bool has_workspace,
                       long long workspace_bytes, bool want_gn, ConvPlan& pl, const int* cfg = nullptr, bool up2 = false,
                       bool w_batched = false) {
   // up2: NB/H/W are the SOURCE geometry; every box is visited once per output phase (4x the tiles, same K loop)
   const int g_force_bn = (cfg && cfg[0]) ? cfg[0] : k2::g_force_bn;
   const int g_force_split = (cfg && cfg[2]) ? cfg[2] : k2::g_force_split;
-  pl.es = (cfg && cfg[3]) ? cfg[3] : k2::g_conv_epi_sets;
   choose_tile(NB, H, W, pl.TN, pl.TH, pl.TW, w_batched);
   pl.tiles_w = (W + pl.TW - 1) / pl.TW;
   pl.tiles_h = (H + pl.TH - 1) / pl.TH;
@@ -268,8 +265,7 @@ int k2_set_tuning(int key, int value) {
     g_pdl = value;
     return 0;
   }
-  if (key == 10) {  // epilogue warp sets of the conv kernel: 1 (consumer warpgroup 0) or 2 (both consumer warpgroups)
-    g_conv_epi_sets = (value == 2) ? 2 : 1;
+  if (key == 10) {  // accepted and ignored: both consumer warpgroups of the conv kernel always drain their own rows
     return 0;
   }
   if (key == 11) {  // GroupNorm apply: blocks per SM the grid is sized for (0 = the kernel's occupancy; round 1 used 4)
@@ -398,7 +394,7 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
     if (residual)
       K2_REQUIRE(ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0, "conv_gemm: residual alignment");
   }
-  int rc = launch_conv_gemm(p, BN, pl.es, static_cast<cudaStream_t>(stream));
+  int rc = launch_conv_gemm(p, BN, static_cast<cudaStream_t>(stream));
   if (rc == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   if (rc == 0 && splits > 1) {
     rc = launch_splitk_finalize(p.ws, splits, p.M_total, Cout, bias, p.residual, ldr, reinterpret_cast<__half*>(out), ldo,

@@ -296,6 +296,13 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t sad
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
                : "r"(saddr));
 }
+// inverse of ldmatrix_x4: lane l's r[m] (a b16 pair) goes to row l / 4, elements 2 (l & 3) + {0, 1} of matrix m, whose eight
+// row addresses lanes 8 m .. 8 m + 7 give
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
 // 16-byte global -> shared copy (L2 only); src_bytes < 16 zero-fills the rest
 __device__ __forceinline__ void cp_async_16(uint32_t saddr, const void* gptr, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(gptr), "r"(src_bytes) : "memory");
@@ -308,6 +315,9 @@ __device__ __forceinline__ void cp_async_wait() {
 
 __device__ __forceinline__ void sts_v4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void sts_v2(uint32_t saddr, uint32_t a, uint32_t b) {
+  asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(saddr), "r"(a), "r"(b) : "memory");
 }
 __device__ __forceinline__ uint4 lds_v4(uint32_t saddr) {
   uint4 v;

@@ -18,10 +18,10 @@
 //     [0, 64) and [64, 128) of the M tile: ONE m64nBNk16 per 16-element K step covers the whole N tile (BN = 16 ... 256), so
 //     each warpgroup reads its A slice from shared memory once per K step, not once per 64 columns.  Both operands are K-major
 //     in the 128 B-swizzled TMA tiles.  Persistent over tiles, smem ring of STAGES (A 16 KB + B BN*128 B).
-//   * Epilogue: the consumers park their register accumulators, BNC columns at a time, in a shared-memory tile with one fp32
-//     row per output pixel; the epilogue warps then read it one ROW per thread (warp ew of a set owns rows [32 ew, 32 ew + 32))
-//     -> + bias (+ residual) -> fp16 rows, fp32 split-K partials or fp32 NCHW, plus the fused GroupNorm partial statistics.
-//     The producer keeps prefetching the next tile's operands meanwhile.
+//   * Epilogue: every consumer warp drains its own 16 accumulator rows from its registers (epilogue_warp), both warpgroups at
+//     once: + bias (+ residual) -> fp16 rows, fp32 split-K partials or fp32 NCHW, plus the fused GroupNorm partial statistics,
+//     through 2 KB of per-warp staging rather than a shared fp32 tile, so the shared memory goes to the operand ring.  The
+//     producer keeps prefetching the next tile's operands meanwhile.
 #include <stdio.h>
 
 #include "k2_common.cuh"
@@ -34,24 +34,16 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int ACC_PAD = 4;                  // fp32 row pitch BNC + 4: row-per-thread float4 reads hit distinct banks
+constexpr int EPI_WARP_BYTES = 16 * 128;  // per consumer warp: its 16 accumulator rows x 128 B (64 fp16 / 32 fp32 columns)
+constexpr int SMEM_LIMIT = 227 * 1024;    // sm_90 opt-in maximum per block
 
-constexpr int EPI_STAGE_FLOATS = 32 * 33;              // per-warp staging: 4224 B (4096 used)
-constexpr int EPI_BYTES = 4 * EPI_STAGE_FLOATS * 4 + 4 * 256 * 4;  // + per-warp bias copy (<= 256 columns)
-constexpr int SMEM_LIMIT = 227 * 1024;                 // sm_90 opt-in maximum per block
-
-// ES = number of epilogue warp SETS (each set = 4 warps covering the 128 accumulator rows).  ES = 1: the warps of consumer
-// warpgroup 0; ES = 2: both consumer warpgroups, set `es` handling the 64-column pairs jp with jp % 2 == es of a staged pass.
-template <int BN, int ES>
+template <int BN>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // columns staged per epilogue pass: 64 (one pass per 64-column block); 128 with two epilogue sets so that both have work
-  static constexpr int BNC = (BN < 64) ? BN : (ES == 2 ? 128 : 64);
-  static_assert(ES == 1 || BN % 128 == 0, "two epilogue sets need N tiles of 128 or 256");
-  static constexpr int ACC_BYTES = BM * (BNC + ACC_PAD) * 4;
+  static constexpr int EPI_BYTES = 8 * (EPI_WARP_BYTES + BN * 4);  // per consumer warp: staging rows + the N tile's bias
   static constexpr int BAR_BYTES = 256;
-  static constexpr int FIXED = ACC_BYTES + ES * EPI_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
+  static constexpr int FIXED = EPI_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
   static constexpr int STAGES = (SMEM_LIMIT - FIXED) / STAGE_BYTES > 6 ? 6 : (SMEM_LIMIT - FIXED) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
   static_assert(STAGES >= 2, "conv_gemm: shared memory does not hold two pipeline stages");
@@ -75,330 +67,243 @@ __device__ __forceinline__ void decode_m_tile(const ConvGemmParams& p, int m_idx
   n0 = tn_i * p.TN;
 }
 
-// N consecutive fp32 of a staged accumulator row, as raw bits
-template <int N>
-__device__ __forceinline__ void acc_ld(const float* src, uint32_t (&r)[N]) {
-#pragma unroll
-  for (int v = 0; v < N / 4; ++v) {
-    const float4 t = *reinterpret_cast<const float4*>(src + 4 * v);
-    r[4 * v] = __float_as_uint(t.x);
-    r[4 * v + 1] = __float_as_uint(t.y);
-    r[4 * v + 2] = __float_as_uint(t.z);
-    r[4 * v + 3] = __float_as_uint(t.w);
-  }
+// ldmatrix.x4 kept in order with the shared-memory stores around it (the "memory" clobber)
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr)
+               : "memory");
 }
 
-// Epilogue of one (128-row x BN-column) pass of an accumulator tile staged in shared memory (`acc`, pitch BN + ACC_PAD):
-// + bias (+ residual) -> fp16 rows (out_mode 0), fp32 split-K partials (out_mode 2) or fp32 NCHW (out_mode 1).  `cbase` is
-// the output column of staged column 0.
+// Epilogue of one consumer warp, rows [16 k, 16 k + 16) of the M tile (k = 4 g + w), straight from its m64nBN fragment
+// (register 4 q + 2 h + e: row l / 4 + 8 h, column 8 q + 2 (l & 3) + e; `cbase` is the output column of column 0): + bias
+// (+ residual) -> fp16 rows (out_mode 0), fp32 split-K partials (out_mode 2) or fp32 NCHW (out_mode 1), plus the fused
+// GroupNorm partial statistics.  Both consumer warpgroups drain their own rows at the same time.
 //
-// A thread owns one accumulator ROW, so storing straight from registers makes every warp store touch 32 different cache
-// lines with 16 bytes each (and every residual load likewise): with short K loops (the attention qkv / proj GEMMs, 12..24
-// chunks) that epilogue, not the tensor core, sets the pace.  The fp16 / split-K paths therefore go through a per-warp
-// shared-memory transpose (32 rows x 128 B, 16-byte pieces XOR-swizzled by the row): registers -> smem by row, smem -> global
-// with 8 lanes per row, i.e. 4 complete 128-byte lines per store instruction; the residual comes in the same way (coalesced
-// load -> smem -> own row), the bias is read as broadcast LDS.128 from a per-warp copy, and the fused GroupNorm statistics
-// are column sums over the staged fp16 tile.
-template <int BN, int ES>
-__device__ __forceinline__ void epilogue_tile(const ConvGemmParams& p, const float* acc, int ew, int lane, int n0, int y0,
-                                              int x0, int cbase, int split, int m_idx, float* stat_smem, int es_arg,
-                                              int phase) {
-  const int es = (ES == 1) ? 0 : es_arg;
-  const int row = ew * 32 + lane;
+// In the fragment a warp store instruction covers 8 rows x 4 column pairs.  The fp16 and split-K paths therefore pass each
+// 64-column (fp16) or 32-column (fp32) block through the warp's 16 x 128 B staging rows (16-byte pieces XOR-swizzled by the
+// row): the residual comes in coalesced, 8 lanes per 128-byte row, and goes to the fragment layout with ldmatrix; the result
+// goes back with stmatrix and out as 16-byte row pieces, 8 lanes per 128-byte line.  The bias is read from the warp's copy
+// (`bsm`, columns cbase ..).  The GroupNorm statistics are column sums over the staged fp16 rows, summed in the order the
+// partial formats have always used: 16 rows in row order per warp, then (gn_mode 1) warp pairs 2e, 2e + 1 folded for
+// e = 0 .. 3 -- the only place where the two warpgroups meet.
+template <int BN>
+__device__ __forceinline__ void epilogue_warp(const ConvGemmParams& p, const float (&acc)[BN / 2], float* epi, uint32_t stg,
+                                              const float* bsm, int k, int lane, int n0, int y0, int x0, int cbase, int split,
+                                              int m_idx, int phase) {
   const int thw = p.TH * p.TW;
-  constexpr int CH = (BN >= 32) ? 32 : 16;  // columns per staged-accumulator read
-  const float* arow = acc + row * (BN + ACC_PAD);  // this thread's accumulator row
-      const int tn = row / thw;
-      const int rem = row - tn * thw;
-      const int th = rem / p.TW;
-      const int tw = rem - th * p.TW;
-      const int n = n0 + tn, y = y0 + th, x = x0 + tw;
-      const bool valid = (tn < p.TN) && (n < p.NB) && (y < p.H) && (x < p.W);
-      const long long out_row = p.up2 ? (static_cast<long long>(n) * (2 * p.H) + (2 * y + (phase >> 1))) * (2 * p.W) + (2 * x + (phase & 1))
-                                      : (static_cast<long long>(n) * p.H + y) * p.W + x;
+  // output row (pixel) of row `row` of the M tile, -1 outside the image; n, y, x: its image and source position
+  auto out_row_of = [&](int row, int& n, int& y, int& x) -> long long {
+    const int tn = row / thw;
+    const int rem = row - tn * thw;
+    const int th = rem / p.TW;
+    const int tw = rem - th * p.TW;
+    n = n0 + tn;
+    y = y0 + th;
+    x = x0 + tw;
+    if (tn >= p.TN || n >= p.NB || y >= p.H || x >= p.W) return -1;
+    return p.up2 ? (static_cast<long long>(n) * (2 * p.H) + (2 * y + (phase >> 1))) * (2 * p.W) + (2 * x + (phase & 1))
+                 : (static_cast<long long>(n) * p.H + y) * p.W + x;
+  };
+  const int t4 = lane & 3, ra = lane >> 2;  // fragment rows ra, ra + 8; columns 8 q + 2 t4 + {0, 1}
+  if constexpr (BN % 64 == 0) {
+    if ((p.out_mode == 0 && p.Cout % 64 == 0) || (p.out_mode == 2 && p.Cout % 32 == 0)) {
+      int n_, y_, x_;
+      const int my_pix = static_cast<int>(out_row_of(16 * k + (lane & 15), n_, y_, x_));
+      const int sub = lane >> 3, piece = lane & 7;
+      int pix[4];  // pixel of the staged rows 4 i + sub this lane copies in and out
+#pragma unroll
+      for (int i = 0; i < 4; ++i) pix[i] = __shfl_sync(0xffffffffu, my_pix, 4 * i + sub);
+      const bool va = __shfl_sync(0xffffffffu, my_pix, ra) >= 0, vb = __shfl_sync(0xffffffffu, my_pix, ra + 8) >= 0;
+      auto row_addr = [&](int i) {
+        const int rr = 4 * i + sub;
+        return stg + rr * 128 + ((piece ^ (rr & 7)) << 4);
+      };
+      // ldmatrix / stmatrix: lanes 8 m .. 8 m + 7 address matrix m = (8-column group q + m / 2, row half m & 1)
+      const int lrow = (lane & 7) + 8 * ((lane >> 3) & 1);
+      auto frag_addr = [&](int q) { return stg + lrow * 128 + (((q + (lane >> 4)) ^ (lane & 7)) << 4); };
+      if (p.out_mode == 2) {
+        // split-K: raw fp32 partial sums [split][M][Cout] (bias / residual / statistics in the finalize pass)
+        float* wsb = p.ws + static_cast<long long>(split) * p.M_total * p.Cout;
+#pragma unroll
+        for (int j = 0; j < BN / 32; ++j) {
+          const int col0 = cbase + j * 32;
+          if (col0 >= p.Cout) break;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int rr = ra + 8 * h;
+              const int i = 16 * j + 4 * q + 2 * h;
+              sts_v2(stg + rr * 128 + (((2 * q + (t4 >> 1)) ^ (rr & 7)) << 4) + ((t4 & 1) << 3), __float_as_uint(acc[i]),
+                     __float_as_uint(acc[i + 1]));
+            }
+          }
+          __syncwarp();
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const uint4 v4 = lds_v4(row_addr(i));
+            if (pix[i] >= 0)
+              *reinterpret_cast<uint4*>(wsb + static_cast<long long>(pix[i]) * p.Cout + col0 + piece * 4) = v4;
+          }
+          __syncwarp();
+        }
+        return;
+      }
+      constexpr int NP = BN / 64;
       // GroupNorm partial row groups stay image-major under up2: (box index) * 4 + phase
       const int m_in = p.up2 ? m_idx - phase * p.m_tiles_phase : m_idx;
       auto part_index = [&](long long base) { return p.up2 ? base * 4 + phase : base; };
-      if constexpr (BN % 64 == 0) {
-        if ((p.out_mode == 0 && p.Cout % 64 == 0) || (p.out_mode == 2 && p.Cout % 32 == 0)) {
-          const uint32_t stage = smem_u32(stat_smem + (es * 4 + ew) * EPI_STAGE_FLOATS);  // [32 rows][8 x 16 B], piece ^= row & 7
-          float* bsm = stat_smem + 4 * ES * EPI_STAGE_FLOATS + (es * 4 + ew) * 256;
-          const int my_pix = valid ? static_cast<int>(out_row) : -1;
-          const int sub = lane >> 3, piece = lane & 7;
-          int pix[8];  // pixel (output row) of the 8 staged rows this lane copies out: rows i*4 + sub
+      __half* outb = reinterpret_cast<__half*>(p.out);
+      float4 st[NP];  // this warp's GroupNorm sums (sum, sumsq) of columns 2 l, 2 l + 1 of each 64-column block
+      uint4 rpre[4];  // residual of the NEXT 64-column block, in flight while the current one is processed
+      auto load_res = [&](int j) {
+        const int c0 = cbase + j * 64;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) pix[i] = __shfl_sync(0xffffffffu, my_pix, i * 4 + sub);
-          const uint32_t own = stage + lane * 128;
-          if (p.out_mode == 2) {
-            // split-K: raw fp32 partial sums [split][M][Cout] (bias / residual / statistics in the finalize pass)
-            float* wsb = p.ws + static_cast<long long>(split) * p.M_total * p.Cout;
-#pragma unroll 1
-            for (int j = 0; j < BN / 32; ++j) {
-              const int col0 = cbase + j * 32;
-              if (col0 >= p.Cout) break;
-              if constexpr (ES > 1) {
-                if ((j % ES) != es) continue;
-              }
-              uint32_t r[32];
-              acc_ld(arow + j * 32, r);
-#pragma unroll
-              for (int v = 0; v < 8; ++v)
-                sts_v4(own + ((v ^ (lane & 7)) << 4), r[v * 4], r[v * 4 + 1], r[v * 4 + 2], r[v * 4 + 3]);
-              __syncwarp();
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int rr = i * 4 + sub;
-                const uint4 v4 = lds_v4(stage + rr * 128 + ((piece ^ (rr & 7)) << 4));
-                if (pix[i] >= 0)
-                  *reinterpret_cast<uint4*>(wsb + static_cast<long long>(pix[i]) * p.Cout + col0 + piece * 4) = v4;
-              }
-              __syncwarp();
-            }
-            return;
-          }
-          constexpr int NP = BN / 64;
-          if (p.bias) {
-#pragma unroll
-            for (int c = lane; c < BN; c += 32) bsm[c] = (cbase + c < p.Cout) ? __ldg(p.bias + cbase + c) : 0.f;
-            __syncwarp();
-          }
-          __half* outb = reinterpret_cast<__half*>(p.out);
-          float4 st[NP];   // fused GroupNorm statistics of this warp's 32 rows: (sum, sumsq) of columns 2l, 2l+1 per pair
-          uint4 rpre[8];   // residual of the NEXT 64-column pair, in flight while the current one is processed
-          auto load_res = [&](int jp) {
-            const int c0 = cbase + jp * 64;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              rpre[i] = make_uint4(0u, 0u, 0u, 0u);
-              if (pix[i] >= 0 && c0 < p.Cout)
-                rpre[i] = *reinterpret_cast<const uint4*>(p.residual + static_cast<long long>(pix[i]) * p.ldr + c0 + piece * 8);
-            }
-          };
-          if constexpr (ES == 1) {
-            if (p.residual) load_res(0);
-          }
-#pragma unroll
-          for (int jp = 0; jp < NP; ++jp) {
-            const int col0 = cbase + jp * 64;
-            st[jp] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (col0 < p.Cout && (ES == 1 || (jp % ES) == es)) {
-              if constexpr (ES > 1) {
-                if (p.residual) load_res(jp);  // no prefetch registers: the second warp set hides the latency instead
-              }
-              if (p.residual) {  // coalesced: 8 lanes x 16 B per row, 4 rows per instruction -> staged by row
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const int rr = i * 4 + sub;
-                  sts_v4(stage + rr * 128 + ((piece ^ (rr & 7)) << 4), rpre[i].x, rpre[i].y, rpre[i].z, rpre[i].w);
-                }
-                __syncwarp();
-              }
-              if constexpr (ES == 1) {
-                if (p.residual && jp + 1 < NP) load_res(jp + 1);
-              }
-#pragma unroll
-              for (int v = 0; v < 8; ++v) {  // 8 columns = one 16-byte piece of the staged row
-                // read per piece: the unread part of the register accumulator is still live while the first passes of a
-                // 256-column tile drain
-                uint32_t r[8];
-                acc_ld(arow + jp * 64 + v * 8, r);
-                float f[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(r[e]);
-                if (p.bias) {
-                  const float4 b0 = *reinterpret_cast<const float4*>(bsm + jp * 64 + v * 8);
-                  const float4 b1 = *reinterpret_cast<const float4*>(bsm + jp * 64 + v * 8 + 4);
-                  f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                  f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                }
-                const uint32_t slot = own + ((v ^ (lane & 7)) << 4);
-                if (p.residual) {
-                  const uint4 rv = lds_v4(slot);
-                  const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float2 t = __half22float2(rh[e]);
-                    f[2 * e] += t.x;
-                    f[2 * e + 1] += t.y;
-                  }
-                }
-                uint32_t o[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const __half2 hh = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
-                  o[e] = valid ? *reinterpret_cast<const uint32_t*>(&hh) : 0u;  // rows outside the image count as zeros
-                }
-                sts_v4(slot, o[0], o[1], o[2], o[3]);
-              }
-              __syncwarp();
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int rr = i * 4 + sub;
-                const uint4 v4 = lds_v4(stage + rr * 128 + ((piece ^ (rr & 7)) << 4));
-                if (pix[i] >= 0)
-                  *reinterpret_cast<uint4*>(outb + static_cast<long long>(pix[i]) * p.ldo + col0 + piece * 8) = v4;
-              }
-              if (p.gn_part) {
-                // statistics of the fp16-ROUNDED stored values: lane l sums columns 2l, 2l+1 over the warp's rows
-                float4 h0 = make_float4(0.f, 0.f, 0.f, 0.f), h1 = make_float4(0.f, 0.f, 0.f, 0.f);  // rows 0-15 / 16-31
-#pragma unroll
-                for (int rr = 0; rr < 32; ++rr) {
-                  const uint32_t w = lds_u32(stage + rr * 128 + (((lane >> 2) ^ (rr & 7)) << 4) + ((lane & 3) << 2));
-                  const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&w));
-                  float4& hacc = (rr < 16) ? h0 : h1;
-                  hacc.x += t.x;
-                  hacc.y = fmaf(t.x, t.x, hacc.y);
-                  hacc.z += t.y;
-                  hacc.w = fmaf(t.y, t.y, hacc.w);
-                }
-                if (p.gn_mode == 2) {
-                  // 16-pixel x 8-image tiles: half warp h of warp ew holds image n0 + 2*ew + h of spatial tile sp
-                  const int per = p.tiles_h * p.tiles_w;
-                  const int sp = m_in % per;
-                  const int img = n0 + 2 * ew;
-                  if (2 * ew < p.TN && img < p.NB)
-                    *reinterpret_cast<float4*>(p.gn_part + part_index(static_cast<long long>(img) * per + sp) * p.Cout + col0 + 2 * lane) = h0;
-                  if (2 * ew + 1 < p.TN && img + 1 < p.NB)
-                    *reinterpret_cast<float4*>(p.gn_part + part_index(static_cast<long long>(img + 1) * per + sp) * p.Cout + col0 + 2 * lane) = h1;
-                } else {
-                  st[jp] = make_float4(h0.x + h1.x, h0.y + h1.y, h0.z + h1.z, h0.w + h1.w);
-                }
-              }
-              __syncwarp();
-            }
-          }
-          if (p.gn_part && p.gn_mode == 1) {
-            // one partial per (M tile, column): the four warps' sums are folded in a fixed order through the (now idle)
-            // staging buffers, so k2_gn_finalize reads a quarter of what per-warp partials would cost
-            if constexpr (ES == 1) {
-              float4* mine = reinterpret_cast<float4*>(stat_smem + ew * EPI_STAGE_FLOATS);
-#pragma unroll
-              for (int jp = 0; jp < NP; ++jp) mine[jp * 32 + lane] = st[jp];
-              named_bar_sync(1, 128);
-              if (ew < NP) {
-                const int col0 = cbase + ew * 64;
-                if (col0 < p.Cout) {
-                  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                  for (int w = 0; w < 4; ++w) {
-                    const float4 t = reinterpret_cast<const float4*>(stat_smem + w * EPI_STAGE_FLOATS)[ew * 32 + lane];
-                    acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
-                  }
-                  *reinterpret_cast<float4*>(p.gn_part + part_index(m_in) * p.Cout + col0 + 2 * lane) = acc;
-                }
-              }
-              named_bar_sync(1, 128);
-            } else {
-              // each warp set folds the pairs it owns (jp % ES == es) among its own four warps: barrier 1 + es
-              float4* mine = reinterpret_cast<float4*>(stat_smem + (es * 4 + ew) * EPI_STAGE_FLOATS);
-#pragma unroll
-              for (int jp = 0; jp < NP; ++jp) mine[jp * 32 + lane] = st[jp];
-              named_bar_sync(1 + es, 128);
-              const int jp_f = es + ew * ES;  // warp ew of the set folds the set's ew-th pair
-              if (jp_f < NP) {
-                const int col0 = cbase + jp_f * 64;
-                if (col0 < p.Cout) {
-                  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                  for (int w = 0; w < 4; ++w) {
-                    const float4 t =
-                        reinterpret_cast<const float4*>(stat_smem + (es * 4 + w) * EPI_STAGE_FLOATS)[jp_f * 32 + lane];
-                    acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
-                  }
-                  *reinterpret_cast<float4*>(p.gn_part + part_index(m_in) * p.Cout + col0 + 2 * lane) = acc;
-                }
-              }
-              named_bar_sync(1 + es, 128);
-            }
-          }
-          return;
+        for (int i = 0; i < 4; ++i) {
+          rpre[i] = make_uint4(0u, 0u, 0u, 0u);
+          if (pix[i] >= 0 && c0 < p.Cout)
+            rpre[i] = *reinterpret_cast<const uint4*>(p.residual + static_cast<long long>(pix[i]) * p.ldr + c0 + piece * 8);
         }
-      }
-#pragma unroll 1
-      for (int j = 0; j < BN / CH; ++j) {
-        uint32_t r[CH];
-        acc_ld(arow + j * CH, r);
-        const int col0 = cbase + j * CH;
-        if (valid && col0 < p.Cout) {
-          if (p.out_mode == 2) {
-            // split-K: raw fp32 partial sums [split][M][Cout] into the workspace (bias/residual in the finalize pass)
-            float* w = p.ws + (static_cast<long long>(split) * p.M_total + out_row) * p.Cout + col0;
-            if (col0 + CH <= p.Cout) {
+      };
+      if (p.residual) load_res(0);
 #pragma unroll
-              for (int v = 0; v < CH / 4; ++v)
-                *reinterpret_cast<uint4*>(w + v * 4) = make_uint4(r[v * 4], r[v * 4 + 1], r[v * 4 + 2], r[v * 4 + 3]);
-            } else {
+      for (int j = 0; j < NP; ++j) {
+        const int col0 = cbase + j * 64;
+        st[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (col0 >= p.Cout) continue;
+        uint32_t res[16];  // residual pairs in fragment layout: [2 q + h]
+        if (p.residual) {
 #pragma unroll
-              for (int e = 0; e < CH; ++e)
-                if (col0 + e < p.Cout) w[e] = __uint_as_float(r[e]);
+          for (int i = 0; i < 4; ++i) sts_v4(row_addr(i), rpre[i].x, rpre[i].y, rpre[i].z, rpre[i].w);
+          __syncwarp();
+#pragma unroll
+          for (int qq = 0; qq < 4; ++qq) {
+            uint32_t r4[4];
+            ldsm_x4(r4, frag_addr(2 * qq));
+#pragma unroll
+            for (int m = 0; m < 4; ++m) res[4 * qq + m] = r4[m];
+          }
+          if (j + 1 < NP) load_res(j + 1);
+          __syncwarp();  // the staged residual is read before the result overwrites it
+        }
+        uint32_t o[16];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float f0 = acc[32 * j + 4 * q + 2 * h], f1 = acc[32 * j + 4 * q + 2 * h + 1];
+            if (p.bias) {
+              const float2 b = *reinterpret_cast<const float2*>(bsm + j * 64 + 8 * q + 2 * t4);
+              f0 += b.x;
+              f1 += b.y;
             }
-          } else if (p.out_mode == 0) {
-            __half* orow = reinterpret_cast<__half*>(p.out) + out_row * p.ldo + col0;
-            const __half* rrow = p.residual ? p.residual + out_row * p.ldr + col0 : nullptr;
-            if (col0 + CH <= p.Cout) {
-#pragma unroll
-              for (int v = 0; v < CH / 8; ++v) {
-                float f[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  f[e] = __uint_as_float(r[v * 8 + e]);
-                  if (p.bias) f[e] += __ldg(p.bias + col0 + v * 8 + e);
-                }
-                if (rrow) {
-                  uint4 rv = *reinterpret_cast<const uint4*>(rrow + v * 8);
-                  const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    float2 t = __half22float2(rh[e]);
-                    f[2 * e] += t.x;
-                    f[2 * e + 1] += t.y;
-                  }
-                }
-                uint4 ov;
-                __half2* oh = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) oh[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
-                *reinterpret_cast<uint4*>(orow + v * 8) = ov;
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < CH; ++e) {
-                if (col0 + e < p.Cout) {
-                  float f = __uint_as_float(r[e]);
-                  if (p.bias) f += __ldg(p.bias + col0 + e);
-                  if (rrow) f += __half2float(rrow[e]);
-                  orow[e] = __float2half_rn(f);
-                }
-              }
+            if (p.residual) {
+              const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&res[2 * q + h]));
+              f0 += t.x;
+              f1 += t.y;
             }
+            const __half2 hh = __floats2half2_rn(f0, f1);
+            o[2 * q + h] = (h ? vb : va) ? *reinterpret_cast<const uint32_t*>(&hh) : 0u;  // rows outside the image: zeros
+          }
+        }
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) stmatrix_x4(frag_addr(2 * qq), o[4 * qq], o[4 * qq + 1], o[4 * qq + 2], o[4 * qq + 3]);
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint4 v4 = lds_v4(row_addr(i));
+          if (pix[i] >= 0) *reinterpret_cast<uint4*>(outb + static_cast<long long>(pix[i]) * p.ldo + col0 + piece * 8) = v4;
+        }
+        if (p.gn_part) {
+          // statistics of the fp16-ROUNDED stored values: lane l sums columns 2 l, 2 l + 1 over the warp's 16 rows
+          float4 hs = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int rr = 0; rr < 16; ++rr) {
+            const uint32_t v = lds_u32(stg + rr * 128 + (((lane >> 2) ^ (rr & 7)) << 4) + ((lane & 3) << 2));
+            const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&v));
+            hs.x += t.x;
+            hs.y = fmaf(t.x, t.x, hs.y);
+            hs.z += t.y;
+            hs.w = fmaf(t.y, t.y, hs.w);
+          }
+          if (p.gn_mode == 2) {
+            // 16-pixel x 8-image tiles: warp k holds image n0 + k of spatial tile sp
+            const int per = p.tiles_h * p.tiles_w;
+            const int sp = m_in % per;
+            const int img = n0 + k;
+            if (k < p.TN && img < p.NB)
+              *reinterpret_cast<float4*>(p.gn_part + part_index(static_cast<long long>(img) * per + sp) * p.Cout + col0 + 2 * lane) = hs;
           } else {
-            // fp32 NCHW (UNet / MoVQ output heads)
-            float* o = reinterpret_cast<float*>(p.out);
-#pragma unroll
-            for (int e = 0; e < CH; ++e) {
-              if (col0 + e < p.Cout) {
-                float f = __uint_as_float(r[e]);
-                if (p.bias) f += __ldg(p.bias + col0 + e);
-                o[((static_cast<long long>(n) * p.Cout + (col0 + e)) * p.H + y) * p.W + x] = f;
-              }
-            }
+            st[j] = hs;
           }
         }
+        __syncwarp();
       }
+      if (p.gn_part && p.gn_mode == 1) {
+        // one partial per (M tile, column): the eight warps' sums are folded in a fixed order through their (now idle)
+        // staging rows, so k2_gn_finalize reads an eighth of what per-warp partials would cost
+        float4* sums = reinterpret_cast<float4*>(epi);  // [warp][128]
+#pragma unroll
+        for (int j = 0; j < NP; ++j) sums[k * 128 + j * 32 + lane] = st[j];
+        named_bar_sync(1, 256);
+        if (k < NP && cbase + k * 64 < p.Cout) {
+          float4 tot = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {  // 32-row groups in row order: the sums of warps 2 e and 2 e + 1
+            const float4 a = sums[(2 * e) * 128 + k * 32 + lane], b = sums[(2 * e + 1) * 128 + k * 32 + lane];
+            tot.x += a.x + b.x;
+            tot.y += a.y + b.y;
+            tot.z += a.z + b.z;
+            tot.w += a.w + b.w;
+          }
+          *reinterpret_cast<float4*>(p.gn_part + part_index(m_in) * p.Cout + cbase + k * 64 + 2 * lane) = tot;
+        }
+        named_bar_sync(1, 256);  // the sums are read before any warp stages the next tile
+      }
+      return;
+    }
+  }
+  // element by element from the fragment: Cout not a multiple of 64 (fp16) / 32 (split-K), N tile 16, fp32 NCHW heads
+  int n[2], y[2], x[2];
+  long long orow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) orow[h] = out_row_of(16 * k + ra + 8 * h, n[h], y[h], x[h]);
+#pragma unroll
+  for (int q = 0; q < BN / 8; ++q) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = cbase + 8 * q + 2 * t4 + e;
+        if (orow[h] < 0 || col >= p.Cout) continue;
+        float f = acc[4 * q + 2 * h + e];
+        if (p.out_mode == 2) {
+          p.ws[(static_cast<long long>(split) * p.M_total + orow[h]) * p.Cout + col] = f;
+          continue;
+        }
+        if (p.bias) f += __ldg(p.bias + col);
+        if (p.out_mode == 0) {
+          if (p.residual) f += __half2float(p.residual[orow[h] * p.ldr + col]);
+          reinterpret_cast<__half*>(p.out)[orow[h] * p.ldo + col] = __float2half_rn(f);
+        } else {
+          reinterpret_cast<float*>(p.out)[((static_cast<long long>(n[h]) * p.Cout + col) * p.H + y[h]) * p.W + x[h]] = f;
+        }
+      }
+    }
+  }
 }
 
 
-template <int BN, int ES>
+template <int BN>
 __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
-  using C = Cfg<BN, ES>;
-  constexpr int BNC = C::BNC;
+  using C = Cfg<BN>;
   constexpr int NA = BN / 2;  // accumulator registers of the m64nBNk16 fragment
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  float* acc_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);
-  float* stat_smem = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + C::ACC_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES + C::ACC_BYTES + ES * EPI_BYTES);
+  float* epi = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES);  // [8 warps][16 x 128 B], then [8 warps][BN] bias
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES);
   uint64_t* empty_bar = full_bar + C::STAGES;
 
   const int warp_idx = threadIdx.x >> 5;
@@ -479,7 +384,10 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
     // ============================ wgmma consumers + epilogue ================================
     setmaxnreg_inc<232>();
     const int g = wg - 1;          // accumulator rows [64 g, 64 g + 64)
-    const int w = warp_idx & 3;    // warp of the warpgroup: rows 16 w .. 16 w + 15 of the warpgroup's 64
+    const int k = warp_idx - 4;    // consumer warp: rows 16 k .. 16 k + 15 of the M tile
+    const uint32_t stg = smem_u32(epi) + k * EPI_WARP_BYTES;
+    float* bsm = epi + 8 * EPI_WARP_BYTES / 4 + k * BN;
+    int bias_cols = -1;  // output column of bsm[0]
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -497,10 +405,10 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
         const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + A_STAGE_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
+        for (int ks = 0; ks < BK / 16; ++ks) {
           // +32 bytes (2 x 16 B units) per 16-element K step inside the 128 B swizzle row
-          const uint64_t adesc = make_wgmma_desc(a_addr) + static_cast<uint64_t>(k * 2);
-          const uint64_t bdesc = make_wgmma_desc(b_addr) + static_cast<uint64_t>(k * 2);
+          const uint64_t adesc = make_wgmma_desc(a_addr) + static_cast<uint64_t>(ks * 2);
+          const uint64_t bdesc = make_wgmma_desc(b_addr) + static_cast<uint64_t>(ks * 2);
           if constexpr (BN == 256) {
             wgmma_m64n256k16(acc, adesc, bdesc, 1u);
           } else if constexpr (BN == 192) {
@@ -525,28 +433,21 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
         }
       }
       wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < NA; ++i) reg_fence(acc[i]);
       if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);  // an empty K range consumed no stage
 
       int n0, y0, x0, mphase;
       decode_m_tile(p, m_idx, n0, y0, x0, mphase);
-      const int r0 = 64 * g + 16 * w + (lane >> 2);
-      const int cq = 2 * (lane & 3);
+      const int cbase = n_idx * BN;
+      if (p.bias && cbase != bias_cols) {  // the warp's bias copy follows the N tile
+        __syncwarp();
 #pragma unroll
-      for (int pass = 0; pass < BN / BNC; ++pass) {
-        named_bar_sync(3, 256);  // the staged tile of the previous pass / tile has been read
-#pragma unroll
-        for (int i = 0; i < NA; i += 2) {
-          // register i: row 16 w + l / 4 + 8 ((i / 2) & 1), column 8 (i / 4) + 2 (l & 3) + (i & 1) of the tile
-          if ((8 * (i >> 2)) / BNC != pass) continue;
-          const int row = r0 + 8 * ((i >> 1) & 1);
-          const int col = 8 * (i >> 2) - pass * BNC + cq;
-          *reinterpret_cast<float2*>(acc_smem + row * (BNC + ACC_PAD) + col) = make_float2(acc[i], acc[i + 1]);
-        }
-        named_bar_sync(3, 256);  // staged tile complete
-        if (ES == 2 || g == 0)
-          epilogue_tile<BNC, ES>(p, acc_smem, w, lane, n0, y0, x0, n_idx * BN + pass * BNC, split, m_idx, stat_smem, g,
-                                 mphase);
+        for (int c = lane; c < BN; c += 32) bsm[c] = (cbase + c < p.Cout) ? __ldg(p.bias + cbase + c) : 0.f;
+        __syncwarp();
+        bias_cols = cbase;
       }
+      epilogue_warp<BN>(p, acc, epi, stg, bsm, k, lane, n0, y0, x0, cbase, split, m_idx, mphase);
     }
   }
 }
@@ -626,18 +527,17 @@ __global__ void __launch_bounds__(256) splitk_finalize_kernel(const float* __res
 }
 
 
-template <int BN, int ES>
+template <int BN>
 int launch_bn(const ConvGemmParams& p, cudaStream_t stream) {
-  using C = Cfg<BN, ES>;
+  using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, ES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       C::SMEM_BYTES));
+    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
   int total = p.m_tiles * p.n_tiles * p.splits;
   int grid = total < num_sms() ? total : num_sms();
-  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN, ES>, dim3(grid), dim3(384), C::SMEM_BYTES, stream, p));
+  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN>, dim3(grid), dim3(384), C::SMEM_BYTES, stream, p));
   return 0;
 }
 
@@ -651,20 +551,13 @@ int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, c
   return 0;
 }
 
-int launch_conv_gemm(const ConvGemmParams& p, int BN, int epilogue_sets, cudaStream_t stream) {
-  if (epilogue_sets == 2) {  // both consumer warpgroups drain the accumulator: short-K GEMMs are epilogue-paced
-    switch (BN) {
-      case 128: return launch_bn<128, 2>(p, stream);
-      case 256: return launch_bn<256, 2>(p, stream);
-      default: break;  // N tile 192 stages 64 columns per pass: a second set would have nothing to drain
-    }
-  }
+int launch_conv_gemm(const ConvGemmParams& p, int BN, cudaStream_t stream) {
   switch (BN) {
-    case 16: return launch_bn<16, 1>(p, stream);
-    case 64: return launch_bn<64, 1>(p, stream);
-    case 128: return launch_bn<128, 1>(p, stream);
-    case 192: return launch_bn<192, 1>(p, stream);
-    case 256: return launch_bn<256, 1>(p, stream);
+    case 16: return launch_bn<16>(p, stream);
+    case 64: return launch_bn<64>(p, stream);
+    case 128: return launch_bn<128>(p, stream);
+    case 192: return launch_bn<192>(p, stream);
+    case 256: return launch_bn<256>(p, stream);
     default: return fail("conv_gemm: unsupported BN");
   }
 }

@@ -83,7 +83,7 @@ struct ConvGemmParams {
                        //    NB/H/W and the tile box are SOURCE geometry, outputs go to pixel (2y + a, 2x + b) of a 2H x 2W image
   int m_tiles_phase;   // up2: tile slots per phase (m_tiles = 4 * m_tiles_phase)
 };
-int launch_conv_gemm(const ConvGemmParams& p, int BN, int epilogue_sets, cudaStream_t stream);
+int launch_conv_gemm(const ConvGemmParams& p, int BN, cudaStream_t stream);
 int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, const float* bias, const __half* residual,
                            int ldr, __half* out, int ldo, float2* gn_part, cudaStream_t stream);
 

@@ -25,9 +25,9 @@ _tune_cache = {}
 
 
 def tune(key, run, m_rows=0):
-    """Launch configuration of one conv / GEMM layer shape: (N tile, pair mode, splits, epilogue warp sets) for
-    k2_conv_gemm_cfg, picked by timing candidates with CUDA events on the current stream: N tile x epilogue sets (bit-identical
-    results) for layers of more than 64 output channels, plus split-K variants for layers of at most TUNE_SMALL_M output rows
+    """Launch configuration of one conv / GEMM layer shape: (N tile, pair mode, splits, epilogue warp sets = 1) for
+    k2_conv_gemm_cfg, picked by timing candidates with CUDA events on the current stream: N tiles (bit-identical results) for
+    layers of more than 64 output channels, plus split-K variants for layers of at most TUNE_SMALL_M output rows
     (m_rows; see above).  Cached per shape and device; None = the library's own choice.  key = (kind, Cout, ...); run(cfg, info)
     must enqueue the launch and report the configuration the library actually used in info."""
     if not TUNE:
@@ -42,8 +42,7 @@ def tune(key, run, m_rows=0):
     best = None
     if cout > 64:
         bns = [bn0] if splits > 1 else [bn for bn in (128, 192, 256) if bn - 64 < cout or bn == bn0]
-        cands = [(bn0, 0, splits, 1)] + [(bn, 0, splits, es) for bn in bns for es in ((1,) if bn == 192 else (1, 2))
-                                        if (bn, es) != (bn0, 1)]
+        cands = [(bn0, 0, splits, 1)] + [(bn, 0, splits, 1) for bn in bns if bn != bn0]
         if 0 < m_rows <= TUNE_SMALL_M and splits == 1:
             for bn in (128, 192, 256):
                 if bn - 64 >= cout:

@@ -2,7 +2,7 @@
 
 Builds the full-size cfg-2 step the way bench.py does (Kandinsky 2.2 decoder UNet with random weights, 4 images x CFG at 96x96
 latents), takes the distinct conv / GEMM layer shapes from the keys the step's launch plan hands the autotuner (the keys of
-launch_plan._tune_cache, counted as the plan is recorded, so also how often the step launches each one), then times every legal (N tile, epilogue warp sets) configuration of each shape, unsplit,
+launch_plan._tune_cache, counted as the plan is recorded, so also how often the step launches each one), then times every legal N tile of each shape, unsplit,
 on fresh tensors of that shape: CUDA events around enough back-to-back launches to fill --min-ms after a warm-up.
 
 Per shape and configuration it reports:
@@ -162,8 +162,7 @@ def main():
         cout = shp["N"]
         cfgs = []
         if cout > 64:  # the tuner's candidates at splits 1
-            cfgs = [(bn, 0, 1, es) for bn in (128, 192, 256) if bn - 64 < cout or bn == info[0]
-                    for es in ((1,) if bn == 192 else (1, 2))]
+            cfgs = [(bn, 0, 1, 1) for bn in (128, 192, 256) if bn - 64 < cout or bn == info[0]]
         if tuple(picked_cfg) not in cfgs:
             cfgs.append(tuple(picked_cfg))
         rows = []
@@ -198,13 +197,13 @@ def main():
 
     print(f"# {res['card']}  (mma_n={args.mma_n})  conv time per step at the picked configurations: {total:.2f} ms")
     print(f"{'shape':44s} {'n':>2s} {'share':>6s} {'pick':>9s}  " + "  ".join(f"{c:>9s}" for c in
-          ("128/1", "128/2", "192/1", "256/1", "256/2")) + "   (TFLOP/s at N tile / epilogue sets, splits 1)")
+          ("128", "192", "256")) + "   (TFLOP/s at N tile, splits 1)")
     for l in layers:
         by = {(r["n_tile"], r["epilogue_sets"]): r["tflops"] for r in l["configs"] if r["splits"] == 1}
         pk = l["picked"]
         print(f"{l['shape'][:44]:44s} {l['launches_per_step']:2d} {100 * l['share_of_conv_time']:5.1f}% "
               f"{pk['n_tile']:>3d}/{pk['epilogue_sets']}/{pk['splits']:<3d}  " +
-              "  ".join(f"{by.get(c, float('nan')):9.1f}" for c in ((128, 1), (128, 2), (192, 1), (256, 1), (256, 2))))
+              "  ".join(f"{by.get(c, float('nan')):9.1f}" for c in ((128, 1), (192, 1), (256, 1))))
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
