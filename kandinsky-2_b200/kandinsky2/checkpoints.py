@@ -40,6 +40,11 @@
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
   qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
 
+* Kandinsky 2.2 ships its MoVQ as a diffusers `VQModel` with `norm_type="spatial"` (the decoder folders' `movq/`).  It is the
+  reference's MOVQ under other names: `diffusers_movq_to_k2` renames it into `vqgan.autoencoder.MOVQ` names and turns the
+  attention's Linear q / k / v / out into the 1x1 convolutions MOVQ registers; `k2_to_diffusers_movq` is its inverse
+  (tests/test_cpu_movq22.py pins both through the network against a diffusers-form forward, tests/movq22_oracle.py).
+
 **Parity unpinned:** diffusers is not part of /root/reference (`setup.py:27` lists it unpinned) and is not installed in the
 build container, so the diffusers-side key names below are restated from the published `UNet2DConditionModel` layout
 (`ResnetDownsampleBlock2D` / `SimpleCrossAttnDownBlock2D` / `UNetMidBlock2DSimpleCrossAttn` / `SimpleCrossAttnUpBlock2D` /
@@ -591,6 +596,78 @@ def load_weights(folder, candidates, what):
     skipped = load_file is None and any(n.endswith(".safetensors") for n in candidates)
     note = " (safetensors is not installed)" if skipped else ""
     raise K2Error(f"{what}: {' or '.join(os.path.join(folder, n) for n in candidates)} not found{note}")
+
+
+# this package's MoVQ names -> diffusers VQModel names: (pattern, replacement) applied in order, before the up-block numbering
+_MOVQ_RENAME = [(r"^encoder\.down\.(\d+)\.block\.", r"encoder.down_blocks.\1.resnets."),
+                (r"^encoder\.down\.(\d+)\.attn\.", r"encoder.down_blocks.\1.attentions."),
+                (r"^encoder\.down\.(\d+)\.downsample\.", r"encoder.down_blocks.\1.downsamplers.0."),
+                (r"^(encoder|decoder)\.mid\.block_1\.", r"\1.mid_block.resnets.0."),
+                (r"^(encoder|decoder)\.mid\.block_2\.", r"\1.mid_block.resnets.1."),
+                (r"^(encoder|decoder)\.mid\.attn_1\.", r"\1.mid_block.attentions.0."),
+                (r"^(encoder|decoder)\.norm_out\.", r"\1.conv_norm_out."),
+                (r"\.upsample\.", ".upsamplers.0."), (r"\.nin_shortcut\.", ".conv_shortcut."),
+                (r"(\.attentions\.\d+\.)q\.", r"\1to_q."), (r"(\.attentions\.\d+\.)k\.", r"\1to_k."),
+                (r"(\.attentions\.\d+\.)v\.", r"\1to_v."), (r"(\.attentions\.\d+\.)proj_out\.", r"\1to_out.0."),
+                (r"^(encoder\..*\.attentions\.\d+\.)norm\.", r"\1group_norm."),
+                (r"^(decoder\..*\.attentions\.\d+\.)norm\.", r"\1spatial_norm.")]
+# the attention names older diffusers conversions wrote (AttentionBlock, before the Attention refactor)
+_MOVQ_LEGACY = re.compile(r"^(.*\.attentions\.\d+\.)(query|key|value|proj_attn)\.(weight|bias)$")
+_MOVQ_LEGACY_NAME = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
+_MOVQ_LINEAR = re.compile(r"\.attentions\.\d+\.(to_q|to_k|to_v|to_out\.0)\.weight$")
+
+
+def _movq_names(ddconfig):
+    """{this package's key: diffusers VQModel key} for every parameter `vqgan.autoencoder.MOVQ(ddconfig, ...)` registers.
+    diffusers numbers the decoder's up_blocks from the lowest resolution, the reference's decoder.up from the highest."""
+    from .vqgan.autoencoder import MOVQ
+    n = len(ddconfig["ch_mult"])
+    names = {}
+    for k in MOVQ(ddconfig, 1, ddconfig["z_channels"], device="meta").state_dict():
+        d = re.sub(r"^decoder\.up\.(\d+)\.block\.", lambda m: f"decoder.up_blocks.{n - 1 - int(m.group(1))}.resnets.", k)
+        d = re.sub(r"^decoder\.up\.(\d+)\.", lambda m: f"decoder.up_blocks.{n - 1 - int(m.group(1))}.", d)
+        d = re.sub(r"^(decoder\.up_blocks\.\d+\.)attn\.", r"\1attentions.", d)
+        for pat, rep in _MOVQ_RENAME:
+            d = re.sub(pat, rep, d)
+        names[k] = d
+    return names
+
+
+def diffusers_movq_to_k2(sd, config):
+    """diffusers `VQModel` state dict (norm_type "spatial": the Kandinsky 2.2 decoder folders' `movq/`) -> `vqgan.autoencoder.MOVQ`
+    keys for the geometry `config` (a MOVQ ddconfig, e.g. the first item of diffusers_compat.movq_config).  The names:
+        encoder.down_blocks.{i}.resnets.{j} / .attentions.{j} / .downsamplers.0   -> encoder.down.{i}.block.{j} / .attn.{j} / .downsample
+        {en,de}coder.mid_block.resnets.{0,1} / .attentions.0                      -> {en,de}coder.mid.block_{1,2} / .attn_1
+        decoder.up_blocks.{i}.resnets.{j} / .attentions.{j} / .upsamplers.0       -> decoder.up.{n-1-i}.block.{j} / .attn.{j} / .upsample
+        {en,de}coder.conv_norm_out -> norm_out;  conv_shortcut -> nin_shortcut
+        attention group_norm (encoder) / spatial_norm (decoder) -> norm;  to_q / to_k / to_v / to_out.0 -> q / k / v / proj_out
+    the SpatialNorm's norm_layer / conv_y / conv_b, conv_in / conv_out, quant_conv, post_quant_conv and quantize.embedding keep
+    their names.  The attention's Linear weights [C, C] become 1x1 convolution weights [C, C, 1, 1].  The names older diffusers
+    conversions gave the attention projections (query / key / value / proj_attn) are taken as to_q / to_k / to_v / to_out.0.
+    Unknown and missing keys raise K2Error naming them.  Restated from diffusers' published layout (diffusers is not a
+    dependency)."""
+    names = _movq_names(config)
+    renamed = {}
+    for k, v in sd.items():
+        m = _MOVQ_LEGACY.match(k)
+        d = f"{m.group(1)}{_MOVQ_LEGACY_NAME[m.group(2)]}.{m.group(3)}" if m else k
+        if d in renamed:
+            raise K2Error(f"diffusers MoVQ state dict: {k!r} and another key both give {d!r}")
+        renamed[d] = v
+    _require_keys(renamed, list(names.values()), "diffusers MoVQ")
+    out = {}
+    for k, d in names.items():
+        t = renamed[d]
+        out[k] = t.reshape(t.shape[0], -1, 1, 1) if _MOVQ_LINEAR.search(d) else t
+    return out
+
+
+def k2_to_diffusers_movq(sd, config):
+    """Inverse of diffusers_movq_to_k2 (export, and the round-trip test): the attention's 1x1 convolution weights become
+    Linear weights [C, C].  Unknown and missing keys raise K2Error naming them."""
+    names = _movq_names(config)
+    _require_keys(sd, list(names), "MoVQ")
+    return {d: sd[k].reshape(sd[k].shape[0], -1) if _MOVQ_LINEAR.search(d) else sd[k] for k, d in names.items()}
 
 
 _DPT_HYBRID_TOP = {"cls_token": "dpt.embeddings.cls_token", "position_embedding": "dpt.embeddings.position_embeddings",

@@ -4,6 +4,8 @@ create_model(**CONFIG_2_1['model_config'], up=False, inpainting=...) returns the
 InpaintText2ImUNet; channel_mult / attention_resolutions strings are resolved exactly as the reference does
 (:33-48: attention 'resolutions' are image_size // res downsample rates).
 """
+import torch
+
 from .unet import InpaintText2ImUNet, Text2ImUNet
 
 
@@ -33,6 +35,15 @@ def create_model(image_size, num_channels, num_res_blocks, channel_mult, attenti
                cache_text_emb=cache_text_emb, text_encoder_in_dim1=text_encoder_in_dim1,
                text_encoder_in_dim2=text_encoder_in_dim2, pooling_type=pooling_type,
                cond_version=version, **kwargs)
+
+
+def create_decoder_unet(model_config, task_type, device, param_dtype=torch.float16):
+    """The decoder UNet of a pipeline: create_model(**model_config) for `task_type` -- "inpainting" adds the image and mask
+    channels, "controlnet" (Kandinsky 2.2 ControlNet-depth) 4 hint-feature channels beside the 4 latent ones."""
+    mc = dict(model_config)
+    if task_type == "controlnet":
+        mc.update(in_channels=mc["in_channels"] + 4, hint_channels=4)
+    return create_model(**mc, up=False, inpainting=(task_type == "inpainting"), device=device, param_dtype=param_dtype)
 
 
 def create_gaussian_diffusion(*args, **kwargs):

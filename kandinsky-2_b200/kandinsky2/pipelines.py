@@ -12,6 +12,7 @@ wrapping its prior / encoders.  img2img / inpainting take a PIL image (encoded b
 """
 import hashlib
 import math
+import os
 
 import torch
 
@@ -19,7 +20,7 @@ from . import ops, parallel
 from ._native import K2Error
 from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, PLMSSampler, UniPCSchedule, create_ddpm_v22,
                                        create_gaussian_diffusion)
-from .model.model_creation import create_model
+from .model.model_creation import create_decoder_unet
 from .utils import prepare_image, prepare_mask, q_sample, uint8_to_pil
 from .vqgan import MOVQ
 
@@ -112,11 +113,8 @@ class _DecoderBase:
         self.device = torch.device(device)
         self.task_type = task_type
         self.use_fp16 = True
-        mc = dict(config["model_config"])
-        if task_type == "controlnet":  # Kandinsky 2.2 ControlNet-depth (BASELINE configs[4]): 4 latent + 4 hint-feature channels
-            mc.update(in_channels=mc["in_channels"] + 4, hint_channels=4)
-        self.model = create_model(**mc, up=False, inpainting=(task_type == "inpainting"), device=self.device,
-                                  param_dtype=torch.float16)
+        mc = config["model_config"]
+        self.model = create_decoder_unet(mc, task_type, self.device)
         if unet_state_dict is not None:
             self.model.load_state_dict(unet_state_dict)
         else:
@@ -325,6 +323,23 @@ class Kandinsky2_2(_DecoderBase):
         generate_controlnet and generate_controlnet_img2img also take a PIL image as hint and build the depth map from it."""
         super().__init__(*args, **kwargs)
         self.depth_estimator = depth_estimator
+
+    @classmethod
+    def from_pretrained(cls, decoder_dir, prior=None, depth_estimator=None, device="cuda"):
+        """A local Kandinsky 2.2 decoder folder in the diffusers layout (kandinsky-2-2-decoder, kandinsky-2-2-decoder-inpaint,
+        kandinsky-2-2-controlnet-depth: model_index.json, unet/, movq/, scheduler/; diffusers_compat.read_decoder_folder) ->
+        the pipeline of the folder's task, its UNet and MoVQ weights cast to the fp16 parameters.  prior: a local
+        kandinsky-2-2-prior folder (PriorEmbedder22.from_pretrained), an embedder object, or None (SyntheticEmbedder).
+        depth_estimator: as for the constructor.  A missing file raises K2Error naming it.  The scheduler_config.json must
+        describe the schedule create_ddpm_v22 computes (diffusers_compat.check_scheduler_config): the released folders' file
+        lacks variance_type and clip_sample_range and is refused (DESIGN.md section 7, the scheduler finding)."""
+        from .diffusers_compat import read_decoder_folder
+        config, task_type, unet_sd, movq_sd = read_decoder_folder(os.fspath(decoder_dir))
+        if isinstance(prior, (str, os.PathLike)):
+            from .model.prior import PriorEmbedder22
+            prior = PriorEmbedder22.from_pretrained(os.fspath(prior), device=device)
+        return cls(config, device, task_type=task_type, embedder=prior, unet_state_dict=unet_sd, movq_state_dict=movq_sd,
+                   depth_estimator=depth_estimator)
 
     def get_new_h_w(self, h, w):  # kandinsky2_2_model.py:46-53 (pixels)
         return math.ceil(h / 64) * 64, math.ceil(w / 64) * 64

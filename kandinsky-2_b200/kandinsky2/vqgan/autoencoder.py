@@ -171,6 +171,29 @@ class MOVQ(nn.Module):
         self._packed, self._plans = None, {}
         return super().load_state_dict(sd, strict=strict, assign=assign)
 
+    @classmethod
+    def from_diffusers(cls, state_dict, config, device="cuda", param_dtype=torch.float16):
+        """From a diffusers `VQModel` state dict and its config.json dict (norm_type "spatial": the Kandinsky 2.2 decoder
+        folders' `movq/`), through diffusers_compat.movq_config and checkpoints.diffusers_movq_to_k2; the weights are cast to
+        param_dtype (fp16, the dtype the 2.2 pipelines load the MoVQ in).  The 2.2 pipelines' movq.decode(latents,
+        force_not_quantize=True) is decode here, and movq.encode(x).latents is encode."""
+        from ..checkpoints import diffusers_movq_to_k2
+        from ..diffusers_compat import movq_config
+        dd, n_embed, embed_dim = movq_config(config)
+        m = cls(dd, n_embed, embed_dim, device=device, param_dtype=param_dtype)
+        m.load_state_dict(diffusers_movq_to_k2(state_dict, dd))
+        return m
+
+    @classmethod
+    def from_pretrained(cls, path, device="cuda", param_dtype=torch.float16):
+        """A local diffusers `VQModel` folder (e.g. the `movq/` of kandinsky-2-2-decoder): config.json and
+        diffusion_pytorch_model{,.fp16}.{safetensors,bin}.  A missing file raises K2Error naming it."""
+        from ..checkpoints import load_weights, read_json
+        from ..diffusers_compat import WEIGHT_FILES
+        what = "MOVQ.from_pretrained"
+        config = read_json(path, "config.json", what)
+        return cls.from_diffusers(load_weights(path, WEIGHT_FILES, what), config, device, param_dtype)
+
     def _apply(self, fn, recurse=True):
         self._packed, self._plans = None, {}
         return super()._apply(fn, recurse)
