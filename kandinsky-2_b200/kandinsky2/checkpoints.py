@@ -38,7 +38,8 @@
   transposes) stay at its call site.  `read_json` and `load_weights` read the component folders the towers load from.
 
 * `lora_to_k2` maps a decoder LoRA in diffusers' attention-processor format onto low-rank factors of the packed
-  qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`).
+  qkv / encoder_kv / proj_out weights (merged on the GPU by `Text2ImUNet.load_lora`); `prior_lora_to_k2` does the same for
+  an adapter of the 2.2 prior's self-attention, onto its c_qkv / c_proj (merged by `PriorTransformer.load_lora`).
 
 * Kandinsky 2.2 ships its MoVQ as a diffusers `VQModel` with `norm_type="spatial"` (the decoder folders' `movq/`).  It is the
   reference's MOVQ under other names: `diffusers_movq_to_k2` renames it into `vqgan.autoencoder.MOVQ` names and turns the
@@ -199,6 +200,63 @@ _LORA_KEY = re.compile(r"^(.+)\.processor\.(to_q|to_k|to_v|to_out|add_k_proj|add
 _LORA_TARGETS = {"qkv": ("to_q", "to_k", "to_v"), "encoder_kv": ("add_k_proj", "add_v_proj"), "proj_out": ("to_out",)}
 
 
+def _read_lora(lora, rx, dims, what):
+    """The factors of an adapter in diffusers' attention-processor form -> {(attention prefix, projection): {"down": fp32 [r, K],
+    "up": fp32 [C, r]}} on the CPU.  rx matches a key into (attention prefix, projection, "down" | "up"); dims(prefix,
+    projection) is (C, K), the projection's output rows and fan-in, or None for a prefix the model does not have.  Raises
+    K2Error naming the first offending key for: PEFT (lora_A / lora_B) or alpha entries, unknown keys, non-floating or non-2-D
+    tensors, a factor without its partner, rank or shape mismatches.  `what` names the model in the unknown-key message."""
+    found = {}
+    for key, t in lora.items():
+        if "lora_A" in key or "lora_B" in key:
+            raise K2Error(f"LoRA key {key!r}: PEFT-format (lora_A / lora_B) adapters are not supported")
+        if "alpha" in key.rsplit(".", 1)[-1]:
+            raise K2Error(f"LoRA key {key!r}: alpha / network_alpha scaling is not supported")
+        m = rx.match(key)
+        if m is None or dims(m.group(1), m.group(2)) is None:
+            raise K2Error(f"LoRA key {key!r} is not an attention-processor LoRA weight of {what}")
+        if not torch.is_tensor(t) or t.dtype not in (torch.float16, torch.bfloat16, torch.float32) or t.dim() != 2:
+            raise K2Error(f"LoRA key {key!r}: expected a 2-D fp16, bf16 or fp32 tensor")
+        found.setdefault((m.group(1), m.group(2)), {})[m.group(3)] = t.detach().to("cpu", torch.float32)
+    for key in lora:
+        dp, proj, which = rx.match(key).groups()
+        pair = found[(dp, proj)]
+        other = "up" if which == "down" else "down"
+        if other not in pair:
+            raise K2Error(f"LoRA key {key!r} has no matching {other} weight")
+        down, up = pair["down"], pair["up"]
+        C, fan_in = dims(dp, proj)
+        if up.shape[1] != down.shape[0]:
+            raise K2Error(f"LoRA key {key!r}: rank mismatch between down {tuple(down.shape)} and up {tuple(up.shape)}")
+        if down.shape[1] != fan_in or up.shape[0] != C:
+            raise K2Error(f"LoRA key {key!r}: expected down [rank, {fan_in}] and up [{C}, rank], got down "
+                          f"{tuple(down.shape)} and up {tuple(up.shape)}")
+    return found
+
+
+def _lora_factors(pairs, projs, C, head_dim):
+    """(up', down') of one packed weight whose rows are the projections `projs` (each C rows; head-interleaved by pack_heads
+    when there are several), from pairs {projection: {"down", "up"}} of the present ones, or None when none is present.
+    down' stacks the present projections' down matrices and up' is block-diagonal (zeros elsewhere), so up' @ down' packs the
+    per-projection deltas up @ down -- the zero terms add exact zeros, so each element's fp32 sum equals that of its own
+    projection.  A missing projection has no delta."""
+    present = [p for p in projs if p in pairs]
+    if not present:
+        return None
+    downs = [pairs[p]["down"] for p in present]
+    R = sum(d.shape[0] for d in downs)
+    ups, col = [], 0
+    for p in projs:
+        u = torch.zeros(C, R)
+        if p in pairs:
+            r = pairs[p]["down"].shape[0]
+            u[:, col:col + r] = pairs[p]["up"]
+            col += r
+        ups.append(u)
+    up = pack_heads(ups, head_dim) if len(projs) > 1 else ups[0]
+    return up.contiguous(), torch.cat(downs, 0).contiguous()
+
+
 def lora_to_k2(lora, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4), num_res_blocks=3, attention_ds=(2, 4, 8),
                model_dim=768, head_dim=64):
     """A LoRA adapter of the decoder UNet in diffusers' attention-processor form -- the keys `AttnProcsLayers` /
@@ -208,9 +266,7 @@ def lora_to_k2(lora, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4
     keyed like the output of diffusers_unet_to_k2 (`middle_block.1.qkv.weight`, `.encoder_kv.weight`, `.proj_out.weight`).
 
     The delta of a projection is up @ down (diffusers' LoRALinearLayer without network_alpha), so
-    up' @ down' = diffusers_unet_to_k2 of the per-projection deltas: for qkv / encoder_kv, down' stacks the present projections'
-    down matrices and up' is block-diagonal (zeros elsewhere) with its rows head-interleaved by pack_heads -- the zero terms
-    add exact zeros, so each element's fp32 sum equals that of its own projection.  A missing projection has no delta.
+    up' @ down' = diffusers_unet_to_k2 of the per-projection deltas (_lora_factors).  A missing projection has no delta.
     Raises K2Error naming the first offending key for anything else: unknown keys, PEFT (lora_A / lora_B) or alpha entries,
     a factor without its partner, rank or shape mismatches, non-floating tensors."""
     inp, mid, out = _topology(in_channels, model_channels, channel_mult, num_res_blocks, attention_ds)
@@ -218,50 +274,45 @@ def lora_to_k2(lora, in_channels=4, model_channels=384, channel_mult=(1, 2, 3, 4
     prefixes = [(dp, kp) for dp, kp, kind in unet_block_map(in_channels, model_channels, channel_mult, num_res_blocks,
                                                              attention_ds) if kind == "attn"]
     blocks = {dp: (kp, c) for (dp, kp), c in zip(prefixes, chans)}  # both lists are in the reference's block order
-    found = {}  # (diffusers prefix, projection) -> {"down": fp32 tensor, "up": fp32 tensor}
-    for key, t in lora.items():
-        if "lora_A" in key or "lora_B" in key:
-            raise K2Error(f"LoRA key {key!r}: PEFT-format (lora_A / lora_B) adapters are not supported")
-        if "alpha" in key.rsplit(".", 1)[-1]:
-            raise K2Error(f"LoRA key {key!r}: alpha / network_alpha scaling is not supported")
-        m = _LORA_KEY.match(key)
-        if m is None or m.group(1) not in blocks:
-            raise K2Error(f"LoRA key {key!r} is not an attention-processor LoRA weight of this UNet")
-        if not torch.is_tensor(t) or t.dtype not in (torch.float16, torch.bfloat16, torch.float32) or t.dim() != 2:
-            raise K2Error(f"LoRA key {key!r}: expected a 2-D fp16, bf16 or fp32 tensor")
-        found.setdefault((m.group(1), m.group(2)), {})[m.group(3)] = t.detach().to("cpu", torch.float32)
-    for key in lora:
-        dp, proj, which = _LORA_KEY.match(key).groups()
-        pair = found[(dp, proj)]
-        other = "up" if which == "down" else "down"
-        if other not in pair:
-            raise K2Error(f"LoRA key {key!r} has no matching {other} weight")
-        down, up = pair["down"], pair["up"]
+
+    def dims(dp, proj):
+        if dp not in blocks:
+            return None
         C = blocks[dp][1]
-        fan_in = model_dim if proj.startswith("add_") else C
-        if up.shape[1] != down.shape[0]:
-            raise K2Error(f"LoRA key {key!r}: rank mismatch between down {tuple(down.shape)} and up {tuple(up.shape)}")
-        if down.shape[1] != fan_in or up.shape[0] != C:
-            raise K2Error(f"LoRA key {key!r}: expected down [rank, {fan_in}] and up [{C}, rank], got down "
-                          f"{tuple(down.shape)} and up {tuple(up.shape)}")
+        return C, model_dim if proj.startswith("add_") else C
+
+    found = _read_lora(lora, _LORA_KEY, dims, "this UNet")
     packed = {}
     for dp, (kp, C) in blocks.items():
         for target, projs in _LORA_TARGETS.items():
-            present = [p for p in projs if (dp, p) in found]
-            if not present:
-                continue
-            downs = [found[(dp, p)]["down"] for p in present]
-            R = sum(d.shape[0] for d in downs)
-            ups, col = [], 0
-            for p in projs:
-                u = torch.zeros(C, R)
-                if (dp, p) in found:
-                    r = found[(dp, p)]["down"].shape[0]
-                    u[:, col:col + r] = found[(dp, p)]["up"]
-                    col += r
-                ups.append(u)
-            up = pack_heads(ups, head_dim) if len(projs) > 1 else ups[0]
-            packed[f"{kp}.{target}.weight"] = (up.contiguous(), torch.cat(downs, 0).contiguous())
+            f = _lora_factors({p: found[(dp, p)] for p in projs if (dp, p) in found}, projs, C, head_dim)
+            if f is not None:
+                packed[f"{kp}.{target}.weight"] = f
+    return packed
+
+
+_PRIOR_LORA_KEY = re.compile(r"^(transformer_blocks\.\d+\.attn1)\.processor\.(to_q|to_k|to_v|to_out)_lora\.(down|up)\.weight$")
+# packed prior weight -> the projections that feed it, in pack_heads order
+_PRIOR_LORA_TARGETS = {"attn.c_qkv": ("to_q", "to_k", "to_v"), "attn.c_proj": ("to_out",)}
+
+
+def prior_lora_to_k2(lora, width, layers, head_dim=64):
+    """A LoRA adapter of the Kandinsky 2.2 diffusion prior in diffusers' attention-processor form -- the keys `AttnProcsLayers`
+    writes for `LoRAAttnProcessor` on the prior's self-attention:
+        transformer_blocks.{i}.attn1.processor.{to_q,to_k,to_v,to_out}_lora.{down,up}.weight,  down [r, width], up [width, r]
+    -> {packed weight key: (up', down')}, fp32, keyed like the output of diffusers_prior_to_k2
+    (`transformer.resblocks.{i}.attn.c_qkv.weight`, `.attn.c_proj.weight`).  to_q / to_k / to_v become one pair with rows
+    head-interleaved like c_qkv (_lora_factors), to_out the pair of c_proj.  Any subset of the projections may be present; a
+    missing one has no delta.  The rank is read from the tensors.  Raises K2Error naming the first offending key as
+    lora_to_k2 does, layer indices outside [0, layers) included."""
+    blocks = {f"transformer_blocks.{i}.attn1": i for i in range(layers)}
+    found = _read_lora(lora, _PRIOR_LORA_KEY, lambda dp, proj: (width, width) if dp in blocks else None, "this prior")
+    packed = {}
+    for dp, i in blocks.items():
+        for target, projs in _PRIOR_LORA_TARGETS.items():
+            f = _lora_factors({p: found[(dp, p)] for p in projs if (dp, p) in found}, projs, width, head_dim)
+            if f is not None:
+                packed[f"transformer.resblocks.{i}.{target}.weight"] = f
     return packed
 
 

@@ -19,6 +19,9 @@ Kandinsky 2.2 runs the same network at CLIP-bigG width (clip_dim = clip_xf_width
 (checkpoints.diffusers_prior_to_k2).  Its sampler is diffusers' UnCLIPScheduler (UnCLIPSchedule, restated), and each sampling
 step is one CUDA graph replay of _PriorStepPlan, whose model output equals `forward` bit for bit under the same GEMM
 configurations; PriorEmbedder22 puts it behind the embedder protocol (tests/test_gpu_zz_prior22.py, DESIGN.md section 7).
+PriorTransformer.load_lora merges a diffusers attention-processor LoRA of the self-attention into the packed attn.qkv /
+attn.proj in place (checkpoints.prior_lora_to_k2, k2_lora_merge), so the step graphs stay as they are
+(tests/test_gpu_zz_prior_lora.py).
 """
 import math
 import os
@@ -92,6 +95,8 @@ class PriorTransformer(nn.Module):
             self.final_ln = None
         self._packed = None
         self._step_plans = {}
+        self._lora = None        # (factors from checkpoints.prior_lora_to_k2, scale) of the loaded adapter
+        self._lora_base = None   # device copies of the unmerged packed attn.qkv / attn.proj while an adapter is merged
 
     def finalize(self):
         """Pack the GEMM weights (fp16 [N, K], K padded to 64) once per checkpoint, the blocks' with their LayerNorm parameters
@@ -104,7 +109,57 @@ class PriorTransformer(nn.Module):
         self._packed = {"layers": pack_layers(get, self.xf_layers, te.weight.device),
                         "text_enc": (ops.pack_conv_weight(te.weight), te.bias.float().contiguous())}
         self._step_plans = {}
+        self._lora_base = None
+        if self._lora is not None:  # a loaded adapter survives re-packing
+            self._merge_lora()
         return self
+
+    # ---------------------------------------------------------------- LoRA adapters, merged into the packed weights
+    _LORA_WEIGHTS = (("attn.qkv", "attn.c_qkv"), ("attn.proj", "attn.c_proj"))
+
+    @property
+    def lora_scale(self):
+        """Scale of the loaded LoRA adapter, None when there is none."""
+        return None if self._lora is None else self._lora[1]
+
+    def load_lora(self, state_dict, scale=1.0):
+        """Merge a LoRA adapter of the self-attention -- diffusers' `LoRAAttnProcessor` weights as `AttnProcsLayers` writes
+        them for the 2.2 prior (checkpoints.prior_lora_to_k2) -- into the packed weights: W = W_base + scale * up @ down,
+        computed by k2_lora_merge in fp32 and rounded once to fp16, two launches per layer (attn.qkv, attn.proj).  The merge
+        writes the packed tensors in place, so captured step graphs keep their addresses and need no rebuild.  On first use the
+        unmerged packed weights are copied on the device (restored by unload_lora).  Loading again replaces the adapter
+        (adapters do not stack; a new scale means loading again).  state_dict() never changes."""
+        from ..checkpoints import prior_lora_to_k2
+        factors = prior_lora_to_k2(state_dict, self.xf_width, self.xf_layers)
+        if not self.text_enc_proj.weight.is_cuda:
+            raise K2Error("k2b200 prior: load_lora merges on the GPU; the prior is not on a CUDA device (no CPU fallback)")
+        if self._packed is None:
+            self.finalize()
+        self._lora = (factors, float(scale))
+        self._merge_lora()
+
+    def unload_lora(self):
+        """Restore the unmerged packed weights (bit-exact) and free their copy."""
+        if self._lora_base is not None and self._packed is not None:
+            for L, base in zip(self._packed["layers"], self._lora_base):
+                for name, _ in self._LORA_WEIGHTS:
+                    L[name][0].copy_(base[name])
+        self._lora = None
+        self._lora_base = None
+
+    def _merge_lora(self):
+        factors, scale = self._lora
+        layers = self._packed["layers"]
+        if self._lora_base is None:
+            self._lora_base = [{name: L[name][0].clone() for name, _ in self._LORA_WEIGHTS} for L in layers]
+        for i, (L, base) in enumerate(zip(layers, self._lora_base)):
+            for name, target in self._LORA_WEIGHTS:
+                f = factors.get(f"transformer.resblocks.{i}.{target}.weight")
+                if f is None:
+                    L[name][0].copy_(base[name])
+                else:
+                    up, down = (t.to(base[name].device) for t in f)
+                    ops.lora_merge(base[name], up, down, scale, out=L[name][0])
 
     def _step_plan(self, B):
         """The UnCLIP sampling step at B samples (2B CFG rows) as a static launch list (_PriorStepPlan), built once per B."""
