@@ -288,6 +288,24 @@ int k2_unipc_step(const float* model_out, int C2, float* x, float* last, float* 
                   const int* counter, int B, int H, int W, float guidance, int cond_first, const float* inpaint_init,
                   const float* inpaint_mask, const float* inpaint_noise, k2_stream_t stream);
 
+/* Heun step (Karras et al. 2022, Algorithm 1 with s_churn = 0, as diffusers' HeunDiscreteScheduler runs it): one of the two
+ * stages of a step per UNet evaluation, CFG closure fused.  x fp32 [B, 4, H, W] (in place) is the latent in the UNet's input
+ * scale, x_ve / sqrt(sigma^2 + 1) with sigma the VE sigma; r = coef, device fp32[8] = {1/alpha, sigma, 1/sigma, c_x, c_d,
+ * alpha', sigma'_vp, stage} (kandinsky2/model/gaussian_diffusion.py: HeunSchedule), staged by k2_step_begin from the step
+ * counter.  Per element:
+ *   eps  = uncond + g (cond - uncond) as in k2_dpm_solver_step;   d = eps  (the VE derivative (x_ve - x0) / sigma);
+ *   d   += r[2] mask (r[0] x - r[1] eps - init)   if inpaint_mask != NULL and inpaint_noise == NULL (2.1: the known region
+ *          replaces the x0 prediction);
+ *   stage 1 (r[7] == 0):  x_prev = x;  d_prev = d;  x' = r[3] x + r[4] d        (the Euler predictor; also the last step);
+ *   stage 2 (r[7] != 0):  x' = r[3] x_prev + r[4] (d_prev + d)                  (the trapezoidal corrector);
+ *   x'   = mask (r[5] init + r[6] inpaint_noise) + (1 - mask) x'   if inpaint_noise != NULL (2.2, after both stages).
+ * x_prev and d_prev (fp32 [B, 4, H, W], owned by the caller's step state) are not read by stage 1, so whatever they hold
+ * (even NaN) cannot reach its result; stage 2 does not write them, and reads x only for the 2.1 blend.  Arguments are checked
+ * before any CUDA call. */
+int k2_heun_step(const float* model_out, int C2, float* x, float* x_prev, float* d_prev, const float* coef, int B, int H, int W,
+                 float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
+                 const float* inpaint_noise, k2_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * MoVQ helpers: nearest-codebook search (quntize.py:89-98; fp32, ties -> lowest index, int64 out),
  * fp32 NCHW -> NHWC transposes for the 4-channel latent, final image quantisation

@@ -518,6 +518,54 @@ __global__ void __launch_bounds__(256) unipc_step_kernel(const UniPCParams p) {
   p.x[i] = xn;
 }
 
+// Heun step (Karras et al. 2022, Algorithm 1 with s_churn = 0; diffusers' HeunDiscreteScheduler), one of its two stages per
+// UNet evaluation, on the latent kept in the UNet's input scale x = x_ve / sqrt(sigma^2 + 1):
+//   d  = eps                                                        (the VE derivative (x_ve - D) / sigma)
+//   d += r[2] m (D - init),  D = r[0] x - r[1] eps                  (2.1 inpainting only: the known region replaces D)
+//   stage 1 (r[7] == 0):  xs = x;  ds = d;  x' = r[3] x + r[4] d    (the Euler predictor, or the plain last step)
+//   stage 2 (r[7] != 0):  x' = r[3] xs + r[4] (ds + d)              (xs, ds: the pre-step latent and d of stage 1)
+// r = {1/alpha, sigma, 1/sigma, c_x, c_d, alpha', sigma'_vp, stage}; HeunSchedule builds the rows.  Stage 1 only writes xs and
+// ds; stage 2 reads them and x only for the 2.1 blend.
+struct HeunParams {
+  const float* model_out;  // [2B, C2, H, W], eps = channels [0, 4)
+  float* x;                // [B, 4, H, W], in place
+  float* xs;               // [B, 4, H, W]: the pre-step latent (stage 1 out, stage 2 in)
+  float* ds;               // [B, 4, H, W]: stage 1's derivative (stage 1 out, stage 2 in)
+  const float* coef;       // device [8]
+  int B, HW, C2;
+  float guidance;
+  int cond_first;
+  const float* init;       // [B,4,H,W] or null
+  const float* mask;       // [B,1,H,W] or null
+  const float* rnoise;     // [B,4,H,W] or null (2.2 inpainting: the known region of x' is re-noised to the next sigma)
+};
+
+__global__ void __launch_bounds__(256) heun_step_kernel(const HeunParams p) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  pdl_wait();
+  pdl_launch();
+  const long long total = static_cast<long long>(p.B) * 4 * p.HW;
+  if (i >= total) return;
+  const float* r = p.coef;
+  const bool second = r[7] != 0.f;
+  const bool replace_d = p.mask && !p.rnoise;
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, p.guidance, p.cond_first);
+  const float m = p.mask ? p.mask[static_cast<long long>(e.b) * p.HW + e.sp] : 0.f;
+  const float xv = (!second || replace_d) ? p.x[i] : 0.f;
+  float d = e.eps;
+  if (replace_d) d = fmaf(r[2] * m, (r[0] * xv - r[1] * e.eps) - p.init[i], d);
+  float xn;
+  if (second) {
+    xn = r[3] * p.xs[i] + r[4] * (p.ds[i] + d);
+  } else {
+    xn = r[3] * xv + r[4] * d;
+    p.xs[i] = xv;
+    p.ds[i] = d;
+  }
+  if (p.mask && p.rnoise) xn = m * (r[5] * p.init[i] + r[6] * p.rnoise[i]) + (1.f - m) * xn;
+  p.x[i] = xn;
+}
+
 // ------------------------------------------------------------------------------------------------
 // MoVQ helpers
 // ------------------------------------------------------------------------------------------------
@@ -972,6 +1020,23 @@ int k2_unipc_step(const float* model_out, int C2, float* x, float* last, float* 
   p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
   const long long total = static_cast<long long>(B) * 4 * H * W;
   K2_CHECK_CUDA(launch_k(unipc_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p));
+  count_launch();
+  return 0;
+}
+
+int k2_heun_step(const float* model_out, int C2, float* x, float* x_prev, float* d_prev, const float* coef, int B, int H, int W,
+                 float guidance, int cond_first, const float* inpaint_init, const float* inpaint_mask,
+                 const float* inpaint_noise, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && x_prev && d_prev && coef, "heun_step: null pointer");
+  K2_REQUIRE(B > 0 && H > 0 && W > 0 && C2 >= 4, "heun_step: B, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE((inpaint_init == nullptr) == (inpaint_mask == nullptr), "heun_step: init and mask go together");
+  K2_REQUIRE(inpaint_noise == nullptr || inpaint_init, "heun_step: inpaint_noise without init / mask");
+  HeunParams p;
+  p.model_out = model_out; p.x = x; p.xs = x_prev; p.ds = d_prev; p.coef = coef;
+  p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
+  p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
+  const long long total = static_cast<long long>(B) * 4 * H * W;
+  K2_CHECK_CUDA(launch_k(heun_step_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p));
   count_launch();
   return 0;
 }

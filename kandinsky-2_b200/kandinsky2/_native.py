@@ -77,6 +77,7 @@ SIGNATURES = {
     "k2_dpm_solver_step": (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
     "k2_dpm_solver_sde_step": (_I, [_P, _I, _P, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
     "k2_unipc_step": (_I, [_P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
+    "k2_heun_step": (_I, [_P, _I, _P, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
     "k2_vq_argmin": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "k2_pointwise_nchw_f32": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "k2_nchw_to_nhwc_f32": (_I, [_P, _P, _I, _I, _I, _I, _P]),

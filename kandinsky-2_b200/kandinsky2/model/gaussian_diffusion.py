@@ -164,6 +164,8 @@ class _SolverSchedule(_Schedule):
     k = k0 .. N-1."""
 
     SPACINGS = ("linspace", "karras")
+    # what a full run's start latent is, in units of the unit Gaussian noise it is drawn from (see _SigmaSchedule)
+    init_noise_scale = 1.0
 
     def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace"):
         ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
@@ -175,13 +177,16 @@ class _SolverSchedule(_Schedule):
         keep = n if keep is None else int(keep)
         if not 1 <= keep <= n:
             raise ValueError(f"{self.SOLVER}: keep must be in [1, {n}], got {keep}")
-        tau, alphas, sigmas = _solver_grid(self.SOLVER, ac, n, spacing)
+        tau, alphas, sigmas = self._grid(ac, n, spacing)
         self.num_steps, self.k0, self.spacing = n, n - keep, spacing
         self.timesteps = tau
         self.alphas = np.append(alphas, 1.0)    # alpha_0 .. alpha_N
         self.sigmas = np.append(sigmas, 0.0)
         self.num_timesteps = keep
         self._dev_tables = {}
+
+    def _grid(self, ac, n, spacing):
+        return _solver_grid(self.SOLVER, ac, n, spacing)
 
     def coef_table(self):
         """float32 [keep, row width]: the step kernel's rows, built in float64 (coef_rows) and cast once."""
@@ -382,6 +387,132 @@ class UniPCSchedule(_SolverSchedule):
         return np.ascontiguousarray(unipc_rows(self.alphas, self.sigmas, first=self.k0)[::-1])
 
 
+def sigma_grid(base_alphas_cumprod, n, spacing):
+    """(model timesteps [n], VE sigmas [n]) of diffusers' EulerDiscreteScheduler / HeunDiscreteScheduler with
+    timestep_spacing="linspace" over a base table, both decreasing.  linspace: t = linspace(0, T-1, n) reversed, fractional, and
+    sigma(t) interpolated linearly in the table's VE sigma s^(t) = sqrt((1 - ac_t) / ac_t); karras (use_karras_sigmas): the
+    Karras grid of karras_timesteps, from s^(T-1) to s^(0), at the timesteps that interpolate log s^ (diffusers' _sigma_to_t).
+    For n = 1 the linspace grid is t = 0 alone, as in diffusers; karras_timesteps then gives s^(T-1)."""
+    ac = np.asarray(base_alphas_cumprod, dtype=np.float64)
+    if spacing == "karras":
+        return karras_timesteps(ac, n)
+    t = np.linspace(0, len(ac) - 1, n)[::-1].copy()
+    return t, np.interp(t, np.arange(len(ac), dtype=np.float64), np.sqrt((1.0 - ac) / ac))
+
+
+class _SigmaSchedule(_SolverSchedule):
+    """The sigma-space samplers of diffusers (Karras et al. 2022, "Elucidating the Design Space of Diffusion-Based Generative
+    Models"): the variance-exploding ODE x_ve = x0 + sigma eps in the VE sigma of the base table, epsilon prediction,
+    s_churn = 0, on sigma_grid's N evaluations and sigma_N = 0.
+
+    diffusers scales the UNet input by scale_model_input, x_ve / sqrt(sigma^2 + 1).  Here the latent is kept in that scale,
+    x = alpha x_ve with alpha = 1 / sqrt(1 + sigma^2), which is the VP form x = alpha x0 + sigma_vp eps (sigma_vp = sigma
+    alpha) of the other solvers: k2_step_begin hands it to the UNet unchanged, the rows carry the scale from one sigma to the
+    next, and after the last step (alpha = 1) it is x_ve itself.  self.alphas / self.sigmas are alpha and sigma_vp
+    (_SolverSchedule), self.ve_sigmas the VE sigmas [N + 1].
+
+    Start: a full run starts from init_noise_scale * z = sigma_vp_0 z, diffusers' init_noise_sigma z (= sigma_0 z in VE, the
+    rule of timestep_spacing "linspace" for both spacings) in the UNet's scale.  img2img (keep = s) starts from
+    start_latent = alpha_k0 latent + sigma_vp_k0 noise, diffusers' add_noise(latent, noise) = latent + sigma_k0 noise at the
+    first kept step, in the same scale.  2.2 inpainting: the known region after a step is the clean latent noised to the next
+    sigma with the run's unit start noise, alpha' init + sigma_vp' z; the rows hold sigma_vp' / init_noise_scale because the
+    kernels are handed the start latent init_noise_scale z.  (diffusers' KandinskyV22InpaintPipeline clones the start
+    latent after the init_noise_sigma scaling and passes it to add_noise, which for these schedulers multiplies the known
+    region's noise by sigma_0 as well; that is not restated.)"""
+
+    def _grid(self, ac, n, spacing):
+        tau, ve = sigma_grid(ac, n, spacing)
+        self.ve_sigmas = np.append(ve, 0.0)
+        alphas = 1.0 / np.sqrt(1.0 + ve ** 2)
+        return tau, alphas, ve * alphas
+
+    @property
+    def init_noise_scale(self):
+        return float(self.sigmas[0])
+
+
+class EulerSchedule(_SigmaSchedule):
+    """diffusers' EulerDiscreteScheduler (ancestral=False; use_karras_sigmas = spacing == "karras") and
+    EulerAncestralDiscreteScheduler (ancestral=True), one evaluation per step:
+        x_ve' = x_ve + (sigma_d - sigma) (x_ve - D) / sigma + sigma_up z,   D = x_ve - sigma eps,
+    sigma_d = sigma', sigma_up = 0 for Euler; sigma_up = sqrt(sigma'^2 (sigma^2 - sigma'^2) / sigma^2),
+    sigma_d = sqrt(sigma'^2 - sigma_up^2) for Euler ancestral, with one Gaussian draw z per step.  In the UNet's scale
+    (_SigmaSchedule) that is affine in (x, D, z), a row of k2_dpm_solver_step (k2_dpm_solver_sde_step when ancestral):
+        {1/alpha, sigma, alpha' sigma_d / (alpha sigma), alpha' (1 - sigma_d / sigma), 0, alpha', sigma_vp' / init_noise_scale,
+         alpha' sigma_up}.
+    Euler is DPM-Solver++ of order 1 (DDIM) on this grid.  The last step, to sigma = 0, lands on D."""
+
+    SOLVER = "Euler"
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace", ancestral=False):
+        super().__init__(base_alphas_cumprod, num_steps, keep=keep, spacing=spacing)
+        self.ancestral = self.draws_noise = bool(ancestral)
+        self.step_kind = "dpmpp_2m_sde" if self.ancestral else "dpmpp_2m"
+
+    def coef_rows(self):
+        """float64 [keep, 8]: the rows of steps k = N-1 .. k0 (table order)."""
+        a, s, ve, n, k0 = self.alphas, self.sigmas, self.ve_sigmas, self.num_steps, self.k0
+        rows = np.zeros((n, 8), dtype=np.float64)
+        for k in range(k0, n):
+            sig, nxt = ve[k], ve[k + 1]
+            down, up = nxt, 0.0
+            if self.ancestral:
+                up = np.sqrt(nxt ** 2 * (sig ** 2 - nxt ** 2) / sig ** 2)
+                down = np.sqrt(nxt ** 2 - up ** 2)
+            rows[k] = (1.0 / a[k], sig, a[k + 1] * down / (a[k] * sig), a[k + 1] * (1.0 - down / sig), 0.0, a[k + 1],
+                       s[k + 1] / s[0], a[k + 1] * up)
+        return np.ascontiguousarray(rows[k0:][::-1])
+
+
+class HeunSchedule(_SigmaSchedule):
+    """diffusers' HeunDiscreteScheduler (use_karras_sigmas = spacing == "karras"): Heun's method, two evaluations per step
+    except the last, which is a plain Euler step to sigma = 0 -- 2 keep - 1 evaluations, at the timesteps
+    t_k0, t_k0+1, t_k0+1, ..., t_N-1, t_N-1 (diffusers' interleaved list from index 2 k0, as img2img's get_timesteps cuts it
+    with the scheduler's order 2).  Step k, d = (x_ve - D) / sigma = eps (the derivative of the VE ODE):
+        stage 1 at sigma_k:        x_ve^p = x_ve + (sigma_k+1 - sigma_k) d_1          (the predictor)
+        stage 2 at sigma_k+1 > 0:  x_ve'  = x_ve + (sigma_k+1 - sigma_k) (d_1 + d_2) / 2
+    with x_ve and d_1 those of stage 1.  The old latent cannot be rebuilt from the predictor without dividing by alpha, so
+    k2_heun_step keeps x and d_1 in buffers of the step state.  One row of 8 floats per evaluation:
+        stage 1:  {1/alpha_k, sigma_k, 1/sigma_k, alpha_k+1 / alpha_k, alpha_k+1 (sigma_k+1 - sigma_k), alpha_k+1,
+                   sigma_vp_k+1 / init_noise_scale, 0}
+        stage 2:  {1/alpha_k+1, sigma_k+1, 1/sigma_k+1, alpha_k+1 / alpha_k, alpha_k+1 (sigma_k+1 - sigma_k) / 2, alpha_k+1,
+                   sigma_vp_k+1 / init_noise_scale, 1}
+    Columns 0-2 serve the 2.1 inpainting rule (the known region replaces D), 5-6 the 2.2 one, after each stage as diffusers'
+    pipeline blends after each scheduler.step."""
+
+    SOLVER = "Heun"
+    draws_noise = False
+    step_kind = "heun"
+
+    def __init__(self, base_alphas_cumprod, num_steps, keep=None, spacing="linspace"):
+        super().__init__(base_alphas_cumprod, num_steps, keep=keep, spacing=spacing)
+        self.num_timesteps = 2 * (self.num_steps - self.k0) - 1
+
+    def _evaluations(self):
+        """[(step k, stage 1 or 2)] in loop order."""
+        out = []
+        for k in range(self.k0, self.num_steps):
+            out.append((k, 1))
+            if k < self.num_steps - 1:
+                out.append((k, 2))
+        return out
+
+    def model_timesteps(self):
+        t = self.timesteps
+        return np.array([t[k] if st == 1 else t[k + 1] for k, st in self._evaluations()][::-1], dtype=np.float32)
+
+    def coef_rows(self):
+        """float64 [2 keep - 1, 8]: one row per evaluation, last evaluation first (table order)."""
+        a, s, ve = self.alphas, self.sigmas, self.ve_sigmas
+        rows = []
+        for k, stage in self._evaluations():
+            j = k if stage == 1 else k + 1                   # where the UNet runs
+            dt = a[k + 1] * (ve[k + 1] - ve[k])
+            rows.append((1.0 / a[j], ve[j], 1.0 / ve[j], a[k + 1] / a[k], dt if stage == 1 else 0.5 * dt, a[k + 1],
+                         s[k + 1] / s[0], float(stage - 1)))
+        return np.ascontiguousarray(np.array(rows, dtype=np.float64)[::-1])
+
+
 def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,
                    clip_range=1e30, threshold_mode=0, init_step=None, inpaint_init=None, inpaint_mask=None,
                    inpaint_renoise=False, step_noise=None, sample_generators=None, callback=None, progress=False):
@@ -571,9 +702,11 @@ class FusedStep:
     k2_dpm_solver_step with DPMSolverSchedule rows, on a history buffer (the previous step's x0) owned by the step state;
     "dpmpp_2m_sde" issues k2_dpm_solver_sde_step the same way, with this step's noise; "unipc" issues k2_unipc_step with
     UniPCSchedule's 16-float rows, which it reads from its own staged table by the step counter, on the last-sample and two-deep
-    D history buffers of the step state."""
+    D history buffers of the step state; "heun" issues k2_heun_step with HeunSchedule's rows (one per evaluation, staged like
+    the DPM rows) on the pre-step latent and derivative buffers of the step state.  EulerSchedule's rows run on the
+    "dpmpp_2m" / "dpmpp_2m_sde" kinds."""
 
-    STEP_KINDS = ("ddpm", "dpmpp_2m", "dpmpp_2m_sde", "unipc")
+    STEP_KINDS = ("ddpm", "dpmpp_2m", "dpmpp_2m_sde", "unipc", "heun")
 
     def __init__(self, model, B, H, W, model_kwargs, guidance_scale, cond_first, clip_range, threshold_mode,
                  inpaint_init=None, inpaint_mask=None, inpaint_noise=None, step_kind="ddpm"):
@@ -590,7 +723,7 @@ class FusedStep:
         self.B = B
         self.guidance, self.cond_first, self.clip, self.mode = guidance_scale, int(cond_first), clip_range, threshold_mode
         self.step_kind = step_kind
-        dpm = step_kind != "ddpm"
+        dpm = step_kind not in ("ddpm", "heun")   # the kinds with a D history
         has_inpaint = inpaint_init is not None
         # buffers and the captured step graph live on the plan, keyed by everything the graph bakes in as a kernel argument
         renoise = inpaint_noise is not None
@@ -609,6 +742,8 @@ class FusedStep:
             if step_kind == "unipc":
                 st.update(last=torch.zeros(B, 4, H, W, **f32), hist2=torch.zeros(B, 4, H, W, **f32),
                           coef16=torch.zeros(UNIPC_ROW, **f32), coef16_seq=torch.zeros(4096, UNIPC_ROW, **f32))
+            if step_kind == "heun":
+                st.update(heun_x=torch.zeros(B, 4, H, W, **f32), heun_d=torch.zeros(B, 4, H, W, **f32))
             states[key] = st
         self.st = st
         self.noise, self.coef, self.work = st["noise"], st["coef"], st["work"]
@@ -644,7 +779,7 @@ class FusedStep:
             st["noise_seq"][:n].copy_(noise_seq)
         self._use_noise_seq = noise_seq is not None
         st["counter"].copy_(torch.tensor([0, n], dtype=torch.int32))
-        for name in ("hist", "last", "hist2"):
+        for name in ("hist", "last", "hist2", "heun_x", "heun_d"):
             if st.get(name) is not None:
                 st[name].zero_()
 
@@ -656,6 +791,10 @@ class FusedStep:
             ops.unipc_step(self.plan.out, x, st["last"], st["hist"], st["hist2"], st["coef16_seq"] if scheduled else st["coef16"],
                            self.guidance, self.cond_first, counter=st["counter"] if scheduled else None,
                            inpaint_init=self.init, inpaint_mask=self.mask, inpaint_noise=self.rnoise)
+            return
+        if self.step_kind == "heun":
+            ops.heun_step(self.plan.out, x, self.st["heun_x"], self.st["heun_d"], self.coef, self.guidance, self.cond_first,
+                          self.init, self.mask, self.rnoise)
             return
         if self.step_kind != "ddpm":
             ops.dpm_solver_step(self.plan.out, x, self.st["hist"], self.coef, self.guidance, self.cond_first, self.init,

@@ -441,6 +441,22 @@ def unipc_step(model_out, x, last, hist1, hist2, coef, guidance, cond_first, cou
     return x
 
 
+def heun_step(model_out, x, x_prev, d_prev, coef, guidance, cond_first, inpaint_init=None, inpaint_mask=None,
+              inpaint_noise=None):
+    """k2_heun_step: x fp32 [B,4,H,W] (the latent in the UNet's input scale) -> the next Heun stage in place.  coef = device
+    fp32 [8] row of HeunSchedule; its stage column picks the predictor (stores x and d in x_prev / d_prev, which it does not
+    read) or the corrector (reads them); see k2b200.h."""
+    tensors = (model_out, x, x_prev, d_prev, coef, inpaint_init, inpaint_mask, inpaint_noise)
+    if not all(t is None or t.is_cuda for t in tensors):
+        raise nat.K2Error("heun_step: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    lib = nat.load()
+    B, _, H, W = x.shape
+    check(lib.k2_heun_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(x_prev), ptr(d_prev), ptr(coef), B, H, W,
+                           float(guidance), int(cond_first), ptr(inpaint_init), ptr(inpaint_mask), ptr(inpaint_noise),
+                           stream_ptr()))
+    return x
+
+
 def vq_argmin(z, codebook):
     """z fp32 [n, dim], codebook fp32 [n_embed, dim] -> int64 [n] (ties -> lowest index)."""
     lib = nat.load()

@@ -18,8 +18,8 @@ import torch
 
 from . import ops, parallel
 from ._native import K2Error
-from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, PLMSSampler, UniPCSchedule, create_ddpm_v22,
-                                       create_gaussian_diffusion)
+from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, EulerSchedule, HeunSchedule, PLMSSampler, UniPCSchedule,
+                                       create_ddpm_v22, create_gaussian_diffusion)
 from .model.model_creation import create_decoder_unet
 from .utils import prepare_image, prepare_mask, q_sample, uint8_to_pil
 from .vqgan import MOVQ
@@ -74,11 +74,19 @@ DPM_SAMPLERS = {"dpmpp_2m_sampler": ("linspace", False), "dpmpp_2m_karras_sample
                 "dpmpp_2m_sde_sampler": ("linspace", True), "dpmpp_2m_sde_karras_sampler": ("karras", True)}
 # UniPC sampler name -> timestep spacing of its UniPCSchedule
 UNIPC_SAMPLERS = {"unipc_sampler": "linspace", "unipc_karras_sampler": "karras"}
-# every multistep-solver sampler name -> (schedule class, its keyword arguments): the one table _decode and the img2img start use
+# every multistep-solver sampler name -> (schedule class, its keyword arguments)
 SOLVER_SAMPLERS = {**{name: (DPMSolverSchedule, dict(spacing=sp, sde=sde)) for name, (sp, sde) in DPM_SAMPLERS.items()},
                    **{name: (UniPCSchedule, dict(spacing=sp)) for name, sp in UNIPC_SAMPLERS.items()}}
-SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(SOLVER_SAMPLERS)
-SAMPLERS_22 = ("ddpm_sampler",) + tuple(SOLVER_SAMPLERS)
+# sigma-space sampler name (diffusers' Euler, Euler ancestral and Heun discrete schedulers) -> (schedule class, its keywords)
+SIGMA_SAMPLERS = {"euler_sampler": (EulerSchedule, dict(spacing="linspace")),
+                  "euler_karras_sampler": (EulerSchedule, dict(spacing="karras")),
+                  "euler_ancestral_sampler": (EulerSchedule, dict(spacing="linspace", ancestral=True)),
+                  "heun_sampler": (HeunSchedule, dict(spacing="linspace")),
+                  "heun_karras_sampler": (HeunSchedule, dict(spacing="karras"))}
+# every name that runs on a _SolverSchedule: the one table _decode and the img2img start use
+SCHEDULE_SAMPLERS = {**SOLVER_SAMPLERS, **SIGMA_SAMPLERS}
+SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(SCHEDULE_SAMPLERS)
+SAMPLERS_22 = ("ddpm_sampler",) + tuple(SCHEDULE_SAMPLERS)
 
 
 def _check_sampler(sampler, allowed):
@@ -88,13 +96,13 @@ def _check_sampler(sampler, allowed):
 
 def _dpm_keep(num_steps, strength):
     """img2img with DPM-Solver++ or UniPC (and the 2.2 DDPM sampler, as diffusers): the last int(N * strength) evaluations run
-    (at least 1)."""
+    (at least 1).  The sigma-space samplers keep as many steps (Heun: 2 keep - 1 evaluations)."""
     return max(min(int(num_steps * strength), num_steps), 1)
 
 
 def _solver_schedule(sampler, diffusion, num_steps, keep=None):
-    """The DPMSolverSchedule / UniPCSchedule of a SOLVER_SAMPLERS name over diffusion's base table."""
-    cls, kw = SOLVER_SAMPLERS[sampler]
+    """The schedule of a SCHEDULE_SAMPLERS name over diffusion's base table."""
+    cls, kw = SCHEDULE_SAMPLERS[sampler]
     return cls(diffusion.base_alphas_cumprod, num_steps, keep=keep, **kw)
 
 
@@ -154,8 +162,7 @@ class _DecoderBase:
         return torch.randn(latent.shape, generator=torch.Generator().manual_seed(self.base_seed)).to(self.device)
 
     def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler):
-        """DPM-Solver++ / UniPC img2img -> (start latent, evaluations kept): the image latent noised to the first kept
-        evaluation."""
+        """img2img of the solver samplers -> (start latent, steps kept): the image latent noised to the first kept step."""
         keep = _dpm_keep(num_steps, strength)
         sched = _solver_schedule(sampler, diffusion, num_steps, keep)
         return sched.start_latent(latent, self._img2img_noise(latent)), keep
@@ -192,8 +199,10 @@ class _DecoderBase:
             noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
         shape = (2 * B, 4, H, W)
         self.model.del_cache()
-        if sampler in SOLVER_SAMPLERS:
+        if sampler in SCHEDULE_SAMPLERS:
             sched = _solver_schedule(sampler, diffusion, num_steps, init_step)
+            if init_step is None and sched.init_noise_scale != 1.0:
+                noise = noise * sched.init_noise_scale   # a full sigma-space run starts from init_noise_sigma z (diffusers)
             samples = sched.sample(self.model, shape, noise=noise, model_kwargs=kw, device=self.device,
                                    guidance_scale=guidance_scale, cond_first=self.cond_first,
                                    sample_generators=self._generators(lo, hi) if sched.draws_noise else None, **blend)
@@ -227,8 +236,12 @@ class Kandinsky2_1(_DecoderBase):
         init_step = s only the last s of them run (img2img), starting from `noise`.  "dpmpp_2m_karras_sampler" places the
         evaluations with Karras sigma spacing, "dpmpp_2m_sde_sampler" / "dpmpp_2m_sde_karras_sampler" run the SDE variant
         (fresh noise every step, drawn per global sample index like p_sampler's).  "unipc_sampler" / "unipc_karras_sampler" run
-        UniPC (DPM-Solver++(2M) plus the UniC corrector, UniPCSchedule) over the same evaluations.  Inpainting: the known region
-        replaces x0 inside the step (p_sampler and the solver samplers; the reference's DDIM / PLMS paths have no such blend)."""
+        UniPC (DPM-Solver++(2M) plus the UniC corrector, UniPCSchedule) over the same evaluations.  "euler_sampler",
+        "euler_karras_sampler", "euler_ancestral_sampler", "heun_sampler" and "heun_karras_sampler" run diffusers' Euler, Euler
+        ancestral and Heun discrete schedulers (EulerSchedule, HeunSchedule: num_steps steps, Heun evaluates the UNet
+        2 num_steps - 1 times; `noise` is then unit noise, scaled to the first sigma unless init_step is given).  Inpainting:
+        the known region replaces x0 inside the step (p_sampler and the solver samplers; the reference's DDIM / PLMS paths have
+        no such blend)."""
         _check_sampler(sampler, SAMPLERS_21)
         full_emb, pooled_emb = self.embedder.text_emb(prompt, batch_size)
         cond = {"full_emb": full_emb.to(self.device), "pooled_emb": pooled_emb.to(self.device),
@@ -276,12 +289,12 @@ class Kandinsky2_1(_DecoderBase):
     def generate_img2img(self, prompt, pil_img, strength=0.7, num_steps=100, batch_size=1, guidance_scale=7, h=512,
                          w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25"):
         """kandinsky2_1_model.py:428-484: encode the image, noise it to step int(T*(1-strength)) and run the remaining steps.
-        With a dpmpp_2m or unipc sampler the last int(num_steps*strength) solver evaluations run (at least 1), from the image
-        noised to the first of them."""
+        With a dpmpp_2m, unipc, euler or heun sampler the last int(num_steps*strength) solver steps run (at least 1), from the
+        image noised to the first of them."""
         _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        if sampler in SOLVER_SAMPLERS:
+        if sampler in SCHEDULE_SAMPLERS:
             x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength, sampler)
         else:
             start_step = int(diffusion.num_timesteps * (1 - strength))
@@ -349,8 +362,9 @@ class Kandinsky2_2(_DecoderBase):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
         106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
         sampler="dpmpp_2m_sampler" (or its Karras / SDE variants, DPM_SAMPLERS): DPM-Solver++(2M) over `steps` evaluations of
-        the same base schedule instead, "unipc_sampler" / "unipc_karras_sampler" UniPC (init_step = the number of evaluations
-        kept for img2img); inpainting re-noises the known region to the next timestep."""
+        the same base schedule instead, "unipc_sampler" / "unipc_karras_sampler" UniPC, the euler / heun names (SIGMA_SAMPLERS)
+        diffusers' Euler, Euler ancestral and Heun schedulers (init_step = the number of steps kept for img2img); inpainting
+        re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}
         return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, create_ddpm_v22(steps), steps, guidance,
@@ -417,7 +431,7 @@ class Kandinsky2_2(_DecoderBase):
         """img2img of the 2.2 methods -> (start latent [1, 4, h, w], the init_step of _decode_loop): the solver samplers'
         _dpm_img2img_start, else diffusers' KandinskyV22Img2ImgPipeline rule -- the last int(steps * strength) DDPM timesteps
         (at least 1) run, from scheduler.add_noise of the image latent at the first of them."""
-        if sampler in SOLVER_SAMPLERS:
+        if sampler in SCHEDULE_SAMPLERS:
             return self._dpm_img2img_start(lat, diffusion, steps, strength, sampler)
         start = _dpm_keep(steps, strength)
         ac = float(diffusion.alphas_cumprod[start - 1])
