@@ -19,13 +19,22 @@ Terms that do not depend on the key, relative to sum_s p_s |v_s|:
                                 MMA's accumulation, l one rescale and BKV / 4 additions per thread, then 2 shuffles, 1 / l and
                                 the product -- fewer than Tkv + 16 roundings in total for BKV = 16 and 128.
 An absolute term: a weight in fp16's subnormal range is rounded to 2^-25 absolute, Tkv 2^-25 max|v| over all keys.
-The caller adds one fp16 ulp of the float64 result (`_ulp16`) for the final rounding."""
+The caller adds one fp16 ulp of the float64 result (`_ulp16`) for the final rounding.
+
+ref_attention_small / check_attention_small do the same for attention_small (csrc/k2_prior.cu), the masked and causal
+attention of the prior and the text towers, with that kernel's own allowance derived where it is computed."""
 import torch
 
-from tests.test_gpu_prior_kernels import _ulp16
-
 U = 2.0 ** -24
+INF = float("inf")
 CHUNK_ELEMS = 2 ** 24    # float64 elements of one [heads, query chunk, keys] intermediate: 128 MB, five alive at once
+
+
+def _ulp16(r):
+    """fp16 ulp at float64 values r: 2^(e - 10) for |r| in [2^e, 2^(e+1)), 2^-24 below 2^-14."""
+    a = r.abs()
+    e = torch.floor(torch.log2(torch.where(a > 0, a, torch.full_like(a, 2.0 ** -30)))).clamp(min=-14)
+    return torch.exp2(e - 10)
 
 
 def ref_attention(q, k, v, scale, chain=None):
@@ -86,3 +95,52 @@ def check_d64(out, qkv, enc, heads, what, scale=0.125):
         u, s = check(out[b].view(T, heads, 64), *ref_attention(q, k, v, scale), (what, b))
         ulps, share = max(ulps, u), max(share, s)
     return ulps, share
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# attention_small (csrc/k2_prior.cu): heads of 64, at most 128 tokens, keep mask and causal mask
+# ------------------------------------------------------------------------------------------------------------------------------
+def ref_attention_small(qkv, heads, keep, causal, scale):
+    """float64 QKVMultiheadAttention with the prior's additive mask (prior.py:92-103, 261-262): where(keep, 0, -inf) plus
+    triu(-inf, 1), added to q.k * scale.  Returns (out [B, T, heads*64], per-element error allowance from the kernel's fp32
+    arithmetic, see below)."""
+    B, T = qkv.shape[:2]
+    q, k, v = qkv.double().view(B, T, heads, 192).split(64, -1)
+    add = torch.zeros(B, 1, T, T, dtype=torch.float64, device=qkv.device)
+    if keep is not None:
+        add = add + torch.where(keep.bool(), 0.0, -INF).double()[:, None, None, :]
+    if causal:
+        add = add + torch.full((T, T), -INF, dtype=torch.float64, device=qkv.device).triu(1)
+    s = torch.einsum("bthc,bshc->bhts", q, k) * scale
+    p = torch.softmax(s + add, -1)
+    o = torch.einsum("bhts,bshc->bthc", p, v)
+    # First-order error of the kernel's fp32 evaluation.  A relative error eta_s of the unnormalised weight of key s moves
+    # the output by sum_s p_s eta_s (v_s - o), at most sum_s p_s eta_s (|v_s| + |o|), where eta_s is bounded by
+    #   2^-18 * scale * sum_c |q_c k_c|   the 64-term fp32 fma chain of the score (gamma_64 = 64 * 2^-24),
+    #   2^-22 * (|s| + |max|)             rounding of the scaled score, of s - max and of its product with log2(e),
+    #   2^-21                             ex2.approx behind __expf.
+    # The P.V chain over <= 128 keys, the sum of the weights and the final multiply by 1 / sum add 2^-16 of sum_s p_s |v_s|.
+    reach = torch.isfinite(add).expand(B, heads, T, T)
+    mx = torch.where(reach, s, -INF).amax(-1, keepdim=True)
+    mx = torch.where(torch.isfinite(mx), mx.abs(), 0.0)
+    eta = 2.0 ** -18 * scale * torch.einsum("bthc,bshc->bhts", q.abs(), k.abs()) + 2.0 ** -22 * (s.abs() + mx) + 2.0 ** -21
+    pe = torch.where(reach, p * eta, 0.0)
+    mag = torch.einsum("bhts,bshc->bthc", p, v.abs())
+    allow = torch.einsum("bhts,bshc->bthc", pe, v.abs()) + pe.sum(-1).transpose(1, 2)[..., None] * o.abs() + 2.0 ** -16 * mag
+    return o.reshape(B, T, heads * 64), allow.reshape(B, T, heads * 64)
+
+
+def check_attention_small(got, qkv, heads, keep, causal, scale, what):
+    ref, allow = ref_attention_small(qkv, heads, keep, causal, scale)
+    got = got.double()
+    dead = torch.isnan(ref)      # query rows that reach no key: NaN in torch, NaN in the kernel (the documented contract)
+    assert torch.equal(torch.isnan(got), dead), (what, "NaN rows differ", int(torch.isnan(got).sum()), int(dead.sum()))
+    r, g, a = ref[~dead], got[~dead], allow[~dead]
+    err = (g - r).abs()
+    bound = _ulp16(r) + a
+    bad = err > bound
+    assert not bad.any(), (what, int(bad.sum()), err[bad][:4].tolist(), r[bad][:4].tolist(), a[bad][:4].tolist())
+    if not r.numel():
+        return 0.0, 0.0
+    # worst error in ulps (large only where the output cancels to near zero), and the largest share of the bound used
+    return (err / _ulp16(r)).max().item(), (err / bound).max().item()
