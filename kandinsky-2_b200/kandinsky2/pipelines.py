@@ -69,22 +69,21 @@ def _new_h_w_latent_21(h, w):  # kandinsky2_1_model.py:106-113 (latent side, /8)
     return math.ceil(h / 64) * 8, math.ceil(w / 64) * 8
 
 
-# DPM-Solver++(2M) sampler name -> (timestep spacing, SDE variant) of its DPMSolverSchedule
-DPM_SAMPLERS = {"dpmpp_2m_sampler": ("linspace", False), "dpmpp_2m_karras_sampler": ("karras", False),
-                "dpmpp_2m_sde_sampler": ("linspace", True), "dpmpp_2m_sde_karras_sampler": ("karras", True)}
-# UniPC sampler name -> timestep spacing of its UniPCSchedule
-UNIPC_SAMPLERS = {"unipc_sampler": "linspace", "unipc_karras_sampler": "karras"}
-# every multistep-solver sampler name -> (schedule class, its keyword arguments)
-SOLVER_SAMPLERS = {**{name: (DPMSolverSchedule, dict(spacing=sp, sde=sde)) for name, (sp, sde) in DPM_SAMPLERS.items()},
-                   **{name: (UniPCSchedule, dict(spacing=sp)) for name, sp in UNIPC_SAMPLERS.items()}}
-# sigma-space sampler name (diffusers' Euler, Euler ancestral and Heun discrete schedulers) -> (schedule class, its keywords)
-SIGMA_SAMPLERS = {"euler_sampler": (EulerSchedule, dict(spacing="linspace")),
-                  "euler_karras_sampler": (EulerSchedule, dict(spacing="karras")),
-                  "euler_ancestral_sampler": (EulerSchedule, dict(spacing="linspace", ancestral=True)),
-                  "heun_sampler": (HeunSchedule, dict(spacing="linspace")),
-                  "heun_karras_sampler": (HeunSchedule, dict(spacing="karras"))}
-# every name that runs on a _SolverSchedule: the one table _decode and the img2img start use
-SCHEDULE_SAMPLERS = {**SOLVER_SAMPLERS, **SIGMA_SAMPLERS}
+# every sampler name that runs on a _SolverSchedule -> (schedule class, its keyword arguments): the one table _decode and
+# the img2img start use.  The euler / heun names are diffusers' Euler, Euler ancestral and Heun discrete schedulers.
+SCHEDULE_SAMPLERS = {
+    "dpmpp_2m_sampler": (DPMSolverSchedule, dict(spacing="linspace", sde=False)),
+    "dpmpp_2m_karras_sampler": (DPMSolverSchedule, dict(spacing="karras", sde=False)),
+    "dpmpp_2m_sde_sampler": (DPMSolverSchedule, dict(spacing="linspace", sde=True)),
+    "dpmpp_2m_sde_karras_sampler": (DPMSolverSchedule, dict(spacing="karras", sde=True)),
+    "unipc_sampler": (UniPCSchedule, dict(spacing="linspace")),
+    "unipc_karras_sampler": (UniPCSchedule, dict(spacing="karras")),
+    "euler_sampler": (EulerSchedule, dict(spacing="linspace")),
+    "euler_karras_sampler": (EulerSchedule, dict(spacing="karras")),
+    "euler_ancestral_sampler": (EulerSchedule, dict(spacing="linspace", ancestral=True)),
+    "heun_sampler": (HeunSchedule, dict(spacing="linspace")),
+    "heun_karras_sampler": (HeunSchedule, dict(spacing="karras")),
+}
 SAMPLERS_21 = ("p_sampler", "ddim_sampler", "plms_sampler") + tuple(SCHEDULE_SAMPLERS)
 SAMPLERS_22 = ("ddpm_sampler",) + tuple(SCHEDULE_SAMPLERS)
 
@@ -361,9 +360,9 @@ class Kandinsky2_2(_DecoderBase):
                      init_step=None, hint=None, sampler="ddpm_sampler"):
         """The body of diffusers KandinskyV22Pipeline.__call__ (reference call sites kandinsky2_2_model.py:78-80,
         106-111,138-141,168-172): uncond rows first, DDPM learned-range step, +-2 clip, no dynamic threshold.
-        sampler="dpmpp_2m_sampler" (or its Karras / SDE variants, DPM_SAMPLERS): DPM-Solver++(2M) over `steps` evaluations of
-        the same base schedule instead, "unipc_sampler" / "unipc_karras_sampler" UniPC, the euler / heun names (SIGMA_SAMPLERS)
-        diffusers' Euler, Euler ancestral and Heun schedulers (init_step = the number of steps kept for img2img); inpainting
+        sampler="dpmpp_2m_sampler" (or its Karras / SDE variants, SCHEDULE_SAMPLERS): DPM-Solver++(2M) over `steps` evaluations
+        of the same base schedule instead, "unipc_sampler" / "unipc_karras_sampler" UniPC, the euler / heun names diffusers'
+        Euler, Euler ancestral and Heun schedulers (init_step = the number of steps kept for img2img); inpainting
         re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}

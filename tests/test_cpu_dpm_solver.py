@@ -1,11 +1,9 @@
 """CPU: the DPM-Solver++(2M) sampler's host side -- DPMSolverSchedule's timestep grid and coefficient rows against the float64
 restatement of the paper (tests/dpm_oracle.py), second-order convergence on Gaussian data whose probability-flow ODE has a
-closed form, the argument checks of k2_dpm_solver_step, and the pipelines' sampler names."""
-import ctypes
-
+closed form.  The argument checks of k2_dpm_solver_step and the pipelines' sampler names are in
+tests/test_cpu_schedule_samplers.py."""
 import numpy as np
 import pytest
-import torch
 
 from tests import dpm_oracle as do
 
@@ -112,54 +110,3 @@ def test_sampler_schedule_approaches_the_flow_endpoint():
         out = do.apply_rows(sch.coef_rows()[::-1], eps, x)
         errs.append(np.abs(out - do.gaussian_flow(x, sch.alphas[0], sch.sigmas[0], 1.0, 0.0, MU, S)).max())
     assert errs[1] < errs[0] / 1.5, errs
-
-
-def test_dpm_solver_step_argument_errors_without_gpu():
-    """k2_dpm_solver_step checks its arguments before any CUDA call: < 0 and a message, also on a machine without a GPU."""
-    from kandinsky2 import _native
-    lib = _native.load()
-    p = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-    ok = [p, 8, p, p, p, 2, 4, 4, 4.0, 1, None, None, None]
-    cases = [({0: None}, "null pointer"), ({2: None}, "null pointer"), ({3: None}, "null pointer"), ({4: None}, "null pointer"),
-             ({1: 3}, "C2 >= 4"), ({5: 0}, "must be >= 1"), ({6: 0}, "must be >= 1"), ({7: -1}, "must be >= 1"),
-             ({10: p}, "init and mask go together"), ({11: p}, "init and mask go together"),
-             ({12: p}, "inpaint_noise without init")]
-    for change, msg in cases:
-        args = list(ok)
-        for i, v in change.items():
-            args[i] = v
-        assert lib.k2_dpm_solver_step(*args, None) < 0, change
-        assert msg in lib.k2_last_error().decode(), (change, lib.k2_last_error())
-
-
-def test_dpm_solver_step_without_gpu_raises():
-    from kandinsky2 import ops
-    from kandinsky2._native import K2Error
-    if torch.cuda.is_available():
-        pytest.skip("checks the CPU-only failure mode")
-    z = torch.zeros(1, 4, 8, 8)
-    with pytest.raises(K2Error):
-        ops.dpm_solver_step(torch.zeros(2, 8, 8, 8), z.clone(), z.clone(), torch.zeros(8), 4.0, True)
-
-
-def test_pipelines_reject_unknown_sampler_names():
-    """Both versions refuse an unknown sampler before doing any work (no GPU needed to see it)."""
-    from kandinsky2.pipelines import Kandinsky2_1, Kandinsky2_2
-    p21 = Kandinsky2_1.__new__(Kandinsky2_1)
-    for call in (lambda s: p21.generate_text2img("x", num_steps=4, sampler=s),
-                 lambda s: p21.mix_images(["a"], [1.0], num_steps=4, sampler=s),
-                 lambda s: p21.generate_img2img("x", None, num_steps=4, sampler=s),
-                 lambda s: p21.generate_inpainting("x", None, None, num_steps=4, sampler=s),
-                 lambda s: p21.generate_img("x", None, sampler=s)):
-        for bad in ("euler", "ddpm_sampler", "dpmpp_2m"):
-            with pytest.raises(ValueError):
-                call(bad)
-    p22 = Kandinsky2_2.__new__(Kandinsky2_2)
-    for call in (lambda s: p22.generate_text2img("x", sampler=s),
-                 lambda s: p22.mix_images(["a"], [1.0], sampler=s),
-                 lambda s: p22.generate_img2img("x", None, sampler=s),
-                 lambda s: p22.generate_inpainting("x", None, None, sampler=s),
-                 lambda s: p22.generate_controlnet("x", None, sampler=s)):
-        for bad in ("euler", "p_sampler", "ddim_sampler", "dpmpp_2m"):
-            with pytest.raises(ValueError):
-                call(bad)

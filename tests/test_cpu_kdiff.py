@@ -1,21 +1,12 @@
 """CPU: the sigma-space samplers' host side -- EulerSchedule / HeunSchedule rows, applied with the step kernels' formulas in
 float64, against the float64 restatement of diffusers' Euler, Euler ancestral and Heun discrete schedulers and their pipeline
-loop (tests/kdiff_oracle.py); the grids, the start latents, Heun's evaluation count, the argument checks of k2_heun_step and the
-pipelines' sampler names."""
-import ctypes
-
+loop (tests/kdiff_oracle.py); the grids, the start latents, Heun's evaluation count and the refusals of bad schedule
+arguments.  The argument checks of k2_heun_step and the pipelines' sampler names are in tests/test_cpu_schedule_samplers.py."""
 import numpy as np
 import pytest
-import torch
 
 from tests import kdiff_oracle as ko
-
-# name -> (oracle scheduler, Karras sigmas, schedule class name, its keywords, kernel formula)
-KINDS = {"euler_sampler": ("euler", False, "EulerSchedule", {}, "dpm"),
-         "euler_karras_sampler": ("euler", True, "EulerSchedule", dict(spacing="karras"), "dpm"),
-         "euler_ancestral_sampler": ("euler_ancestral", False, "EulerSchedule", dict(ancestral=True), "dpm"),
-         "heun_sampler": ("heun", False, "HeunSchedule", {}, "heun"),
-         "heun_karras_sampler": ("heun", True, "HeunSchedule", dict(spacing="karras"), "heun")}
+from tests.sampler_cases import KINDS, _schedule
 
 
 def _ac(version="2.2"):
@@ -24,12 +15,6 @@ def _ac(version="2.2"):
     if version == "2.1":
         return create_gaussian_diffusion(**CONFIG_2_1["diffusion_config"]).base_alphas_cumprod
     return create_ddpm_v22(50).base_alphas_cumprod
-
-
-def _schedule(name, ac, n, keep=None):
-    from kandinsky2.model import gaussian_diffusion as gd
-    _, _, cls, kw, _ = KINDS[name]
-    return getattr(gd, cls)(ac, n, keep=keep, **kw)
 
 
 def _eps(x, t):
@@ -49,7 +34,7 @@ def test_rows_with_kernel_formula_reproduce_oracle_loop(name, n, version):
     """The float64 rows applied with the kernels' formula == diffusers' scheduler loop restated in float64, to 1e-12, for both
     base tables, with and without img2img truncation; the fp32 table is the rows cast once and the model timesteps are the
     scheduler's (fp32)."""
-    kind, karras, _, _, formula = KINDS[name]
+    kind, karras, formula = KINDS[name]
     ac = _ac(version)
     rng = np.random.default_rng(n)
     z = rng.standard_normal(256)
@@ -84,7 +69,7 @@ def test_inpainting_rules_in_rows_match_oracle(name, renoise):
     """The 2.1 rule (the known region replaces pred_original_sample) and the 2.2 rule (the known region re-noised to the next
     sigma with the unit start noise, the clean latent at the end) through the rows == the oracle loop, to 1e-12; with the 2.2
     rule the known region of the result is the clean latent exactly."""
-    kind, karras, _, _, formula = KINDS[name]
+    kind, karras, formula = KINDS[name]
     ac = _ac()
     n = 10
     rng = np.random.default_rng(5)
@@ -169,82 +154,3 @@ def test_schedule_rejects_bad_arguments():
         for n, keep, spacing in ((0, None, "linspace"), (10, 0, "linspace"), (10, 11, "linspace"), (10, None, "exponential")):
             with pytest.raises(ValueError):
                 cls(ac, n, keep=keep, spacing=spacing)
-
-
-def test_existing_schedules_unchanged():
-    """The DPM++ and UniPC schedules keep a start noise scale of 1 and their grids; the existing sampler names map as before."""
-    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, UniPCSchedule, _solver_grid
-    from kandinsky2.pipelines import DPM_SAMPLERS, SOLVER_SAMPLERS, UNIPC_SAMPLERS
-    ac = _ac()
-    for cls in (DPMSolverSchedule, UniPCSchedule):
-        for spacing in ("linspace", "karras"):
-            sch = cls(ac, 10, spacing=spacing)
-            tau, alpha, sigma = _solver_grid("x", ac, 10, spacing)
-            assert sch.init_noise_scale == 1.0 and np.array_equal(sch.timesteps, tau) and np.array_equal(sch.alphas[:-1], alpha)
-    for name, (sp, sde) in DPM_SAMPLERS.items():
-        assert SOLVER_SAMPLERS[name] == (DPMSolverSchedule, dict(spacing=sp, sde=sde))
-    for name, sp in UNIPC_SAMPLERS.items():
-        assert SOLVER_SAMPLERS[name] == (UniPCSchedule, dict(spacing=sp))
-
-
-def test_heun_step_argument_errors_without_gpu():
-    """k2_heun_step checks its arguments before any CUDA call: < 0 and a message, also on a machine without a GPU."""
-    from kandinsky2 import _native
-    lib = _native.load()
-    p = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-    ok = [p, 8, p, p, p, p, 2, 4, 4, 4.0, 1, None, None, None]
-    cases = [({0: None}, "null pointer"), ({2: None}, "null pointer"), ({3: None}, "null pointer"), ({4: None}, "null pointer"),
-             ({5: None}, "null pointer"), ({1: 3}, "C2 >= 4"), ({6: 0}, "must be >= 1"), ({7: 0}, "must be >= 1"),
-             ({8: -1}, "must be >= 1"), ({11: p}, "init and mask go together"), ({12: p}, "init and mask go together"),
-             ({13: p}, "inpaint_noise without init")]
-    for change, msg in cases:
-        args = list(ok)
-        for i, v in change.items():
-            args[i] = v
-        assert lib.k2_heun_step(*args, None) < 0, change
-        assert msg in lib.k2_last_error().decode(), (change, lib.k2_last_error())
-
-
-def test_heun_step_without_gpu_raises():
-    from kandinsky2 import ops
-    from kandinsky2._native import K2Error
-    if torch.cuda.is_available():
-        pytest.skip("checks the CPU-only failure mode")
-    z = torch.zeros(1, 4, 8, 8)
-    with pytest.raises(K2Error):
-        ops.heun_step(torch.zeros(2, 8, 8, 8), z.clone(), z.clone(), z.clone(), torch.zeros(8), 4.0, True)
-
-
-def test_pipelines_accept_the_new_names_and_reject_unknown_ones():
-    """Both versions get past the sampler-name check with each new name on every method (the bare objects then fail for lack of
-    an embedder, which is not a sampler-name error) and refuse unknown names; SCHEDULE_SAMPLERS maps each new name beside the
-    DPM++ and UniPC ones."""
-    from kandinsky2.model.gaussian_diffusion import EulerSchedule, HeunSchedule
-    from kandinsky2.pipelines import (SAMPLERS_21, SAMPLERS_22, SCHEDULE_SAMPLERS, SIGMA_SAMPLERS, SOLVER_SAMPLERS, Kandinsky2_1,
-                                      Kandinsky2_2)
-    assert set(SIGMA_SAMPLERS) == set(KINDS) and set(SCHEDULE_SAMPLERS) == set(SOLVER_SAMPLERS) | set(SIGMA_SAMPLERS)
-    assert SCHEDULE_SAMPLERS["heun_karras_sampler"] == (HeunSchedule, dict(spacing="karras"))
-    assert SCHEDULE_SAMPLERS["euler_ancestral_sampler"] == (EulerSchedule, dict(spacing="linspace", ancestral=True))
-    p21 = Kandinsky2_1.__new__(Kandinsky2_1)
-    p22 = Kandinsky2_2.__new__(Kandinsky2_2)
-    calls = [lambda s: p21.generate_text2img("x", num_steps=4, sampler=s),
-             lambda s: p21.mix_images(["a"], [1.0], num_steps=4, sampler=s),
-             lambda s: p21.generate_img2img("x", None, num_steps=4, sampler=s),
-             lambda s: p21.generate_inpainting("x", None, None, num_steps=4, sampler=s),
-             lambda s: p21.generate_img("x", None, sampler=s),
-             lambda s: p22.generate_text2img("x", sampler=s),
-             lambda s: p22.mix_images(["a"], [1.0], sampler=s),
-             lambda s: p22.generate_img2img("x", None, sampler=s),
-             lambda s: p22.generate_inpainting("x", None, None, sampler=s),
-             lambda s: p22.generate_controlnet("x", None, sampler=s),
-             lambda s: p22.generate_controlnet_img2img("x", None, None, sampler=s)]
-    for name in KINDS:
-        assert name in SAMPLERS_21 and name in SAMPLERS_22
-        for call in calls:
-            with pytest.raises(Exception) as ei:
-                call(name)
-            assert "unknown sampler" not in str(ei.value), (name, ei.value)
-    for bad in ("euler", "heun", "euler_a_sampler", "heun_ancestral_sampler", "euler_ancestral_karras_sampler", "dpm2_sampler"):
-        for call in calls:
-            with pytest.raises(ValueError, match="unknown sampler"):
-                call(bad)

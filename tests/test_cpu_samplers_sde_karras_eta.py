@@ -1,8 +1,8 @@
 """CPU: the host side of the DPM-Solver++(2M) SDE variant, Karras sigma spacing and DDIM with eta > 0 -- coefficient rows
 against the float64 restatements (tests/dpm_sde_oracle.py, tests/ddim_eta_oracle.py), weak convergence of the SDE on Gaussian
 data, the Karras grid's known answers, the DDIM eta oracle against the reference's own sampler (tests/golden/ddim_eta_tiny.pt),
-the argument checks of k2_dpm_solver_sde_step and the pipelines' new sampler names."""
-import ctypes
+and the refusals of bad eta.  The argument checks of k2_dpm_solver_sde_step and the pipelines' sampler names are in
+tests/test_cpu_schedule_samplers.py."""
 import os
 
 import numpy as np
@@ -226,62 +226,3 @@ def test_eta_refusals():
     with pytest.raises(ValueError):
         _ddim(5.0, 10)
     assert _ddim(1.0, 10).draws_noise
-
-
-# ---- the C entry and the pipelines' names --------------------------------------------------------------------------------
-def test_dpm_solver_sde_step_argument_errors_without_gpu():
-    """k2_dpm_solver_sde_step checks its arguments before any CUDA call: < 0 and a message, also without a GPU."""
-    from kandinsky2 import _native
-    lib = _native.load()
-    p = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-    ok = [p, 8, p, p, p, p, 2, 4, 4, 4.0, 1, None, None, None]
-    cases = [({4: None}, "null noise"), ({0: None}, "null pointer"), ({2: None}, "null pointer"), ({3: None}, "null pointer"),
-             ({5: None}, "null pointer"), ({1: 3}, "C2 >= 4"), ({6: 0}, "must be >= 1"), ({7: 0}, "must be >= 1"),
-             ({8: -1}, "must be >= 1"), ({11: p}, "init and mask go together"), ({12: p}, "init and mask go together"),
-             ({13: p}, "inpaint_noise without init")]
-    for change, msg in cases:
-        args = list(ok)
-        for i, v in change.items():
-            args[i] = v
-        assert lib.k2_dpm_solver_sde_step(*args, None) < 0, change
-        err = lib.k2_last_error().decode()
-        assert msg in err and "dpm_solver_sde_step" in err, (change, err)
-
-
-def test_dpm_solver_sde_step_without_gpu_raises():
-    from kandinsky2 import ops
-    from kandinsky2._native import K2Error
-    if torch.cuda.is_available():
-        pytest.skip("checks the CPU-only failure mode")
-    z = torch.zeros(1, 4, 8, 8)
-    with pytest.raises(K2Error):
-        ops.dpm_solver_step(torch.zeros(2, 8, 8, 8), z.clone(), z.clone(), torch.zeros(8), 4.0, True, noise=z.clone())
-
-
-NEW_NAMES = ("dpmpp_2m_karras_sampler", "dpmpp_2m_sde_sampler", "dpmpp_2m_sde_karras_sampler")
-
-
-def test_pipelines_accept_the_new_sampler_names():
-    """Both versions get past the sampler-name check with each new name (the bare objects below then fail for lack of an
-    embedder, which is not a sampler-name error), and map every dpmpp_2m name to its (spacing, sde)."""
-    from kandinsky2.pipelines import DPM_SAMPLERS, SAMPLERS_21, SAMPLERS_22, Kandinsky2_1, Kandinsky2_2
-    assert DPM_SAMPLERS == {"dpmpp_2m_sampler": ("linspace", False), "dpmpp_2m_karras_sampler": ("karras", False),
-                            "dpmpp_2m_sde_sampler": ("linspace", True), "dpmpp_2m_sde_karras_sampler": ("karras", True)}
-    p21 = Kandinsky2_1.__new__(Kandinsky2_1)
-    p22 = Kandinsky2_2.__new__(Kandinsky2_2)
-    calls = [lambda s: p21.generate_text2img("x", num_steps=4, sampler=s),
-             lambda s: p21.mix_images(["a"], [1.0], num_steps=4, sampler=s),
-             lambda s: p21.generate_img2img("x", None, num_steps=4, sampler=s),
-             lambda s: p21.generate_inpainting("x", None, None, num_steps=4, sampler=s),
-             lambda s: p21.generate_img("x", None, sampler=s),
-             lambda s: p22.generate_text2img("x", sampler=s),
-             lambda s: p22.mix_images(["a"], [1.0], sampler=s),
-             lambda s: p22.generate_img2img("x", None, sampler=s),
-             lambda s: p22.generate_inpainting("x", None, None, sampler=s),
-             lambda s: p22.generate_controlnet("x", None, sampler=s)]
-    for name in NEW_NAMES:
-        assert name in SAMPLERS_21 and name in SAMPLERS_22
-        for call in calls:
-            with pytest.raises(Exception) as ei:
-                call(name)
-            assert "unknown sampler" not in str(ei.value), (name, ei.value)

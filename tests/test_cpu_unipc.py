@@ -1,12 +1,10 @@
 """CPU: the UniPC sampler's host side -- unipc_rows / UniPCSchedule against the float64 restatement of the paper and of diffusers'
 step order (tests/unipc_oracle.py), UniP-2 bh2 without the corrector against DPMSolverSchedule, third-order convergence with
-the corrector on Gaussian data whose probability-flow ODE has a closed form, the argument checks of k2_unipc_step, and the
-pipelines' sampler names."""
-import ctypes
-
+the corrector on Gaussian data whose probability-flow ODE has a closed form, both inpainting rules and the refusals of bad
+schedule arguments.  The argument checks of k2_unipc_step and the pipelines' sampler names are in
+tests/test_cpu_schedule_samplers.py."""
 import numpy as np
 import pytest
-import torch
 
 from tests import dpm_oracle as do
 from tests import unipc_oracle as uo
@@ -176,87 +174,3 @@ def test_schedule_rejects_bad_arguments():
         unipc_rows(sch.alphas, sch.sigmas, order=3)
     with pytest.raises(ValueError):            # a second-order step to sigma = 0 is undefined (r = 0)
         unipc_rows(sch.alphas, sch.sigmas, lower_order_final=False)
-
-
-def test_existing_schedules_unchanged():
-    """DPMSolverSchedule's grid is the restatement of its linspace / Karras spacing (bit for bit) and its rows are still 8
-    floats; the DDPM and DDIM tables keep their shape and step kind."""
-    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, create_ddpm_v22, karras_timesteps
-    ac = _ac()
-    for n in (1, 7, 20):
-        tau, alpha, sigma = do.grid(ac, n)
-        sch = DPMSolverSchedule(ac, n)
-        assert np.array_equal(sch.timesteps, tau) and np.array_equal(sch.alphas, alpha) and np.array_equal(sch.sigmas, sigma)
-        t, s_hat = karras_timesteps(ac, n)
-        kar = DPMSolverSchedule(ac, n, spacing="karras", sde=True)
-        a = 1.0 / np.sqrt(1.0 + s_hat ** 2)
-        assert np.array_equal(kar.timesteps, t) and np.array_equal(kar.alphas[:-1], a)
-        assert np.array_equal(kar.sigmas[:-1], s_hat * a)
-        assert sch.coef_table().shape == (n, 8) and sch.step_kind == "dpmpp_2m" and kar.step_kind == "dpmpp_2m_sde"
-    d = create_ddpm_v22(50)
-    assert d.coef_table().shape == (50, 8) and d.step_kind == "ddpm"
-
-
-def test_unipc_step_argument_errors_without_gpu():
-    """k2_unipc_step checks its arguments before any CUDA call: < 0 and a message, also on a machine without a GPU."""
-    from kandinsky2 import _native
-    lib = _native.load()
-    p = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-    ok = [p, 8, p, p, p, p, p, None, 2, 4, 4, 4.0, 1, None, None, None]
-    cases = [({0: None}, "null pointer"), ({2: None}, "null pointer"), ({3: None}, "null pointer"), ({4: None}, "null pointer"),
-             ({5: None}, "null pointer"), ({6: None}, "null pointer"), ({1: 3}, "C2 >= 4"), ({8: 0}, "must be >= 1"),
-             ({9: 0}, "must be >= 1"), ({10: -1}, "must be >= 1"), ({13: p}, "init and mask go together"),
-             ({14: p}, "init and mask go together"), ({15: p}, "inpaint_noise without init")]
-    for change, msg in cases:
-        args = list(ok)
-        for i, v in change.items():
-            args[i] = v
-        assert lib.k2_unipc_step(*args, None) < 0, change
-        assert msg in lib.k2_last_error().decode(), (change, lib.k2_last_error())
-
-
-def test_unipc_step_without_gpu_raises():
-    from kandinsky2 import ops
-    from kandinsky2._native import K2Error
-    if torch.cuda.is_available():
-        pytest.skip("checks the CPU-only failure mode")
-    z = torch.zeros(1, 4, 8, 8)
-    with pytest.raises(K2Error):
-        ops.unipc_step(torch.zeros(2, 8, 8, 8), z.clone(), z.clone(), z.clone(), z.clone(), torch.zeros(16), 4.0, True)
-
-
-UNIPC_NAMES = ("unipc_sampler", "unipc_karras_sampler")
-
-
-def test_pipelines_accept_unipc_names_and_reject_unknown_ones():
-    """Both versions get past the sampler-name check with each UniPC name on every method (the bare objects then fail for lack
-    of an embedder, which is not a sampler-name error) and refuse unknown names; one table maps every solver name."""
-    from kandinsky2.model.gaussian_diffusion import DPMSolverSchedule, UniPCSchedule
-    from kandinsky2.pipelines import (DPM_SAMPLERS, SAMPLERS_21, SAMPLERS_22, SOLVER_SAMPLERS, UNIPC_SAMPLERS, Kandinsky2_1,
-                                      Kandinsky2_2)
-    assert UNIPC_SAMPLERS == {"unipc_sampler": "linspace", "unipc_karras_sampler": "karras"}
-    assert set(SOLVER_SAMPLERS) == set(DPM_SAMPLERS) | set(UNIPC_SAMPLERS)
-    assert SOLVER_SAMPLERS["unipc_karras_sampler"] == (UniPCSchedule, dict(spacing="karras"))
-    assert SOLVER_SAMPLERS["dpmpp_2m_sde_sampler"] == (DPMSolverSchedule, dict(spacing="linspace", sde=True))
-    p21 = Kandinsky2_1.__new__(Kandinsky2_1)
-    p22 = Kandinsky2_2.__new__(Kandinsky2_2)
-    calls = [lambda s: p21.generate_text2img("x", num_steps=4, sampler=s),
-             lambda s: p21.mix_images(["a"], [1.0], num_steps=4, sampler=s),
-             lambda s: p21.generate_img2img("x", None, num_steps=4, sampler=s),
-             lambda s: p21.generate_inpainting("x", None, None, num_steps=4, sampler=s),
-             lambda s: p21.generate_img("x", None, sampler=s),
-             lambda s: p22.generate_text2img("x", sampler=s),
-             lambda s: p22.mix_images(["a"], [1.0], sampler=s),
-             lambda s: p22.generate_img2img("x", None, sampler=s),
-             lambda s: p22.generate_inpainting("x", None, None, sampler=s),
-             lambda s: p22.generate_controlnet("x", None, sampler=s)]
-    for name in UNIPC_NAMES:
-        assert name in SAMPLERS_21 and name in SAMPLERS_22
-        for call in calls:
-            with pytest.raises(Exception) as ei:
-                call(name)
-            assert "unknown sampler" not in str(ei.value), (name, ei.value)
-    for bad in ("unipc", "unipc_bh1_sampler", "uni_pc_sampler", "unipc_sde_sampler"):
-        for call in calls:
-            with pytest.raises(ValueError, match="unknown sampler"):
-                call(bad)
