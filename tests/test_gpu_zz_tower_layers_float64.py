@@ -53,7 +53,7 @@ _INPUTS = {"layernorm_f16": {0: "x"}, "gemm_rows": {0: "x", "residual": "res"}, 
            "clip_patchify": {0: "pix"}, "linear": {0: "x"}, "f16_to_f32": {0: "x"}, "readout_rows_f16": {0: "x"},
            "prior_tokens": {0: "x"}, "timestep_embedding": {0: "t"}}
 
-_NECK = "the DPT neck and head (readout, convolutions, resampling): convolutions, the plan-blocks style is their follow-up"
+_NECK = "the DPT neck and head (readout, convolutions, resampling): test_gpu_zz_depth_blocks_float64.py"
 _NECK_KINDS = {"conv", "relu", "bilinear", "depth_to_space", "subsample"}
 _BIT_KINDS = {"im2col", "conv", "conv_stride2_at_1", "conv_gemm", "gn_stats", "gn_finalize", "gn_act", "maxpool", "subsample",
               "relu"}
@@ -352,7 +352,7 @@ def _dpt_hybrid():
     sd = {k: v.cuda() for k, v in ho.synth_weights(cfg, 31, last_bias=ho.REAL_LAST_BIAS).items()}
     est = DPTDepthEstimator.from_transformers(sd, cfg)
     pix = torch.randn(1, 3, 384, 384, generator=torch.Generator().manual_seed(2)).cuda()
-    bit = "the BiT backbone (convolutions, GroupNorm, pooling): out of scope here, the plan-blocks style is its follow-up"
+    bit = "the BiT backbone (convolutions, GroupNorm, pooling): test_gpu_zz_depth_blocks_float64.py"
     return dict(name="DPT-Hybrid ViT", sd=sd, fmt="dpt", L=12, obj=est, eps=1e-12,
                 run=lambda g: (est.predicted_depth(pix, use_graph=g),), plan=lambda: est._plan(1, 384, 384),
                 t=dict(heads=12, hd=64, scale=0.125, eps=1e-12, act="gelu", post_ln=False, attn="fused", causal=False),
