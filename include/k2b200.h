@@ -237,6 +237,31 @@ int k2_step_begin(const float* x, float* x_in, long long n, float* t_in, int nt,
                   const float* coef_seq, const float* noise_seq, float* noise, const int* counter, k2_stream_t stream);
 int k2_step_end(int* counter, k2_stream_t stream);
 
+/* The same step for a continuously refilled batch of S slots, each slot a request at its own step of its own schedule
+ * (kandinsky2/batching.py; Kandinsky 2.2 row order: unconditional row s, conditional row S + s of the CFG-doubled UNet batch).
+ * state is a device int32 [2][S] = (k_s, steps_s); slot s is ACTIVE while 0 <= k_s < steps_s (and, for the tables,
+ * k_s < kmax); k_s = -1 marks a free slot.  n = 4 H W floats per slot.
+ *   k2_slot_step_begin: for an active slot, x_in rows s and S + s = x[s]; t_in[s] = t_in[S + s] = ts_tab[s][k_s];
+ *     coef_out[s][0:8) = coef_tab[s][k_s][0:8); noise[s] = noise_tab[s][k_s] if noise_tab != NULL.  For any other slot the same
+ *     places get zeros, so the UNet only sees finite input whatever the slot's buffers hold.  x fp32 [S][n], x_in [2S][n],
+ *     t_in [2S], coef_out [S][8], ts_tab [S][kmax], coef_tab [S][kmax][8], noise_tab [S][kmax][n], noise [S][n].
+ *   k2_slot_step_end: k_s += 1 for every active slot (a slot past its last step becomes inactive by itself).
+ *   k2_slot_sampler_step: k2_sampler_step (threshold_mode 0, +-clip, cond_first 0, no inpainting) per slot, with the slot's
+ *     coefficient row coef[s] (the coef_out above) and guidance scale guidance[s] (device fp32 [S]); work fp32 [S][n].
+ *   k2_slot_dpm_solver_step: k2_dpm_solver_step (cond_first 0, no inpainting) per slot, rows and guidance as above, hist fp32
+ *     [S][n] per slot.
+ * The step entries run the same kernels as their batch forms, so an active slot's result is bit-identical to the batch form
+ * applied to that slot alone; they neither read nor write an inactive slot's elements (its rows of model_out may hold NaN).
+ * Arguments are checked before any CUDA call. */
+int k2_slot_step_begin(const float* x, float* x_in, int S, long long n, float* t_in, float* coef_out, const float* ts_tab,
+                       const float* coef_tab, int kmax, const float* noise_tab, float* noise, const int* state,
+                       k2_stream_t stream);
+int k2_slot_step_end(int* state, int S, k2_stream_t stream);
+int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream);
+int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, k2_stream_t stream);
+
 /* PLMS / DDIM update with an explicit epsilon history (replaces PLMSSampler.p_sample_plms, samplers.py:571-637, and the
  * CFG closure): e_t = uncond + g (cond - uncond) from model_out's first 4 channels (C2 channels per sample);
  * e' = coef[4] e_t + coef[5] hist0 + coef[6] hist1 + coef[7] hist2 (NULL history entries are skipped);

@@ -259,7 +259,29 @@ struct SamplerParams {
   const float* rnoise;     // [B,4,H,W] or null: inpainting blends x_{t-1} with the re-noised init (diffusers) instead of x0
   float* x0;               // work [B*4*HW]
   float* sval;             // work scalar (dynamic threshold s)
+  const int* slots;        // slot form: int32 [2][B] = (step k_s, steps of the slot); coef is [B][8], guidance gscale[B]
+  const float* gscale;
 };
+
+// A slot of a continuously refilled batch (k2_slot_step_begin) is active while 0 <= k_s < steps_s; the slot forms of the step
+// kernels leave the elements of every other slot untouched and never read its rows.
+__device__ __forceinline__ bool slot_active(const int* state, int S, int s) {
+  const int k = state[s];
+  return k >= 0 && k < state[S + s];
+}
+
+// The coefficient row and guidance scale of element i: the call's own (kSlots = false), or those of the element's slot, when
+// that slot is active (kSlots = true; false for an idle slot).
+template <bool kSlots>
+__device__ __forceinline__ bool step_row(const int* slots, const float* gscale, long long i, int B, int HW, int width,
+                                         const float*& coef, float& guidance) {
+  if (!kSlots) return true;
+  const int s = static_cast<int>(i / (4LL * HW));
+  if (!slot_active(slots, B, s)) return false;
+  coef += static_cast<long long>(width) * s;
+  guidance = gscale[s];
+  return true;
+}
 
 // Element i of a [B, 4, HW] latent: its sample b, its pixel sp and the CFG epsilon eu + g (ec - eu) of its channel, read from the
 // eps channels of model_out [2B, C2, HW] (the conditional rows come first when cond_first; kandinsky2_1_model.py:222-233)
@@ -282,14 +304,18 @@ __device__ __forceinline__ CfgElem cfg_elem(const float* model_out, long long i,
   return e;
 }
 
+template <bool kSlots>
 __global__ void __launch_bounds__(256) sampler_x0_kernel(const SamplerParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
-  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, 8, p.guidance, p.cond_first);
-  float x0 = p.coef[0] * p.x[i] - p.coef[1] * e.eps;
+  const float* coef = p.coef;
+  float guidance = p.guidance;
+  if (!step_row<kSlots>(p.slots, p.gscale, i, p.B, p.HW, 8, coef, guidance)) return;
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, 8, guidance, p.cond_first);
+  float x0 = coef[0] * p.x[i] - coef[1] * e.eps;
   x0 = fminf(fmaxf(x0, -p.clip), p.clip);
   if (p.mask && !p.rnoise) {  // Kandinsky 2.1: the known region replaces x0 (denoised_fun, kandinsky2_1_model.py:237-243)
     const float m = p.mask[static_cast<long long>(e.b) * p.HW + e.sp];
@@ -352,12 +378,16 @@ __global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* _
   }
 }
 
+template <bool kSlots>
 __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
+  const float* coef = p.coef;
+  float guidance = p.guidance;  // (the CFG combination happened in sampler_x0_kernel)
+  if (!step_row<kSlots>(p.slots, p.gscale, i, p.B, p.HW, 8, coef, guidance)) return;
   const int sp = static_cast<int>(i % p.HW);
   const int c = static_cast<int>((i / p.HW) % 4);
   const int b = static_cast<int>(i / (4LL * p.HW));
@@ -367,19 +397,19 @@ __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p
     const float s = *p.sval;
     x0 = fminf(fmaxf(x0, -s), s) / s;
   }
-  const float mean = p.coef[2] * x0 + p.coef[3] * p.x[i];
+  const float mean = coef[2] * x0 + coef[3] * p.x[i];
   const float v = p.model_out[(static_cast<long long>(bc) * 8 + 4 + c) * p.HW + sp];
   const float frac = (v + 1.f) * 0.5f;
-  const float logvar = frac * p.coef[5] + (1.f - frac) * p.coef[4];
+  const float logvar = frac * coef[5] + (1.f - frac) * coef[4];
   // noise is not read at a step without noise (coef[6] = 0): whatever it holds, even NaN, cannot reach the result
   float xp = mean;
-  if (p.coef[6] != 0.f) xp = mean + p.coef[6] * expf(0.5f * logvar) * p.noise[i];
+  if (coef[6] != 0.f) xp = mean + coef[6] * expf(0.5f * logvar) * p.noise[i];
   if (p.mask && p.rnoise) {
     // Kandinsky 2.2 (diffusers KandinskyV22InpaintPipeline): after the scheduler step the known region is replaced by the
     // clean latent noised to the NEXT timestep with the run's initial noise; coef[7] = sqrt(alphas_cumprod[t_next]), 1 at
     // the last step (which is also the pipeline's final blend with the clean latent)
     const float m = p.mask[static_cast<long long>(b) * p.HW + sp];
-    const float c = p.coef[7];
+    const float c = coef[7];
     const float sgm = sqrtf(fmaxf(0.f, 1.f - c * c));
     xp = m * (c * p.init[i] + sgm * p.rnoise[i]) + (1.f - m) * xp;
   }
@@ -439,30 +469,35 @@ struct DpmParams {
   const float* mask;       // [B,1,H,W] or null
   const float* rnoise;     // [B,4,H,W] or null (2.2 inpainting: the known region is re-noised to the next timestep)
   const float* noise;      // [B,4,H,W] (the SDE entry) or null (the ODE entry): this step's Gaussian noise z
+  const int* slots;        // slot form: int32 [2][B] = (step k_s, steps of the slot); coef is [B][8], guidance gscale[B]
+  const float* gscale;
 };
 
-// kNoise: the SDE entry's instantiation; the ODE one has no noise term at all.
-template <bool kNoise>
+// kNoise: the SDE entry's instantiation; the ODE one has no noise term at all.  kSlots: the slot form (k2_slot_dpm_solver_step).
+template <bool kNoise, bool kSlots = false>
 __global__ void __launch_bounds__(256) dpm_solver_step_kernel(const DpmParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
   pdl_launch();
   const long long total = static_cast<long long>(p.B) * 4 * p.HW;
   if (i >= total) return;
-  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, p.guidance, p.cond_first);
+  const float* coef = p.coef;
+  float guidance = p.guidance;
+  if (!step_row<kSlots>(p.slots, p.gscale, i, p.B, p.HW, 8, coef, guidance)) return;
+  const CfgElem e = cfg_elem(p.model_out, i, p.B, p.HW, p.C2, guidance, p.cond_first);
   const float xv = p.x[i];
-  float x0 = p.coef[0] * xv - p.coef[1] * e.eps;
+  float x0 = coef[0] * xv - coef[1] * e.eps;
   const float m = p.mask ? p.mask[static_cast<long long>(e.b) * p.HW + e.sp] : 0.f;
   if (p.mask && !p.rnoise) x0 = x0 * (1.f - m) + p.init[i] * m;  // Kandinsky 2.1: the known region replaces x0
-  float xn = p.coef[2] * xv + p.coef[3] * x0;
-  const float cp = p.coef[4];
+  float xn = coef[2] * xv + coef[3] * x0;
+  const float cp = coef[4];
   if (cp != 0.f) xn += cp * p.hist[i];  // a first-order step never reads the history: it may hold anything, NaN included
   if (kNoise) {
-    const float cn = p.coef[7];
+    const float cn = coef[7];
     if (cn != 0.f) xn += cn * p.noise[i];  // likewise the noise on a noise-free row (the SDE's last step)
   }
   p.hist[i] = x0;
-  if (p.mask && p.rnoise) xn = m * (p.coef[5] * p.init[i] + p.coef[6] * p.rnoise[i]) + (1.f - m) * xn;
+  if (p.mask && p.rnoise) xn = m * (coef[5] * p.init[i] + coef[6] * p.rnoise[i]) + (1.f - m) * xn;
   p.x[i] = xn;
 }
 
@@ -856,10 +891,11 @@ int k2_sampler_step(const float* model_out, float* x, const float* noise, const 
   p.threshold_mode = (threshold_mode == 1 || threshold_mode == 3) ? 1 : 0;
   p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise;
   p.x0 = work; p.sval = work + static_cast<long long>(B) * 4 * H * W;
+  p.slots = nullptr; p.gscale = nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long total = static_cast<long long>(B) * 4 * H * W;
   if (do_front) {
-    K2_CHECK_CUDA(launch_k(sampler_x0_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+    K2_CHECK_CUDA(launch_k(sampler_x0_kernel<false>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
     count_launch();
   }
   if (do_pct) {
@@ -868,7 +904,7 @@ int k2_sampler_step(const float* model_out, float* x, const float* noise, const 
     count_launch();
   }
   if (do_post) {
-    K2_CHECK_CUDA(launch_k(sampler_post_kernel, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+    K2_CHECK_CUDA(launch_k(sampler_post_kernel<false>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
     count_launch();
   }
   K2_CHECK_CUDA(cudaGetLastError());
@@ -917,6 +953,100 @@ int k2_step_begin(const float* x, float* x_in, long long n, float* t_in, int nt,
 int k2_step_end(int* counter, k2_stream_t stream) {
   K2_REQUIRE(counter, "step_end: null counter");
   K2_CHECK_CUDA(launch_k(step_end_kernel, dim3(1), dim3(1), 0, static_cast<cudaStream_t>(stream), counter));
+  count_launch();
+  return 0;
+}
+
+// The continuously refilled batch: S slots, each at its own step k_s of its own tables (state = int32 [2][S] = (k_s, steps_s),
+// active while 0 <= k_s < steps_s).  Rows: unconditional s, conditional S + s.  One CTA row (blockIdx.y) per slot.
+__global__ void __launch_bounds__(256) slot_step_begin_kernel(const float* __restrict__ x, float* __restrict__ x_in, int S,
+                                                              long long n, float* __restrict__ t_in, float* __restrict__ coef_out,
+                                                              const float* __restrict__ ts_tab, const float* __restrict__ coef_tab,
+                                                              int kmax, const float* __restrict__ noise_tab,
+                                                              float* __restrict__ noise, const int* __restrict__ state) {
+  pdl_wait();
+  pdl_launch();
+  const int s = blockIdx.y;
+  const int k = state[s];
+  const bool active = k >= 0 && k < state[S + s] && k < kmax;  // an idle slot hands the UNet zeros, never its stale rows
+  const long long row = static_cast<long long>(s) * kmax + (active ? k : 0);
+  const long long base = static_cast<long long>(s) * n;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float v = active ? x[base + i] : 0.f;
+    x_in[base + i] = v;
+    x_in[static_cast<long long>(S) * n + base + i] = v;
+    if (noise_tab) noise[base + i] = active ? noise_tab[row * n + i] : 0.f;
+  }
+  if (blockIdx.x == 0) {
+    if (threadIdx.x == 0) {
+      const float t = active ? ts_tab[row] : 0.f;
+      t_in[s] = t;
+      t_in[S + s] = t;
+    }
+    if (threadIdx.x < 8) coef_out[s * 8 + threadIdx.x] = active ? coef_tab[row * 8 + threadIdx.x] : 0.f;
+  }
+}
+__global__ void slot_step_end_kernel(int* state, int S) {
+  pdl_wait();
+  pdl_launch();
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < S && slot_active(state, S, s)) state[s] += 1;
+}
+
+int k2_slot_step_begin(const float* x, float* x_in, int S, long long n, float* t_in, float* coef_out, const float* ts_tab,
+                       const float* coef_tab, int kmax, const float* noise_tab, float* noise, const int* state,
+                       k2_stream_t stream) {
+  K2_REQUIRE(x && x_in && t_in && coef_out && ts_tab && coef_tab && state, "slot_step_begin: null pointer");
+  K2_REQUIRE(S >= 1 && S <= 65535 && n >= 1 && kmax >= 1, "slot_step_begin: S in [1, 65535], n and kmax must be >= 1");
+  K2_REQUIRE(noise_tab == nullptr || noise, "slot_step_begin: noise_tab without a noise buffer");
+  K2_REQUIRE(n <= 256LL * 0x7fffffffLL, "slot_step_begin: n too large");
+  K2_CHECK_CUDA(launch_k(slot_step_begin_kernel, dim3(blocks_for(n, 256), S), dim3(256), 0,
+                         static_cast<cudaStream_t>(stream), x, x_in, S, n, t_in, coef_out, ts_tab, coef_tab, kmax, noise_tab,
+                         noise, state));
+  count_launch();
+  return 0;
+}
+
+int k2_slot_step_end(int* state, int S, k2_stream_t stream) {
+  K2_REQUIRE(state, "slot_step_end: null state");
+  K2_REQUIRE(S >= 1, "slot_step_end: S must be >= 1");
+  K2_CHECK_CUDA(launch_k(slot_step_end_kernel, dim3(blocks_for(S, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), state,
+                         S));
+  count_launch();
+  return 0;
+}
+
+int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && noise && coef && guidance && state && work, "slot_sampler_step: null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1, "slot_sampler_step: S, H, W must be >= 1");
+  SamplerParams p;
+  p.model_out = model_out; p.x = x; p.noise = noise; p.coef = coef;
+  p.B = S; p.HW = H * W; p.guidance = 0.f; p.cond_first = 0; p.clip = clip; p.threshold_mode = 0;
+  p.init = nullptr; p.mask = nullptr; p.rnoise = nullptr;
+  p.x0 = work; p.sval = nullptr; p.slots = state; p.gscale = guidance;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long total = static_cast<long long>(S) * 4 * H * W;
+  K2_CHECK_CUDA(launch_k(sampler_x0_kernel<true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+  count_launch();
+  K2_CHECK_CUDA(launch_k(sampler_post_kernel<true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+  count_launch();
+  return 0;
+}
+
+int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && hist && coef && guidance && state, "slot_dpm_solver_step: null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1 && C2 >= 4, "slot_dpm_solver_step: S, H, W must be >= 1 and C2 >= 4");
+  DpmParams p;
+  p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
+  p.B = S; p.HW = H * W; p.C2 = C2; p.guidance = 0.f; p.cond_first = 0;
+  p.init = nullptr; p.mask = nullptr; p.rnoise = nullptr; p.noise = nullptr;
+  p.slots = state; p.gscale = guidance;
+  const long long total = static_cast<long long>(S) * 4 * H * W;
+  K2_CHECK_CUDA(launch_k(dpm_solver_step_kernel<false, true>, dim3(blocks_for(total, 256)), dim3(256), 0,
+                         static_cast<cudaStream_t>(stream), p));
   count_launch();
   return 0;
 }
@@ -985,6 +1115,7 @@ static int dpm_step(const char* name, const float* model_out, int C2, float* x, 
   p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
   p.B = B; p.HW = H * W; p.C2 = C2; p.guidance = guidance; p.cond_first = cond_first;
   p.init = inpaint_init; p.mask = inpaint_mask; p.rnoise = inpaint_noise; p.noise = noise;
+  p.slots = nullptr; p.gscale = nullptr;
   const long long total = static_cast<long long>(B) * 4 * H * W;
   K2_CHECK_CUDA(launch_k(noise ? dpm_solver_step_kernel<true> : dpm_solver_step_kernel<false>, dim3(blocks_for(total, 256)),
                          dim3(256), 0, static_cast<cudaStream_t>(stream), p));

@@ -419,6 +419,30 @@ class Text2ImUNet(nn.Module):
             self.cache = out
         return out
 
+    def bind_slot(self, plan, slot, negative_emb, positive_emb):
+        """Write the conditioning of slot `slot` of a plan of N = 2 S rows (Kandinsky 2.2 row order: negative_emb's row
+        `slot`, positive_emb's row S + slot; image embeddings [image_encoder_in_dim]) into the plan's xf_proj and encoder K/V
+        rows, leaving every other row and every buffer address (so a CUDA graph captured on the plan) as it is.
+        Each output row of get_text_emb depends on its input row alone, but the encoder K/V GEMM picks its split-K factor
+        from its row count (k2_conv_gemm), which changes the fp32 summation order; so the rows are computed at the plan's batch
+        (the other input rows zero), and a slot's conditioning has the same bits in every slot and, at S = 1, those
+        generate_text2img(batch_size=1) binds.  The model's cached conditioning is left untouched."""
+        if self.cond_version == "2.1" or self.hint_channels:
+            raise K2Error("bind_slot: only the Kandinsky 2.2 text2img UNet takes per-slot conditioning")
+        S = plan.N // 2
+        if not 0 <= slot < S:
+            raise K2Error(f"bind_slot: slot {slot} outside [0, {S})")
+        emb = torch.zeros(plan.N, negative_emb.shape[-1], device=plan.dev, dtype=torch.float32)
+        emb[slot] = negative_emb.reshape(-1).to(emb.device, torch.float32)
+        emb[S + slot] = positive_emb.reshape(-1).to(emb.device, torch.float32)
+        saved, keep = self.cache, self.cache_text_emb
+        self.cache, self.cache_text_emb = None, False
+        try:
+            cond = self.get_text_emb(image_emb=emb)
+        finally:
+            self.cache, self.cache_text_emb = saved, keep
+        plan.bind_rows(cond, (slot, S + slot))
+
     # ---------------------------------------------------------------- forward
     def forward(self, x, timesteps, full_emb=None, pooled_emb=None, image_emb=None, inpaint_image=None,
                 inpaint_mask=None, hint=None):
@@ -497,6 +521,18 @@ class _Plan(LaunchPlan):
                 raise K2Error("context length changed between forwards: call del_cache() and rebuild the plan")
             buf.copy_(src)
         self._bound = cond
+
+    def bind_rows(self, cond, rows):
+        """Copy rows `rows` of a get_text_emb result computed at this plan's batch into the plan's conditioning buffers, in
+        place (Text2ImUNet.bind_slot)."""
+        idx = torch.tensor(rows, device=self.dev, dtype=torch.long)
+        self.xf_proj[idx] = cond["xf_proj"][idx]
+        for p, buf in self.enc_kv.items():
+            src = cond["enc_kv"][p]
+            if buf.shape != src.shape:
+                raise K2Error("bind_rows: the conditioning was not computed at this plan's batch and context length")
+            buf[idx] = src[idx]
+        self._bound = None
 
     # program -----------------------------------------------------------------------------------
     def _build(self):

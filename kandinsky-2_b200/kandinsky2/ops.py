@@ -396,6 +396,78 @@ def step_end(counter):
     check(nat.load().k2_step_end(ptr(counter), stream_ptr()))
 
 
+def _slot_check(who, S, n, f32=(), state=None, shaped=()):
+    """Refuse what the slot kernels would read wrongly: host tensors, fp32 operands that are not contiguous fp32, a state that
+    is not a contiguous int32 [2, S], and operands whose element count is not the one the kernel indexes (shaped: (name,
+    tensor, expected numel))."""
+    tensors = [t for _, t in f32 if t is not None] + ([state] if state is not None else [])
+    if not all(t.is_cuda for t in tensors):
+        raise nat.K2Error(f"{who}: tensors must live on a CUDA sm_90 device (no CPU fallback)")
+    for name, t in f32:
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous()):
+            raise nat.K2Error(f"{who}: {name} must be a contiguous float32 tensor, got {t.dtype}"
+                              f"{'' if t.is_contiguous() else ' (not contiguous)'}")
+    if state is not None and (state.dtype != torch.int32 or not state.is_contiguous() or tuple(state.shape) != (2, S)):
+        raise nat.K2Error(f"{who}: state must be a contiguous int32 [2, {S}] tensor, got {state.dtype} {tuple(state.shape)}")
+    for name, t, numel in shaped:
+        if t is not None and t.numel() != numel:
+            raise nat.K2Error(f"{who}: {name} must hold {numel} elements for {S} slots of {n}, got {tuple(t.shape)}")
+
+
+def slot_step_begin(x, x_in, t_in, coef_out, ts_tab, coef_tab, noise_tab, noise, state):
+    """k2_slot_step_begin: x fp32 [S, 4, H, W] -> x_in rows s and S + s of every active slot, t_in [2S], coef_out [S, 8] and
+    noise [S, 4, H, W] from the slot's row k_s of ts_tab [S, kmax], coef_tab [S, kmax, 8] and noise_tab [S, kmax, 4, H, W]
+    (or None); state = device int32 [2, S] = (k_s, steps_s); see k2b200.h."""
+    S = x.shape[0]
+    n = x[0].numel()
+    kmax = ts_tab.shape[-1]
+    _slot_check("slot_step_begin", S, n,
+                f32=(("x", x), ("x_in", x_in), ("t_in", t_in), ("coef_out", coef_out), ("ts_tab", ts_tab),
+                     ("coef_tab", coef_tab), ("noise_tab", noise_tab), ("noise", noise)), state=state,
+                shaped=(("x_in", x_in, 2 * S * n), ("t_in", t_in, 2 * S), ("coef_out", coef_out, 8 * S),
+                        ("ts_tab", ts_tab, S * kmax), ("coef_tab", coef_tab, 8 * S * kmax),
+                        ("noise_tab", noise_tab, S * kmax * n), ("noise", noise, S * n)))
+    check(nat.load().k2_slot_step_begin(ptr(x), ptr(x_in), S, n, ptr(t_in), ptr(coef_out), ptr(ts_tab), ptr(coef_tab), kmax,
+                                        ptr(noise_tab), ptr(noise), ptr(state), stream_ptr()))
+
+
+def slot_step_end(state):
+    """k2_slot_step_end: k_s += 1 for every active slot of state = device int32 [2, S]."""
+    _slot_check("slot_step_end", state.shape[-1], 0, state=state)
+    check(nat.load().k2_slot_step_end(ptr(state), state.shape[-1], stream_ptr()))
+
+
+def _slot_step_operands(who, model_out, x, coef, guidance, state, c2, others):
+    S, C, H, W = x.shape
+    n = 4 * H * W
+    if C != 4:
+        raise nat.K2Error(f"{who}: x must be [S, 4, H, W], got {tuple(x.shape)}")
+    _slot_check(who, S, n, f32=(("model_out", model_out), ("x", x), ("coef", coef), ("guidance", guidance)) + others,
+                state=state, shaped=(("model_out", model_out, 2 * S * c2 * H * W), ("coef", coef, 8 * S),
+                                     ("guidance", guidance, S)) + tuple((name, t, S * n) for name, t in others))
+    return S, H, W
+
+
+def slot_sampler_step(model_out, x, noise, coef, guidance, state, work, clip=2.0):
+    """k2_slot_sampler_step: the Kandinsky 2.2 DDPM step of every active slot of x fp32 [S, 4, H, W] in place, with the
+    slot's row of coef [S, 8] and its guidance [S] (device fp32); model_out [2S, 8, H, W], noise and work fp32 [S, 4, H, W]."""
+    S, H, W = _slot_step_operands("slot_sampler_step", model_out, x, coef, guidance, state, 8,
+                                  (("noise", noise), ("work", work)))
+    check(nat.load().k2_slot_sampler_step(ptr(model_out), ptr(x), ptr(noise), ptr(coef), ptr(guidance), ptr(state), S, H, W,
+                                          float(clip), ptr(work), stream_ptr()))
+    return x
+
+
+def slot_dpm_solver_step(model_out, x, hist, coef, guidance, state):
+    """k2_slot_dpm_solver_step: the DPM-Solver++(2M) step of every active slot of x fp32 [S, 4, H, W] in place, hist [S, 4, H, W]
+    per slot, model_out [2S, C2, H, W], rows and guidance as slot_sampler_step."""
+    S, H, W = _slot_step_operands("slot_dpm_solver_step", model_out, x, coef, guidance, state, model_out.shape[1],
+                                  (("hist", hist),))
+    check(nat.load().k2_slot_dpm_solver_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef), ptr(guidance),
+                                             ptr(state), S, H, W, stream_ptr()))
+    return x
+
+
 def plms_step(model_out, x, out, hist, store, coef, guidance, cond_first):
     """hist: list of up to 3 fp32 [B,4,H,W] tensors, newest first (None entries allowed)."""
     lib = nat.load()

@@ -152,9 +152,11 @@ class _DecoderBase:
             return self.image_encoder.encode(image.to(self.device))
         return self.image_encoder.encode(prepare_image(image, w=w, h=h).to(self.device))
 
-    def _generators(self, lo, hi):
-        """One device RNG stream per GLOBAL sample index (step noise independent of world size / batch position)."""
-        return [torch.Generator(device=self.device).manual_seed(self.base_seed * 7919 + gi) for gi in range(lo, hi)]
+    def _generators(self, lo, hi, base_seed=None):
+        """One device RNG stream per GLOBAL sample index (step noise independent of world size / batch position); base_seed
+        defaults to the pipeline's."""
+        seed = self.base_seed if base_seed is None else base_seed
+        return [torch.Generator(device=self.device).manual_seed(seed * 7919 + gi) for gi in range(lo, hi)]
 
     def _img2img_noise(self, latent):
         """Seeded by base_seed alone: every img2img call on one image starts from the same noisy latent."""
@@ -389,6 +391,14 @@ class Kandinsky2_2(_DecoderBase):
         if prior_kw is None:
             return self.embedder.image_emb(negative_decoder_prompt, batch_size)
         return self.embedder.image_emb(negative_decoder_prompt, batch_size, **{**prior_kw, "negative_prior_prompt": ""})
+
+    def batcher(self, max_batch, h, w, sampler="ddpm_sampler", max_steps=100):
+        """A batching.Batcher: text2img requests submitted one at a time and served from one continuously refilled batch of
+        max_batch slots at h x w (rounded up to multiples of 64, as generate_text2img does), every slot at its own denoising
+        step.  sampler: "ddpm_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's
+        decoder_steps (the per-slot tables are sized for it)."""
+        from .batching import Batcher
+        return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps)
 
     def generate_text2img(self, prompt, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                           prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
