@@ -105,6 +105,17 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
                      int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
                      const int* cfg, long long w_batch_stride, k2_stream_t stream);
 
+/* k2_conv_gemm_cfg in batched mode with the weight matrix of each image CHOSEN: image n of the NB images multiplies slab
+ * w_map[n] of n_slabs slabs, Wp + w_map[n] * w_batch_stride (w_batch_stride > 0).  w_map: DEVICE int32 [NB], read by the
+ * kernel when it runs, so a captured CUDA graph follows the map's current contents.  Slabs may repeat and need not all be
+ * used.  Bias, residual, fp16 / fp32 output and the fused GroupNorm partials are those of batched mode; tiles never span
+ * images and K is never split.  A map entry outside [0, n_slabs) multiplies zeros (TMA's out-of-bounds fill); callers write
+ * only valid entries.  The Kandinsky 2.2 batcher runs its attention projections this way, one adapter slab per request. */
+int k2_conv_gemm_wmap(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const void* w_packed, int w_rows,
+                      int Ktot, int ldw, int Cout, const float* bias, const void* residual, int ldr, void* out, int ldo,
+                      int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
+                      const int* cfg, long long w_batch_stride, int n_slabs, const int* w_map, k2_stream_t stream);
+
 /* The decisions k2_conv_gemm takes for a geometry -- M tile box, N tile, split-K factor, how the GroupNorm
  * partials come out -- without touching a pointer or the GPU (host arithmetic only; for tests, tooling and the caller's
  * scratch sizing).  taps: 9 if any source is a 3x3, else 1; Ktot as for k2_conv_gemm; workspace_bytes 0 = no workspace;

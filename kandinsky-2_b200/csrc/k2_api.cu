@@ -287,10 +287,13 @@ int k2_conv_gemm(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const vo
                           workspace, workspace_bytes, gn_partial, info, nullptr, 0, stream);
 }
 
-int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const void* w_packed, int w_rows,
-                     int Ktot, int ldw, int Cout, const float* bias, const void* residual, int ldr, void* out, int ldo,
-                     int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
-                     const int* cfg, long long w_batch_stride, k2_stream_t stream) {
+}  // extern "C"
+
+// k2_conv_gemm_cfg, and k2_conv_gemm_wmap when w_map is not null (n_slabs >= 1, checked by the caller)
+static int conv_gemm_impl(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const void* w_packed, int w_rows, int Ktot,
+                          int ldw, int Cout, const float* bias, const void* residual, int ldr, void* out, int ldo, int out_mode,
+                          void* workspace, long long workspace_bytes, float* gn_partial, int* info, const int* cfg,
+                          long long w_batch_stride, int n_slabs, const int* w_map, k2_stream_t stream) {
   K2_REQUIRE(w_batch_stride >= 0 && w_batch_stride % 8 == 0, "conv_gemm_cfg: w_batch_stride must be a multiple of 8 elements");
   // out_mode 2 (raw fp32 split-K partials into the workspace) is internal: the split-K plan sets it and adds the finalize pass
   K2_REQUIRE(out_mode == 0 || out_mode == 1, "conv_gemm: out_mode must be 0 (fp16 rows) or 1 (fp32 NCHW)");
@@ -311,6 +314,11 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
   if (ldw == 0) ldw = Ktot;
   K2_REQUIRE(ldw >= Ktot && ldw % 8 == 0 && (reinterpret_cast<uintptr_t>(w_packed) & 15) == 0,
              "conv_gemm: weight row stride / alignment");
+  if (out_mode == 0) {
+    K2_REQUIRE(ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "conv_gemm: out alignment");
+    if (residual)
+      K2_REQUIRE(ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0, "conv_gemm: residual alignment");
+  }
   ConvGemmParams p;
   memset(&p, 0, sizeof p);
   p.NB = NB;
@@ -347,6 +355,7 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
             cfg, up2, w_batched);
   K2_REQUIRE(!w_batched || (!up2 && pl.TN == 1), "conv_gemm_cfg: batched weights need single-image tiles");
   p.w_batched = w_batched ? 1 : 0;
+  p.w_map = w_map;
   plan_to_info(pl, info);
   p.TN = pl.TN;
   p.TH = pl.TH;
@@ -375,7 +384,8 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
   p.n_tiles = (Cout + BN - 1) / BN;
   p.Cout = Cout;
   {
-    uint64_t dims[3] = {static_cast<uint64_t>(Ktot), static_cast<uint64_t>(w_rows), static_cast<uint64_t>(w_batched ? NB : 1)};
+    const int slabs = w_map ? n_slabs : (w_batched ? NB : 1);
+    uint64_t dims[3] = {static_cast<uint64_t>(Ktot), static_cast<uint64_t>(w_rows), static_cast<uint64_t>(slabs)};
     uint64_t str[2] = {static_cast<uint64_t>(ldw) * 2,
                        (w_batched ? static_cast<uint64_t>(w_batch_stride) : static_cast<uint64_t>(ldw) * w_rows) * 2};
     uint32_t box[3] = {64, static_cast<uint32_t>(BN), 1};
@@ -389,11 +399,6 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
   p.out_mode = (splits > 1) ? 2 : out_mode;
   p.gn_part = (fuse_stats == 1) ? reinterpret_cast<float2*>(gn_partial) : nullptr;
   p.gn_mode = (fuse_stats == 1) ? (p.TN == 1 ? 1 : 2) : 0;
-  if (out_mode == 0) {
-    K2_REQUIRE(ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "conv_gemm: out alignment");
-    if (residual)
-      K2_REQUIRE(ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0, "conv_gemm: residual alignment");
-  }
   int rc = launch_conv_gemm(p, BN, static_cast<cudaStream_t>(stream));
   if (rc == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   if (rc == 0 && splits > 1) {
@@ -403,6 +408,29 @@ int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, cons
     if (rc == 0) g_launches.fetch_add(1, std::memory_order_relaxed);
   }
   return rc;
+}
+
+extern "C" {
+
+int k2_conv_gemm_cfg(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const void* w_packed, int w_rows,
+                     int Ktot, int ldw, int Cout, const float* bias, const void* residual, int ldr, void* out, int ldo,
+                     int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
+                     const int* cfg, long long w_batch_stride, k2_stream_t stream) {
+  return conv_gemm_impl(srcs, nsrc, NB, H, W, w_packed, w_rows, Ktot, ldw, Cout, bias, residual, ldr, out, ldo, out_mode,
+                        workspace, workspace_bytes, gn_partial, info, cfg, w_batch_stride, 0, nullptr, stream);
+}
+
+int k2_conv_gemm_wmap(const K2ConvSrc* srcs, int nsrc, int NB, int H, int W, const void* w_packed, int w_rows,
+                      int Ktot, int ldw, int Cout, const float* bias, const void* residual, int ldr, void* out, int ldo,
+                      int out_mode, void* workspace, long long workspace_bytes, float* gn_partial, int* info,
+                      const int* cfg, long long w_batch_stride, int n_slabs, const int* w_map, k2_stream_t stream) {
+  K2_REQUIRE(w_map != nullptr, "conv_gemm_wmap: null w_map");
+  K2_REQUIRE((reinterpret_cast<uintptr_t>(w_map) & 3) == 0, "conv_gemm_wmap: w_map must be 4-byte aligned");
+  K2_REQUIRE(n_slabs >= 1, "conv_gemm_wmap: n_slabs must be >= 1");
+  K2_REQUIRE(w_batch_stride > 0, "conv_gemm_wmap: w_batch_stride must be > 0 (the elements between two slabs)");
+  K2_REQUIRE(srcs != nullptr && w_packed != nullptr && out != nullptr, "conv_gemm_wmap: null source, weight or output");
+  return conv_gemm_impl(srcs, nsrc, NB, H, W, w_packed, w_rows, Ktot, ldw, Cout, bias, residual, ldr, out, ldo, out_mode,
+                        workspace, workspace_bytes, gn_partial, info, cfg, w_batch_stride, n_slabs, w_map, stream);
 }
 
 int k2_conv_plan(int NB, int H, int W, int taps, int Ktot, int Cout, int out_mode, long long workspace_bytes,

@@ -295,7 +295,9 @@ __device__ __forceinline__ void epilogue_warp(const ConvGemmParams& p, const flo
 }
 
 
-template <int BN>
+// WMAP: image n multiplies weight slab p.w_map[n] (k2_conv_gemm_wmap); otherwise slab n when p.w_batched, else the one
+// weight matrix.  The flag only adds the map read, so the WMAP = false instances are the kernel as it was without it.
+template <int BN, bool WMAP>
 __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   using C = Cfg<BN>;
   constexpr int NA = BN / 2;  // accumulator registers of the m64nBNk16 fragment
@@ -356,6 +358,9 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
         }
         int tap = rem / p.seg_kchunks[s];
         int c = rem - tap * p.seg_kchunks[s];
+        // tiles never span images in batched mode (TN == 1); a slab index outside [0, n_slabs) loads TMA's zero fill
+        int wslab = 0;
+        if constexpr (WMAP) wslab = __ldg(p.w_map + n0);
         for (int kc = k0; kc < k1; ++kc) {
           const int taps = p.seg_taps[s];
           const int dy = (taps == 9) ? (tap / 3 - 1) : (taps == 4 ? (tap >> 1) + (phase >> 1) - 1 : 0);
@@ -365,7 +370,7 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
           uint8_t* sB = sA + A_STAGE_BYTES;
           mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
           tma_load_4d(sA, &p.tmA[s], &full_bar[stage], c * BK, x0 + dx, y0 + dy, n0);
-          tma_load_3d(sB, &p.tmB, &full_bar[stage], (kb + kc) * BK, n_idx * BN, p.w_batched ? n0 : 0);
+          tma_load_3d(sB, &p.tmB, &full_bar[stage], (kb + kc) * BK, n_idx * BN, WMAP ? wslab : (p.w_batched ? n0 : 0));
           if (++stage == C::STAGES) {
             stage = 0;
             ring_phase ^= 1;
@@ -527,18 +532,31 @@ __global__ void __launch_bounds__(256) splitk_finalize_kernel(const float* __res
 }
 
 
-template <int BN>
+template <int BN, bool WMAP>
 int launch_bn(const ConvGemmParams& p, cudaStream_t stream) {
   using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    K2_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, WMAP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       C::SMEM_BYTES));
     attr_set = true;
   }
   int total = p.m_tiles * p.n_tiles * p.splits;
   int grid = total < num_sms() ? total : num_sms();
-  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN>, dim3(grid), dim3(384), C::SMEM_BYTES, stream, p));
+  K2_CHECK_CUDA(launch_k(conv_gemm_kernel<BN, WMAP>, dim3(grid), dim3(384), C::SMEM_BYTES, stream, p));
   return 0;
+}
+
+template <bool WMAP>
+int launch_wmap(const ConvGemmParams& p, int BN, cudaStream_t stream) {
+  switch (BN) {
+    case 16: return launch_bn<16, WMAP>(p, stream);
+    case 64: return launch_bn<64, WMAP>(p, stream);
+    case 128: return launch_bn<128, WMAP>(p, stream);
+    case 192: return launch_bn<192, WMAP>(p, stream);
+    case 256: return launch_bn<256, WMAP>(p, stream);
+    default: return fail("conv_gemm: unsupported BN");
+  }
 }
 
 }  // namespace
@@ -552,14 +570,7 @@ int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, c
 }
 
 int launch_conv_gemm(const ConvGemmParams& p, int BN, cudaStream_t stream) {
-  switch (BN) {
-    case 16: return launch_bn<16>(p, stream);
-    case 64: return launch_bn<64>(p, stream);
-    case 128: return launch_bn<128>(p, stream);
-    case 192: return launch_bn<192>(p, stream);
-    case 256: return launch_bn<256>(p, stream);
-    default: return fail("conv_gemm: unsupported BN");
-  }
+  return p.w_map ? launch_wmap<true>(p, BN, stream) : launch_wmap<false>(p, BN, stream);
 }
 
 }  // namespace k2

@@ -82,6 +82,7 @@ struct ConvGemmParams {
   int up2;             // 1: source 0 has taps == 4: 3x3 conv over the nearest-2x upsampled source as four 2x2 phase convs;
                        //    NB/H/W and the tile box are SOURCE geometry, outputs go to pixel (2y + a, 2x + b) of a 2H x 2W image
   int m_tiles_phase;   // up2: tile slots per phase (m_tiles = 4 * m_tiles_phase)
+  const int* w_map;    // w_batched only, or null: image n multiplies weight slab w_map[n] of tmB's n_slabs instead of slab n
 };
 int launch_conv_gemm(const ConvGemmParams& p, int BN, cudaStream_t stream);
 int launch_splitk_finalize(const float* ws, int splits, long long M, int Cout, const float* bias, const __half* residual,

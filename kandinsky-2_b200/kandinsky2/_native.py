@@ -37,6 +37,8 @@ SIGNATURES = {
                          ctypes.POINTER(ctypes.c_int), _P]),
     "k2_conv_gemm_cfg": (_I, [ctypes.POINTER(K2ConvSrc), _I, _I, _I, _I, _P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _LL, _P,
                              ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), _LL, _P]),
+    "k2_conv_gemm_wmap": (_I, [ctypes.POINTER(K2ConvSrc), _I, _I, _I, _I, _P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _LL,
+                              _P, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), _LL, _I, _P, _P]),
     "k2_sn_apply": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P, _I, _P, _I, _P]),
     "k2_transpose_f16": (_I, [_P, _I, _P, _I, _I, _I, _P]),
     "k2_gn_finalize": (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _F, _P, _P]),

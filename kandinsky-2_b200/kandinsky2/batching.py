@@ -12,6 +12,13 @@ start latent and per-step noise draws, the same tables (create_ddpm_v22 / the SC
 conditioning and step kernels.  Its result does not depend on the other slots: the UNet's normalisation, attention and
 convolutions are per image, the conditioning is written per row (Text2ImUNet.bind_slot) and the slot step kernels read and
 write only the rows of active slots.  An idle slot still costs a full row of UNet compute.
+
+With max_loras = L > 0 each request may name a LoRA adapter registered with add_lora.  The attention layers' qkv and proj_out
+weights then live in slab tables of 1 + L fp16 copies per layer (slab 0: the pipeline's packed weights when the batcher was
+made, slabs 1 .. L: base + scale * up @ down of a registered adapter, merged by k2_lora_merge as load_lora merges), and both
+GEMMs run batched, rows s and S + s of slot s multiplying the slab a device map names (k2_conv_gemm_wmap).  A slot's encoder
+K/V rows are computed at admission with its adapter's merged encoder_kv weights.  Registering, removing and admitting write
+slabs, the map and conditioning rows in place, so the step graph never changes.
 """
 import collections
 
@@ -26,13 +33,15 @@ from .model.unet import _Plan
 BATCHER_SAMPLERS = ("ddpm_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
 
 
-def check_batcher_args(max_batch, h, w, sampler, max_steps):
+def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0):
     """Refuse what a Batcher cannot serve, before any work: ValueError naming the argument."""
     if sampler not in BATCHER_SAMPLERS:
         raise ValueError(f"batcher: sampler {sampler!r} is not served; use one of {', '.join(BATCHER_SAMPLERS)}")
     for name, v in (("max_batch", max_batch), ("h", h), ("w", w), ("max_steps", max_steps)):
         if isinstance(v, bool) or not isinstance(v, int) or v < 1:
             raise ValueError(f"batcher: {name} must be a positive int, got {v!r}")
+    if isinstance(max_loras, bool) or not isinstance(max_loras, int) or max_loras < 0:
+        raise ValueError(f"batcher: max_loras must be an int >= 0, got {max_loras!r}")
 
 
 def request_tables(sampler, steps):
@@ -92,7 +101,7 @@ class SlotQueue:
 
 
 class _Request:
-    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive")
+    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora")
 
 
 class Batcher:
@@ -100,8 +109,8 @@ class Batcher:
 
     RUN_AHEAD = 2   # replayed steps the host may have in flight on the GPU when it admits (2: the GPU never waits on admission)
 
-    def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100):
-        check_batcher_args(max_batch, h, w, sampler, max_steps)
+    def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
+        check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras)
         if pipe.task_type != "text2img":
             raise ValueError(f"batcher: serves text2img pipelines only, this one is {pipe.task_type!r}")
         self.pipe, self.sampler, self.max_steps = pipe, sampler, max_steps
@@ -112,8 +121,26 @@ class Batcher:
             model.finalize()
         self._packed = model._packed
         dev = pipe.device
+        self.max_loras = max_loras
+        self._loras = {}   # adapter name -> (slab index, {attention layer -> merged encoder_kv weight})
+        self.w_map = None
+        slabs = None
+        if max_loras:
+            # allocated once, so the graph's addresses never change; slab 0 and its encoder_kv weights are copies, so
+            # load_lora / unload_lora on the pipeline leave this batcher's weights as they were
+            self.w_map = torch.zeros(2 * S, device=dev, dtype=torch.int32)
+            layers, self._wenc0 = {}, {}
+            for name, a in model._packed["attn"].items():
+                tabs = []
+                for key in ("wqkv", "wproj"):
+                    t = torch.zeros((1 + max_loras,) + tuple(a[key].shape), device=dev, dtype=torch.float16)
+                    t[0].copy_(a[key])
+                    tabs.append(t)
+                layers[name] = tuple(tabs)
+                self._wenc0[name] = a["wenc"].clone()
+            slabs = dict(map=self.w_map, layers=layers)
         # a plan of its own: another call on the pipeline at the same geometry must not rebind these rows
-        self.plan = p = _Plan(model, 2 * S, H, W, model.num_image_embs)
+        self.plan = p = _Plan(model, 2 * S, H, W, model.num_image_embs, attn_slabs=slabs)
         p.xf_proj.zero_()
         for buf in p.enc_kv.values():
             buf.zero_()
@@ -153,12 +180,53 @@ class Batcher:
             ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state)
         ops.slot_step_end(self.state)
 
+    def add_lora(self, name, state_dict, scale=1.0):
+        """Register a LoRA adapter of the decoder's attention blocks under `name` (the format Text2ImUNet.load_lora takes):
+        merged into a free slab from the UNet's unmerged weights, as load_lora(state_dict, scale) would merge it, so the
+        slab's bits are those load_lora writes.  Adapters do not stack with one the pipeline has loaded.  Requests submitted
+        with lora=name use it."""
+        if not self.max_loras:
+            raise ValueError("add_lora: this batcher was made with max_loras=0; make one with max_loras > 0")
+        if name in self._loras:
+            raise ValueError(f"add_lora: an adapter named {name!r} is already registered")
+        used = {k for k, _ in self._loras.values()}
+        free = [k for k in range(1, self.max_loras + 1) if k not in used]
+        if not free:
+            raise ValueError(f"add_lora: all {self.max_loras} adapter slabs are in use; remove_lora one first")
+        model = self.pipe.model
+        if model._packed is not self._packed:
+            raise K2Error("batcher: the UNet's weights were reloaded after the batcher was made; make a new one")
+        factors, scale = model.lora_factors(state_dict), float(scale)
+        k, wenc = free[0], {}
+        for p, a in self._packed["attn"].items():
+            base = model._lora_base[p] if model._lora_base is not None else a
+            wqkv, wproj = self.plan.attn_slabs["layers"][p]
+            wenc[p] = torch.empty_like(base["wenc"])
+            targets = {"wqkv": wqkv[k], "wproj": wproj[k], "wenc": wenc[p]}
+            for key, proj in model._LORA_WEIGHTS:   # what Text2ImUNet._merge_lora writes into the packed weights
+                f = factors.get(p + proj + ".weight")
+                targets[key].copy_(base[key])
+                if f is not None:
+                    up, down = (t.to(base[key].device) for t in f)
+                    ops.lora_merge(base[key], up, down, scale, out=targets[key])
+        self._loras[name] = (k, wenc)
+
+    def remove_lora(self, name):
+        """Unregister adapter `name`, freeing its slab; refused while a waiting or active request uses it."""
+        if name not in self._loras:
+            raise ValueError(f"remove_lora: no adapter named {name!r} is registered")
+        if any(r.lora == name for r in self._requests.values()):
+            raise ValueError(f"remove_lora: adapter {name!r} is used by a waiting or active request")
+        del self._loras[name]
+
     def submit(self, prompt=None, *, image_embeds=None, negative_image_embeds=None, decoder_steps=50, decoder_guidance_scale=4,
-               seed=None, prior_steps=25, prior_guidance_scale=4, negative_prior_prompt="", negative_decoder_prompt=""):
+               seed=None, prior_steps=25, prior_guidance_scale=4, negative_prior_prompt="", negative_decoder_prompt="",
+               lora=None):
         """Queue one image -> its handle (the key of its image in what step() / run() return).  Either a prompt, whose image
         embeddings the pipeline's embedder makes now at batch 1 as generate_text2img does (the prior keywords as there), or
         image_embeds and negative_image_embeds ([1, D] or [D]) as diffusers' KandinskyV22Pipeline takes them.  seed plays the
-        part of the pipeline's base_seed for global sample 0 (default: the pipeline's base_seed)."""
+        part of the pipeline's base_seed for global sample 0 (default: the pipeline's base_seed).  lora: the name of an
+        adapter registered with add_lora, or None for the weights slab 0 holds."""
         pipe = self.pipe
         if (prompt is None) == (image_embeds is None):
             raise ValueError("submit: pass either a prompt or image_embeds")
@@ -172,7 +240,10 @@ class Batcher:
         if isinstance(decoder_steps, bool) or not isinstance(decoder_steps, int) or not 1 <= decoder_steps <= self.max_steps:
             raise ValueError(f"submit: decoder_steps must be an int in [1, {self.max_steps}] (the batcher's max_steps), "
                              f"got {decoder_steps!r}")
+        if lora is not None and lora not in self._loras:
+            raise ValueError(f"submit: no adapter named {lora!r} is registered (Batcher.add_lora)")
         r = _Request()
+        r.lora = lora
         r.steps, r.guidance = decoder_steps, float(decoder_guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
         r.ts, r.coef = request_tables(self.sampler, decoder_steps)
@@ -206,7 +277,12 @@ class Batcher:
 
     def _stage(self, s, r):
         pipe, H, W = self.pipe, self.x.shape[2], self.x.shape[3]
-        pipe.model.bind_slot(self.plan, s, r.negative, r.positive)
+        if self.w_map is None:
+            pipe.model.bind_slot(self.plan, s, r.negative, r.positive)
+        else:
+            k, wenc = self._loras[r.lora] if r.lora is not None else (0, self._wenc0)
+            pipe.model.bind_slot(self.plan, s, r.negative, r.positive, wenc=wenc)
+            self._set_slab(s, k)
         k = r.steps
         self.ts_tab[s, :k].copy_(r.ts)
         self.coef_tab[s, :k].copy_(r.coef)
@@ -238,7 +314,14 @@ class Batcher:
         for s, handle in self.queue.advance():
             done[handle] = self.pipe._finish(self.x[s:s + 1], self.h, self.w)[0]
             del self._requests[handle]
+            if self.w_map is not None:
+                self._set_slab(s, 0)   # idle slots use slab 0, so a removed adapter's slab is read by no slot
         return done
+
+    def _set_slab(self, s, k):
+        S = self.x.shape[0]
+        self.w_map[s] = k
+        self.w_map[S + s] = k
 
     def run(self):
         """step() until every submitted request is finished -> {handle: PIL image} of all of them."""

@@ -144,7 +144,7 @@ class LaunchPlan:
         self._add(step, "join", 0)
 
     def _conv(self, srcs, w, cout, out, flops, bias=None, residual=None, want_stats=True, part_slot=None, out_mode=0,
-              geom=None, w_batch_stride=0, kind="conv_gemm"):
+              geom=None, w_batch_stride=0, w_map=None, n_slabs=0, kind="conv_gemm"):
         """conv_gemm step; with want_stats the epilogue also writes GroupNorm partial statistics of `out` (when the
         launch geometry allows it: k2b200.h), remembered in self._parts for the consumer's norm.  The launch
         configuration (N tile, epilogue warp sets) is timed once per distinct layer shape (tune) and baked in."""
@@ -156,9 +156,10 @@ class LaunchPlan:
         info = [0] * 7
         run = lambda cfg, info=None: ops.conv_gemm(srcs, w, cout, bias=bias, residual=residual, out=out, gn_part=part,
                                                    info=info, cfg=cfg, out_mode=out_mode, geom=geom,
-                                                   w_batch_stride=w_batch_stride)
+                                                   w_batch_stride=w_batch_stride, w_map=w_map, n_slabs=n_slabs)
+        # a mapped layer (one weight slab chosen per image) never shares an unmapped layer's configuration
         key = ("conv", cout, tuple(out.shape), geom, tuple((t.shape[-1], taps) for t, taps in srcs), residual is not None,
-               part is not None, out_mode, w_batch_stride > 0)
+               part is not None, out_mode, w_batch_stride > 0, w_map is not None)
         cfg = tune(key, run, m_rows=out.shape[0] * out.shape[1] * out.shape[2] if out_mode == 0 and geom is None else 0)
         self._add(lambda: run(cfg, info), kind, flops)
         if part is not None and info[5]:

@@ -318,15 +318,19 @@ class Text2ImUNet(nn.Module):
         need no rebuild; the cached conditioning is dropped because the encoder K/V projections use the merged weights.
         On first use the unmerged packed weights are copied on the device (restored by unload_lora).  Loading again
         replaces the adapter (adapters do not stack; a new scale means loading again).  state_dict() never changes."""
-        from ..checkpoints import lora_to_k2
-        factors = lora_to_k2(state_dict, in_channels=self.in_channels, model_channels=self.model_channels,
-                             channel_mult=self.channel_mult, num_res_blocks=self.num_res_blocks,
-                             attention_ds=self.attention_resolutions, model_dim=self.model_dim,
-                             head_dim=self.num_head_channels)
+        factors = self.lora_factors(state_dict)
         if self._packed is None:
             self.finalize()
         self._lora = (factors, float(scale))
         self._merge_lora()
+
+    def lora_factors(self, state_dict):
+        """{packed weight key: (up, down)} of an adapter of this UNet's attention blocks (checkpoints.lora_to_k2)."""
+        from ..checkpoints import lora_to_k2
+        return lora_to_k2(state_dict, in_channels=self.in_channels, model_channels=self.model_channels,
+                          channel_mult=self.channel_mult, num_res_blocks=self.num_res_blocks,
+                          attention_ds=self.attention_resolutions, model_dim=self.model_dim,
+                          head_dim=self.num_head_channels)
 
     def unload_lora(self):
         """Restore the unmerged packed weights (bit-exact), free their copy and drop the cached conditioning."""
@@ -419,14 +423,16 @@ class Text2ImUNet(nn.Module):
             self.cache = out
         return out
 
-    def bind_slot(self, plan, slot, negative_emb, positive_emb):
+    def bind_slot(self, plan, slot, negative_emb, positive_emb, wenc=None):
         """Write the conditioning of slot `slot` of a plan of N = 2 S rows (Kandinsky 2.2 row order: negative_emb's row
         `slot`, positive_emb's row S + slot; image embeddings [image_encoder_in_dim]) into the plan's xf_proj and encoder K/V
         rows, leaving every other row and every buffer address (so a CUDA graph captured on the plan) as it is.
         Each output row of get_text_emb depends on its input row alone, but the encoder K/V GEMM picks its split-K factor
         from its row count (k2_conv_gemm), which changes the fp32 summation order; so the rows are computed at the plan's batch
         (the other input rows zero), and a slot's conditioning has the same bits in every slot and, at S = 1, those
-        generate_text2img(batch_size=1) binds.  The model's cached conditioning is left untouched."""
+        generate_text2img(batch_size=1) binds.  The model's cached conditioning is left untouched.
+        wenc ({attention layer -> packed encoder_kv weight}, or None = the packed weights): the weights the slot's encoder K/V
+        rows are computed with, e.g. the encoder_kv weights an adapter merges (the batcher's per-request adapters)."""
         if self.cond_version == "2.1" or self.hint_channels:
             raise K2Error("bind_slot: only the Kandinsky 2.2 text2img UNet takes per-slot conditioning")
         S = plan.N // 2
@@ -441,6 +447,9 @@ class Text2ImUNet(nn.Module):
             cond = self.get_text_emb(image_emb=emb)
         finally:
             self.cache, self.cache_text_emb = saved, keep
+        if wenc is not None:
+            attn = self._packed["attn"]
+            cond["enc_kv"] = {p: ops.gemm_rows(cond["xf_out"], w, w.shape[0], bias=attn[p]["benc"]) for p, w in wenc.items()}
         plan.bind_rows(cond, (slot, S + slot))
 
     # ---------------------------------------------------------------- forward
@@ -487,7 +496,11 @@ class InpaintText2ImUNet(Text2ImUNet):
 class _Plan(LaunchPlan):
     """Static launch list + buffers of one forward at a fixed (N, H, W); replayed eagerly or as a CUDA graph."""
 
-    def __init__(self, model, N, H, W, ctx):
+    def __init__(self, model, N, H, W, ctx, attn_slabs=None):
+        """attn_slabs (or None: the packed weights): dict(map=device int32 [N], layers={attention layer -> (wqkv fp16
+        [slabs, 3C, C], wproj fp16 [slabs, C, C])}).  Image n's qkv and proj_out GEMMs then multiply slab map[n] of its
+        layer's tables (k2_conv_gemm_wmap), read when the launch runs: rewriting the map or a slab changes what a replay of
+        the plan computes without moving a buffer."""
         pk = model._packed
         dev = pk["te0_w"].device
         super().__init__(dev, N)
@@ -506,6 +519,7 @@ class _Plan(LaunchPlan):
         self.xf_proj = torch.zeros(N, 4 * model.model_channels, **f32)
         self.enc_kv = {}
         self._bound = None
+        self.attn_slabs = attn_slabs
         self._build()
 
     def bind(self, cond):
@@ -644,7 +658,17 @@ class _Plan(LaunchPlan):
         enc = self._new(N, self.ctx, 2 * ch)
         self.enc_kv[p] = enc
         self._norm(a, None, d["g"], d["b"], xn, act=0)
-        self._gemm(xn.view(N, T, ch), d["wqkv"], 3 * ch, qkv, 2 * N * T * 3 * ch * ch, bias=d["bqkv"])
+        wproj, mapped = d["wproj"], {}
+        if self.attn_slabs is None:
+            self._gemm(xn.view(N, T, ch), d["wqkv"], 3 * ch, qkv, 2 * N * T * 3 * ch * ch, bias=d["bqkv"])
+        else:
+            # batched GEMMs over the N images of T tokens, image n with slab map[n]
+            wqkv, wproj = self.attn_slabs["layers"][p]
+            mapped = dict(w_map=self.attn_slabs["map"], n_slabs=wqkv.shape[0])
+            self._conv([(xn, 1)], wqkv[0], 3 * ch, qkv.view(N, Hh, Ww, 3 * ch), 2 * N * T * 3 * ch * ch, bias=d["bqkv"],
+                       want_stats=False, w_batch_stride=wqkv.stride(0), **mapped)
+            mapped["w_batch_stride"] = wproj.stride(0)
+            wproj = wproj[0]
         S(lambda: ops.attention_d64(qkv, heads, enc, out=att), "attention", 4 * N * T * (T + self.ctx) * ch)
-        self._conv([(att.view(N, Hh, Ww, ch), 1)], d["wproj"], ch, o, 2 * N * T * ch * ch, bias=d["bproj"], residual=a)
+        self._conv([(att.view(N, Hh, Ww, ch), 1)], wproj, ch, o, 2 * N * T * ch * ch, bias=d["bproj"], residual=a, **mapped)
         return o

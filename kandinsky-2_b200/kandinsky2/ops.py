@@ -105,16 +105,20 @@ def _workspace(dev):
 
 
 def conv_gemm(srcs, w_packed, cout, bias=None, residual=None, out=None, out_mode=0, geom=None, gn_part=None, info=None,
-              cfg=None, w_batch_stride=0):
+              cfg=None, w_batch_stride=0, w_map=None, n_slabs=0):
     """srcs: list of (tensor NHWC fp16 [NB,H,W,C], taps); taps = 9 (3x3), 1 (1x1) or 4 (single source: 3x3 over its nearest-2x
     upsampling, weights from pack_conv_weight_up2, output [NB,2H,2W,cout]).  Returns fp16 [NB,H,W,cout] (out_mode 0) or
     fp32 NCHW [NB,cout,H,W] (out_mode 1).  geom=(NB,H,W) overrides the geometry (GEMM on flat rows).
     cfg = (N tile, pair mode, splits, epilogue sets) overrides the library's choice (k2_conv_gemm_cfg; 0 = auto).
     w_batch_stride > 0: batched GEMM, image n uses the weight matrix at w_packed + n * w_batch_stride elements (w_packed is then
-    any fp16 tensor whose data_ptr() is matrix 0, shape[0] / shape[1] / stride(0) = rows / K / row stride of ONE matrix)."""
+    any fp16 tensor whose data_ptr() is matrix 0, shape[0] / shape[1] / stride(0) = rows / K / row stride of ONE matrix).
+    w_map (device int32 [NB], with n_slabs >= 1 and w_batch_stride > 0): image n uses slab w_map[n] of the n_slabs matrices
+    instead of matrix n (k2_conv_gemm_wmap); the kernel reads the map when it runs, so a captured graph follows its contents."""
     lib = nat.load()
     t0 = srcs[0][0]
     NB, H, W = geom if geom is not None else t0.shape[:3]
+    if w_map is not None:
+        _check_w_map(w_map, NB, n_slabs)
     if srcs[0][1] == 4:  # 3x3 conv over the nearest-2x upsampling of the source: geometry = the OUTPUT's
         H, W = 2 * H, 2 * W
     arr = (K2ConvSrc * len(srcs))()
@@ -135,13 +139,29 @@ def conv_gemm(srcs, w_packed, cout, bias=None, residual=None, out=None, out_mode
     ws = _workspace(t0.device)
     _info = (ctypes.c_int * 7)()
     _cfg = (ctypes.c_int * 4)(*cfg) if cfg is not None else None
-    check(lib.k2_conv_gemm_cfg(arr, len(srcs), NB, H, W, ptr(w_packed), w_packed.shape[0], w_packed.shape[1],
-                               w_packed.stride(0), cout,
-                               ptr(bias), ptr(residual), ldr, ptr(out), ldo, out_mode, ptr(ws), ws.numel(), ptr(gn_part),
-                               _info, _cfg, int(w_batch_stride), stream_ptr()))
+    args = (arr, len(srcs), NB, H, W, ptr(w_packed), w_packed.shape[0], w_packed.shape[1], w_packed.stride(0), cout,
+            ptr(bias), ptr(residual), ldr, ptr(out), ldo, out_mode, ptr(ws), ws.numel(), ptr(gn_part), _info, _cfg,
+            int(w_batch_stride))
+    if w_map is None:
+        check(lib.k2_conv_gemm_cfg(*args, stream_ptr()))
+    else:
+        check(lib.k2_conv_gemm_wmap(*args, int(n_slabs), ptr(w_map), stream_ptr()))
     if info is not None:
         info[:] = list(_info)
     return out
+
+
+def _check_w_map(w_map, NB, n_slabs):
+    """The weight-slab map of a mapped batched GEMM: a contiguous int32 device tensor of one entry per image."""
+    if not torch.is_tensor(w_map) or not w_map.is_cuda:
+        raise nat.K2Error("conv_gemm: w_map must be an int32 tensor on a CUDA sm_90 device (the kernel reads it)")
+    if w_map.dtype != torch.int32 or not w_map.is_contiguous():
+        raise nat.K2Error(f"conv_gemm: w_map must be a contiguous int32 tensor, got {w_map.dtype}"
+                          f"{'' if w_map.is_contiguous() else ' (non-contiguous)'}")
+    if w_map.numel() != NB:
+        raise nat.K2Error(f"conv_gemm: w_map must hold one slab index per image ({NB}), got {tuple(w_map.shape)}")
+    if isinstance(n_slabs, bool) or not isinstance(n_slabs, int) or n_slabs < 1:
+        raise nat.K2Error(f"conv_gemm: n_slabs must be an int >= 1 with a w_map, got {n_slabs!r}")
 
 
 def conv_plan(NB, H, W, taps, ktot, cout, out_mode=0, workspace_bytes=_CONV_WS_BYTES, want_gn_partial=True):

@@ -392,13 +392,15 @@ class Kandinsky2_2(_DecoderBase):
             return self.embedder.image_emb(negative_decoder_prompt, batch_size)
         return self.embedder.image_emb(negative_decoder_prompt, batch_size, **{**prior_kw, "negative_prior_prompt": ""})
 
-    def batcher(self, max_batch, h, w, sampler="ddpm_sampler", max_steps=100):
+    def batcher(self, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
         """A batching.Batcher: text2img requests submitted one at a time and served from one continuously refilled batch of
         max_batch slots at h x w (rounded up to multiples of 64, as generate_text2img does), every slot at its own denoising
         step.  sampler: "ddpm_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's
-        decoder_steps (the per-slot tables are sized for it)."""
+        decoder_steps (the per-slot tables are sized for it).  max_loras > 0 lets each request name its own LoRA adapter of
+        the decoder (Batcher.add_lora, submit(lora=...)); the batcher then keeps copies of the attention weights, so
+        load_lora / unload_lora on this pipeline afterwards do not change what it computes."""
         from .batching import Batcher
-        return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps)
+        return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
 
     def generate_text2img(self, prompt, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                           prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
