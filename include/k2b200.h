@@ -249,7 +249,8 @@ int k2_step_begin(const float* x, float* x_in, long long n, float* t_in, int nt,
 int k2_step_end(int* counter, k2_stream_t stream);
 
 /* The same step for a continuously refilled batch of S slots, each slot a request at its own step of its own schedule
- * (kandinsky2/batching.py; Kandinsky 2.2 row order: unconditional row s, conditional row S + s of the CFG-doubled UNet batch).
+ * (kandinsky2/batching.py; row order, unless cond_first says otherwise: unconditional row s, conditional row S + s of the
+ * CFG-doubled UNet batch, as Kandinsky 2.2 orders them).
  * state is a device int32 [2][S] = (k_s, steps_s); slot s is ACTIVE while 0 <= k_s < steps_s (and, for the tables,
  * k_s < kmax); k_s = -1 marks a free slot.  n = 4 H W floats per slot.
  *   k2_slot_step_begin: for an active slot, x_in rows s and S + s = x[s]; t_in[s] = t_in[S + s] = ts_tab[s][k_s];
@@ -261,6 +262,11 @@ int k2_step_end(int* counter, k2_stream_t stream);
  *     coefficient row coef[s] (the coef_out above) and guidance scale guidance[s] (device fp32 [S]); work fp32 [S][n].
  *   k2_slot_dpm_solver_step: k2_dpm_solver_step (cond_first 0, no inpainting) per slot, rows and guidance as above, hist fp32
  *     [S][n] per slot.
+ *   k2_slot_sampler_step_ex: k2_slot_sampler_step with the row order cond_first (1: conditional row s, unconditional row
+ *     S + s, the Kandinsky 2.1 order) and threshold_mode 0 or 1.  threshold_mode 1 is k2_sampler_step's dynamic threshold
+ *     with each slot's own percentile: sval[s] = max(99.5th percentile of |x0| over slot s's n elements, 1), written to sval
+ *     (device fp32 [S], required) and applied to that slot alone, which is what k2_sampler_step computes at B = 1.
+ *   k2_slot_dpm_solver_step_ex: k2_slot_dpm_solver_step with the row order cond_first.
  * The step entries run the same kernels as their batch forms, so an active slot's result is bit-identical to the batch form
  * applied to that slot alone; they neither read nor write an inactive slot's elements (its rows of model_out may hold NaN).
  * Arguments are checked before any CUDA call. */
@@ -272,6 +278,11 @@ int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, c
                          const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream);
 int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
                             const int* state, int S, int H, int W, k2_stream_t stream);
+int k2_slot_sampler_step_ex(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
+                            float* work, k2_stream_t stream);
+int k2_slot_dpm_solver_step_ex(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                               const int* state, int S, int H, int W, int cond_first, k2_stream_t stream);
 
 /* PLMS / DDIM update with an explicit epsilon history (replaces PLMSSampler.p_sample_plms, samplers.py:571-637, and the
  * CFG closure): e_t = uncond + g (cond - uncond) from model_out's first 4 channels (C2 channels per sample);

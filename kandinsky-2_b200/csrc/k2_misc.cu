@@ -258,7 +258,7 @@ struct SamplerParams {
   const float* mask;       // [B,1,H,W] or null
   const float* rnoise;     // [B,4,H,W] or null: inpainting blends x_{t-1} with the re-noised init (diffusers) instead of x0
   float* x0;               // work [B*4*HW]
-  float* sval;             // work scalar (dynamic threshold s)
+  float* sval;             // work scalar (dynamic threshold s); slot form: [B], one per slot
   const int* slots;        // slot form: int32 [2][B] = (step k_s, steps of the slot); coef is [B][8], guidance gscale[B]
   const float* gscale;
 };
@@ -358,11 +358,21 @@ __device__ float radix_select(const float* __restrict__ v, int n, int rank, unsi
   return __uint_as_float(prefix);
 }
 
-__global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* __restrict__ x0, int n, float* sval) {
+// kSlots: the slot form (k2_slot_sampler_step_ex), one CTA per slot s = blockIdx.x of gridDim.x slots: the percentile of slot
+// s's own n elements x0[s n, (s + 1) n) into sval[s]; an idle slot reads and writes nothing.
+template <bool kSlots>
+__global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* __restrict__ x0, int n, float* sval,
+                                                                  const int* __restrict__ slots) {
   __shared__ unsigned int hist[256];
   __shared__ unsigned int sh[2];
   pdl_wait();
   pdl_launch();
+  if (kSlots) {
+    const int s = blockIdx.x;
+    if (!slot_active(slots, gridDim.x, s)) return;
+    x0 += static_cast<long long>(n) * s;
+    sval += s;
+  }
   const double pos = 0.995 * static_cast<double>(n - 1);
   int lo = static_cast<int>(floor(pos));
   const double frac = pos - lo;
@@ -378,7 +388,8 @@ __global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* _
   }
 }
 
-template <bool kSlots>
+// kSlotThreshold (slot form only): the dynamic threshold of an element is its slot's sval[s] (k2_slot_sampler_step_ex)
+template <bool kSlots, bool kSlotThreshold = false>
 __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_wait();
@@ -394,7 +405,7 @@ __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p
   const int bc = p.cond_first ? b : b + p.B;
   float x0 = p.x0[i];
   if (p.threshold_mode == 1) {
-    const float s = *p.sval;
+    const float s = kSlotThreshold ? p.sval[b] : *p.sval;
     x0 = fminf(fmaxf(x0, -s), s) / s;
   }
   const float mean = coef[2] * x0 + coef[3] * p.x[i];
@@ -899,8 +910,8 @@ int k2_sampler_step(const float* model_out, float* x, const float* noise, const 
     count_launch();
   }
   if (do_pct) {
-    K2_CHECK_CUDA(launch_k(sampler_percentile_kernel, dim3(1), dim3(1024), 0, st, static_cast<const float*>(p.x0), 4 * H * W,
-                           p.sval));
+    K2_CHECK_CUDA(launch_k(sampler_percentile_kernel<false>, dim3(1), dim3(1024), 0, st, static_cast<const float*>(p.x0),
+                           4 * H * W, p.sval, static_cast<const int*>(nullptr)));
     count_launch();
   }
   if (do_post) {
@@ -1017,31 +1028,61 @@ int k2_slot_step_end(int* state, int S, k2_stream_t stream) {
   return 0;
 }
 
-int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
-                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream) {
-  K2_REQUIRE(model_out && x && noise && coef && guidance && state && work, "slot_sampler_step: null pointer");
-  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1, "slot_sampler_step: S, H, W must be >= 1");
+// The slot steps' shared bodies: the old entries are the new ones at cond_first 0 without the threshold (`name` prefixes the
+// error messages).
+static int slot_sampler_step(const char* name, const float* model_out, float* x, const float* noise, const float* coef,
+                             const float* guidance, const int* state, int S, int H, int W, float clip, int cond_first,
+                             int threshold_mode, float* sval, float* work, k2_stream_t stream) {
+  const std::string who(name);
+  K2_REQUIRE(model_out && x && noise && coef && guidance && state && work, who + ": null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1, who + ": S, H, W must be >= 1");
+  K2_REQUIRE(cond_first == 0 || cond_first == 1, who + ": cond_first must be 0 or 1");
+  K2_REQUIRE(threshold_mode == 0 || threshold_mode == 1, who + ": threshold_mode must be 0 or 1");
+  K2_REQUIRE(threshold_mode == 0 || sval, who + ": threshold_mode 1 needs sval");
   SamplerParams p;
   p.model_out = model_out; p.x = x; p.noise = noise; p.coef = coef;
-  p.B = S; p.HW = H * W; p.guidance = 0.f; p.cond_first = 0; p.clip = clip; p.threshold_mode = 0;
+  p.B = S; p.HW = H * W; p.guidance = 0.f; p.cond_first = cond_first; p.clip = clip; p.threshold_mode = threshold_mode;
   p.init = nullptr; p.mask = nullptr; p.rnoise = nullptr;
-  p.x0 = work; p.sval = nullptr; p.slots = state; p.gscale = guidance;
+  p.x0 = work; p.sval = sval; p.slots = state; p.gscale = guidance;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long total = static_cast<long long>(S) * 4 * H * W;
   K2_CHECK_CUDA(launch_k(sampler_x0_kernel<true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
   count_launch();
-  K2_CHECK_CUDA(launch_k(sampler_post_kernel<true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+  if (threshold_mode == 1) {
+    K2_CHECK_CUDA(launch_k(sampler_percentile_kernel<true>, dim3(S), dim3(1024), 0, st, static_cast<const float*>(work),
+                           4 * H * W, sval, state));
+    count_launch();
+    K2_CHECK_CUDA(launch_k(sampler_post_kernel<true, true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+  } else {
+    K2_CHECK_CUDA(launch_k(sampler_post_kernel<true>, dim3(blocks_for(total, 256)), dim3(256), 0, st, p));
+  }
   count_launch();
   return 0;
 }
 
-int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
-                            const int* state, int S, int H, int W, k2_stream_t stream) {
-  K2_REQUIRE(model_out && x && hist && coef && guidance && state, "slot_dpm_solver_step: null pointer");
-  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1 && C2 >= 4, "slot_dpm_solver_step: S, H, W must be >= 1 and C2 >= 4");
+int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream) {
+  return slot_sampler_step("slot_sampler_step", model_out, x, noise, coef, guidance, state, S, H, W, clip, 0, 0, nullptr, work,
+                           stream);
+}
+
+int k2_slot_sampler_step_ex(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
+                            float* work, k2_stream_t stream) {
+  return slot_sampler_step("slot_sampler_step_ex", model_out, x, noise, coef, guidance, state, S, H, W, clip, cond_first,
+                           threshold_mode, sval, work, stream);
+}
+
+static int slot_dpm_solver_step(const char* name, const float* model_out, int C2, float* x, float* hist, const float* coef,
+                                const float* guidance, const int* state, int S, int H, int W, int cond_first,
+                                k2_stream_t stream) {
+  const std::string who(name);
+  K2_REQUIRE(model_out && x && hist && coef && guidance && state, who + ": null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1 && C2 >= 4, who + ": S, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE(cond_first == 0 || cond_first == 1, who + ": cond_first must be 0 or 1");
   DpmParams p;
   p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
-  p.B = S; p.HW = H * W; p.C2 = C2; p.guidance = 0.f; p.cond_first = 0;
+  p.B = S; p.HW = H * W; p.C2 = C2; p.guidance = 0.f; p.cond_first = cond_first;
   p.init = nullptr; p.mask = nullptr; p.rnoise = nullptr; p.noise = nullptr;
   p.slots = state; p.gscale = guidance;
   const long long total = static_cast<long long>(S) * 4 * H * W;
@@ -1049,6 +1090,17 @@ int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* his
                          static_cast<cudaStream_t>(stream), p));
   count_launch();
   return 0;
+}
+
+int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, k2_stream_t stream) {
+  return slot_dpm_solver_step("slot_dpm_solver_step", model_out, C2, x, hist, coef, guidance, state, S, H, W, 0, stream);
+}
+
+int k2_slot_dpm_solver_step_ex(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                               const int* state, int S, int H, int W, int cond_first, k2_stream_t stream) {
+  return slot_dpm_solver_step("slot_dpm_solver_step_ex", model_out, C2, x, hist, coef, guidance, state, S, H, W, cond_first,
+                              stream);
 }
 
 int k2_upsample2x_nhwc(const void* x, int ldx, void* y, int ldy, int NB, int H, int W, int C, k2_stream_t stream) {

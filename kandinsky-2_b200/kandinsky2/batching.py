@@ -1,17 +1,20 @@
-"""Continuous batching of Kandinsky 2.2 text2img requests: one CFG-doubled UNet batch of S slots, every slot a request at its
-own denoising step, refilled from a FIFO queue as requests finish.
+"""Continuous batching of Kandinsky 2.2 (Batcher) and 2.1 (Batcher21) text2img requests: one CFG-doubled UNet batch of S
+slots, every slot a request at its own denoising step, refilled from a FIFO queue as requests finish.
 
-Rows follow the 2.2 layout, unconditional s and conditional S + s for slot s.  The device keeps per slot its step index, its
-timestep / coefficient / per-step noise tables and its guidance scale (k2b200.h: k2_slot_step_begin); one step of the whole
+Rows follow the version's layout: for slot s, unconditional s and conditional S + s in 2.2, the reverse in 2.1.  The device
+keeps per slot its step index, its timestep / coefficient / per-step noise tables and its guidance scale (k2b200.h:
+k2_slot_step_begin); one step of the whole
 batch is ONE captured CUDA graph (k2_slot_step_begin, the UNet plan, the slot form of the sampler step, k2_slot_step_end)
 whose buffers never move, so admitting a request is a handful of copies into them and the host loop reads nothing back from
 the device: it knows from its own bookkeeping which slot finishes at which step.
 
 A request computes what generate_text2img(batch_size=1) computes on a pipeline whose base_seed is the request's seed: the same
-start latent and per-step noise draws, the same tables (create_ddpm_v22 / the SCHEDULE_SAMPLERS builders), the same
-conditioning and step kernels.  Its result does not depend on the other slots: the UNet's normalisation, attention and
-convolutions are per image, the conditioning is written per row (Text2ImUNet.bind_slot) and the slot step kernels read and
-write only the rows of active slots.  An idle slot still costs a full row of UNet compute.
+start latent and per-step noise draws, the same tables (request_tables / request_tables_21: the builders the sampling loops
+use), the same conditioning and step kernels.  Its result does not depend on the other slots: the UNet's normalisation,
+attention and convolutions are per image, the conditioning is written per row (Text2ImUNet.bind_slot) and the slot step
+kernels read and write only the rows of active slots.  2.1's p_sampler clips x0 with the 99.5 percentile of the request's own
+x0 (at batch 1 the reference's "sample 0" is the request itself): the slot step computes one percentile per slot.  An idle
+slot still costs a full row of UNet compute.
 
 With max_loras = L > 0 each request may name a LoRA adapter registered with add_lora.  The attention layers' qkv and proj_out
 weights then live in slab tables of 1 + L fp16 copies per layer (slab 0: the pipeline's packed weights when the batcher was
@@ -27,16 +30,26 @@ import torch
 from . import ops, parallel
 from ._native import K2Error
 from .launch_plan import capture_graph
-from .model.gaussian_diffusion import create_ddpm_v22
+from .model.gaussian_diffusion import DDIMSampler, create_ddpm_v22, create_gaussian_diffusion
 from .model.unet import _Plan
 
 BATCHER_SAMPLERS = ("ddpm_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
+# Kandinsky 2.1's: PLMS is not among them, its first step evaluates the UNet twice and it keeps its epsilon history on the host
+BATCHER_SAMPLERS_21 = ("p_sampler", "ddim_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
+
+# sampler -> (its slot step: "ddpm" = ops.slot_sampler_step, "dpm" = ops.slot_dpm_solver_step; the +-clip of x0 and the
+# threshold_mode of the "ddpm" step; whether the step draws noise), as the sampling loops run each sampler
+SLOT_STEPS = {"ddpm_sampler": ("ddpm", 2.0, 0, True),
+              "p_sampler": ("ddpm", 2.0, 1, True),      # p_sample_loop(clip_denoised=True): +-2, then the dynamic threshold
+              "ddim_sampler": ("ddpm", 1e30, 0, False),  # DDIMSampler: eta 0, linear coefficients, no clamp
+              "dpmpp_2m_sampler": ("dpm", None, 0, False),
+              "dpmpp_2m_karras_sampler": ("dpm", None, 0, False)}
 
 
-def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0):
+def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0, samplers=BATCHER_SAMPLERS):
     """Refuse what a Batcher cannot serve, before any work: ValueError naming the argument."""
-    if sampler not in BATCHER_SAMPLERS:
-        raise ValueError(f"batcher: sampler {sampler!r} is not served; use one of {', '.join(BATCHER_SAMPLERS)}")
+    if sampler not in samplers:
+        raise ValueError(f"batcher: sampler {sampler!r} is not served; use one of {', '.join(samplers)}")
     for name, v in (("max_batch", max_batch), ("h", h), ("w", w), ("max_steps", max_steps)):
         if isinstance(v, bool) or not isinstance(v, int) or v < 1:
             raise ValueError(f"batcher: {name} must be a positive int, got {v!r}")
@@ -49,7 +62,27 @@ def request_tables(sampler, steps):
     loop of generate_text2img stages for `sampler` at decoder_steps = steps, from the same schedule builders."""
     from .pipelines import _solver_schedule
     diffusion = create_ddpm_v22(steps)
-    sched = diffusion if sampler == "ddpm_sampler" else _solver_schedule(sampler, diffusion, steps)
+    return _loop_rows(diffusion if sampler == "ddpm_sampler" else _solver_schedule(sampler, diffusion, steps))
+
+
+def request_tables_21(sampler, steps, diffusion_config):
+    """request_tables for Kandinsky 2.1 at num_steps = steps: the rows its sampling loops stage for `sampler` over the
+    pipeline's diffusion_config.  p_sampler respaces the diffusion to `steps`; ddim_sampler runs DDIMSampler's schedule over
+    the un-respaced one (timesteps range(0, 1000, 1000 // steps): more rows than steps when steps does not divide 1000); the
+    solvers run _solver_schedule over its base table."""
+    from .pipelines import _solver_schedule
+    if sampler == "p_sampler":
+        return _loop_rows(create_gaussian_diffusion(**dict(diffusion_config, timestep_respacing=str(steps))))
+    diffusion = create_gaussian_diffusion(**diffusion_config)
+    if sampler == "ddim_sampler":
+        sched = DDIMSampler(None, diffusion)
+        sched.make_schedule(steps)
+        return _loop_rows(sched)
+    return _loop_rows(_solver_schedule(sampler, diffusion, steps))
+
+
+def _loop_rows(sched):
+    """(timesteps, coefficient rows) of a schedule in the order _sampling_loop runs them, last table row first."""
     coef, ts = sched._tables("cpu")
     order = torch.arange(sched.num_timesteps - 1, -1, -1)
     return ts[order].contiguous(), coef[order].contiguous()
@@ -101,21 +134,36 @@ class SlotQueue:
 
 
 class _Request:
-    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora")
+    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora", "full", "pooled")
+
+
+def _check_embedding(name, e, dim):
+    if e is not None and (not torch.is_tensor(e) or e.numel() != dim or e.dim() not in (1, 2) or not e.is_floating_point()):
+        raise ValueError(f"submit: {name} must be one floating-point image embedding, [1, {dim}] or [{dim}], got "
+                         f"{tuple(e.shape) if torch.is_tensor(e) else type(e).__name__}")
+
+
+def _check_steps(name, steps, max_steps):
+    if isinstance(steps, bool) or not isinstance(steps, int) or not 1 <= steps <= max_steps:
+        raise ValueError(f"submit: {name} must be an int in [1, {max_steps}] (the batcher's max_steps), got {steps!r}")
 
 
 class Batcher:
-    """Requests of one geometry and one sampler served from max_batch slots (Kandinsky2_2.batcher builds it)."""
+    """Kandinsky 2.2 requests of one geometry and one sampler served from max_batch slots (Kandinsky2_2.batcher builds it).
+    What differs between the versions is a class attribute or one of the methods Batcher21 overrides: the sampler set, the
+    row order, the geometry and context length, the tables, submit's keywords and the conditioning a slot is bound to."""
 
     RUN_AHEAD = 2   # replayed steps the host may have in flight on the GPU when it admits (2: the GPU never waits on admission)
+    SAMPLERS = BATCHER_SAMPLERS
+    COND_FIRST = 0   # 2.2: the unconditional row of slot s is s
 
     def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
-        check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras)
+        self._check_args(max_batch, h, w, sampler, max_steps, max_loras)
         if pipe.task_type != "text2img":
             raise ValueError(f"batcher: serves text2img pipelines only, this one is {pipe.task_type!r}")
         self.pipe, self.sampler, self.max_steps = pipe, sampler, max_steps
-        self.h, self.w = pipe.get_new_h_w(h, w)
-        S, H, W = max_batch, self.h // 8, self.w // 8
+        self.h, self.w, H, W = self._geometry(h, w)
+        S = max_batch
         model = pipe.model
         if model._packed is None:
             model.finalize()
@@ -140,7 +188,7 @@ class Batcher:
                 self._wenc0[name] = a["wenc"].clone()
             slabs = dict(map=self.w_map, layers=layers)
         # a plan of its own: another call on the pipeline at the same geometry must not rebind these rows
-        self.plan = p = _Plan(model, 2 * S, H, W, model.num_image_embs, attn_slabs=slabs)
+        self.plan = p = _Plan(model, 2 * S, H, W, self._context(), attn_slabs=slabs)
         p.xf_proj.zero_()
         for buf in p.enc_kv.values():
             buf.zero_()
@@ -151,11 +199,14 @@ class Batcher:
         self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
         self.coef = torch.zeros(S, 8, **f32)
         self.guidance = torch.zeros(S, **f32)
-        ddpm = sampler == "ddpm_sampler"
-        # the DDPM step's noise for every step of every slot, drawn at admission: S x max_steps x 4 H W floats
-        self.noise_tab = torch.zeros(S, max_steps, 4, H, W, **f32) if ddpm else None
+        kind, self.clip, self.threshold_mode, draws_noise = SLOT_STEPS[sampler]
+        ddpm = kind == "ddpm"
+        # the DDPM step's noise for every step of every slot, drawn at admission: S x max_steps x 4 H W floats (DDIM at eta 0
+        # reads no noise: its noise buffer stays zero)
+        self.noise_tab = torch.zeros(S, max_steps, 4, H, W, **f32) if draws_noise else None
         self.noise = torch.zeros(S, 4, H, W, **f32) if ddpm else None
         self.work = torch.zeros(S, 4, H, W, **f32) if ddpm else None
+        self.sval = torch.zeros(S, **f32) if self.threshold_mode else None   # each slot's dynamic threshold
         self.hist = None if ddpm else torch.zeros(S, 4, H, W, **f32)
         self.queue = SlotQueue(S)
         self._requests = {}
@@ -174,11 +225,23 @@ class Batcher:
         ops.slot_step_begin(self.x, p.x_in, p.t_in, self.coef, self.ts_tab, self.coef_tab, self.noise_tab, self.noise,
                             self.state)
         p.launch()
-        if self.sampler == "ddpm_sampler":
-            ops.slot_sampler_step(p.out, self.x, self.noise, self.coef, self.guidance, self.state, self.work)
+        if self.hist is None:
+            ops.slot_sampler_step(p.out, self.x, self.noise, self.coef, self.guidance, self.state, self.work, self.clip,
+                                  cond_first=self.COND_FIRST, threshold_mode=self.threshold_mode, sval=self.sval)
         else:
-            ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state)
+            ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state, cond_first=self.COND_FIRST)
         ops.slot_step_end(self.state)
+
+    def _check_args(self, max_batch, h, w, sampler, max_steps, max_loras):
+        check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras, self.SAMPLERS)
+
+    def _geometry(self, h, w):
+        """-> (decoded image height, width, latent height, width): 2.2 rounds the image up to multiples of 64."""
+        h, w = self.pipe.get_new_h_w(h, w)
+        return h, w, h // 8, w // 8
+
+    def _context(self):
+        return self.pipe.model.num_image_embs
 
     def add_lora(self, name, state_dict, scale=1.0):
         """Register a LoRA adapter of the decoder's attention blocks under `name` (the format Text2ImUNet.load_lora takes):
@@ -233,18 +296,13 @@ class Batcher:
         if image_embeds is not None and negative_image_embeds is None:
             raise ValueError("submit: image_embeds needs negative_image_embeds")
         for name, e in (("image_embeds", image_embeds), ("negative_image_embeds", negative_image_embeds)):
-            if e is not None and (not torch.is_tensor(e) or e.numel() != self._emb_dim or e.dim() not in (1, 2)
-                                  or not e.is_floating_point()):
-                raise ValueError(f"submit: {name} must be one floating-point image embedding, [1, {self._emb_dim}] or "
-                                 f"[{self._emb_dim}], got {tuple(e.shape) if torch.is_tensor(e) else type(e).__name__}")
-        if isinstance(decoder_steps, bool) or not isinstance(decoder_steps, int) or not 1 <= decoder_steps <= self.max_steps:
-            raise ValueError(f"submit: decoder_steps must be an int in [1, {self.max_steps}] (the batcher's max_steps), "
-                             f"got {decoder_steps!r}")
+            _check_embedding(name, e, self._emb_dim)
+        _check_steps("decoder_steps", decoder_steps, self.max_steps)
         if lora is not None and lora not in self._loras:
             raise ValueError(f"submit: no adapter named {lora!r} is registered (Batcher.add_lora)")
         r = _Request()
         r.lora = lora
-        r.steps, r.guidance = decoder_steps, float(decoder_guidance_scale)
+        r.guidance = float(decoder_guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
         r.ts, r.coef = request_tables(self.sampler, decoder_steps)
         if prompt is not None:
@@ -252,10 +310,18 @@ class Batcher:
             r.positive, r.negative = pipe._embeds(prompt, 1, negative_decoder_prompt, pk)
         else:
             r.positive, r.negative = image_embeds, negative_image_embeds
+        return self._enqueue(r)
+
+    def _enqueue(self, r):
+        """Queue a request whose tables are set -> its handle; it runs one step per row of its tables."""
+        r.steps = r.ts.shape[0]
+        if r.steps > self.max_steps:
+            raise ValueError(f"submit: the request's schedule has {r.steps} steps, more than the batcher's max_steps "
+                             f"{self.max_steps}")
         handle = self._next_handle
         self._next_handle += 1
         self._requests[handle] = r
-        self.queue.submit(handle, decoder_steps)
+        self.queue.submit(handle, r.steps)
         return handle
 
     def _admit(self):
@@ -275,14 +341,18 @@ class Batcher:
                 del self._requests[handle]
                 raise
 
-    def _stage(self, s, r):
-        pipe, H, W = self.pipe, self.x.shape[2], self.x.shape[3]
+    def _bind(self, s, r):
+        """Write request r's conditioning into slot s's rows of the plan."""
         if self.w_map is None:
-            pipe.model.bind_slot(self.plan, s, r.negative, r.positive)
+            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive)
         else:
             k, wenc = self._loras[r.lora] if r.lora is not None else (0, self._wenc0)
-            pipe.model.bind_slot(self.plan, s, r.negative, r.positive, wenc=wenc)
+            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, wenc=wenc)
             self._set_slab(s, k)
+
+    def _stage(self, s, r):
+        pipe, H, W = self.pipe, self.x.shape[2], self.x.shape[3]
+        self._bind(s, r)
         k = r.steps
         self.ts_tab[s, :k].copy_(r.ts)
         self.coef_tab[s, :k].copy_(r.coef)
@@ -291,7 +361,7 @@ class Batcher:
         if self.noise_tab is not None:
             gen = pipe._generators(0, 1, base_seed=r.seed)[0]
             self.noise_tab[s, :k].copy_(torch.randn(k, 4, H, W, device=pipe.device, generator=gen))
-        else:
+        if self.hist is not None:
             self.hist[s].zero_()
         self.guidance[s] = r.guidance
         self.state[:, s] = torch.tensor([0, k], dtype=torch.int32)
@@ -329,3 +399,60 @@ class Batcher:
         while self.queue.waiting or self.queue.busy():
             out.update(self.step())
         return out
+
+
+class Batcher21(Batcher):
+    """Kandinsky 2.1 requests of one geometry and one sampler served from max_batch slots (Kandinsky2_1.batcher builds it).
+    Slot s owns the conditional row s and the unconditional row S + s.  Each row is conditioned on the text encoder's
+    full_emb / pooled_emb and an image embedding, so the plan's context is num_image_embs + the text length.  Decoded images
+    are cropped to h x w from the latent grid _new_h_w_latent_21(h, w), as generate_text2img crops them.  p_sampler's step
+    clips each slot's x0 with that slot's own 99.5 percentile."""
+
+    SAMPLERS = BATCHER_SAMPLERS_21
+    COND_FIRST = 1
+
+    def __init__(self, pipe, max_batch, h, w, sampler="ddim_sampler", max_steps=100, max_loras=0):
+        super().__init__(pipe, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
+
+    def _check_args(self, max_batch, h, w, sampler, max_steps, max_loras):
+        super()._check_args(max_batch, h, w, sampler, max_steps, max_loras)
+        if max_loras:
+            raise ValueError("batcher: max_loras must be 0 for Kandinsky 2.1; per-request LoRA adapters serve 2.2 only")
+
+    def _geometry(self, h, w):
+        return (h, w) + tuple(self.pipe.get_new_h_w(h, w))
+
+    def _context(self):
+        # the text rows' length is the embedder's: read it once from the embedding of ""
+        self._text_len = self.pipe.embedder.text_emb("", 1)[0].shape[1]
+        return self.pipe.model.num_image_embs + self._text_len
+
+    def submit(self, prompt, *, image_embeds=None, negative_image_embeds=None, num_steps=100, guidance_scale=7,
+               negative_decoder_prompt="", seed=None):
+        """Queue one image of Kandinsky2_1.generate_text2img(prompt, batch_size=1, ...) -> its handle (the key of its image in
+        what step() / run() return).  The text rows are the embedder's text_emb(prompt, 1); the image rows those
+        generate_text2img makes (the prior's embedding of prompt, and the zero image embedding or, with
+        negative_decoder_prompt, the prior's embedding of that).  image_embeds / negative_image_embeds ([1, D] or [D]) replace
+        either: prompt="" with image_embeds=embedder.interpolate(items, weights, 1) is mix_images(items, weights,
+        batch_size=1).  seed plays the part of the pipeline's base_seed (default: the pipeline's base_seed)."""
+        pipe = self.pipe
+        if not isinstance(prompt, str):
+            raise ValueError(f"submit: prompt must be a str, got {type(prompt).__name__}")
+        for name, e in (("image_embeds", image_embeds), ("negative_image_embeds", negative_image_embeds)):
+            _check_embedding(name, e, self._emb_dim)
+        _check_steps("num_steps", num_steps, self.max_steps)
+        r = _Request()
+        r.lora = None
+        r.guidance = float(guidance_scale)
+        r.seed = pipe.base_seed if seed is None else int(seed)
+        r.ts, r.coef = request_tables_21(self.sampler, num_steps, pipe.config["diffusion_config"])
+        r.full, r.pooled = pipe.embedder.text_emb(prompt, 1)
+        if r.full.shape[1] != self._text_len:
+            raise ValueError(f"submit: the embedder's text rows have length {r.full.shape[1]}, the batcher's {self._text_len}")
+        r.positive = image_embeds if image_embeds is not None else pipe.embedder.image_emb(prompt, 1)
+        r.negative = (negative_image_embeds if negative_image_embeds is not None
+                      else pipe._negative_image_emb(1, negative_decoder_prompt))
+        return self._enqueue(r)
+
+    def _bind(self, s, r):
+        self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, full_emb=r.full, pooled_emb=r.pooled)

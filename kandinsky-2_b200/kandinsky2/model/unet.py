@@ -423,28 +423,42 @@ class Text2ImUNet(nn.Module):
             self.cache = out
         return out
 
-    def bind_slot(self, plan, slot, negative_emb, positive_emb, wenc=None):
-        """Write the conditioning of slot `slot` of a plan of N = 2 S rows (Kandinsky 2.2 row order: negative_emb's row
-        `slot`, positive_emb's row S + slot; image embeddings [image_encoder_in_dim]) into the plan's xf_proj and encoder K/V
-        rows, leaving every other row and every buffer address (so a CUDA graph captured on the plan) as it is.
+    def bind_slot(self, plan, slot, negative_emb, positive_emb, wenc=None, full_emb=None, pooled_emb=None):
+        """Write the conditioning of slot `slot` of a plan of N = 2 S rows into the plan's xf_proj and encoder K/V rows, leaving
+        every other row and every buffer address (so a CUDA graph captured on the plan) as it is.  Image embeddings are
+        [image_encoder_in_dim].  Kandinsky 2.2: negative_emb goes to row `slot`, positive_emb to row S + slot.  Kandinsky 2.1
+        (the conditional rows first): row `slot` takes positive_emb, full_emb[0] and pooled_emb[0], row S + slot takes
+        negative_emb, full_emb[1] and pooled_emb[1] (full_emb [2, text_len, text_encoder_in_dim1], pooled_emb [2,
+        text_encoder_in_dim2]: the conditional and unconditional rows the text encoder gives for one prompt).
         Each output row of get_text_emb depends on its input row alone, but the encoder K/V GEMM picks its split-K factor
         from its row count (k2_conv_gemm), which changes the fp32 summation order; so the rows are computed at the plan's batch
         (the other input rows zero), and a slot's conditioning has the same bits in every slot and, at S = 1, those
         generate_text2img(batch_size=1) binds.  The model's cached conditioning is left untouched.
         wenc ({attention layer -> packed encoder_kv weight}, or None = the packed weights): the weights the slot's encoder K/V
         rows are computed with, e.g. the encoder_kv weights an adapter merges (the batcher's per-request adapters)."""
-        if self.cond_version == "2.1" or self.hint_channels:
-            raise K2Error("bind_slot: only the Kandinsky 2.2 text2img UNet takes per-slot conditioning")
+        v21 = self.cond_version == "2.1"
+        if self.hint_channels:
+            raise K2Error("bind_slot: only the text2img UNets take per-slot conditioning")
+        if v21 != (full_emb is not None) or v21 != (pooled_emb is not None):
+            raise K2Error("bind_slot: the Kandinsky 2.1 UNet needs full_emb and pooled_emb, the 2.2 one takes neither")
         S = plan.N // 2
         if not 0 <= slot < S:
             raise K2Error(f"bind_slot: slot {slot} outside [0, {S})")
+        first, second = (positive_emb, negative_emb) if v21 else (negative_emb, positive_emb)
         emb = torch.zeros(plan.N, negative_emb.shape[-1], device=plan.dev, dtype=torch.float32)
-        emb[slot] = negative_emb.reshape(-1).to(emb.device, torch.float32)
-        emb[S + slot] = positive_emb.reshape(-1).to(emb.device, torch.float32)
+        emb[slot] = first.reshape(-1).to(emb.device, torch.float32)
+        emb[S + slot] = second.reshape(-1).to(emb.device, torch.float32)
+        text = {}
+        if v21:
+            for name, t in (("full_emb", full_emb), ("pooled_emb", pooled_emb)):
+                rows = torch.zeros((plan.N,) + tuple(t.shape[1:]), device=plan.dev, dtype=torch.float32)
+                rows[slot] = t[0]
+                rows[S + slot] = t[1]
+                text[name] = rows
         saved, keep = self.cache, self.cache_text_emb
         self.cache, self.cache_text_emb = None, False
         try:
-            cond = self.get_text_emb(image_emb=emb)
+            cond = self.get_text_emb(image_emb=emb, **text)
         finally:
             self.cache, self.cache_text_emb = saved, keep
         if wenc is not None:

@@ -468,23 +468,27 @@ def _slot_step_operands(who, model_out, x, coef, guidance, state, c2, others):
     return S, H, W
 
 
-def slot_sampler_step(model_out, x, noise, coef, guidance, state, work, clip=2.0):
-    """k2_slot_sampler_step: the Kandinsky 2.2 DDPM step of every active slot of x fp32 [S, 4, H, W] in place, with the
-    slot's row of coef [S, 8] and its guidance [S] (device fp32); model_out [2S, 8, H, W], noise and work fp32 [S, 4, H, W]."""
+def slot_sampler_step(model_out, x, noise, coef, guidance, state, work, clip=2.0, *, cond_first=0, threshold_mode=0, sval=None):
+    """k2_slot_sampler_step_ex: the DDPM / DDIM step of every active slot of x fp32 [S, 4, H, W] in place, with the slot's row
+    of coef [S, 8] and its guidance [S] (device fp32); model_out [2S, 8, H, W], noise and work fp32 [S, 4, H, W].
+    cond_first: the row order (0: unconditional row s, conditional row S + s, Kandinsky 2.2; 1: the reverse, Kandinsky 2.1).
+    threshold_mode 1 clips each slot's x0 with its own dynamic threshold, written to sval fp32 [S]."""
     S, H, W = _slot_step_operands("slot_sampler_step", model_out, x, coef, guidance, state, 8,
                                   (("noise", noise), ("work", work)))
-    check(nat.load().k2_slot_sampler_step(ptr(model_out), ptr(x), ptr(noise), ptr(coef), ptr(guidance), ptr(state), S, H, W,
-                                          float(clip), ptr(work), stream_ptr()))
+    _slot_check("slot_sampler_step", S, 1, f32=(("sval", sval),), shaped=(("sval", sval, S),))
+    check(nat.load().k2_slot_sampler_step_ex(ptr(model_out), ptr(x), ptr(noise), ptr(coef), ptr(guidance), ptr(state), S, H, W,
+                                             float(clip), int(cond_first), int(threshold_mode), ptr(sval), ptr(work),
+                                             stream_ptr()))
     return x
 
 
-def slot_dpm_solver_step(model_out, x, hist, coef, guidance, state):
-    """k2_slot_dpm_solver_step: the DPM-Solver++(2M) step of every active slot of x fp32 [S, 4, H, W] in place, hist [S, 4, H, W]
-    per slot, model_out [2S, C2, H, W], rows and guidance as slot_sampler_step."""
+def slot_dpm_solver_step(model_out, x, hist, coef, guidance, state, *, cond_first=0):
+    """k2_slot_dpm_solver_step_ex: the DPM-Solver++(2M) step of every active slot of x fp32 [S, 4, H, W] in place, hist
+    [S, 4, H, W] per slot, model_out [2S, C2, H, W], rows, guidance and cond_first as slot_sampler_step."""
     S, H, W = _slot_step_operands("slot_dpm_solver_step", model_out, x, coef, guidance, state, model_out.shape[1],
                                   (("hist", hist),))
-    check(nat.load().k2_slot_dpm_solver_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef), ptr(guidance),
-                                             ptr(state), S, H, W, stream_ptr()))
+    check(nat.load().k2_slot_dpm_solver_step_ex(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef),
+                                                ptr(guidance), ptr(state), S, H, W, int(cond_first), stream_ptr()))
     return x
 
 

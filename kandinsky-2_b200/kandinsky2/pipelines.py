@@ -262,9 +262,20 @@ class Kandinsky2_1(_DecoderBase):
 
     def _image_embs(self, prompt, batch_size, negative_decoder_prompt=""):
         pos = self.embedder.image_emb(prompt, batch_size)
-        neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == ""
-               else self.embedder.image_emb(negative_decoder_prompt, batch_size))
-        return torch.cat([pos, neg], 0)
+        return torch.cat([pos, self._negative_image_emb(batch_size, negative_decoder_prompt)], 0)
+
+    def _negative_image_emb(self, batch_size, negative_decoder_prompt):
+        return (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == ""
+                else self.embedder.image_emb(negative_decoder_prompt, batch_size))
+
+    def batcher(self, max_batch, h, w, sampler="ddim_sampler", max_steps=100, max_loras=0):
+        """A batching.Batcher21: text2img requests submitted one at a time and served from one continuously refilled batch
+        of max_batch slots at h x w, every slot at its own denoising step; each request computes what
+        generate_text2img(batch_size=1) computes.  sampler: "p_sampler" (with the dynamic threshold of each request's own x0),
+        "ddim_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's steps (the per-slot
+        tables are sized for it).  Per-request LoRA adapters are not served here: max_loras must be 0."""
+        from .batching import Batcher21
+        return Batcher21(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
 
     def generate_text2img(self, prompt, num_steps=100, batch_size=1, guidance_scale=7, h=512, w=512,
                           sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25", negative_prior_prompt="",
