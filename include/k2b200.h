@@ -258,15 +258,13 @@ int k2_step_end(int* counter, k2_stream_t stream);
  *     places get zeros, so the UNet only sees finite input whatever the slot's buffers hold.  x fp32 [S][n], x_in [2S][n],
  *     t_in [2S], coef_out [S][8], ts_tab [S][kmax], coef_tab [S][kmax][8], noise_tab [S][kmax][n], noise [S][n].
  *   k2_slot_step_end: k_s += 1 for every active slot (a slot past its last step becomes inactive by itself).
- *   k2_slot_sampler_step: k2_sampler_step (threshold_mode 0, +-clip, cond_first 0, no inpainting) per slot, with the slot's
- *     coefficient row coef[s] (the coef_out above) and guidance scale guidance[s] (device fp32 [S]); work fp32 [S][n].
- *   k2_slot_dpm_solver_step: k2_dpm_solver_step (cond_first 0, no inpainting) per slot, rows and guidance as above, hist fp32
- *     [S][n] per slot.
- *   k2_slot_sampler_step_ex: k2_slot_sampler_step with the row order cond_first (1: conditional row s, unconditional row
- *     S + s, the Kandinsky 2.1 order) and threshold_mode 0 or 1.  threshold_mode 1 is k2_sampler_step's dynamic threshold
- *     with each slot's own percentile: sval[s] = max(99.5th percentile of |x0| over slot s's n elements, 1), written to sval
- *     (device fp32 [S], required) and applied to that slot alone, which is what k2_sampler_step computes at B = 1.
- *   k2_slot_dpm_solver_step_ex: k2_slot_dpm_solver_step with the row order cond_first.
+ *   k2_slot_sampler_step / k2_slot_dpm_solver_step: k2_sampler_step (+-clip, no inpainting) / k2_dpm_solver_step (no
+ *     inpainting) per slot, with the slot's coefficient row coef[s] (the coef_out above) and guidance scale guidance[s]
+ *     (device fp32 [S]); work and hist fp32 [S][n] per slot.  cond_first is the row order (1: conditional row s,
+ *     unconditional row S + s, the Kandinsky 2.1 order).  threshold_mode 1 is k2_sampler_step's dynamic threshold with each
+ *     slot's own percentile: sval[s] = max(99.5th percentile of |x0| over slot s's n elements, 1), written to sval (device
+ *     fp32 [S], required; unused at threshold_mode 0) and applied to that slot alone, which is what k2_sampler_step computes
+ *     at B = 1.
  * The step entries run the same kernels as their batch forms, so an active slot's result is bit-identical to the batch form
  * applied to that slot alone; they neither read nor write an inactive slot's elements (its rows of model_out may hold NaN).
  * Arguments are checked before any CUDA call. */
@@ -275,14 +273,10 @@ int k2_slot_step_begin(const float* x, float* x_in, int S, long long n, float* t
                        k2_stream_t stream);
 int k2_slot_step_end(int* state, int S, k2_stream_t stream);
 int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
-                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream);
+                         const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
+                         float* work, k2_stream_t stream);
 int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
-                            const int* state, int S, int H, int W, k2_stream_t stream);
-int k2_slot_sampler_step_ex(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
-                            const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
-                            float* work, k2_stream_t stream);
-int k2_slot_dpm_solver_step_ex(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
-                               const int* state, int S, int H, int W, int cond_first, k2_stream_t stream);
+                            const int* state, int S, int H, int W, int cond_first, k2_stream_t stream);
 
 /* PLMS / DDIM update with an explicit epsilon history (replaces PLMSSampler.p_sample_plms, samplers.py:571-637, and the
  * CFG closure): e_t = uncond + g (cond - uncond) from model_out's first 4 channels (C2 channels per sample);

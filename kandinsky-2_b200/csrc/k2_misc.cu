@@ -358,7 +358,7 @@ __device__ float radix_select(const float* __restrict__ v, int n, int rank, unsi
   return __uint_as_float(prefix);
 }
 
-// kSlots: the slot form (k2_slot_sampler_step_ex), one CTA per slot s = blockIdx.x of gridDim.x slots: the percentile of slot
+// kSlots: the slot form (k2_slot_sampler_step), one CTA per slot s = blockIdx.x of gridDim.x slots: the percentile of slot
 // s's own n elements x0[s n, (s + 1) n) into sval[s]; an idle slot reads and writes nothing.
 template <bool kSlots>
 __global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* __restrict__ x0, int n, float* sval,
@@ -388,7 +388,7 @@ __global__ void __launch_bounds__(1024) sampler_percentile_kernel(const float* _
   }
 }
 
-// kSlotThreshold (slot form only): the dynamic threshold of an element is its slot's sval[s] (k2_slot_sampler_step_ex)
+// kSlotThreshold (slot form only): the dynamic threshold of an element is its slot's sval[s] (k2_slot_sampler_step)
 template <bool kSlots, bool kSlotThreshold = false>
 __global__ void __launch_bounds__(256) sampler_post_kernel(const SamplerParams p) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -1028,17 +1028,14 @@ int k2_slot_step_end(int* state, int S, k2_stream_t stream) {
   return 0;
 }
 
-// The slot steps' shared bodies: the old entries are the new ones at cond_first 0 without the threshold (`name` prefixes the
-// error messages).
-static int slot_sampler_step(const char* name, const float* model_out, float* x, const float* noise, const float* coef,
-                             const float* guidance, const int* state, int S, int H, int W, float clip, int cond_first,
-                             int threshold_mode, float* sval, float* work, k2_stream_t stream) {
-  const std::string who(name);
-  K2_REQUIRE(model_out && x && noise && coef && guidance && state && work, who + ": null pointer");
-  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1, who + ": S, H, W must be >= 1");
-  K2_REQUIRE(cond_first == 0 || cond_first == 1, who + ": cond_first must be 0 or 1");
-  K2_REQUIRE(threshold_mode == 0 || threshold_mode == 1, who + ": threshold_mode must be 0 or 1");
-  K2_REQUIRE(threshold_mode == 0 || sval, who + ": threshold_mode 1 needs sval");
+int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
+                         const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
+                         float* work, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && noise && coef && guidance && state && work, "slot_sampler_step: null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1, "slot_sampler_step: S, H, W must be >= 1");
+  K2_REQUIRE(cond_first == 0 || cond_first == 1, "slot_sampler_step: cond_first must be 0 or 1");
+  K2_REQUIRE(threshold_mode == 0 || threshold_mode == 1, "slot_sampler_step: threshold_mode must be 0 or 1");
+  K2_REQUIRE(threshold_mode == 0 || sval, "slot_sampler_step: threshold_mode 1 needs sval");
   SamplerParams p;
   p.model_out = model_out; p.x = x; p.noise = noise; p.coef = coef;
   p.B = S; p.HW = H * W; p.guidance = 0.f; p.cond_first = cond_first; p.clip = clip; p.threshold_mode = threshold_mode;
@@ -1060,26 +1057,11 @@ static int slot_sampler_step(const char* name, const float* model_out, float* x,
   return 0;
 }
 
-int k2_slot_sampler_step(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
-                         const int* state, int S, int H, int W, float clip, float* work, k2_stream_t stream) {
-  return slot_sampler_step("slot_sampler_step", model_out, x, noise, coef, guidance, state, S, H, W, clip, 0, 0, nullptr, work,
-                           stream);
-}
-
-int k2_slot_sampler_step_ex(const float* model_out, float* x, const float* noise, const float* coef, const float* guidance,
-                            const int* state, int S, int H, int W, float clip, int cond_first, int threshold_mode, float* sval,
-                            float* work, k2_stream_t stream) {
-  return slot_sampler_step("slot_sampler_step_ex", model_out, x, noise, coef, guidance, state, S, H, W, clip, cond_first,
-                           threshold_mode, sval, work, stream);
-}
-
-static int slot_dpm_solver_step(const char* name, const float* model_out, int C2, float* x, float* hist, const float* coef,
-                                const float* guidance, const int* state, int S, int H, int W, int cond_first,
-                                k2_stream_t stream) {
-  const std::string who(name);
-  K2_REQUIRE(model_out && x && hist && coef && guidance && state, who + ": null pointer");
-  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1 && C2 >= 4, who + ": S, H, W must be >= 1 and C2 >= 4");
-  K2_REQUIRE(cond_first == 0 || cond_first == 1, who + ": cond_first must be 0 or 1");
+int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
+                            const int* state, int S, int H, int W, int cond_first, k2_stream_t stream) {
+  K2_REQUIRE(model_out && x && hist && coef && guidance && state, "slot_dpm_solver_step: null pointer");
+  K2_REQUIRE(S >= 1 && H >= 1 && W >= 1 && C2 >= 4, "slot_dpm_solver_step: S, H, W must be >= 1 and C2 >= 4");
+  K2_REQUIRE(cond_first == 0 || cond_first == 1, "slot_dpm_solver_step: cond_first must be 0 or 1");
   DpmParams p;
   p.model_out = model_out; p.x = x; p.hist = hist; p.coef = coef;
   p.B = S; p.HW = H * W; p.C2 = C2; p.guidance = 0.f; p.cond_first = cond_first;
@@ -1090,17 +1072,6 @@ static int slot_dpm_solver_step(const char* name, const float* model_out, int C2
                          static_cast<cudaStream_t>(stream), p));
   count_launch();
   return 0;
-}
-
-int k2_slot_dpm_solver_step(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
-                            const int* state, int S, int H, int W, k2_stream_t stream) {
-  return slot_dpm_solver_step("slot_dpm_solver_step", model_out, C2, x, hist, coef, guidance, state, S, H, W, 0, stream);
-}
-
-int k2_slot_dpm_solver_step_ex(const float* model_out, int C2, float* x, float* hist, const float* coef, const float* guidance,
-                               const int* state, int S, int H, int W, int cond_first, k2_stream_t stream) {
-  return slot_dpm_solver_step("slot_dpm_solver_step_ex", model_out, C2, x, hist, coef, guidance, state, S, H, W, cond_first,
-                              stream);
 }
 
 int k2_upsample2x_nhwc(const void* x, int ldx, void* y, int ldy, int NB, int H, int W, int C, k2_stream_t stream) {

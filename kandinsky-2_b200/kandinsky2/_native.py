@@ -77,10 +77,8 @@ SIGNATURES = {
     "k2_step_end": (_I, [_P, _P]),
     "k2_slot_step_begin": (_I, [_P, _P, _I, _LL, _P, _P, _P, _P, _I, _P, _P, _P, _P]),
     "k2_slot_step_end": (_I, [_P, _I, _P]),
-    "k2_slot_sampler_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P, _P]),
-    "k2_slot_dpm_solver_step": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
-    "k2_slot_sampler_step_ex": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _I, _I, _P, _P, _P]),
-    "k2_slot_dpm_solver_step_ex": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "k2_slot_sampler_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _I, _I, _P, _P, _P]),
+    "k2_slot_dpm_solver_step": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "k2_plms_step": (_I, [_P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _I, _P]),
     "k2_dpm_solver_step": (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),
     "k2_dpm_solver_sde_step": (_I, [_P, _I, _P, _P, _P, _P, _I, _I, _I, _F, _I, _P, _P, _P, _P]),

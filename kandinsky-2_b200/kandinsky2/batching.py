@@ -9,19 +9,20 @@ whose buffers never move, so admitting a request is a handful of copies into the
 the device: it knows from its own bookkeeping which slot finishes at which step.
 
 A request computes what generate_text2img(batch_size=1) computes on a pipeline whose base_seed is the request's seed: the same
-start latent and per-step noise draws, the same tables (request_tables / request_tables_21: the builders the sampling loops
-use), the same conditioning and step kernels.  Its result does not depend on the other slots: the UNet's normalisation,
-attention and convolutions are per image, the conditioning is written per row (Text2ImUNet.bind_slot) and the slot step
-kernels read and write only the rows of active slots.  2.1's p_sampler clips x0 with the 99.5 percentile of the request's own
-x0 (at batch 1 the reference's "sample 0" is the request itself): the slot step computes one percentile per slot.  An idle
-slot still costs a full row of UNet compute.
+start latent and per-step noise draws, the same tables (request_tables: the rows of the schedule the pipeline's sampling loop
+runs), the same conditioning, and the step that loop runs, set as the loop sets it from the schedule and the pipeline (step
+kernel, noise, clamp of x0, dynamic threshold, row order).  Its result does not depend on the other slots: the UNet's
+normalisation, attention and convolutions are per image, the conditioning is written per row (Text2ImUNet.bind_slot) and the
+slot step kernels read and write only the rows of active slots.  2.1's p_sampler clips x0 with the 99.5 percentile of the
+request's own x0 (at batch 1 the reference's "sample 0" is the request itself): the slot step computes one percentile per
+slot.  An idle slot still costs a full row of UNet compute.
 
 With max_loras = L > 0 each request may name a LoRA adapter registered with add_lora.  The attention layers' qkv and proj_out
 weights then live in slab tables of 1 + L fp16 copies per layer (slab 0: the pipeline's packed weights when the batcher was
-made, slabs 1 .. L: base + scale * up @ down of a registered adapter, merged by k2_lora_merge as load_lora merges), and both
-GEMMs run batched, rows s and S + s of slot s multiplying the slab a device map names (k2_conv_gemm_wmap).  A slot's encoder
-K/V rows are computed at admission with its adapter's merged encoder_kv weights.  Registering, removing and admitting write
-slabs, the map and conditioning rows in place, so the step graph never changes.
+made, slabs 1 .. L: base + scale * up @ down of a registered adapter, merged by ops.lora_merge_weights as load_lora merges),
+and both GEMMs run batched, rows s and S + s of slot s multiplying the slab a device map names (k2_conv_gemm_wmap).  A
+slot's encoder K/V rows are computed at admission with its adapter's merged encoder_kv weights.  Registering, removing and
+admitting write slabs, the map and conditioning rows in place, so the step graph never changes.
 """
 import collections
 
@@ -30,20 +31,13 @@ import torch
 from . import ops, parallel
 from ._native import K2Error
 from .launch_plan import capture_graph
-from .model.gaussian_diffusion import DDIMSampler, create_ddpm_v22, create_gaussian_diffusion
+from .model.gaussian_diffusion import SpacedDiffusion
 from .model.unet import _Plan
+from .pipelines import _sampler_schedule
 
 BATCHER_SAMPLERS = ("ddpm_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
 # Kandinsky 2.1's: PLMS is not among them, its first step evaluates the UNet twice and it keeps its epsilon history on the host
 BATCHER_SAMPLERS_21 = ("p_sampler", "ddim_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
-
-# sampler -> (its slot step: "ddpm" = ops.slot_sampler_step, "dpm" = ops.slot_dpm_solver_step; the +-clip of x0 and the
-# threshold_mode of the "ddpm" step; whether the step draws noise), as the sampling loops run each sampler
-SLOT_STEPS = {"ddpm_sampler": ("ddpm", 2.0, 0, True),
-              "p_sampler": ("ddpm", 2.0, 1, True),      # p_sample_loop(clip_denoised=True): +-2, then the dynamic threshold
-              "ddim_sampler": ("ddpm", 1e30, 0, False),  # DDIMSampler: eta 0, linear coefficients, no clamp
-              "dpmpp_2m_sampler": ("dpm", None, 0, False),
-              "dpmpp_2m_karras_sampler": ("dpm", None, 0, False)}
 
 
 def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0, samplers=BATCHER_SAMPLERS):
@@ -57,28 +51,11 @@ def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0, sampler
         raise ValueError(f"batcher: max_loras must be an int >= 0, got {max_loras!r}")
 
 
-def request_tables(sampler, steps):
-    """(model timesteps fp32 [steps], coefficient rows fp32 [steps, 8]) of one request in loop order: the rows the sampling
-    loop of generate_text2img stages for `sampler` at decoder_steps = steps, from the same schedule builders."""
-    from .pipelines import _solver_schedule
-    diffusion = create_ddpm_v22(steps)
-    return _loop_rows(diffusion if sampler == "ddpm_sampler" else _solver_schedule(sampler, diffusion, steps))
-
-
-def request_tables_21(sampler, steps, diffusion_config):
-    """request_tables for Kandinsky 2.1 at num_steps = steps: the rows its sampling loops stage for `sampler` over the
-    pipeline's diffusion_config.  p_sampler respaces the diffusion to `steps`; ddim_sampler runs DDIMSampler's schedule over
-    the un-respaced one (timesteps range(0, 1000, 1000 // steps): more rows than steps when steps does not divide 1000); the
-    solvers run _solver_schedule over its base table."""
-    from .pipelines import _solver_schedule
-    if sampler == "p_sampler":
-        return _loop_rows(create_gaussian_diffusion(**dict(diffusion_config, timestep_respacing=str(steps))))
-    diffusion = create_gaussian_diffusion(**diffusion_config)
-    if sampler == "ddim_sampler":
-        sched = DDIMSampler(None, diffusion)
-        sched.make_schedule(steps)
-        return _loop_rows(sched)
-    return _loop_rows(_solver_schedule(sampler, diffusion, steps))
+def request_tables(pipe, sampler, steps):
+    """(model timesteps fp32 [n], coefficient rows fp32 [n, 8]) of one request in loop order: the rows the sampling loop of
+    pipe.generate_text2img stages for `sampler` at `steps` steps, from the schedule it runs (n = steps, except for DDIM, whose
+    timesteps range(0, 1000, 1000 // steps) are more than steps when steps does not divide 1000)."""
+    return _loop_rows(_sampler_schedule(sampler, pipe._diffusion(sampler, steps), steps))
 
 
 def _loop_rows(sched):
@@ -151,11 +128,11 @@ def _check_steps(name, steps, max_steps):
 class Batcher:
     """Kandinsky 2.2 requests of one geometry and one sampler served from max_batch slots (Kandinsky2_2.batcher builds it).
     What differs between the versions is a class attribute or one of the methods Batcher21 overrides: the sampler set, the
-    row order, the geometry and context length, the tables, submit's keywords and the conditioning a slot is bound to."""
+    geometry and context length, submit's keywords and the conditioning a slot is bound to.  The tables, the step and the row
+    order are the pipeline's."""
 
     RUN_AHEAD = 2   # replayed steps the host may have in flight on the GPU when it admits (2: the GPU never waits on admission)
     SAMPLERS = BATCHER_SAMPLERS
-    COND_FIRST = 0   # 2.2: the unconditional row of slot s is s
 
     def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
         self._check_args(max_batch, h, w, sampler, max_steps, max_loras)
@@ -199,11 +176,17 @@ class Batcher:
         self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
         self.coef = torch.zeros(S, 8, **f32)
         self.guidance = torch.zeros(S, **f32)
-        kind, self.clip, self.threshold_mode, draws_noise = SLOT_STEPS[sampler]
-        ddpm = kind == "ddpm"
+        # the step settings the sampling loop reads from its schedule and the pipeline, read from the schedule at two steps
+        # (the fewest a DDPM schedule has; the settings do not depend on the count): step_kind "ddpm" runs on
+        # ops.slot_sampler_step, "dpmpp_2m" on ops.slot_dpm_solver_step
+        sched = _sampler_schedule(sampler, pipe._diffusion(sampler, 2), 2)
+        ddpm = sched.step_kind == "ddpm"
+        self.clip = sched.clip_range
+        self.threshold_mode = int(isinstance(sched, SpacedDiffusion) and pipe.dynamic_threshold)
+        self.cond_first = int(pipe.cond_first)
         # the DDPM step's noise for every step of every slot, drawn at admission: S x max_steps x 4 H W floats (DDIM at eta 0
         # reads no noise: its noise buffer stays zero)
-        self.noise_tab = torch.zeros(S, max_steps, 4, H, W, **f32) if draws_noise else None
+        self.noise_tab = torch.zeros(S, max_steps, 4, H, W, **f32) if sched.draws_noise else None
         self.noise = torch.zeros(S, 4, H, W, **f32) if ddpm else None
         self.work = torch.zeros(S, 4, H, W, **f32) if ddpm else None
         self.sval = torch.zeros(S, **f32) if self.threshold_mode else None   # each slot's dynamic threshold
@@ -227,9 +210,9 @@ class Batcher:
         p.launch()
         if self.hist is None:
             ops.slot_sampler_step(p.out, self.x, self.noise, self.coef, self.guidance, self.state, self.work, self.clip,
-                                  cond_first=self.COND_FIRST, threshold_mode=self.threshold_mode, sval=self.sval)
+                                  cond_first=self.cond_first, threshold_mode=self.threshold_mode, sval=self.sval)
         else:
-            ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state, cond_first=self.COND_FIRST)
+            ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state, cond_first=self.cond_first)
         ops.slot_step_end(self.state)
 
     def _check_args(self, max_batch, h, w, sampler, max_steps, max_loras):
@@ -259,19 +242,13 @@ class Batcher:
         model = self.pipe.model
         if model._packed is not self._packed:
             raise K2Error("batcher: the UNet's weights were reloaded after the batcher was made; make a new one")
-        factors, scale = model.lora_factors(state_dict), float(scale)
-        k, wenc = free[0], {}
+        factors = model.lora_factors(state_dict)
+        k, wenc, out = free[0], {}, {}   # out: id(packed weight) -> where this adapter's merge of it goes
         for p, a in self._packed["attn"].items():
-            base = model._lora_base[p] if model._lora_base is not None else a
             wqkv, wproj = self.plan.attn_slabs["layers"][p]
-            wenc[p] = torch.empty_like(base["wenc"])
-            targets = {"wqkv": wqkv[k], "wproj": wproj[k], "wenc": wenc[p]}
-            for key, proj in model._LORA_WEIGHTS:   # what Text2ImUNet._merge_lora writes into the packed weights
-                f = factors.get(p + proj + ".weight")
-                targets[key].copy_(base[key])
-                if f is not None:
-                    up, down = (t.to(base[key].device) for t in f)
-                    ops.lora_merge(base[key], up, down, scale, out=targets[key])
+            wenc[p] = a["wenc"].clone()   # so its padding columns, which a merge leaves alone, are the packed weight's
+            out.update({id(a["wqkv"]): wqkv[k], id(a["wproj"]): wproj[k], id(a["wenc"]): wenc[p]})
+        ops.lora_merge_weights([(key, base, out[id(w)]) for key, base, w in model.lora_weights()], factors, float(scale))
         self._loras[name] = (k, wenc)
 
     def remove_lora(self, name):
@@ -304,7 +281,7 @@ class Batcher:
         r.lora = lora
         r.guidance = float(decoder_guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
-        r.ts, r.coef = request_tables(self.sampler, decoder_steps)
+        r.ts, r.coef = request_tables(pipe, self.sampler, decoder_steps)
         if prompt is not None:
             pk = pipe._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
             r.positive, r.negative = pipe._embeds(prompt, 1, negative_decoder_prompt, pk)
@@ -409,7 +386,6 @@ class Batcher21(Batcher):
     clips each slot's x0 with that slot's own 99.5 percentile."""
 
     SAMPLERS = BATCHER_SAMPLERS_21
-    COND_FIRST = 1
 
     def __init__(self, pipe, max_batch, h, w, sampler="ddim_sampler", max_steps=100, max_loras=0):
         super().__init__(pipe, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
@@ -445,7 +421,7 @@ class Batcher21(Batcher):
         r.lora = None
         r.guidance = float(guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
-        r.ts, r.coef = request_tables_21(self.sampler, num_steps, pipe.config["diffusion_config"])
+        r.ts, r.coef = request_tables(pipe, self.sampler, num_steps)
         r.full, r.pooled = pipe.embedder.text_emb(prompt, 1)
         if r.full.shape[1] != self._text_len:
             raise ValueError(f"submit: the embedder's text rows have length {r.full.shape[1]}, the batcher's {self._text_len}")

@@ -51,10 +51,12 @@ def space_timesteps(num_timesteps, section_counts):
 class _Schedule:
     """What _sampling_loop needs of a schedule: coef_table() (fp32 [n, 8] step-kernel rows) and model_timesteps() (what the UNet
     sees, [n]) in the same index order; the loop runs the rows n-1 .. 0.  Each schedule also states whether its step draws
-    noise and which step kernel applies its rows (step_kind, one of FusedStep.STEP_KINDS; FusedStep's doc lists them)."""
+    noise, which step kernel applies its rows (step_kind, one of FusedStep.STEP_KINDS; FusedStep's doc lists them) and the
+    +-clip_range clamp of x0 its loop applies by default (1e30: none)."""
 
     draws_noise = True
     step_kind = "ddpm"
+    clip_range = 1e30
 
     def _tables(self, device):
         """-> (coef fp32 [n, 8] or [n, 16], model timesteps fp32 [n]) on `device`, built once per device."""
@@ -67,6 +69,8 @@ class _Schedule:
 
 class SpacedDiffusion(_Schedule):
     """Learned-range / epsilon diffusion over a subset of the base timesteps (respace.py:75-118)."""
+
+    clip_range = 2.0   # the reference's clip_denoised clamp of x0 (gaussian_diffusion.py:284-294)
 
     def __init__(self, use_timesteps, betas, rescale_timesteps=False):
         base_betas = np.array(betas, dtype=np.float64)
@@ -121,7 +125,7 @@ class SpacedDiffusion(_Schedule):
     @torch.no_grad()
     def p_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, model_kwargs=None,
                       device=None, progress=False, init_step=None, *, guidance_scale=1.0, cond_first=True,
-                      clip_range=2.0, inpaint_init=None, inpaint_mask=None, step_noise=None, callback=None,
+                      clip_range=None, inpaint_init=None, inpaint_mask=None, step_noise=None, callback=None,
                       sample_generators=None, inpaint_renoise=False):
         """Reference signature (gaussian_diffusion.py:384-425) with `model` being the k2b200 UNet module itself:
         the CFG closure, the clamp of denoised_fun and the optional inpainting blend are fused into the step
@@ -514,10 +518,12 @@ class HeunSchedule(_SigmaSchedule):
 
 
 def _sampling_loop(schedule, model, shape, *, guidance_scale, cond_first, noise=None, model_kwargs=None, device=None,
-                   clip_range=1e30, threshold_mode=0, init_step=None, inpaint_init=None, inpaint_mask=None,
+                   clip_range=None, threshold_mode=0, init_step=None, inpaint_init=None, inpaint_mask=None,
                    inpaint_renoise=False, step_noise=None, sample_generators=None, callback=None, progress=False):
     """Shared host loop over the rows n-1 .. 0 of a _Schedule, n = init_step when given (SpacedDiffusion img2img; the other
-    schedules cut their tables themselves), else num_timesteps."""
+    schedules cut their tables themselves), else num_timesteps.  clip_range=None: the schedule's."""
+    if clip_range is None:
+        clip_range = schedule.clip_range
     model_kwargs = dict(model_kwargs or {})
     if device is None:
         device = next(model.parameters()).device
@@ -660,7 +666,7 @@ class PLMSSampler(DDIMSampler):
         device = next(model.parameters()).device
         x_full = x_T.float().to(device) if x_T is not None else torch.randn(batch_size, C, H, W, device=device)
         x = x_full[:B].clone()  # the caller's noise tensor is left untouched, like the reference
-        step = FusedStep(model, B, H, W, dict(conditioning or {}), guidance_scale, cond_first, 1e30, 0)
+        step = FusedStep(model, B, H, W, dict(conditioning or {}), guidance_scale, cond_first, self.clip_range, 0)
         a_t, a_p = self.ddim_alphas, self.ddim_alphas_prev
         ts = self.ddim_timesteps.astype(np.float32)
         n = self.num_timesteps

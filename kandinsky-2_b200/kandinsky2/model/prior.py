@@ -148,18 +148,12 @@ class PriorTransformer(nn.Module):
         self._lora_base = None
 
     def _merge_lora(self):
-        factors, scale = self._lora
         layers = self._packed["layers"]
         if self._lora_base is None:
             self._lora_base = [{name: L[name][0].clone() for name, _ in self._LORA_WEIGHTS} for L in layers]
-        for i, (L, base) in enumerate(zip(layers, self._lora_base)):
-            for name, target in self._LORA_WEIGHTS:
-                f = factors.get(f"transformer.resblocks.{i}.{target}.weight")
-                if f is None:
-                    L[name][0].copy_(base[name])
-                else:
-                    up, down = (t.to(base[name].device) for t in f)
-                    ops.lora_merge(base[name], up, down, scale, out=L[name][0])
+        weights = [(f"transformer.resblocks.{i}.{target}.weight", base[name], L[name][0])
+                   for i, (L, base) in enumerate(zip(layers, self._lora_base)) for name, target in self._LORA_WEIGHTS]
+        ops.lora_merge_weights(weights, *self._lora)
 
     def _step_plan(self, B):
         """The UnCLIP sampling step at B samples (2B CFG rows) as a static launch list (_PriorStepPlan), built once per B."""

@@ -342,20 +342,19 @@ class Text2ImUNet(nn.Module):
         self._lora_base = None
         self.cache = None
 
-    def _merge_lora(self):
-        factors, scale = self._lora
-        attn = self._packed["attn"]
-        if self._lora_base is None:
-            self._lora_base = {p: {name: a[name].clone() for name, _ in self._LORA_WEIGHTS} for p, a in attn.items()}
-        for p, a in attn.items():
+    def lora_weights(self):
+        """(adapter key, unmerged weight, packed weight) of every packed attention weight an adapter changes, the form
+        ops.lora_merge_weights takes; the unmerged weight is the packed one while no adapter is merged."""
+        for p, a in self._packed["attn"].items():
+            base = a if self._lora_base is None else self._lora_base[p]
             for name, target in self._LORA_WEIGHTS:
-                base = self._lora_base[p][name]
-                f = factors.get(p + target + ".weight")
-                if f is None:
-                    a[name].copy_(base)
-                else:
-                    up, down = (t.to(base.device) for t in f)
-                    ops.lora_merge(base, up, down, scale, out=a[name])
+                yield p + target + ".weight", base[name], a[name]
+
+    def _merge_lora(self):
+        if self._lora_base is None:
+            self._lora_base = {p: {name: a[name].clone() for name, _ in self._LORA_WEIGHTS}
+                               for p, a in self._packed["attn"].items()}
+        ops.lora_merge_weights(self.lora_weights(), *self._lora)
         self.cache = None
 
     def _skip_weight(self, d, c0, c1):

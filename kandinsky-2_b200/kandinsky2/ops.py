@@ -469,26 +469,26 @@ def _slot_step_operands(who, model_out, x, coef, guidance, state, c2, others):
 
 
 def slot_sampler_step(model_out, x, noise, coef, guidance, state, work, clip=2.0, *, cond_first=0, threshold_mode=0, sval=None):
-    """k2_slot_sampler_step_ex: the DDPM / DDIM step of every active slot of x fp32 [S, 4, H, W] in place, with the slot's row
+    """k2_slot_sampler_step: the DDPM / DDIM step of every active slot of x fp32 [S, 4, H, W] in place, with the slot's row
     of coef [S, 8] and its guidance [S] (device fp32); model_out [2S, 8, H, W], noise and work fp32 [S, 4, H, W].
     cond_first: the row order (0: unconditional row s, conditional row S + s, Kandinsky 2.2; 1: the reverse, Kandinsky 2.1).
     threshold_mode 1 clips each slot's x0 with its own dynamic threshold, written to sval fp32 [S]."""
     S, H, W = _slot_step_operands("slot_sampler_step", model_out, x, coef, guidance, state, 8,
                                   (("noise", noise), ("work", work)))
     _slot_check("slot_sampler_step", S, 1, f32=(("sval", sval),), shaped=(("sval", sval, S),))
-    check(nat.load().k2_slot_sampler_step_ex(ptr(model_out), ptr(x), ptr(noise), ptr(coef), ptr(guidance), ptr(state), S, H, W,
-                                             float(clip), int(cond_first), int(threshold_mode), ptr(sval), ptr(work),
-                                             stream_ptr()))
+    check(nat.load().k2_slot_sampler_step(ptr(model_out), ptr(x), ptr(noise), ptr(coef), ptr(guidance), ptr(state), S, H, W,
+                                          float(clip), int(cond_first), int(threshold_mode), ptr(sval), ptr(work),
+                                          stream_ptr()))
     return x
 
 
 def slot_dpm_solver_step(model_out, x, hist, coef, guidance, state, *, cond_first=0):
-    """k2_slot_dpm_solver_step_ex: the DPM-Solver++(2M) step of every active slot of x fp32 [S, 4, H, W] in place, hist
+    """k2_slot_dpm_solver_step: the DPM-Solver++(2M) step of every active slot of x fp32 [S, 4, H, W] in place, hist
     [S, 4, H, W] per slot, model_out [2S, C2, H, W], rows, guidance and cond_first as slot_sampler_step."""
     S, H, W = _slot_step_operands("slot_dpm_solver_step", model_out, x, coef, guidance, state, model_out.shape[1],
                                   (("hist", hist),))
-    check(nat.load().k2_slot_dpm_solver_step_ex(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef),
-                                                ptr(guidance), ptr(state), S, H, W, int(cond_first), stream_ptr()))
+    check(nat.load().k2_slot_dpm_solver_step(ptr(model_out), model_out.shape[1], ptr(x), ptr(hist), ptr(coef),
+                                             ptr(guidance), ptr(state), S, H, W, int(cond_first), stream_ptr()))
     return x
 
 
@@ -655,6 +655,19 @@ def lora_merge(base, up, down, scale, out=None):
     check(lib.k2_lora_merge(ptr(base), base.stride(0), ptr(up), ptr(down), rows, cols, rank, float(scale), ptr(out),
                             out.stride(0), stream_ptr()))
     return out
+
+
+def lora_merge_weights(weights, factors, scale):
+    """Merge one LoRA adapter into a model's weights: for each (adapter key, unmerged fp16 weight, out) of `weights`, out =
+    the unmerged weight when factors ({adapter key: (up, down)}) has no pair for the key, else lora_merge(base, up, down,
+    scale, out=out), which leaves out's columns past the factors' width as they were."""
+    for key, base, out in weights:
+        f = factors.get(key)
+        if f is None:
+            out.copy_(base)
+        else:
+            up, down = (t.to(base.device) for t in f)
+            lora_merge(base, up, down, scale, out=out)
 
 
 def set_tuning(key, value):

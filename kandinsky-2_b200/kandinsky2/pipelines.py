@@ -19,7 +19,7 @@ import torch
 from . import ops, parallel
 from ._native import K2Error
 from .model.gaussian_diffusion import (DDIMSampler, DPMSolverSchedule, EulerSchedule, HeunSchedule, PLMSSampler, UniPCSchedule,
-                                       create_ddpm_v22, create_gaussian_diffusion)
+                                       _SolverSchedule, create_ddpm_v22, create_gaussian_diffusion)
 from .model.model_creation import create_decoder_unet
 from .utils import prepare_image, prepare_mask, q_sample, uint8_to_pil
 from .vqgan import MOVQ
@@ -99,10 +99,19 @@ def _dpm_keep(num_steps, strength):
     return max(min(int(num_steps * strength), num_steps), 1)
 
 
-def _solver_schedule(sampler, diffusion, num_steps, keep=None):
-    """The schedule of a SCHEDULE_SAMPLERS name over diffusion's base table."""
-    cls, kw = SCHEDULE_SAMPLERS[sampler]
-    return cls(diffusion.base_alphas_cumprod, num_steps, keep=keep, **kw)
+def _sampler_schedule(sampler, diffusion, num_steps, init_step=None):
+    """The schedule the sampling loop of `sampler` runs over `diffusion` (the version's _diffusion(sampler, num_steps)): a
+    SCHEDULE_SAMPLERS name's _SolverSchedule over the base table (init_step: the evaluations kept), DDIMSampler or
+    PLMSSampler with its schedule made (kandinsky2_1_model.py:259-284: un-respaced, eta 0; init_step: the last timestep kept),
+    else the SpacedDiffusion itself ("p_sampler", "ddpm_sampler"; p_sample_loop takes init_step)."""
+    if sampler in SCHEDULE_SAMPLERS:
+        cls, kw = SCHEDULE_SAMPLERS[sampler]
+        return cls(diffusion.base_alphas_cumprod, num_steps, keep=init_step, **kw)
+    if sampler in ("ddim_sampler", "plms_sampler"):
+        sched = (DDIMSampler if sampler == "ddim_sampler" else PLMSSampler)(None, diffusion)
+        sched.make_schedule(num_steps, init_step=init_step)
+        return sched
+    return diffusion
 
 
 class _DecoderBase:
@@ -165,7 +174,7 @@ class _DecoderBase:
     def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler):
         """img2img of the solver samplers -> (start latent, steps kept): the image latent noised to the first kept step."""
         keep = _dpm_keep(num_steps, strength)
-        sched = _solver_schedule(sampler, diffusion, num_steps, keep)
+        sched = _sampler_schedule(sampler, diffusion, num_steps, keep)
         return sched.start_latent(latent, self._img2img_noise(latent)), keep
 
     @torch.no_grad()
@@ -200,23 +209,22 @@ class _DecoderBase:
             noise = noise[rows].contiguous()   # a caller-supplied start latent covers the GLOBAL batch: keep this rank's rows
         shape = (2 * B, 4, H, W)
         self.model.del_cache()
-        if sampler in SCHEDULE_SAMPLERS:
-            sched = _solver_schedule(sampler, diffusion, num_steps, init_step)
+        sched = _sampler_schedule(sampler, diffusion, num_steps, init_step)
+        if isinstance(sched, _SolverSchedule):
             if init_step is None and sched.init_noise_scale != 1.0:
                 noise = noise * sched.init_noise_scale   # a full sigma-space run starts from init_noise_sigma z (diffusers)
             samples = sched.sample(self.model, shape, noise=noise, model_kwargs=kw, device=self.device,
                                    guidance_scale=guidance_scale, cond_first=self.cond_first,
                                    sample_generators=self._generators(lo, hi) if sched.draws_noise else None, **blend)
-        elif sampler in ("ddim_sampler", "plms_sampler"):  # kandinsky2_1_model.py:259-284: un-respaced schedule, eta 0
-            cls = DDIMSampler if sampler == "ddim_sampler" else PLMSSampler
-            samples, _ = cls(self.model, diffusion).sample(num_steps, 2 * B, (4, H, W), conditioning=kw, x_T=noise,
-                                                           init_step=init_step, guidance_scale=guidance_scale,
-                                                           cond_first=self.cond_first)
+        elif isinstance(sched, DDIMSampler):   # and PLMSSampler
+            sched.model = self.model   # _sampler_schedule makes the schedule without a model
+            samples, _ = sched.sample(num_steps, 2 * B, (4, H, W), conditioning=kw, x_T=noise, init_step=init_step,
+                                      guidance_scale=guidance_scale, cond_first=self.cond_first)
         else:  # "p_sampler" (2.1), "ddpm_sampler" (2.2)
-            samples = diffusion.p_sample_loop(self.model, shape, device=self.device, noise=noise, model_kwargs=kw,
-                                              init_step=init_step, guidance_scale=guidance_scale, cond_first=self.cond_first,
-                                              clip_denoised=self.dynamic_threshold,
-                                              sample_generators=self._generators(lo, hi), **blend)
+            samples = sched.p_sample_loop(self.model, shape, device=self.device, noise=noise, model_kwargs=kw,
+                                          init_step=init_step, guidance_scale=guidance_scale, cond_first=self.cond_first,
+                                          clip_denoised=self.dynamic_threshold, sample_generators=self._generators(lo, hi),
+                                          **blend)
         self.model.del_cache()
         return self._finish(samples[:B], *image_hw)
 
@@ -379,8 +387,11 @@ class Kandinsky2_2(_DecoderBase):
         re-noises the known region to the next timestep."""
         _check_sampler(sampler, SAMPLERS_22)
         cond = {"image_emb": torch.cat([negative_embeds, image_embeds], 0).to(self.device).float()}
-        return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, create_ddpm_v22(steps), steps, guidance,
-                            noise=latents, init_step=init_step, inpaint=inpaint, hint=hint)
+        return self._decode(cond, batch_size, (h // 8, w // 8), (h, w), sampler, self._diffusion(sampler, steps), steps,
+                            guidance, noise=latents, init_step=init_step, inpaint=inpaint, hint=hint)
+
+    def _diffusion(self, sampler, steps):
+        return create_ddpm_v22(steps)
 
     def _prior_kwargs(self, prior_steps, prior_guidance_scale, negative_prior_prompt):
         """The call's prior keywords for an embedder that runs the prior (`runs_prior`, e.g. model.prior.PriorEmbedder22); None
@@ -444,8 +455,7 @@ class Kandinsky2_2(_DecoderBase):
         pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
         pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
         lat = self._encode_image(image, h, w)
-        diffusion = create_ddpm_v22(decoder_steps)
-        x, start = self._img2img_start(lat, diffusion, decoder_steps, strength, sampler)
+        x, start = self._img2img_start(lat, self._diffusion(sampler, decoder_steps), decoder_steps, strength, sampler)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, sampler=sampler)
 
@@ -530,7 +540,7 @@ class Kandinsky2_2(_DecoderBase):
                    self.embedder.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
                                          **{**pk, "negative_prior_prompt": ""}))
         lat = self._encode_image(image, h, w)
-        x, start = self._img2img_start(lat, create_ddpm_v22(decoder_steps), decoder_steps, strength, sampler)
+        x, start = self._img2img_start(lat, self._diffusion(sampler, decoder_steps), decoder_steps, strength, sampler)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start,
                                  hint=self._hint(self._depth_hint(hint), h, w),

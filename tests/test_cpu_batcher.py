@@ -23,17 +23,22 @@ def test_admission_is_fifo_into_the_lowest_free_slot_and_slots_are_reused():
 
 
 @pytest.mark.parametrize("sampler", ["ddpm_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler"])
-@pytest.mark.parametrize("steps", [2, 7, 50])
-def test_request_tables_are_the_sampling_loops(sampler, steps):
-    """A request's staged tables are the rows _sampling_loop stages for generate_text2img(decoder_steps=steps): the schedule's
-    coefficient table and model timesteps, last table row first."""
+@pytest.mark.parametrize("steps", [2, 7, 50, 100])
+def test_request_tables_of_a_22_pipeline_are_its_sampling_loops(sampler, steps):
+    """A request's staged tables, built from the pipeline (request_tables(pipe, ...)), are the rows _sampling_loop stages for
+    Kandinsky2_2.generate_text2img(decoder_steps=steps): the schedule's coefficient table and model timesteps, last table row
+    first."""
     import numpy as np
     from kandinsky2.batching import request_tables
     from kandinsky2.model.gaussian_diffusion import create_ddpm_v22
-    from kandinsky2.pipelines import _solver_schedule
-    ts, coef = request_tables(sampler, steps)
+    from kandinsky2.pipelines import SCHEDULE_SAMPLERS, Kandinsky2_2
+    ts, coef = request_tables(Kandinsky2_2.__new__(Kandinsky2_2), sampler, steps)
     d = create_ddpm_v22(steps)
-    sched = d if sampler == "ddpm_sampler" else _solver_schedule(sampler, d, steps)
+    if sampler == "ddpm_sampler":
+        sched = d
+    else:
+        cls, kw = SCHEDULE_SAMPLERS[sampler]
+        sched = cls(d.base_alphas_cumprod, steps, **kw)
     want_coef = sched.coef_table()[::-1]
     want_ts = np.asarray(sched.model_timesteps(), dtype=np.float32)[::-1]
     assert ts.dtype == coef.dtype == torch.float32 and coef.shape == (steps, 8) and ts.shape == (steps,)
@@ -68,7 +73,8 @@ def test_batcher_refuses_other_tasks():
 
 
 P = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-# entry point -> (its arguments before the stream, all valid; [(the changed arguments, the message)])
+# entry point -> (its arguments before the stream, all valid; [(the changed arguments, the message)]); each message
+# names the entry point without its k2_ prefix
 SLOT_ARGUMENTS = {
     "k2_slot_step_begin": (
         [P, P, 4, 64, P, P, P, P, 10, P, P, P],
@@ -77,27 +83,35 @@ SLOT_ARGUMENTS = {
          ({2: 70000}, "S in"), ({3: 0}, "n and kmax"), ({8: 0}, "n and kmax"), ({10: None}, "noise_tab without")]),
     "k2_slot_step_end": ([P, 4], [({0: None}, "null state"), ({1: 0}, "S must be")]),
     "k2_slot_sampler_step": (
-        [P, P, P, P, P, P, 4, 8, 8, 2.0, P],
-        [({i: None}, "null pointer") for i in (0, 1, 2, 3, 4, 5, 10)] + [({6: 0}, "must be >= 1"), ({7: 0}, "must be >= 1"),
-                                                                          ({8: -2}, "must be >= 1")]),
+        [P, P, P, P, P, P, 4, 8, 8, 2.0, 1, 1, P, P],
+        [({i: None}, "null pointer") for i in (0, 1, 2, 3, 4, 5, 13)]
+        + [({6: 0}, "must be >= 1"), ({7: 0}, "must be >= 1"), ({8: -2}, "must be >= 1"),
+           ({10: 2}, "cond_first must be 0 or 1"), ({10: -1}, "cond_first must be 0 or 1"),
+           ({11: 2}, "threshold_mode must be 0 or 1"), ({11: 3}, "threshold_mode must be 0 or 1"),
+           ({11: -1}, "threshold_mode must be 0 or 1"), ({12: None}, "threshold_mode 1 needs sval")]),
     "k2_slot_dpm_solver_step": (
-        [P, 8, P, P, P, P, P, 4, 8, 8],
-        [({i: None}, "null pointer") for i in (0, 2, 3, 4, 5, 6)] + [({1: 3}, "C2 >= 4"), ({7: 0}, "must be >= 1"),
-                                                                     ({9: 0}, "must be >= 1")]),
+        [P, 8, P, P, P, P, P, 4, 8, 8, 1],
+        [({i: None}, "null pointer") for i in (0, 2, 3, 4, 5, 6)]
+        + [({1: 3}, "C2 >= 4"), ({7: 0}, "must be >= 1"), ({9: 0}, "must be >= 1"), ({10: 2}, "cond_first must be 0 or 1"),
+           ({10: -1}, "cond_first must be 0 or 1")]),
 }
 
 
-@pytest.mark.parametrize("name", sorted(SLOT_ARGUMENTS))
-def test_slot_entry_points_refuse_bad_arguments_without_a_gpu(name):
+SLOT_CASES = [(name, changes, msg) for name, (_, cases) in sorted(SLOT_ARGUMENTS.items()) for changes, msg in cases]
+
+
+@pytest.mark.parametrize("name,changes,msg", SLOT_CASES,
+                         ids=[f"{n}-{','.join(f'{i}={v}' for i, v in c.items())}" for n, c, _ in SLOT_CASES])
+def test_slot_entry_point_refuses_each_bad_argument_without_a_gpu(name, changes, msg):
+    """Each bad argument alone makes the entry point fail before any CUDA call, with a message that names the entry point."""
     from kandinsky2 import _native
     lib = _native.load()
-    good, cases = SLOT_ARGUMENTS[name]
-    for changes, msg in cases:
-        args = list(good)
-        for i, v in changes.items():
-            args[i] = v
-        assert getattr(lib, name)(*args, None) != 0, (name, changes)
-        assert msg in lib.k2_last_error().decode(), (name, changes, lib.k2_last_error())
+    args = list(SLOT_ARGUMENTS[name][0])
+    for i, v in changes.items():
+        args[i] = v
+    assert getattr(lib, name)(*args, None) != 0
+    err = lib.k2_last_error().decode()
+    assert msg in err and f"{name[3:]}: " in err, err
 
 
 @pytest.mark.parametrize("op,args", [("slot_step_end", lambda t: (t,)),

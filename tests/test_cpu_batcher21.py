@@ -1,8 +1,5 @@
 """CPU: the host side of the Kandinsky 2.1 batcher (batching.Batcher21) -- the per-request tables against the schedules the 2.1
-sampling loops build, what Kandinsky2_1.batcher and submit refuse, and the argument checks of the cond-first / thresholded
-slot step entry points without a GPU."""
-import ctypes
-
+sampling loops build, what Kandinsky2_1.batcher and submit refuse, and what the slot step ops refuse without a GPU."""
 import numpy as np
 import pytest
 import torch
@@ -19,15 +16,16 @@ def _bare_pipe(task_type="text2img"):
 
 
 @pytest.mark.parametrize("sampler", SAMPLERS_21)
-@pytest.mark.parametrize("steps", [2, 7, 50, 100])
-def test_request_tables_are_the_21_sampling_loops(sampler, steps):
-    """A request's staged tables are the rows _sampling_loop stages for Kandinsky2_1.generate_text2img(num_steps=steps): the
-    schedule the pipeline builds for `sampler` over its _diffusion, last table row first."""
-    from kandinsky2.batching import request_tables_21
+@pytest.mark.parametrize("steps", [2, 7, 25, 50, 100])
+def test_request_tables_of_a_21_pipeline_are_its_sampling_loops(sampler, steps):
+    """A request's staged tables, built from the pipeline (request_tables(pipe, ...)), are the rows _sampling_loop stages for
+    Kandinsky2_1.generate_text2img(num_steps=steps): the schedule the pipeline builds for `sampler` over its _diffusion, last
+    table row first."""
+    from kandinsky2.batching import request_tables
     from kandinsky2.model.gaussian_diffusion import DDIMSampler
-    from kandinsky2.pipelines import _solver_schedule
+    from kandinsky2.pipelines import SCHEDULE_SAMPLERS
     pipe = _bare_pipe()
-    ts, coef = request_tables_21(sampler, steps, pipe.config["diffusion_config"])
+    ts, coef = request_tables(pipe, sampler, steps)
     diffusion = pipe._diffusion(sampler, steps)
     if sampler == "p_sampler":
         sched = diffusion
@@ -35,7 +33,8 @@ def test_request_tables_are_the_21_sampling_loops(sampler, steps):
         sched = DDIMSampler(None, diffusion)
         sched.make_schedule(steps)
     else:
-        sched = _solver_schedule(sampler, diffusion, steps)
+        cls, kw = SCHEDULE_SAMPLERS[sampler]
+        sched = cls(diffusion.base_alphas_cumprod, steps, **kw)
     want_coef = sched.coef_table()[::-1]
     want_ts = np.asarray(sched.model_timesteps(), dtype=np.float32)[::-1]
     n = sched.num_timesteps
@@ -102,38 +101,6 @@ def test_submit21_refuses_bad_requests(prompt, kw, what):
     with pytest.raises(ValueError, match=what):
         b.submit(prompt, **kw)
     assert not b.queue.waiting and not b._requests
-
-
-P = ctypes.c_void_p(256)   # never dereferenced: every call below fails its checks first
-# entry point -> (its arguments before the stream, all valid; [(the changed arguments, the message)])
-SLOT_EX_ARGUMENTS = {
-    "k2_slot_sampler_step_ex": (
-        [P, P, P, P, P, P, 4, 8, 8, 2.0, 1, 1, P, P],
-        [({i: None}, "null pointer") for i in (0, 1, 2, 3, 4, 5, 13)]
-        + [({6: 0}, "must be >= 1"), ({7: 0}, "must be >= 1"), ({8: -2}, "must be >= 1"),
-           ({10: 2}, "cond_first must be 0 or 1"), ({10: -1}, "cond_first must be 0 or 1"),
-           ({11: 2}, "threshold_mode must be 0 or 1"), ({11: 3}, "threshold_mode must be 0 or 1"),
-           ({11: -1}, "threshold_mode must be 0 or 1"), ({12: None}, "threshold_mode 1 needs sval")]),
-    "k2_slot_dpm_solver_step_ex": (
-        [P, 8, P, P, P, P, P, 4, 8, 8, 1],
-        [({i: None}, "null pointer") for i in (0, 2, 3, 4, 5, 6)]
-        + [({1: 3}, "C2 >= 4"), ({7: 0}, "must be >= 1"), ({9: 0}, "must be >= 1"), ({10: 2}, "cond_first must be 0 or 1"),
-           ({10: -1}, "cond_first must be 0 or 1")]),
-}
-
-
-@pytest.mark.parametrize("name", sorted(SLOT_EX_ARGUMENTS))
-def test_slot_ex_entry_points_refuse_bad_arguments_without_a_gpu(name):
-    from kandinsky2 import _native
-    lib = _native.load()
-    good, cases = SLOT_EX_ARGUMENTS[name]
-    for changes, msg in cases:
-        args = list(good)
-        for i, v in changes.items():
-            args[i] = v
-        assert getattr(lib, name)(*args, None) != 0, (name, changes)
-        err = lib.k2_last_error().decode()
-        assert msg in err and f"{name[3:]}: " in err, (name, changes, err)
 
 
 @pytest.mark.parametrize("op,args", [

@@ -56,10 +56,11 @@ def test_batcher_refuses_a_negative_max_loras():
 
 
 def _bare_batcher(max_loras, slots=2, emb_dim=16, max_steps=10):
-    """A Batcher with its host state only (no pipeline, plan or graph): enough for the registry's refusals."""
+    """A Batcher with its host state only (a bare pipeline, no plan or graph): enough for the registry's refusals."""
     from kandinsky2.batching import Batcher, SlotQueue
+    from kandinsky2.pipelines import Kandinsky2_2
     b = Batcher.__new__(Batcher)
-    b.pipe, b.max_steps, b._emb_dim, b.max_loras = None, max_steps, emb_dim, max_loras
+    b.pipe, b.max_steps, b._emb_dim, b.max_loras = Kandinsky2_2.__new__(Kandinsky2_2), max_steps, emb_dim, max_loras
     b.queue, b._requests, b._loras = SlotQueue(slots), {}, {}
     b.sampler, b._next_handle = "ddpm_sampler", 0
     b.state = torch.full((2, slots), 7, dtype=torch.int32)
@@ -70,7 +71,7 @@ def _emb():
     return dict(image_embeds=torch.zeros(16), negative_image_embeds=torch.zeros(16), decoder_steps=5, seed=0)
 
 
-def test_registry_refusals():
+def test_registry_refusals_on_a_bare_pipeline():
     """add_lora refuses a batcher made without slabs, a duplicate name and a full table before touching a weight; submit
     refuses an unknown adapter; remove_lora refuses an unknown name and an adapter a waiting request uses."""
     with pytest.raises(ValueError, match="max_loras=0"):
