@@ -1,5 +1,6 @@
-"""Continuous batching of Kandinsky 2.2 (Batcher) and 2.1 (Batcher21) text2img requests: one CFG-doubled UNet batch of S
-slots, every slot a request at its own denoising step, refilled from a FIFO queue as requests finish.
+"""Continuous batching of Kandinsky 2.2 (Batcher) and 2.1 (Batcher21) text2img and img2img requests, and of Kandinsky 2.2
+ControlNet-depth requests: one CFG-doubled UNet batch of S slots, every slot a request at its own denoising step, refilled from
+a FIFO queue as requests finish.
 
 Rows follow the version's layout: for slot s, unconditional s and conditional S + s in 2.2, the reverse in 2.1.  The device
 keeps per slot its step index, its timestep / coefficient / per-step noise tables and its guidance scale (k2b200.h:
@@ -17,6 +18,13 @@ slot step kernels read and write only the rows of active slots.  2.1's p_sampler
 request's own x0 (at batch 1 the reference's "sample 0" is the request itself): the slot step computes one percentile per
 slot.  An idle slot still costs a full row of UNet compute.
 
+An img2img request (submit(image=, strength=)) computes what generate_img2img(batch_size=1) computes: its image is encoded at
+submit, the pipeline's _img2img_start noises it to the first step its rule keeps, and the request runs only the rows that
+step keeps (request_tables(..., init_step)), so requests of different lengths share the batch.  Its start latent replaces the
+fresh draw when it is admitted; the solvers' history is zeroed as for any request, and their tables make the first kept step
+first order.  A batcher of a ControlNet-depth pipeline gives every request its own depth hint: the hint stem runs at admission
+(Text2ImUNet.bind_slot(hint=)) and writes the slot's rows of the plan's hint_in, which the step graph's stem reads.
+
 With max_loras = L > 0 each request may name a LoRA adapter registered with add_lora.  The attention layers' qkv and proj_out
 weights then live in slab tables of 1 + L fp16 copies per layer (slab 0: the pipeline's packed weights when the batcher was
 made, slabs 1 .. L: base + scale * up @ down of a registered adapter, merged by ops.lora_merge_weights as load_lora merges),
@@ -25,6 +33,7 @@ slot's encoder K/V rows are computed at admission with its adapter's merged enco
 admitting write slabs, the map and conditioning rows in place, so the step graph never changes.
 """
 import collections
+import inspect
 
 import torch
 
@@ -51,17 +60,20 @@ def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0, sampler
         raise ValueError(f"batcher: max_loras must be an int >= 0, got {max_loras!r}")
 
 
-def request_tables(pipe, sampler, steps):
+def request_tables(pipe, sampler, steps, init_step=None):
     """(model timesteps fp32 [n], coefficient rows fp32 [n, 8]) of one request in loop order: the rows the sampling loop of
     pipe.generate_text2img stages for `sampler` at `steps` steps, from the schedule it runs (n = steps, except for DDIM, whose
-    timesteps range(0, 1000, 1000 // steps) are more than steps when steps does not divide 1000)."""
-    return _loop_rows(_sampler_schedule(sampler, pipe._diffusion(sampler, steps), steps))
+    timesteps range(0, 1000, 1000 // steps) are more than steps when steps does not divide 1000).  init_step: the one
+    pipe._img2img_start returns, for the rows of generate_img2img's loop -- the solver schedules and DDIM cut their own tables
+    to it, the loop over a SpacedDiffusion runs its rows init_step - 1 .. 0."""
+    sched = _sampler_schedule(sampler, pipe._diffusion(sampler, steps), steps, init_step)
+    return _loop_rows(sched, init_step if isinstance(sched, SpacedDiffusion) else None)
 
 
-def _loop_rows(sched):
-    """(timesteps, coefficient rows) of a schedule in the order _sampling_loop runs them, last table row first."""
+def _loop_rows(sched, init_step=None):
+    """(timesteps, coefficient rows) of a schedule in the order _sampling_loop runs them: the rows [:init_step], last first."""
     coef, ts = sched._tables("cpu")
-    order = torch.arange(sched.num_timesteps - 1, -1, -1)
+    order = torch.arange(sched.num_timesteps)[:init_step].flip(0)
     return ts[order].contiguous(), coef[order].contiguous()
 
 
@@ -111,13 +123,21 @@ class SlotQueue:
 
 
 class _Request:
-    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora", "full", "pooled")
+    __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora", "full", "pooled", "start", "hint")
 
 
 def _check_embedding(name, e, dim):
     if e is not None and (not torch.is_tensor(e) or e.numel() != dim or e.dim() not in (1, 2) or not e.is_floating_point()):
         raise ValueError(f"submit: {name} must be one floating-point image embedding, [1, {dim}] or [{dim}], got "
                          f"{tuple(e.shape) if torch.is_tensor(e) else type(e).__name__}")
+
+
+def _check_img2img(image, strength):
+    if image is None and strength is not None:
+        raise ValueError("submit: strength without image; strength is the noise level an img2img request's image starts at")
+    if strength is not None and (isinstance(strength, bool) or not isinstance(strength, (int, float)) or
+                                 not 0 <= strength <= 1):
+        raise ValueError(f"submit: strength must be a number in [0, 1], got {strength!r}")
 
 
 def _check_steps(name, steps, max_steps):
@@ -128,18 +148,22 @@ def _check_steps(name, steps, max_steps):
 class Batcher:
     """Kandinsky 2.2 requests of one geometry and one sampler served from max_batch slots (Kandinsky2_2.batcher builds it).
     What differs between the versions is a class attribute or one of the methods Batcher21 overrides: the sampler set, the
-    geometry and context length, submit's keywords and the conditioning a slot is bound to.  The tables, the step and the row
-    order are the pipeline's."""
+    tasks, the geometry and context length, submit's keywords, the image latent and the conditioning a slot is bound to.  The
+    tables, the img2img start, the step and the row order are the pipeline's."""
 
     RUN_AHEAD = 2   # replayed steps the host may have in flight on the GPU when it admits (2: the GPU never waits on admission)
     SAMPLERS = BATCHER_SAMPLERS
+    TASKS = ("text2img", "controlnet")
+    hinted = False   # True on a ControlNet pipeline's batcher: every request brings its own depth hint
 
     def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
         self._check_args(max_batch, h, w, sampler, max_steps, max_loras)
-        if pipe.task_type != "text2img":
-            raise ValueError(f"batcher: serves text2img pipelines only, this one is {pipe.task_type!r}")
+        if pipe.task_type not in self.TASKS:
+            raise ValueError(f"batcher: serves {' and '.join(self.TASKS)} pipelines only, this one is {pipe.task_type!r}")
         self.pipe, self.sampler, self.max_steps = pipe, sampler, max_steps
+        self.hinted = pipe.task_type == "controlnet"
         self.h, self.w, H, W = self._geometry(h, w)
+        self._latent_hw = (H, W)
         S = max_batch
         model = pipe.model
         if model._packed is None:
@@ -261,12 +285,17 @@ class Batcher:
 
     def submit(self, prompt=None, *, image_embeds=None, negative_image_embeds=None, decoder_steps=50, decoder_guidance_scale=4,
                seed=None, prior_steps=25, prior_guidance_scale=4, negative_prior_prompt="", negative_decoder_prompt="",
-               lora=None):
+               lora=None, image=None, strength=None, hint=None, prior_strength=None):
         """Queue one image -> its handle (the key of its image in what step() / run() return).  Either a prompt, whose image
         embeddings the pipeline's embedder makes now at batch 1 as generate_text2img does (the prior keywords as there), or
         image_embeds and negative_image_embeds ([1, D] or [D]) as diffusers' KandinskyV22Pipeline takes them.  seed plays the
         part of the pipeline's base_seed for global sample 0 (default: the pipeline's base_seed).  lora: the name of an
-        adapter registered with add_lora, or None for the weights slab 0 holds."""
+        adapter registered with add_lora, or None for the weights slab 0 holds.
+        image (a PIL image, an image tensor or an encoded latent, as generate_img2img takes it) makes the request img2img, the
+        image encoded now: generate_img2img(batch_size=1), strength defaulting to its default.  On a ControlNet batcher hint
+        (a [1, 3, h, w] / [3, h, w] depth map, or a PIL image with the pipeline's depth_estimator) is required: the request
+        is generate_controlnet(batch_size=1), or with an image generate_controlnet_img2img(batch_size=1, strength=,
+        prior_strength=) -- prior_strength runs the prior from the image's embedding as that method does."""
         pipe = self.pipe
         if (prompt is None) == (image_embeds is None):
             raise ValueError("submit: pass either a prompt or image_embeds")
@@ -277,17 +306,72 @@ class Batcher:
         _check_steps("decoder_steps", decoder_steps, self.max_steps)
         if lora is not None and lora not in self._loras:
             raise ValueError(f"submit: no adapter named {lora!r} is registered (Batcher.add_lora)")
+        _check_img2img(image, strength)
+        self._check_hint(hint)
+        if prior_strength is not None and (not self.hinted or prompt is None or image is None):
+            raise ValueError("submit: prior_strength (generate_controlnet_img2img's) needs a ControlNet batcher, a prompt and "
+                             "an image")
+        pk = pipe._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt) if prompt is not None else None
+        if prior_strength is not None:
+            pipe._check_prior_strength(prior_strength, pk)
         r = _Request()
         r.lora = lora
         r.guidance = float(decoder_guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
-        r.ts, r.coef = request_tables(pipe, self.sampler, decoder_steps)
-        if prompt is not None:
-            pk = pipe._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
+        r.hint = self._slot_hint(hint)
+        r.start, init_step = self._img2img_start(image, strength, decoder_steps, r.seed)
+        r.ts, r.coef = request_tables(pipe, self.sampler, decoder_steps, init_step)
+        if prompt is None:
+            r.positive, r.negative = image_embeds, negative_image_embeds
+        elif prior_strength is None:
             r.positive, r.negative = pipe._embeds(prompt, 1, negative_decoder_prompt, pk)
         else:
-            r.positive, r.negative = image_embeds, negative_image_embeds
+            r.positive, r.negative = pipe._controlnet_img2img_embeds(prompt, image, 1, negative_decoder_prompt, pk,
+                                                                     prior_strength)
         return self._enqueue(r)
+
+    def _check_hint(self, hint):
+        if self.hinted and hint is None:
+            raise ValueError("submit: a ControlNet batcher needs hint= (the request's depth map)")
+        if not self.hinted and hint is not None:
+            raise ValueError("submit: hint is taken by the batcher of a task_type='controlnet' pipeline only")
+
+    def _slot_hint(self, hint):
+        """The request's depth map as generate_controlnet takes it -> fp32 [1, 3, h, w] on the device (None: no hint)."""
+        if hint is None:
+            return None
+        pipe = self.pipe
+        hint = pipe._depth_hint(hint)
+        if not (torch.is_tensor(hint) and hint.dim() in (3, 4) and hint.shape[-3] == 3 and (hint.dim() == 3 or
+                                                                                             hint.shape[0] == 1)):
+            raise ValueError("submit: hint must be one depth map, a [1, 3, h, w] or [3, h, w] tensor (or a PIL image when the "
+                             f"pipeline has a depth_estimator), got {tuple(hint.shape) if torch.is_tensor(hint) else type(hint)}")
+        return pipe._hint(hint, self.h, self.w).to(pipe.device)
+
+    def _image_latent(self, image):
+        """The latent generate_img2img starts from: the MoVQ encoding of image at the batcher's h x w."""
+        return self.pipe._encode_image(image, self.h, self.w)
+
+    def _img2img_start(self, image, strength, steps, seed):
+        """-> (start latent [1, 4, H, W], init_step) of the pipeline's img2img rule with base_seed = seed, or (None, None) for
+        a request without an image.  Refuses an image whose latent is not the batcher's grid and a strength whose rule keeps
+        no step."""
+        if image is None:
+            return None, None
+        pipe = self.pipe
+        if strength is None:   # the default of the method the request stands for
+            method = pipe.generate_controlnet_img2img if self.hinted else pipe.generate_img2img
+            strength = inspect.signature(method).parameters["strength"].default
+        lat = self._image_latent(image)
+        grid = (1, 4) + tuple(self._latent_hw)
+        if tuple(lat.shape) != grid:
+            raise ValueError(f"submit: the image's latent is {list(lat.shape)}, the batcher's latent grid is {list(grid)}: pass "
+                             f"an image of the batcher's {self.h} x {self.w}, or a PIL image")
+        x, start = pipe._img2img_start(lat, pipe._diffusion(self.sampler, steps), steps, strength, self.sampler,
+                                       base_seed=seed)
+        if start < 1:
+            raise ValueError(f"submit: strength {strength} keeps no denoising step of {self.sampler} at {steps} steps")
+        return x, start
 
     def _enqueue(self, r):
         """Queue a request whose tables are set -> its handle; it runs one step per row of its tables."""
@@ -321,10 +405,10 @@ class Batcher:
     def _bind(self, s, r):
         """Write request r's conditioning into slot s's rows of the plan."""
         if self.w_map is None:
-            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive)
+            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, hint=r.hint)
         else:
             k, wenc = self._loras[r.lora] if r.lora is not None else (0, self._wenc0)
-            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, wenc=wenc)
+            self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, wenc=wenc, hint=r.hint)
             self._set_slab(s, k)
 
     def _stage(self, s, r):
@@ -333,8 +417,12 @@ class Batcher:
         k = r.steps
         self.ts_tab[s, :k].copy_(r.ts)
         self.coef_tab[s, :k].copy_(r.coef)
-        # the draws of generate_text2img(batch_size=1) with base_seed = r.seed (_DecoderBase._decode, _sampling_loop)
-        self.x[s].copy_(parallel.sample_noise(range(1), (4, H, W), base_seed=r.seed, device=pipe.device)[0])
+        # the draws of generate_text2img(batch_size=1) with base_seed = r.seed (_DecoderBase._decode, _sampling_loop), or the
+        # img2img start latent made at submit; the DDPM noise below is drawn for the k rows the request runs
+        if r.start is not None:
+            self.x[s].copy_(r.start[0])
+        else:
+            self.x[s].copy_(parallel.sample_noise(range(1), (4, H, W), base_seed=r.seed, device=pipe.device)[0])
         if self.noise_tab is not None:
             gen = pipe._generators(0, 1, base_seed=r.seed)[0]
             self.noise_tab[s, :k].copy_(torch.randn(k, 4, H, W, device=pipe.device, generator=gen))
@@ -386,6 +474,7 @@ class Batcher21(Batcher):
     clips each slot's x0 with that slot's own 99.5 percentile."""
 
     SAMPLERS = BATCHER_SAMPLERS_21
+    TASKS = ("text2img",)
 
     def __init__(self, pipe, max_batch, h, w, sampler="ddim_sampler", max_steps=100, max_loras=0):
         super().__init__(pipe, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
@@ -398,30 +487,37 @@ class Batcher21(Batcher):
     def _geometry(self, h, w):
         return (h, w) + tuple(self.pipe.get_new_h_w(h, w))
 
+    def _image_latent(self, image):
+        return super()._image_latent(image) * self.pipe.scale   # as generate_img2img scales it
+
     def _context(self):
         # the text rows' length is the embedder's: read it once from the embedding of ""
         self._text_len = self.pipe.embedder.text_emb("", 1)[0].shape[1]
         return self.pipe.model.num_image_embs + self._text_len
 
     def submit(self, prompt, *, image_embeds=None, negative_image_embeds=None, num_steps=100, guidance_scale=7,
-               negative_decoder_prompt="", seed=None):
+               negative_decoder_prompt="", seed=None, image=None, strength=None):
         """Queue one image of Kandinsky2_1.generate_text2img(prompt, batch_size=1, ...) -> its handle (the key of its image in
         what step() / run() return).  The text rows are the embedder's text_emb(prompt, 1); the image rows those
         generate_text2img makes (the prior's embedding of prompt, and the zero image embedding or, with
         negative_decoder_prompt, the prior's embedding of that).  image_embeds / negative_image_embeds ([1, D] or [D]) replace
         either: prompt="" with image_embeds=embedder.interpolate(items, weights, 1) is mix_images(items, weights,
-        batch_size=1).  seed plays the part of the pipeline's base_seed (default: the pipeline's base_seed)."""
+        batch_size=1).  seed plays the part of the pipeline's base_seed (default: the pipeline's base_seed).  image (a PIL image,
+        an image tensor or an encoded latent) makes it Kandinsky2_1.generate_img2img(prompt, image, strength, batch_size=1),
+        the image encoded now, strength defaulting to that method's default."""
         pipe = self.pipe
         if not isinstance(prompt, str):
             raise ValueError(f"submit: prompt must be a str, got {type(prompt).__name__}")
         for name, e in (("image_embeds", image_embeds), ("negative_image_embeds", negative_image_embeds)):
             _check_embedding(name, e, self._emb_dim)
         _check_steps("num_steps", num_steps, self.max_steps)
+        _check_img2img(image, strength)
         r = _Request()
-        r.lora = None
+        r.lora = r.hint = None
         r.guidance = float(guidance_scale)
         r.seed = pipe.base_seed if seed is None else int(seed)
-        r.ts, r.coef = request_tables(pipe, self.sampler, num_steps)
+        r.start, init_step = self._img2img_start(image, strength, num_steps, r.seed)
+        r.ts, r.coef = request_tables(pipe, self.sampler, num_steps, init_step)
         r.full, r.pooled = pipe.embedder.text_emb(prompt, 1)
         if r.full.shape[1] != self._text_len:
             raise ValueError(f"submit: the embedder's text rows have length {r.full.shape[1]}, the batcher's {self._text_len}")

@@ -422,7 +422,7 @@ class Text2ImUNet(nn.Module):
             self.cache = out
         return out
 
-    def bind_slot(self, plan, slot, negative_emb, positive_emb, wenc=None, full_emb=None, pooled_emb=None):
+    def bind_slot(self, plan, slot, negative_emb, positive_emb, wenc=None, full_emb=None, pooled_emb=None, hint=None):
         """Write the conditioning of slot `slot` of a plan of N = 2 S rows into the plan's xf_proj and encoder K/V rows, leaving
         every other row and every buffer address (so a CUDA graph captured on the plan) as it is.  Image embeddings are
         [image_encoder_in_dim].  Kandinsky 2.2: negative_emb goes to row `slot`, positive_emb to row S + slot.  Kandinsky 2.1
@@ -434,10 +434,13 @@ class Text2ImUNet(nn.Module):
         (the other input rows zero), and a slot's conditioning has the same bits in every slot and, at S = 1, those
         generate_text2img(batch_size=1) binds.  The model's cached conditioning is left untouched.
         wenc ({attention layer -> packed encoder_kv weight}, or None = the packed weights): the weights the slot's encoder K/V
-        rows are computed with, e.g. the encoder_kv weights an adapter merges (the batcher's per-request adapters)."""
+        rows are computed with, e.g. the encoder_kv weights an adapter merges (the batcher's per-request adapters).
+        hint (ControlNet UNets only, which need it): the slot's depth map [1, 3, 8h, 8w]; its hint features are computed by
+        the hint stem at the plan's batch, the map in rows `slot` and S + slot and zeros elsewhere, since the stem's
+        convolutions too pick split-K from the row count: at S = 1 they are what generate_controlnet binds."""
         v21 = self.cond_version == "2.1"
-        if self.hint_channels:
-            raise K2Error("bind_slot: only the text2img UNets take per-slot conditioning")
+        if bool(self.hint_channels) != (hint is not None):
+            raise K2Error("bind_slot: a ControlNet UNet needs hint= (the slot's depth map), a text2img UNet takes none")
         if v21 != (full_emb is not None) or v21 != (pooled_emb is not None):
             raise K2Error("bind_slot: the Kandinsky 2.1 UNet needs full_emb and pooled_emb, the 2.2 one takes neither")
         S = plan.N // 2
@@ -454,6 +457,10 @@ class Text2ImUNet(nn.Module):
                 rows[slot] = t[0]
                 rows[S + slot] = t[1]
                 text[name] = rows
+        if hint is not None:
+            rows = torch.zeros((plan.N,) + tuple(hint.shape[1:]), device=plan.dev, dtype=torch.float32)
+            rows[slot] = rows[S + slot] = hint[0].to(plan.dev, torch.float32)
+            text["hint"] = rows
         saved, keep = self.cache, self.cache_text_emb
         self.cache, self.cache_text_emb = None, False
         try:
@@ -554,6 +561,8 @@ class _Plan(LaunchPlan):
         place (Text2ImUNet.bind_slot)."""
         idx = torch.tensor(rows, device=self.dev, dtype=torch.long)
         self.xf_proj[idx] = cond["xf_proj"][idx]
+        if self.m.hint_channels:
+            self.hint_in[idx] = cond["hint_feat"][idx]
         for p, buf in self.enc_kv.items():
             src = cond["enc_kv"][p]
             if buf.shape != src.shape:

@@ -167,15 +167,17 @@ class _DecoderBase:
         seed = self.base_seed if base_seed is None else base_seed
         return [torch.Generator(device=self.device).manual_seed(seed * 7919 + gi) for gi in range(lo, hi)]
 
-    def _img2img_noise(self, latent):
-        """Seeded by base_seed alone: every img2img call on one image starts from the same noisy latent."""
-        return torch.randn(latent.shape, generator=torch.Generator().manual_seed(self.base_seed)).to(self.device)
+    def _img2img_noise(self, latent, base_seed=None):
+        """Seeded by base_seed alone (default: the pipeline's): every img2img call on one image starts from the same noisy
+        latent."""
+        seed = self.base_seed if base_seed is None else base_seed
+        return torch.randn(latent.shape, generator=torch.Generator().manual_seed(seed)).to(self.device)
 
-    def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler):
+    def _dpm_img2img_start(self, latent, diffusion, num_steps, strength, sampler, base_seed=None):
         """img2img of the solver samplers -> (start latent, steps kept): the image latent noised to the first kept step."""
         keep = _dpm_keep(num_steps, strength)
         sched = _sampler_schedule(sampler, diffusion, num_steps, keep)
-        return sched.start_latent(latent, self._img2img_noise(latent)), keep
+        return sched.start_latent(latent, self._img2img_noise(latent, base_seed)), keep
 
     @torch.no_grad()
     def _decode(self, cond, batch_size, latent_hw, image_hw, sampler, diffusion, num_steps, guidance_scale, *, noise=None,
@@ -281,7 +283,8 @@ class Kandinsky2_1(_DecoderBase):
         of max_batch slots at h x w, every slot at its own denoising step; each request computes what
         generate_text2img(batch_size=1) computes.  sampler: "p_sampler" (with the dynamic threshold of each request's own x0),
         "ddim_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's steps (the per-slot
-        tables are sized for it).  Per-request LoRA adapters are not served here: max_loras must be 0."""
+        tables are sized for it).  Per-request LoRA adapters are not served here: max_loras must be 0.  submit(image=...,
+        strength=...) queues an img2img request, which computes what generate_img2img(batch_size=1) computes."""
         from .batching import Batcher21
         return Batcher21(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
 
@@ -314,18 +317,25 @@ class Kandinsky2_1(_DecoderBase):
         _check_sampler(sampler, SAMPLERS_21)
         diffusion = self._diffusion(sampler, num_steps)
         image = self._encode_image(pil_img, h, w) * self.scale
-        if sampler in SCHEDULE_SAMPLERS:
-            x, start_step = self._dpm_img2img_start(image, diffusion, num_steps, strength, sampler)
-        else:
-            start_step = int(diffusion.num_timesteps * (1 - strength))
-            dc = self.config["diffusion_config"]
-            x = q_sample(image, diffusion.timestep_map[start_step - 1], schedule_name=dc["noise_schedule"],
-                         num_steps=dc["steps"], noise=self._img2img_noise(image))
+        x, start_step = self._img2img_start(image, diffusion, num_steps, strength, sampler)
         x = x.repeat(2 * batch_size, 1, 1, 1)
         image_emb = self._image_embs(prompt, batch_size)
         return self.generate_img(prompt=prompt, img_prompt=image_emb, batch_size=batch_size,
                                  guidance_scale=guidance_scale, h=h, w=w, sampler=sampler, num_steps=num_steps,
                                  diffusion=diffusion, noise=x, init_step=start_step)
+
+    def _img2img_start(self, image, diffusion, num_steps, strength, sampler, base_seed=None):
+        """img2img of 2.1 -> (start latent [1, 4, h, w], the init_step of generate_img): the solver samplers'
+        _dpm_img2img_start, else the reference's rule (kandinsky2_1_model.py:463-470) -- start_step = int(T * (1 - strength))
+        of the diffusion's T timesteps, from q_sample of the image latent at timestep_map[start_step - 1].  start_step < 1
+        keeps no step.  base_seed: the seed of the noise (default: the pipeline's)."""
+        if sampler in SCHEDULE_SAMPLERS:
+            return self._dpm_img2img_start(image, diffusion, num_steps, strength, sampler, base_seed)
+        start_step = int(diffusion.num_timesteps * (1 - strength))
+        dc = self.config["diffusion_config"]
+        x = q_sample(image, diffusion.timestep_map[start_step - 1], schedule_name=dc["noise_schedule"],
+                     num_steps=dc["steps"], noise=self._img2img_noise(image, base_seed))
+        return x, start_step
 
     def generate_inpainting(self, prompt, pil_img, img_mask, num_steps=100, batch_size=1, guidance_scale=7, h=512,
                             w=512, sampler="ddim_sampler", prior_cf_scale=4, prior_steps="25",
@@ -420,7 +430,9 @@ class Kandinsky2_2(_DecoderBase):
         step.  sampler: "ddpm_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's
         decoder_steps (the per-slot tables are sized for it).  max_loras > 0 lets each request name its own LoRA adapter of
         the decoder (Batcher.add_lora, submit(lora=...)); the batcher then keeps copies of the attention weights, so
-        load_lora / unload_lora on this pipeline afterwards do not change what it computes."""
+        load_lora / unload_lora on this pipeline afterwards do not change what it computes.  submit(image=..., strength=...)
+        queues an img2img request (generate_img2img).  On a task_type="controlnet" pipeline every request takes its own depth
+        hint and computes what generate_controlnet, or with an image generate_controlnet_img2img, computes."""
         from .batching import Batcher
         return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
 
@@ -459,15 +471,16 @@ class Kandinsky2_2(_DecoderBase):
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start, sampler=sampler)
 
-    def _img2img_start(self, lat, diffusion, steps, strength, sampler):
+    def _img2img_start(self, lat, diffusion, steps, strength, sampler, base_seed=None):
         """img2img of the 2.2 methods -> (start latent [1, 4, h, w], the init_step of _decode_loop): the solver samplers'
         _dpm_img2img_start, else diffusers' KandinskyV22Img2ImgPipeline rule -- the last int(steps * strength) DDPM timesteps
-        (at least 1) run, from scheduler.add_noise of the image latent at the first of them."""
+        (at least 1) run, from scheduler.add_noise of the image latent at the first of them.  base_seed: the seed of the noise
+        (default: the pipeline's)."""
         if sampler in SCHEDULE_SAMPLERS:
-            return self._dpm_img2img_start(lat, diffusion, steps, strength, sampler)
+            return self._dpm_img2img_start(lat, diffusion, steps, strength, sampler, base_seed)
         start = _dpm_keep(steps, strength)
         ac = float(diffusion.alphas_cumprod[start - 1])
-        return ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * self._img2img_noise(lat), start
+        return ac ** 0.5 * lat + (1.0 - ac) ** 0.5 * self._img2img_noise(lat, base_seed), start
 
     @staticmethod
     def _hint(hint, h, w):
@@ -528,23 +541,30 @@ class Kandinsky2_2(_DecoderBase):
         if self.task_type != "controlnet":
             raise ValueError("generate_controlnet_img2img needs a pipeline built with task_type='controlnet'")
         pk = self._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt)
-        if prior_strength is not None and (pk is None or not hasattr(self.embedder, "emb2emb")):
-            raise ValueError("prior_strength needs an embedder that runs the prior from an image embedding "
-                             "(runs_prior and emb2emb, e.g. model.prior.PriorEmbedder22)")
+        self._check_prior_strength(prior_strength, pk)
         h, w = self.get_new_h_w(h, w)
-        if prior_strength is None:
-            pos, neg = self._embeds(prompt, batch_size, negative_decoder_prompt, pk)
-        else:
-            pos = self.embedder.emb2emb(prompt, image, batch_size, strength=prior_strength, **pk)
-            neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == "" else
-                   self.embedder.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
-                                         **{**pk, "negative_prior_prompt": ""}))
+        pos, neg = self._controlnet_img2img_embeds(prompt, image, batch_size, negative_decoder_prompt, pk, prior_strength)
         lat = self._encode_image(image, h, w)
         x, start = self._img2img_start(lat, self._diffusion(sampler, decoder_steps), decoder_steps, strength, sampler)
         return self._decode_loop(pos, neg, batch_size, decoder_steps, decoder_guidance_scale, h, w,
                                  latents=x.repeat(2 * batch_size, 1, 1, 1), init_step=start,
                                  hint=self._hint(self._depth_hint(hint), h, w),
                                  sampler=sampler)
+
+    def _check_prior_strength(self, prior_strength, prior_kw):
+        if prior_strength is not None and (prior_kw is None or not hasattr(self.embedder, "emb2emb")):
+            raise ValueError("prior_strength needs an embedder that runs the prior from an image embedding "
+                             "(runs_prior and emb2emb, e.g. model.prior.PriorEmbedder22)")
+
+    def _controlnet_img2img_embeds(self, prompt, image, batch_size, negative_decoder_prompt, prior_kw, prior_strength):
+        """(positive, decoder negative) image embeddings of generate_controlnet_img2img (its docstring gives the rule)."""
+        if prior_strength is None:
+            return self._embeds(prompt, batch_size, negative_decoder_prompt, prior_kw)
+        pos = self.embedder.emb2emb(prompt, image, batch_size, strength=prior_strength, **prior_kw)
+        neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == "" else
+               self.embedder.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
+                                     **{**prior_kw, "negative_prior_prompt": ""}))
+        return pos, neg
 
     def generate_inpainting(self, prompt, pil_img, img_mask, batch_size=1, decoder_steps=50, prior_steps=25,
                             decoder_guidance_scale=4, prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="",
