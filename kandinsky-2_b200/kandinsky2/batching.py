@@ -31,16 +31,25 @@ made, slabs 1 .. L: base + scale * up @ down of a registered adapter, merged by 
 and both GEMMs run batched, rows s and S + s of slot s multiplying the slab a device map names (k2_conv_gemm_wmap).  A
 slot's encoder K/V rows are computed at admission with its adapter's merged encoder_kv weights.  Registering, removing and
 admitting write slabs, the map and conditioning rows in place, so the step graph never changes.
+
+PriorBatcher serves the Kandinsky 2.2 prior the same way: S slots, each an image_emb(prompt, 1) or emb2emb(prompt, image, 1)
+request at its own UnCLIP step of its own tables, one replay of model.prior._PriorSlotPlan per step, results left on the
+device.  A decoder Batcher made with prior_slots = P > 0 runs the pipeline's embedding rules against prior requests instead of
+prior calls at submit; a request waits until its embeddings are done and then joins the decoder queue (requests ready at the
+same prior step in submit order).  step() replays one prior step before the decoder step while the prior batch has work,
+and prior steps back to back until a prior request finishes when a decoder slot is free and no ready request can take it.
 """
 import collections
 import inspect
 
+import numpy as np
 import torch
 
 from . import ops, parallel
 from ._native import K2Error
 from .launch_plan import capture_graph
 from .model.gaussian_diffusion import SpacedDiffusion
+from .model.prior import UnCLIPSchedule, _PriorSlotPlan
 from .model.unet import _Plan
 from .pipelines import _sampler_schedule
 
@@ -155,11 +164,17 @@ class Batcher:
     SAMPLERS = BATCHER_SAMPLERS
     TASKS = ("text2img", "controlnet")
     hinted = False   # True on a ControlNet pipeline's batcher: every request brings its own depth hint
+    prior = None     # the PriorBatcher of a batcher made with prior_slots > 0
 
-    def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
+    def __init__(self, pipe, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0, prior_slots=0):
         self._check_args(max_batch, h, w, sampler, max_steps, max_loras)
         if pipe.task_type not in self.TASKS:
             raise ValueError(f"batcher: serves {' and '.join(self.TASKS)} pipelines only, this one is {pipe.task_type!r}")
+        if isinstance(prior_slots, bool) or not isinstance(prior_slots, int) or prior_slots < 0:
+            raise ValueError(f"batcher: prior_slots must be an int >= 0, got {prior_slots!r}")
+        if prior_slots and not hasattr(pipe.embedder, "batcher"):
+            raise ValueError("batcher: prior_slots > 0 needs an embedder that samples the prior in a batch (batcher(max_batch), "
+                             f"e.g. model.prior.PriorEmbedder22); this pipeline's is a {type(pipe.embedder).__name__}")
         self.pipe, self.sampler, self.max_steps = pipe, sampler, max_steps
         self.hinted = pipe.task_type == "controlnet"
         self.h, self.w, H, W = self._geometry(h, w)
@@ -218,6 +233,11 @@ class Batcher:
         self.queue = SlotQueue(S)
         self._requests = {}
         self._next_handle = 0
+        # prompt requests' image embeddings sampled in a batch of prior slots: a decoder request waits in _held (handle ->
+        # embeddings still missing) until the prior requests in _waiting_on (prior handle -> (handle, "positive" /
+        # "negative")) are done
+        self.prior = pipe.embedder.batcher(prior_slots) if prior_slots else None
+        self._held, self._waiting_on = {}, {}
         self._emb_dim = pipe.config["model_config"]["image_encoder_in_dim"]
         # one event per replayed step, the newest RUN_AHEAD of them: step() waits for the oldest before it admits, so the host
         # stays at most RUN_AHEAD steps ahead of the GPU and a request that arrives while a slot is free joins the batch at the
@@ -314,6 +334,8 @@ class Batcher:
         pk = pipe._prior_kwargs(prior_steps, prior_guidance_scale, negative_prior_prompt) if prompt is not None else None
         if prior_strength is not None:
             pipe._check_prior_strength(prior_strength, pk)
+        # with prior slots the pipeline's embedding rules run against _PriorQueue: prior requests, checked, queued by _enqueue
+        embedder = _PriorQueue(self.prior, pipe.embedder) if self.prior is not None else None
         r = _Request()
         r.lora = lora
         r.guidance = float(decoder_guidance_scale)
@@ -324,10 +346,10 @@ class Batcher:
         if prompt is None:
             r.positive, r.negative = image_embeds, negative_image_embeds
         elif prior_strength is None:
-            r.positive, r.negative = pipe._embeds(prompt, 1, negative_decoder_prompt, pk)
+            r.positive, r.negative = pipe._embeds(prompt, 1, negative_decoder_prompt, pk, embedder)
         else:
             r.positive, r.negative = pipe._controlnet_img2img_embeds(prompt, image, 1, negative_decoder_prompt, pk,
-                                                                     prior_strength)
+                                                                     prior_strength, embedder)
         return self._enqueue(r)
 
     def _check_hint(self, hint):
@@ -374,7 +396,8 @@ class Batcher:
         return x, start
 
     def _enqueue(self, r):
-        """Queue a request whose tables are set -> its handle; it runs one step per row of its tables."""
+        """Queue a request whose tables are set -> its handle; it runs one step per row of its tables.  An embedding that is
+        a prior request (_PriorRequest) is queued on the prior batcher, and the request waits for it in _held."""
         r.steps = r.ts.shape[0]
         if r.steps > self.max_steps:
             raise ValueError(f"submit: the request's schedule has {r.steps} steps, more than the batcher's max_steps "
@@ -382,8 +405,53 @@ class Batcher:
         handle = self._next_handle
         self._next_handle += 1
         self._requests[handle] = r
-        self.queue.submit(handle, r.steps)
+        waits = [name for name in ("positive", "negative") if isinstance(getattr(r, name), _PriorRequest)]
+        if not waits:
+            self.queue.submit(handle, r.steps)
+            return handle
+        self._held[handle] = len(waits)
+        for name in waits:
+            self._waiting_on[self.prior.enqueue(getattr(r, name))] = (handle, name)
         return handle
+
+    def _prior_step(self):
+        """One step of the prior batch; the embeddings it finished go to their requests, and the requests that now have all
+        of theirs join the decoder queue in submit order -> whether a prior request finished.  A prior request whose
+        admission failed is gone from the prior batcher: its decoder request is dropped too (and the result of its other
+        prior request, if any, discarded), then the error propagates, as for a failed decoder admission."""
+        try:
+            done = self.prior.step()
+        except BaseException:
+            lost = {self._waiting_on[ph][0] for ph in self._waiting_on if ph not in self.prior._requests}
+            for ph in [ph for ph, (handle, _) in self._waiting_on.items() if handle in lost]:
+                del self._waiting_on[ph]
+            for handle in lost:
+                del self._held[handle], self._requests[handle]
+            raise
+        ready = []
+        for ph, emb in done.items():
+            if ph not in self._waiting_on:   # the other embedding of a dropped request
+                continue
+            handle, name = self._waiting_on.pop(ph)
+            setattr(self._requests[handle], name, emb)
+            self._held[handle] -= 1
+            if not self._held[handle]:
+                del self._held[handle]
+                ready.append(handle)
+        for handle in sorted(ready):
+            self.queue.submit(handle, self._requests[handle].steps)
+        return bool(done)
+
+    def _run_prior(self):
+        """The prior steps of one step(): while a decoder slot is free and no ready request can take it, prior steps back to
+        back until a prior request finishes; otherwise one prior step while the prior batch has work."""
+        if not self.prior.pending():
+            return
+        if None in self.queue.holder and not self.queue.waiting:
+            while self.prior.pending() and not self._prior_step():
+                pass
+        else:
+            self._prior_step()
 
     def _admit(self):
         """Stage waiting requests into free slots, one at a time: a request holds its slot in the host bookkeeping only once
@@ -438,6 +506,8 @@ class Batcher:
             raise K2Error("batcher: the UNet's weights were reloaded after the batcher was made; make a new one")
         if len(self._events) >= self.RUN_AHEAD:
             self._events.popleft().synchronize()   # waits for a step to end; reads nothing back
+        if self.prior is not None:
+            self._run_prior()
         self._admit()
         if not self.queue.busy():
             return {}
@@ -461,7 +531,7 @@ class Batcher:
     def run(self):
         """step() until every submitted request is finished -> {handle: PIL image} of all of them."""
         out = {}
-        while self.queue.waiting or self.queue.busy():
+        while self.queue.waiting or self.queue.busy() or (self.prior is not None and self._held):
             out.update(self.step())
         return out
 
@@ -528,3 +598,167 @@ class Batcher21(Batcher):
 
     def _bind(self, s, r):
         self.pipe.model.bind_slot(self.plan, s, r.negative, r.positive, full_emb=r.full, pooled_emb=r.pooled)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the Kandinsky 2.2 prior in continuously refilled slots
+# ------------------------------------------------------------------------------------------------------------------------------
+def prior_request_tables(steps, keep=None):
+    """(timesteps fp32 [n], coefficient rows fp32 [n, 8]) of one prior request in loop order, n = keep or steps: the rows
+    _PriorStepPlan.set_schedule stages from UnCLIPSchedule(steps, keep=keep)."""
+    sched = UnCLIPSchedule(steps, keep=keep)
+    return torch.from_numpy(sched.timesteps.astype(np.float32)), torch.from_numpy(sched.coef_table())
+
+
+class _PriorRequest:
+    __slots__ = ("steps", "guidance", "rows", "ts", "coef", "x", "noise")
+
+
+class PriorBatcher:
+    """Kandinsky 2.2 prior requests served from max_batch slots (PriorEmbedder22.batcher builds it): one UnCLIP sampling step of
+    every slot is ONE replay of a captured _PriorSlotPlan graph, each slot at its own step of its own tables, refilled from
+    a FIFO queue as requests finish.  A request computes what the embedder's image_emb(prompt, 1, ...) -- or with an image
+    emb2emb(prompt, image, 1, strength, ...) -- computes: the CLIP rows, guidance and generator of its _call_args, the same
+    draws in the same order, UnCLIPSchedule's tables, and a slot step that runs the batch step's kernels on the slot's rows
+    alone.  Its result stays on the device.  The host reads nothing back: it knows from its own bookkeeping which slot
+    finishes at which step."""
+
+    MAX_STEPS = 1000   # table rows per slot, _PriorStepPlan's limit
+
+    def __init__(self, embedder, max_batch):
+        if isinstance(max_batch, bool) or not isinstance(max_batch, int) or max_batch < 1:
+            raise ValueError(f"prior batcher: max_batch must be a positive int, got {max_batch!r}")
+        self.embedder = embedder
+        prior = embedder.prior
+        if prior._packed is None:
+            prior.finalize()
+        self._weights = (prior._packed, prior._lora)
+        # a plan of its own: a batch-1 image_emb call between steps must not rebind these rows
+        self.plan = _PriorSlotPlan(prior, max_batch, self.MAX_STEPS)   # recorded by running it once, every slot idle
+        self.queue = SlotQueue(max_batch)
+        self._requests = {}
+        self._next_handle = 0
+        torch.cuda.synchronize()
+        self.graph = capture_graph(self.plan.launch)
+
+    def submit(self, prompt, *, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None, image=None,
+               strength=None):
+        """Queue one image embedding -> its handle (the key of its embedding in what step() / run() return).  Without image:
+        image_emb(prompt, 1, prior_steps, prior_guidance_scale, negative_prior_prompt); with one (a CLIP image embedding [1, D]
+        / [D], or a PIL image for the embedder's clip_image): emb2emb(prompt, image, 1, strength, ...), strength defaulting to
+        emb2emb's.  Unset keywords are the embedder's defaults."""
+        return self.enqueue(self.request(prompt, prior_steps=prior_steps, prior_guidance_scale=prior_guidance_scale,
+                                         negative_prior_prompt=negative_prior_prompt, image=image, strength=strength))
+
+    def request(self, prompt, *, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None, image=None,
+                strength=None):
+        """The request submit queues, checked and drawn but not queued (enqueue queues it)."""
+        emb = self.embedder
+        steps = emb.prior_steps if prior_steps is None else prior_steps
+        if isinstance(steps, bool) or not isinstance(steps, int) or not 2 <= steps <= self.MAX_STEPS:
+            raise ValueError(f"submit: prior_steps must be an int in [2, {self.MAX_STEPS}], got {steps!r}")
+        keep = None
+        if image is None and strength is not None:
+            raise ValueError("submit: strength without image; strength is how much of the prior an image request runs")
+        if image is not None:
+            if strength is None:   # emb2emb's default
+                strength = inspect.signature(type(emb).emb2emb).parameters["strength"].default
+            if isinstance(strength, bool) or not isinstance(strength, (int, float)):
+                raise ValueError(f"submit: strength must be a number in [0, 1], got {strength!r}")
+            keep = emb._emb2emb_keep(steps, strength, who="submit")
+            D = emb.prior.clip_dim
+            if torch.is_tensor(image) and tuple(image.shape) not in ((D,), (1, D)):
+                raise ValueError(f"submit: image must be one CLIP image embedding, [1, {D}] or [{D}], or a PIL image; got "
+                                 f"{list(image.shape)}")
+            start = emb._image_embedding(image, 1, who="submit: image")
+        steps, g, rows, gen = emb._call_args(prompt, 1, steps, prior_guidance_scale, negative_prior_prompt)
+        dev, D = emb.clip_mean.device, emb.prior.clip_dim
+        r = _PriorRequest()
+        # image_emb's draws: x_T, then the step noise; emb2emb's: z, then the noise of the kept steps
+        x = torch.randn(1, D, device=dev, generator=gen)
+        r.noise = torch.randn(steps if keep is None else keep, 1, D, device=dev, generator=gen)
+        r.x = x if keep is None else UnCLIPSchedule(steps, keep=keep).start_latent(start, x)
+        r.ts, r.coef = prior_request_tables(steps, keep)
+        r.steps, r.guidance, r.rows = r.ts.shape[0], g, rows
+        return r
+
+    def enqueue(self, r):
+        """Queue a request made by request() -> its handle."""
+        handle = self._next_handle
+        self._next_handle += 1
+        self._requests[handle] = r
+        self.queue.submit(handle, r.steps)
+        return handle
+
+    def pending(self):
+        """Whether a request is waiting or being sampled."""
+        return bool(self.queue.waiting) or self.queue.busy()
+
+    def _admit(self):
+        """Stage waiting requests into free slots, one at a time, as Batcher._admit does."""
+        while True:
+            got = self.queue.admit(limit=1)
+            if not got:
+                return
+            s, handle = got[0]
+            try:
+                self._stage(s, self._requests[handle])
+            except BaseException:
+                self.queue.release(s)
+                self.plan.state[:, s] = torch.tensor([-1, 0], dtype=torch.int32)
+                del self._requests[handle]
+                raise
+
+    def _stage(self, s, r):
+        p, k = self.plan, r.steps
+        p.bind_slot(s, *r.rows)
+        p.ts_tab[s, :k].copy_(r.ts)
+        p.coef_tab[s, :k].copy_(r.coef)
+        p.noise_tab[s, :k].copy_(r.noise[:, 0])
+        p.x[s].copy_(r.x[0])
+        p.guidance[s] = r.guidance
+        p.state[:, s] = torch.tensor([0, k], dtype=torch.int32)
+
+    def step(self):
+        """Admit waiting requests into free slots, run one UnCLIP step of every occupied slot (one graph replay) -> {handle:
+        fp32 [1, clip_dim] on the device} of the requests it finished, each a tensor of its own (x * clip_std + clip_mean,
+        as sample_prior22 finishes)."""
+        prior = self.embedder.prior
+        if prior._packed is not self._weights[0] or prior._lora is not self._weights[1]:
+            raise K2Error("prior batcher: the prior's packed weights changed after the batcher was made (load_lora, "
+                          "unload_lora or a reload); make a new one")
+        self._admit()
+        if not self.queue.busy():
+            return {}
+        self.graph.replay()
+        done = {}
+        emb = self.embedder
+        for s, handle in self.queue.advance():
+            done[handle] = self.plan.x[s:s + 1] * emb.clip_std + emb.clip_mean
+            del self._requests[handle]
+        return done
+
+    def run(self):
+        """step() until every submitted request is finished -> {handle: embedding} of all of them."""
+        out = {}
+        while self.pending():
+            out.update(self.step())
+        return out
+
+
+class _PriorQueue:
+    """The embedder calls of the pipeline's embedding rules (Kandinsky2_2._embeds, _negative, _controlnet_img2img_embeds) at
+    batch 1 as prior requests: image_emb and emb2emb return a PriorBatcher request, checked but not queued (Batcher._enqueue
+    queues it once the whole decoder request is checked); zero_image_emb is the embedder's own."""
+
+    def __init__(self, prior, embedder):
+        self.prior, self.embedder = prior, embedder
+
+    def image_emb(self, prompt, batch_size, **prior_kw):
+        return self.prior.request(prompt, **prior_kw)
+
+    def emb2emb(self, prompt, image, batch_size, strength, **prior_kw):
+        return self.prior.request(prompt, image=image, strength=strength, **prior_kw)
+
+    def zero_image_emb(self, batch_size):
+        return self.embedder.zero_image_emb(batch_size)

@@ -33,7 +33,7 @@ import torch.nn as nn
 
 from .. import ops
 from .._native import K2Error
-from ..launch_plan import LaunchPlan
+from ..launch_plan import LaunchPlan, tune
 from .encoder import pack_layers, record_layers
 from .gaussian_diffusion import SpacedDiffusion, space_timesteps
 
@@ -415,50 +415,33 @@ class UnCLIPSchedule:
         return self.rows().astype(np.float32)
 
 
-class _PriorStepPlan(LaunchPlan):
-    """One UnCLIP sampling step of the prior at B samples, on static buffers, as ONE launch list (replayed as one CUDA graph):
-    k2_step_begin (x duplicated for the 2B CFG rows, this step's t / row / noise picked by the device-side counter), the time
-    embedding and its two linears, clip_img_proj, the token rows 78 and 79 written into the sequence, the 20 pre-LayerNorm
-    layers of model/encoder.py with the masked k2_attention_small as the attention, the final LayerNorm of the last
-    token (a strided view), out_proj, k2_sampler_step and k2_step_end.  What does not change from step to step -- the text
-    token rows, the text_emb_proj and prd_emb rows with their positional embedding, the keep mask -- is written once per call
-    by bind().  Layer 0 reads the sequence buffer as its residual input.
+class _PriorNet(LaunchPlan):
+    """The prior network of one UnCLIP sampling step over N CFG rows, as launches recorded into a plan: the buffers the step
+    plans share (x_in, t_in, the sequence, the keep mask, model_out) and the recording of the time embedding and its two
+    linears, clip_img_proj, the token rows 78 and 79 written into the sequence, the 20 pre-LayerNorm layers of
+    model/encoder.py with the masked k2_attention_small as the attention, the final LayerNorm of the last token (a strided
+    view) and out_proj.  Every launch has the eager forward's arguments.  _PriorStepPlan (one call at B samples) and
+    _PriorSlotPlan (S slots, each at its own step) put their step begin / sampler step / step end around it."""
 
-    Every launch has the eager forward's arguments, so the model output (self.model_out[:, :clip_dim]) equals
-    PriorTransformer.forward bit for bit under the same GEMM configurations (the per-shape tuner may pick split-K, which
-    reorders fp32 sums; with launch_plan.TUNE_SMALL_M = 0 it only picks among bit-identical configurations)."""
-
-    def __init__(self, model, B):
+    def __init__(self, model, N):
         dev = model._packed["text_enc"][0].device
-        super().__init__(dev, 2 * B)
-        self.m, self.B = model, B
-        N, W, D, n, ctx = 2 * B, model.xf_width, model.clip_dim, model.text_ctx + model.ext_len, model.text_ctx
+        super().__init__(dev, N)
+        self.m = model
+        W, D, n = model.xf_width, model.clip_dim, model.text_ctx + model.ext_len
         if D % 4:
             raise K2Error("k2b200 prior: clip_dim must be a multiple of 4 (the sampler step sees it as [4, 1, clip_dim / 4])")
         self.N, self.n = N, n
         f32 = dict(device=dev, dtype=torch.float32)
-        self.x = torch.zeros(B, D, **f32)                   # the sample, updated in place every step
         self.x_in = torch.zeros(N, D, **f32)
         self.t_in = torch.zeros(N, **f32)
-        self.coef = torch.zeros(8, **f32)
-        self.noise = torch.zeros(B, D, **f32)
-        self.work = torch.empty(B * D + 4096, **f32)
-        self.counter = torch.zeros(2, device=dev, dtype=torch.int32)
-        self.ts_seq = torch.zeros(1000, **f32)
-        self.coef_seq = torch.zeros(1000, 8, **f32)
-        self.noise_seq = torch.zeros(1000, B, D, **f32)
-        self.guidance = 4.0
-        # model_out [2B, 2 * clip_dim]: out_proj writes the first clip_dim columns of each row, the variance half stays zero
+        # model_out [N, 2 * clip_dim]: out_proj writes the first clip_dim columns of each row, the variance half stays zero
         self.model_out = torch.zeros(N, 2 * D, **f32)
         self.seq = torch.zeros(N, n, W, device=dev, dtype=torch.float16)
         self.keep = torch.ones(N, n, device=dev, dtype=torch.uint8)
         self.pos16 = model.positional_embedding[0].half().contiguous()
-        self._te32 = torch.empty(N * ctx, W, **f32)
-        self._row32 = torch.empty(N, W, **f32)
-        self._build()
 
-    def _build(self):
-        m, pk, N, n, W, B = self.m, self.m._packed, self.N, self.n, self.m.xf_width, self.B
+    def _record_network(self):
+        m, pk, N, n, W = self.m, self.m._packed, self.N, self.n, self.m.xf_width
         D, ctx, H = m.clip_dim, m.text_ctx, m.xf_heads
         S = self._add
         f32 = dict(device=self.dev, dtype=torch.float32)
@@ -466,8 +449,6 @@ class _PriorStepPlan(LaunchPlan):
         te0, te2, img, outp = (lw(getattr(m.time_embed, "0")), lw(getattr(m.time_embed, "2")), lw(m.clip_img_proj),
                                lw(m.out_proj))
         e0, e1, tok_t, tok_x = (torch.empty(N, W, **f32) for _ in range(4))
-        S(lambda: ops.step_begin(self.x, self.x_in, self.t_in, self.coef, self.ts_seq, self.coef_seq, self.noise_seq, self.noise,
-                                 self.counter), "step")
         S(lambda: ops.timestep_embedding(self.t_in, W, out=e0), "timestep_embedding")
         S(lambda: ops.linear(e0, *te0, out=e1), "linear", 2 * N * W * W)
         S(lambda: ops.linear(e1, *te2, silu_in=True, out=tok_t), "linear", 2 * N * W * W)
@@ -488,25 +469,68 @@ class _PriorStepPlan(LaunchPlan):
         else:
             S(lambda: ops.f16_to_f32(last, out=last32), "widen")
         S(lambda: ops.linear(last32, *outp, out=self.model_out[:, :D]), "linear", 2 * N * W * D)
+
+    def _fixed_rows(self, text_emb, text_enc, mask, seq, keep, te32, row32):
+        """The conditioning of len(seq) CFG rows -> the sequence rows that stay fixed for every step and the keep mask, written
+        into seq / keep with the eager forward's arithmetic (text_enc_proj GEMM, text_emb_proj linear, prd_emb, + positional
+        rows); te32 / row32: fp32 scratch of [rows * text_ctx, W] / [rows, W]."""
+        m, W, ctx = self.m, self.m.xf_width, self.m.text_ctx
+        N = seq.shape[0]
+        keep.copy_(torch.nn.functional.pad(mask.bool(), (0, m.ext_len), value=True).to(torch.uint8))
+        wte, bte = m._packed["text_enc"]
+        te16 = ops.f32_to_f16(text_enc.float().contiguous()).reshape(N * ctx, m.clip_xf_width)
+        ops.f16_to_f32(ops.gemm_rows(te16, wte, W, bias=bte), out=te32)
+        for b in range(N):
+            ops.prior_tokens(te32[b * ctx:(b + 1) * ctx], self.pos16[:ctx], seq[b, :ctx])
+        ops.linear(text_emb.float().contiguous(), m.text_emb_proj.weight.float().contiguous(), m.text_emb_proj.bias.float(),
+                   out=row32)
+        ops.prior_tokens(row32, self.pos16[ctx:ctx + 1].expand(N, W), seq[:, ctx])
+        ops.prior_tokens(m.prd_emb[0].float().expand(N, W), self.pos16[ctx + 3:ctx + 4].expand(N, W), seq[:, ctx + 3])
+
+
+class _PriorStepPlan(_PriorNet):
+    """One UnCLIP sampling step of the prior at B samples, on static buffers, as ONE launch list (replayed as one CUDA graph):
+    k2_step_begin (x duplicated for the 2B CFG rows, this step's t / row / noise picked by the device-side counter), the
+    network of _PriorNet, k2_sampler_step and k2_step_end.  What does not change from step to step -- the text token rows,
+    the text_emb_proj and prd_emb rows with their positional embedding, the keep mask -- is written once per call by bind().
+    Layer 0 reads the sequence buffer as its residual input.
+
+    Every launch has the eager forward's arguments, so the model output (self.model_out[:, :clip_dim]) equals
+    PriorTransformer.forward bit for bit under the same GEMM configurations (the per-shape tuner may pick split-K, which
+    reorders fp32 sums; with launch_plan.TUNE_SMALL_M = 0 it only picks among bit-identical configurations)."""
+
+    def __init__(self, model, B):
+        super().__init__(model, 2 * B)
+        self.B = B
+        D, W, ctx = model.clip_dim, model.xf_width, model.text_ctx
+        f32 = dict(device=self.dev, dtype=torch.float32)
+        self.x = torch.zeros(B, D, **f32)                   # the sample, updated in place every step
+        self.coef = torch.zeros(8, **f32)
+        self.noise = torch.zeros(B, D, **f32)
+        self.work = torch.empty(B * D + 4096, **f32)
+        self.counter = torch.zeros(2, device=self.dev, dtype=torch.int32)
+        self.ts_seq = torch.zeros(1000, **f32)
+        self.coef_seq = torch.zeros(1000, 8, **f32)
+        self.noise_seq = torch.zeros(1000, B, D, **f32)
+        self.guidance = 4.0
+        self._te32 = torch.empty(self.N * ctx, W, **f32)
+        self._row32 = torch.empty(self.N, W, **f32)
+        self._build()
+
+    def _build(self):
+        N, B, D = self.N, self.B, self.m.clip_dim
+        self._add(lambda: ops.step_begin(self.x, self.x_in, self.t_in, self.coef, self.ts_seq, self.coef_seq, self.noise_seq,
+                                         self.noise, self.counter), "step")
+        self._record_network()
         x4, n4, mo8 = self.x.view(B, 4, 1, D // 4), self.noise.view(B, 4, 1, D // 4), self.model_out.view(N, 8, 1, D // 4)
-        S(lambda: ops.sampler_step(mo8, x4, n4, self.coef, self.guidance, 0, clip=10.0, threshold_mode=0, work=self.work),
-          "sampler_step")
-        S(lambda: ops.step_end(self.counter), "step")
+        self._add(lambda: ops.sampler_step(mo8, x4, n4, self.coef, self.guidance, 0, clip=10.0, threshold_mode=0,
+                                           work=self.work), "sampler_step")
+        self._add(lambda: ops.step_end(self.counter), "step")
 
     def bind(self, text_emb, text_enc, mask):
         """This call's conditioning (2B rows, [uncond | cond]) -> the sequence rows that stay fixed for every step and the keep
-        mask, with the eager forward's arithmetic (text_enc_proj GEMM, text_emb_proj linear, prd_emb, + positional rows)."""
-        m, N, n, W, ctx = self.m, self.N, self.n, self.m.xf_width, self.m.text_ctx
-        self.keep.copy_(torch.nn.functional.pad(mask.bool(), (0, m.ext_len), value=True).to(torch.uint8))
-        wte, bte = m._packed["text_enc"]
-        te16 = ops.f32_to_f16(text_enc.float().contiguous()).reshape(N * ctx, m.clip_xf_width)
-        ops.f16_to_f32(ops.gemm_rows(te16, wte, W, bias=bte), out=self._te32)
-        for b in range(N):
-            ops.prior_tokens(self._te32[b * ctx:(b + 1) * ctx], self.pos16[:ctx], self.seq[b, :ctx])
-        ops.linear(text_emb.float().contiguous(), m.text_emb_proj.weight.float().contiguous(), m.text_emb_proj.bias.float(),
-                   out=self._row32)
-        ops.prior_tokens(self._row32, self.pos16[ctx:ctx + 1].expand(N, W), self.seq[:, ctx])
-        ops.prior_tokens(m.prd_emb[0].float().expand(N, W), self.pos16[ctx + 3:ctx + 4].expand(N, W), self.seq[:, ctx + 3])
+        mask (_fixed_rows)."""
+        self._fixed_rows(text_emb, text_enc, mask, self.seq, self.keep, self._te32, self._row32)
 
     def set_schedule(self, sched, x_T, step_noise, guidance, use_graph=True):
         """Stage a run: the schedule's kept timesteps and rows, x_T [B, clip_dim], step_noise [keep, B, clip_dim]; resets the
@@ -524,6 +548,81 @@ class _PriorStepPlan(LaunchPlan):
         self.noise_seq[:k].copy_(step_noise)
         self.x.copy_(x_T)
         self.counter.copy_(torch.tensor([0, k], dtype=torch.int32))
+
+
+class _PriorSlotPlan(_PriorNet):
+    """One UnCLIP sampling step of S slots, each slot a request at its own step of its own tables (batching.PriorBatcher), as
+    ONE launch list over 2S CFG rows (unconditional row s, conditional row S + s): k2_slot_step_begin on x [S, 4, 1,
+    clip_dim / 4] (so a slot's n is clip_dim), the network of _PriorNet, k2_slot_sampler_step (clip 10, the unconditional
+    rows first, no threshold, each slot's guidance from the device array `guidance` [S]) and k2_slot_step_end.  state is the
+    device int32 [2, S] (k_s, steps_s) of k2b200.h; the tables hold max_steps rows per slot.  bind_slot writes one slot's
+    fixed sequence rows and keep-mask rows; what a slot's step computes depends on its own rows alone."""
+
+    def __init__(self, model, S, max_steps=1000):
+        super().__init__(model, 2 * S)
+        self.S = S
+        D, W, n, ctx = model.clip_dim, model.xf_width, self.n, model.text_ctx
+        f32 = dict(device=self.dev, dtype=torch.float32)
+        self.x = torch.zeros(S, D, **f32)
+        self.coef = torch.zeros(S, 8, **f32)
+        self.noise = torch.zeros(S, D, **f32)
+        self.work = torch.zeros(S, D, **f32)
+        self.guidance = torch.zeros(S, **f32)
+        self.state = torch.tensor([[-1] * S, [0] * S], device=self.dev, dtype=torch.int32)
+        self.ts_tab = torch.zeros(S, max_steps, **f32)
+        self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
+        self.noise_tab = torch.zeros(S, max_steps, D, **f32)
+        # bind_slot computes a slot's rows at bind's B = 1 shapes (2 rows) here, then copies them into rows s and S + s
+        self._seq2 = torch.zeros(2, n, W, device=self.dev, dtype=torch.float16)
+        self._keep2 = torch.ones(2, n, device=self.dev, dtype=torch.uint8)
+        self._te32 = torch.empty(2 * ctx, W, **f32)
+        self._row32 = torch.empty(2, W, **f32)
+        self._build()
+
+    def _build(self):
+        S, N, D = self.S, self.N, self.m.clip_dim
+        x4, n4, w4 = (t.view(S, 4, 1, D // 4) for t in (self.x, self.noise, self.work))
+        mo8 = self.model_out.view(N, 8, 1, D // 4)
+        self._add(lambda: ops.slot_step_begin(x4, self.x_in, self.t_in, self.coef, self.ts_tab, self.coef_tab, self.noise_tab,
+                                              n4, self.state), "step")
+        self._record_network()
+        self._add(lambda: ops.slot_sampler_step(mo8, x4, n4, self.coef, self.guidance, self.state, w4, 10.0, cond_first=0,
+                                                threshold_mode=0), "sampler_step")
+        self._add(lambda: ops.slot_step_end(self.state), "step")
+
+    def _gemm(self, x, w, cout, out, flops, bias=None, residual=None):
+        """The layers' flat-row GEMM at 2S rows, pinned to the N tile and split-K factor the batch-1 plan (_PriorStepPlan at
+        B = 1: 2 CFG rows) runs it with -- the choice tune() caches for the 2-row shape, as the library then applies it.  The
+        library's own cycle model picks the split-K factor from the row count, and a split changes the fp32 summation order;
+        pinned, every row sums as at batch 1, so a slot computes what image_emb(prompt, 1) computes."""
+        rows, n = x.shape[0], x.shape[1]
+        x2, out2 = x[:2], out[:2]
+        res2 = residual[:2] if residual is not None else None
+        run2 = lambda cfg, info=None: ops.gemm_rows(x2, w, cout, bias=bias, residual=res2, out=out2, cfg=cfg,  # noqa: E731
+                                                    info=info)
+        info = [0] * 7
+        run2(tune(("gemm", cout, tuple(x2.shape), residual is not None), run2, m_rows=2 * n), info)
+        cfg = (info[0], 0, info[2], 1)
+        got = [0] * 7
+        self._add(lambda: ops.gemm_rows(x, w, cout, bias=bias, residual=residual, out=out, cfg=cfg, info=got), "conv_gemm",
+                  flops)
+        if (got[0], got[2]) != (cfg[0], cfg[2]):
+            raise K2Error(f"k2b200 prior: the GEMM of {rows} x {n} rows to {cout} columns cannot take the batch-1 plan's N tile "
+                          f"{cfg[0]} and split-K factor {cfg[2]} (it ran {got[0]} / {got[2]}); use fewer slots")
+        self._parts.pop(out.data_ptr(), None)
+
+    def bind_slot(self, s, text_emb, text_enc, mask):
+        """Slot s's conditioning (2 rows, [uncond | cond]) -> its fixed sequence rows (the text tokens, the text_emb_proj and
+        prd_emb rows, with their positional rows) and keep-mask rows, computed as bind computes them at B = 1 and copied into
+        rows s and S + s; no other row changes, so the rows have the same bits in every slot."""
+        if not 0 <= s < self.S:
+            raise K2Error(f"bind_slot: slot {s} outside [0, {self.S})")
+        ctx = self.m.text_ctx
+        self._fixed_rows(text_emb, text_enc, mask, self._seq2, self._keep2, self._te32, self._row32)
+        for src, row in ((0, s), (1, self.S + s)):
+            self.seq[row, :ctx + 1].copy_(self._seq2[src, :ctx + 1])
+            self.seq[row, ctx + 3].copy_(self._seq2[src, ctx + 3])
+            self.keep[row].copy_(self._keep2[src])
 
 
 @torch.no_grad()
@@ -669,29 +768,48 @@ class PriorEmbedder22:
         x * clip_std + clip_mean (post_process_latents), as for image_emb.  Rows, guidance and the negative prior prompt are
         image_emb's; the generator draws z [B, clip_dim] first, then the step noise [keep, B, clip_dim]."""
         steps = self.prior_steps if prior_steps is None else int(prior_steps)
-        strength = float(strength)
-        if not 0.0 <= strength <= 1.0:
-            raise ValueError(f"PriorEmbedder22.emb2emb: strength must be in [0, 1], got {strength}")
-        keep = min(int(steps * strength), steps)
-        if keep == 0:
-            raise ValueError(f"PriorEmbedder22.emb2emb: strength {strength} keeps no step of {steps} (int(N * strength) = 0)")
+        keep = self._emb2emb_keep(steps, strength)
         sched = UnCLIPSchedule(steps, keep=keep)
         dev, B, D = self.clip_mean.device, batch_size, self.prior.clip_dim
-        if torch.is_tensor(image):
-            emb = image.float().reshape(-1, D) if image.dim() == 1 else image.float()
-            if emb.dim() != 2 or emb.shape[1] != D or emb.shape[0] not in (1, B):
-                raise ValueError(f"PriorEmbedder22.emb2emb: an image embedding must be [1, {D}] or [{B}, {D}], got "
-                                 f"{list(image.shape)}")
-        else:
-            if self.clip_image is None:
-                raise K2Error("PriorEmbedder22.emb2emb: a PIL image needs clip_image=")
-            emb = self.clip_image(image).float().reshape(1, D)
-        emb = emb.to(dev).expand(B, D)
+        emb = self._image_embedding(image, B)
         steps, g, rows, gen = self._call_args(prompt, B, steps, prior_guidance_scale, negative_prior_prompt)
         z = torch.randn(B, D, device=dev, generator=gen)
         noise = torch.randn(keep, B, D, device=dev, generator=gen)
         return sample_prior22(self.prior, *rows, steps, g, self.clip_mean, self.clip_std, sched.start_latent(emb, z), noise,
                               use_graph=self.use_cuda_graph, keep=keep).float().cpu()
+
+    def batcher(self, max_batch):
+        """A batching.PriorBatcher: image_emb(prompt, 1, ...) and emb2emb(prompt, image, 1, ...) requests submitted one at a
+        time and sampled in one continuously refilled batch of max_batch slots, every slot at its own UnCLIP step, one CUDA
+        graph replay per step; each result is the embedding the batch-1 call computes, left on the device."""
+        from ..batching import PriorBatcher
+        return PriorBatcher(self, max_batch)
+
+    @staticmethod
+    def _emb2emb_keep(steps, strength, who="PriorEmbedder22.emb2emb"):
+        """The UnCLIP steps emb2emb runs of `steps` at `strength` (get_timesteps): min(int(N * strength), N); ValueError for
+        a strength outside [0, 1] or one that keeps no step."""
+        strength = float(strength)
+        if not 0.0 <= strength <= 1.0:
+            raise ValueError(f"{who}: strength must be in [0, 1], got {strength}")
+        keep = min(int(steps * strength), steps)
+        if keep == 0:
+            raise ValueError(f"{who}: strength {strength} keeps no step of {steps} (int(N * strength) = 0)")
+        return keep
+
+    def _image_embedding(self, image, B, who="PriorEmbedder22.emb2emb"):
+        """emb2emb's image -> its CLIP image embedding [B, clip_dim] on the device: a tensor [1, clip_dim] / [clip_dim]
+        (repeated) or [B, clip_dim], or a PIL image through clip_image."""
+        dev, D = self.clip_mean.device, self.prior.clip_dim
+        if torch.is_tensor(image):
+            emb = image.float().reshape(-1, D) if image.dim() == 1 else image.float()
+            if emb.dim() != 2 or emb.shape[1] != D or emb.shape[0] not in (1, B):
+                raise ValueError(f"{who}: an image embedding must be [1, {D}] or [{B}, {D}], got {list(image.shape)}")
+        else:
+            if self.clip_image is None:
+                raise K2Error(f"{who}: a PIL image needs clip_image=")
+            emb = self.clip_image(image).float().reshape(1, D)
+        return emb.to(dev).expand(B, D)
 
     def zero_image_emb(self, batch_size):
         """diffusers' KandinskyV22PriorPipeline.get_zero_embed: the CLIP image tower on all-zero pixel_values, supplied by the

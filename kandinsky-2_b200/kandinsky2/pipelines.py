@@ -411,20 +411,23 @@ class Kandinsky2_2(_DecoderBase):
         return dict(prior_steps=prior_steps, prior_guidance_scale=prior_guidance_scale,
                     negative_prior_prompt=negative_prior_prompt)
 
-    def _embeds(self, prompt, batch_size, negative_decoder_prompt, prior_kw=None):
+    def _embeds(self, prompt, batch_size, negative_decoder_prompt, prior_kw=None, embedder=None):
         """(image embedding of prompt, decoder negative): the negative is zero_image_emb when negative_decoder_prompt is "",
-        else the prior's embedding of negative_decoder_prompt guided against "" (kandinsky2_2_model.py:72-76)."""
-        pos = self.embedder.image_emb(prompt, batch_size, **(prior_kw or {}))
-        return pos, self._negative(batch_size, negative_decoder_prompt, prior_kw)
+        else the prior's embedding of negative_decoder_prompt guided against "" (kandinsky2_2_model.py:72-76).  embedder:
+        what takes the embedder calls (default: the pipeline's; the batcher passes one that queues prior requests)."""
+        emb = self.embedder if embedder is None else embedder
+        pos = emb.image_emb(prompt, batch_size, **(prior_kw or {}))
+        return pos, self._negative(batch_size, negative_decoder_prompt, prior_kw, emb)
 
-    def _negative(self, batch_size, negative_decoder_prompt, prior_kw):
+    def _negative(self, batch_size, negative_decoder_prompt, prior_kw, embedder=None):
+        emb = self.embedder if embedder is None else embedder
         if negative_decoder_prompt == "":
-            return self.embedder.zero_image_emb(batch_size)
+            return emb.zero_image_emb(batch_size)
         if prior_kw is None:
-            return self.embedder.image_emb(negative_decoder_prompt, batch_size)
-        return self.embedder.image_emb(negative_decoder_prompt, batch_size, **{**prior_kw, "negative_prior_prompt": ""})
+            return emb.image_emb(negative_decoder_prompt, batch_size)
+        return emb.image_emb(negative_decoder_prompt, batch_size, **{**prior_kw, "negative_prior_prompt": ""})
 
-    def batcher(self, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0):
+    def batcher(self, max_batch, h, w, sampler="ddpm_sampler", max_steps=100, max_loras=0, prior_slots=0):
         """A batching.Batcher: text2img requests submitted one at a time and served from one continuously refilled batch of
         max_batch slots at h x w (rounded up to multiples of 64, as generate_text2img does), every slot at its own denoising
         step.  sampler: "ddpm_sampler", "dpmpp_2m_sampler" or "dpmpp_2m_karras_sampler"; max_steps bounds a request's
@@ -432,9 +435,13 @@ class Kandinsky2_2(_DecoderBase):
         the decoder (Batcher.add_lora, submit(lora=...)); the batcher then keeps copies of the attention weights, so
         load_lora / unload_lora on this pipeline afterwards do not change what it computes.  submit(image=..., strength=...)
         queues an img2img request (generate_img2img).  On a task_type="controlnet" pipeline every request takes its own depth
-        hint and computes what generate_controlnet, or with an image generate_controlnet_img2img, computes."""
+        hint and computes what generate_controlnet, or with an image generate_controlnet_img2img, computes.
+        prior_slots = P > 0 (an embedder with batcher(), e.g. model.prior.PriorEmbedder22) samples the prompts' image
+        embeddings in a continuously refilled batch of P prior slots (batching.PriorBatcher) instead of one prior call per
+        submit; a request joins the decoder queue when its embeddings are done.  0: the embedder runs at submit."""
         from .batching import Batcher
-        return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras)
+        return Batcher(self, max_batch, h, w, sampler=sampler, max_steps=max_steps, max_loras=max_loras,
+                       prior_slots=prior_slots)
 
     def generate_text2img(self, prompt, batch_size=1, decoder_steps=50, prior_steps=25, decoder_guidance_scale=4,
                           prior_guidance_scale=4, h=512, w=512, negative_prior_prompt="", negative_decoder_prompt="",
@@ -556,14 +563,17 @@ class Kandinsky2_2(_DecoderBase):
             raise ValueError("prior_strength needs an embedder that runs the prior from an image embedding "
                              "(runs_prior and emb2emb, e.g. model.prior.PriorEmbedder22)")
 
-    def _controlnet_img2img_embeds(self, prompt, image, batch_size, negative_decoder_prompt, prior_kw, prior_strength):
-        """(positive, decoder negative) image embeddings of generate_controlnet_img2img (its docstring gives the rule)."""
+    def _controlnet_img2img_embeds(self, prompt, image, batch_size, negative_decoder_prompt, prior_kw, prior_strength,
+                                   embedder=None):
+        """(positive, decoder negative) image embeddings of generate_controlnet_img2img (its docstring gives the rule);
+        embedder as for _embeds."""
         if prior_strength is None:
-            return self._embeds(prompt, batch_size, negative_decoder_prompt, prior_kw)
-        pos = self.embedder.emb2emb(prompt, image, batch_size, strength=prior_strength, **prior_kw)
-        neg = (self.embedder.zero_image_emb(batch_size) if negative_decoder_prompt == "" else
-               self.embedder.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
-                                     **{**prior_kw, "negative_prior_prompt": ""}))
+            return self._embeds(prompt, batch_size, negative_decoder_prompt, prior_kw, embedder)
+        emb = self.embedder if embedder is None else embedder
+        pos = emb.emb2emb(prompt, image, batch_size, strength=prior_strength, **prior_kw)
+        neg = (emb.zero_image_emb(batch_size) if negative_decoder_prompt == "" else
+               emb.emb2emb(negative_decoder_prompt, image, batch_size, strength=1.0,
+                           **{**prior_kw, "negative_prior_prompt": ""}))
         return pos, neg
 
     def generate_inpainting(self, prompt, pil_img, img_mask, batch_size=1, decoder_steps=50, prior_steps=25,
