@@ -3,11 +3,10 @@ ControlNet-depth requests: one CFG-doubled UNet batch of S slots, every slot a r
 a FIFO queue as requests finish.
 
 Rows follow the version's layout: for slot s, unconditional s and conditional S + s in 2.2, the reverse in 2.1.  The device
-keeps per slot its step index, its timestep / coefficient / per-step noise tables and its guidance scale (k2b200.h:
-k2_slot_step_begin); one step of the whole
-batch is ONE captured CUDA graph (k2_slot_step_begin, the UNet plan, the slot form of the sampler step, k2_slot_step_end)
-whose buffers never move, so admitting a request is a handful of copies into them and the host loop reads nothing back from
-the device: it knows from its own bookkeeping which slot finishes at which step.
+keeps per slot its step index, its timestep / coefficient / per-step noise tables and its guidance scale (SlotSteps, k2b200.h:
+k2_slot_step_begin); one step of the whole batch is ONE captured CUDA graph (SlotSteps.begin, the UNet plan, SlotSteps.step,
+SlotSteps.end) whose buffers never move, so admitting a request is a handful of copies into them and the host loop
+(_SlotBatcher) reads nothing back from the device: it knows from its own bookkeeping which slot finishes at which step.
 
 A request computes what generate_text2img(batch_size=1) computes on a pipeline whose base_seed is the request's seed: the same
 start latent and per-step noise draws, the same tables (request_tables: the rows of the schedule the pipeline's sampling loop
@@ -33,11 +32,12 @@ slot's encoder K/V rows are computed at admission with its adapter's merged enco
 admitting write slabs, the map and conditioning rows in place, so the step graph never changes.
 
 PriorBatcher serves the Kandinsky 2.2 prior the same way: S slots, each an image_emb(prompt, 1) or emb2emb(prompt, image, 1)
-request at its own UnCLIP step of its own tables, one replay of model.prior._PriorSlotPlan per step, results left on the
-device.  A decoder Batcher made with prior_slots = P > 0 runs the pipeline's embedding rules against prior requests instead of
-prior calls at submit; a request waits until its embeddings are done and then joins the decoder queue (requests ready at the
-same prior step in submit order).  step() replays one prior step before the decoder step while the prior batch has work,
-and prior steps back to back until a prior request finishes when a decoder slot is free and no ready request can take it.
+request at its own UnCLIP step of its own tables, one graph replay per step (SlotSteps around the prior network of
+model.prior._PriorSlotPlan), results left on the device.  A decoder Batcher made with prior_slots = P > 0 runs the
+pipeline's embedding rules against prior requests instead of prior calls at submit; a request waits until its embeddings
+are done and then joins the decoder queue (requests ready at the same prior step in submit order).  step() replays one
+prior step before the decoder step while the prior batch has work, and prior steps back to back until a prior request
+finishes when a decoder slot is free and no ready request can take it.
 """
 import collections
 import inspect
@@ -58,15 +58,20 @@ BATCHER_SAMPLERS = ("ddpm_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler
 BATCHER_SAMPLERS_21 = ("p_sampler", "ddim_sampler", "dpmpp_2m_sampler", "dpmpp_2m_karras_sampler")
 
 
+def _check_int(who, name, v, lo, hi=None):
+    """Refuse v unless it is an int (a bool is not) in [lo, hi], hi None for no upper bound: ValueError naming the argument."""
+    if isinstance(v, bool) or not isinstance(v, int) or v < lo or (hi is not None and v > hi):
+        bounds = f">= {lo}" if hi is None else f"in [{lo}, {hi}]"
+        raise ValueError(f"{who}: {name} must be an int {bounds}, got {v!r}")
+
+
 def check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras=0, samplers=BATCHER_SAMPLERS):
     """Refuse what a Batcher cannot serve, before any work: ValueError naming the argument."""
     if sampler not in samplers:
         raise ValueError(f"batcher: sampler {sampler!r} is not served; use one of {', '.join(samplers)}")
-    for name, v in (("max_batch", max_batch), ("h", h), ("w", w), ("max_steps", max_steps)):
-        if isinstance(v, bool) or not isinstance(v, int) or v < 1:
-            raise ValueError(f"batcher: {name} must be a positive int, got {v!r}")
-    if isinstance(max_loras, bool) or not isinstance(max_loras, int) or max_loras < 0:
-        raise ValueError(f"batcher: max_loras must be an int >= 0, got {max_loras!r}")
+    for name, v, lo in (("max_batch", max_batch, 1), ("h", h, 1), ("w", w, 1), ("max_steps", max_steps, 1),
+                        ("max_loras", max_loras, 0)):
+        _check_int("batcher", name, v, lo)
 
 
 def request_tables(pipe, sampler, steps, init_step=None):
@@ -131,6 +136,142 @@ class SlotQueue:
         return any(h is not None for h in self.holder)
 
 
+class SlotSteps:
+    """The device side of S slots, each at its own step of its own tables of max_steps rows: state int32 [2, S] = (k_s, steps_s)
+    of k2b200.h (idle: [-1, 0]), the latents x [S, *shape] and the step kernels' operands.  begin, step and end launch one
+    step of every active slot around the network; stage and idle are the only writers of state."""
+
+    def __init__(self, S, shape, max_steps, device, kind="ddpm", draws_noise=True, clip=10.0, cond_first=0,
+                 threshold_mode=0):
+        ddpm = kind == "ddpm"
+        self.S, self.clip, self.cond_first, self.threshold_mode = S, clip, cond_first, threshold_mode
+        f32 = dict(device=device, dtype=torch.float32)
+        self.x = torch.zeros(S, *shape, **f32)
+        self.state = torch.tensor([[-1] * S, [0] * S], device=device, dtype=torch.int32)
+        self.ts_tab = torch.zeros(S, max_steps, **f32)
+        self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
+        self.coef = torch.zeros(S, 8, **f32)
+        self.guidance = torch.zeros(S, **f32)
+        self.noise_tab = torch.zeros(S, max_steps, *shape, **f32) if draws_noise else None
+        self.noise = torch.zeros(S, *shape, **f32) if ddpm else None
+        self.work = torch.zeros(S, *shape, **f32) if ddpm else None
+        self.sval = torch.zeros(S, **f32) if threshold_mode else None   # each slot's dynamic threshold
+        self.hist = None if ddpm else torch.zeros(S, *shape, **f32)
+
+    def begin(self, x_in, t_in):
+        ops.slot_step_begin(self.x, x_in, t_in, self.coef, self.ts_tab, self.coef_tab, self.noise_tab, self.noise, self.state)
+
+    def step(self, model_out):
+        if self.hist is None:
+            ops.slot_sampler_step(model_out, self.x, self.noise, self.coef, self.guidance, self.state, self.work, self.clip,
+                                  cond_first=self.cond_first, threshold_mode=self.threshold_mode, sval=self.sval)
+        else:
+            ops.slot_dpm_solver_step(model_out, self.x, self.hist, self.coef, self.guidance, self.state,
+                                     cond_first=self.cond_first)
+
+    def end(self):
+        ops.slot_step_end(self.state)
+
+    def stage(self, s, ts, coef, x, guidance, noise=None):
+        """Slot s starts a request of k = len(ts) steps from latent x, with its k rows of tables and, when the step draws
+        noise, its k steps' noise (x and noise reshaped to the slot's latents); its solver history is zeroed."""
+        k = ts.shape[0]
+        self.ts_tab[s, :k].copy_(ts)
+        self.coef_tab[s, :k].copy_(coef)
+        self.x[s].copy_(x.reshape(self.x.shape[1:]))
+        if noise is not None:
+            self.noise_tab[s, :k].copy_(noise.reshape((k,) + self.x.shape[1:]))
+        if self.hist is not None:
+            self.hist[s].zero_()
+        self.guidance[s] = guidance
+        self.state[:, s] = torch.tensor([0, k], dtype=torch.int32)
+
+    def idle(self, s):
+        self.state[:, s] = torch.tensor([-1, 0], dtype=torch.int32)
+
+
+class _SlotBatcher:
+    """The host loop of a batcher: requests registered under handles, a SlotQueue, and one step of every occupied slot per
+    graph replay.  A subclass makes plan and slots (SlotSteps), calls _capture, and gives _stage(s, r) (bind r's conditioning,
+    then slots.stage) and _weights() (once they change, a step raises K2Error(WEIGHTS_CHANGED))."""
+
+    def __init__(self, S):
+        self.queue = SlotQueue(S)
+        self._requests = {}
+        self._next_handle = 0
+
+    def _capture(self, model_out):
+        self._model_out = model_out   # the plan's output, as the step kernel reads it
+        self._weights0 = self._weights()
+        self._launch()  # warm-up with every slot idle (changes nothing): one-time cudaFuncSetAttribute calls are not capturable
+        torch.cuda.synchronize()
+        self.graph = capture_graph(self._launch)
+
+    def _launch(self):
+        self.slots.begin(self.plan.x_in, self.plan.t_in)
+        self.plan.launch()
+        self.slots.step(self._model_out)
+        self.slots.end()
+
+    def _check_weights(self):
+        if any(a is not b for a, b in zip(self._weights(), self._weights0)):
+            raise K2Error(self.WEIGHTS_CHANGED)
+
+    def _enqueue(self, r, ready=True):
+        """Register request r -> its handle; a ready request joins the queue for its r.steps steps."""
+        handle = self._next_handle
+        self._next_handle += 1
+        self._requests[handle] = r
+        if ready:
+            self.queue.submit(handle, r.steps)
+        return handle
+
+    def pending(self):
+        """Whether a request is waiting or being sampled."""
+        return bool(self.queue.waiting) or self.queue.busy()
+
+    def _admit(self):
+        """Stage waiting requests into free slots, one at a time: a request holds its slot in the host bookkeeping only once
+        its conditioning, tables, latent and noise are written, so a failed admission leaves no slot that would be stepped
+        and finished from another request's buffers."""
+        while True:
+            got = self.queue.admit(limit=1)
+            if not got:
+                return
+            s, handle = got[0]
+            try:
+                self._stage(s, self._requests[handle])
+            except BaseException:
+                self.queue.release(s)
+                self.slots.idle(s)
+                del self._requests[handle]
+                raise
+
+    def _before_admit(self):
+        pass
+
+    def _step_slots(self):
+        """Admit waiting requests into free slots and run one step of every occupied slot (one graph replay) -> [(slot,
+        handle)] of the requests it finished, no longer registered, or None when no slot was occupied (no replay)."""
+        self._check_weights()
+        self._before_admit()
+        self._admit()
+        if not self.queue.busy():
+            return None
+        self.graph.replay()
+        done = self.queue.advance()
+        for _, handle in done:
+            del self._requests[handle]
+        return done
+
+    def run(self):
+        """step() until every submitted request is finished -> {handle: result} of all of them."""
+        out = {}
+        while self.pending():
+            out.update(self.step())
+        return out
+
+
 class _Request:
     __slots__ = ("steps", "guidance", "seed", "ts", "coef", "negative", "positive", "lora", "full", "pooled", "start", "hint")
 
@@ -149,12 +290,7 @@ def _check_img2img(image, strength):
         raise ValueError(f"submit: strength must be a number in [0, 1], got {strength!r}")
 
 
-def _check_steps(name, steps, max_steps):
-    if isinstance(steps, bool) or not isinstance(steps, int) or not 1 <= steps <= max_steps:
-        raise ValueError(f"submit: {name} must be an int in [1, {max_steps}] (the batcher's max_steps), got {steps!r}")
-
-
-class Batcher:
+class Batcher(_SlotBatcher):
     """Kandinsky 2.2 requests of one geometry and one sampler served from max_batch slots (Kandinsky2_2.batcher builds it).
     What differs between the versions is a class attribute or one of the methods Batcher21 overrides: the sampler set, the
     tasks, the geometry and context length, submit's keywords, the image latent and the conditioning a slot is bound to.  The
@@ -163,6 +299,7 @@ class Batcher:
     RUN_AHEAD = 2   # replayed steps the host may have in flight on the GPU when it admits (2: the GPU never waits on admission)
     SAMPLERS = BATCHER_SAMPLERS
     TASKS = ("text2img", "controlnet")
+    WEIGHTS_CHANGED = "batcher: the UNet's weights were reloaded after the batcher was made; make a new one"
     hinted = False   # True on a ControlNet pipeline's batcher: every request brings its own depth hint
     prior = None     # the PriorBatcher of a batcher made with prior_slots > 0
 
@@ -170,8 +307,7 @@ class Batcher:
         self._check_args(max_batch, h, w, sampler, max_steps, max_loras)
         if pipe.task_type not in self.TASKS:
             raise ValueError(f"batcher: serves {' and '.join(self.TASKS)} pipelines only, this one is {pipe.task_type!r}")
-        if isinstance(prior_slots, bool) or not isinstance(prior_slots, int) or prior_slots < 0:
-            raise ValueError(f"batcher: prior_slots must be an int >= 0, got {prior_slots!r}")
+        _check_int("batcher", "prior_slots", prior_slots, 0)
         if prior_slots and not hasattr(pipe.embedder, "batcher"):
             raise ValueError("batcher: prior_slots > 0 needs an embedder that samples the prior in a batch (batcher(max_batch), "
                              f"e.g. model.prior.PriorEmbedder22); this pipeline's is a {type(pipe.embedder).__name__}")
@@ -183,7 +319,6 @@ class Batcher:
         model = pipe.model
         if model._packed is None:
             model.finalize()
-        self._packed = model._packed
         dev = pipe.device
         self.max_loras = max_loras
         self._loras = {}   # adapter name -> (slab index, {attention layer -> merged encoder_kv weight})
@@ -208,31 +343,12 @@ class Batcher:
         p.xf_proj.zero_()
         for buf in p.enc_kv.values():
             buf.zero_()
-        f32 = dict(device=dev, dtype=torch.float32)
-        self.x = torch.zeros(S, 4, H, W, **f32)
-        self.state = torch.tensor([[-1] * S, [0] * S], device=dev, dtype=torch.int32)
-        self.ts_tab = torch.zeros(S, max_steps, **f32)
-        self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
-        self.coef = torch.zeros(S, 8, **f32)
-        self.guidance = torch.zeros(S, **f32)
         # the step settings the sampling loop reads from its schedule and the pipeline, read from the schedule at two steps
-        # (the fewest a DDPM schedule has; the settings do not depend on the count): step_kind "ddpm" runs on
-        # ops.slot_sampler_step, "dpmpp_2m" on ops.slot_dpm_solver_step
+        # (the fewest a DDPM schedule has; the settings do not depend on the count)
         sched = _sampler_schedule(sampler, pipe._diffusion(sampler, 2), 2)
-        ddpm = sched.step_kind == "ddpm"
-        self.clip = sched.clip_range
-        self.threshold_mode = int(isinstance(sched, SpacedDiffusion) and pipe.dynamic_threshold)
-        self.cond_first = int(pipe.cond_first)
-        # the DDPM step's noise for every step of every slot, drawn at admission: S x max_steps x 4 H W floats (DDIM at eta 0
-        # reads no noise: its noise buffer stays zero)
-        self.noise_tab = torch.zeros(S, max_steps, 4, H, W, **f32) if sched.draws_noise else None
-        self.noise = torch.zeros(S, 4, H, W, **f32) if ddpm else None
-        self.work = torch.zeros(S, 4, H, W, **f32) if ddpm else None
-        self.sval = torch.zeros(S, **f32) if self.threshold_mode else None   # each slot's dynamic threshold
-        self.hist = None if ddpm else torch.zeros(S, 4, H, W, **f32)
-        self.queue = SlotQueue(S)
-        self._requests = {}
-        self._next_handle = 0
+        self.slots = SlotSteps(S, (4, H, W), max_steps, dev, sched.step_kind, sched.draws_noise, sched.clip_range,
+                               int(pipe.cond_first), int(isinstance(sched, SpacedDiffusion) and pipe.dynamic_threshold))
+        super().__init__(S)
         # prompt requests' image embeddings sampled in a batch of prior slots: a decoder request waits in _held (handle ->
         # embeddings still missing) until the prior requests in _waiting_on (prior handle -> (handle, "positive" /
         # "negative")) are done
@@ -243,21 +359,10 @@ class Batcher:
         # stays at most RUN_AHEAD steps ahead of the GPU and a request that arrives while a slot is free joins the batch at the
         # next step on the GPU's clock, not after everything already enqueued
         self._events = collections.deque()
-        self._launch()  # warm-up with every slot idle (changes nothing): one-time cudaFuncSetAttribute calls are not capturable
-        torch.cuda.synchronize()
-        self.graph = capture_graph(self._launch)
+        self._capture(p.out)
 
-    def _launch(self):
-        p = self.plan
-        ops.slot_step_begin(self.x, p.x_in, p.t_in, self.coef, self.ts_tab, self.coef_tab, self.noise_tab, self.noise,
-                            self.state)
-        p.launch()
-        if self.hist is None:
-            ops.slot_sampler_step(p.out, self.x, self.noise, self.coef, self.guidance, self.state, self.work, self.clip,
-                                  cond_first=self.cond_first, threshold_mode=self.threshold_mode, sval=self.sval)
-        else:
-            ops.slot_dpm_solver_step(p.out, self.x, self.hist, self.coef, self.guidance, self.state, cond_first=self.cond_first)
-        ops.slot_step_end(self.state)
+    def _weights(self):
+        return (self.pipe.model._packed,)
 
     def _check_args(self, max_batch, h, w, sampler, max_steps, max_loras):
         check_batcher_args(max_batch, h, w, sampler, max_steps, max_loras, self.SAMPLERS)
@@ -283,12 +388,11 @@ class Batcher:
         free = [k for k in range(1, self.max_loras + 1) if k not in used]
         if not free:
             raise ValueError(f"add_lora: all {self.max_loras} adapter slabs are in use; remove_lora one first")
+        self._check_weights()
         model = self.pipe.model
-        if model._packed is not self._packed:
-            raise K2Error("batcher: the UNet's weights were reloaded after the batcher was made; make a new one")
         factors = model.lora_factors(state_dict)
         k, wenc, out = free[0], {}, {}   # out: id(packed weight) -> where this adapter's merge of it goes
-        for p, a in self._packed["attn"].items():
+        for p, a in model._packed["attn"].items():
             wqkv, wproj = self.plan.attn_slabs["layers"][p]
             wenc[p] = a["wenc"].clone()   # so its padding columns, which a merge leaves alone, are the packed weight's
             out.update({id(a["wqkv"]): wqkv[k], id(a["wproj"]): wproj[k], id(a["wenc"]): wenc[p]})
@@ -323,7 +427,7 @@ class Batcher:
             raise ValueError("submit: image_embeds needs negative_image_embeds")
         for name, e in (("image_embeds", image_embeds), ("negative_image_embeds", negative_image_embeds)):
             _check_embedding(name, e, self._emb_dim)
-        _check_steps("decoder_steps", decoder_steps, self.max_steps)
+        _check_int("submit", "decoder_steps", decoder_steps, 1, self.max_steps)
         if lora is not None and lora not in self._loras:
             raise ValueError(f"submit: no adapter named {lora!r} is registered (Batcher.add_lora)")
         _check_img2img(image, strength)
@@ -336,13 +440,7 @@ class Batcher:
             pipe._check_prior_strength(prior_strength, pk)
         # with prior slots the pipeline's embedding rules run against _PriorQueue: prior requests, checked, queued by _enqueue
         embedder = _PriorQueue(self.prior, pipe.embedder) if self.prior is not None else None
-        r = _Request()
-        r.lora = lora
-        r.guidance = float(decoder_guidance_scale)
-        r.seed = pipe.base_seed if seed is None else int(seed)
-        r.hint = self._slot_hint(hint)
-        r.start, init_step = self._img2img_start(image, strength, decoder_steps, r.seed)
-        r.ts, r.coef = request_tables(pipe, self.sampler, decoder_steps, init_step)
+        r = self._request(decoder_guidance_scale, seed, image, strength, decoder_steps, lora, self._slot_hint(hint))
         if prompt is None:
             r.positive, r.negative = image_embeds, negative_image_embeds
         elif prior_strength is None:
@@ -374,6 +472,16 @@ class Batcher:
         """The latent generate_img2img starts from: the MoVQ encoding of image at the batcher's h x w."""
         return self.pipe._encode_image(image, self.h, self.w)
 
+    def _request(self, guidance, seed, image, strength, steps, lora=None, hint=None):
+        """A request with its guidance, seed (default: the pipeline's base_seed), img2img start latent and tables."""
+        r = _Request()
+        r.lora, r.hint = lora, hint
+        r.guidance = float(guidance)
+        r.seed = self.pipe.base_seed if seed is None else int(seed)
+        r.start, init_step = self._img2img_start(image, strength, steps, r.seed)
+        r.ts, r.coef = request_tables(self.pipe, self.sampler, steps, init_step)
+        return r
+
     def _img2img_start(self, image, strength, steps, seed):
         """-> (start latent [1, 4, H, W], init_step) of the pipeline's img2img rule with base_seed = seed, or (None, None) for
         a request without an image.  Refuses an image whose latent is not the batcher's grid and a strength whose rule keeps
@@ -402,14 +510,10 @@ class Batcher:
         if r.steps > self.max_steps:
             raise ValueError(f"submit: the request's schedule has {r.steps} steps, more than the batcher's max_steps "
                              f"{self.max_steps}")
-        handle = self._next_handle
-        self._next_handle += 1
-        self._requests[handle] = r
         waits = [name for name in ("positive", "negative") if isinstance(getattr(r, name), _PriorRequest)]
-        if not waits:
-            self.queue.submit(handle, r.steps)
-            return handle
-        self._held[handle] = len(waits)
+        handle = super()._enqueue(r, ready=not waits)
+        if waits:
+            self._held[handle] = len(waits)
         for name in waits:
             self._waiting_on[self.prior.enqueue(getattr(r, name))] = (handle, name)
         return handle
@@ -453,23 +557,6 @@ class Batcher:
         else:
             self._prior_step()
 
-    def _admit(self):
-        """Stage waiting requests into free slots, one at a time: a request holds its slot in the host bookkeeping only once
-        its conditioning, tables, latent and noise are written, so a failed admission leaves no slot that would be stepped
-        and decoded from another request's buffers."""
-        while True:
-            got = self.queue.admit(limit=1)
-            if not got:
-                return
-            s, handle = got[0]
-            try:
-                self._stage(s, self._requests[handle])
-            except BaseException:
-                self.queue.release(s)
-                self.state[:, s] = torch.tensor([-1, 0], dtype=torch.int32)
-                del self._requests[handle]
-                raise
-
     def _bind(self, s, r):
         """Write request r's conditioning into slot s's rows of the plan."""
         if self.w_map is None:
@@ -480,60 +567,46 @@ class Batcher:
             self._set_slab(s, k)
 
     def _stage(self, s, r):
-        pipe, H, W = self.pipe, self.x.shape[2], self.x.shape[3]
+        pipe, (H, W) = self.pipe, self._latent_hw
         self._bind(s, r)
-        k = r.steps
-        self.ts_tab[s, :k].copy_(r.ts)
-        self.coef_tab[s, :k].copy_(r.coef)
         # the draws of generate_text2img(batch_size=1) with base_seed = r.seed (_DecoderBase._decode, _sampling_loop), or the
-        # img2img start latent made at submit; the DDPM noise below is drawn for the k rows the request runs
-        if r.start is not None:
-            self.x[s].copy_(r.start[0])
-        else:
-            self.x[s].copy_(parallel.sample_noise(range(1), (4, H, W), base_seed=r.seed, device=pipe.device)[0])
-        if self.noise_tab is not None:
+        # img2img start latent made at submit; the DDPM noise below is drawn for the rows the request runs
+        x = r.start if r.start is not None else parallel.sample_noise(range(1), (4, H, W), base_seed=r.seed, device=pipe.device)
+        noise = None
+        if self.slots.noise_tab is not None:
             gen = pipe._generators(0, 1, base_seed=r.seed)[0]
-            self.noise_tab[s, :k].copy_(torch.randn(k, 4, H, W, device=pipe.device, generator=gen))
-        if self.hist is not None:
-            self.hist[s].zero_()
-        self.guidance[s] = r.guidance
-        self.state[:, s] = torch.tensor([0, k], dtype=torch.int32)
+            noise = torch.randn(r.steps, 4, H, W, device=pipe.device, generator=gen)
+        self.slots.stage(s, r.ts, r.coef, x, r.guidance, noise)
 
-    def step(self):
-        """Admit waiting requests into free slots, run one denoising step of every occupied slot (one graph replay), decode
-        the requests that step finished -> {handle: PIL image}."""
-        if self.pipe.model._packed is not self._packed:
-            raise K2Error("batcher: the UNet's weights were reloaded after the batcher was made; make a new one")
+    def _before_admit(self):
         if len(self._events) >= self.RUN_AHEAD:
             self._events.popleft().synchronize()   # waits for a step to end; reads nothing back
         if self.prior is not None:
             self._run_prior()
-        self._admit()
-        if not self.queue.busy():
+
+    def step(self):
+        """Admit waiting requests into free slots, run one denoising step of every occupied slot (one graph replay), decode
+        the requests that step finished -> {handle: PIL image}."""
+        finished = self._step_slots()
+        if finished is None:
             return {}
-        self.graph.replay()
         ev = torch.cuda.Event()
         ev.record()
         self._events.append(ev)
         done = {}
-        for s, handle in self.queue.advance():
-            done[handle] = self.pipe._finish(self.x[s:s + 1], self.h, self.w)[0]
-            del self._requests[handle]
+        for s, handle in finished:
+            done[handle] = self.pipe._finish(self.slots.x[s:s + 1], self.h, self.w)[0]
             if self.w_map is not None:
                 self._set_slab(s, 0)   # idle slots use slab 0, so a removed adapter's slab is read by no slot
         return done
 
     def _set_slab(self, s, k):
-        S = self.x.shape[0]
         self.w_map[s] = k
-        self.w_map[S + s] = k
+        self.w_map[self.slots.S + s] = k
 
-    def run(self):
-        """step() until every submitted request is finished -> {handle: PIL image} of all of them."""
-        out = {}
-        while self.queue.waiting or self.queue.busy() or (self.prior is not None and self._held):
-            out.update(self.step())
-        return out
+    def pending(self):
+        """Whether a request is waiting for its embeddings, waiting for a slot or being denoised."""
+        return super().pending() or bool(self._held)
 
 
 class Batcher21(Batcher):
@@ -580,14 +653,9 @@ class Batcher21(Batcher):
             raise ValueError(f"submit: prompt must be a str, got {type(prompt).__name__}")
         for name, e in (("image_embeds", image_embeds), ("negative_image_embeds", negative_image_embeds)):
             _check_embedding(name, e, self._emb_dim)
-        _check_steps("num_steps", num_steps, self.max_steps)
+        _check_int("submit", "num_steps", num_steps, 1, self.max_steps)
         _check_img2img(image, strength)
-        r = _Request()
-        r.lora = r.hint = None
-        r.guidance = float(guidance_scale)
-        r.seed = pipe.base_seed if seed is None else int(seed)
-        r.start, init_step = self._img2img_start(image, strength, num_steps, r.seed)
-        r.ts, r.coef = request_tables(pipe, self.sampler, num_steps, init_step)
+        r = self._request(guidance_scale, seed, image, strength, num_steps)
         r.full, r.pooled = pipe.embedder.text_emb(prompt, 1)
         if r.full.shape[1] != self._text_len:
             raise ValueError(f"submit: the embedder's text rows have length {r.full.shape[1]}, the batcher's {self._text_len}")
@@ -614,32 +682,34 @@ class _PriorRequest:
     __slots__ = ("steps", "guidance", "rows", "ts", "coef", "x", "noise")
 
 
-class PriorBatcher:
+class PriorBatcher(_SlotBatcher):
     """Kandinsky 2.2 prior requests served from max_batch slots (PriorEmbedder22.batcher builds it): one UnCLIP sampling step of
-    every slot is ONE replay of a captured _PriorSlotPlan graph, each slot at its own step of its own tables, refilled from
-    a FIFO queue as requests finish.  A request computes what the embedder's image_emb(prompt, 1, ...) -- or with an image
-    emb2emb(prompt, image, 1, strength, ...) -- computes: the CLIP rows, guidance and generator of its _call_args, the same
-    draws in the same order, UnCLIPSchedule's tables, and a slot step that runs the batch step's kernels on the slot's rows
-    alone.  Its result stays on the device.  The host reads nothing back: it knows from its own bookkeeping which slot
-    finishes at which step."""
+    every slot is ONE graph replay (SlotSteps around the prior network of a _PriorSlotPlan), each slot at its own step of its
+    own tables, refilled from a FIFO queue as requests finish.  A request computes what the embedder's image_emb(prompt, 1,
+    ...) -- or with an image emb2emb(prompt, image, 1, strength, ...) -- computes: the CLIP rows, guidance and generator of its
+    _call_args, the same draws in the same order, UnCLIPSchedule's tables, and a slot step that runs the batch step's kernels
+    on the slot's rows alone.  Its result stays on the device.  The host reads nothing back: it knows from its own
+    bookkeeping which slot finishes at which step."""
 
     MAX_STEPS = 1000   # table rows per slot, _PriorStepPlan's limit
+    WEIGHTS_CHANGED = ("prior batcher: the prior's packed weights changed after the batcher was made (load_lora, unload_lora "
+                       "or a reload); make a new one")
 
     def __init__(self, embedder, max_batch):
-        if isinstance(max_batch, bool) or not isinstance(max_batch, int) or max_batch < 1:
-            raise ValueError(f"prior batcher: max_batch must be a positive int, got {max_batch!r}")
+        _check_int("prior batcher", "max_batch", max_batch, 1)
         self.embedder = embedder
         prior = embedder.prior
         if prior._packed is None:
             prior.finalize()
-        self._weights = (prior._packed, prior._lora)
         # a plan of its own: a batch-1 image_emb call between steps must not rebind these rows
-        self.plan = _PriorSlotPlan(prior, max_batch, self.MAX_STEPS)   # recorded by running it once, every slot idle
-        self.queue = SlotQueue(max_batch)
-        self._requests = {}
-        self._next_handle = 0
-        torch.cuda.synchronize()
-        self.graph = capture_graph(self.plan.launch)
+        self.plan = _PriorSlotPlan(prior, max_batch)
+        # a slot's clip_dim floats as the step kernels see them, [4, 1, clip_dim / 4]; SlotSteps' defaults are the prior's
+        self.slots = SlotSteps(max_batch, (4, 1, prior.clip_dim // 4), self.MAX_STEPS, self.plan.dev)
+        super().__init__(max_batch)
+        self._capture(self.plan.model_out.view((2 * max_batch, 8) + self.slots.x.shape[2:]))
+
+    def _weights(self):
+        return self.embedder.prior._packed, self.embedder.prior._lora
 
     def submit(self, prompt, *, prior_steps=None, prior_guidance_scale=None, negative_prior_prompt=None, image=None,
                strength=None):
@@ -655,8 +725,7 @@ class PriorBatcher:
         """The request submit queues, checked and drawn but not queued (enqueue queues it)."""
         emb = self.embedder
         steps = emb.prior_steps if prior_steps is None else prior_steps
-        if isinstance(steps, bool) or not isinstance(steps, int) or not 2 <= steps <= self.MAX_STEPS:
-            raise ValueError(f"submit: prior_steps must be an int in [2, {self.MAX_STEPS}], got {steps!r}")
+        _check_int("submit", "prior_steps", steps, 2, self.MAX_STEPS)
         keep = None
         if image is None and strength is not None:
             raise ValueError("submit: strength without image; strength is how much of the prior an image request runs")
@@ -684,66 +753,19 @@ class PriorBatcher:
 
     def enqueue(self, r):
         """Queue a request made by request() -> its handle."""
-        handle = self._next_handle
-        self._next_handle += 1
-        self._requests[handle] = r
-        self.queue.submit(handle, r.steps)
-        return handle
-
-    def pending(self):
-        """Whether a request is waiting or being sampled."""
-        return bool(self.queue.waiting) or self.queue.busy()
-
-    def _admit(self):
-        """Stage waiting requests into free slots, one at a time, as Batcher._admit does."""
-        while True:
-            got = self.queue.admit(limit=1)
-            if not got:
-                return
-            s, handle = got[0]
-            try:
-                self._stage(s, self._requests[handle])
-            except BaseException:
-                self.queue.release(s)
-                self.plan.state[:, s] = torch.tensor([-1, 0], dtype=torch.int32)
-                del self._requests[handle]
-                raise
+        return self._enqueue(r)
 
     def _stage(self, s, r):
-        p, k = self.plan, r.steps
-        p.bind_slot(s, *r.rows)
-        p.ts_tab[s, :k].copy_(r.ts)
-        p.coef_tab[s, :k].copy_(r.coef)
-        p.noise_tab[s, :k].copy_(r.noise[:, 0])
-        p.x[s].copy_(r.x[0])
-        p.guidance[s] = r.guidance
-        p.state[:, s] = torch.tensor([0, k], dtype=torch.int32)
+        self.plan.bind_slot(s, *r.rows)
+        self.slots.stage(s, r.ts, r.coef, r.x, r.guidance, r.noise)
 
     def step(self):
         """Admit waiting requests into free slots, run one UnCLIP step of every occupied slot (one graph replay) -> {handle:
         fp32 [1, clip_dim] on the device} of the requests it finished, each a tensor of its own (x * clip_std + clip_mean,
         as sample_prior22 finishes)."""
-        prior = self.embedder.prior
-        if prior._packed is not self._weights[0] or prior._lora is not self._weights[1]:
-            raise K2Error("prior batcher: the prior's packed weights changed after the batcher was made (load_lora, "
-                          "unload_lora or a reload); make a new one")
-        self._admit()
-        if not self.queue.busy():
-            return {}
-        self.graph.replay()
-        done = {}
         emb = self.embedder
-        for s, handle in self.queue.advance():
-            done[handle] = self.plan.x[s:s + 1] * emb.clip_std + emb.clip_mean
-            del self._requests[handle]
-        return done
-
-    def run(self):
-        """step() until every submitted request is finished -> {handle: embedding} of all of them."""
-        out = {}
-        while self.pending():
-            out.update(self.step())
-        return out
+        return {handle: self.slots.x[s:s + 1].view(1, -1) * emb.clip_std + emb.clip_mean
+                for s, handle in self._step_slots() or ()}
 
 
 class _PriorQueue:

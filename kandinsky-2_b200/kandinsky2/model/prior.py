@@ -420,8 +420,8 @@ class _PriorNet(LaunchPlan):
     plans share (x_in, t_in, the sequence, the keep mask, model_out) and the recording of the time embedding and its two
     linears, clip_img_proj, the token rows 78 and 79 written into the sequence, the 20 pre-LayerNorm layers of
     model/encoder.py with the masked k2_attention_small as the attention, the final LayerNorm of the last token (a strided
-    view) and out_proj.  Every launch has the eager forward's arguments.  _PriorStepPlan (one call at B samples) and
-    _PriorSlotPlan (S slots, each at its own step) put their step begin / sampler step / step end around it."""
+    view) and out_proj.  Every launch has the eager forward's arguments.  _PriorStepPlan (one call at B samples) puts its
+    step begin / sampler step / step end around it; batching.PriorBatcher puts the slot step's around a _PriorSlotPlan."""
 
     def __init__(self, model, N):
         dev = model._packed["text_enc"][0].device
@@ -551,44 +551,21 @@ class _PriorStepPlan(_PriorNet):
 
 
 class _PriorSlotPlan(_PriorNet):
-    """One UnCLIP sampling step of S slots, each slot a request at its own step of its own tables (batching.PriorBatcher), as
-    ONE launch list over 2S CFG rows (unconditional row s, conditional row S + s): k2_slot_step_begin on x [S, 4, 1,
-    clip_dim / 4] (so a slot's n is clip_dim), the network of _PriorNet, k2_slot_sampler_step (clip 10, the unconditional
-    rows first, no threshold, each slot's guidance from the device array `guidance` [S]) and k2_slot_step_end.  state is the
-    device int32 [2, S] (k_s, steps_s) of k2b200.h; the tables hold max_steps rows per slot.  bind_slot writes one slot's
-    fixed sequence rows and keep-mask rows; what a slot's step computes depends on its own rows alone."""
+    """The prior network of _PriorNet over the 2S CFG rows of S slots (unconditional row s, conditional row S + s), each slot a
+    request at its own step of its own tables (batching.PriorBatcher, which launches the slot step around it).  bind_slot
+    writes one slot's fixed sequence rows and keep-mask rows; what a slot's rows compute depends on its own rows alone."""
 
-    def __init__(self, model, S, max_steps=1000):
+    def __init__(self, model, S):
         super().__init__(model, 2 * S)
         self.S = S
-        D, W, n, ctx = model.clip_dim, model.xf_width, self.n, model.text_ctx
+        W, n, ctx = model.xf_width, self.n, model.text_ctx
         f32 = dict(device=self.dev, dtype=torch.float32)
-        self.x = torch.zeros(S, D, **f32)
-        self.coef = torch.zeros(S, 8, **f32)
-        self.noise = torch.zeros(S, D, **f32)
-        self.work = torch.zeros(S, D, **f32)
-        self.guidance = torch.zeros(S, **f32)
-        self.state = torch.tensor([[-1] * S, [0] * S], device=self.dev, dtype=torch.int32)
-        self.ts_tab = torch.zeros(S, max_steps, **f32)
-        self.coef_tab = torch.zeros(S, max_steps, 8, **f32)
-        self.noise_tab = torch.zeros(S, max_steps, D, **f32)
         # bind_slot computes a slot's rows at bind's B = 1 shapes (2 rows) here, then copies them into rows s and S + s
         self._seq2 = torch.zeros(2, n, W, device=self.dev, dtype=torch.float16)
         self._keep2 = torch.ones(2, n, device=self.dev, dtype=torch.uint8)
         self._te32 = torch.empty(2 * ctx, W, **f32)
         self._row32 = torch.empty(2, W, **f32)
-        self._build()
-
-    def _build(self):
-        S, N, D = self.S, self.N, self.m.clip_dim
-        x4, n4, w4 = (t.view(S, 4, 1, D // 4) for t in (self.x, self.noise, self.work))
-        mo8 = self.model_out.view(N, 8, 1, D // 4)
-        self._add(lambda: ops.slot_step_begin(x4, self.x_in, self.t_in, self.coef, self.ts_tab, self.coef_tab, self.noise_tab,
-                                              n4, self.state), "step")
         self._record_network()
-        self._add(lambda: ops.slot_sampler_step(mo8, x4, n4, self.coef, self.guidance, self.state, w4, 10.0, cond_first=0,
-                                                threshold_mode=0), "sampler_step")
-        self._add(lambda: ops.slot_step_end(self.state), "step")
 
     def _gemm(self, x, w, cout, out, flops, bias=None, residual=None):
         """The layers' flat-row GEMM at 2S rows, pinned to the N tile and split-K factor the batch-1 plan (_PriorStepPlan at

@@ -58,7 +58,7 @@ def run_batcher(b, prompts, arrive, steps):
         while nxt < len(prompts) and arrive[nxt] <= now:
             handles[b.submit(prompts[nxt], decoder_steps=steps, seed=nxt)] = nxt
             nxt += 1
-        if not (b.queue.waiting or b.queue.busy()):
+        if not b.pending():
             _wait_until(t0, arrive[nxt])
             continue
         for h in b.step():

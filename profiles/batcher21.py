@@ -43,7 +43,7 @@ def run_batcher(b, prompts, arrive, steps):
         while nxt < len(prompts) and arrive[nxt] <= now:
             handles[b.submit(prompts[nxt], num_steps=steps, seed=nxt)] = nxt
             nxt += 1
-        if not (b.queue.waiting or b.queue.busy()):
+        if not b.pending():
             _wait_until(t0, arrive[nxt])
             continue
         for h in b.step():
@@ -135,7 +135,7 @@ def main():
     res["batcher"] = _summary(arrive, run_batcher(b, prompts, arrive, steps))
     res["single"] = _summary(arrive, run_calls(pipe, prompts, arrive, steps, 1, size))
     res["groups"] = _summary(arrive, run_calls(pipe, prompts, arrive, steps, S, size))
-    H, W = b.x.shape[2:]
+    H, W = b.slots.x.shape[2:]
     res["percentile_kernel_us"] = dict(slots=S, latent=[H, W], **percentile_kernels_us(S, H, W))
     line = json.dumps(res)
     print(line)

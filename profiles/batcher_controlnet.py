@@ -54,7 +54,7 @@ def run_batcher(b, reqs, arrive, steps):
             prompt, image, hint, strength = reqs[nxt]
             handles[b.submit(prompt, image=image, hint=hint, strength=strength, decoder_steps=steps, seed=nxt)] = nxt
             nxt += 1
-        if not (b.queue.waiting or b.queue.busy()):
+        if not b.pending():
             _wait_until(t0, arrive[nxt])
             continue
         for h in b.step():

@@ -65,7 +65,7 @@ def run_batcher(b, prompts, arrive, steps):
         while nxt < len(prompts) and arrive[nxt] <= now:
             handles[b.submit(prompts[nxt], decoder_steps=steps, seed=nxt)] = nxt
             nxt += 1
-        if not (b.queue.waiting or b.queue.busy() or (b.prior is not None and b._held)):
+        if not b.pending():
             _wait_until(t0, arrive[nxt])
             continue
         for h in b.step():
@@ -88,7 +88,7 @@ def _event_ms(fn, reps):
 
 def _fill(b, steps):
     """Every decoder slot (and prior slot) of b busy for at least `steps` more replays."""
-    for i in range(b.x.shape[0]):
+    for i in range(b.slots.S):
         b.submit(f"warm-up {i}", decoder_steps=steps, seed=100 + i)
     while b.queue.waiting or (b.prior is not None and b._held):
         b.step()

@@ -126,11 +126,12 @@ def test_slot_ops_refuse_host_tensors(op, args):
 
 def _bare_batcher(slots=2, emb_dim=16, max_steps=10):
     """A Batcher with its host state only (no pipeline, plan or graph): enough for submit's checks and the admission loop."""
-    from kandinsky2.batching import Batcher, SlotQueue
+    from kandinsky2.batching import Batcher, SlotSteps, _SlotBatcher
     b = Batcher.__new__(Batcher)
     b.pipe, b.max_steps, b._emb_dim = None, max_steps, emb_dim
-    b.queue, b._requests = SlotQueue(slots), {}
-    b.state = torch.full((2, slots), 7, dtype=torch.int32)
+    _SlotBatcher.__init__(b, slots)
+    b.slots = SlotSteps(slots, (4, 1, 1), max_steps, "cpu")
+    b.slots.state.fill_(7)
     return b
 
 
@@ -165,6 +166,6 @@ def test_failed_admission_frees_its_slot_and_keeps_the_queue():
     with pytest.raises(RuntimeError, match="bad embedding"):
         b._admit()
     assert staged == [(0, 0)] and b.queue.holder == [0, None, None] and [h for h, _ in b.queue.waiting] == [2, 3]
-    assert b.state[:, 1].tolist() == [-1, 0] and 1 not in b._requests
+    assert b.slots.state[:, 1].tolist() == [-1, 0] and 1 not in b._requests
     b._admit()
     assert staged == [(0, 0), (1, 2), (2, 3)] and b.queue.holder == [0, 2, 3]

@@ -81,10 +81,10 @@ def test_batcher21_refuses_other_tasks(task):
 
 
 def _bare_batcher21(emb_dim=16, max_steps=10):
-    from kandinsky2.batching import Batcher21, SlotQueue
+    from kandinsky2.batching import Batcher21, _SlotBatcher
     b = Batcher21.__new__(Batcher21)
     b.pipe, b.max_steps, b._emb_dim = None, max_steps, emb_dim
-    b.queue, b._requests = SlotQueue(2), {}
+    _SlotBatcher.__init__(b, 2)
     return b
 
 

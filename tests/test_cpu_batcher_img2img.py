@@ -112,14 +112,15 @@ def test_21_img2img_start_is_the_earlier_inline_rule(sampler, strength):
 
 def _bare_batcher(version="2.2", task_type="text2img", sampler=None, grid=(8, 8), max_steps=60):
     """A batcher with its host state only (no plan or graph) over a bare pipeline: enough for submit's checks."""
-    from kandinsky2.batching import Batcher, Batcher21, SlotQueue
+    from kandinsky2.batching import Batcher, Batcher21, _SlotBatcher
     cls = Batcher21 if version == "2.1" else Batcher
     b = cls.__new__(cls)
     b.pipe = _bare_pipe(version, task_type, grid)
     b.sampler = sampler or ("p_sampler" if version == "2.1" else "ddpm_sampler")
     b.max_steps, b._emb_dim, b.h, b.w, b._latent_hw = max_steps, 16, 64, 64, (8, 8)
     b.hinted = task_type == "controlnet"
-    b.queue, b._requests, b._loras = SlotQueue(2), {}, {}
+    b._loras = {}
+    _SlotBatcher.__init__(b, 2)
     return b
 
 

@@ -57,13 +57,12 @@ def test_batcher_refuses_a_negative_max_loras():
 
 def _bare_batcher(max_loras, slots=2, emb_dim=16, max_steps=10):
     """A Batcher with its host state only (a bare pipeline, no plan or graph): enough for the registry's refusals."""
-    from kandinsky2.batching import Batcher, SlotQueue
+    from kandinsky2.batching import Batcher, _SlotBatcher
     from kandinsky2.pipelines import Kandinsky2_2
     b = Batcher.__new__(Batcher)
     b.pipe, b.max_steps, b._emb_dim, b.max_loras = Kandinsky2_2.__new__(Kandinsky2_2), max_steps, emb_dim, max_loras
-    b.queue, b._requests, b._loras = SlotQueue(slots), {}, {}
-    b.sampler, b._next_handle = "ddpm_sampler", 0
-    b.state = torch.full((2, slots), 7, dtype=torch.int32)
+    b._loras, b.sampler = {}, "ddpm_sampler"
+    _SlotBatcher.__init__(b, slots)
     return b
 
 

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from kandinsky2.batching import Batcher, PriorBatcher, SlotQueue, _PriorRequest, _Request, prior_request_tables
+from kandinsky2.batching import Batcher, PriorBatcher, SlotSteps, _PriorRequest, _Request, _SlotBatcher, prior_request_tables
 from kandinsky2.model.prior import PriorEmbedder22, UnCLIPSchedule
 
 D = 8
@@ -40,7 +40,8 @@ def _clip_text(prompts):
 
 
 def _bare_prior(slots=2):
-    """A PriorBatcher without a GPU: a real PriorEmbedder22 on the CPU around a stand-in prior, no plan and no graph."""
+    """A PriorBatcher without a GPU: a real PriorEmbedder22 on the CPU around a stand-in prior, its slots on the CPU, no plan
+    and no graph."""
     calls = []
 
     def clip_text(prompts):
@@ -49,8 +50,9 @@ def _bare_prior(slots=2):
     emb = PriorEmbedder22(types.SimpleNamespace(clip_dim=D, _packed="w", _lora=None), clip_text, torch.zeros(D), torch.ones(D),
                           clip_image=lambda img: torch.linspace(-1, 1, D)[None], prior_steps=10, seed=3)
     pb = object.__new__(PriorBatcher)
-    pb.embedder, pb._weights = emb, ("w", None)
-    pb.queue, pb._requests, pb._next_handle = SlotQueue(slots), {}, 0
+    pb.embedder, pb._weights0 = emb, ("w", None)
+    _SlotBatcher.__init__(pb, slots)
+    pb.slots = SlotSteps(slots, (4, 1, D // 4), PriorBatcher.MAX_STEPS, "cpu")
     return pb, calls
 
 
@@ -143,8 +145,8 @@ class _ScriptedPrior:
 
 def _bare_batcher(prior, slots=2):
     b = object.__new__(Batcher)
-    b.max_steps, b.prior = 50, prior
-    b.queue, b._requests, b._next_handle, b._held, b._waiting_on = SlotQueue(slots), {}, 0, {}, {}
+    b.max_steps, b.prior, b._held, b._waiting_on = 50, prior, {}, {}
+    _SlotBatcher.__init__(b, slots)
     return b
 
 
@@ -210,14 +212,12 @@ class _Event:
 def _scheduled(monkeypatch, slots=2, prior_slots=2):
     monkeypatch.setattr(torch.cuda, "Event", _Event)
     pb, _ = _bare_prior(prior_slots)
-    pb.plan = types.SimpleNamespace(x=torch.zeros(prior_slots, D),
-                                    state=torch.zeros(2, prior_slots, dtype=torch.int32))
     pb.graph = _Counter()
     pb._stage = lambda s, r: None
     b = _bare_batcher(pb, slots)
     b.graph, b._events, b.w_map, b.h, b.w = _Counter(), collections.deque(), None, 64, 64
-    b.x = torch.zeros(slots, 4, 1, 1)
-    b._packed = "unet"
+    b.slots = SlotSteps(slots, (4, 1, 1), b.max_steps, "cpu")
+    b._weights0 = ("unet",)
     b.pipe = types.SimpleNamespace(model=types.SimpleNamespace(_packed="unet"), _finish=lambda x, h, w: ["image"])
     b._stage = lambda s, r: None
     return b, pb

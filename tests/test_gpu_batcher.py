@@ -179,7 +179,7 @@ def _step(b, latents):
 
 def _run(b, latents):
     out = {}
-    while b.queue.waiting or b.queue.busy():
+    while b.pending():
         out.update(_step(b, latents))
     return out
 
@@ -247,8 +247,9 @@ def test_one_step_is_one_graph_replay():
     pipe = _pipe("2.2", "text2img")
     b = pipe.batcher(2, 64, 64, max_steps=8)
     g0 = b.graph
-    bufs = [b.x, b.state, b.ts_tab, b.coef_tab, b.coef, b.guidance, b.noise_tab, b.noise, b.work, b.plan.x_in, b.plan.t_in,
-            b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
+    sl = b.slots
+    bufs = [sl.x, sl.state, sl.ts_tab, sl.coef_tab, sl.coef, sl.guidance, sl.noise_tab, sl.noise, sl.work, b.plan.x_in,
+            b.plan.t_in, b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
     ptrs = [t.data_ptr() for t in bufs]
     calls = []
     orig = g0.replay
@@ -257,7 +258,7 @@ def test_one_step_is_one_graph_replay():
     for i, n in enumerate((3, 5, 2)):
         b.submit(f"prompt {i}", decoder_steps=n, seed=i)
     steps = finished = 0
-    while b.queue.waiting or b.queue.busy():
+    while b.pending():
         before = len(calls)
         finished += len(b.step())
         steps += 1

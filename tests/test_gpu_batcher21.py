@@ -183,7 +183,8 @@ def test_one_step_is_one_graph_replay():
     pipe = _pipe("2.1", "text2img")
     b = pipe.batcher(2, 64, 64, sampler="p_sampler", max_steps=8)
     g0 = b.graph
-    bufs = [b.x, b.state, b.ts_tab, b.coef_tab, b.coef, b.guidance, b.noise_tab, b.noise, b.work, b.sval, b.plan.x_in,
+    sl = b.slots
+    bufs = [sl.x, sl.state, sl.ts_tab, sl.coef_tab, sl.coef, sl.guidance, sl.noise_tab, sl.noise, sl.work, sl.sval, b.plan.x_in,
             b.plan.t_in, b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
     ptrs = [t.data_ptr() for t in bufs]
     calls = []
@@ -193,7 +194,7 @@ def test_one_step_is_one_graph_replay():
     for i, n in enumerate((3, 5, 2)):
         b.submit(f"prompt {i}", num_steps=n, seed=i)
     steps = finished = 0
-    while b.queue.waiting or b.queue.busy():
+    while b.pending():
         before = len(calls)
         finished += len(b.step())
         steps += 1

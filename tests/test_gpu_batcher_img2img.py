@@ -211,7 +211,8 @@ def test_one_step_is_one_graph_replay_whatever_the_mix():
     b = pipe.batcher(2, 64, 64, max_steps=8, max_loras=1)
     b.add_lora("A", _lora(pipe.model, 4, 51))
     g0 = b.graph
-    bufs = [b.x, b.state, b.ts_tab, b.coef_tab, b.coef, b.guidance, b.noise_tab, b.noise, b.work, b.w_map, b.plan.x_in,
+    sl = b.slots
+    bufs = [sl.x, sl.state, sl.ts_tab, sl.coef_tab, sl.coef, sl.guidance, sl.noise_tab, sl.noise, sl.work, b.w_map, b.plan.x_in,
             b.plan.hint_in, b.plan.t_in, b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
     ptrs = [t.data_ptr() for t in bufs]
     calls = []
@@ -222,7 +223,7 @@ def test_one_step_is_one_graph_replay_whatever_the_mix():
     b.submit("prompt 1", hint=_hint(64, 64, 2), image=photo, strength=0.5, decoder_steps=8, seed=1, lora="A")
     b.submit("prompt 2", hint=_hint(64, 64, 3), image=photo, strength=0.3, decoder_steps=8, seed=2)
     steps = finished = 0
-    while b.queue.waiting or b.queue.busy():
+    while b.pending():
         before = len(calls)
         finished += len(b.step())
         steps += 1

@@ -242,7 +242,7 @@ def test_registry_keeps_one_graph_and_its_addresses():
     m = pipe.model
     b = pipe.batcher(2, 64, 64, max_steps=8, max_loras=2)
     g0 = b.graph
-    bufs = [b.x, b.state, b.w_map, b.plan.x_in, b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
+    bufs = [b.slots.x, b.slots.state, b.w_map, b.plan.x_in, b.plan.out, b.plan.xf_proj] + list(b.plan.enc_kv.values())
     bufs += [t for pair in b.plan.attn_slabs["layers"].values() for t in pair]
     ptrs = [t.data_ptr() for t in bufs]
     calls = []
@@ -253,7 +253,7 @@ def test_registry_keeps_one_graph_and_its_addresses():
     b.submit("prompt 0", decoder_steps=3, seed=0, lora="A")
     b.submit("prompt 1", decoder_steps=2, seed=1, lora="B")
     steps = 0
-    while b.queue.waiting or b.queue.busy():
+    while b.pending():
         before = len(calls)
         b.step()
         steps += 1

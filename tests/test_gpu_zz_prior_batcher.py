@@ -120,13 +120,13 @@ def test_idle_slots_poisoned_with_nan_do_not_reach_active_slots(tiny):
     req = _mixed(D)[0]
     clean = _alone(emb, 4, req)
     pb = emb.batcher(4)
-    p = pb.plan
+    p, sl = pb.plan, pb.slots
     h = pb.submit(*req[0], **req[1])
     got = pb.step()
     S = 4
     for s in range(1, S):
-        for t in (p.x[s], p.noise[s], p.work[s], p.model_out[s], p.model_out[S + s], p.noise_tab[s], p.ts_tab[s],
-                  p.coef_tab[s]):
+        for t in (sl.x[s], sl.noise[s], sl.work[s], p.model_out[s], p.model_out[S + s], sl.noise_tab[s], sl.ts_tab[s],
+                  sl.coef_tab[s]):
             t.fill_(NAN)
     while pb.pending():
         got.update(pb.step())
@@ -158,9 +158,9 @@ def test_the_default_tuner_and_one_replay_per_step(tiny):
     pb = emb.batcher(4)
     calls, orig = [], pb.graph.replay
     pb.graph.replay = lambda: (calls.append(1), orig())[1]
-    p = pb.plan
-    bufs = lambda: [t.data_ptr() for t in (p.x, p.state, p.ts_tab, p.coef_tab, p.noise_tab, p.guidance, p.seq,  # noqa: E731
-                                           p.keep, p.model_out)]
+    p, sl = pb.plan, pb.slots
+    bufs = lambda: [t.data_ptr() for t in (sl.x, sl.state, sl.ts_tab, sl.coef_tab, sl.noise_tab, sl.guidance,  # noqa: E731
+                                           p.seq, p.keep, p.model_out)]
     ptrs = bufs()
     hs = [pb.submit(*r[0], **r[1]) for r in reqs]
     out, steps = {}, 0
